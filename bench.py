@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- MNIST training images/s of the fused LeNet step on N B200s (BASELINE.json metric, config[1]).
+"""bench.py -- MNIST training images/s of the fused LeNet step on N H100s (BASELINE.json metric, config[1]).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 A "step" is one pass of the hot path (forward + backward + packed-gradient reduction [+ all-reduce] + SGD update,
@@ -13,11 +13,16 @@ Main.cpp:157-171 batched) over one batch of B = 256 synthetic MNIST-shaped image
             u8 images + labels are copied from PINNED host memory inside the timed region (chunked, double-buffered
             copy stream) and every step's error sum is read back to the host
   roofline  fused gradient kernel alone: algorithmic flops / bytes per launch over its average duration (CUDA events,
-            pcnn_time_fused_kernel), against the fp32 FMA rate measured live on this GPU and the measured HBM peak
-            of MEASURED_PEAKS.json.  The fused LeNet step is fp32-FMA bound (AI = 122 flop/B, SURVEY.md 8d); both
+            pcnn_time_fused_kernel), against the fp32 FMA rate measured live on this GPU and the data-sheet HBM
+            bandwidth of this H100 model (SXM 3.35, NVL 3.9, PCIe 2.0 TB/s).  The fused LeNet step is fp32-FMA bound (AI = 122 flop/B, SURVEY.md 8d); both
             fractions are reported, `bound` names the larger one
   cpu_baseline  the unmodified reference (oracle/_ref, else the oracle port) timed on one host core on a bounded sample
   clocks    nvidia-smi SM clock / throttle reasons sampled while the GPU phases run
+
+--dump-outputs DIR writes what the timed steps computed, as the engine hands it to a caller after the last timed step:
+DIR/params.npy (the 2,343 parameters, float32), DIR/grads.npy (that step's packed gradient, float32) and DIR/err_sum.npy
+(the engine's accumulated error sum, float64).  The data set and the initial parameters are fixed, so the same arguments give the same
+inputs on every run and two builds can be compared output for output.
 
 --impl reference times the reference's own CPU implementation (all host cores, independent replicas) for the same
 metric; rank 0 only under torchrun.
@@ -38,15 +43,17 @@ sys.path.insert(0, ROOT)
 FLOPS_PER_IMAGE = 383948            # SURVEY.md 8d: fused train step, 191,974 MAC
 BYTES_PER_IMAGE_U8 = 788            # 784 B image + 4 B label (SURVEY.md 8d); fp32 input would be 3,140
 PARAM_BYTES = 2344 * 4              # packed parameters read once per CTA-wave; counted once per launch
-DATASET_IMAGES = 262144             # 205 MB of u8 images > 126 MB L2: every step reads its batch from HBM
+DATASET_IMAGES = 262144             # 205 MB of u8 images > 50 MB L2: every step reads its batch from HBM
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    """HBM bandwidth of this card from NVIDIA's H100 data sheets (GB/s): SXM 3,350, NVL 3,900, PCIe 2,000."""
+    import torch
+    name = torch.cuda.get_device_name()
+    for key, gbs in (("NVL", 3900.0), ("PCIe", 2000.0)):
+        if key in name:
+            return gbs, f"NVIDIA H100 {key} data sheet ({name})"
+    return 3350.0, f"NVIDIA H100 SXM data sheet ({name})"
 
 
 class ClockSampler:
@@ -89,15 +96,6 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
-def measured_traffic(kernel, batch, steps):
-    """DRAM bytes of one launch from profiles/traffic.json ({kernel: {batch: bytes_per_step}}), or None."""
-    try:
-        d = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        return float(d[kernel][str(batch)]["dram_bytes_per_step"]) * steps
-    except Exception:
-        return None
-
-
 def synthetic(n, seed):
     rng = np.random.default_rng(seed)
     return rng.integers(0, 256, (n, 784), dtype=np.uint8), rng.integers(0, 10, n, dtype=np.uint8)
@@ -109,7 +107,7 @@ MNIST_DIR = os.path.join(ROOT, "oracle", "_ref", "data")
 def load_training_set(copies=5):
     """The real MNIST training split (the four IDX files staged by oracle/Makefile next to the compiled reference) through
     the engine's own loader, concatenated `copies` times so that the device-resident set (235 MB) is larger than the
-    126 MB L2 -- every step then reads its batch from HBM.  Falls back to synthetic MNIST-shaped bytes when the files
+    50 MB L2 -- every step then reads its batch from HBM.  Falls back to synthetic MNIST-shaped bytes when the files
     are absent.  Returns (images u8 [n,784], labels u8 [n], description)."""
     img, lab = os.path.join(MNIST_DIR, "train-images.idx3-ubyte"), os.path.join(MNIST_DIR, "train-labels.idx1-ubyte")
     if os.path.exists(img) and os.path.exists(lab):
@@ -213,7 +211,7 @@ def run_reference_arm(a):
 def conv_roofline(eng, pkg, stream, hbm_peak, peak_src, n_img=128, iters=10):
     """BASELINE.json's second metric: HBM GB/s of the conv forward + weight gradient + input gradient against the roofline, on
     configs[4] (synthetic 224x224x3 -> 64 filters 3x3, bf16 NHWC, valid padding; SURVEY.md 8d: 6,609,408 algorithmic bytes per
-    image per pass).  Every pass streams 846 MB (> 126 MB L2); CUDA events on the engine's stream, 3 warm-up launches."""
+    image per pass).  Every pass streams 846 MB (> 50 MB L2); CUDA events on the engine's stream, 3 warm-up launches."""
     import torch
     N, H, W, C, K, R, S = n_img, 224, 224, 3, 64, 3, 3
     P, Q = H - R + 1, W - S + 1
@@ -249,14 +247,14 @@ def conv_roofline(eng, pkg, stream, hbm_peak, peak_src, n_img=128, iters=10):
         out[name] = {"ms": ms, "GBps": gb, "frac": gb / hbm_peak}
     tot = ms_f + ms_w + ms_d
     gb = 3 * alg / (tot * 1e-3) / 1e9
-    return {"workload": "conv 224x224x3 -> 64x3x3, bf16 NHWC, tcgen05 kernels (BASELINE.json configs[4])", "images": N,
+    return {"workload": "conv 224x224x3 -> 64x3x3, bf16 NHWC, wgmma kernels (BASELINE.json configs[4])", "images": N,
             "algorithmic_bytes_per_pass": alg, "passes": out, "fwd_bwd": {"ms": tot, "GBps": gb, "frac": gb / hbm_peak},
             "peak": hbm_peak, "unit": "GB/s", "peak_source": peak_src, "l2": "846 MB per pass, larger than L2"}
 
 
 def reference_cuda_baseline(samples=20000):
-    """The reference's own GPU path (CUDA/main.cu + layer.cu, unmodified, built for sm_100a by oracle/Makefile) timed on
-    this B200 with a device synchronise around learn() -- batch 1, ~38 driver calls per image (SURVEY.md 2.2).  Baseline
+    """The reference's own GPU path (CUDA/main.cu + layer.cu, unmodified, built for sm_90a by oracle/Makefile) timed on
+    this H100 with a device synchronise around learn() -- batch 1, ~38 driver calls per image (SURVEY.md 2.2).  Baseline
     only: it is numerically wrong in two kernels and is never used as a checker."""
     exe = os.path.join(ROOT, "oracle", "_ref", "cuda_ref_bench")
     if not os.path.exists(exe):
@@ -267,10 +265,19 @@ def reference_cuda_baseline(samples=20000):
             if ln.startswith("REF_CUDA"):
                 kv = dict(x.split("=") for x in ln.split()[1:])
                 return {"value": float(kv["images_per_s"]), "unit": "images/s", "samples": int(kv["samples"]),
-                        "seconds": float(kv["seconds"]), "kind": "reference CUDA/ (unmodified, sm_100a, batch 1, device-synchronised wall clock)"}
+                        "seconds": float(kv["seconds"]), "kind": "reference CUDA/ (unmodified, sm_90a, batch 1, device-synchronised wall clock)"}
         return {"unavailable": (r.stderr or r.stdout)[-200:]}
     except Exception as exc:
         return {"unavailable": str(exc)[:200]}
+
+
+def dump_outputs(out_dir, eng):
+    """What the timed steps hand back: parameters after the last step, that step's packed gradient, the error sum."""
+    os.makedirs(out_dir, exist_ok=True)
+    eng.sync()
+    np.save(os.path.join(out_dir, "params.npy"), eng.get_params().astype(np.float32))
+    np.save(os.path.join(out_dir, "grads.npy"), eng.get_grads().astype(np.float32))
+    np.save(os.path.join(out_dir, "err_sum.npy"), np.array([eng.err_sum()], np.float64))
 
 
 def run_ours(a):
@@ -422,6 +429,8 @@ def run_ours(a):
     barrier()
     ms = e0.elapsed_time(e1)
     launches = eng.launch_count() - l0
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, eng)
     if world > 1:
         t = torch.tensor([ms], device="cuda")
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -525,9 +534,6 @@ def run_ours(a):
         roof = {"bound": "fp32_fma" if frac_f >= frac_h else "hbm",
                 "achieved": tf if frac_f >= frac_h else gbs, "peak": fp32_peak if frac_f >= frac_h else hbm_peak,
                 "unit": "TFLOP/s" if frac_f >= frac_h else "GB/s", "frac": max(frac_f, frac_h),
-                # dram__bytes_read.sum + dram__bytes_write.sum of this kernel per step, read from the summary that
-                # scripts/ncu_traffic.py wrote from the round's `ncu --set full` capture (null when no capture matches)
-                "traffic": measured_traffic("k_train_persist" if persistent else "k_fused", B, launch_steps),
                 "kernel": kernel, "kernel_ms": launch_ms,
                 "fp32": {"achieved": tf, "peak": fp32_peak, "unit": "TFLOP/s", "frac": frac_f,
                          "peak_source": "measured live (pcnn_measure_fp32_peak FFMA micro-benchmark)"},
@@ -585,6 +591,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=200)
     ap.add_argument("--batch", type=int, default=256, help="images per GPU per step (BASELINE.json configs[1]: 256)")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the timed steps' results (params, grads, err_sum) as .npy files into DIR")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-conv", action="store_true", help="skip the conv fwd+bwd roofline block (N = 1 only)")
     ap.add_argument("--persist-tune", type=int, default=0, help="pcnn_persist_tune knob (profiling runs: 2 = clusters without the cooperative attribute)")

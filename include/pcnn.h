@@ -1,5 +1,5 @@
 /*
- * include/pcnn.h -- C ABI of the B200-native LeNet/MNIST training engine (libpcnn.so).
+ * include/pcnn.h -- C ABI of the H100-native LeNet/MNIST training engine (libpcnn.so).
  *
  * This is the drop-in boundary for the hot path of Tamerkobba/Parallel-CNN: the 18 layer functions of
  * Sequential/layer.h and the driver entry points of Sequential/Main.cpp.  The reference has no FFI layer
@@ -14,7 +14,7 @@
  *   - "dev" pointers are CUDA device pointers on the context's device; "host" pointers are ordinary memory.
  *   - every call enqueues on the context's stream; only *_sync / *_d2h / get_* / *_host calls block.
  *   - one context per GPU, not thread-safe per context (the reference is single-threaded global state).
- *   - there is NO CPU fallback: on a machine without a usable sm_100 GPU pcnn_create fails with
+ *   - there is NO CPU fallback: on a machine without a usable sm_90 GPU pcnn_create fails with
  *     PCNN_ERR_NOGPU and nothing else computes.
  *
  * Packed parameter vector (PCNN_NPARAM = 2,343 floats), also the layout of the packed gradient:
@@ -54,7 +54,7 @@ typedef enum {
     PCNN_ERR_NCCL = -3,   /* NCCL missing or a collective failed */
     PCNN_ERR_STATE = -4,  /* call not valid in the current state (no dataset bound, comm not initialised...) */
     PCNN_ERR_IO = -5,     /* file problems other than the mnist_load codes */
-    PCNN_ERR_NOGPU = -6   /* no CUDA device / not compute capability 10.x */
+    PCNN_ERR_NOGPU = -6   /* no CUDA device / not compute capability 9.0 */
 } pcnn_status;
 
 #define PCNN_MAX_PEERS 8   /* GPUs of one NVSwitch domain the in-kernel gradient exchange addresses */
@@ -185,15 +185,16 @@ int pcnn_measure_fp32_peak(pcnn_ctx *ctx, float *tflops_out);
 int pcnn_measure_tma_read(pcnn_ctx *ctx, const void *dev_bf16, int N, int P, int Q, int mode, int iters, float *gbps_out);
 /* store rate (GB/s) of the forward convolution's epilogue with everything but the stores removed: y viewed as [N][P][row_elems]
  * bf16, tiles of 128 rows x 256 columns walked like the forward kernel (image height H on the input side, H % 32 == 0).  mode 0 =
- * the kernel's own pattern (boxes {64 columns, 32 rows}, 128-byte swizzle), 1 / 2 = boxes of 128 / 256 columns without swizzle,
- * 3 = per-row 1-D bulk stores of 128 bytes, 4 = four boxes per commit group, 5 = 32-byte st.global.v8 from registers (no TMA),
+ * boxes {64 columns, 32 rows} with 128-byte swizzle, 1 / 2 = boxes of 128 / 256 columns without swizzle,
+ * 3 = per-row 1-D bulk stores of 128 bytes, 4 = four boxes per commit group, 5 = 16-byte st.global.v4 from registers (no TMA),
  * 6 = half TMA boxes, half direct stores; hot = 1 aims every tile at the first row block (an
  * L2-resident target).  The ceiling the forward kernel's store phase is measured against.  The tensor is OVERWRITTEN with
  * unspecified values (the staging buffers are never filled). */
 int pcnn_measure_tma_write(pcnn_ctx *ctx, void *dev_bf16, int N, int P, int H, int row_elems, int mode, int hot, int iters, float *gbps_out);
-/* SM clocks per tcgen05.mma (kind::f16 bf16, K = 16, shape M x N, operands K- or MN-major in shared memory) when one thread
- * issues `reps` of them back to back over `nacc` rotating accumulators: the issue-rate table the convolution kernels are
- * designed against (small-N instructions are far from the tensor-pipe peak). */
+/* SM clocks per M x N x 16 bf16 product on the wgmma tensor cores (operands K- or MN-major in shared memory) when each of the
+ * M / 64 warpgroups issues `reps` m64nNk16 back to back into one register accumulator: the issue-rate table the convolution
+ * kernels are designed against (small-N instructions are far from the tensor-pipe peak).  `nacc` (1, 2, 4, 8 with
+ * N * nacc <= 512) is validated only: register accumulators are not rotated. */
 int pcnn_measure_mma_rate(pcnn_ctx *ctx, int M, int N, int a_mn_major, int b_mn_major, int nacc, int reps, float *clk_per_mma);
 
 /* ------------------------------------------------------------------ data parallelism (not in the reference; SURVEY.md 8e)
@@ -223,8 +224,7 @@ int pcnn_set_step_mode(pcnn_ctx *ctx, int mode);
  * pcnn_learn_host enqueue its host copies BEFORE the kernel launch (needed wherever launches block the calling thread:
  * kernel-replay profilers; CUDA_LAUNCH_BLOCKING=1 is detected by itself); bit 3 keeps the two-stage gradient exchange on 2
  * GPUs (default there: cluster shares stored straight into the peer's memory); bit 4 sends pinned host images of
- * pcnn_learn_host through the staged copy stream instead of letting the kernel pull them.  Measurement knobs for the runs
- * under profiles/.
+ * pcnn_learn_host through the staged copy stream instead of letting the kernel pull them.  Measurement knobs for A/B runs.
  * out6[5] of pcnn_persist_info: bit 0 = cooperative launch, bit 1 = direct exchange used. */
 int pcnn_persist_info(pcnn_ctx *ctx, int *out6);
 int pcnn_persist_tune(pcnn_ctx *ctx, int max_cluster);
@@ -262,7 +262,7 @@ int pcnn_l5_forward(pcnn_ctx *ctx, const float *params_dev, const void *images_d
 
 /* ------------------------------------------------------------------ bf16 tensor-core convolution (SURVEY.md x3; BASELINE configs 3, 5)
  * The reference's conv semantics (valid, stride 1, cross-correlation, layer.h:118-130) generalised to C input channels,
- * K filters of R x S taps, on tcgen05 tensor cores with TMEM accumulators and TMA-fed operands (csrc/conv_tc.cu).
+ * K filters of R x S taps, on the wgmma tensor cores with register accumulators and TMA-fed operands (csrc/conv_tc.cu).
  * Activations are NHWC bf16 with a row pitch of `row_pitch` elements (>= W*C, multiple of 8); filters fp32 KRSC on the
  * host (rounded to bf16 once, at plan creation); output NHWC bf16 [N][H-R+1][W-S+1][K], bias and optional sigmoid fused.
  * Constraint of this round: some pixel block Qt with (Qt+S-1)*C <= 32, Qt*K <= 256 and Qt*K % 16 == 0 must exist
@@ -281,14 +281,14 @@ int pcnn_conv_tc_plan_create_strided(pcnn_ctx *ctx, int N, int H, int W, int C, 
                                      pcnn_conv_plan **plan_out);
 int pcnn_conv_tc_plan_destroy(pcnn_ctx *ctx, pcnn_conv_plan *plan);
 int pcnn_conv_tc_fwd(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *x_bf16_dev, void *y_bf16_dev);
-/* Backward passes of the same convolution (bf16 operands, fp32 accumulation, deterministic; tcgen05 kernels, see
+/* Backward passes of the same convolution (bf16 operands, fp32 accumulation, deterministic; wgmma kernels, see
  * pcnn_conv_bwd_select): weight gradient fp32 KRSC [ref: layer.h:371-395 bp_weight_c1, without its /576] and input gradient
  * bf16 NHWC in x's layout.  row_pitch / image_rows as for the forward plan (0 = dense). */
 int pcnn_conv_wgrad(pcnn_ctx *ctx, const void *x_bf16_dev, const void *dy_bf16_dev, float *dw_f32_dev, int N, int H, int W, int C,
                     int K, int R, int S, int row_pitch, int image_rows);
 int pcnn_conv_dgrad(pcnn_ctx *ctx, const void *dy_bf16_dev, const float *filt_f32_dev, void *dx_bf16_dev, int N, int H, int W,
                     int C, int K, int R, int S, int row_pitch, int image_rows);
-/* Which kernels pcnn_conv_wgrad / pcnn_conv_dgrad may use.  PCNN_CONV_BWD_TENSOR (default): the tcgen05 kernels only (any filter
+/* Which kernels pcnn_conv_wgrad / pcnn_conv_dgrad may use.  PCNN_CONV_BWD_TENSOR (default): the wgmma kernels only (any filter
  * count up to 256: counts that are not a multiple of 64 are zero-padded to one in an extra pass over dy) -- a shape they
  * cannot take is an ERROR (PCNN_ERR_ARG naming the restriction), never a silent detour.  PCNN_CONV_BWD_REFERENCE: the
  * deterministic FMA-pipe kernels of csrc/conv_bwd.cu for every shape (any C, K, taps): a second implementation the tests
@@ -297,7 +297,7 @@ typedef enum { PCNN_CONV_BWD_TENSOR = 0, PCNN_CONV_BWD_REFERENCE = 1 } pcnn_conv
 int pcnn_conv_bwd_select(pcnn_ctx *ctx, int path);
 /* Host-only query (works without a GPU): which kernels pcnn_conv_wgrad / pcnn_conv_dgrad pick for a shape and how they tile it.
  * out9 = { wgrad on tensor cores, dy rows per tile, pixels per tile, stages,
- *          dgrad on tensor cores, column strips, output pixels per lane quarter, TMEM slot groups in flight, stages } */
+ *          dgrad on tensor cores, column strips, output pixels per lane quarter, partial dx rows kept in registers (R), stages } */
 int pcnn_conv_bwd_plan_info(int N, int H, int W, int C, int K, int R, int S, int *out9);
 /* Zero padding for the valid-padding kernels above (SURVEY.md 8f row 4): pcnn_pad_nhwc_bf16 embeds dense [N][H][W][C] images into
  * a zeroed canvas [N][dst_image_rows][dst_row_pitch] at row offset pad_h, pixel offset pad_w (0 = the tight canvas

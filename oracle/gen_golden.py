@@ -9,6 +9,9 @@ output of the reference's own code on real MNIST bytes:
   reference_vectors.npz  seed-1 parameters, per-sample activations / backward buffers, parameter states after
                          1, 1000 and 60000 steps, per-step error norms, classifications
   reference_scalars.json the SURVEY.md Appendix B numbers re-measured here (err, error rate, sums, FNV hashes)
+  reference_ops_random.json SHA-256 of the bits of every operator of layer.h on seeded random inputs (oracle_lib.ops_chain)
+
+`gen_golden.py ops` writes only reference_ops_random.json.
 """
 import json
 import os
@@ -23,10 +26,19 @@ import oracle_lib as O  # noqa: E402
 N_TRAIN_SUB, N_TEST_SUB = 1024, 256
 
 
+def ops_golden(ref):
+    digests = {k: O.bits_digest(v) for k, v in O.ops_chain(ref, reference=True).items()}
+    with open(os.path.join(O.GOLDEN, "reference_ops_random.json"), "w") as f:
+        json.dump(digests, f, indent=1, sort_keys=True)
+
+
 def main():
     ref = O.reference()
     if ref is None:
-        raise SystemExit("oracle/_ref/libref_seq.so missing: run `make -C oracle` where /root/reference exists")
+        raise SystemExit("oracle/_ref/libref_seq.so missing: run `make -C oracle` where the reference sources exist")
+    ops_golden(ref)
+    if sys.argv[1:] == ["ops"]:
+        return
     data = O.full_mnist()
     if data is None:
         raise SystemExit("oracle/_ref/data missing")

@@ -1,7 +1,7 @@
 // oracle/ref_cuda_harness.cu -- TEST / BASELINE INFRASTRUCTURE ONLY (never linked into the product).
 //
 // Times the reference's OWN GPU path (CUDA/main.cu + CUDA/layer.cu, unmodified, compiled where they lie under
-// /root/reference for sm_100a) on the same B200 as the engine: the only GPU-vs-GPU anchor this project has
+// the reference sources for sm_90a) on the same H100 as the engine: the only GPU-vs-GPU anchor this project has
 // (BASELINE.md section 3.4, SURVEY.md 2.2).  The reference's own timer wraps asynchronous launches with clock() and never
 // synchronises (CUDA/main.cu:71-72, 107-108, 115-117, 160-161), so this harness brackets learn() with
 // cudaDeviceSynchronize() and a wall clock instead.  main.cu is included as a translation unit with its main() renamed,

@@ -1,9 +1,9 @@
 """parallel-cnn_b200 -- Python host mirror of the libpcnn.so C ABI (include/pcnn.h).
 
-The product is the CUDA library built from csrc/ (hand-written sm_100a kernels behind a plain C ABI that replaces
+The product is the CUDA library built from csrc/ (hand-written sm_90a kernels behind a plain C ABI that replaces
 /root/reference/Sequential/layer.h + Main.cpp for the LeNet/MNIST training path).  This module only binds that ABI
 with ctypes so tests, bench.py and __graft_entry__ can drive it; it carries NO compute of its own and NO CPU
-fallback: if libpcnn.so is missing or no sm_100 GPU is present, every compute entry point raises.
+fallback: if libpcnn.so is missing or no sm_90 GPU is present, every compute entry point raises.
 
 The directory name contains a hyphen, so import it through ``pcnn_loader.load()`` at the repo root (which registers
 it as the module ``parallel_cnn_b200``).

@@ -1,7 +1,7 @@
 // parallel-cnn_b200/csrc/conv_bwd.cu -- weight- and input-gradient of the generic NHWC bf16 convolution (SURVEY.md x3).
 //
 // Entry points + the general-shape kernels on the fp32 FMA pipe (bf16 operands, fp32 accumulation, deterministic two-stage
-// reduction, no atomics).  Shapes the tensor cores can take (64 filters; conv_wgrad_tc.cu, conv_dgrad_tc.cu) are routed to the tcgen05
+// reduction, no atomics).  Shapes the tensor cores can take (64 filters; conv_wgrad_tc.cu, conv_dgrad_tc.cu) are routed to the wgmma
 // kernels, which are the roofline path: both passes move the same 6.6 MB/image as the forward pass (config 5) and are
 // HBM-bound at 170 MFLOP per 6.6 MB, which the FMA pipe cannot sustain (SURVEY.md 8d).  PCNN_CONV_BWD=fma forces the
 // FMA-pipe kernels (used by the tests to check both paths against the oracle).
@@ -350,7 +350,7 @@ extern "C" int pcnn_crop_nhwc_bf16(pcnn_ctx *ctx, const void *src_bf16, void *ds
 // Which kernels the backward entry points would pick for a shape and how they tile it (pure host logic, no device needed):
 // out[0] = weight gradient on the tensor cores (0/1), out[1..3] = its dy rows per tile, pixels per tile, stages;
 // out[4] = input gradient on the tensor cores (0/1), out[5..8] = its column strips, output pixels per lane quarter,
-// TMEM slot groups in flight, stages.  Pointer alignment and row pitch are assumed to qualify (16 bytes, multiple of 8).
+// partial dx rows each consumer thread keeps in registers (R), stages.  Pointer alignment and row pitch are assumed to qualify (16 bytes, multiple of 8).
 extern "C" int pcnn_conv_bwd_plan_info(int N, int H, int W, int C, int K, int R, int S, int *out9) {
     PCNN_REQUIRE(out9 && N > 0 && H >= R && W >= S && C > 0 && K > 0 && R > 0 && S > 0, PCNN_ERR_ARG, "pcnn_conv_bwd_plan_info: bad argument");
     for (int i = 0; i < 9; ++i) out9[i] = 0;

@@ -2,26 +2,20 @@
 //
 //     dx[n][h][w][c] = sum_{k,r,s} dy[n][h-r][w-s][k] * f[k][r][s][c]
 //
-// Access pattern first: a first version put 128 dy ROWS of one pixel column on the TMEM lanes (col2im folded into the TMEM
-// column offset); its TMA boxes gathered 128-byte pieces of 128 different rows, and a TMA pipeline with that pattern tops
-// out at 3.6-4.4 TB/s on B200 (pcnn_measure_tma_read, mode 2) against 6.7-7.1 TB/s for contiguous boxes -- the kernel sat
-// exactly on that ceiling (4.6 TB/s, profiles/r01_README.md).  Here every TMA box is a contiguous run of one dy row:
-//   (More than 64 filters: K/64 channel groups per dy row -- K/64 x 4 boxes per stage and K/64 x 4 MMAs per row; K <= 256.)
+// Access pattern first: every TMA box is a contiguous run of one dy row (pcnn_measure_tma_read mode 3 measures that pattern;
+// mode 2, boxes gathering 128-byte pieces of different rows, is the alternative it was chosen over).
+//   (More than 64 filters: K/64 channel groups per dy row -- K/64 x 4 boxes per stage and K/64 x 4 MMA steps per row; K <= 256.)
 //   * A CTA owns a strip of <= 120 output columns and walks DOWN the rows of its share of the images.  One dy row of the
-//     strip is an A operand [128 pixels x 64 channels] (4 boxes of <= 32 pixels, one per TMEM lane quarter, overlapping by
-//     S-1 pixels so that the shift along s never crosses a warp).
-//   * The accumulator is a RING OF OUTPUT ROWS in TMEM: slot t holds dx row t of the walk as SCP = 4*ceil(S*C/4) columns
-//     (s, c).  dy row p contributes to rows p .. p+R-1, i.e. to R consecutive slots = one window of R*SCP columns, so the sum
-//     over r is done by the tensor core (4 MMAs M=128, N=48, K=16 per dy row against a constant 6 KB filter matrix whose
-//     columns are (r, s, c)) and the window slides by one slot per row.  Row t is complete once dy row t has been added; it
-//     is then drained by the epilogue (sum over s = a shuffle across lanes, bf16, coalesced store) and re-zeroed.
-//   * Flow control is per group of 8 slots (tcgen05.commit -> tfull, epilogue -> tempty), NG groups in flight.
-//   * A CTA's share starts mid-image in general: the R-1 rows above it are replayed with filter variants that keep only the
-//     contributions landing inside the share (0.5 % extra reads at config 5).
-// TMEM addressing: the accumulator window of a tcgen05.mma must start on a multiple of 4 columns (an arbitrary column faults
-// with "misaligned address" on B200), hence SCP = 4*ceil(S*C/4) columns per slot.
-// Issue budget (pcnn_measure_mma_rate): one tcgen05.mma of N <= 112 occupies the issue/tensor path ~56-70 clk whatever its
-// size, so 4 MMAs per 15 KB of dy fit under the ~630 clk of HBM time those bytes cost one SM.
+//     strip is an A operand [128 pixels x 64 channels] (4 boxes of <= 32 pixels, one per lane quarter, overlapping by
+//     S-1 pixels so that the shift along s never crosses a quarter).
+//   * Two warpgroups multiply it (64 pixels each) with a constant filter matrix whose N = NW columns are (r, s, c):
+//     D[pixel][(r, s, c)] = sum_k dy[pixel][k] f[k][r][s][c], fresh for every dy row (wgmma, register accumulators).
+//   * dy row p contributes to dx rows p .. p+R-1.  Each consumer thread owns a few (pixel, c) outputs of the strip and keeps
+//     R partial rows of them in registers (a ring): after dy row p it adds sum_s D[pixel + S-1-s][(r, s, c)] to partial row
+//     r, writes partial row 0 (= dx row p, now complete) and shifts the ring by one row.  D passes through shared memory
+//     because the shift along s crosses the accumulator's register layout.
+//   * A CTA's share starts mid-image in general: the R-1 dy rows above it are replayed and only the rows of the share are
+//     written (0.5 % extra reads at config 5).
 #include "tc_common.cuh"
 
 #include <stdlib.h>
@@ -30,17 +24,16 @@ using namespace pcnn_tc;
 
 namespace {
 
-constexpr int D2_THREADS = 192;          // warp 0 TMA producer, warp 1 MMA issuer + TMEM owner, warps 2-5 epilogue (lane quarters)
+constexpr int D2_THREADS = 288;          // warps 0-7 two consumer warpgroups, warp 8 TMA producer
+constexpr int D2_CONSUMERS = 256;
 constexpr int D2_HALF_BYTES = 16384;     // one group of 64 channels: 4 quarters x 32 pixel rows x 128 B
 constexpr int D2_MAX_STAGES = 11;
-constexpr int D2_MAX_NG = 6;
-constexpr int D2_GROUP = 8;
-constexpr int D2_SMEM_BUDGET = 200 * 1024;
+constexpr int D2_SMEM_BUDGET = 225 * 1024;
 
 struct Dgrad2Params {
     int n_img, H, W, P, Q;
     int nstrips, strip_w, oq, bp;        // strips per row, output columns per strip / per lane quarter, pixels per TMA box
-    int ng, ring, stages;                // slot groups in flight, ring slots (8 * ng), smem stages
+    int stages;                          // smem stages
     int KH;                              // channels / 64: a TMA box holds 64 channels (one 128-byte swizzle row per pixel)
     long long T;                         // n_img * H output rows in walk order
     long long dx_pitch, dx_image_rows;
@@ -48,29 +41,24 @@ struct Dgrad2Params {
 };
 
 struct Dgrad2Ctl {
-    unsigned long long full[D2_MAX_STAGES], empty[D2_MAX_STAGES], tfull[D2_MAX_NG], tempty[D2_MAX_NG], bfull;
-    uint32_t tmem_base;
+    unsigned long long full[D2_MAX_STAGES], empty[D2_MAX_STAGES], bfull;
 };
 
-// F_v[n][k] for window column n = r' * SCP + s * C + c: f[k][r' + v][s][c] (variant v drops the first v filter rows), zero padding
-// layout [variant][channel group of 64][nw][64]
-__global__ void k_dgrad2_build_variants(const float *__restrict__ f, __nv_bfloat16 *__restrict__ T, int nw, int scp, int K, int R, int S,
-                                        int C) {
-    const int total = R * nw * K, KH = K / 64;
+// F[kh][n][kl] for column n = r * S * C + s * C + c: f[kh * 64 + kl][r][s][c], zero past R * S * C
+__global__ void k_dgrad2_build_filter(const float *__restrict__ f, __nv_bfloat16 *__restrict__ T, int nw, int K, int R, int S, int C) {
+    const int total = nw * K;
     for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += gridDim.x * blockDim.x) {
-        const int kl = idx % 64, n = (idx / 64) % nw, kh = (idx / (64 * nw)) % KH, v = idx / (64 * nw * KH), k = kh * 64 + kl;
-        const int r = n / scp + v, j = n % scp;
+        const int kl = idx % 64, n = (idx / 64) % nw, kh = idx / (64 * nw), k = kh * 64 + kl;
         float val = 0.0f;
-        if (r < R && j < S * C) val = f[(((long)k * R + r) * S + j / C) * C + j % C];
+        if (n < R * S * C) val = f[(long)k * R * S * C + n];
         T[idx] = __float2bfloat16_rn(val);
     }
 }
 
-// the rows one CTA feeds to the tensor core, in order: R-1 replayed rows above its share, then its own rows
+// the rows one CTA walks, in order: R-1 replayed rows above its share, then its own rows
 struct RowWalk {
     long long t0, t1;       // share [t0, t1) of the walk
-    int H, P;
-    __device__ RowWalk(const Dgrad2Params &p, int idx, int cnt) : H(p.H), P(p.P) {
+    __device__ RowWalk(const Dgrad2Params &p, int idx, int cnt) {
         const long long L = (p.T + cnt - 1) / cnt;
         t0 = (long long)idx * L;
         t1 = t0 + L < p.T ? t0 + L : p.T;
@@ -78,20 +66,26 @@ struct RowWalk {
     }
 };
 
+template <int R, int S, int C> struct DgradShape {
+    static constexpr int SC = S * C, NW = (R * SC + 15) / 16 * 16, DST = NW + 4;   // D staging row stride (floats)
+    static constexpr int ITEMS = (4 * 32 * C + D2_CONSUMERS - 1) / D2_CONSUMERS;   // (quarter, pixel, c) outputs per thread
+};
+
 template <int R, int S, int C, int KHC>
 __global__ void __launch_bounds__(D2_THREADS, 1)
 k_conv_tc_dgrad_rows(const __grid_constant__ CUtensorMap map_dy, const __grid_constant__ CUtensorMap map_b, const Dgrad2Params p) {
-    constexpr int SC = S * C, SCP = (SC + 3) / 4 * 4, NW = (R * SCP + 15) / 16 * 16;
+    using SH = DgradShape<R, S, C>;
+    constexpr int SC = SH::SC, NW = SH::NW, DST = SH::DST, ITEMS = SH::ITEMS;
     extern __shared__ unsigned char smem_dyn[];
     unsigned char *base = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
     constexpr int BMAT = NW * 128;
-    // KHC > 0: the channel-group count is a compile-time constant (64 filters: KHC = 1 keeps the single issuing thread's loop
-    // free of the group bookkeeping -- the runtime loop cost 146 -> 187 us at config 5); KHC = 0: p.KH groups at run time
+    // KHC > 0: the channel-group count is a compile-time constant; KHC = 0: p.KH groups at run time
     const int KH = KHC > 0 ? KHC : p.KH, STAGE = KH * D2_HALF_BYTES;
-    unsigned char *bvar = base;                                         // [R][KH][NW][64] bf16, SWIZZLE_128B
-    unsigned char *astage = base + (size_t)R * KH * BMAT;               // [stages][KH][4][32][64] bf16, SWIZZLE_128B
-    Dgrad2Ctl &B = *reinterpret_cast<Dgrad2Ctl *>(astage + (size_t)p.stages * STAGE);
-    const int NST = p.stages, NG = p.ng, RING = p.ring;
+    unsigned char *bmat = base;                                         // [KH][NW][64] bf16, SWIZZLE_128B
+    unsigned char *astage = base + (size_t)KH * BMAT;                   // [stages][KH][4][32][64] bf16, SWIZZLE_128B
+    float *dst = reinterpret_cast<float *>(astage + (size_t)p.stages * STAGE);   // [128][DST] fp32
+    Dgrad2Ctl &B = *reinterpret_cast<Dgrad2Ctl *>(dst + 128 * DST);
+    const int NST = p.stages;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     // this CTA's strip of output columns and its share of the row walk
@@ -104,40 +98,27 @@ k_conv_tc_dgrad_rows(const __grid_constant__ CUtensorMap map_dy, const __grid_co
     const int h_first = (int)(walk.t0 % p.H);
     const int n_first = (int)(walk.t0 / p.H);
     const int warm = h_first < R - 1 ? h_first : R - 1;               // replayed rows above the share (same image)
+    const long long nrows = nel + warm;
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < NST; ++i) { bar_init(&B.full[i], 1); bar_init(&B.empty[i], 1); }
-        for (int i = 0; i < NG; ++i) { bar_init(&B.tfull[i], 1); bar_init(&B.tempty[i], 4); }
+        for (int i = 0; i < NST; ++i) { bar_init(&B.full[i], 1); bar_init(&B.empty[i], D2_CONSUMERS / 32); }
         bar_init(&B.bfull, 1);
         fence_barrier_init();
     }
-    // pixel rows a box does not cover (box of bp < 32 pixels) must hold finite values: their TMEM lanes are never read
+    // pixel rows a box does not cover (box of bp < 32 pixels) must hold finite values: their D rows are never read
     for (int i = threadIdx.x * 16; i < NST * STAGE; i += D2_THREADS * 16) *reinterpret_cast<uint4 *>(astage + i) = make_uint4(0, 0, 0, 0);
     fence_proxy_async_smem();
-    if (warp == 1) tc_alloc(&B.tmem_base, 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = B.tmem_base;
-    if (warp >= 2) {   // every MMA accumulates: the whole ring starts at zero
-        const uint32_t t0 = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-#pragma unroll
-        for (int ch = 0; ch < 16; ++ch) tc_st_zero_32x32(t0 + ch * 32);
-        tc_wait_st();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
+    if (nel <= 0) return;
 
-    if (warp == 0) {
+    if (warp == D2_CONSUMERS / 32) {
         // ===== TMA producer =====
-        if (lane == 0 && nel > 0) {
-            bar_expect_tx(&B.bfull, (unsigned)(R * KH * BMAT));
-            for (int v = 0; v < R * KH; ++v) tma_load_2d(bvar + (size_t)v * BMAT, &map_b, 0, v * NW, &B.bfull);
+        if (lane == 0) {
+            bar_expect_tx(&B.bfull, (unsigned)(KH * BMAT));
+            for (int kh = 0; kh < KH; ++kh) tma_load_2d(bmat + (size_t)kh * BMAT, &map_b, 0, kh * NW, &B.bfull);
             int stage = 0;
             unsigned ph = 0;
             int n = n_first, h = h_first - warm;
-            const long long nrows = nel + warm;
             for (long long i = 0; i < nrows; ++i) {
                 if (h < p.P) {
                     bar_wait_relaxed(&B.empty[stage], ph ^ 1u, 32);
@@ -153,127 +134,97 @@ k_conv_tc_dgrad_rows(const __grid_constant__ CUtensorMap map_dy, const __grid_co
                 if (++h == p.H) { h = 0; ++n; }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        if (lane == 0 && nel > 0) {
-            const uint32_t idesc = umma_idesc_bf16(128, NW);
-            const uint64_t adesc0 = umma_desc_k_sw128(s_u32(astage)), bdesc0 = umma_desc_k_sw128(s_u32(bvar));
-            bar_wait(&B.bfull, 0);
-            int stage = 0;
-            unsigned ph = 0;
-            int h = h_first - warm;
-            int pos = 0;                                   // ring slot of the current element
-            int G = 0, ing = 0;                            // group index, elements done in it
-            const long long nrows = nel + warm;
-            for (long long i = 0; i < nrows; ++i) {
-                const bool warmrow = i < warm;
-                if (!warmrow && ing == 0 && G + 1 >= NG) {
-                    // the windows of group G reach into ring group (G + 1) % NG: its previous occupant must be drained
-                    const int rg = (G + 1) % NG;
-                    bar_wait(&B.tempty[rg], (unsigned)(((G + 1) / NG - 1) & 1));
-                    tc_fence_after();
-                }
-                if (h < p.P) {
-                    bar_wait(&B.full[stage], ph);
-                    tc_fence_after();
-                    uint64_t ad = adesc0 + (uint64_t)((uint32_t)stage * ((uint32_t)STAGE >> 4));
-                    uint64_t bd = bdesc0 + (uint64_t)((uint32_t)(warmrow ? warm - (int)i : 0) * ((uint32_t)(KH * BMAT) >> 4));
-                    const uint32_t dcol = tmem + (uint32_t)(pos * SCP);
-                    for (int kh = 0; kh < KH; ++kh) {          // 64 channels = 4 K steps of 16
-#pragma unroll
-                        for (int ks = 0; ks < 4; ++ks) tc_mma_bf16(dcol, ad + (uint64_t)(ks * 2), bd + (uint64_t)(ks * 2), idesc, 1u);
-                        ad += D2_HALF_BYTES >> 4;
-                        bd += BMAT >> 4;
-                    }
-                    tc_commit(&B.empty[stage]);
-                    if (++stage == NST) { stage = 0; ph ^= 1u; }
-                }
-                if (++h == p.H) h = 0;
-                if (!warmrow) {
-                    if (++ing == D2_GROUP || i == nrows - 1) {
-                        tc_commit(&B.tfull[G % NG]);
-                        ++G;
-                        ing = 0;
-                    }
-                    if (++pos == RING) pos = 0;
-                }
-            }
-        }
-    } else {
-        // ===== epilogue: drain completed rows, sum over s across lanes, store, re-zero =====
-        const int quarter = warp & 3;
-        const uint32_t tq = tmem + ((uint32_t)(quarter * 32) << 16);
-        const int w_q0 = w_strip + quarter * p.oq;
-        int nvalid = w_end - w_q0;                           // output pixels of this quarter
-        if (nvalid > p.oq) nvalid = p.oq;
-        int n = n_first, h = h_first, pos = 0;
-        const int ngroups = (int)((nel + D2_GROUP - 1) / D2_GROUP);
-        for (int G = 0; G < ngroups; ++G) {
-            bar_wait_relaxed(&B.tfull[G % NG], (unsigned)((G / NG) & 1), 64);
-            tc_fence_after();
-            long long left = nel - (long long)G * D2_GROUP;
-            const int nsl = left < D2_GROUP ? (int)left : D2_GROUP;
-            for (int i = 0; i < nsl; ++i) {
-                uint32_t v[SCP], u[SCP];
-                const uint32_t c0 = tq + (uint32_t)(pos * SCP);
-#pragma unroll
-                for (int j = 0; j < SCP; j += 4) tc_ld_32x4(c0 + j, v[j], v[j + 1], v[j + 2], v[j + 3]);
-                const bool tail = pos < R - 1;               // rows written past the ring end by the previous lap
-                if (tail) {
-#pragma unroll
-                    for (int j = 0; j < SCP; j += 4) tc_ld_32x4(tq + (uint32_t)((RING + pos) * SCP) + j, u[j], u[j + 1], u[j + 2], u[j + 3]);
-                }
-                tc_wait_ld();
-                float o[C];
-#pragma unroll
-                for (int c = 0; c < C; ++c) o[c] = 0.0f;
-#pragma unroll
-                for (int s = 0; s < S; ++s) {
-#pragma unroll
-                    for (int c = 0; c < C; ++c) {
-                        float x = __uint_as_float(v[s * C + c]);
-                        if (tail) x += __uint_as_float(u[s * C + c]);
-                        // lane l holds dy pixel (first + l); output pixel l of the quarter needs dy pixel l + (S-1) - s
-                        if (S - 1 - s > 0) x = __shfl_down_sync(0xFFFFFFFFu, x, S - 1 - s);
-                        o[c] += x;
-                    }
-                }
-                if (lane < nvalid) {
-                    __nv_bfloat16 *dst = p.dx + ((long long)n * p.dx_image_rows + h) * p.dx_pitch + (long long)(w_q0 + lane) * C;
-#pragma unroll
-                    for (int c = 0; c < C; ++c) dst[c] = __float2bfloat16_rn(o[c]);
-                }
-#pragma unroll
-                for (int j = 0; j < SCP; j += 4) tc_st_zero_32x4(c0 + j);
-                if (tail) {
-#pragma unroll
-                    for (int j = 0; j < SCP; j += 4) tc_st_zero_32x4(tq + (uint32_t)((RING + pos) * SCP) + j);
-                }
-                if (++pos == RING) pos = 0;
-                if (++h == p.H) { h = 0; ++n; }
-            }
-            tc_wait_st();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) bar_arrive(&B.tempty[G % NG]);
-        }
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tc_dealloc(tmem, 512);
+
+    // ===== consumers: D = dy row x F on the tensor cores, then the ring of partial dx rows in registers =====
+    const int tid = threadIdx.x, wg = warp >> 2, wq = warp & 3;
+    int it_q[ITEMS], it_l[ITEMS], it_c[ITEMS];
+    bool it_ok[ITEMS];
+    float ring[ITEMS][R];
+#pragma unroll
+    for (int k = 0; k < ITEMS; ++k) {
+        const int item = tid + k * D2_CONSUMERS;
+        it_q[k] = item / (32 * C);
+        it_l[k] = (item / C) % 32;
+        it_c[k] = item % C;
+        int nvalid = w_end - (w_strip + it_q[k] * p.oq);
+        if (nvalid > p.oq) nvalid = p.oq;
+        it_ok[k] = item < 4 * 32 * C && it_l[k] < nvalid;
+#pragma unroll
+        for (int r = 0; r < R; ++r) ring[k][r] = 0.0f;
+    }
+    bar_wait(&B.bfull, 0);
+    const uint32_t b0 = s_u32(bmat), a_base = s_u32(astage) + (uint32_t)(wg * 64 * 128);
+    int stage = 0;
+    unsigned ph = 0;
+    int n = n_first, h = h_first - warm;
+    for (long long i = 0; i < nrows; ++i) {
+        if (h < p.P) {
+            float acc[NW / 2];
+            bar_wait(&B.full[stage], ph);
+            wg_fence();
+            for (int kh = 0; kh < KH; ++kh) {          // 64 channels = 4 K steps of 16
+                const uint32_t a0 = a_base + (uint32_t)(stage * STAGE + kh * D2_HALF_BYTES), bk = b0 + (uint32_t)(kh * BMAT);
+#pragma unroll
+                for (int ks = 0; ks < 4; ++ks)
+                    wgmma_bf16<0, 0>(acc, gmma_desc_k_sw128(a0 + ks * 32), gmma_desc_k_sw128(bk + ks * 32), (kh | ks) != 0 ? 1u : 0u);
+            }
+            wg_commit();
+            wg_wait<0>();
+            wg_hold(acc);
+            __syncwarp();
+            if (lane == 0) bar_arrive(&B.empty[stage]);
+            if (++stage == NST) { stage = 0; ph ^= 1u; }
+#pragma unroll
+            for (int j = 0; j < NW / 8; ++j)
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+                    const int row = wg * 64 + wg_row(2 * hh, wq, lane), col = wg_col(4 * j, lane);
+                    *reinterpret_cast<float2 *>(dst + row * DST + col) = make_float2(acc[4 * j + 2 * hh], acc[4 * j + 2 * hh + 1]);
+                }
+            asm volatile("bar.sync 1, %0;" ::"n"(D2_CONSUMERS) : "memory");
+#pragma unroll
+            for (int k = 0; k < ITEMS; ++k) {
+                // lane l of quarter g holds dy pixel (first + l); output pixel l needs dy pixel l + (S-1) - s
+                const float *d = dst + (it_q[k] * 32 + it_l[k]) * DST + it_c[k];
+                if (it_ok[k]) {
+#pragma unroll
+                    for (int r = 0; r < R; ++r) {
+                        float t = 0.0f;
+#pragma unroll
+                        for (int s = 0; s < S; ++s) t += d[(S - 1 - s) * DST + r * SC + s * C];
+                        ring[k][r] += t;
+                    }
+                }
+            }
+            asm volatile("bar.sync 1, %0;" ::"n"(D2_CONSUMERS) : "memory");   // D staging free for the next row
+        }
+        // dx row h is complete (its last contribution is dy row h); rows above the share are not this CTA's
+        if (i >= warm) {
+#pragma unroll
+            for (int k = 0; k < ITEMS; ++k)
+                if (it_ok[k])
+                    p.dx[((long long)n * p.dx_image_rows + h) * p.dx_pitch + (long long)(w_strip + it_q[k] * p.oq + it_l[k]) * C + it_c[k]] =
+                        __float2bfloat16_rn(ring[k][0]);
+        }
+#pragma unroll
+        for (int k = 0; k < ITEMS; ++k) {
+#pragma unroll
+            for (int r = 0; r + 1 < R; ++r) ring[k][r] = ring[k][r + 1];
+            ring[k][R - 1] = 0.0f;
+        }
+        if (++h == p.H) { h = 0; ++n; }
     }
 }
 
-struct Geometry { int scp, nw, ng; };
+// NW (filter-matrix columns) and the shared-memory bytes that do not depend on the stage count
+struct Geometry { int nw; size_t fixed; };
 
-Geometry geometry(int R, int S, int C) {
+Geometry geometry(int R, int S, int C, int KH) {
     Geometry g;
-    g.scp = (S * C + 3) / 4 * 4;
-    g.nw = (R * g.scp + 15) / 16 * 16;
-    g.ng = 0;
-    while (g.ng < D2_MAX_NG && (D2_GROUP * (g.ng + 1) + R - 1) * g.scp + (g.nw - R * g.scp) <= 512) ++g.ng;
+    g.nw = (R * S * C + 15) / 16 * 16;
+    g.fixed = (size_t)KH * g.nw * 128 + (size_t)128 * (g.nw + 4) * 4 + sizeof(Dgrad2Ctl) + 1024;
     return g;
 }
 
@@ -300,19 +251,18 @@ bool pcnn_conv_dgrad_rows_ok(int N, int H, int W, int C, int K, int R, int S, co
     const bool inst = (R == 3 && S == 3 && (C == 1 || C == 2 || C == 3 || C == 4 || C == 8)) || (R == 5 && S == 5 && (C == 1 || C == 3)) ||
                       (R == 7 && S == 7 && C == 1);
     if (!inst) return false;
-    const Geometry g = geometry(R, S, C);
-    return g.ng >= 2 && g.nw <= 256 && S <= 16;
+    const Geometry g = geometry(R, S, C, K / 64);
+    return g.nw <= 256 && S <= 16 && g.fixed + 2 * (size_t)(K / 64) * D2_HALF_BYTES <= (size_t)D2_SMEM_BUDGET;
 }
 
 // host-side tiling of the row-streaming input gradient, for pcnn_conv_bwd_plan_info (no GPU needed)
 void pcnn_conv_dgrad_rows_info(int H, int W, int C, int K, int R, int S, int *out4) {
-    const Geometry g = geometry(R, S, C);
+    const Geometry g = geometry(R, S, C, K / 64);
     const int oq_max = 32 - (S - 1);
     const int nstrips = (W + 4 * oq_max - 1) / (4 * oq_max), strip_w = (W + nstrips - 1) / nstrips;
     const size_t stage_bytes = (size_t)(K / 64) * D2_HALF_BYTES;
-    const size_t fixed = (size_t)R * (K / 64) * g.nw * 128 + sizeof(Dgrad2Ctl) + 1024;
-    int st = stage_bytes ? (int)(((size_t)D2_SMEM_BUDGET - fixed) / stage_bytes) : 0;
-    out4[0] = nstrips; out4[1] = (strip_w + 3) / 4; out4[2] = g.ng; out4[3] = st > D2_MAX_STAGES ? D2_MAX_STAGES : st;
+    int st = stage_bytes ? (int)(((size_t)D2_SMEM_BUDGET - g.fixed) / stage_bytes) : 0;
+    out4[0] = nstrips; out4[1] = (strip_w + 3) / 4; out4[2] = R; out4[3] = st > D2_MAX_STAGES ? D2_MAX_STAGES : st;
     (void)H;
 }
 
@@ -321,7 +271,7 @@ int pcnn_conv_dgrad_rows(pcnn_ctx *ctx, const void *dy_bf16, const float *filt_f
                          int R, int S, int row_pitch, int image_rows, int dy_channels) {
     const uint64_t KD = dy_channels > 0 ? (uint64_t)dy_channels : (uint64_t)K;
     pcnn_device_guard guard(ctx->device);
-    const Geometry g = geometry(R, S, C);
+    const Geometry g = geometry(R, S, C, K / 64);
     Dgrad2Params p;
     memset(&p, 0, sizeof(p));
     p.n_img = N; p.H = H; p.W = W; p.P = H - R + 1; p.Q = W - S + 1;
@@ -330,25 +280,22 @@ int pcnn_conv_dgrad_rows(pcnn_ctx *ctx, const void *dy_bf16, const float *filt_f
     p.strip_w = (W + p.nstrips - 1) / p.nstrips;
     p.oq = (p.strip_w + 3) / 4;
     p.bp = p.oq + S - 1;
-    p.ng = g.ng;
-    p.ring = D2_GROUP * g.ng;
     p.T = (long long)N * H;
     p.dx_pitch = row_pitch > 0 ? row_pitch : W * C;
     p.dx_image_rows = image_rows > 0 ? image_rows : H;
     p.dx = reinterpret_cast<__nv_bfloat16 *>(dx_bf16);
     p.KH = K / 64;
     const size_t stage_bytes = (size_t)p.KH * D2_HALF_BYTES;
-    const size_t fixed = (size_t)R * p.KH * g.nw * 128 + sizeof(Dgrad2Ctl) + 1024;
-    int st = (int)(((size_t)D2_SMEM_BUDGET - fixed) / stage_bytes);
+    int st = (int)(((size_t)D2_SMEM_BUDGET - g.fixed) / stage_bytes);
     p.stages = st > D2_MAX_STAGES ? D2_MAX_STAGES : st;
-    PCNN_REQUIRE(p.stages >= 2, PCNN_ERR_ARG, "pcnn_conv_dgrad: filter variants leave no room for two stages");
-    const size_t smem = fixed + (size_t)p.stages * stage_bytes;
+    PCNN_REQUIRE(p.stages >= 2, PCNN_ERR_ARG, "pcnn_conv_dgrad: the filter matrix leaves no room for two stages");
+    const size_t smem = g.fixed + (size_t)p.stages * stage_bytes;
 
     __nv_bfloat16 *T = nullptr;
-    const size_t t_elems = (size_t)R * g.nw * K;
+    const size_t t_elems = (size_t)g.nw * K;
     int rc = pcnn_scratch(ctx, t_elems * 2, (void **)&T);
     if (rc) return rc;
-    k_dgrad2_build_variants<<<(int)((t_elems + 255) / 256), 256, 0, ctx->stream>>>(filt_f32_dev, T, g.nw, g.scp, K, R, S, C);
+    k_dgrad2_build_filter<<<(int)((t_elems + 255) / 256), 256, 0, ctx->stream>>>(filt_f32_dev, T, g.nw, K, R, S, C);
     PCNN_CHECK_LAUNCH(ctx);
 
     CUtensorMap map_dy, map_b;
@@ -359,7 +306,7 @@ int pcnn_conv_dgrad_rows(pcnn_ctx *ctx, const void *dy_bf16, const float *filt_f
         if ((rc = make_map_bf16(&map_dy, const_cast<void *>(dy_bf16), 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B,
                                 CU_TENSOR_MAP_L2_PROMOTION_L2_256B)))
             return rc;
-        const uint64_t bd[2] = {64, (uint64_t)R * p.KH * g.nw};        // [variant][channel group][nw] rows of 64 channels
+        const uint64_t bd[2] = {64, (uint64_t)p.KH * g.nw};            // [channel group][nw] rows of 64 channels
         const uint64_t bs[1] = {128};
         const uint32_t bb[2] = {64, (uint32_t)g.nw};
         if ((rc = make_map_bf16(&map_b, T, 2, bd, bs, bb, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return rc;

@@ -1,5 +1,5 @@
-// parallel-cnn_b200/csrc/conv_tc.cu -- bf16 convolution forward on the 5th-generation tensor cores (SURVEY.md x3,
-// BASELINE.json configs 3 and 5): tcgen05.mma with TMEM accumulators, operands staged by TMA, no im2col pass.
+// parallel-cnn_b200/csrc/conv_tc.cu -- bf16 convolution forward on the Hopper tensor cores (SURVEY.md x3, BASELINE.json
+// configs 3 and 5): wgmma with register accumulators, operands staged by TMA, no im2col pass.
 //
 // Formulation ("row-Toeplitz implicit GEMM").  The reference's conv is a valid, stride-1 cross-correlation
 // (Sequential/layer.h:118-130); for NHWC activations one output row is
@@ -12,41 +12,37 @@
 //     (row r of the filter = the same box shifted down by r rows): zero im2col traffic, the 16x..25x expansion of
 //     im2col never exists anywhere, not even in shared memory;
 //   * B = R matrices [Qt*K x 32] (<= 48 KB) built once on the host from the filter bank, resident in shared memory;
-//   * D = [128 x Qt*K] fp32 in TMEM (256 columns, double buffered = the whole 512-column TMEM of the SM);
-//   * per tile 2*R tcgen05.mma (M=128, N=Qt*K, K=16) issued by one elected thread, epilogue (bias, optional sigmoid,
-//     bf16 pack, store) by four warps reading TMEM with tcgen05.ld while the next tile's MMAs run.
+//   * D = [128 x Qt*K] fp32 in the registers of two warpgroups (64 rows each, N = Qt*K rounded up to 32 <= 256);
+//   * per tile and warpgroup 2*R wgmma (M=64, N, K=16), then the epilogue (bias, optional sigmoid, bf16 pack, store)
+//     straight from the accumulator registers while the producer warp already stages the next tiles.
 // Density: LeNet c1 (C=1, K=6, 5x5, Qt=24): 25/32 of K and 6*24/144 of N are useful but the band itself is sparse
 // (17 % of the issued MACs are useful); config 5 (C=3, K=64, 3x3, Qt=4): 28 %.  The tensor pipe has > 10x headroom over
 // the HBM time of these layers (AI 10-26 flop/B), which is the point: the layer is HBM-bound and the tensor cores are
 // what lets a bf16 kernel reach the HBM roofline where the fp32 FMA pipe cannot (SURVEY.md 8d).
 //
-// Warp roles (192 threads, 1 CTA/SM, persistent over tiles): warp 0 = TMA producer, warp 1 = TMEM owner + MMA issuer,
-// warps 2-5 = epilogue (TMEM lane quarter = warp % 4).
+//
+// Warp roles (288 threads, 1 CTA/SM, persistent over tiles): warps 0-7 = two consumer warpgroups (MMA + epilogue, output rows
+// 0-63 and 64-127 of a tile), warp 8 = TMA producer.
 #include "tc_common.cuh"
 
 #include <vector>
 
 using namespace pcnn_tc;
 
-#ifndef PCNN_DBG_CONV
-#define PCNN_DBG_CONV 0        // 1, 2, 3: measurement builds of the forward kernel (see the epilogue); never shipped
-#endif
-
 namespace {
 
-constexpr int TC_THREADS = 320;         // warp 0 TMA, warp 1 MMA, warps 2-9 epilogue (two per TMEM lane quarter)
-constexpr int TC_EPI_WARPS = 8;
-constexpr int TC_M = 128;          // output rows per tile (TMEM lanes)
+constexpr int TC_THREADS = 288;
+constexpr int TC_CONSUMER_WARPS = 8;
+constexpr int TC_M = 128;          // output rows per tile (two warpgroups of 64)
 constexpr int TC_KCHUNK = 32;      // bf16 elements per filter row r (64 B = one SWIZZLE_64B span)
 constexpr int TC_MAX_STAGES = 4;
 constexpr int TC_SMEM_BUDGET = 225 * 1024;
 constexpr int TC_MAX_R = 5;
 constexpr int A_TILE_BYTES = TC_M * TC_KCHUNK * 2;   // 8 KB
-constexpr int OUT_STAGE_BYTES = 2 * 4096;            // per epilogue warp: two [32 rows x 64 cols] bf16 boxes for the TMA store
 
 struct ConvTcParams {
     int n_img, H, P, Q, K, R;      // images, input rows per image, valid output rows/cols, filters, filter rows
-    int Qt, ncols;                 // output pixels per tile, Qt * K
+    int Qt, ncols, npad;           // output pixels per tile, Qt * K, MMA width (ncols rounded up to 32)
     int C;                         // input channels (column offset of a tile = q0 * stride * C elements)
     int stride;                    // step of the window in both directions (1 = the reference's conv, layer.h:118-130)
     int x_pitch;                   // elements between input rows: filter row r of a stride-s conv reads view row r / s at
@@ -56,17 +52,15 @@ struct ConvTcParams {
     int stages;                    // activation stages that fit next to the V * R Toeplitz matrices
     int n_mtiles, n_qtiles;
     int act;                       // 0: none, 1: sigmoid (the reference's activation, layer.h:81-83)
-    int tma_store;                 // 1: epilogue writes y with cp.async.bulk.tensor stores (H % 32 == 0, 16-B row pitch)
     long long y_row_elems;         // Q * K
     __nv_bfloat16 *y;
     const float *bias;             // [K] or null
 };
 
-// dynamic shared memory, 1024-byte aligned:  [V*R Toeplitz matrices of ncols*64 B] [stages*R activation tiles of 8 KB] [ctl]
+// dynamic shared memory, 1024-byte aligned:  [V*R Toeplitz matrices of npad*64 B] [stages*R activation tiles of 8 KB] [ctl]
 struct ConvTcCtl {
     float bias[256];
-    unsigned long long full[TC_MAX_STAGES], empty[TC_MAX_STAGES], tfull[2], tempty[2], bfull;
-    uint32_t tmem_base;
+    unsigned long long full[TC_MAX_STAGES], empty[TC_MAX_STAGES], bfull;
 };
 struct ConvTcSmemView {
     unsigned char *base;
@@ -75,86 +69,54 @@ struct ConvTcSmemView {
     __device__ __forceinline__ unsigned char *a(int stage, int r) const {
         return base + (size_t)V * R * bmat + (size_t)(stage * R + r) * A_TILE_BYTES;
     }
-    __device__ __forceinline__ unsigned char *out(int epi_warp) const {      // 32 rows x 512 B per epilogue warp
-        return base + (size_t)V * R * bmat + (size_t)stages * R * A_TILE_BYTES + (size_t)epi_warp * OUT_STAGE_BYTES;
-    }
     __device__ __forceinline__ ConvTcCtl &ctl() const {
-        return *reinterpret_cast<ConvTcCtl *>(base + (size_t)V * R * bmat + (size_t)stages * R * A_TILE_BYTES + TC_EPI_WARPS * OUT_STAGE_BYTES);
+        return *reinterpret_cast<ConvTcCtl *>(base + (size_t)V * R * bmat + (size_t)stages * R * A_TILE_BYTES);
     }
 };
-static size_t conv_tc_smem_bytes(int V, int R, int ncols, int stages) {
-    return (size_t)V * R * ncols * TC_KCHUNK * 2 + (size_t)stages * R * A_TILE_BYTES + TC_EPI_WARPS * OUT_STAGE_BYTES + sizeof(ConvTcCtl) + 1024;
+static size_t conv_tc_smem_bytes(int V, int R, int npad, int stages) {
+    return (size_t)V * R * npad * TC_KCHUNK * 2 + (size_t)stages * R * A_TILE_BYTES + sizeof(ConvTcCtl) + 1024;
 }
 
-// Explicit shared-space accesses for the epilogue.  Through generic pointers the compiler must assume that the staging-buffer
-// stores alias the bias table, so every group of 8 outputs waited for its own bias load (ncu: 32 % of the stall samples on the
-// FADDs behind LD.E.128; ~3,500 cycles per tile).  Non-volatile ld.shared can be hoisted and kept in registers.
-__device__ __forceinline__ float4 lds_f4(uint32_t addr) {
-    float4 v;
-    asm("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-    return v;
-}
-__device__ __forceinline__ void sts_u4(uint32_t addr, const uint4 &v) {
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w));
-}
-// sigmoid for a bf16 result: 0.5 + 0.5 tanh(x / 2) with ONE transcendental (MUFU.TANH) instead of two (EX2 + RCP) -- the
-// epilogue of a sigmoid layer is bound by the 16-lane MUFU pipe.  tanh.approx is good to ~5e-4 absolute, a quarter of a bf16 ulp
-// of the result; the test bound (2^-8 |ref| + 1e-3) is unchanged.
+// sigmoid for a bf16 result: 0.5 + 0.5 tanh(x / 2) with ONE transcendental (MUFU.TANH) instead of two (EX2 + RCP).
+// tanh.approx is good to ~5e-4 absolute, a quarter of a bf16 ulp of the result; the test bound (2^-8 |ref| + 1e-3) is unchanged.
 __device__ __forceinline__ float sigmoid_bf16(float x) {
     float t;
     asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.5f * x));
     return fmaf(t, 0.5f, 0.5f);
 }
-template <int N> __device__ __forceinline__ void load_bias_regs(float (&b)[N], uint32_t addr) {
-#pragma unroll
-    for (int j = 0; j < N; j += 4) {
-        const float4 q = lds_f4(addr + j * 4);
-        b[j] = q.x; b[j + 1] = q.y; b[j + 2] = q.z; b[j + 3] = q.w;
-    }
-}
 
-// ACT (0 none, 1 sigmoid), BIAS and the store path are compile-time: the epilogue is straight-line code per variant (as
-// run-time flags they were re-tested for every group of 8 outputs)
-template <int ACT, bool BIAS, bool TMA_ST>
+// ACT (0 none, 1 sigmoid) and the MMA width N are compile-time; a missing bias reads as zeros from the shared bias table
+template <int ACT, int N>
 __global__ void __launch_bounds__(TC_THREADS, 1)
-k_conv_tc_fwd(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_b,
-              const __grid_constant__ CUtensorMap map_y, const ConvTcParams p) {
+k_conv_tc_fwd(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_b, const ConvTcParams p) {
     extern __shared__ unsigned char smem_dyn[];
     ConvTcSmemView sv;
     sv.base = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
-    sv.R = p.R; sv.bmat = p.ncols * TC_KCHUNK * 2; sv.stages = p.stages; sv.V = p.V;
+    sv.R = p.R; sv.bmat = N * TC_KCHUNK * 2; sv.stages = p.stages; sv.V = p.V;
     ConvTcCtl &S = sv.ctl();
     const int NST = p.stages;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int ntiles = p.n_mtiles * p.n_qtiles;
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < NST; ++i) { bar_init(&S.full[i], 1); bar_init(&S.empty[i], 1); }
-        for (int i = 0; i < 2; ++i) { bar_init(&S.tfull[i], 1); bar_init(&S.tempty[i], TC_EPI_WARPS); }
+        for (int i = 0; i < NST; ++i) { bar_init(&S.full[i], 1); bar_init(&S.empty[i], TC_CONSUMER_WARPS); }
         bar_init(&S.bfull, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        fence_barrier_init();
     }
     for (int i = threadIdx.x; i < 256; i += TC_THREADS) S.bias[i] = (p.bias && i < p.ncols) ? p.bias[i % p.K] : 0.0f;
-    if (warp == 1) {   // TMEM: all 512 columns (two accumulators of up to 256 columns)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(&S.tmem_base)), "r"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = S.tmem_base;
 
-    if (warp == 0) {
+    if (warp == TC_CONSUMER_WARPS) {
         // ===== TMA producer: the Toeplitz operand once, then R activation boxes per tile =====
         if (lane == 0) {
-            bar_expect_tx(&S.bfull, (unsigned)(p.V * p.R * p.ncols * TC_KCHUNK * 2));
+            bar_expect_tx(&S.bfull, (unsigned)(p.V * p.R * N * TC_KCHUNK * 2));
             for (int v = 0; v < p.V; ++v)
-                for (int r = 0; r < p.R; ++r) tma_load_2d(sv.b(v, r), &map_b, 0, (v * p.R + r) * p.ncols, &S.bfull);
+                for (int r = 0; r < p.R; ++r) tma_load_2d(sv.b(v, r), &map_b, 0, (v * p.R + r) * N, &S.bfull);
             int it = 0;
             for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
                 const int stage = it % NST;
                 const unsigned ph = (unsigned)(it / NST) & 1u;
-                bar_wait_relaxed(&S.empty[stage], ph ^ 1u, 32);   // NST stages of slack: no need to spin on the MMA warp's sub-partition
+                bar_wait_relaxed(&S.empty[stage], ph ^ 1u, 32);
                 const int mt = tile / p.n_qtiles, qt = tile % p.n_qtiles;
                 bar_expect_tx(&S.full[stage], (unsigned)(p.R * A_TILE_BYTES));
                 for (int r = 0; r < p.R; ++r)
@@ -162,184 +124,72 @@ k_conv_tc_fwd(const __grid_constant__ CUtensorMap map_x, const __grid_constant__
                                 mt * TC_M + r / p.stride, &S.full[stage]);
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        if (lane == 0) {
-            const uint32_t idesc = umma_idesc_bf16(TC_M, p.ncols);
-            bar_wait(&S.bfull, 0);
-            int it = 0;
-            for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-                const int stage = it % NST;
-                const unsigned ph = (unsigned)(it / NST) & 1u;
-                const int acc = it & 1;
-                const unsigned aph = (unsigned)(it >> 1) & 1u;
-                bar_wait(&S.tempty[acc], aph ^ 1u);            // epilogue has drained this accumulator
-                bar_wait(&S.full[stage], ph);                   // activations have landed
-                tc_fence_after();
-                const uint32_t d = tmem + (uint32_t)(acc * 256);
-                const int var = (tile % p.n_qtiles) % p.V;      // which 16-byte remainder this pixel block starts at
-                for (int r = 0; r < p.R; ++r) {
-                    const uint32_t a0 = s_u32(sv.a(stage, r)), b0 = s_u32(sv.b(var, r));
-#pragma unroll
-                    for (int ks = 0; ks < TC_KCHUNK / 16; ++ks)   // K = 16 bf16 = 32 bytes per instruction
-                        tc_mma_bf16(d, umma_desc_k_sw64(a0 + ks * 32), umma_desc_k_sw64(b0 + ks * 32), idesc,
-                                    (r | ks) != 0 ? 1u : 0u);
-                }
-                tc_commit(&S.empty[stage]);                     // smem stage reusable once these MMAs retire
-                tc_commit(&S.tfull[acc]);                       // accumulator complete
-            }
-        }
-    } else {
-        // ===== epilogue warps: TMEM -> registers -> bias / activation -> bf16 -> HBM =====
-        // A TMEM lane is an output row, so tcgen05.ld hands every thread 32 columns of ITS row.
-        //  * TMA-store path (image height a multiple of 32, 16-byte row pitch of y): the warp parks 32 rows x 64 columns
-        //    in shared memory in the SWIZZLE_128B pattern and one lane issues cp.async.bulk.tensor (a 3-D box
-        //    {64 cols, 32 rows, 1 image} of y): the store is asynchronous, rows p >= P and columns q >= Q fall outside the
-        //    tensor and are clipped by the hardware, and the warps go straight back to draining TMEM.
-        //  * direct path otherwise: 16-byte stores from registers (each lane its own row).
-        const int quarter = warp & 3;                           // TMEM lanes this warp may read
-        const int colhalf = (warp - 2) >> 2;                    // two warps share a lane quarter: even / odd column boxes
-        unsigned char *obuf = sv.out(warp - 2);                 // 2 x 4 KB, 1024-byte aligned
-        const uint32_t obuf_s = s_u32(obuf), bias_s = s_u32(S.bias);
-        const uint32_t lane_row = (uint32_t)lane * 128u, lane_sw = (uint32_t)lane & 7u;
-        // TMA-store path: the warp's 64 columns of an iteration are colhalf * 64 + 128 i + [0, 64).  The bias table repeats with
-        // period K, so when K divides 128 the 64 values are the same in every iteration and tile: they live in registers
-        const bool bias_inv = (128 % p.K) == 0;
-        float bz[64];
-        if (TMA_ST && BIAS && bias_inv) load_bias_regs(bz, bias_s + colhalf * 64 * 4);
-        int ob = 0;
-        int it = 0;
-        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-            const int acc = it & 1;
-            const unsigned aph = (unsigned)(it >> 1) & 1u;
-            const int mt = tile / p.n_qtiles, qt = tile % p.n_qtiles;
-            bar_wait(&S.tfull[acc], aph);
-            tc_fence_after();
-#if PCNN_DBG_CONV == 3      // measurement build: the epilogue only hands the accumulator back (load + MMA pipeline alone)
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) bar_arrive(&S.tempty[acc]);
-            continue;
-#endif
-            const int q0 = qt * p.Qt;
-            int valid_cols = (p.Q - q0) * p.K;
-            if (valid_cols > p.ncols) valid_cols = p.ncols;
-            if (TMA_ST) {
-                const long long m0 = (long long)mt * TC_M + quarter * 32;      // first row of this warp: n * H + p
-                const int n = (int)(m0 / p.H), pr = (int)(m0 % p.H);           // H % 32 == 0: the 32 rows share n
-                const bool group_ok = n < p.n_img && pr < p.P;
-                for (int col0 = colhalf * 64; col0 < p.ncols; col0 += 128) {
-                    const uint32_t buf = obuf_s + ob * 4096;
-                    if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");   // buffer `ob` is free again
-                    __syncwarp();
-                    uint32_t vv[2][32];
-                    const uint32_t tbase = tmem + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * 256 + col0);
-                    tc_ld_32x32(tbase, vv[0]);                                   // both halves in flight, one wait
-                    if (col0 + 32 < p.ncols) tc_ld_32x32(tbase + 32, vv[1]);
-                    if (BIAS && !bias_inv) load_bias_regs(bz, bias_s + col0 * 4);   // behind the TMEM loads' latency
-                    tc_wait_ld();
-#pragma unroll
-                    for (int half = 0; half < 2; ++half) {
-                        const int c0 = col0 + half * 32;
-                        if (c0 < p.ncols) {
-                            uint32_t (&v)[32] = vv[half];
-#pragma unroll
-                            for (int j = 0; j < 32; j += 8) {
-                                float f[8];
-#pragma unroll
-                                for (int u = 0; u < 8; ++u) {
-                                    f[u] = __uint_as_float(v[j + u]);
-                                    if (BIAS) f[u] += bz[half * 32 + j + u];
-                                    if (ACT == 1) f[u] = sigmoid_bf16(f[u]);
-                                }
-                                uint4 o;
-                                __nv_bfloat162 t0 = __floats2bfloat162_rn(f[0], f[1]), t1 = __floats2bfloat162_rn(f[2], f[3]);
-                                __nv_bfloat162 t2 = __floats2bfloat162_rn(f[4], f[5]), t3 = __floats2bfloat162_rn(f[6], f[7]);
-                                o.x = *reinterpret_cast<uint32_t *>(&t0); o.y = *reinterpret_cast<uint32_t *>(&t1);
-                                o.z = *reinterpret_cast<uint32_t *>(&t2); o.w = *reinterpret_cast<uint32_t *>(&t3);
-                                const int chunk = half * 4 + (j >> 3);                     // 16-byte chunk of the 128-byte row
-                                sts_u4(buf + lane_row + ((chunk ^ lane_sw) << 4), o);
-                            }
-                        }
-                    }
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");          // generic-proxy writes -> TMA reads
-                    __syncwarp();
-#if PCNN_DBG_CONV == 1      // measurement build: no global stores at all
-                    if (false) {
-#else
-                    if (lane == 0 && group_ok && col0 < valid_cols) {
-#endif
-#if PCNN_DBG_CONV == 2      // measurement build: every store lands on the first row block (L2-resident target)
-                        asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%1, %2, %3}], [%4];" ::"l"(&map_y),
-                                     "r"(q0 * p.K + col0), "r"(pr % 32), "r"(0), "r"(buf)
-                                     : "memory");
-#else
-                        asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%1, %2, %3}], [%4];" ::"l"(&map_y),
-                                     "r"(q0 * p.K + col0), "r"(pr), "r"(n), "r"(buf)
-                                     : "memory");
-#endif
-                        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                    }
-                    ob ^= 1;
-                }
-            } else {
-                const long long m = (long long)mt * TC_M + quarter * 32 + lane;     // global output-row index n * H + p
-                const int n = (int)(m / p.H), pr = (int)(m % p.H);
-                const bool row_ok = n < p.n_img && pr < p.P;
-                __nv_bfloat16 *yrow = p.y + ((long long)n * p.P + pr) * p.y_row_elems + (long long)q0 * p.K;
-                for (int c0 = colhalf * 32; c0 < p.ncols; c0 += 64) {
-                    uint32_t v[32];
-                    tc_ld_32x32(tmem + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * 256 + c0), v);
-                    float b32[32];
-                    if (BIAS) load_bias_regs(b32, bias_s + c0 * 4);
-                    tc_wait_ld();
-                    if (row_ok) {
-#pragma unroll
-                        for (int j = 0; j < 32; j += 8) {
-                            if (c0 + j >= valid_cols) break;
-                            float f[8];
-#pragma unroll
-                            for (int u = 0; u < 8; ++u) {
-                                f[u] = __uint_as_float(v[j + u]);
-                                if (BIAS) f[u] += b32[j + u];
-                                if (ACT == 1) f[u] = sigmoid_bf16(f[u]);
-                            }
-                            if (c0 + j + 8 <= valid_cols && ((reinterpret_cast<uintptr_t>(yrow + c0 + j) & 15) == 0)) {
-                                uint4 o;
-                                __nv_bfloat162 t0 = __floats2bfloat162_rn(f[0], f[1]), t1 = __floats2bfloat162_rn(f[2], f[3]);
-                                __nv_bfloat162 t2 = __floats2bfloat162_rn(f[4], f[5]), t3 = __floats2bfloat162_rn(f[6], f[7]);
-                                o.x = *reinterpret_cast<uint32_t *>(&t0); o.y = *reinterpret_cast<uint32_t *>(&t1);
-                                o.z = *reinterpret_cast<uint32_t *>(&t2); o.w = *reinterpret_cast<uint32_t *>(&t3);
-                                *reinterpret_cast<uint4 *>(yrow + c0 + j) = o;
-                            } else {
-                                for (int u = 0; u < 8 && c0 + j + u < valid_cols; ++u) yrow[c0 + j + u] = __float2bfloat16_rn(f[u]);
-                            }
-                        }
-                    }
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) bar_arrive(&S.tempty[acc]);
-        }
-        if (TMA_ST && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // all stores landed
-        __syncwarp();
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512));
+
+    // ===== consumer warpgroups: MMA into registers, then bias / activation -> bf16 -> HBM =====
+    const int wg = warp >> 2, wq = warp & 3;
+    const uint32_t bias_s = s_u32(S.bias);
+    bar_wait(&S.bfull, 0);
+    int it = 0;
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
+        const int stage = it % NST;
+        const unsigned ph = (unsigned)(it / NST) & 1u;
+        const int mt = tile / p.n_qtiles, qt = tile % p.n_qtiles;
+        const int var = qt % p.V;                          // which 16-byte remainder this pixel block starts at
+        float acc[N / 2];
+        bar_wait(&S.full[stage], ph);
+        wg_fence();
+        for (int r = 0; r < p.R; ++r) {
+            const uint32_t a0 = s_u32(sv.a(stage, r)) + (uint32_t)(wg * 64 * TC_KCHUNK * 2), b0 = s_u32(sv.b(var, r));
+#pragma unroll
+            for (int ks = 0; ks < TC_KCHUNK / 16; ++ks)    // K = 16 bf16 = 32 bytes per instruction
+                wgmma_bf16<0, 0>(acc, gmma_desc_k_sw64(a0 + ks * 32), gmma_desc_k_sw64(b0 + ks * 32), (r | ks) != 0 ? 1u : 0u);
+        }
+        wg_commit();
+        wg_wait<0>();
+        wg_hold(acc);
+        __syncwarp();
+        if (lane == 0) bar_arrive(&S.empty[stage]);       // smem stage reusable: this warp's MMAs have retired
+
+        const int q0 = qt * p.Qt;
+        int valid_cols = (p.Q - q0) * p.K;
+        if (valid_cols > p.ncols) valid_cols = p.ncols;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const long long m = (long long)mt * TC_M + wg * 64 + wg_row(2 * h, wq, lane);   // output row n * H + p
+            const int n = (int)(m / p.H), pr = (int)(m % p.H);
+            if (n >= p.n_img || pr >= p.P) continue;
+            __nv_bfloat16 *yrow = p.y + ((long long)n * p.P + pr) * p.y_row_elems + (long long)q0 * p.K;
+#pragma unroll
+            for (int j = 0; j < N / 8; ++j) {
+                const int c = wg_col(4 * j, lane);
+                if (c >= valid_cols) continue;
+                float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+                float2 bb;
+                asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(bb.x), "=f"(bb.y) : "r"(bias_s + (uint32_t)c * 4u));
+                f0 += bb.x; f1 += bb.y;
+                if (ACT == 1) { f0 = sigmoid_bf16(f0); f1 = sigmoid_bf16(f1); }
+                if (c + 1 < valid_cols && ((reinterpret_cast<uintptr_t>(yrow + c) & 3) == 0)) {
+                    *reinterpret_cast<__nv_bfloat162 *>(yrow + c) = __floats2bfloat162_rn(f0, f1);
+                } else {
+                    yrow[c] = __float2bfloat16_rn(f0);
+                    if (c + 1 < valid_cols) yrow[c + 1] = __float2bfloat16_rn(f1);
+                }
+            }
+        }
     }
 }
 
-typedef void (*conv_tc_fwd_fn)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const ConvTcParams);
-static const void *conv_tc_fwd_variant(bool sigmoid, bool bias, bool tma_store) {
-    static const conv_tc_fwd_fn table[8] = {
-        k_conv_tc_fwd<0, false, false>, k_conv_tc_fwd<1, false, false>, k_conv_tc_fwd<0, true, false>, k_conv_tc_fwd<1, true, false>,
-        k_conv_tc_fwd<0, false, true>,  k_conv_tc_fwd<1, false, true>,  k_conv_tc_fwd<0, true, true>,  k_conv_tc_fwd<1, true, true>};
-    return reinterpret_cast<const void *>(table[(sigmoid ? 1 : 0) | (bias ? 2 : 0) | (tma_store ? 4 : 0)]);
+typedef void (*conv_tc_fwd_fn)(const CUtensorMap, const CUtensorMap, const ConvTcParams);
+#define PCNN_FWD_ROW(N) {k_conv_tc_fwd<0, N>, k_conv_tc_fwd<1, N>}
+static const void *conv_tc_fwd_variant(bool sigmoid, int npad) {
+    static const conv_tc_fwd_fn table[8][2] = {PCNN_FWD_ROW(32),  PCNN_FWD_ROW(64),  PCNN_FWD_ROW(96),  PCNN_FWD_ROW(128),
+                                               PCNN_FWD_ROW(160), PCNN_FWD_ROW(192), PCNN_FWD_ROW(224), PCNN_FWD_ROW(256)};
+    return reinterpret_cast<const void *>(table[npad / 32 - 1][sigmoid ? 1 : 0]);
 }
+#undef PCNN_FWD_ROW
+
 
 // fp32 [rows][w] -> bf16 [rows][pitch] (zero padded), for building the padded NHWC activations the TMA map needs
 __global__ void k_f32_to_bf16_rows(const float *__restrict__ src, __nv_bfloat16 *__restrict__ dst, long rows, int w, int pitch) {
@@ -364,24 +214,6 @@ int make_map_2d(CUtensorMap *map, void *base, uint64_t inner, uint64_t outer, ui
     if (r != CUDA_SUCCESS) {
         pcnn_set_error("cuTensorMapEncodeTiled failed (%d) for [%llu x %llu] pitch %llu box [%u x %u]", (int)r,
                        (unsigned long long)inner, (unsigned long long)outer, (unsigned long long)pitch_bytes, box_inner, box_outer);
-        return PCNN_ERR_CUDA;
-    }
-    return PCNN_OK;
-}
-
-// y viewed as [N][P][Q*K] bf16, boxes of {64 columns, 32 rows, 1 image}, SWIZZLE_128B (128-byte box rows)
-int make_map_y(CUtensorMap *map, void *base, uint64_t row_elems, uint64_t P, uint64_t N) {
-    encode_tiled_fn enc;
-    int rc = get_encode(&enc);
-    if (rc) return rc;
-    cuuint64_t dims[3] = {row_elems, P, N};
-    cuuint64_t strides[2] = {row_elems * 2, row_elems * 2 * P};
-    cuuint32_t box[3] = {64, 32, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        pcnn_set_error("cuTensorMapEncodeTiled failed (%d) for the output tensor", (int)r);
         return PCNN_ERR_CUDA;
     }
     return PCNN_OK;
@@ -437,7 +269,7 @@ extern "C" int pcnn_conv_tc_plan_create_strided(pcnn_ctx *ctx, int N, int H, int
         int max_delta = 0;
         for (int i = 0; i < v; ++i) max_delta = max_delta > (i * t * stride * C) % 8 ? max_delta : (i * t * stride * C) % 8;
         if (max_delta + ((t - 1) * stride + S) * C > TC_KCHUNK) continue;
-        const size_t fixed = (size_t)v * R * t * K * TC_KCHUNK * 2 + TC_EPI_WARPS * OUT_STAGE_BYTES + sizeof(ConvTcCtl) + 1024;
+        const size_t fixed = (size_t)v * R * ((t * K + 31) / 32 * 32) * TC_KCHUNK * 2 + sizeof(ConvTcCtl) + 1024;
         if (fixed + 2 * (size_t)R * A_TILE_BYTES > (size_t)TC_SMEM_BUDGET) continue;
         int st = (int)(((size_t)TC_SMEM_BUDGET - fixed) / ((size_t)R * A_TILE_BYTES));
         Qt = t; V = v; stages = st > TC_MAX_STAGES ? TC_MAX_STAGES : st;
@@ -453,15 +285,14 @@ extern "C" int pcnn_conv_tc_plan_create_strided(pcnn_ctx *ctx, int N, int H, int
     pl->W = W; pl->S = S; pl->row_pitch = row_pitch; pl->stride = stride; pl->in_image_rows = image_rows;
     ConvTcParams &p = pl->p;
     // rows are counted in units of `stride` input rows: tile row m = n * (image_rows / stride) + p
-    p.n_img = N; p.H = image_rows / stride; p.P = P; p.Q = Q; p.K = K; p.R = R; p.Qt = Qt; p.ncols = Qt * K; p.C = C; p.V = V; p.stages = stages;
+    p.n_img = N; p.H = image_rows / stride; p.P = P; p.Q = Q; p.K = K; p.R = R; p.Qt = Qt; p.ncols = Qt * K; p.npad = (Qt * K + 31) / 32 * 32; p.C = C; p.V = V; p.stages = stages;
     p.stride = stride; p.x_pitch = row_pitch;
     p.n_mtiles = (int)(((long long)N * p.H + TC_M - 1) / TC_M);
     p.n_qtiles = (Q + Qt - 1) / Qt;
     p.act = act;
     p.y_row_elems = (long long)Q * K;
-    p.tma_store = (p.H % 32 == 0 && ((long long)Q * K * 2) % 16 == 0) ? 1 : 0;
-    // Toeplitz operands: T_{v,r}[(ql, k)][kk] = f[k][r][s][c] where kk = delta_v + (ql + s) * C + c
-    std::vector<uint16_t> t((size_t)V * R * p.ncols * TC_KCHUNK, 0);
+    // Toeplitz operands: T_{v,r}[(ql, k)][kk] = f[k][r][s][c] where kk = delta_v + (ql + s) * C + c; rows ncols..npad-1 stay zero
+    std::vector<uint16_t> t((size_t)V * R * p.npad * TC_KCHUNK, 0);
     for (int v = 0; v < V; ++v) {
         const int delta = (v * Qt * stride * C) % 8;
         for (int r = 0; r < R; ++r)
@@ -469,7 +300,7 @@ extern "C" int pcnn_conv_tc_plan_create_strided(pcnn_ctx *ctx, int N, int H, int
                 for (int k = 0; k < K; ++k)
                     for (int s = 0; s < S; ++s)
                         for (int c = 0; c < C; ++c)
-                            t[(((size_t)v * R + r) * p.ncols + ql * K + k) * TC_KCHUNK + delta + (ql * stride + s) * C + c] =
+                            t[(((size_t)v * R + r) * p.npad + ql * K + k) * TC_KCHUNK + delta + (ql * stride + s) * C + c] =
                                 f32_to_bf16_bits(filt_host[(((size_t)k * R + r) * S + s) * C + c]);
     }
     PCNN_CUDA(cudaMalloc(&pl->d_toeplitz, t.size() * 2));
@@ -479,12 +310,12 @@ extern "C" int pcnn_conv_tc_plan_create_strided(pcnn_ctx *ctx, int N, int H, int
         PCNN_CUDA(cudaMemcpy(pl->d_bias, bias_host, K * sizeof(float), cudaMemcpyHostToDevice));
     }
     p.bias = pl->d_bias;
-    int rc = make_map_2d(&pl->map_b, pl->d_toeplitz, TC_KCHUNK, (uint64_t)V * R * p.ncols, TC_KCHUNK * 2, TC_KCHUNK, (uint32_t)p.ncols);
+    int rc = make_map_2d(&pl->map_b, pl->d_toeplitz, TC_KCHUNK, (uint64_t)V * R * p.npad, TC_KCHUNK * 2, TC_KCHUNK, (uint32_t)p.npad);
     if (rc) return rc;
     static bool configured[64] = {};        // function attributes are per device
     if (!configured[ctx->device & 63]) {
-        for (int v = 0; v < 8; ++v)
-            PCNN_CUDA(cudaFuncSetAttribute(conv_tc_fwd_variant(v & 1, (v >> 1) & 1, (v >> 2) & 1), cudaFuncAttributeMaxDynamicSharedMemorySize,
+        for (int v = 0; v < 16; ++v)
+            PCNN_CUDA(cudaFuncSetAttribute(conv_tc_fwd_variant(v & 1, 32 * (v / 2 + 1)), cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            TC_SMEM_BUDGET + 2048));
         configured[ctx->device & 63] = true;
     }
@@ -513,16 +344,11 @@ extern "C" int pcnn_conv_tc_fwd(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void 
     int rc = make_map_2d(&map_x, const_cast<void *>(x_bf16), (uint64_t)plan->row_pitch * plan->stride, (uint64_t)p.n_img * p.H,
                          (uint64_t)plan->row_pitch * plan->stride * 2, TC_KCHUNK, TC_M);
     if (rc) return rc;
-    CUtensorMap map_y = map_x;                          // placeholder when the direct-store epilogue is used
-    if (p.tma_store) {
-        PCNN_REQUIRE(((uintptr_t)y_bf16 & 15) == 0, PCNN_ERR_ARG, "pcnn_conv_tc_fwd: output must be 16-byte aligned");
-        if ((rc = make_map_y(&map_y, y_bf16, (uint64_t)p.y_row_elems, (uint64_t)p.P, (uint64_t)p.n_img))) return rc;
-    }
     const int ntiles = p.n_mtiles * p.n_qtiles;
     const int grid = ntiles < ctx->sm_count ? ntiles : ctx->sm_count;
-    void *args[] = {&map_x, &plan->map_b, &map_y, &p};
-    PCNN_CUDA(cudaLaunchKernel(conv_tc_fwd_variant(p.act == 1, p.bias != nullptr, p.tma_store != 0), dim3((unsigned)grid), dim3(TC_THREADS), args,
-                               conv_tc_smem_bytes(p.V, p.R, p.ncols, p.stages), ctx->stream));
+    void *args[] = {&map_x, &plan->map_b, &p};
+    PCNN_CUDA(cudaLaunchKernel(conv_tc_fwd_variant(p.act == 1, p.npad), dim3((unsigned)grid), dim3(TC_THREADS), args,
+                               conv_tc_smem_bytes(p.V, p.R, p.npad, p.stages), ctx->stream));
     PCNN_CHECK_LAUNCH(ctx);
     return PCNN_OK;
 }

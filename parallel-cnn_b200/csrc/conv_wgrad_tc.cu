@@ -1,23 +1,22 @@
-// parallel-cnn_b200/csrc/conv_wgrad_tc.cu -- weight gradient of the NHWC bf16 convolution (64 filters) on the tcgen05 tensor cores.
+// parallel-cnn_b200/csrc/conv_wgrad_tc.cu -- weight gradient of the NHWC bf16 convolution (64 filters) on the Hopper tensor cores.
 //
 //     dw[k][r][s][c] = sum_{n,p,q} dy[n][p][q][k] * x[n][p+r][q+s][c]           [ref: layer.h:371-395 bp_weight_c1, without /576]
 //
 // SURVEY.md x3 / BASELINE.json config 5: dy [N,222,222,64] is 95 % of the 6.6 MB/image this pass moves and the pass is
-// HBM-bound (SURVEY.md 8d), so: dy crosses HBM -> shared memory once by TMA and is consumed there by tcgen05.mma.
+// HBM-bound (SURVEY.md 8d), so: dy crosses HBM -> shared memory once by TMA and is consumed there by wgmma.
 //   * The reduction runs over pixels, the slow axis of both tensors.  dy needs no transposition: a TMA tile
 //     [RB rows][PC pixels][64 filters] is an MN-major B operand as it lands (one 128-byte swizzled row per pixel; the RB
 //     rows are RB atoms along N, N = RB * 64 <= 256).
 //   * The other operand is the Hankel matrix of the x rows, A[(rho, s, c)][pixel q] = x[p0 + rho][(q + s) * C + c] for the
-//     RB + R - 1 input rows a block of RB dy rows touches (54 of M = 64 rows at config 5); eight warps build it in shared
+//     RB + R - 1 input rows a block of RB dy rows touches (54 of M = 64 rows at config 5); four warps build it in shared
 //     memory from the x row segments (x is 5 % of the traffic; the 9x expansion never leaves the SM).
 //     (More than 64 filters: K/64 boxes per tile, the accumulator columns become (filter group, row, filter), K <= 256.)
-//   * D[(rho, s, c)][(row, k)] accumulates in ONE 64 x 256 TMEM accumulator for the whole kernel; the entries with
-//     rho - row = r in [0, R) are the gradient, the others are discarded.  At the end each CTA folds the RB row blocks,
-//     writes one 1,728-float partial, and a second kernel adds the partials in a fixed order (deterministic, no atomics).
-// Why this shape: one tcgen05.mma costs the issuing thread and the tensor path ~56-70 clk for any N <= 112 and N/2 clk
-// above (pcnn_measure_mma_rate), and a first version with one dy row per tile (dy as the M = 64 operand, N = 32) was bound
-// by exactly that: 14 MMAs per 28 KB, 5.2 TB/s with a minimal issue loop, 4.1 TB/s with a careless one, 6.3 TB/s with the
-// MMAs removed.  With N = 192 one instruction consumes 6 KB of dy and the kernel streams 6.1 TB/s (92 % of the HBM peak).
+//   * D[(rho, s, c)][(row, k)] accumulates in ONE 64 x N (N = RB * 64 <= 256) register accumulator of one warpgroup for
+//     the whole kernel; the entries with rho - row = r in [0, R) are the gradient, the others are discarded.  At the end each
+//     CTA folds the RB row blocks, writes one 1,728-float partial, and a second kernel adds the partials in a fixed order
+//     (deterministic, no atomics).
+//   * Large N matters: one wgmma of N = 192 consumes 6 KB of dy, so the MMA issue stream stays far below the HBM time of
+//     the bytes it consumes.
 #include "tc_common.cuh"
 
 #include <stdlib.h>
@@ -26,10 +25,11 @@ using namespace pcnn_tc;
 
 namespace {
 
-constexpr int W2_BUILD_WARPS = 8;
-constexpr int W2_THREADS = 64 + 32 * W2_BUILD_WARPS;   // warp 0 TMA producer, warp 1 MMA issuer + TMEM owner, warps 2-9 Hankel builders
+constexpr int W2_BUILD_WARPS = 4;
+constexpr int W2_THREADS = 160 + 32 * W2_BUILD_WARPS;  // warps 0-3 MMA warpgroup, warps 4-7 Hankel builders, warp 8 TMA producer
+constexpr int W2_PRODUCER_WARP = 4 + W2_BUILD_WARPS;
 constexpr int W2_MAX_STAGES = 6;
-constexpr int W2_ITEMS = 4;                            // 16-byte units of the Hankel tile per builder thread
+constexpr int W2_ITEMS = 8;                            // 16-byte units of the Hankel tile per builder thread
 constexpr int W2_SMEM_BUDGET = 222 * 1024;
 constexpr int W2_DUMP_STRIDE = 257;                    // floats per accumulator row in the read-out staging (bank spread)
 
@@ -47,8 +47,7 @@ struct Wgrad2Params {
 };
 
 struct Wgrad2Ctl {
-    unsigned long long full[W2_MAX_STAGES], empty[W2_MAX_STAGES], bready[W2_MAX_STAGES], tdone;
-    uint32_t tmem_base;
+    unsigned long long full[W2_MAX_STAGES], empty[W2_MAX_STAGES], bready[W2_MAX_STAGES];
 };
 
 __device__ __forceinline__ unsigned short lds_u16(uint32_t saddr) {
@@ -68,8 +67,8 @@ __device__ __forceinline__ int xseg_copy_bytes(const Wgrad2Params &p, int chunk)
     return avail < p.xseg_bytes ? avail : p.xseg_bytes;
 }
 
-// CT = compile-time input-channel count (the gather stride of the Hankel builder), 0 = run-time
-template <int CT>
+// CT = compile-time input-channel count (the gather stride of the Hankel builder), 0 = run-time; N = accumulator columns
+template <int CT, int N>
 __global__ void __launch_bounds__(W2_THREADS, 1)
 k_conv_tc_wgrad_rows(const __grid_constant__ CUtensorMap map_dy, const Wgrad2Params p) {
     const int C = CT > 0 ? CT : p.C;
@@ -77,7 +76,6 @@ k_conv_tc_wgrad_rows(const __grid_constant__ CUtensorMap map_dy, const Wgrad2Par
     unsigned char *base = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
     const int dy_half = p.RB * p.PC * 128;              // one box: [RB][PC][64] bf16, SWIZZLE_128B
     const int dy_bytes = p.KH * dy_half;                // [KH filter groups][RB][PC][64]
-    const int ncols = p.KH * p.RB * 64;                 // accumulator columns (group, row, filter)
     const int hk_bytes = 64 * p.PC * 2;                 // Hankel tile [64][PC] bf16, K-major 8x8 core matrices
     const int x_bytes = p.NXR * p.xseg_stride;
     unsigned char *DY = base;
@@ -89,23 +87,20 @@ k_conv_tc_wgrad_rows(const __grid_constant__ CUtensorMap map_dy, const Wgrad2Par
     const int tiles_per_img = p.n_pb * p.n_ch;
     const int ntiles = p.n_img * tiles_per_img;
     const int SBO = p.KO * 128;                         // bytes between 8-row groups of the Hankel tile
-    const int tmem_cols = ncols <= 64 ? 64 : (ncols <= 128 ? 128 : 256);
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < NST; ++i) { bar_init(&S.full[i], 1); bar_init(&S.empty[i], 1); bar_init(&S.bready[i], W2_BUILD_WARPS); }
-        bar_init(&S.tdone, 1);
+        for (int i = 0; i < NST; ++i) { bar_init(&S.full[i], 1); bar_init(&S.empty[i], 4); bar_init(&S.bready[i], W2_BUILD_WARPS); }
         fence_barrier_init();
     }
     // Hankel rows >= nreal and everything the x copies do not reach stay zero / finite for the whole kernel
     for (int i = threadIdx.x * 16; i < NST * (hk_bytes + x_bytes); i += W2_THREADS * 16) *reinterpret_cast<uint4 *>(HK + i) = make_uint4(0, 0, 0, 0);
     fence_proxy_async_smem();
-    if (warp == 1) tc_alloc(&S.tmem_base, (unsigned)tmem_cols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = S.tmem_base;
 
-    if (warp == 0) {
+    // every role ends at named barrier 1 (all W2_THREADS threads): then every copy has landed and every MMA has retired, and the
+    // stages are free for the read-out staging
+    float *dump = reinterpret_cast<float *>(base);
+    if (warp == W2_PRODUCER_WARP) {
         // ===== TMA producer: one dy box [64 filters x PC pixels x RB rows] and NXR x row segments per tile =====
         if (lane == 0) {
             int stage = 0;
@@ -128,37 +123,38 @@ k_conv_tc_wgrad_rows(const __grid_constant__ CUtensorMap map_dy, const Wgrad2Par
                 if (++stage == NST) { stage = 0; ph ^= 1u; }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer: D[64 x RB*64] += Hankel[64 x 16 pixels] * dy[16 pixels x RB*64]; invariant operands, constant adds =====
-        if (lane == 0) {
-            const uint32_t idesc = umma_idesc_bf16(64, ncols, /*A K-major*/ 0, /*B MN-major*/ 1);
-            const uint64_t adesc0 = umma_desc_k_none(s_u32(HK), 128, (uint32_t)SBO);
-            const uint64_t bdesc0 = umma_desc(s_u32(DY), (uint32_t)(p.PC * 128), 1024, 2);   // LBO = next dy row, SBO = next 8 pixels
-            const uint32_t a_step = (uint32_t)hk_bytes >> 4, b_step = (uint32_t)dy_bytes >> 4;
-            const int nk = p.PC / 16;
-            int stage = 0;
-            unsigned ph = 0;
-            bool first = true;
-            for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-                bar_wait(&S.full[stage], ph);
-                bar_wait(&S.bready[stage], ph);
-                tc_fence_after();
-                uint64_t ad = adesc0 + (uint64_t)((uint32_t)stage * a_step), bd = bdesc0 + (uint64_t)((uint32_t)stage * b_step);
-                tc_mma_bf16(tmem, ad, bd, idesc, first ? 0u : 1u);
-                for (int ks = 1; ks < nk; ++ks) {
-                    ad += 256 >> 4;                          // 16 pixels of the Hankel tile: two 128-byte core matrices
-                    bd += 2048 >> 4;                         // 16 pixels of dy: two 1024-byte swizzle groups
-                    tc_mma_bf16(tmem, ad, bd, idesc, 1u);
-                }
-                first = false;
-                tc_commit(&S.empty[stage]);
-                if (++stage == NST) { stage = 0; ph ^= 1u; }
-            }
-            tc_commit(&S.tdone);
+        asm volatile("bar.sync 1, %0;" ::"n"(W2_THREADS) : "memory");
+    } else if (warp < 4) {
+        // ===== MMA warpgroup: D[64 x RB*64] += Hankel[64 x 16 pixels] * dy[16 pixels x RB*64] (dy MN-major) =====
+        float acc[N / 2];                               // live in this branch only (the builder warps stay small)
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) acc[i] = 0.0f;
+        const uint32_t a_step = (uint32_t)hk_bytes, b_step = (uint32_t)dy_bytes;
+        const int nk = p.PC / 16;
+        int stage = 0;
+        unsigned ph = 0;
+        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+            bar_wait(&S.full[stage], ph);
+            bar_wait(&S.bready[stage], ph);
+            const uint32_t a0 = s_u32(HK) + (uint32_t)stage * a_step, b0 = s_u32(DY) + (uint32_t)stage * b_step;
+            wg_fence();
+            for (int ks = 0; ks < nk; ++ks)              // 16 pixels: two 128-byte core matrices of the Hankel tile, two
+                                                         // 1024-byte swizzle groups of dy
+                wgmma_bf16<0, 1>(acc, gmma_desc_k_none(a0 + ks * 256, 128, (uint32_t)SBO), gmma_desc_mn_sw128(b0 + ks * 2048, (uint32_t)(p.PC * 128)), 1u);
+            wg_commit();
+            wg_wait<0>();
+            wg_hold(acc);
+            __syncwarp();
+            if (lane == 0) bar_arrive(&S.empty[stage]);
+            if (++stage == NST) { stage = 0; ph ^= 1u; }
         }
+        asm volatile("bar.sync 1, %0;" ::"n"(W2_THREADS) : "memory");
+        // ===== read-out: accumulator -> shared memory =====
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) dump[wg_row(i, warp, lane) * W2_DUMP_STRIDE + wg_col(i, lane)] = acc[i];
     } else {
         // ===== Hankel builders: 16-byte units = 8 pixels of one row (rho, j); shared-memory loads and stores by address =====
-        const int b = threadIdx.x - 64;
+        const int b = threadIdx.x - 128;
         const int units = ((p.nreal + 7) / 8) * 8 * p.KO;
         int src_off[W2_ITEMS], dst_off[W2_ITEMS], e0s[W2_ITEMS];
 #pragma unroll
@@ -181,26 +177,23 @@ k_conv_tc_wgrad_rows(const __grid_constant__ CUtensorMap map_dy, const Wgrad2Par
         for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
             bar_wait_relaxed(&S.full[stage], ph, 32);
             const uint32_t xs = x_s + (uint32_t)(stage * x_bytes), hs = hk_s + (uint32_t)(stage * hk_bytes);
-            unsigned short e[W2_ITEMS][8];
-#pragma unroll
-            for (int i = 0; i < W2_ITEMS; ++i) {             // all gathers in flight before the first use
-                const uint32_t src = xs + (uint32_t)(src_off[i] >= 0 ? src_off[i] : 0);
-#pragma unroll
-                for (int u = 0; u < 8; ++u) e[i][u] = lds_u16(src + (uint32_t)(u * C * 2));
-            }
             int lim0 = 0;
             if (p.guard) lim0 = p.W * C - ((tile % tiles_per_img) % p.n_ch) * p.PC * C;   // row elements at or after the segment start
 #pragma unroll
             for (int i = 0; i < W2_ITEMS; ++i) {
                 if (src_off[i] >= 0) {
+                    const uint32_t src = xs + (uint32_t)src_off[i];
+                    unsigned short e[8];
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) e[u] = lds_u16(src + (uint32_t)(u * C * 2));
                     if (p.guard) {
 #pragma unroll
                         for (int u = 0; u < 8; ++u)
-                            if (e0s[i] + u * C >= lim0) e[i][u] = 0;
+                            if (e0s[i] + u * C >= lim0) e[u] = 0;
                     }
                     uint4 o;
-                    o.x = e[i][0] | ((uint32_t)e[i][1] << 16); o.y = e[i][2] | ((uint32_t)e[i][3] << 16);
-                    o.z = e[i][4] | ((uint32_t)e[i][5] << 16); o.w = e[i][6] | ((uint32_t)e[i][7] << 16);
+                    o.x = e[0] | ((uint32_t)e[1] << 16); o.y = e[2] | ((uint32_t)e[3] << 16);
+                    o.z = e[4] | ((uint32_t)e[5] << 16); o.w = e[6] | ((uint32_t)e[7] << 16);
                     sts_v4(hs + (uint32_t)dst_off[i], o);
                 }
             }
@@ -209,26 +202,10 @@ k_conv_tc_wgrad_rows(const __grid_constant__ CUtensorMap map_dy, const Wgrad2Par
             if (lane == 0) bar_arrive(&S.bready[stage]);
             if (++stage == NST) { stage = 0; ph ^= 1u; }
         }
+        asm volatile("bar.sync 1, %0;" ::"n"(W2_THREADS) : "memory");
     }
 
-    // ===== read-out: accumulator -> shared memory, fold the RB row blocks, one partial per CTA =====
-    float *dump = reinterpret_cast<float *>(base);      // the stages are free once every MMA has retired
-    if (warp >= 2 && warp < 6) {
-        bar_wait_relaxed(&S.tdone, 0, 64);
-        tc_fence_after();
-        const int quarter = warp & 3;                   // an M = 64 accumulator keeps row n in TMEM lane (n / 16) * 32 + n % 16
-        const int n = quarter * 16 + lane;
-        for (int c0 = 0; c0 < ncols; c0 += 32) {
-            uint32_t v[32];
-            tc_ld_32x32(tmem + ((uint32_t)(quarter * 32) << 16) + (uint32_t)c0, v);
-            tc_wait_ld();
-            if (lane < 16) {
-#pragma unroll
-                for (int i = 0; i < 32; ++i) dump[n * W2_DUMP_STRIDE + c0 + i] = __uint_as_float(v[i]);
-            }
-        }
-    }
-    tc_fence_before();
+    // ===== fold the RB row blocks of the dumped accumulator, one partial per CTA =====
     __syncthreads();
     {
         // dw[k][r][j] = sum over row blocks rb of D[(rb + r) * SC + j][rb * 64 + k]
@@ -240,10 +217,6 @@ k_conv_tc_wgrad_rows(const __grid_constant__ CUtensorMap map_dy, const Wgrad2Par
             for (int rb = 0; rb < p.RB; ++rb) s += dump[((rb + r) * p.SC + j) * W2_DUMP_STRIDE + (kh * p.RB + rb) * 64 + kl];
             dst[o] = s;
         }
-    }
-    if (warp == 1) {
-        tc_fence_after();
-        tc_dealloc(tmem, (unsigned)tmem_cols);
     }
 }
 
@@ -264,10 +237,8 @@ __global__ void __launch_bounds__(256) k_conv_tc_wgrad_rows_reduce(const float *
 
 struct Plan { int RB, PC, stages; size_t stage_bytes, smem; bool ok; };
 
-// Tile shape: dy rows per tile RB (N = RB * 64) and pixels per tile PC.  Measured at config 5 (profiles/r01_README.md): what
-// matters is that the tiles cover the [P x Q] plane with little padding (PC = 112 covers Q = 222 in two chunks: 139-147 us;
-// PC = 80 in three: 149-244 us) and that at least three stages fit; RB = 3 (139 us) ~ RB = 2 (141 us) < RB = 4 (147 us, two
-// stages).
+// Tile shape: dy rows per tile RB (N = RB * 64) and pixels per tile PC.  What matters is that the tiles cover the [P x Q]
+// plane with little padding (PC = 112 covers Q = 222 in two chunks, PC = 80 needs three) and that at least three stages fit.
 Plan plan_for(int P, int Q, int C, int R, int S, int KH) {
     Plan pl;
     memset(&pl, 0, sizeof(pl));
@@ -297,16 +268,25 @@ Plan plan_for(int P, int Q, int C, int R, int S, int KH) {
     return pl;
 }
 
-template <int CT>
+template <int CT, int N>
 int launch_rows(pcnn_ctx *ctx, const CUtensorMap &map_dy, const Wgrad2Params &p, int grid, size_t smem) {
     static bool configured[64] = {};        // function attributes are per device
     if (!configured[ctx->device & 63]) {
-        PCNN_CUDA(cudaFuncSetAttribute(k_conv_tc_wgrad_rows<CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, W2_SMEM_BUDGET + 2048));
+        PCNN_CUDA(cudaFuncSetAttribute(k_conv_tc_wgrad_rows<CT, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, W2_SMEM_BUDGET + 2048));
         configured[ctx->device & 63] = true;
     }
-    k_conv_tc_wgrad_rows<CT><<<grid, W2_THREADS, smem, ctx->stream>>>(map_dy, p);
+    k_conv_tc_wgrad_rows<CT, N><<<grid, W2_THREADS, smem, ctx->stream>>>(map_dy, p);
     PCNN_CHECK_LAUNCH(ctx);
     return PCNN_OK;
+}
+template <int CT>
+int launch_rows_n(pcnn_ctx *ctx, const CUtensorMap &map_dy, const Wgrad2Params &p, int grid, size_t smem) {
+    switch (p.KH * p.RB) {                  // accumulator columns = 64 x (filter groups x dy rows per tile) <= 256
+        case 1: return launch_rows<CT, 64>(ctx, map_dy, p, grid, smem);
+        case 2: return launch_rows<CT, 128>(ctx, map_dy, p, grid, smem);
+        case 3: return launch_rows<CT, 192>(ctx, map_dy, p, grid, smem);
+        default: return launch_rows<CT, 256>(ctx, map_dy, p, grid, smem);
+    }
 }
 
 }  // namespace
@@ -359,8 +339,8 @@ int pcnn_conv_wgrad_rows(pcnn_ctx *ctx, const void *x_bf16, const void *dy_bf16,
                                 CU_TENSOR_MAP_L2_PROMOTION_L2_256B)))
             return rc;
     }
-    rc = C == 3 ? launch_rows<3>(ctx, map_dy, p, grid, pl.smem) : C == 1 ? launch_rows<1>(ctx, map_dy, p, grid, pl.smem)
-       : C == 4 ? launch_rows<4>(ctx, map_dy, p, grid, pl.smem) : launch_rows<0>(ctx, map_dy, p, grid, pl.smem);
+    rc = C == 3 ? launch_rows_n<3>(ctx, map_dy, p, grid, pl.smem) : C == 1 ? launch_rows_n<1>(ctx, map_dy, p, grid, pl.smem)
+       : C == 4 ? launch_rows_n<4>(ctx, map_dy, p, grid, pl.smem) : launch_rows_n<0>(ctx, map_dy, p, grid, pl.smem);
     if (rc) return rc;
     k_conv_tc_wgrad_rows_reduce<<<(nout + 31) / 32, 256, 0, ctx->stream>>>(p.slots, dw_f32, grid, nout);
     PCNN_CHECK_LAUNCH(ctx);

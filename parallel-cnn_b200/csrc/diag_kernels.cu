@@ -162,8 +162,8 @@ namespace {
 //   mode 2: 4 warps x 1 box {256 cols, 32 rows}, SWIZZLE_NONE (16 KB per instruction, 512-byte rows)
 //   mode 3: mode 0 with every lane issuing 1-D bulk stores of its own 128-byte row piece (no tensor map)
 //   mode 4: 4 warps x 4 boxes {64 cols, 32 rows} issued back to back by one lane, then one commit (group of 16 KB)
-//   mode 5: no TMA: every lane writes its row's 128-byte piece with four 32-byte st.global.v8 (SASS STG.256), 8 warps
-//   mode 6: half and half: the even column boxes by TMA (mode 0), the odd ones by direct 32-byte stores (mode 5)
+//   mode 5: no TMA: every lane writes its row's 128-byte piece with eight 16-byte st.global.v4 (STG.128, the widest on sm_90), 8 warps
+//   mode 6: half and half: the even column boxes by TMA (mode 0), the odd ones by direct 16-byte stores (mode 5)
 // `hot` = 1 makes every tile land on the first row block (an L2-resident target instead of HBM).
 struct StoreParams {
     int mode, hot, n_img, P, H, n_mtiles, n_qtiles, row_elems;
@@ -187,14 +187,14 @@ __global__ void __launch_bounds__(256, 1) k_tma_store_probe(const __grid_constan
         if (p.hot) { n = 0; pr = pr % 32; }
         const int c_tile = qt * 256;
         if (p.mode == 5 || (p.mode == 6 && colhalf == 1)) {
-            // direct path: every lane owns a row and writes its 128-byte piece as four 32-byte (full-sector) stores from registers
+            // direct path: every lane owns a row and writes its 128-byte piece as eight 16-byte stores from registers
             if (ok && pr + lane < p.P)
                 for (int col0 = colhalf * 64; col0 < 256; col0 += 128) {
                     if (c_tile + col0 + 64 > p.row_elems) continue;
                     unsigned char *dst = p.y + (((long long)n * p.P + pr + lane) * p.row_elems + c_tile + col0) * 2;
 #pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        asm volatile("st.global.v8.b32 [%0], {%1, %1, %1, %1, %1, %1, %1, %1};" ::"l"(dst + k * 32), "r"(tile + k) : "memory");
+                    for (int k = 0; k < 8; ++k)
+                        asm volatile("st.global.v4.b32 [%0], {%1, %1, %1, %1};" ::"l"(dst + k * 16), "r"(tile + k / 2) : "memory");
                 }
         } else if (p.mode == 0 || p.mode == 3 || p.mode == 6) {
             for (int col0 = colhalf * 64; col0 < 256; col0 += 128) {
@@ -316,46 +316,56 @@ extern "C" int pcnn_measure_tma_write(pcnn_ctx *ctx, void *dev_bf16, int N, int 
     return PCNN_OK;
 }
 
-// ---- tcgen05.mma issue/throughput probe -------------------------------------------------------------------------------
-// One CTA, one issuing thread: `reps` back-to-back tcgen05.mma (kind::f16, K = 16) on zero operands, rotating over `nacc`
-// accumulators, then one commit; reports SM clocks per MMA.  The convolution kernels size their MMAs against this table.
+// ---- wgmma issue/throughput probe -------------------------------------------------------------------------------------
+// One CTA of M / 64 warpgroups, each issuing `reps` back-to-back wgmma m64nNk16 on zero operands into its own register
+// accumulator (the 64-row halves of an M = 128 product are independent, as in the forward kernel's two consumer
+// warpgroups), then one wait; reports SM clocks per M x N x 16 product.  The convolution kernels size their MMAs against
+// this table.
 namespace {
 
-__global__ void __launch_bounds__(64, 1) k_mma_rate(int M, int N, int a_mn, int b_mn, int nacc, int reps, int walk, long long *out) {
+// A_MN / B_MN: operand majors as compile-time constants, so the timed loop is one straight wgmma stream
+template <int N, int A_MN, int B_MN>
+__global__ void __launch_bounds__(256, 1) k_mma_rate(int reps, int walk, long long *out) {
+    constexpr bool a_mn = A_MN != 0, b_mn = B_MN != 0;
     extern __shared__ unsigned char smem_dyn[];
     unsigned char *base = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
-    __shared__ unsigned long long bar;
-    __shared__ uint32_t tmem_slot;
-    for (int i = threadIdx.x * 16; i < 96 * 1024; i += 64 * 16) *reinterpret_cast<uint4 *>(base + i) = make_uint4(0, 0, 0, 0);
+    for (int i = threadIdx.x * 16; i < 96 * 1024; i += blockDim.x * 16) *reinterpret_cast<uint4 *>(base + i) = make_uint4(0, 0, 0, 0);
     fence_proxy_async_smem();
-    if (threadIdx.x == 0) { bar_init(&bar, 1); fence_barrier_init(); }
-    if (threadIdx.x < 32) tc_alloc(&tmem_slot, 512);
-    tc_fence_before();
+    const uint64_t ad = a_mn ? gmma_desc_mn_sw128(s_u32(base), 8192) : gmma_desc_k_sw128(s_u32(base));
+    const uint64_t bd = b_mn ? gmma_desc_mn_sw128(s_u32(base + 32768), 8192) : gmma_desc_k_sw128(s_u32(base + 32768));
+    // walk = 1: every MMA reads fresh operand tiles (A advances by its K-step footprint, B likewise, wrapping in 32 KB)
+    const uint32_t a_adv = walk ? (uint32_t)((a_mn ? 2048 : 32) >> 4) : 0u, b_adv = walk ? (uint32_t)((b_mn ? 2048 : 32) >> 4) : 0u;
+    const uint32_t a_wrap = a_mn ? 16u : 4u, b_wrap = b_mn ? 16u : 4u;     // steps before returning to the start
+    float acc[N / 2];
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) acc[i] = 0.0f;
+    wg_hold(acc);                                       // the zeroing stays ahead of the fence: one unbroken wgmma stream
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_slot;
-    if (threadIdx.x == 0) {
-        const uint32_t idesc = umma_idesc_bf16(M, N, a_mn, b_mn);
-        const uint64_t ad = a_mn ? umma_desc_mn_sw128(s_u32(base)) : umma_desc_k_sw128(s_u32(base));
-        const uint64_t bd = b_mn ? umma_desc(s_u32(base + 32768), 8192, 1024, 2) : umma_desc_k_sw128(s_u32(base + 32768));
-        const uint32_t accmask = (uint32_t)nacc - 1u, acc_cols = 512u / (uint32_t)nacc;
-        const long long t0 = clock64();
-        // walk = 1: every MMA reads fresh operand tiles (A advances by its K-step footprint, B likewise, wrapping in 32 KB)
-        const uint32_t a_adv = walk ? (uint32_t)((a_mn ? 2048 : 32) >> 4) : 0u, b_adv = walk ? (uint32_t)((b_mn ? 2048 : 32) >> 4) : 0u;
-        const uint32_t a_wrap = a_mn ? 16u : 4u, b_wrap = b_mn ? 16u : 4u;     // steps before returning to the start
-#pragma unroll 4
-        for (int i = 0; i < reps; ++i)
-            tc_mma_bf16(tmem + ((uint32_t)i & accmask) * acc_cols, ad + (uint64_t)(((uint32_t)i % a_wrap) * a_adv),
-                        bd + (uint64_t)(((uint32_t)i % b_wrap) * b_adv), idesc, 1u);
-        tc_commit(&bar);
-        bar_wait(&bar, 0);
-        const long long t1 = clock64();
-        out[0] = t1 - t0;
+    const long long t0 = clock64();
+    wg_fence();
+    for (int i = 0; i < reps; ++i) {
+        const uint64_t a = ad + (uint64_t)(((uint32_t)i % a_wrap) * a_adv), b = bd + (uint64_t)(((uint32_t)i % b_wrap) * b_adv);
+        wgmma_bf16<A_MN, B_MN>(acc, a, b, 1u);
     }
-    tc_fence_before();
+    wg_commit();
+    wg_wait<0>();
+    wg_hold(acc);
     __syncthreads();
-    if (threadIdx.x < 32) { tc_fence_after(); tc_dealloc(tmem, 512); }
+    const long long t1 = clock64();
+    float s = 0.0f;
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) s += acc[i];
+    if (threadIdx.x == 0) out[0] = t1 - t0 + (s != 0.0f ? 1 : 0);   // the operands are zero: s == 0 keeps the sum live only
 }
+
+typedef void (*mma_rate_fn)(int, int, long long *);
+template <int... Ns> struct MmaRateTable {
+    static const void *get(int N, int a_mn, int b_mn) {
+        static const mma_rate_fn t[][4] = {{k_mma_rate<Ns, 0, 0>, k_mma_rate<Ns, 0, 1>, k_mma_rate<Ns, 1, 0>, k_mma_rate<Ns, 1, 1>}...};
+        return reinterpret_cast<const void *>(t[N / 16 - 1][(a_mn ? 2 : 0) | (b_mn ? 1 : 0)]);
+    }
+};
+using MmaRate = MmaRateTable<16, 32, 48, 64, 80, 96, 112, 128, 144, 160, 176, 192, 208, 224, 240, 256>;
 
 }  // namespace
 
@@ -364,9 +374,12 @@ extern "C" int pcnn_measure_mma_rate(pcnn_ctx *ctx, int M, int N, int a_mn_major
                      (nacc == 1 || nacc == 2 || nacc == 4 || nacc == 8) && N * nacc <= 512,
                  PCNN_ERR_ARG, "pcnn_measure_mma_rate: bad argument");
     pcnn_device_guard g(ctx->device);
+    const void *fn = MmaRate::get(N, a_mn_major, b_mn_major);
     static bool configured[64] = {};        // function attributes are per device
     if (!configured[ctx->device & 63]) {
-        PCNN_CUDA(cudaFuncSetAttribute(k_mma_rate, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+        for (int n = 16; n <= 256; n += 16)
+            for (int v = 0; v < 4; ++v)
+                PCNN_CUDA(cudaFuncSetAttribute(MmaRate::get(n, v & 2, v & 1), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
         configured[ctx->device & 63] = true;
     }
     long long *out = nullptr;
@@ -374,7 +387,9 @@ extern "C" int pcnn_measure_mma_rate(pcnn_ctx *ctx, int M, int N, int a_mn_major
     if (rc) return rc;
     long long h = 0;
     for (int i = 0; i < 2; ++i) {      // second launch is the measurement (first warms the instruction cache)
-        k_mma_rate<<<1, 64, 98 * 1024, ctx->stream>>>(M, N, a_mn_major, b_mn_major, nacc, reps, getenv("PCNN_MMA_WALK") ? atoi(getenv("PCNN_MMA_WALK")) : 1, out);
+        int walk = getenv("PCNN_MMA_WALK") ? atoi(getenv("PCNN_MMA_WALK")) : 1;
+        void *args[] = {&reps, &walk, &out};
+        PCNN_CUDA(cudaLaunchKernel(fn, dim3(1), dim3(128 * (M / 64)), args, 98 * 1024, ctx->stream));
         PCNN_CHECK_LAUNCH(ctx);
     }
     PCNN_CUDA(cudaMemcpyAsync(&h, out, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));

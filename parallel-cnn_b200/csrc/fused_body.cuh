@@ -280,7 +280,7 @@ __device__ __forceinline__ void image_pass(FusedSmem<InT> &S, const ThreadId &id
     }
     // Single-lane blocks (TMA issue by lane 0 of warp 0, label fetch by lane 24 of warp 6) leave their warp diverged:
     // ptxas places the reconvergence point far downstream, and the butterfly shuffles below were then executed by
-    // a partial warp (observed on B200: warp 0's FC partial sums lost lane 0).  Reconverge explicitly.
+    // a partial warp (observed once: warp 0's FC partial sums lost lane 0).  Reconverge explicitly.
     __syncwarp();
 
     // ---- P1: c1 (5x5 valid conv, layer.h:105-140) + sigmoid, s1 (4x4/4 weighted sum, layer.h:143-181) + sigmoid

@@ -491,7 +491,7 @@ static int learn_host_chunked(pcnn_ctx *ctx, const void *host_images, int pixel_
     pcnn_device_guard g(ctx->device);
     const size_t px = (pixel_type == PCNN_F32 ? 4 : 1);
     // Chunks of ~16 MiB (80 steps at B = 256 u8): the per-chunk fixed cost (two copies, two memsets, events, one launch, one
-    // read-back: ~40 us measured) is then < 5 % of the chunk's compute; the first chunk is ~2 MiB so that the copy nothing
+    // read-back) is then small next to the chunk's compute; the first chunk is ~2 MiB so that the copy nothing
     // can overlap with stays short.
     long chunk_samples = ((long)(16 << 20) / (long)(PCNN_IMG * px));
     chunk_samples = (chunk_samples / B) * B;
@@ -553,7 +553,7 @@ static int learn_host_chunked(pcnn_ctx *ctx, const void *host_images, int pixel_
 }
 
 // Persistent mode: ONE cooperative launch per epoch.  The epoch's samples are staged in HBM chunk by chunk on the copy
-// stream (180 GB of HBM: the whole host dataset fits, up to HS_SEGMENT_BYTES per launch); every chunk is followed by a
+// stream (80 GB of HBM: the whole host dataset fits, up to HS_SEGMENT_BYTES per launch); every chunk is followed by a
 // 4-byte flag copy, and the kernel -- launched right after the FIRST chunk has been enqueued -- waits on the flag of a
 // sample's chunk before it issues that sample's bulk copy.  Per-step error sums go straight to mapped pinned host memory.
 // Host work per call: one launch, 2 copies per chunk, one blocking read-back at the end; no per-chunk synchronisation.

@@ -7,7 +7,7 @@
 // parameters in shared memory (nothing but the 784-byte image crosses HBM per sample), per-CTA partial gradients,
 // fixed-order slot reduction + update in a second kernel: deterministic, no atomics.
 // The image pass is register-tiled and balanced phase by phase (see k_l5_step); the first version of this file (one thread per
-// output, parameter-stationary gradient sums with up to 864-term serial chains) ran at 152 us per 256-image step.
+// output, parameter-stationary gradient sums with up to 864-term serial chains) was bound by those serial chains.
 #include "pcnn_internal.h"
 #include "fused_body.cuh"
 

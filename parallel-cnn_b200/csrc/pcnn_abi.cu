@@ -40,8 +40,8 @@ extern "C" int pcnn_create(pcnn_ctx **out, int device, void *stream) {
     PCNN_REQUIRE(device < ndev, PCNN_ERR_ARG, "pcnn_create: device %d out of range (%d devices)", device, ndev);
     cudaDeviceProp prop;
     PCNN_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) {
-        pcnn_set_error("pcnn_create: device %d is sm_%d%d; libpcnn.so carries sm_100a code only", device,
+    if (prop.major != 9 || prop.minor != 0) {
+        pcnn_set_error("pcnn_create: device %d is sm_%d%d; libpcnn.so carries sm_90a code only", device,
                        prop.major, prop.minor);
         return PCNN_ERR_NOGPU;
     }

@@ -2,15 +2,17 @@
 // `nsteps` consecutive mini-batch steps without returning to the host, the gradient reduction, the SGD update, the
 // multi-GPU exchange and the parameter broadcast all inside the kernel.  Round 1 synchronised the steps with two fenced
 // grid barriers; this version is a dataflow over thread-block clusters, asynchronous distributed-shared-memory stores and
-// tagged words in L2 (A/B numbers of both: profiles/r02_persist_phase_trace_ab.jsonl).
+// tagged words in L2.
 #include "fused_body.cuh"
 
 using namespace pcnn_fused;
 
 namespace {
 
-constexpr int XS_MAXC = 40;          // clusters per rank the direct exchange has room for (a B200 holds 33 clusters of 8)
-constexpr int PCNN_DIRECT_MAX_WORLD = 2;   // measured: 2 GPUs 9.86 vs 10.95 us per step; 4 GPUs 11.27 vs 11.14 (no gain: 3 x 0.6 MB of stores per step and GPU)
+constexpr int XS_MAXC = 40;          // clusters per rank the direct exchange has room for (an H100 holds 16 clusters of 8)
+// most GPUs the direct exchange serves: each GPU stores (N - 1) x 0.6 MB per step into its peers, which grows with N while the
+// L2 hop it saves does not.  Multi-GPU step times have not been measured on H100; 2 is the world size the scheme was built for.
+constexpr int PCNN_DIRECT_MAX_WORLD = 2;
 static size_t p2p_inbox_bytes() { return (size_t)2 * PCNN_MAX_PEERS * NPACK * sizeof(uint2); }
 static size_t p2p_xslots_bytes() { return (size_t)2 * PCNN_MAX_PEERS * XS_MAXC * NPACK * sizeof(unsigned long long); }
 
@@ -246,7 +248,7 @@ __device__ __forceinline__ int step_images(FusedSmem<InT> &S, const ThreadId &id
 }
 
 // DIRECT (2 GPUs, see PersistArgs::xslots) is compile-time: as a run-time flag the generalised slot addressing of the owner gather
-// cost every configuration 0.65 us per step (8.49 -> 9.13 us on one GPU, scripts/step_ab_raw.py).
+// is paid by every configuration, one GPU included (compare builds with scripts/step_ab_raw.py).
 template <typename InT, int CS, bool DIRECT>
 __global__ void __launch_bounds__(NT, FUSED_CTAS_PER_SM) k_train_persist(const PersistArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -341,8 +343,8 @@ __global__ void __launch_bounds__(NT, FUSED_CTAS_PER_SM) k_train_persist(const P
         PCNN_TRACE2(1);
 
         // Images in pinned HOST memory (pcnn_learn_host): the NEXT step's first image is requested now, a whole step ahead, so that
-        // the ~2 us of PCIe latency disappear behind the step; the other staging buffer is free (one image per CTA and step;
-        // with more, the in-step prefetch chain owns it).  Device-resident data keep the late request (0.08 us per step cheaper).
+        // the PCIe latency disappears behind the step; the other staging buffer is free (one image per CTA and step;
+        // with more, the in-step prefetch chain owns it).  Device-resident data keep the late request (no PCIe latency to hide).
         const bool early_issue = a.early != 0 && nb <= G;
         if (early_issue && t == 0 && s + 1 < a.nsteps) {
             long long ecur = cursor + stride;
@@ -699,9 +701,8 @@ int pcnn_persist_run(pcnn_ctx *ctx, const pcnn_split_binding &s, int B, long nst
             int grid = 0, cs = 1;
             persist_geometry(ctx, B, &grid, &cs);
             // 2 GPUs: the cluster shares go straight into the peer's memory and the owners gather ranks x clusters slots (one
-            // NVLink hop replaces an L2 hop + the separate exchange: 9.86 vs 10.95 us per step).  With more GPUs the per-step
-            // NVLink volume of that scheme ((N - 1) x 0.6 MB per GPU) costs what it saves (4 GPUs: 11.27 vs 11.14 us) and the
-            // owners exchange their 9.4 KB of sums instead
+            // NVLink hop replaces an L2 hop + the separate exchange).  With more GPUs the per-step NVLink volume of that scheme
+            // ((N - 1) x 0.6 MB per GPU) grows and the owners exchange their 9.4 KB of sums instead (PCNN_DIRECT_MAX_WORLD)
             a.direct = (ctx->world >= 2 && ctx->world <= PCNN_DIRECT_MAX_WORLD && cs > 1 && grid / cs <= XS_MAXC && grid > 16 &&
                         !ctx->persist_no_direct) ? 1 : 0;
             const void *fn;

@@ -1,4 +1,4 @@
-// parallel-cnn_b200/driver/main.cpp -- the training driver of the reference (Sequential/Main.cpp) on the B200 engine.
+// parallel-cnn_b200/driver/main.cpp -- the training driver of the reference (Sequential/Main.cpp) on the H100 engine.
 //
 // Same entry points and the same stdout lines as the reference driver [ref: Sequential/Main.cpp:36-214]:
 //   loaddata()      -> reads the four IDX files under data/ (u8 payload kept as u8, return codes checked)

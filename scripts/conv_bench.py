@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""scripts/conv_bench.py -- throughput of the bf16 tcgen05 convolution forward (BASELINE.json configs 3 and 5) against the
+"""scripts/conv_bench.py -- throughput of the bf16 wgmma convolution forward (BASELINE.json configs 3 and 5) against the
 HBM roofline.  Algorithmic bytes per image are SURVEY.md 8d's: each operand crosses HBM once (input read + output written,
 bf16): LeNet c1 8,480 B, 224x224x3 -> 64 x 3x3: 6,609,408 B.  CUDA-event timing over back-to-back launches after warm-up;
-the working set of every measured point except the smallest batches exceeds the 126 MB L2."""
+the working set of every measured point except the smallest batches exceeds the 50 MB L2."""
 import json
 import os
 import sys
@@ -19,7 +19,7 @@ torch.cuda.set_device(0)
 stream = torch.cuda.Stream()
 torch.cuda.set_stream(stream)
 eng = pkg.Engine(0, stream.cuda_stream)
-HBM = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
+HBM = 3350.0                        # GB/s, NVIDIA H100 SXM data sheet (HBM3)
 rng = np.random.default_rng(1234)
 only = sys.argv[1] if len(sys.argv) > 1 else "all"
 
@@ -124,7 +124,7 @@ if only in ("all", "cfg5"):
 eng.close()
 if only == "wprobe":                                                   # what a pure WRITE stream / pure READ stream / copy reach on this GPU
     # library fill / reduce / copy kernels as a yardstick for the store-dominated forward pass (807 MB written, 39 MB read):
-    # MEASURED_PEAKS.json's HBM number is a COPY (half reads, half writes)
+    # the data-sheet HBM number counts reads and writes together
     nbytes = 807 << 20
     buf = torch.empty((nbytes // 4,), dtype=torch.int32, device="cuda")
     src = torch.ones((nbytes // 4,), dtype=torch.int32, device="cuda")

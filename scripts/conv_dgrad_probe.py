@@ -1,7 +1,6 @@
 #!/usr/bin/env python
-"""scripts/conv_dgrad_probe.py -- why bench.py's conv block timed the input gradient at 187 us while scripts/conv_bench.py
-timed the same call at 146 us (round-1 VERDICT "what's weak" 4): the same shape (config 5, N = 128) with the operands of
-either harness, in either order, plus fresh allocations."""
+"""scripts/conv_dgrad_probe.py -- whether bench.py's conv block and scripts/conv_bench.py time the input gradient alike:
+the same shape (config 5, N = 128) with the operands of either harness, in either order, plus fresh allocations."""
 import json
 import os
 import sys

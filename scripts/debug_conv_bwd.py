@@ -31,7 +31,7 @@ if what == "wgrad":
     rel = np.linalg.norm((got - ref).astype(np.float64)) / np.linalg.norm(ref.astype(np.float64))
     print("wgrad", sys.argv[2:9], tag, "rel-L2", rel, "ref[0,0,0,:]", ref[0, 0, 0], "got", got[0, 0, 0], flush=True)
     if rel > 1e-3:
-        # which k rows match?  (diagnoses the TMEM lane map of an M = 64 accumulator)
+        # which k rows match?  (diagnoses the row map of an M = 64 accumulator)
         for k in range(0, K, 8):
             e = np.abs(got[k] - ref[k]).max() / (np.abs(ref[k]).max() + 1e-9)
             print("  k", k, "max rel err", e)

@@ -24,7 +24,7 @@ eng = pkg.Engine(0, stream.cuda_stream)
 rng = np.random.default_rng(7)
 NPARAM = 5152
 FLOPS_PER_IMAGE = 2 * 6 * 576 * 25 * 2 + 2 * 16 * 64 * 150 * 3 + 2 * 10 * 256 * 3 + 2 * 6 * 144 * 16 * 3
-NSET = 262144                                               # 205 MB of u8 pixels > 126 MB L2
+NSET = 262144                                               # 205 MB of u8 pixels > 50 MB L2
 
 imgs = torch.randint(0, 256, (NSET, 784), dtype=torch.uint8, device="cuda")
 labs = torch.randint(0, 10, (NSET,), dtype=torch.uint8, device="cuda")

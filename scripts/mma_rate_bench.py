@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""scripts/mma_rate_bench.py -- SM clocks per tcgen05.mma for the instruction shapes the convolution kernels can choose from."""
+"""scripts/mma_rate_bench.py -- SM clocks per wgmma product for the instruction shapes the convolution kernels can choose from."""
 import json
 import os
 import sys

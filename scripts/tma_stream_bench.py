@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """scripts/tma_stream_bench.py -- streaming-read ceiling of a TMA pipeline over dy [N,222,222,64] bf16 (config 5's big tensor) for the
-box shapes of the convolution backward kernels (pcnn_measure_tma_read), next to MEASURED_PEAKS.json's HBM copy rate."""
+box shapes of the convolution backward kernels (pcnn_measure_tma_read), next to the H100 SXM data-sheet HBM bandwidth (3.35 TB/s)."""
 import json
 import os
 import sys

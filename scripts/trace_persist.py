@@ -1,8 +1,7 @@
 #!/usr/bin/env python
 """scripts/trace_persist.py -- per-phase timing of the persistent training kernel from its own %globaltimer stamps
 (CTA 0's view): parameter fetch, images, epilogue + cluster reduce, owner gather, exchange/update/publish.
-`--cluster=1` traces the variant without thread-block clusters.  (The round-1 grid-barrier kernel this replaced is in
-profiles/r02_persist_phase_trace_ab.jsonl, measured in the same call.)
+`--cluster=1` traces the variant without thread-block clusters.
 
     python scripts/trace_persist.py [B,B,...] [--cluster=1]
 """

@@ -1,6 +1,6 @@
 """ctypes access to the parity checkers under oracle/ (TEST INFRASTRUCTURE ONLY).
 
-`oracle()` loads oracle/liblenet_oracle.so, the C restatement of /root/reference/Sequential/layer.h + Main.cpp.
+`oracle()` loads oracle/liblenet_oracle.so, the C restatement of the reference's Sequential/layer.h + Main.cpp.
 `reference()` loads oracle/_ref/libref_seq.so, the unmodified reference compiled where it lies (None when absent).
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs import this module.
 """
@@ -93,7 +93,7 @@ def oracle():
 
 
 def reference(native=False):
-    """The unmodified reference, or None when oracle/_ref was not built (no /root/reference at build time).
+    """The unmodified reference, or None when oracle/_ref was not built (no reference sources at build time).
     native=True: the same sources built -O3 with FMA contraction (bench.py's best-CPU timing; NOT a parity checker)."""
     global _ref, _ref_native
     if native:
@@ -120,6 +120,57 @@ def reference(native=False):
         L.ref_vectorNorm.restype = C.c_float
         _ref = L
     return _ref
+
+
+def bits_digest(a):
+    """SHA-256 of the float32 bit patterns of `a` (equal digests = bit-identical arrays)."""
+    import hashlib
+    return hashlib.sha256(np.ascontiguousarray(a, np.float32).tobytes()).hexdigest()
+
+
+def ops_chain(lib, reference, seed=1234, trials=5):
+    """Every operator of Sequential/layer.h on seeded random inputs, chained as one train step chains them, through `lib`:
+    the unmodified reference (reference=True, ref_* symbols) or the C restatement (orc_* symbols).  Returns
+    {"<trial>.<op>": float32 array}; tests/golden/reference_ops_random.json holds bits_digest() of the reference's result."""
+    rng = np.random.default_rng(seed)
+    pre = "ref_" if reference else "orc_"
+    fn = lambda name: getattr(lib, pre + name)
+    make_error = lib.ref_makeError if reference else lib.orc_make_error
+    norm = lib.ref_vectorNorm if reference else lib.orc_vector_norm
+    f32 = lambda n: np.empty(n, np.float32)
+
+    def r(*shape, lo=-1.0, hi=1.0):
+        return np.ascontiguousarray(rng.uniform(lo, hi, shape).astype(np.float32))
+
+    out = {}
+    for t in range(trials):
+        inp, w1, b1 = r(784, lo=0, hi=1), r(150, lo=-.5, hi=.5), r(6, lo=-.5, hi=.5)
+        o1 = f32(3456); fn("fp_c1")(fp(inp), fp(o1), fp(w1), fp(b1))
+        s1 = f32(3456); fn("apply_step_function")(fp(o1), fp(s1), 3456)
+        w2, b2 = r(16), r(1)
+        p1 = f32(216); fn("fp_s1")(fp(s1), fp(p1), fp(w2), fp(b2))
+        x216, wf, bf = r(216, lo=0, hi=1), r(2160), r(10)
+        f1 = f32(10); fn("fp_preact_f")(fp(x216), fp(f1), fp(wf)); fn("fp_bias_f")(fp(f1), fp(bf))
+        out10 = r(10, lo=0, hi=1)
+        e1 = f32(10); make_error(fp(e1), fp(out10), t, 10)
+        nrm = np.array([norm(fp(e1), 10)], np.float32)
+        d1 = f32(2160); fn("bp_weight_f")(fp(d1), fp(e1), fp(x216))
+        bfa = bf.copy(); fn("bp_bias_f")(fp(bfa), fp(e1))
+        q1 = f32(216); fn("bp_output_s1")(fp(q1), fp(wf), fp(e1))
+        t1 = f32(216); fn("bp_preact_s1")(fp(t1), fp(q1), fp(p1))
+        g1 = f32(16); fn("bp_weight_s1")(fp(g1), fp(t1), fp(s1))
+        b2a = b2.copy(); fn("bp_bias_s1")(fp(b2a), fp(t1))
+        u1 = f32(3456); fn("bp_output_c1")(fp(u1), fp(w2), fp(t1))
+        v1 = f32(3456); fn("bp_preact_c1")(fp(v1), fp(u1), fp(o1))
+        h1 = f32(150); fn("bp_weight_c1")(fp(h1), fp(v1), fp(inp))
+        b1a = b1.copy(); fn("bp_bias_c1")(fp(b1a), fp(v1))
+        wa = wf.copy(); fn("apply_grad")(fp(wa), fp(d1), 2160)
+        for name, v in (("fp_c1", o1), ("apply_step_function", s1), ("fp_s1", p1), ("fp_f", f1), ("make_error", e1),
+                        ("vector_norm", nrm), ("bp_weight_f", d1), ("bp_bias_f", bfa), ("bp_output_s1", q1),
+                        ("bp_preact_s1", t1), ("bp_weight_s1", g1), ("bp_bias_s1", b2a), ("bp_output_c1", u1),
+                        ("bp_preact_c1", v1), ("bp_weight_c1", h1), ("bp_bias_c1", b1a), ("apply_grad", wa)):
+            out[f"{t}.{name}"] = v
+    return out
 
 
 # ---------------------------------------------------------------- LeNet-5-style variant (oracle/lenet5_oracle.c; parity unpinned)

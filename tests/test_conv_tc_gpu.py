@@ -1,4 +1,4 @@
-"""GPU parity tests of the bf16 tcgen05 convolution (csrc/conv_tc.cu, SURVEY.md x3).
+"""GPU parity tests of the bf16 wgmma convolution (csrc/conv_tc.cu, SURVEY.md x3).
 
 PARITY UNPINNED by the reference (no bf16 / tensor-core path exists there).  The checker is the direct convolution
 orc_conv_fwd_nhwc (oracle/lenet_oracle.c: the reference's conv semantics, layer.h:118-130, generalised to C channels and
@@ -204,7 +204,7 @@ def test_conv_wgrad_and_dgrad_vs_oracle(eng, pkg, shape):
                                    (2, 40, 40, 3, 16, 3, 3, 0),       # 16 filters
                                    (1, 24, 32, 3, 96, 3, 3, 0)])      # 96 filters -> two groups of 64
 def test_filter_counts_that_are_not_multiples_of_64_run_on_the_tensor_cores(eng, pkg, shape):
-    """K % 64 != 0: dy is zero-padded to the next multiple of 64 filters and the 64-filter tcgen05 kernels run (VERDICT r1 item 7);
+    """K % 64 != 0: dy is zero-padded to the next multiple of 64 filters and the 64-filter wgmma kernels run (VERDICT r1 item 7);
     results against the oracle and against the reference kernels, launch counts prove the tensor-core path ran."""
     N, H, W, C, K, R, S, pitch = shape
     pitch = pitch or W * C
@@ -274,7 +274,7 @@ BWD_TC_SHAPES = [(1, 224, 224, 3, 64, 3, 3),      # config 5
 
 @pytest.mark.parametrize("shape", BWD_TC_SHAPES)
 def test_tensor_core_wgrad_and_dgrad_vs_oracle_and_fma_path(eng, pkg, shape):
-    """The tcgen05 backward kernels (csrc/conv_wgrad_tc.cu, csrc/conv_dgrad_tc.cu; 64 filters) against the oracle on the same bf16-rounded operands, and
+    """The wgmma backward kernels (csrc/conv_wgrad_tc.cu, csrc/conv_dgrad_tc.cu; 64 filters) against the oracle on the same bf16-rounded operands, and
     against the FMA-pipe kernels of csrc/conv_bwd.cu (pcnn_conv_bwd_select).  fp32 accumulation everywhere:
     wgrad rel-L2 <= 1e-5 vs the oracle; dgrad |d| <= 2^-8 |ref| + 1e-3 (one bf16 rounding of the result)."""
     N, H, W, C, K, R, S = shape
@@ -342,16 +342,17 @@ def test_tensor_core_dgrad_honours_row_and_image_pitch(eng, pkg):
 
 
 def test_measurement_probes_report_sane_rates(eng, pkg):
-    """pcnn_measure_mma_rate / pcnn_measure_tma_read (the tables DESIGN.md 3.7 designs against): one small tcgen05.mma costs tens
-    of clocks, not hundreds; a TMA pipeline with contiguous boxes streams well above 1 TB/s and faster than the row-gather one."""
+    """pcnn_measure_mma_rate / pcnn_measure_tma_read (the tables DESIGN.md 3.7 designs against): one small M = 128 wgmma product costs
+    tens of clocks, not hundreds; a TMA pipeline streams well above 1 TB/s with contiguous boxes and with the row-gather boxes alike
+    (on H100 both reach the same HBM ceiling: 2,812 vs 2,814 GB/s measured, so neither is required to beat the other)."""
     clk = eng.measure_mma_rate(128, 64, 0, 0, 1, 2000)
     assert 30.0 < clk < 200.0, clk
-    assert eng.measure_mma_rate(128, 256, 0, 0, 1, 2000) > 1.5 * clk         # N = 256 runs at the tensor-pipe peak (128 clk)
+    assert eng.measure_mma_rate(128, 256, 0, 0, 1, 2000) > 1.5 * clk         # N = 256 is bound by the tensor pipe, not by issue
     N, P, Q = 16, 222, 222
     buf = eng.array((N, P, Q, 64), np.uint16)
     contiguous = eng.measure_tma_read(buf, N, P, Q, 3, 5)
     gather = eng.measure_tma_read(buf, N, P, Q, 2, 5)
-    assert contiguous > 1000.0 and gather > 300.0 and contiguous > gather, (contiguous, gather)
+    assert contiguous > 1000.0 and gather > 1000.0, (contiguous, gather)
 
 
 def test_same_padding_convolution_through_pad_and_crop(eng, pkg):

@@ -51,7 +51,7 @@ DROPIN = os.path.join(O.ROOT, "oracle", "_ref", "seq_main_b200")
 
 
 @needs_data
-@pytest.mark.skipif(not os.path.exists(DROPIN), reason="oracle/_ref/seq_main_b200 is built where /root/reference exists (oracle/Makefile: dropin)")
+@pytest.mark.skipif(not os.path.exists(DROPIN), reason="oracle/_ref/seq_main_b200 is built where the reference sources exist (oracle/Makefile: dropin)")
 def test_the_reference_driver_itself_runs_on_the_engine(golden):
     """INTEGRATION.md section 1, literally: the reference's own Sequential/Main.cpp, with only its two host dereferences of
     device memory rewritten (Main.cpp:168, :191), compiled against include/layer.h and linked to libpcnn.so.  Every one of

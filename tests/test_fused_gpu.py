@@ -222,7 +222,7 @@ def test_full_epoch_reproduces_reference_headline(eng, pkg, golden):
     """Config 1 of BASELINE.json: the whole of Main.cpp (learn + test) at batch 1 on the real dataset."""
     full = O.full_mnist()
     if full is None:
-        pytest.skip("full MNIST IDX files not staged under oracle/_ref/data (built where /root/reference exists)")
+        pytest.skip("full MNIST IDX files not staged under oracle/_ref/data (built where the reference sources exist)")
     tr, trl, te, tel = full
     eng.dataset_upload(pkg.TRAIN_SET, tr, trl)
     eng.dataset_upload(pkg.TEST_SET, te, tel)

@@ -96,6 +96,6 @@ def test_data_parallel_equals_single_gpu(mode, batch):
     assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
     assert "MGPU_OK" in r.stdout, r.stdout[-3000:]
     log_dir = os.environ.get("PCNN_MGPU_LOG_DIR")
-    if log_dir:      # scripts/gpu_multi.sh keeps the workers' lines as committed evidence (profiles/)
+    if log_dir:      # optional: keep the workers' parity lines as a log
         with open(os.path.join(log_dir, f"mgpu_parity_n{world}.log"), "a") as f:
             f.write("".join(ln + "\n" for ln in r.stdout.splitlines() if "mode=" in ln or "MGPU" in ln))
