@@ -265,13 +265,14 @@ int pcnn_l5_forward(pcnn_ctx *ctx, const float *params_dev, const void *images_d
  * K filters of R x S taps, on the wgmma tensor cores with register accumulators and TMA-fed operands (csrc/conv_tc.cu).
  * Activations are NHWC bf16 with a row pitch of `row_pitch` elements (>= W*C, multiple of 8); filters fp32 KRSC on the
  * host (rounded to bf16 once, at plan creation); output NHWC bf16 [N][H-R+1][W-S+1][K], bias and optional sigmoid fused.
+ * Pad contents are ignored by the forward, the weight gradient and the input gradient alike: the pad columns W*C ..
+ * row_pitch-1 and the pad rows H .. image_rows-1 of x may hold anything, NaN included, without changing a result bit.
  * Constraint of this round: some pixel block Qt with (Qt+S-1)*C <= 32, Qt*K <= 256 and Qt*K % 16 == 0 must exist
  * (LeNet c1: Qt = 24; 224x224x3 -> 64 x 3x3: Qt = 4).  PARITY UNPINNED by the reference (it has no bf16 path): the
  * checker is orc_conv_fwd_nhwc in oracle/lenet_oracle.c on the bf16-rounded operands. */
 typedef struct pcnn_conv_plan pcnn_conv_plan;
 int pcnn_conv_tc_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int row_pitch,
-                             int image_rows /* rows between consecutive images in memory, >= H; 0 = H.  A multiple of
-                                               32 lets the epilogue use asynchronous TMA stores */,
+                             int image_rows /* rows between consecutive images in memory, >= H; 0 = H */,
                              int act, const float *filt_host, const float *bias_host, pcnn_conv_plan **plan_out);
 /* the same with a window step of `stride` (1..4) in both directions (SURVEY.md 8f row 4): y [N][(H-R)/stride+1][(W-S)/stride+1][K];
  * rows per image (image_rows, or H) must be a multiple of the stride; the pixel block then needs ((Qt-1)*stride+S)*C <= 32.
@@ -280,6 +281,11 @@ int pcnn_conv_tc_plan_create_strided(pcnn_ctx *ctx, int N, int H, int W, int C, 
                                      int image_rows, int act, const float *filt_host, const float *bias_host,
                                      pcnn_conv_plan **plan_out);
 int pcnn_conv_tc_plan_destroy(pcnn_ctx *ctx, pcnn_conv_plan *plan);
+/* Host-only query (works without a GPU and without a context): how pcnn_conv_tc_plan_create_strided tiles a shape.
+ * out5 = { Qt output pixels per tile, V Toeplitz alignment variants, activation stages, row tiles of 128 rows, pixel tiles per row }.
+ * The persistent kernel runs min(tiles, SMs) CTAs over the n_mtiles * n_qtiles tiles.  Shapes the plan refuses return the same
+ * error here. */
+int pcnn_conv_tc_plan_info(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows, int *out5);
 int pcnn_conv_tc_fwd(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *x_bf16_dev, void *y_bf16_dev);
 /* Backward passes of the same convolution (bf16 operands, fp32 accumulation, deterministic; wgmma kernels, see
  * pcnn_conv_bwd_select): weight gradient fp32 KRSC [ref: layer.h:371-395 bp_weight_c1, without its /576] and input gradient

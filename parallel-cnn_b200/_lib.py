@@ -114,6 +114,7 @@ _SIG = {
     "pcnn_conv_tc_plan_create": [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _pvp],
     "pcnn_conv_tc_plan_create_strided": [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _pvp],
     "pcnn_conv_tc_plan_destroy": [_vp, _vp],
+    "pcnn_conv_tc_plan_info": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_conv_tc_fwd": [_vp, _vp, _vp, _vp],
     "pcnn_f32_to_bf16_rows": [_vp, _vp, _vp, _l, _i, _i],
     "pcnn_conv_bwd_plan_info": [_i, _i, _i, _i, _i, _i, _i, _vp],
@@ -160,6 +161,23 @@ def init_params_reference():
     p = np.empty(NPARAM, np.float32)
     check("pcnn_init_params_reference", lib().pcnn_init_params_reference(p.ctypes.data))
     return p
+
+
+def conv_tc_plan_info(N, H, W, C, K, R, S, stride=1, row_pitch=None, image_rows=0):
+    """How the forward convolution plan tiles a shape (pcnn_conv_tc_plan_info; host only, no GPU).  row_pitch None = W*C
+    rounded up to 8 elements, as ConvPlan."""
+    pitch = (W * C + 7) // 8 * 8 if row_pitch is None else row_pitch
+    out = (_i * 5)()
+    check("pcnn_conv_tc_plan_info", lib().pcnn_conv_tc_plan_info(N, H, W, C, K, R, S, int(stride), int(pitch), int(image_rows), out))
+    return dict(Qt=out[0], V=out[1], stages=out[2], n_mtiles=out[3], n_qtiles=out[4], tiles=out[3] * out[4])
+
+
+def conv_bwd_plan_info(N, H, W, C, K, R, S):
+    """Which kernels the backward passes pick for a shape and how they tile it (pcnn_conv_bwd_plan_info; host only, no GPU)."""
+    out = (_i * 9)()
+    check("pcnn_conv_bwd_plan_info", lib().pcnn_conv_bwd_plan_info(N, H, W, C, K, R, S, out))
+    return dict(wgrad_tc=bool(out[0]), wgrad_rb=out[1], wgrad_pc=out[2], wgrad_stages=out[3],
+                dgrad_tc=bool(out[4]), dgrad_strips=out[5], dgrad_oq=out[6], dgrad_ring=out[7], dgrad_stages=out[8])
 
 
 def mnist_load_u8(image_file, label_file):

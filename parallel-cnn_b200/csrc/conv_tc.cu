@@ -8,7 +8,8 @@
 // Toeplitz matrix that depends only on (w - q).  Tiling the output row into blocks of Qt pixels makes the band a
 // small CONSTANT matrix: for a block starting at q0 only the (Qt+S-1)*C <= 32 input elements from column q0*C matter,
 // and T_r restricted to them is the same [32 x Qt*K] matrix for every block, every row and every image.  So
-//   * A tiles are plain 2-D TMA boxes [128 rows x 32 elements] of the activation tensor viewed as [N*H][W*C]
+//   * A tiles are plain TMA boxes [128 rows x 32 elements] of the activation tensor viewed as [N*H][W*C] (rows `pitch` apart;
+//     the view is 3-D for window steps > 1, see pcnn_conv_tc_fwd)
 //     (row r of the filter = the same box shifted down by r rows): zero im2col traffic, the 16x..25x expansion of
 //     im2col never exists anywhere, not even in shared memory;
 //   * B = R matrices [Qt*K x 32] (<= 48 KB) built once on the host from the filter bank, resident in shared memory;
@@ -44,9 +45,9 @@ struct ConvTcParams {
     int n_img, H, P, Q, K, R;      // images, input rows per image, valid output rows/cols, filters, filter rows
     int Qt, ncols, npad;           // output pixels per tile, Qt * K, MMA width (ncols rounded up to 32)
     int C;                         // input channels (column offset of a tile = q0 * stride * C elements)
-    int stride;                    // step of the window in both directions (1 = the reference's conv, layer.h:118-130)
-    int x_pitch;                   // elements between input rows: filter row r of a stride-s conv reads view row r / s at
-                                   // column offset (r % s) * x_pitch of the input viewed as [N * H / s][s * x_pitch]
+    int stride;                    // step of the window in both directions (1 = the reference's conv, layer.h:118-130); filter
+                                   // row r of a stride-s conv reads sub-row r % s of view row r / s of the input viewed as
+                                   // [N * H / s][s][W * C] (see pcnn_conv_tc_fwd)
     int V;                         // Toeplitz variants: the box start is rounded down to 8 elements (16 B, a TMA
                                    // requirement on the global address), the remainder (q0*C) % 8 selects the variant
     int stages;                    // activation stages that fit next to the V * R Toeplitz matrices
@@ -120,8 +121,8 @@ k_conv_tc_fwd(const __grid_constant__ CUtensorMap map_x, const __grid_constant__
                 const int mt = tile / p.n_qtiles, qt = tile % p.n_qtiles;
                 bar_expect_tx(&S.full[stage], (unsigned)(p.R * A_TILE_BYTES));
                 for (int r = 0; r < p.R; ++r)
-                    tma_load_2d(sv.a(stage, r), &map_x, ((qt * p.Qt * p.stride * p.C) & ~7) + (r % p.stride) * p.x_pitch,
-                                mt * TC_M + r / p.stride, &S.full[stage]);
+                    tma_load_3d(sv.a(stage, r), &map_x, (qt * p.Qt * p.stride * p.C) & ~7, r % p.stride, mt * TC_M + r / p.stride,
+                                &S.full[stage]);
             }
         }
         return;
@@ -242,10 +243,11 @@ extern "C" int pcnn_conv_tc_plan_create(pcnn_ctx *ctx, int N, int H, int W, int 
     return pcnn_conv_tc_plan_create_strided(ctx, N, H, W, C, K, R, S, 1, row_pitch, image_rows, act, filt_host, bias_host, out);
 }
 
-extern "C" int pcnn_conv_tc_plan_create_strided(pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch,
-                                                int image_rows, int act, const float *filt_host, const float *bias_host,
-                                                pcnn_conv_plan **out) {
-    PCNN_REQUIRE(ctx && filt_host && out, PCNN_ERR_ARG, "pcnn_conv_tc_plan_create: NULL argument");
+// Tiling of the forward convolution (host logic only, no device): pixel block Qt, its alignment variants V, activation stages
+// and the tile grid.  pcnn_conv_tc_plan_create_strided builds its plan from it and pcnn_conv_tc_plan_info reports it.
+struct ConvTcShape { int Qt, V, stages, P, Q, rows, n_mtiles, n_qtiles; };
+
+static int conv_tc_shape(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows, ConvTcShape *out) {
     PCNN_REQUIRE(stride >= 1 && stride <= 4, PCNN_ERR_ARG, "pcnn_conv_tc_plan_create: stride %d outside 1..4", stride);
     PCNN_REQUIRE(N > 0 && H >= R && W >= S && C > 0 && K > 0 && R > 0 && R <= TC_MAX_R && S > 0, PCNN_ERR_ARG,
                  "pcnn_conv_tc_plan_create: bad shape N=%d H=%d W=%d C=%d K=%d R=%d S=%d", N, H, W, C, K, R, S);
@@ -276,6 +278,32 @@ extern "C" int pcnn_conv_tc_plan_create_strided(pcnn_ctx *ctx, int N, int H, int
     }
     PCNN_REQUIRE(Qt > 0, PCNN_ERR_ARG,
                  "pcnn_conv_tc_plan_create: no pixel block with ((Qt-1)*stride+S)*C (+ alignment remainder) <= 32, Qt*K <= 256, %%16 == 0");
+    out->Qt = Qt; out->V = V; out->stages = stages; out->P = P; out->Q = Q;
+    out->rows = image_rows / stride;                  // tile rows per image: units of `stride` input rows
+    out->n_mtiles = (int)(((long long)N * out->rows + TC_M - 1) / TC_M);
+    out->n_qtiles = (Q + Qt - 1) / Qt;
+    return PCNN_OK;
+}
+
+extern "C" int pcnn_conv_tc_plan_info(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows,
+                                      int *out5) {
+    PCNN_REQUIRE(out5, PCNN_ERR_ARG, "pcnn_conv_tc_plan_info: NULL argument");
+    ConvTcShape sh;
+    int rc = conv_tc_shape(N, H, W, C, K, R, S, stride, row_pitch, image_rows, &sh);
+    if (rc) return rc;
+    out5[0] = sh.Qt; out5[1] = sh.V; out5[2] = sh.stages; out5[3] = sh.n_mtiles; out5[4] = sh.n_qtiles;
+    return PCNN_OK;
+}
+
+extern "C" int pcnn_conv_tc_plan_create_strided(pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch,
+                                                int image_rows, int act, const float *filt_host, const float *bias_host,
+                                                pcnn_conv_plan **out) {
+    PCNN_REQUIRE(ctx && filt_host && out, PCNN_ERR_ARG, "pcnn_conv_tc_plan_create: NULL argument");
+    ConvTcShape sh;
+    int rc = conv_tc_shape(N, H, W, C, K, R, S, stride, row_pitch, image_rows, &sh);
+    if (rc) return rc;
+    if (image_rows <= 0) image_rows = H;
+    const int Qt = sh.Qt, V = sh.V;
     pcnn_device_guard g(ctx->device);
     struct PlanGuard {                       // frees a half-built plan on every early return below
         pcnn_conv_plan *p;
@@ -285,12 +313,11 @@ extern "C" int pcnn_conv_tc_plan_create_strided(pcnn_ctx *ctx, int N, int H, int
     pl->W = W; pl->S = S; pl->row_pitch = row_pitch; pl->stride = stride; pl->in_image_rows = image_rows;
     ConvTcParams &p = pl->p;
     // rows are counted in units of `stride` input rows: tile row m = n * (image_rows / stride) + p
-    p.n_img = N; p.H = image_rows / stride; p.P = P; p.Q = Q; p.K = K; p.R = R; p.Qt = Qt; p.ncols = Qt * K; p.npad = (Qt * K + 31) / 32 * 32; p.C = C; p.V = V; p.stages = stages;
-    p.stride = stride; p.x_pitch = row_pitch;
-    p.n_mtiles = (int)(((long long)N * p.H + TC_M - 1) / TC_M);
-    p.n_qtiles = (Q + Qt - 1) / Qt;
+    p.n_img = N; p.H = sh.rows; p.P = sh.P; p.Q = sh.Q; p.K = K; p.R = R; p.Qt = Qt; p.ncols = Qt * K; p.npad = (Qt * K + 31) / 32 * 32; p.C = C; p.V = V;
+    p.stages = sh.stages; p.stride = stride;
+    p.n_mtiles = sh.n_mtiles; p.n_qtiles = sh.n_qtiles;
     p.act = act;
-    p.y_row_elems = (long long)Q * K;
+    p.y_row_elems = (long long)sh.Q * K;
     // Toeplitz operands: T_{v,r}[(ql, k)][kk] = f[k][r][s][c] where kk = delta_v + (ql + s) * C + c; rows ncols..npad-1 stay zero
     std::vector<uint16_t> t((size_t)V * R * p.npad * TC_KCHUNK, 0);
     for (int v = 0; v < V; ++v) {
@@ -310,7 +337,7 @@ extern "C" int pcnn_conv_tc_plan_create_strided(pcnn_ctx *ctx, int N, int H, int
         PCNN_CUDA(cudaMemcpy(pl->d_bias, bias_host, K * sizeof(float), cudaMemcpyHostToDevice));
     }
     p.bias = pl->d_bias;
-    int rc = make_map_2d(&pl->map_b, pl->d_toeplitz, TC_KCHUNK, (uint64_t)V * R * p.npad, TC_KCHUNK * 2, TC_KCHUNK, (uint32_t)p.npad);
+    rc = make_map_2d(&pl->map_b, pl->d_toeplitz, TC_KCHUNK, (uint64_t)V * R * p.npad, TC_KCHUNK * 2, TC_KCHUNK, (uint32_t)p.npad);
     if (rc) return rc;
     static bool configured[64] = {};        // function attributes are per device
     if (!configured[ctx->device & 63]) {
@@ -340,10 +367,18 @@ extern "C" int pcnn_conv_tc_fwd(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void 
     ConvTcParams p = plan->p;
     p.y = reinterpret_cast<__nv_bfloat16 *>(y_bf16);
     CUtensorMap map_x;
-    // stride s: the input viewed as [N * rows / s] rows of s * pitch elements (see ConvTcParams::x_pitch)
-    int rc = make_map_2d(&map_x, const_cast<void *>(x_bf16), (uint64_t)plan->row_pitch * plan->stride, (uint64_t)p.n_img * p.H,
-                         (uint64_t)plan->row_pitch * plan->stride * 2, TC_KCHUNK, TC_M);
-    if (rc) return rc;
+    // the input viewed as [N * rows / s][s][W * C] with rows `row_pitch` elements apart (stride s; s = 1 is the plain [N * rows][W * C]).
+    // The inner extent is the row itself, not the pitch: a box reaching past column W*C reads zeros, so whatever the pad
+    // elements hold (rows past H are never read by a valid output) cannot reach a result, not even a NaN through the zero
+    // entries of the Toeplitz operand.  The boxes are {32 elements, 1, 128 rows}: the same 8 KB tile as a 2-D box.
+    {
+        const uint64_t dims[3] = {(uint64_t)plan->W * p.C, (uint64_t)plan->stride, (uint64_t)p.n_img * p.H};
+        const uint64_t str[2] = {(uint64_t)plan->row_pitch * 2, (uint64_t)plan->row_pitch * plan->stride * 2};
+        const uint32_t box[3] = {TC_KCHUNK, 1, TC_M};
+        int rc = make_map_bf16(&map_x, const_cast<void *>(x_bf16), 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B,
+                               CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+        if (rc) return rc;
+    }
     const int ntiles = p.n_mtiles * p.n_qtiles;
     const int grid = ntiles < ctx->sm_count ? ntiles : ctx->sm_count;
     void *args[] = {&map_x, &plan->map_b, &p};

@@ -156,16 +156,17 @@ k_conv_tc_wgrad_rows(const __grid_constant__ CUtensorMap map_dy, const Wgrad2Par
         // ===== Hankel builders: 16-byte units = 8 pixels of one row (rho, j); shared-memory loads and stores by address =====
         const int b = threadIdx.x - 128;
         const int units = ((p.nreal + 7) / 8) * 8 * p.KO;
-        int src_off[W2_ITEMS], dst_off[W2_ITEMS], e0s[W2_ITEMS];
+        int src_off[W2_ITEMS], dst_off[W2_ITEMS], e0s[W2_ITEMS], rhos[W2_ITEMS];
 #pragma unroll
         for (int i = 0; i < W2_ITEMS; ++i) {
             const int L = b + i * (32 * W2_BUILD_WARPS);
-            src_off[i] = -1; dst_off[i] = 0; e0s[i] = 0;
+            src_off[i] = -1; dst_off[i] = 0; e0s[i] = 0; rhos[i] = 0;
             if (L < units) {
                 const int n8 = L / (p.KO * 8), rem = L % (p.KO * 8), kk = rem >> 3, nl = rem & 7, n = n8 * 8 + nl;
                 if (n < p.nreal) {
                     const int rho = n / p.SC, j = n % p.SC;
                     e0s[i] = kk * 8 * C + j;                 // element of the x segment feeding pixel 8*kk of the tile
+                    rhos[i] = rho;
                     src_off[i] = rho * p.xseg_stride + e0s[i] * 2;
                     dst_off[i] = n8 * SBO + kk * 128 + nl * 16;
                 }
@@ -177,15 +178,20 @@ k_conv_tc_wgrad_rows(const __grid_constant__ CUtensorMap map_dy, const Wgrad2Par
         for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
             bar_wait_relaxed(&S.full[stage], ph, 32);
             const uint32_t xs = x_s + (uint32_t)(stage * x_bytes), hs = hk_s + (uint32_t)(stage * hk_bytes);
+            const int rem = tile % tiles_per_img;
             int lim0 = 0;
-            if (p.guard) lim0 = p.W * C - ((tile % tiles_per_img) % p.n_ch) * p.PC * C;   // row elements at or after the segment start
+            if (p.guard) lim0 = p.W * C - (rem % p.n_ch) * p.PC * C;   // row elements at or after the segment start
+            // x rows past the image (a ragged last row block) were not copied for this tile: the stage still holds rows of an
+            // earlier tile, possibly of another chunk whose pad elements the guard above does not cover.  Their Hankel rows meet
+            // only the zero dy rows past P, so they are built as zeros (0 * NaN would poison the gradient).
+            const int nx = p.H - (rem / p.n_ch) * p.RB;
 #pragma unroll
             for (int i = 0; i < W2_ITEMS; ++i) {
                 if (src_off[i] >= 0) {
                     const uint32_t src = xs + (uint32_t)src_off[i];
                     unsigned short e[8];
 #pragma unroll
-                    for (int u = 0; u < 8; ++u) e[u] = lds_u16(src + (uint32_t)(u * C * 2));
+                    for (int u = 0; u < 8; ++u) e[u] = rhos[i] < nx ? lds_u16(src + (uint32_t)(u * C * 2)) : (unsigned short)0;
                     if (p.guard) {
 #pragma unroll
                         for (int u = 0; u < 8; ++u)

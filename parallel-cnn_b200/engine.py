@@ -424,10 +424,12 @@ class ConvPlan:
 
 
 def f32_to_bf16_bits(a):
-    """numpy float32 -> uint16 bf16 bit patterns (round to nearest even), the rounding the kernels use"""
+    """numpy float32 -> uint16 bf16 bit patterns (round to nearest even), the rounding the kernels use; NaN -> the quiet NaN
+    0x7FC0 (rounding the payload could carry into the exponent and the sign: 0x7FFFFFFF would become -0)"""
     u = np.ascontiguousarray(a, np.float32).view(np.uint32).astype(np.uint64)
+    nan = (u & 0x7FFFFFFF) > 0x7F800000
     u = u + 0x7FFF + ((u >> 16) & 1)
-    return (u >> 16).astype(np.uint16)
+    return np.where(nan, 0x7FC0, u >> 16).astype(np.uint16)
 
 
 def bf16_bits_to_f32(b):

@@ -98,7 +98,7 @@ if only in ("all", "lenet"):
     for N in (1024, 8192, 65536):
         run("lenet_c1_bf16_sigmoid (config 3 shape)", N, 28, 28, 1, 6, 5, 5, 1, 20)
     for N in (8192, 65536):
-        run("lenet_c1_bf16_sigmoid, 32-row image pitch (TMA-store epilogue)", N, 28, 28, 1, 6, 5, 5, 1, 20, image_rows=32)
+        run("lenet_c1_bf16_sigmoid, 32-row image pitch (rows 28..31 padding)", N, 28, 28, 1, 6, 5, 5, 1, 20, image_rows=32)
 if only == "lenet1024":                                                # BASELINE configs[2]: LeNet c1 shape, batch 1024
     run("lenet_c1_bf16_sigmoid (config 3 shape)", 1024, 28, 28, 1, 6, 5, 5, 1, 2)
 if only == "fwd128":                                                   # the profiler's target
@@ -116,7 +116,7 @@ if only == "fwdab":                                                    # forward
     run("224x224x3->64x3x3 bf16 (config 5), bias", 128, 224, 224, 3, 64, 3, 3, 0, 20)
     run("224x224x3->64x3x3 bf16 (config 5), no bias", 128, 224, 224, 3, 64, 3, 3, 0, 20, bias=False)
     run("224x224x3->64x3x3 bf16 (config 5), bias + sigmoid", 128, 224, 224, 3, 64, 3, 3, 1, 20)
-    run("lenet_c1_bf16_sigmoid, 32-row image pitch (TMA-store epilogue)", 65536, 28, 28, 1, 6, 5, 5, 1, 20, image_rows=32)
+    run("lenet_c1_bf16_sigmoid, 32-row image pitch (rows 28..31 padding)", 65536, 28, 28, 1, 6, 5, 5, 1, 20, image_rows=32)
     run("lenet_c1_bf16_sigmoid (config 3 shape)", 65536, 28, 28, 1, 6, 5, 5, 1, 20)
 if only in ("all", "cfg5"):
     for N in (1, 8, 32, 128):

@@ -1,6 +1,7 @@
 """CPU tests (no GPU) of the host-side logic and of the C-ABI library as a loadable object.  No compute entry point is
 called here: without a GPU pcnn_create must fail loudly (no CPU fallback)."""
 import ctypes as C
+import math
 import os
 import struct
 
@@ -13,7 +14,7 @@ import oracle_lib as O
 def test_library_exports_every_declared_symbol(pkg):
     L = pkg.lib()
     names = pkg.declared_symbols()
-    assert len(names) >= 60
+    assert len(names) >= 60 and "pcnn_conv_tc_plan_info" in names
     for n in names:
         assert hasattr(L, n), f"libpcnn.so does not export {n} declared in include/pcnn.h"
     assert L.pcnn_version() == 200
@@ -208,3 +209,43 @@ def test_bench_reference_arm_prints_the_contract_line():
     r1 = subprocess.run([sys.executable, os.path.join(root, "bench.py"), "--impl", "reference", "--steps", "1", "--warmup", "0", "--gpus", "2"],
                         capture_output=True, text=True, timeout=120, env=dict(os.environ, RANK="1", WORLD_SIZE="2"))
     assert r1.returncode == 0 and r1.stdout.strip() == ""
+
+
+def test_forward_conv_plan_query_is_host_logic(pkg):
+    """pcnn_conv_tc_plan_info needs no GPU and no context: the tiling pcnn_conv_tc_plan_create_strided uses, and the same refusals."""
+    cfg5 = pkg.conv_tc_plan_info(128, 224, 224, 3, 64, 3, 3)
+    assert cfg5 == dict(Qt=4, V=2, stages=4, n_mtiles=224, n_qtiles=56, tiles=12544)     # 128 * 224 rows / 128; 222 = 55 x 4 + 2
+    lenet = pkg.conv_tc_plan_info(8192, 28, 28, 1, 6, 5, 5, row_pitch=32, image_rows=32)
+    assert (lenet["Qt"], lenet["V"], lenet["n_mtiles"], lenet["n_qtiles"]) == (24, 1, 2048, 1)
+    s2 = pkg.conv_tc_plan_info(64, 224, 224, 3, 64, 3, 3, stride=2)
+    assert s2["n_mtiles"] == 64 * 112 // 128 and s2["n_qtiles"] == -(-111 // s2["Qt"])
+    for bad in [dict(C=64), dict(row_pitch=28, C=1), dict(stride=5), dict(image_rows=27, C=1)]:
+        a = dict(N=1, H=28, W=28, C=3, K=64, R=3, S=3, stride=1, row_pitch=None, image_rows=0)
+        a.update(bad)
+        with pytest.raises(pkg.PcnnError):
+            pkg.conv_tc_plan_info(**a)
+
+
+@pytest.mark.parametrize("sm_count", [114, 132])
+def test_multi_tile_conv_cases_reach_their_regime(pkg, sm_count):
+    """The multi-tile cases of test_conv_tc_gpu.py on an H100 PCIe (114 SMs) and SXM (132 SMs), from the host-side plan queries:
+    forward / weight gradient run more than 2 x stages tiles on every CTA (the stage ring wraps at least twice); the input
+    gradient has more rows per share than stages and shares that cross an image boundary; the padding cases of the weight
+    gradient walk a CTA through several pixel chunks with a ragged last row block."""
+    import conv_ref as CR
+    for N, H, W, C, K, R, S, stride, pitch, rows, _ in CR.FWD_MULTI:
+        g = CR.fwd_regime(pkg, N, H, W, C, K, R, S, sm_count, stride, pitch, rows)
+        assert g["min_tiles_per_cta"] > 2 * g["stages"], g
+    seen = dict(ragged=0, chunks=0, dgrad_only=0)
+    for N, H, W, C, K, R, S, _, _ in CR.BWD_MULTI + CR.WGRAD_PAD:
+        w, d = CR.wgrad_regime(pkg, N, H, W, C, K, R, S, sm_count), CR.dgrad_regime(pkg, N, H, W, C, K, R, S, sm_count)
+        assert d["max_rows_per_share"] > d["stages"] and d["shares_crossing_images"] > 0, d
+        if w is None:
+            seen["dgrad_only"] += 1
+            continue
+        assert w["min_tiles_per_cta"] > 2 * w["stages"], w
+        seen["ragged"] += w["ragged"]
+        seen["chunks"] += w["n_ch"] >= 2
+    assert seen["ragged"] >= 3 and seen["chunks"] >= 2 and seen["dgrad_only"] == 2, seen
+    w = CR.wgrad_regime(pkg, *CR.WGRAD_PAD[0][:7], sm_count)
+    assert w["ragged"] and math.gcd(w["n_ch"], w["grid"]) == 1     # consecutive tiles of a CTA (grid apart) change chunk

@@ -164,3 +164,39 @@ def test_lenet5_variant_oracle_backward_is_the_gradient_of_its_forward(golden):
         num = -(loss(pp) - loss(pm)) / (2 * eps)            # negative gradient, like the packed vector
         ana = g[j] * scale[j]
         assert abs(num - ana) <= 3e-2 * max(abs(ana), abs(num)) + 2e-4, (int(j), num, ana)
+
+
+# --------------------------------------------------------------------------- float64 convolution references (tests/conv_ref.py)
+CONV_REF_SHAPES = [  # N, H, W, C, K, R, S, stride (the backward passes run at stride 1)
+    (2, 9, 11, 1, 6, 3, 3, 1), (2, 12, 10, 2, 16, 5, 5, 2), (1, 13, 14, 3, 64, 7, 7, 3), (2, 8, 9, 4, 96, 3, 3, 1),
+    (1, 10, 12, 8, 256, 5, 5, 2), (1, 11, 11, 3, 256, 7, 7, 1), (3, 7, 8, 8, 64, 3, 3, 3), (2, 15, 13, 1, 96, 5, 5, 3),
+]
+
+
+def _within_one_ulp(ref64, got32):
+    r = ref64.astype(np.float32)
+    return np.all(np.abs(r - got32) <= np.spacing(np.maximum(np.abs(r), np.abs(got32))))
+
+
+@pytest.mark.parametrize("shape", CONV_REF_SHAPES, ids=["x".join(map(str, s)) for s in CONV_REF_SHAPES])
+def test_float64_conv_references_match_the_c_oracle(shape):
+    """conv_fwd_f64 / conv_wgrad_f64 / conv_dgrad_f64 (im2col-by-shift + BLAS, for the multi-tile GPU tests) against the
+    direct loops of orc_conv_*_nhwc: the same sums in float64 in another order, so they agree within 1 fp32 ulp."""
+    import conv_ref as CR
+    N, H, W, C, K, R, S, stride = shape
+    rng = np.random.default_rng(sum(shape))
+    x = rng.uniform(0, 1, (N, H, W, C)).astype(np.float32)
+    f = rng.uniform(-0.5, 0.5, (K, R, S, C)).astype(np.float32)
+    b = rng.uniform(-0.5, 0.5, K).astype(np.float32)
+    P, Q = (H - R) // stride + 1, (W - S) // stride + 1
+    y = np.empty((N, P, Q, K), np.float32)
+    O.oracle().orc_conv_fwd_nhwc_strided(O.fp(x.reshape(-1)), O.fp(f.reshape(-1)), O.fp(b), O.fp(y.reshape(-1)), N, H, W, C, K, R, S, stride)
+    assert _within_one_ulp(CR.conv_fwd_f64(x, f, b, stride), y)
+    P1, Q1 = H - R + 1, W - S + 1
+    dy = rng.uniform(-1, 1, (N, P1, Q1, K)).astype(np.float32)
+    dw = np.empty((K, R, S, C), np.float32)
+    dx = np.empty((N, H, W, C), np.float32)
+    O.oracle().orc_conv_wgrad_nhwc(O.fp(x.reshape(-1)), O.fp(dy.reshape(-1)), O.fp(dw.reshape(-1)), N, H, W, C, K, R, S)
+    O.oracle().orc_conv_dgrad_nhwc(O.fp(dy.reshape(-1)), O.fp(f.reshape(-1)), O.fp(dx.reshape(-1)), N, H, W, C, K, R, S)
+    assert _within_one_ulp(CR.conv_wgrad_f64(x, dy, R, S), dw)
+    assert _within_one_ulp(CR.conv_dgrad_f64(dy, f), dx)
