@@ -276,7 +276,7 @@ int pcnn_conv_tc_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C, int K, i
                              int act, const float *filt_host, const float *bias_host, pcnn_conv_plan **plan_out);
 /* the same with a window step of `stride` (1..4) in both directions (SURVEY.md 8f row 4): y [N][(H-R)/stride+1][(W-S)/stride+1][K];
  * rows per image (image_rows, or H) must be a multiple of the stride; the pixel block then needs ((Qt-1)*stride+S)*C <= 32.
- * Backward passes of strided convolutions are not built. */
+ * Its backward passes are pcnn_conv_wgrad_strided / pcnn_conv_dgrad_strided. */
 int pcnn_conv_tc_plan_create_strided(pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch,
                                      int image_rows, int act, const float *filt_host, const float *bias_host,
                                      pcnn_conv_plan **plan_out);
@@ -294,6 +294,20 @@ int pcnn_conv_wgrad(pcnn_ctx *ctx, const void *x_bf16_dev, const void *dy_bf16_d
                     int K, int R, int S, int row_pitch, int image_rows);
 int pcnn_conv_dgrad(pcnn_ctx *ctx, const void *dy_bf16_dev, const float *filt_f32_dev, void *dx_bf16_dev, int N, int H, int W,
                     int C, int K, int R, int S, int row_pitch, int image_rows);
+/* The same for a window step of `stride` (1..4; anything else is PCNN_ERR_ARG), the gradients of pcnn_conv_tc_fwd with a plan
+ * from pcnn_conv_tc_plan_create_strided.  dy is [N][(H-R)/stride+1][(W-S)/stride+1][K], as that forward writes it;
+ *     dw[k][r][s][c] = sum_{n,p,q} dy[n][p][q][k] * x[n][p*stride+r][q*stride+s][c]
+ *     dx[n][h][w][c] = sum_{k,r,s} dy[n][(h-r)/stride][(w-s)/stride][k] * f[k][r][s][c]   over the (r, s) that divide exactly.
+ * Every element of the H x W image of dx is written: rows and columns no window covers ((H-R) % stride != 0,
+ * (W-S) % stride != 0, or the gaps between windows when stride > R or S) get 0; pad columns and rows are never written.  The
+ * pad rules above hold unchanged, and rows per image need not be a multiple of the stride.  The tensor-core input gradient
+ * exists at strides 1 and 2 for 3x3 taps with C in {1,2,3,4,8}, 5x5 with C in {1,3} and 7x7 with C = 1, and at strides 3
+ * and 4 for 3x3 taps with C in {1,2,3}; the weight gradient needs ((RB-1)*stride + R)*S*C <= 64 for some RB >= 1.  Stride 1
+ * is exactly pcnn_conv_wgrad / pcnn_conv_dgrad. */
+int pcnn_conv_wgrad_strided(pcnn_ctx *ctx, const void *x_bf16_dev, const void *dy_bf16_dev, float *dw_f32_dev, int N, int H, int W,
+                            int C, int K, int R, int S, int stride, int row_pitch, int image_rows);
+int pcnn_conv_dgrad_strided(pcnn_ctx *ctx, const void *dy_bf16_dev, const float *filt_f32_dev, void *dx_bf16_dev, int N, int H, int W,
+                            int C, int K, int R, int S, int stride, int row_pitch, int image_rows);
 /* Which kernels pcnn_conv_wgrad / pcnn_conv_dgrad may use.  PCNN_CONV_BWD_TENSOR (default): the wgmma kernels only (any filter
  * count up to 256: counts that are not a multiple of 64 are zero-padded to one in an extra pass over dy) -- a shape they
  * cannot take is an ERROR (PCNN_ERR_ARG naming the restriction), never a silent detour.  PCNN_CONV_BWD_REFERENCE: the
@@ -303,8 +317,11 @@ typedef enum { PCNN_CONV_BWD_TENSOR = 0, PCNN_CONV_BWD_REFERENCE = 1 } pcnn_conv
 int pcnn_conv_bwd_select(pcnn_ctx *ctx, int path);
 /* Host-only query (works without a GPU): which kernels pcnn_conv_wgrad / pcnn_conv_dgrad pick for a shape and how they tile it.
  * out9 = { wgrad on tensor cores, dy rows per tile, pixels per tile, stages,
- *          dgrad on tensor cores, column strips, output pixels per lane quarter, partial dx rows kept in registers (R), stages } */
+ *          dgrad on tensor cores, column strips, output pixels per lane quarter, partial dx rows each consumer thread keeps
+ *          in registers (stride * ((R-1)/stride + 1); R at stride 1), stages } */
 int pcnn_conv_bwd_plan_info(int N, int H, int W, int C, int K, int R, int S, int *out9);
+/* the same for pcnn_conv_wgrad_strided / pcnn_conv_dgrad_strided (stride 1..4, else PCNN_ERR_ARG) */
+int pcnn_conv_bwd_plan_info_strided(int N, int H, int W, int C, int K, int R, int S, int stride, int *out9);
 /* Zero padding for the valid-padding kernels above (SURVEY.md 8f row 4): pcnn_pad_nhwc_bf16 embeds dense [N][H][W][C] images into
  * a zeroed canvas [N][dst_image_rows][dst_row_pitch] at row offset pad_h, pixel offset pad_w (0 = the tight canvas
  * [H + 2 pad_h][(W + 2 pad_w) * C]); a "same" convolution is pad -> pcnn_conv_tc_fwd, its input gradient is

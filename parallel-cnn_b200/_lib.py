@@ -122,6 +122,9 @@ _SIG = {
     "pcnn_crop_nhwc_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i],
     "pcnn_conv_wgrad": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i],
     "pcnn_conv_dgrad": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i],
+    "pcnn_conv_wgrad_strided": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
+    "pcnn_conv_dgrad_strided": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
+    "pcnn_conv_bwd_plan_info_strided": [_i, _i, _i, _i, _i, _i, _i, _i, _vp],
 }
 _RESTYPE = {"pcnn_last_error_string": C.c_char_p, "pcnn_mnist_free": None}
 
@@ -172,10 +175,11 @@ def conv_tc_plan_info(N, H, W, C, K, R, S, stride=1, row_pitch=None, image_rows=
     return dict(Qt=out[0], V=out[1], stages=out[2], n_mtiles=out[3], n_qtiles=out[4], tiles=out[3] * out[4])
 
 
-def conv_bwd_plan_info(N, H, W, C, K, R, S):
-    """Which kernels the backward passes pick for a shape and how they tile it (pcnn_conv_bwd_plan_info; host only, no GPU)."""
+def conv_bwd_plan_info(N, H, W, C, K, R, S, stride=1):
+    """Which kernels the backward passes pick for a shape and how they tile it (pcnn_conv_bwd_plan_info_strided; host only,
+    no GPU).  dgrad_ring: partial dx rows each consumer thread keeps in registers."""
     out = (_i * 9)()
-    check("pcnn_conv_bwd_plan_info", lib().pcnn_conv_bwd_plan_info(N, H, W, C, K, R, S, out))
+    check("pcnn_conv_bwd_plan_info_strided", lib().pcnn_conv_bwd_plan_info_strided(N, H, W, C, K, R, S, int(stride), out))
     return dict(wgrad_tc=bool(out[0]), wgrad_rb=out[1], wgrad_pc=out[2], wgrad_stages=out[3],
                 dgrad_tc=bool(out[4]), dgrad_strips=out[5], dgrad_oq=out[6], dgrad_ring=out[7], dgrad_stages=out[8])
 

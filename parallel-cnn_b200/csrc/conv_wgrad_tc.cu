@@ -1,18 +1,21 @@
 // parallel-cnn_b200/csrc/conv_wgrad_tc.cu -- weight gradient of the NHWC bf16 convolution (64 filters) on the Hopper tensor cores.
 //
-//     dw[k][r][s][c] = sum_{n,p,q} dy[n][p][q][k] * x[n][p+r][q+s][c]           [ref: layer.h:371-395 bp_weight_c1, without /576]
+//     dw[k][r][s][c] = sum_{n,p,q} dy[n][p][q][k] * x[n][p*st+r][q*st+s][c]     [ref: layer.h:371-395 bp_weight_c1, without /576]
+//
+// (st = the window step of the forward, 1..4, a run-time parameter; st = 1 is the reference's conv.)
 //
 // SURVEY.md x3 / BASELINE.json config 5: dy [N,222,222,64] is 95 % of the 6.6 MB/image this pass moves and the pass is
 // HBM-bound (SURVEY.md 8d), so: dy crosses HBM -> shared memory once by TMA and is consumed there by wgmma.
 //   * The reduction runs over pixels, the slow axis of both tensors.  dy needs no transposition: a TMA tile
 //     [RB rows][PC pixels][64 filters] is an MN-major B operand as it lands (one 128-byte swizzled row per pixel; the RB
 //     rows are RB atoms along N, N = RB * 64 <= 256).
-//   * The other operand is the Hankel matrix of the x rows, A[(rho, s, c)][pixel q] = x[p0 + rho][(q + s) * C + c] for the
-//     RB + R - 1 input rows a block of RB dy rows touches (54 of M = 64 rows at config 5); four warps build it in shared
-//     memory from the x row segments (x is 5 % of the traffic; the 9x expansion never leaves the SM).
+//   * The other operand is the Hankel matrix of the x rows, A[(rho, s, c)][pixel q] = x[p0*st + rho][(q*st + s) * C + c] for
+//     the NXR = (RB - 1) * st + R input rows a block of RB dy rows touches (54 of M = 64 rows at config 5); four warps build
+//     it in shared memory from the x row segments, gathering every st*C-th element (x is 5 % of the traffic; the 9x
+//     expansion never leaves the SM).
 //     (More than 64 filters: K/64 boxes per tile, the accumulator columns become (filter group, row, filter), K <= 256.)
 //   * D[(rho, s, c)][(row, k)] accumulates in ONE 64 x N (N = RB * 64 <= 256) register accumulator of one warpgroup for
-//     the whole kernel; the entries with rho - row = r in [0, R) are the gradient, the others are discarded.  At the end each
+//     the whole kernel; the entries with rho - row * st = r in [0, R) are the gradient, the others are discarded.  At the end each
 //     CTA folds the RB row blocks, writes one 1,728-float partial, and a second kernel adds the partials in a fixed order
 //     (deterministic, no atomics).
 //   * Large N matters: one wgmma of N = 192 consumes 6 KB of dy, so the MMA issue stream stays far below the HBM time of
@@ -35,7 +38,8 @@ constexpr int W2_DUMP_STRIDE = 257;                    // floats per accumulator
 
 struct Wgrad2Params {
     int n_img, H, P, Q, W, C, R, SC;
-    int RB, NXR, PC, KO;                   // dy rows per tile, x rows per tile, pixels per tile, PC / 8
+    int st;                                // window step (1..4)
+    int RB, NXR, PC, KO;                   // dy rows per tile, x rows per tile ((RB-1)*st + R), pixels per tile, PC / 8
     int KH;                                // filters / 64: a TMA box (and an MMA atom along N) holds 64 filters
     int nreal, nout;                       // Hankel rows in use (NXR * SC), outputs per filter (R * SC)
     int n_pb, n_ch, stages;                // row blocks per image, pixel chunks per row, smem stages
@@ -61,13 +65,13 @@ __device__ __forceinline__ void sts_v4(uint32_t saddr, uint4 v) {
 
 // bytes of x row segment `chunk` that exist in the row (a multiple of 16; 0 when the chunk starts past the row)
 __device__ __forceinline__ int xseg_copy_bytes(const Wgrad2Params &p, int chunk) {
-    const int start = chunk * p.PC * p.C * 2;
+    const int start = chunk * p.PC * p.st * p.C * 2;
     int avail = p.xrow_bytes - start;
     if (avail < 0) avail = 0;
     return avail < p.xseg_bytes ? avail : p.xseg_bytes;
 }
 
-// CT = compile-time input-channel count (the gather stride of the Hankel builder), 0 = run-time; N = accumulator columns
+// CT = compile-time input-channel count (the gather stride of the Hankel builder is st * C), 0 = run-time; N = accumulator columns
 template <int CT, int N>
 __global__ void __launch_bounds__(W2_THREADS, 1)
 k_conv_tc_wgrad_rows(const __grid_constant__ CUtensorMap map_dy, const Wgrad2Params p) {
@@ -109,7 +113,7 @@ k_conv_tc_wgrad_rows(const __grid_constant__ CUtensorMap map_dy, const Wgrad2Par
                 const int n = tile / tiles_per_img, rem = tile % tiles_per_img, pb = rem / p.n_ch, ch = rem % p.n_ch;
                 const int p0 = pb * p.RB;
                 const int xb = xseg_copy_bytes(p, ch);
-                int nx = p.H - p0;                        // x rows p0 .. p0 + NXR - 1 that exist
+                int nx = p.H - p0 * p.st;                 // x rows p0*st .. p0*st + NXR - 1 that exist
                 if (nx > p.NXR) nx = p.NXR;
                 bar_wait_relaxed(&S.empty[stage], ph ^ 1u, 32);
                 bar_expect_tx(&S.full[stage], (unsigned)(dy_bytes + nx * xb));
@@ -118,7 +122,7 @@ k_conv_tc_wgrad_rows(const __grid_constant__ CUtensorMap map_dy, const Wgrad2Par
                 if (xb > 0)
                     for (int r = 0; r < nx; ++r)
                         tma_load_1d(X + (size_t)stage * x_bytes + (size_t)r * p.xseg_stride,
-                                    p.x + ((long long)n * p.x_image_rows + p0 + r) * p.x_pitch + (long long)ch * p.PC * C, (unsigned)xb,
+                                    p.x + ((long long)n * p.x_image_rows + p0 * p.st + r) * p.x_pitch + (long long)ch * p.PC * p.st * C, (unsigned)xb,
                                     &S.full[stage]);
                 if (++stage == NST) { stage = 0; ph ^= 1u; }
             }
@@ -156,6 +160,7 @@ k_conv_tc_wgrad_rows(const __grid_constant__ CUtensorMap map_dy, const Wgrad2Par
         // ===== Hankel builders: 16-byte units = 8 pixels of one row (rho, j); shared-memory loads and stores by address =====
         const int b = threadIdx.x - 128;
         const int units = ((p.nreal + 7) / 8) * 8 * p.KO;
+        const int gs = p.st * C;                     // x elements between consecutive pixels of the Hankel row
         int src_off[W2_ITEMS], dst_off[W2_ITEMS], e0s[W2_ITEMS], rhos[W2_ITEMS];
 #pragma unroll
         for (int i = 0; i < W2_ITEMS; ++i) {
@@ -165,7 +170,7 @@ k_conv_tc_wgrad_rows(const __grid_constant__ CUtensorMap map_dy, const Wgrad2Par
                 const int n8 = L / (p.KO * 8), rem = L % (p.KO * 8), kk = rem >> 3, nl = rem & 7, n = n8 * 8 + nl;
                 if (n < p.nreal) {
                     const int rho = n / p.SC, j = n % p.SC;
-                    e0s[i] = kk * 8 * C + j;                 // element of the x segment feeding pixel 8*kk of the tile
+                    e0s[i] = kk * 8 * gs + j;                // element of the x segment feeding pixel 8*kk of the tile
                     rhos[i] = rho;
                     src_off[i] = rho * p.xseg_stride + e0s[i] * 2;
                     dst_off[i] = n8 * SBO + kk * 128 + nl * 16;
@@ -180,22 +185,22 @@ k_conv_tc_wgrad_rows(const __grid_constant__ CUtensorMap map_dy, const Wgrad2Par
             const uint32_t xs = x_s + (uint32_t)(stage * x_bytes), hs = hk_s + (uint32_t)(stage * hk_bytes);
             const int rem = tile % tiles_per_img;
             int lim0 = 0;
-            if (p.guard) lim0 = p.W * C - (rem % p.n_ch) * p.PC * C;   // row elements at or after the segment start
+            if (p.guard) lim0 = p.W * C - (rem % p.n_ch) * p.PC * gs;   // row elements at or after the segment start
             // x rows past the image (a ragged last row block) were not copied for this tile: the stage still holds rows of an
             // earlier tile, possibly of another chunk whose pad elements the guard above does not cover.  Their Hankel rows meet
             // only the zero dy rows past P, so they are built as zeros (0 * NaN would poison the gradient).
-            const int nx = p.H - (rem / p.n_ch) * p.RB;
+            const int nx = p.H - (rem / p.n_ch) * p.RB * p.st;
 #pragma unroll
             for (int i = 0; i < W2_ITEMS; ++i) {
                 if (src_off[i] >= 0) {
                     const uint32_t src = xs + (uint32_t)src_off[i];
                     unsigned short e[8];
 #pragma unroll
-                    for (int u = 0; u < 8; ++u) e[u] = rhos[i] < nx ? lds_u16(src + (uint32_t)(u * C * 2)) : (unsigned short)0;
+                    for (int u = 0; u < 8; ++u) e[u] = rhos[i] < nx ? lds_u16(src + (uint32_t)(u * gs * 2)) : (unsigned short)0;
                     if (p.guard) {
 #pragma unroll
                         for (int u = 0; u < 8; ++u)
-                            if (e0s[i] + u * C >= lim0) e[u] = 0;
+                            if (e0s[i] + u * gs >= lim0) e[u] = 0;
                     }
                     uint4 o;
                     o.x = e[0] | ((uint32_t)e[1] << 16); o.y = e[2] | ((uint32_t)e[3] << 16);
@@ -214,13 +219,13 @@ k_conv_tc_wgrad_rows(const __grid_constant__ CUtensorMap map_dy, const Wgrad2Par
     // ===== fold the RB row blocks of the dumped accumulator, one partial per CTA =====
     __syncthreads();
     {
-        // dw[k][r][j] = sum over row blocks rb of D[(rb + r) * SC + j][rb * 64 + k]
+        // dw[k][r][j] = sum over row blocks rb of D[(rb * st + r) * SC + j][rb * 64 + k]
         const int K = p.KH * 64;
         float *dst = p.slots + (size_t)blockIdx.x * K * p.nout;
         for (int o = threadIdx.x; o < K * p.nout; o += W2_THREADS) {
             const int k = o / p.nout, rj = o % p.nout, r = rj / p.SC, j = rj % p.SC, kh = k >> 6, kl = k & 63;
             float s = 0.0f;
-            for (int rb = 0; rb < p.RB; ++rb) s += dump[((rb + r) * p.SC + j) * W2_DUMP_STRIDE + (kh * p.RB + rb) * 64 + kl];
+            for (int rb = 0; rb < p.RB; ++rb) s += dump[((rb * p.st + r) * p.SC + j) * W2_DUMP_STRIDE + (kh * p.RB + rb) * 64 + kl];
             dst[o] = s;
         }
     }
@@ -243,20 +248,24 @@ __global__ void __launch_bounds__(256) k_conv_tc_wgrad_rows_reduce(const float *
 
 struct Plan { int RB, PC, stages; size_t stage_bytes, smem; bool ok; };
 
+// x elements a tile of PC pixels reads from each x row: ((PC - 1) * st + S) * C, plus one pixel of slack in the stride
+int xseg_stride_bytes(int PC, int C, int S, int st) { return (((PC - 1) * st + S + 1) * C * 2 + 127) / 128 * 128; }
+
 // Tile shape: dy rows per tile RB (N = RB * 64) and pixels per tile PC.  What matters is that the tiles cover the [P x Q]
 // plane with little padding (PC = 112 covers Q = 222 in two chunks, PC = 80 needs three) and that at least three stages fit.
-Plan plan_for(int P, int Q, int C, int R, int S, int KH) {
+Plan plan_for(int P, int Q, int C, int R, int S, int KH, int st) {
     Plan pl;
     memset(&pl, 0, sizeof(pl));
     const int SC = S * C;
     double best = -1.0;
     for (int RB = 4; RB >= 1; --RB) {
-        if ((RB + R - 1) * SC > 64 || RB * KH * 64 > 256) continue;
+        const int nxr = (RB - 1) * st + R;
+        if (nxr * SC > 64 || RB * KH * 64 > 256) continue;
         for (int PC = 128; PC >= 32; PC -= 16) {
-            const int units = (((RB + R - 1) * SC + 7) / 8) * 8 * (PC / 8);
+            const int units = ((nxr * SC + 7) / 8) * 8 * (PC / 8);
             if (units > W2_ITEMS * 32 * W2_BUILD_WARPS) continue;
-            const size_t xseg = (size_t)(((PC + S) * C * 2 + 127) / 128 * 128);
-            const size_t stage = (size_t)KH * RB * PC * 128 + (size_t)64 * PC * 2 + (size_t)(RB + R - 1) * xseg;
+            const size_t xseg = (size_t)xseg_stride_bytes(PC, C, S, st);
+            const size_t stage = (size_t)KH * RB * PC * 128 + (size_t)64 * PC * 2 + (size_t)nxr * xseg;
             int st = (int)(((size_t)W2_SMEM_BUDGET - sizeof(Wgrad2Ctl) - 1024) / stage);
             if (st > W2_MAX_STAGES) st = W2_MAX_STAGES;
             if (st < 2) continue;
@@ -297,36 +306,36 @@ int launch_rows_n(pcnn_ctx *ctx, const CUtensorMap &map_dy, const Wgrad2Params &
 
 }  // namespace
 
-bool pcnn_conv_wgrad_rows_ok(int N, int H, int W, int C, int K, int R, int S, int row_pitch, const void *x, const void *dy) {
+bool pcnn_conv_wgrad_rows_ok(int N, int H, int W, int C, int K, int R, int S, int st, int row_pitch, const void *x, const void *dy) {
     if (K % 64 || K > 256 || ((uintptr_t)dy & 15) || ((uintptr_t)x & 15) || row_pitch % 8 || N <= 0 || H < R || W < S) return false;
-    return plan_for(H - R + 1, W - S + 1, C, R, S, K / 64).ok;
+    return plan_for((H - R) / st + 1, (W - S) / st + 1, C, R, S, K / 64, st).ok;
 }
 
 // host-side tile choice of the weight gradient, for pcnn_conv_bwd_plan_info (no GPU needed)
-void pcnn_conv_wgrad_rows_info(int H, int W, int C, int K, int R, int S, int *out4) {
-    const Plan pl = plan_for(H - R + 1, W - S + 1, C, R, S, K / 64);
+void pcnn_conv_wgrad_rows_info(int H, int W, int C, int K, int R, int S, int st, int *out4) {
+    const Plan pl = plan_for((H - R) / st + 1, (W - S) / st + 1, C, R, S, K / 64, st);
     out4[0] = pl.ok ? 1 : 0; out4[1] = pl.RB; out4[2] = pl.PC; out4[3] = pl.stages;
 }
 
 // dy_channels: filters dy really holds per pixel (<= K, multiple of 8: 16-byte pixel pitch); the TMA boxes stay 64 channels
 // wide and the hardware fills channels dy_channels..63 of a box with zeros, so a 16- or 32-filter gradient needs no padded copy
 int pcnn_conv_wgrad_rows(pcnn_ctx *ctx, const void *x_bf16, const void *dy_bf16, float *dw_f32, int N, int H, int W, int C, int K,
-                         int R, int S, int row_pitch, int image_rows, int dy_channels) {
+                         int R, int S, int st, int row_pitch, int image_rows, int dy_channels) {
     const uint64_t KD = dy_channels > 0 ? (uint64_t)dy_channels : (uint64_t)K;
     pcnn_device_guard g(ctx->device);
-    const int P = H - R + 1, Q = W - S + 1;
-    const Plan pl = plan_for(P, Q, C, R, S, K / 64);
+    const int P = (H - R) / st + 1, Q = (W - S) / st + 1;
+    const Plan pl = plan_for(P, Q, C, R, S, K / 64, st);
     PCNN_REQUIRE(pl.ok, PCNN_ERR_ARG, "pcnn_conv_wgrad: shape does not fit the tensor-core kernel");
     Wgrad2Params p;
     memset(&p, 0, sizeof(p));
-    p.n_img = N; p.H = H; p.P = P; p.Q = Q; p.W = W; p.C = C; p.R = R; p.SC = S * C;
-    p.RB = pl.RB; p.NXR = pl.RB + R - 1; p.PC = pl.PC; p.KO = pl.PC / 8; p.KH = K / 64;
+    p.n_img = N; p.H = H; p.P = P; p.Q = Q; p.W = W; p.C = C; p.R = R; p.SC = S * C; p.st = st;
+    p.RB = pl.RB; p.NXR = (pl.RB - 1) * st + R; p.PC = pl.PC; p.KO = pl.PC / 8; p.KH = K / 64;
     p.nreal = p.NXR * p.SC; p.nout = R * p.SC;
     p.n_pb = (P + p.RB - 1) / p.RB; p.n_ch = (Q + p.PC - 1) / p.PC; p.stages = pl.stages;
     p.x_pitch = row_pitch > 0 ? row_pitch : W * C;
     p.x_image_rows = image_rows > 0 ? image_rows : H;
-    p.xseg_bytes = ((p.PC + S - 1) * C * 2 + 15) / 16 * 16;
-    p.xseg_stride = ((p.PC + S) * C * 2 + 127) / 128 * 128;
+    p.xseg_bytes = (((p.PC - 1) * st + S) * C * 2 + 15) / 16 * 16;
+    p.xseg_stride = xseg_stride_bytes(p.PC, C, S, st);
     p.xrow_bytes = (W * C * 2 + 15) / 16 * 16;
     PCNN_REQUIRE((long long)p.xrow_bytes <= p.x_pitch * 2 && p.xseg_bytes <= p.xseg_stride, PCNN_ERR_ARG, "pcnn_conv_wgrad: row pitch");
     p.guard = (W * C * 2) % 16 != 0;

@@ -52,9 +52,9 @@ def run(name, N, H, W, C, K, R, S, act, iters, image_rows=0, bias=True):
     del x, y
 
 
-def run_bwd(name, N, H, W, C, K, R, S, iters):
+def run_bwd(name, N, H, W, C, K, R, S, iters, stride=1):
     """wgrad and dgrad of the same layer: algorithmic bytes = dy read + x read (wgrad) / dy read + dx written (dgrad), bf16."""
-    P, Q = H - R + 1, W - S + 1
+    P, Q = (H - R) // stride + 1, (W - S) // stride + 1
     xb = torch.randint(0, 0x3F80, (N, H, W, C), dtype=torch.int16, device="cuda")
     dyb = torch.randint(0, 0x3F80, (N, P, Q, K), dtype=torch.int16, device="cuda")
     dyb ^= (torch.randint(0, 2, (N, P, Q, K), dtype=torch.int16, device="cuda") << 15)      # random signs
@@ -63,8 +63,8 @@ def run_bwd(name, N, H, W, C, K, R, S, iters):
     dx = torch.empty((N, H, W, C), dtype=torch.int16, device="cuda")
     alg = N * (H * W * C + P * Q * K) * 2
     flops = 2.0 * N * P * Q * K * R * S * C
-    for what, fn in (("wgrad", lambda: eng.conv_wgrad(xb, dyb, dw, N, H, W, C, K, R, S)),
-                     ("dgrad", lambda: eng.conv_dgrad(dyb, f, dx, N, H, W, C, K, R, S))):
+    for what, fn in (("wgrad", lambda: eng.conv_wgrad(xb, dyb, dw, N, H, W, C, K, R, S, stride=stride)),
+                     ("dgrad", lambda: eng.conv_dgrad(dyb, f, dx, N, H, W, C, K, R, S, stride=stride))):
         for _ in range(3):
             fn()
         torch.cuda.synchronize()
@@ -79,7 +79,7 @@ def run_bwd(name, N, H, W, C, K, R, S, iters):
         torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / iters
         print(json.dumps({"case": name + " " + what, "host_enqueue_us": host_us, "N": N, "ms": ms, "img_per_s": N / (ms * 1e-3), "alg_GBps": alg / (ms * 1e-3) / 1e9,
-                          "hbm_frac": alg / (ms * 1e-3) / 1e9 / HBM, "useful_TFLOPs": flops / (ms * 1e-3) / 1e12,
+                          "hbm_frac": alg / (ms * 1e-3) / 1e9 / HBM, "useful_TFLOPs": flops / (ms * 1e-3) / 1e12, "stride": stride,
                           "path": os.environ.get("PCNN_CONV_BWD", "tc"), "working_set_MB": alg / 1e6}), flush=True)
     del xb, dyb, dx
 
@@ -94,6 +94,9 @@ if only == "bwdk128":                                                  # 128 fil
     run_bwd("224x224x3->128x3x3 bf16", 64, 224, 224, 3, 128, 3, 3, 10)
 if only == "bwd128":                                                   # the profiler's target: few launches
     run_bwd("224x224x3->64x3x3 bf16 (config 5)", 128, 224, 224, 3, 64, 3, 3, 2)
+if only == "bwds2":                                                    # config 5 at stride 2 next to stride 1 (same launch count)
+    run_bwd("224x224x3->64x3x3 bf16 (config 5)", 128, 224, 224, 3, 64, 3, 3, 10)
+    run_bwd("224x224x3->64x3x3 bf16 (config 5), stride 2", 128, 224, 224, 3, 64, 3, 3, 10, stride=2)
 if only in ("all", "lenet"):
     for N in (1024, 8192, 65536):
         run("lenet_c1_bf16_sigmoid (config 3 shape)", N, 28, 28, 1, 6, 5, 5, 1, 20)
