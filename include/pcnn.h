@@ -287,6 +287,23 @@ int pcnn_conv_tc_plan_destroy(pcnn_ctx *ctx, pcnn_conv_plan *plan);
  * error here. */
 int pcnn_conv_tc_plan_info(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows, int *out5);
 int pcnn_conv_tc_fwd(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *x_bf16_dev, void *y_bf16_dev);
+/* Forward for wide channel counts (csrc/conv_wide_tc.cu): the same contract as pcnn_conv_tc_plan_create_strided (x NHWC bf16 with
+ * row_pitch and image_rows, filters fp32 KRSC rounded to bf16 once here, optional bias, act 0 none / 1 sigmoid, y dense NHWC bf16
+ * [N][(H-R)/stride+1][(W-S)/stride+1][K], pad columns and pad rows of x ignored, NaN included), computed as a tap-major implicit
+ * GEMM on wgmma with the channels as the reduction.  The plan is run by pcnn_conv_tc_fwd (which then also needs y 16-byte aligned)
+ * and freed by pcnn_conv_tc_plan_destroy.  Its domain is exactly the shapes that
+ *   - pcnn_conv_tc_plan_info refuses (a shape the row-Toeplitz plan takes is refused here with a message naming
+ *     pcnn_conv_tc_plan_create: no shape has two forward kernels),
+ *   - have C % 8 == 0, K % 8 == 0 and K <= 256, 1 <= R, S <= 7, stride 1..4,
+ *   - and satisfy the pitch rules (row_pitch >= W*C and a multiple of 8, image_rows >= H or 0 for H).
+ * Everything else is PCNN_ERR_ARG with a message naming the rule.  Rows per image need not be a multiple of the stride. */
+int pcnn_conv_wide_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch,
+                               int image_rows, int act, const float *filt_host, const float *bias_host, pcnn_conv_plan **plan_out);
+/* Host-only query (no GPU, no context): how pcnn_conv_wide_plan_create tiles a shape; its refusals are the create call's.
+ * out8 = { Pt output rows x Qt output columns of one image per tile (Pt * Qt = 128), 64-channel chunks per tap, stages, tiles
+ * (N * blocks per image), pixel blocks down a column of the image, pixel blocks along a row, MMA width (K rounded up to 16) }.
+ * The tiles issue tiles * 128 output pixels for the N * P * Q they compute. */
+int pcnn_conv_wide_plan_info(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows, int *out8);
 /* Backward passes of the same convolution (bf16 operands, fp32 accumulation, deterministic; wgmma kernels, see
  * pcnn_conv_bwd_select): weight gradient fp32 KRSC [ref: layer.h:371-395 bp_weight_c1, without its /576] and input gradient
  * bf16 NHWC in x's layout.  row_pitch / image_rows as for the forward plan (0 = dense). */

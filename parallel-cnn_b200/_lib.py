@@ -116,6 +116,8 @@ _SIG = {
     "pcnn_conv_tc_plan_destroy": [_vp, _vp],
     "pcnn_conv_tc_plan_info": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_conv_tc_fwd": [_vp, _vp, _vp, _vp],
+    "pcnn_conv_wide_plan_create": [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _pvp],
+    "pcnn_conv_wide_plan_info": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_f32_to_bf16_rows": [_vp, _vp, _vp, _l, _i, _i],
     "pcnn_conv_bwd_plan_info": [_i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_pad_nhwc_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i],
@@ -173,6 +175,17 @@ def conv_tc_plan_info(N, H, W, C, K, R, S, stride=1, row_pitch=None, image_rows=
     out = (_i * 5)()
     check("pcnn_conv_tc_plan_info", lib().pcnn_conv_tc_plan_info(N, H, W, C, K, R, S, int(stride), int(pitch), int(image_rows), out))
     return dict(Qt=out[0], V=out[1], stages=out[2], n_mtiles=out[3], n_qtiles=out[4], tiles=out[3] * out[4])
+
+
+def conv_wide_plan_info(N, H, W, C, K, R, S, stride=1, row_pitch=None, image_rows=0):
+    """How the wide-channel forward plan tiles a shape (pcnn_conv_wide_plan_info; host only, no GPU).  row_pitch None = W*C
+    rounded up to 8 elements, as WideConvPlan.  issued_pixels / useful_pixels: output pixels the tiles cover / compute."""
+    pitch = (W * C + 7) // 8 * 8 if row_pitch is None else row_pitch
+    out = (_i * 8)()
+    check("pcnn_conv_wide_plan_info", lib().pcnn_conv_wide_plan_info(N, H, W, C, K, R, S, int(stride), int(pitch), int(image_rows), out))
+    P, Q = (H - R) // stride + 1, (W - S) // stride + 1
+    return dict(Pt=out[0], Qt=out[1], chunks=out[2], stages=out[3], tiles=out[4], n_pb=out[5], n_qb=out[6], npad=out[7],
+                issued_pixels=out[4] * out[0] * out[1], useful_pixels=N * P * Q)
 
 
 def conv_bwd_plan_info(N, H, W, C, K, R, S, stride=1):

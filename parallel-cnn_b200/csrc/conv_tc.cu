@@ -78,14 +78,6 @@ static size_t conv_tc_smem_bytes(int V, int R, int npad, int stages) {
     return (size_t)V * R * npad * TC_KCHUNK * 2 + (size_t)stages * R * A_TILE_BYTES + sizeof(ConvTcCtl) + 1024;
 }
 
-// sigmoid for a bf16 result: 0.5 + 0.5 tanh(x / 2) with ONE transcendental (MUFU.TANH) instead of two (EX2 + RCP).
-// tanh.approx is good to ~5e-4 absolute, a quarter of a bf16 ulp of the result; the test bound (2^-8 |ref| + 1e-3) is unchanged.
-__device__ __forceinline__ float sigmoid_bf16(float x) {
-    float t;
-    asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.5f * x));
-    return fmaf(t, 0.5f, 0.5f);
-}
-
 // ACT (0 none, 1 sigmoid) and the MMA width N are compile-time; a missing bias reads as zeros from the shared bias table
 template <int ACT, int N>
 __global__ void __launch_bounds__(TC_THREADS, 1)
@@ -228,10 +220,18 @@ struct pcnn_conv_plan {
     void *d_toeplitz = nullptr;     // [R][ncols][32] bf16
     float *d_bias = nullptr;
     CUtensorMap map_b;
+    ConvWidePlan *wide = nullptr;   // non-null: a plan of pcnn_conv_wide_plan_create (conv_wide_tc.cu), nothing above is used
 };
+
+pcnn_conv_plan *conv_plan_wrap_wide(ConvWidePlan *w) {
+    pcnn_conv_plan *pl = new pcnn_conv_plan();
+    pl->wide = w;
+    return pl;
+}
 
 static void free_plan(pcnn_conv_plan *plan) {
     if (!plan) return;
+    if (plan->wide) conv_wide_free(plan->wide);
     if (plan->d_toeplitz) cudaFree(plan->d_toeplitz);
     if (plan->d_bias) cudaFree(plan->d_bias);
     delete plan;
@@ -364,6 +364,7 @@ extern "C" int pcnn_conv_tc_fwd(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void 
     PCNN_REQUIRE(ctx && plan && x_bf16 && y_bf16, PCNN_ERR_ARG, "pcnn_conv_tc_fwd: NULL argument");
     PCNN_REQUIRE(((uintptr_t)x_bf16 & 15) == 0, PCNN_ERR_ARG, "pcnn_conv_tc_fwd: activations must be 16-byte aligned");
     pcnn_device_guard g(ctx->device);
+    if (plan->wide) return conv_wide_fwd(ctx, plan->wide, x_bf16, y_bf16);
     ConvTcParams p = plan->p;
     p.y = reinterpret_cast<__nv_bfloat16 *>(y_bf16);
     CUtensorMap map_x;

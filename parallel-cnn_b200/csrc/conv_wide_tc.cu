@@ -1,0 +1,343 @@
+// parallel-cnn_b200/csrc/conv_wide_tc.cu -- bf16 convolution forward for wide channel counts on the Hopper tensor cores
+// (pcnn_conv_wide_plan_create): the shapes the row-Toeplitz forward of conv_tc.cu refuses, C % 8 == 0, K <= 256.
+//
+// Formulation ("tap-major implicit GEMM").  With M = output pixels, N = filters and the reduction over (r, s, c):
+//     y[n][p][q][k] = sum_{r,s}  sum_c  x[n][p*st + r][q*st + s][c] * f[k][r][s][c]
+// i.e. R*S GEMMs whose A operand is the input shifted by the tap (r, s) and whose B operand is the filter slice f[:, r, s, :].
+// The reduction runs in steps of 64 channels (one 128-byte SWIZZLE_128B row per pixel / filter), R*S*ceil(C/64) steps per
+// tile, four m64nNk16 per step and warpgroup.  Nothing is expanded in memory:
+//   * A: a tile is a Pt x Qt block of output pixels of one image (Pt * Qt = 128).  For tap (r, s) the block reads one TMA box
+//     {64 channels, Qt, Pt, 1} of the map of x that starts at input row r % st and column s % st and steps st rows and st
+//     pixels (one map per such phase, at most st^2 = 16): box coordinate (q0 + s / st, p0 + r / st) is then input pixel
+//     ((p0 + pp) * st + r, (q0 + qq) * st + s) for the block's pixel (pp, qq).  The map extents stop at the last row / pixel of
+//     the image and at channel C: everything outside is zero-filled, pad rows and columns of x are never read.
+//   * B: the filters rounded to bf16 once, KRSC on the device, viewed as {C, R*S, K}: a box {64, 1, Npad} is the K-major
+//     operand of one step; channels >= C and filters >= K are zero-filled by TMA, and a box never reaches the next tap.
+//   * D: [128 x Npad] fp32 in the registers of two warpgroups (rows 0-63 / 64-127 of the block), Npad = K rounded up to 16.
+//   * Epilogue: bias, optional sigmoid, bf16, written to a shared staging tile per warpgroup (SWIZZLE_128B, conflict-free),
+//     then stored by TMA through a map of y {K, Q, P, N} that clips pixels outside the image and channels >= K.  The store
+//     drains while the warpgroup already runs the next tile's MMAs; the staging tile is reused once its store has been read.
+// Pixel blocks on small images issue more pixels than they compute: pcnn_conv_wide_plan_info reports both.
+//
+// Warp roles (288 threads, 1 CTA/SM, persistent over tiles): warps 0-7 = two consumer warpgroups, warp 8 = TMA producer.
+#include "tc_common.cuh"
+
+#include <vector>
+
+using namespace pcnn_tc;
+
+namespace {
+
+constexpr int WD_THREADS = 288;
+constexpr int WD_CONSUMER_WARPS = 8;
+constexpr int WD_M = 128;                 // output pixels per tile (two warpgroups of 64)
+constexpr int WD_KC = 64;                 // channels per reduction step (128 B rows, SWIZZLE_128B)
+constexpr int WD_MAX_STAGES = 8;
+constexpr int WD_SMEM_BUDGET = 225 * 1024;
+constexpr int WD_A_BYTES = WD_M * WD_KC * 2;       // 16 KB
+constexpr int WD_STG_BYTES = 64 * WD_KC * 2;       // one staging sub-tile: 64 pixels x 64 channels, 8 KB
+constexpr int WD_MAX_RS = 7;
+
+struct ConvWideParams {
+    int Pt, Qt;                  // pixel block: Pt output rows x Qt output columns
+    int n_pb, n_qb, tiles;       // blocks per image column / row, N * n_pb * n_qb
+    int R, S, stride, nch;       // taps, window step, 64-channel chunks per tap
+    int stages, K;
+    const float *bias;           // [K] or null
+};
+
+struct ConvWideMaps {
+    CUtensorMap x[16];           // phase (r % st, s % st) at index (r % st) * st + s % st
+    CUtensorMap w;               // filters {C, R*S, K}
+    CUtensorMap y;               // output {K, Q, P, N}
+};
+
+struct ConvWideCtl {
+    float bias[256];
+    unsigned long long full[WD_MAX_STAGES], empty[WD_MAX_STAGES];
+};
+
+// dynamic shared memory, 1024-byte aligned: [2 x nsub staging sub-tiles] [stages x (A tile, B tile)] [ctl]
+static size_t wide_stage_bytes(int npad) { return (size_t)WD_A_BYTES + (size_t)npad * WD_KC * 2; }
+static size_t wide_staging_bytes(int npad) { return 2 * (size_t)((npad + 63) / 64) * WD_STG_BYTES; }
+static size_t wide_smem_bytes(int npad, int stages) {
+    return wide_staging_bytes(npad) + (size_t)stages * wide_stage_bytes(npad) + sizeof(ConvWideCtl) + 1024;
+}
+
+template <int ACT, int N>
+__global__ void __launch_bounds__(WD_THREADS, 1)
+k_conv_wide_fwd(const __grid_constant__ ConvWideMaps m, const ConvWideParams p) {
+    constexpr int NSUB = (N + 63) / 64;
+    constexpr int B_BYTES = N * WD_KC * 2;
+    extern __shared__ unsigned char smem_dyn[];
+    unsigned char *base = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
+    unsigned char *stg = base;
+    unsigned char *ring = base + 2 * NSUB * WD_STG_BYTES;
+    const int NST = p.stages;
+    ConvWideCtl &S = *reinterpret_cast<ConvWideCtl *>(ring + (size_t)NST * (WD_A_BYTES + B_BYTES));
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int nsteps = p.R * p.S * p.nch;
+
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < NST; ++i) { bar_init(&S.full[i], 1); bar_init(&S.empty[i], WD_CONSUMER_WARPS); }
+        fence_barrier_init();
+    }
+    for (int i = threadIdx.x; i < 256; i += WD_THREADS) S.bias[i] = (p.bias && i < p.K) ? p.bias[i] : 0.0f;
+    __syncthreads();
+
+    if (warp == WD_CONSUMER_WARPS) {
+        // ===== TMA producer: per tile and step one box of x and one box of filters =====
+        if (lane == 0) {
+            int it = 0;
+            for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x) {
+                const int n = tile / (p.n_pb * p.n_qb), rem = tile % (p.n_pb * p.n_qb);
+                const int p0 = (rem / p.n_qb) * p.Pt, q0 = (rem % p.n_qb) * p.Qt;
+                for (int r = 0; r < p.R; ++r)
+                    for (int s = 0; s < p.S; ++s) {
+                        const CUtensorMap *mx = &m.x[(r % p.stride) * p.stride + s % p.stride];
+                        for (int ch = 0; ch < p.nch; ++ch, ++it) {
+                            const int stage = it % NST;
+                            const unsigned ph = (unsigned)(it / NST) & 1u;
+                            bar_wait_relaxed(&S.empty[stage], ph ^ 1u, 32);
+                            unsigned char *a = ring + (size_t)stage * (WD_A_BYTES + B_BYTES);
+                            bar_expect_tx(&S.full[stage], (unsigned)(WD_A_BYTES + B_BYTES));
+                            tma_load_4d(a, mx, ch * WD_KC, q0 + s / p.stride, p0 + r / p.stride, n, &S.full[stage]);
+                            tma_load_3d(a + WD_A_BYTES, &m.w, ch * WD_KC, r * p.S + s, 0, &S.full[stage]);
+                        }
+                    }
+            }
+        }
+        return;
+    }
+
+    // ===== consumer warpgroups: MMA into registers, then bias / activation -> bf16 -> staging -> TMA store =====
+    const int wg = warp >> 2, wq = warp & 3;
+    const int tid_wg = threadIdx.x & 127;
+    unsigned char *my_stg = stg + (size_t)wg * NSUB * WD_STG_BYTES;
+    const uint32_t stg_s = s_u32(my_stg), bias_s = s_u32(S.bias);
+    // the warpgroup's half of the block: rows pp in [wg * Pt/2, +Pt/2) of the block, or columns [wg * 64, +64) when Pt = 1
+    const int dp = p.Pt >= 2 ? wg * (p.Pt / 2) : 0, dq = p.Pt >= 2 ? 0 : wg * 64;
+    int it = 0;
+    for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x) {
+        float acc[N / 2];
+        for (int step = 0; step < nsteps; ++step, ++it) {
+            const int stage = it % NST;
+            bar_wait(&S.full[stage], (unsigned)(it / NST) & 1u);
+            const uint32_t a0 = s_u32(ring + (size_t)stage * (WD_A_BYTES + B_BYTES)) + (uint32_t)(wg * 64 * WD_KC * 2);
+            const uint32_t b0 = s_u32(ring + (size_t)stage * (WD_A_BYTES + B_BYTES) + WD_A_BYTES);
+            wg_fence();
+#pragma unroll
+            for (int ks = 0; ks < WD_KC / 16; ++ks)       // K = 16 bf16 = 32 bytes per instruction
+                wgmma_bf16<0, 0>(acc, gmma_desc_k_sw128(a0 + ks * 32), gmma_desc_k_sw128(b0 + ks * 32), (step | ks) != 0 ? 1u : 0u);
+            wg_commit();
+            if (step > 0) {                               // the previous step's MMAs have retired: its stage is free
+                wg_wait<1>();
+                __syncwarp();
+                if (lane == 0) bar_arrive(&S.empty[(it - 1) % NST]);
+            }
+        }
+        wg_wait<0>();
+        wg_hold(acc);
+        __syncwarp();
+        if (lane == 0) bar_arrive(&S.empty[(it - 1) % NST]);
+
+        // the previous tile's stores have read the staging tile
+        if (tid_wg == 0) bulk_wait_read0();
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = wg_row(2 * h, wq, lane);      // pixel of the warpgroup's half, 0..63
+#pragma unroll
+            for (int j = 0; j < N / 8; ++j) {
+                const int c = wg_col(4 * j, lane);
+                float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+                float2 bb;
+                asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(bb.x), "=f"(bb.y) : "r"(bias_s + (uint32_t)c * 4u));
+                f0 += bb.x; f1 += bb.y;
+                if (ACT == 1) { f0 = sigmoid_bf16(f0); f1 = sigmoid_bf16(f1); }
+                __nv_bfloat162 v = __floats2bfloat162_rn(f0, f1);
+                // sub-tile j / 8 holds channels 64 (j / 8) ..; 16-byte chunk j % 8 of the row, XOR-swizzled by row % 8 (SWIZZLE_128B)
+                const uint32_t addr = stg_s + (uint32_t)((j / 8) * WD_STG_BYTES + row * 128 + (((j % 8) ^ (row & 7)) << 4) + (lane & 3) * 4);
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(*reinterpret_cast<uint32_t *>(&v)) : "memory");
+            }
+        }
+        fence_proxy_async_smem();
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+        if (tid_wg == 0) {
+            const int n = tile / (p.n_pb * p.n_qb), rem = tile % (p.n_pb * p.n_qb);
+            const int p0 = (rem / p.n_qb) * p.Pt, q0 = (rem % p.n_qb) * p.Qt;
+#pragma unroll
+            for (int sub = 0; sub < NSUB; ++sub) tma_store_4d(&m.y, my_stg + sub * WD_STG_BYTES, sub * 64, q0 + dq, p0 + dp, n);
+            bulk_commit();
+        }
+    }
+    if (tid_wg == 0) bulk_wait0();
+}
+
+typedef void (*conv_wide_fn)(const ConvWideMaps, const ConvWideParams);
+#define PCNN_WIDE_ROW(N) {k_conv_wide_fwd<0, N>, k_conv_wide_fwd<1, N>}
+static const void *conv_wide_variant(bool sigmoid, int npad) {
+    static const conv_wide_fn table[16][2] = {
+        PCNN_WIDE_ROW(16),  PCNN_WIDE_ROW(32),  PCNN_WIDE_ROW(48),  PCNN_WIDE_ROW(64),  PCNN_WIDE_ROW(80),  PCNN_WIDE_ROW(96),
+        PCNN_WIDE_ROW(112), PCNN_WIDE_ROW(128), PCNN_WIDE_ROW(144), PCNN_WIDE_ROW(160), PCNN_WIDE_ROW(176), PCNN_WIDE_ROW(192),
+        PCNN_WIDE_ROW(208), PCNN_WIDE_ROW(224), PCNN_WIDE_ROW(240), PCNN_WIDE_ROW(256)};
+    return reinterpret_cast<const void *>(table[npad / 16 - 1][sigmoid ? 1 : 0]);
+}
+#undef PCNN_WIDE_ROW
+
+// Tiling of the wide forward (host logic only): pixel block, chunks, stages and the tile grid.
+struct ConvWideShape { int Pt, Qt, nch, stages, tiles, n_pb, n_qb, npad, P, Q; };
+
+static int conv_wide_shape(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows,
+                           ConvWideShape *out) {
+    PCNN_REQUIRE(stride >= 1 && stride <= 4, PCNN_ERR_ARG, "pcnn_conv_wide_plan_create: stride %d outside 1..4", stride);
+    PCNN_REQUIRE(R >= 1 && R <= WD_MAX_RS && S >= 1 && S <= WD_MAX_RS, PCNN_ERR_ARG,
+                 "pcnn_conv_wide_plan_create: R = %d, S = %d: taps must be 1..7 in each direction", R, S);
+    PCNN_REQUIRE(N > 0 && H >= R && W >= S && C > 0 && K > 0, PCNN_ERR_ARG,
+                 "pcnn_conv_wide_plan_create: bad shape N=%d H=%d W=%d C=%d K=%d R=%d S=%d", N, H, W, C, K, R, S);
+    PCNN_REQUIRE(K % 8 == 0 && K <= 256, PCNN_ERR_ARG,
+                 "pcnn_conv_wide_plan_create: K = %d filters: K %% 8 == 0 and K <= 256 are required", K);
+    PCNN_REQUIRE(C % 8 == 0, PCNN_ERR_ARG,
+                 "pcnn_conv_wide_plan_create: C = %d channels: C %% 8 == 0 is required (16-byte pixel stride of the TMA map)", C);
+    PCNN_REQUIRE(row_pitch >= W * C && row_pitch % 8 == 0, PCNN_ERR_ARG,
+                 "pcnn_conv_wide_plan_create: row pitch %d must be >= W*C and a multiple of 8 elements (TMA 16-byte strides)", row_pitch);
+    if (image_rows <= 0) image_rows = H;
+    PCNN_REQUIRE(image_rows >= H, PCNN_ERR_ARG, "pcnn_conv_wide_plan_create: image pitch of %d rows is smaller than H = %d", image_rows, H);
+    int tc[5];
+    PCNN_REQUIRE(pcnn_conv_tc_plan_info(N, H, W, C, K, R, S, stride, row_pitch, image_rows, tc) != PCNN_OK, PCNN_ERR_ARG,
+                 "pcnn_conv_wide_plan_create: this shape is served by the row-Toeplitz forward: use pcnn_conv_tc_plan_create");
+    const int P = (H - R) / stride + 1, Q = (W - S) / stride + 1;
+    // pixel block: the Pt x Qt = 128 split that issues the fewest pixels; ties go to the wider block (longer contiguous rows)
+    long long best = -1;
+    for (int qt = 128; qt >= 1; qt /= 2) {
+        const int pt = WD_M / qt;
+        const long long blocks = (long long)((P + pt - 1) / pt) * ((Q + qt - 1) / qt);
+        if (best < 0 || blocks < best) { best = blocks; out->Pt = pt; out->Qt = qt; }
+    }
+    out->n_pb = (P + out->Pt - 1) / out->Pt;
+    out->n_qb = (Q + out->Qt - 1) / out->Qt;
+    PCNN_REQUIRE((long long)N * best < (1LL << 31), PCNN_ERR_ARG, "pcnn_conv_wide_plan_create: %lld tiles exceed the int range",
+                 (long long)N * best);
+    out->tiles = (int)(N * best);
+    out->nch = (C + WD_KC - 1) / WD_KC;
+    out->npad = (K + 15) / 16 * 16;
+    const size_t fixed = wide_smem_bytes(out->npad, 0);
+    int st = (int)(((size_t)WD_SMEM_BUDGET - fixed) / wide_stage_bytes(out->npad));
+    out->stages = st > WD_MAX_STAGES ? WD_MAX_STAGES : st;
+    out->P = P; out->Q = Q;
+    return PCNN_OK;
+}
+
+}  // namespace
+
+struct ConvWidePlan {
+    ConvWideParams p;
+    ConvWideShape sh;
+    int N, H, W, C, row_pitch, image_rows, act;
+    void *d_filt = nullptr;      // [K][R*S][C] bf16
+    float *d_bias = nullptr;
+    CUtensorMap map_w;
+};
+
+void conv_wide_free(ConvWidePlan *w) {
+    if (!w) return;
+    if (w->d_filt) cudaFree(w->d_filt);
+    if (w->d_bias) cudaFree(w->d_bias);
+    delete w;
+}
+
+extern "C" int pcnn_conv_wide_plan_info(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows,
+                                        int *out8) {
+    PCNN_REQUIRE(out8, PCNN_ERR_ARG, "pcnn_conv_wide_plan_info: NULL argument");
+    ConvWideShape sh;
+    int rc = conv_wide_shape(N, H, W, C, K, R, S, stride, row_pitch, image_rows, &sh);
+    if (rc) return rc;
+    out8[0] = sh.Pt; out8[1] = sh.Qt; out8[2] = sh.nch; out8[3] = sh.stages;
+    out8[4] = sh.tiles; out8[5] = sh.n_pb; out8[6] = sh.n_qb; out8[7] = sh.npad;
+    return PCNN_OK;
+}
+
+extern "C" int pcnn_conv_wide_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch,
+                                          int image_rows, int act, const float *filt_host, const float *bias_host,
+                                          pcnn_conv_plan **out) {
+    PCNN_REQUIRE(ctx && filt_host && out, PCNN_ERR_ARG, "pcnn_conv_wide_plan_create: NULL argument");
+    PCNN_REQUIRE(act == 0 || act == 1, PCNN_ERR_ARG, "pcnn_conv_wide_plan_create: act %d is not 0 (none) or 1 (sigmoid)", act);
+    ConvWideShape sh;
+    int rc = conv_wide_shape(N, H, W, C, K, R, S, stride, row_pitch, image_rows, &sh);
+    if (rc) return rc;
+    pcnn_device_guard g(ctx->device);
+    struct PlanGuard {                       // frees a half-built plan on every early return below
+        ConvWidePlan *p;
+        ~PlanGuard() { conv_wide_free(p); }
+    } guard{new ConvWidePlan()};
+    ConvWidePlan *pl = guard.p;
+    pl->sh = sh;
+    pl->N = N; pl->H = H; pl->W = W; pl->C = C; pl->row_pitch = row_pitch; pl->image_rows = image_rows > 0 ? image_rows : H;
+    pl->act = act;
+    ConvWideParams &p = pl->p;
+    p.Pt = sh.Pt; p.Qt = sh.Qt; p.n_pb = sh.n_pb; p.n_qb = sh.n_qb; p.tiles = sh.tiles;
+    p.R = R; p.S = S; p.stride = stride; p.nch = sh.nch; p.stages = sh.stages; p.K = K;
+    const size_t nf = (size_t)K * R * S * C;
+    std::vector<uint16_t> fb(nf);
+    for (size_t i = 0; i < nf; ++i) fb[i] = f32_to_bf16_bits(filt_host[i]);
+    PCNN_CUDA(cudaMalloc(&pl->d_filt, nf * 2));
+    PCNN_CUDA(cudaMemcpy(pl->d_filt, fb.data(), nf * 2, cudaMemcpyHostToDevice));
+    if (bias_host) {
+        PCNN_CUDA(cudaMalloc((void **)&pl->d_bias, K * sizeof(float)));
+        PCNN_CUDA(cudaMemcpy(pl->d_bias, bias_host, K * sizeof(float), cudaMemcpyHostToDevice));
+    }
+    p.bias = pl->d_bias;
+    {
+        const uint64_t dims[3] = {(uint64_t)C, (uint64_t)R * S, (uint64_t)K};
+        const uint64_t str[2] = {(uint64_t)C * 2, (uint64_t)R * S * C * 2};
+        const uint32_t box[3] = {WD_KC, 1, (uint32_t)sh.npad};
+        rc = make_map_bf16(&pl->map_w, pl->d_filt, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+        if (rc) return rc;
+    }
+    static bool configured[64] = {};        // function attributes are per device
+    if (!configured[ctx->device & 63]) {
+        for (int v = 0; v < 32; ++v)
+            PCNN_CUDA(cudaFuncSetAttribute(conv_wide_variant(v & 1, 16 * (v / 2 + 1)), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           WD_SMEM_BUDGET + 2048));
+        configured[ctx->device & 63] = true;
+    }
+    *out = conv_plan_wrap_wide(pl);
+    guard.p = nullptr;
+    return PCNN_OK;
+}
+
+int conv_wide_fwd(pcnn_ctx *ctx, const ConvWidePlan *pl, const void *x_bf16, void *y_bf16) {
+    PCNN_REQUIRE(((uintptr_t)y_bf16 & 15) == 0, PCNN_ERR_ARG, "pcnn_conv_tc_fwd: the output must be 16-byte aligned (TMA stores)");
+    const ConvWideShape &sh = pl->sh;
+    const int st = pl->p.stride, C = pl->C, K = pl->p.K;
+    ConvWideMaps m;
+    memset(&m, 0, sizeof(m));
+    m.w = pl->map_w;
+    // x phase (rb, sb): input rows rb, rb + st, ... and pixels sb, sb + st, ... of every image; extents end at the image's last
+    // row and pixel, so a box never reads pad rows, pad columns or the next image
+    for (int rb = 0; rb < st && rb < pl->p.R; ++rb)
+        for (int sb = 0; sb < st && sb < pl->p.S; ++sb) {
+            const uint64_t dims[4] = {(uint64_t)C, (uint64_t)((pl->W - sb + st - 1) / st), (uint64_t)((pl->H - rb + st - 1) / st),
+                                      (uint64_t)pl->N};
+            const uint64_t str[3] = {(uint64_t)st * C * 2, (uint64_t)st * pl->row_pitch * 2, (uint64_t)pl->image_rows * pl->row_pitch * 2};
+            const uint32_t box[4] = {WD_KC, (uint32_t)sh.Qt, (uint32_t)sh.Pt, 1};
+            void *base = const_cast<char *>(static_cast<const char *>(x_bf16)) + ((size_t)rb * pl->row_pitch + (size_t)sb * C) * 2;
+            int rc = make_map_bf16(&m.x[rb * st + sb], base, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B,
+                                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+            if (rc) return rc;
+        }
+    {
+        const uint64_t dims[4] = {(uint64_t)K, (uint64_t)sh.Q, (uint64_t)sh.P, (uint64_t)pl->N};
+        const uint64_t str[3] = {(uint64_t)K * 2, (uint64_t)sh.Q * K * 2, (uint64_t)sh.P * sh.Q * K * 2};
+        const uint32_t box[4] = {64, (uint32_t)(sh.Pt >= 2 ? sh.Qt : 64), (uint32_t)(sh.Pt >= 2 ? sh.Pt / 2 : 1), 1};
+        int rc = make_map_bf16(&m.y, y_bf16, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE);
+        if (rc) return rc;
+    }
+    ConvWideParams p = pl->p;
+    const int grid = p.tiles < ctx->sm_count ? p.tiles : ctx->sm_count;
+    void *args[] = {&m, &p};
+    PCNN_CUDA(cudaLaunchKernel(conv_wide_variant(pl->act == 1, sh.npad), dim3((unsigned)grid), dim3(WD_THREADS), args,
+                               wide_smem_bytes(sh.npad, p.stages), ctx->stream));
+    PCNN_CHECK_LAUNCH(ctx);
+    return PCNN_OK;
+}

@@ -215,6 +215,12 @@ int pcnn_persist_run(pcnn_ctx *ctx, const pcnn_split_binding &s, int B, long nst
 int pcnn_persist_check(pcnn_ctx *ctx);
 // comm.cu
 int pcnn_comm_allreduce_packed(pcnn_ctx *ctx);
+// conv_wide_tc.cu: the wide-channel forward.  conv_tc.cu owns the opaque pcnn_conv_plan; a plan made by
+// pcnn_conv_wide_plan_create holds a ConvWidePlan, which pcnn_conv_tc_fwd runs and pcnn_conv_tc_plan_destroy frees.
+struct ConvWidePlan;
+int conv_wide_fwd(pcnn_ctx *ctx, const ConvWidePlan *w, const void *x_bf16, void *y_bf16);
+void conv_wide_free(ConvWidePlan *w);
+pcnn_conv_plan *conv_plan_wrap_wide(ConvWidePlan *w);   // conv_tc.cu; takes ownership
 // pcnn_abi.cu: at least `bytes` of device scratch, valid until the next call that asks for more (work using it must be
 // enqueued on ctx->stream)
 int pcnn_scratch(pcnn_ctx *ctx, size_t bytes, void **out);

@@ -79,6 +79,23 @@ __device__ __forceinline__ void tma_load_4d(void *dst, const CUtensorMap *map, i
         "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(s_u32(bar))
         : "memory");
 }
+// shared -> global tensor store (out-of-range elements of the box are not written), and its bulk-group bookkeeping
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap *map, const void *src, int c0, int c1, int c2, int c3) {
+    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%1, %2, %3, %4}], [%5];" ::"l"(map), "r"(c0), "r"(c1),
+                 "r"(c2), "r"(c3), "r"(s_u32(src))
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
+// sigmoid for a bf16 result: 0.5 + 0.5 tanh(x / 2) with ONE transcendental (MUFU.TANH) instead of two (EX2 + RCP).
+// tanh.approx is good to ~5e-4 absolute, a quarter of a bf16 ulp of the result; the test bound (2^-8 |ref| + 1e-3) is unchanged.
+__device__ __forceinline__ float sigmoid_bf16(float x) {
+    float t;
+    asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.5f * x));
+    return fmaf(t, 0.5f, 0.5f);
+}
 
 
 // ---- wgmma (Hopper warpgroup MMA: D[64 x N] fp32 in registers += A[64 x 16] * B[16 x N], operands in shared memory) ----------

@@ -425,6 +425,25 @@ class ConvPlan:
             pass
 
 
+class WideConvPlan(ConvPlan):
+    """The wide-channel forward (pcnn_conv_wide_plan_create): the shapes ConvPlan refuses, C % 8 == 0, K % 8 == 0, K <= 256.
+    Run and closed like ConvPlan."""
+
+    def __init__(self, engine, N, H, W, C, K, R, S, filt, bias=None, act=0, row_pitch=None, image_rows=0, stride=1):
+        self.engine = engine
+        self.shape = (N, H, W, C, K, R, S)
+        self.row_pitch = int(row_pitch if row_pitch is not None else (W * C + 7) // 8 * 8)
+        filt = np.ascontiguousarray(filt, np.float32)
+        assert filt.size == K * R * S * C
+        b = None if bias is None else np.ascontiguousarray(bias, np.float32)
+        plan = C_.c_void_p()
+        check("pcnn_conv_wide_plan_create",
+              lib().pcnn_conv_wide_plan_create(engine.ctx, N, H, W, C, K, R, S, int(stride), self.row_pitch, int(image_rows), int(act),
+                                               filt.ctypes.data, None if b is None else b.ctypes.data, C_.byref(plan)))
+        self.plan = plan
+        self.out_shape = (N, (H - R) // stride + 1, (W - S) // stride + 1, K)
+
+
 def f32_to_bf16_bits(a):
     """numpy float32 -> uint16 bf16 bit patterns (round to nearest even), the rounding the kernels use; NaN -> the quiet NaN
     0x7FC0 (rounding the payload could carry into the exponent and the sign: 0x7FFFFFFF would become -0)"""
@@ -439,4 +458,4 @@ def bf16_bits_to_f32(b):
 
 
 C_ = C
-__all__ = ["Engine", "DeviceArray", "ConvPlan", "f32_to_bf16_bits", "bf16_bits_to_f32", "TRAIN_SET", "TEST_SET", "U8", "F32"]
+__all__ = ["Engine", "DeviceArray", "ConvPlan", "WideConvPlan", "f32_to_bf16_bits", "bf16_bits_to_f32", "TRAIN_SET", "TEST_SET", "U8", "F32"]

@@ -84,6 +84,65 @@ def run_bwd(name, N, H, W, C, K, R, S, iters, stride=1):
     del xb, dyb, dx
 
 
+def card():
+    """name and power limit of GPU 0, read (never set) in the same run as the measurement"""
+    import subprocess
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                             text=True, timeout=30).stdout.strip()
+        name, power = [t.strip() for t in out.split(",")]
+    except Exception:
+        name, power = torch.cuda.get_device_name(0), "unknown"
+    return name, power
+
+
+def run_wide(name, N, H, W, C, K, R, S, stride, iters):
+    """the wide-channel forward (WideConvPlan) next to torch.nn.functional.conv2d (cuDNN) on the same bf16 channels-last tensors.
+    Bound: the larger of flops / 989 TFLOP/s (H100 SXM dense bf16) and bytes / 3.35 TB/s, bytes = N * (H*W*C + P*Q*K) * 2."""
+    P, Q = (H - R) // stride + 1, (W - S) // stride + 1
+    f = rng.uniform(-0.5, 0.5, (K, R, S, C)).astype(np.float32)
+    b = rng.uniform(-0.5, 0.5, K).astype(np.float32)
+    plan = pkg.WideConvPlan(eng, N, H, W, C, K, R, S, f, b, stride=stride)
+    info = pkg.conv_wide_plan_info(N, H, W, C, K, R, S, stride)
+    x = torch.randint(0, 0x3F80, (N, H, W, C), dtype=torch.int16, device="cuda")   # positive bf16 bit patterns < 1.0
+    y = torch.empty((N, P, Q, K), dtype=torch.int16, device="cuda")
+    xt = x.view(torch.bfloat16).permute(0, 3, 1, 2)                                  # NCHW view of NHWC memory: channels-last
+    wt = torch.from_numpy(f).permute(0, 3, 1, 2).to("cuda", torch.bfloat16).contiguous(memory_format=torch.channels_last)
+    bt = torch.from_numpy(b).to("cuda", torch.bfloat16)
+
+    def timeit(fn):
+        for _ in range(5):
+            fn()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        for _ in range(iters):
+            fn()
+        e1.record(stream)
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / iters
+
+    ms = timeit(lambda: plan.fwd(x, y))
+    ms_cudnn = timeit(lambda: torch.nn.functional.conv2d(xt, wt, bt, stride=stride))
+    alg = N * (H * W * C + P * Q * K) * 2
+    flops = 2.0 * N * P * Q * K * R * S * C
+    t_tc, t_hbm = flops / 989e12, alg / 3.35e12
+    gpu, power = card()
+    print(json.dumps({"case": name, "N": N, "ms": ms, "useful_TFLOPs": flops / (ms * 1e-3) / 1e12, "alg_GBps": alg / (ms * 1e-3) / 1e9,
+                      "bound": "tensor" if t_tc >= t_hbm else "hbm", "bound_frac": max(t_tc, t_hbm) / (ms * 1e-3),
+                      "cudnn_ms": ms_cudnn, "cudnn_bound_frac": max(t_tc, t_hbm) / (ms_cudnn * 1e-3),
+                      "useful_pixel_share": info["useful_pixels"] / info["issued_pixels"], "tile": f"{info['Pt']}x{info['Qt']}",
+                      "stages": info["stages"], "gpu": gpu, "power_limit": power}), flush=True)
+    plan.close()
+    del x, y, xt
+
+
+if only == "wide":                                                     # wide channel counts (WideConvPlan), cuDNN beside them
+    run_wide("56x56x64->64 3x3", 128, 56, 56, 64, 64, 3, 3, 1, 20)
+    run_wide("28x28x128->128 3x3", 128, 28, 28, 128, 128, 3, 3, 1, 20)
+    run_wide("14x14x256->256 3x3", 128, 14, 14, 256, 256, 3, 3, 1, 20)
+    run_wide("56x56x64->256 1x1", 128, 56, 56, 64, 256, 1, 1, 1, 20)
+    run_wide("56x56x64->128 3x3 stride 2", 128, 56, 56, 64, 128, 3, 3, 2, 20)
 if only in ("all", "bwd"):
     for N in (8, 32, 128):
         run_bwd("224x224x3->64x3x3 bf16 (config 5)", N, 224, 224, 3, 64, 3, 3, 10)
