@@ -304,6 +304,21 @@ int pcnn_conv_wide_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C, int K,
  * (N * blocks per image), pixel blocks down a column of the image, pixel blocks along a row, MMA width (K rounded up to 16) }.
  * The tiles issue tiles * 128 output pixels for the N * P * Q they compute. */
 int pcnn_conv_wide_plan_info(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows, int *out8);
+/* Gradients of pcnn_conv_tc_fwd with a plan from pcnn_conv_wide_plan_create (csrc/conv_wide_bwd_tc.cu), on the tensor cores only
+ * (pcnn_conv_bwd_select does not apply).  The formulas, dy [N][(H-R)/stride+1][(W-S)/stride+1][K] dense, dw fp32 KRSC and dx bf16
+ * in x's layout are those of pcnn_conv_wgrad_strided / pcnn_conv_dgrad_strided: every element of the H x W x C image of dx is
+ * written (rows and columns no window covers get 0), pad columns and pad rows of dx are never written, and the pad contents of x
+ * are ignored, NaN included.  x, dy and dx must be 16-byte aligned.  The domain is exactly pcnn_conv_wide_plan_info's, refused
+ * with the same rule text naming the called function.  Both are deterministic: reruns are bit-identical. */
+int pcnn_conv_wide_wgrad(pcnn_ctx *ctx, const void *x_bf16_dev, const void *dy_bf16_dev, float *dw_f32_dev, int N, int H, int W, int C,
+                         int K, int R, int S, int stride, int row_pitch, int image_rows);
+int pcnn_conv_wide_dgrad(pcnn_ctx *ctx, const void *dy_bf16_dev, const float *filt_f32_dev, void *dx_bf16_dev, int N, int H, int W,
+                         int C, int K, int R, int S, int stride, int row_pitch, int image_rows);
+/* Host-only query (no GPU, no context): how those two tile a shape; refusals as theirs, naming pcnn_conv_wide_bwd_info.
+ * out10 = { weight gradient: row blocks R*S*ceil(C/64) of 64 GEMM rows (a work unit takes two), pixel ranges, pixel blocks per
+ *           range (the fewest; the forward's Pt x Qt blocks), stages, work units (row-block pairs x ranges);
+ *           input gradient: Pt, Qt of its pixel block of one phase's grid, channel groups, stages, tiles } */
+int pcnn_conv_wide_bwd_info(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows, int *out10);
 /* Backward passes of the same convolution (bf16 operands, fp32 accumulation, deterministic; wgmma kernels, see
  * pcnn_conv_bwd_select): weight gradient fp32 KRSC [ref: layer.h:371-395 bp_weight_c1, without its /576] and input gradient
  * bf16 NHWC in x's layout.  row_pitch / image_rows as for the forward plan (0 = dense). */

@@ -118,6 +118,9 @@ _SIG = {
     "pcnn_conv_tc_fwd": [_vp, _vp, _vp, _vp],
     "pcnn_conv_wide_plan_create": [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _pvp],
     "pcnn_conv_wide_plan_info": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
+    "pcnn_conv_wide_wgrad": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
+    "pcnn_conv_wide_dgrad": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
+    "pcnn_conv_wide_bwd_info": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_f32_to_bf16_rows": [_vp, _vp, _vp, _l, _i, _i],
     "pcnn_conv_bwd_plan_info": [_i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_pad_nhwc_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i],
@@ -186,6 +189,16 @@ def conv_wide_plan_info(N, H, W, C, K, R, S, stride=1, row_pitch=None, image_row
     P, Q = (H - R) // stride + 1, (W - S) // stride + 1
     return dict(Pt=out[0], Qt=out[1], chunks=out[2], stages=out[3], tiles=out[4], n_pb=out[5], n_qb=out[6], npad=out[7],
                 issued_pixels=out[4] * out[0] * out[1], useful_pixels=N * P * Q)
+
+
+def conv_wide_bwd_info(N, H, W, C, K, R, S, stride=1, row_pitch=None, image_rows=0):
+    """How the wide-channel gradients tile a shape (pcnn_conv_wide_bwd_info; host only, no GPU).  row_pitch None = W*C rounded
+    up to 8 elements, as WideConvPlan.  wgrad_units = row-block pairs x pixel ranges; wgrad_blocks_per_split is the fewest."""
+    pitch = (W * C + 7) // 8 * 8 if row_pitch is None else row_pitch
+    out = (_i * 10)()
+    check("pcnn_conv_wide_bwd_info", lib().pcnn_conv_wide_bwd_info(N, H, W, C, K, R, S, int(stride), int(pitch), int(image_rows), out))
+    return dict(wgrad_row_blocks=out[0], wgrad_splits=out[1], wgrad_blocks_per_split=out[2], wgrad_stages=out[3], wgrad_units=out[4],
+                dgrad_Pt=out[5], dgrad_Qt=out[6], dgrad_groups=out[7], dgrad_stages=out[8], dgrad_tiles=out[9])
 
 
 def conv_bwd_plan_info(N, H, W, C, K, R, S, stride=1):

@@ -357,7 +357,11 @@ int pcnn_conv_wgrad_rows(pcnn_ctx *ctx, const void *x_bf16, const void *dy_bf16,
     rc = C == 3 ? launch_rows_n<3>(ctx, map_dy, p, grid, pl.smem) : C == 1 ? launch_rows_n<1>(ctx, map_dy, p, grid, pl.smem)
        : C == 4 ? launch_rows_n<4>(ctx, map_dy, p, grid, pl.smem) : launch_rows_n<0>(ctx, map_dy, p, grid, pl.smem);
     if (rc) return rc;
-    k_conv_tc_wgrad_rows_reduce<<<(nout + 31) / 32, 256, 0, ctx->stream>>>(p.slots, dw_f32, grid, nout);
+    return pcnn_conv_wgrad_reduce_slots(ctx, p.slots, dw_f32, grid, nout);
+}
+
+int pcnn_conv_wgrad_reduce_slots(pcnn_ctx *ctx, const float *slots, float *dw, int nslots, int nout) {
+    k_conv_tc_wgrad_rows_reduce<<<(nout + 31) / 32, 256, 0, ctx->stream>>>(slots, dw, nslots, nout);
     PCNN_CHECK_LAUNCH(ctx);
     return PCNN_OK;
 }

@@ -185,39 +185,43 @@ static const void *conv_wide_variant(bool sigmoid, int npad) {
 }
 #undef PCNN_WIDE_ROW
 
-// Tiling of the wide forward (host logic only): pixel block, chunks, stages and the tile grid.
-struct ConvWideShape { int Pt, Qt, nch, stages, tiles, n_pb, n_qb, npad, P, Q; };
+}  // namespace
 
-static int conv_wide_shape(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows,
-                           ConvWideShape *out) {
-    PCNN_REQUIRE(stride >= 1 && stride <= 4, PCNN_ERR_ARG, "pcnn_conv_wide_plan_create: stride %d outside 1..4", stride);
-    PCNN_REQUIRE(R >= 1 && R <= WD_MAX_RS && S >= 1 && S <= WD_MAX_RS, PCNN_ERR_ARG,
-                 "pcnn_conv_wide_plan_create: R = %d, S = %d: taps must be 1..7 in each direction", R, S);
-    PCNN_REQUIRE(N > 0 && H >= R && W >= S && C > 0 && K > 0, PCNN_ERR_ARG,
-                 "pcnn_conv_wide_plan_create: bad shape N=%d H=%d W=%d C=%d K=%d R=%d S=%d", N, H, W, C, K, R, S);
-    PCNN_REQUIRE(K % 8 == 0 && K <= 256, PCNN_ERR_ARG,
-                 "pcnn_conv_wide_plan_create: K = %d filters: K %% 8 == 0 and K <= 256 are required", K);
-    PCNN_REQUIRE(C % 8 == 0, PCNN_ERR_ARG,
-                 "pcnn_conv_wide_plan_create: C = %d channels: C %% 8 == 0 is required (16-byte pixel stride of the TMA map)", C);
-    PCNN_REQUIRE(row_pitch >= W * C && row_pitch % 8 == 0, PCNN_ERR_ARG,
-                 "pcnn_conv_wide_plan_create: row pitch %d must be >= W*C and a multiple of 8 elements (TMA 16-byte strides)", row_pitch);
-    if (image_rows <= 0) image_rows = H;
-    PCNN_REQUIRE(image_rows >= H, PCNN_ERR_ARG, "pcnn_conv_wide_plan_create: image pitch of %d rows is smaller than H = %d", image_rows, H);
-    int tc[5];
-    PCNN_REQUIRE(pcnn_conv_tc_plan_info(N, H, W, C, K, R, S, stride, row_pitch, image_rows, tc) != PCNN_OK, PCNN_ERR_ARG,
-                 "pcnn_conv_wide_plan_create: this shape is served by the row-Toeplitz forward: use pcnn_conv_tc_plan_create");
-    const int P = (H - R) / stride + 1, Q = (W - S) / stride + 1;
-    // pixel block: the Pt x Qt = 128 split that issues the fewest pixels; ties go to the wider block (longer contiguous rows)
+// The pixel block of a P x Q output image: the Pt x Qt = 128 split that issues the fewest pixels; ties go to the wider block
+// (longer contiguous rows).  Returns the blocks per image.
+long long conv_wide_pixel_block(int P, int Q, int *Pt, int *Qt) {
     long long best = -1;
     for (int qt = 128; qt >= 1; qt /= 2) {
         const int pt = WD_M / qt;
         const long long blocks = (long long)((P + pt - 1) / pt) * ((Q + qt - 1) / qt);
-        if (best < 0 || blocks < best) { best = blocks; out->Pt = pt; out->Qt = qt; }
+        if (best < 0 || blocks < best) { best = blocks; *Pt = pt; *Qt = qt; }
     }
+    return best;
+}
+
+int conv_wide_shape(const char *fn, int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows,
+                    ConvWideShape *out) {
+    PCNN_REQUIRE(stride >= 1 && stride <= 4, PCNN_ERR_ARG, "%s: stride %d outside 1..4", fn, stride);
+    PCNN_REQUIRE(R >= 1 && R <= WD_MAX_RS && S >= 1 && S <= WD_MAX_RS, PCNN_ERR_ARG,
+                 "%s: R = %d, S = %d: taps must be 1..7 in each direction", fn, R, S);
+    PCNN_REQUIRE(N > 0 && H >= R && W >= S && C > 0 && K > 0, PCNN_ERR_ARG,
+                 "%s: bad shape N=%d H=%d W=%d C=%d K=%d R=%d S=%d", fn, N, H, W, C, K, R, S);
+    PCNN_REQUIRE(K % 8 == 0 && K <= 256, PCNN_ERR_ARG,
+                 "%s: K = %d filters: K %% 8 == 0 and K <= 256 are required", fn, K);
+    PCNN_REQUIRE(C % 8 == 0, PCNN_ERR_ARG,
+                 "%s: C = %d channels: C %% 8 == 0 is required (16-byte pixel stride of the TMA map)", fn, C);
+    PCNN_REQUIRE(row_pitch >= W * C && row_pitch % 8 == 0, PCNN_ERR_ARG,
+                 "%s: row pitch %d must be >= W*C and a multiple of 8 elements (TMA 16-byte strides)", fn, row_pitch);
+    if (image_rows <= 0) image_rows = H;
+    PCNN_REQUIRE(image_rows >= H, PCNN_ERR_ARG, "%s: image pitch of %d rows is smaller than H = %d", fn, image_rows, H);
+    int tc[5];
+    PCNN_REQUIRE(pcnn_conv_tc_plan_info(N, H, W, C, K, R, S, stride, row_pitch, image_rows, tc) != PCNN_OK, PCNN_ERR_ARG,
+                 "%s: this shape is served by the row-Toeplitz forward: use pcnn_conv_tc_plan_create", fn);
+    const int P = (H - R) / stride + 1, Q = (W - S) / stride + 1;
+    const long long best = conv_wide_pixel_block(P, Q, &out->Pt, &out->Qt);
     out->n_pb = (P + out->Pt - 1) / out->Pt;
     out->n_qb = (Q + out->Qt - 1) / out->Qt;
-    PCNN_REQUIRE((long long)N * best < (1LL << 31), PCNN_ERR_ARG, "pcnn_conv_wide_plan_create: %lld tiles exceed the int range",
-                 (long long)N * best);
+    PCNN_REQUIRE((long long)N * best < (1LL << 31), PCNN_ERR_ARG, "%s: %lld tiles exceed the int range", fn, (long long)N * best);
     out->tiles = (int)(N * best);
     out->nch = (C + WD_KC - 1) / WD_KC;
     out->npad = (K + 15) / 16 * 16;
@@ -228,7 +232,21 @@ static int conv_wide_shape(int N, int H, int W, int C, int K, int R, int S, int 
     return PCNN_OK;
 }
 
-}  // namespace
+// x phase (rb, sb) of the window step: input rows rb, rb + st, ... and pixels sb, sb + st, ... of every image; the extents end at
+// the image's last row and pixel, so a box never reads pad rows, pad columns or the next image
+int conv_wide_x_maps(CUtensorMap *maps, const void *x_bf16, int N, int H, int W, int C, int R, int S, int st, int row_pitch,
+                     int image_rows, int Pt, int Qt) {
+    for (int rb = 0; rb < st && rb < R; ++rb)
+        for (int sb = 0; sb < st && sb < S; ++sb) {
+            const uint64_t dims[4] = {(uint64_t)C, (uint64_t)((W - sb + st - 1) / st), (uint64_t)((H - rb + st - 1) / st), (uint64_t)N};
+            const uint64_t str[3] = {(uint64_t)st * C * 2, (uint64_t)st * row_pitch * 2, (uint64_t)image_rows * row_pitch * 2};
+            const uint32_t box[4] = {WD_KC, (uint32_t)Qt, (uint32_t)Pt, 1};
+            void *base = const_cast<char *>(static_cast<const char *>(x_bf16)) + ((size_t)rb * row_pitch + (size_t)sb * C) * 2;
+            int rc = make_map_bf16(&maps[rb * st + sb], base, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+            if (rc) return rc;
+        }
+    return PCNN_OK;
+}
 
 struct ConvWidePlan {
     ConvWideParams p;
@@ -250,7 +268,7 @@ extern "C" int pcnn_conv_wide_plan_info(int N, int H, int W, int C, int K, int R
                                         int *out8) {
     PCNN_REQUIRE(out8, PCNN_ERR_ARG, "pcnn_conv_wide_plan_info: NULL argument");
     ConvWideShape sh;
-    int rc = conv_wide_shape(N, H, W, C, K, R, S, stride, row_pitch, image_rows, &sh);
+    int rc = conv_wide_shape("pcnn_conv_wide_plan_create", N, H, W, C, K, R, S, stride, row_pitch, image_rows, &sh);
     if (rc) return rc;
     out8[0] = sh.Pt; out8[1] = sh.Qt; out8[2] = sh.nch; out8[3] = sh.stages;
     out8[4] = sh.tiles; out8[5] = sh.n_pb; out8[6] = sh.n_qb; out8[7] = sh.npad;
@@ -263,7 +281,7 @@ extern "C" int pcnn_conv_wide_plan_create(pcnn_ctx *ctx, int N, int H, int W, in
     PCNN_REQUIRE(ctx && filt_host && out, PCNN_ERR_ARG, "pcnn_conv_wide_plan_create: NULL argument");
     PCNN_REQUIRE(act == 0 || act == 1, PCNN_ERR_ARG, "pcnn_conv_wide_plan_create: act %d is not 0 (none) or 1 (sigmoid)", act);
     ConvWideShape sh;
-    int rc = conv_wide_shape(N, H, W, C, K, R, S, stride, row_pitch, image_rows, &sh);
+    int rc = conv_wide_shape("pcnn_conv_wide_plan_create", N, H, W, C, K, R, S, stride, row_pitch, image_rows, &sh);
     if (rc) return rc;
     pcnn_device_guard g(ctx->device);
     struct PlanGuard {                       // frees a half-built plan on every early return below
@@ -313,24 +331,13 @@ int conv_wide_fwd(pcnn_ctx *ctx, const ConvWidePlan *pl, const void *x_bf16, voi
     ConvWideMaps m;
     memset(&m, 0, sizeof(m));
     m.w = pl->map_w;
-    // x phase (rb, sb): input rows rb, rb + st, ... and pixels sb, sb + st, ... of every image; extents end at the image's last
-    // row and pixel, so a box never reads pad rows, pad columns or the next image
-    for (int rb = 0; rb < st && rb < pl->p.R; ++rb)
-        for (int sb = 0; sb < st && sb < pl->p.S; ++sb) {
-            const uint64_t dims[4] = {(uint64_t)C, (uint64_t)((pl->W - sb + st - 1) / st), (uint64_t)((pl->H - rb + st - 1) / st),
-                                      (uint64_t)pl->N};
-            const uint64_t str[3] = {(uint64_t)st * C * 2, (uint64_t)st * pl->row_pitch * 2, (uint64_t)pl->image_rows * pl->row_pitch * 2};
-            const uint32_t box[4] = {WD_KC, (uint32_t)sh.Qt, (uint32_t)sh.Pt, 1};
-            void *base = const_cast<char *>(static_cast<const char *>(x_bf16)) + ((size_t)rb * pl->row_pitch + (size_t)sb * C) * 2;
-            int rc = make_map_bf16(&m.x[rb * st + sb], base, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B,
-                                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
-            if (rc) return rc;
-        }
+    int rc = conv_wide_x_maps(m.x, x_bf16, pl->N, pl->H, pl->W, C, pl->p.R, pl->p.S, st, pl->row_pitch, pl->image_rows, sh.Pt, sh.Qt);
+    if (rc) return rc;
     {
         const uint64_t dims[4] = {(uint64_t)K, (uint64_t)sh.Q, (uint64_t)sh.P, (uint64_t)pl->N};
         const uint64_t str[3] = {(uint64_t)K * 2, (uint64_t)sh.Q * K * 2, (uint64_t)sh.P * sh.Q * K * 2};
         const uint32_t box[4] = {64, (uint32_t)(sh.Pt >= 2 ? sh.Qt : 64), (uint32_t)(sh.Pt >= 2 ? sh.Pt / 2 : 1), 1};
-        int rc = make_map_bf16(&m.y, y_bf16, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE);
+        rc = make_map_bf16(&m.y, y_bf16, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE);
         if (rc) return rc;
     }
     ConvWideParams p = pl->p;

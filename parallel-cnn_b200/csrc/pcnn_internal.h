@@ -221,6 +221,15 @@ struct ConvWidePlan;
 int conv_wide_fwd(pcnn_ctx *ctx, const ConvWidePlan *w, const void *x_bf16, void *y_bf16);
 void conv_wide_free(ConvWidePlan *w);
 pcnn_conv_plan *conv_plan_wrap_wide(ConvWidePlan *w);   // conv_tc.cu; takes ownership
+// The domain and tiling of the wide forward, which its gradients (conv_wide_bwd_tc.cu) share: one rule, refused with
+// PCNN_ERR_ARG and a message that names `fn`, the caller's entry point.  conv_wide_pixel_block picks the Pt x Qt = 128 block
+// of a P x Q image and returns the blocks per image.
+struct ConvWideShape { int Pt, Qt, nch, stages, tiles, n_pb, n_qb, npad, P, Q; };
+int conv_wide_shape(const char *fn, int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows,
+                    ConvWideShape *out);
+long long conv_wide_pixel_block(int P, int Q, int *Pt, int *Qt);
+// conv_wgrad_tc.cu: dw[o] = sum over i of slots[i][o] for o < nout, in a fixed order (deterministic, no atomics)
+int pcnn_conv_wgrad_reduce_slots(pcnn_ctx *ctx, const float *slots, float *dw, int nslots, int nout);
 // pcnn_abi.cu: at least `bytes` of device scratch, valid until the next call that asks for more (work using it must be
 // enqueued on ctx->stream)
 int pcnn_scratch(pcnn_ctx *ctx, size_t bytes, void **out);

@@ -383,6 +383,18 @@ class Engine:
         self._call("pcnn_conv_dgrad_strided", _p(dy_bf16), _p(filt_f32), _p(dx_bf16), N, H, W, Cin, K, R, S, int(stride), int(row_pitch),
                    int(image_rows))
 
+    def conv_wide_wgrad(self, x_bf16, dy_bf16, dw_f32, N, H, W, Cin, K, R, S, row_pitch=None, image_rows=0, stride=1):
+        """weight gradient of WideConvPlan's forward (pcnn_conv_wide_wgrad); row_pitch None = W*Cin rounded up to 8, as the plan"""
+        pitch = (W * Cin + 7) // 8 * 8 if row_pitch is None else row_pitch
+        self._call("pcnn_conv_wide_wgrad", _p(x_bf16), _p(dy_bf16), _p(dw_f32), N, H, W, Cin, K, R, S, int(stride), int(pitch),
+                   int(image_rows))
+
+    def conv_wide_dgrad(self, dy_bf16, filt_f32, dx_bf16, N, H, W, Cin, K, R, S, row_pitch=None, image_rows=0, stride=1):
+        """input gradient of WideConvPlan's forward (pcnn_conv_wide_dgrad) into dx in x's layout"""
+        pitch = (W * Cin + 7) // 8 * 8 if row_pitch is None else row_pitch
+        self._call("pcnn_conv_wide_dgrad", _p(dy_bf16), _p(filt_f32), _p(dx_bf16), N, H, W, Cin, K, R, S, int(stride), int(pitch),
+                   int(image_rows))
+
     def pad_nhwc(self, src_bf16, dst_bf16, N, H, W, Cin, pad_h, pad_w, dst_row_pitch=0, dst_image_rows=0):
         self._call("pcnn_pad_nhwc_bf16", _p(src_bf16), _p(dst_bf16), N, H, W, Cin, int(pad_h), int(pad_w), int(dst_row_pitch), int(dst_image_rows))
 

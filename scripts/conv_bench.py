@@ -137,12 +137,64 @@ def run_wide(name, N, H, W, C, K, R, S, stride, iters):
     del x, y, xt
 
 
+def run_wide_bwd(name, N, H, W, C, K, R, S, stride, iters):
+    """the wide-channel gradients (pcnn_conv_wide_wgrad / pcnn_conv_wide_dgrad) next to cuDNN's
+    (torch.ops.aten.convolution_backward with one gradient selected) on the same bf16 channels-last tensors.  Bound as in
+    run_wide: the larger of flops / 989 TFLOP/s and bytes / 3.35 TB/s, bytes = N * (H*W*C + P*Q*K) * 2 (the two tensors each
+    pass reads or writes once; the filters are small)."""
+    P, Q = (H - R) // stride + 1, (W - S) // stride + 1
+    info = pkg.conv_wide_bwd_info(N, H, W, C, K, R, S, stride)
+    x = torch.randint(0, 0x3F80, (N, H, W, C), dtype=torch.int16, device="cuda")   # positive bf16 bit patterns < 1.0
+    dy = torch.randint(0, 0x3F80, (N, P, Q, K), dtype=torch.int16, device="cuda")
+    dy ^= (torch.randint(0, 2, (N, P, Q, K), dtype=torch.int16, device="cuda") << 15)   # random signs
+    f = torch.rand((K, R, S, C), dtype=torch.float32, device="cuda") - 0.5
+    dw = torch.empty((K, R, S, C), dtype=torch.float32, device="cuda")
+    dx = torch.empty((N, H, W, C), dtype=torch.int16, device="cuda")
+    xt, dyt = x.view(torch.bfloat16).permute(0, 3, 1, 2), dy.view(torch.bfloat16).permute(0, 3, 1, 2)   # channels-last views
+    wt = f.permute(0, 3, 1, 2).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+    alg = N * (H * W * C + P * Q * K) * 2
+    flops = 2.0 * N * P * Q * K * R * S * C
+    t_bound = max(flops / 989e12, alg / 3.35e12)
+    gpu, power = card()
+
+    def timeit(fn):
+        for _ in range(5):
+            fn()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        for _ in range(iters):
+            fn()
+        e1.record(stream)
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / iters
+
+    def cudnn(mask):
+        return torch.ops.aten.convolution_backward(dyt, xt, wt, None, [stride, stride], [0, 0], [1, 1], False, [0, 0], 1, mask)
+
+    for what, fn, mask in (("wgrad", lambda: eng.conv_wide_wgrad(x, dy, dw, N, H, W, C, K, R, S, stride=stride), [False, True, False]),
+                           ("dgrad", lambda: eng.conv_wide_dgrad(dy, f, dx, N, H, W, C, K, R, S, stride=stride), [True, False, False])):
+        ms = timeit(fn)
+        ms_cudnn = timeit(lambda: cudnn(mask))
+        print(json.dumps({"case": f"{name} {what}", "N": N, "ms": ms, "useful_TFLOPs": flops / (ms * 1e-3) / 1e12,
+                          "bound": "tensor" if flops / 989e12 >= alg / 3.35e12 else "hbm", "bound_frac": t_bound / (ms * 1e-3),
+                          "cudnn_ms": ms_cudnn, "cudnn_TFLOPs": flops / (ms_cudnn * 1e-3) / 1e12, "cudnn_bound_frac": t_bound / (ms_cudnn * 1e-3),
+                          "tiling": {k: v for k, v in info.items() if k.startswith(what)}, "gpu": gpu, "power_limit": power}), flush=True)
+    del x, dy, dx, xt, dyt
+
+
 if only == "wide":                                                     # wide channel counts (WideConvPlan), cuDNN beside them
     run_wide("56x56x64->64 3x3", 128, 56, 56, 64, 64, 3, 3, 1, 20)
     run_wide("28x28x128->128 3x3", 128, 28, 28, 128, 128, 3, 3, 1, 20)
     run_wide("14x14x256->256 3x3", 128, 14, 14, 256, 256, 3, 3, 1, 20)
     run_wide("56x56x64->256 1x1", 128, 56, 56, 64, 256, 1, 1, 1, 20)
     run_wide("56x56x64->128 3x3 stride 2", 128, 56, 56, 64, 128, 3, 3, 2, 20)
+if only == "widebwd":                                                  # gradients of the same five layers, cuDNN beside them
+    run_wide_bwd("56x56x64->64 3x3", 128, 56, 56, 64, 64, 3, 3, 1, 20)
+    run_wide_bwd("28x28x128->128 3x3", 128, 28, 28, 128, 128, 3, 3, 1, 20)
+    run_wide_bwd("14x14x256->256 3x3", 128, 14, 14, 256, 256, 3, 3, 1, 20)
+    run_wide_bwd("56x56x64->256 1x1", 128, 56, 56, 64, 256, 1, 1, 1, 20)
+    run_wide_bwd("56x56x64->128 3x3 stride 2", 128, 56, 56, 64, 128, 3, 3, 2, 20)
 if only in ("all", "bwd"):
     for N in (8, 32, 128):
         run_bwd("224x224x3->64x3x3 bf16 (config 5)", N, 224, 224, 3, 64, 3, 3, 10)
