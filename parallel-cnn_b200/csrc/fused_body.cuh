@@ -10,22 +10,35 @@ constexpr int NWK = FUSED_WORKERS;
 constexpr int NWARP = NT / 32;          // 7
 constexpr int RED_STRIDE = 27;          // 25 c1 taps + c1 bias sum, padded to an odd stride
 
-template <typename InT> struct FusedSmem {
-    alignas(16) float params[NPACK];                 // packed parameters (9,376 B)
+// the buffers of one image stream through 224 threads: staging, fp32 image, per-image reduction scratch
+template <typename InT> struct ImageSmem {
     alignas(16) float imgf[2][PCNN_IMG];             // fp32 image, double buffered
     alignas(16) InT stage[2][PCNN_IMG];              // raw staging target of the bulk copies (u8 path only)
     alignas(16) float red[NWK * RED_STRIDE];         // epilogue scratch
     float fc_red[NWARP][PCNN_F];
     float red_s1[NWARP][17];
+    int label[2];
+    alignas(8) unsigned long long mbar[2];           // image stages
+};
+
+// what half 1 of a two-image CTA (persistent kernel) hands to half 0, which adds it to its own image's entries (image 0 +
+// image 1) and pushes each packed entry once
+struct PairXchg {
+    float fw[PCNN_F][NWK];                           // f-layer weight gradient, column t of worker t
+    float fb[PCNN_F + 1];                            // f bias gradient, error
+    float tail[173];                                 // c1 taps + c1 bias sums (36 windows), s1 taps + s1 bias (7 warps)
+};
+
+template <typename InT> struct FusedSmem : ImageSmem<InT> {
+    alignas(16) float params[NPACK];                 // packed parameters (9,376 B)
     float dpre_f[PCNN_F];
     float f_out[PCNN_F];
     float part[NT];                                  // persistent kernel: slot-phase partial sums of the owned chunk
     alignas(16) float recv[NPACK + 16];              // persistent kernel: [cluster rank][my share] gradient pieces pushed by the peers
     float accf[PCNN_F * NT];                         // persistent kernel, several images per CTA: thread-private sums of the f-layer weight gradient
     float lut[256];                                  // u8 pixel -> fp32 (mnist.h:145 + Main.cpp:64), filled once per kernel
-    int label[2];
-    alignas(8) unsigned long long mbar[5];           // [0],[1]: image stages, [2]: parameters (bulk copy or peer pushes),
-                                                     // [3]: gradient pieces pushed by the cluster peers
+    alignas(8) unsigned long long params_bar;        // parameters (bulk copy or peer pushes)
+    alignas(8) unsigned long long grads_bar;         // gradient pieces pushed by the cluster peers
     // host-streaming gate of the persistent kernel (written and read by thread 0 only)
     const void *gate_images;
     const unsigned *gate_ready;
@@ -125,6 +138,14 @@ __device__ __forceinline__ void dsmem_st_async_f2(uint32_t addr, float x, float 
                  "r"(mbar_addr)
                  : "memory");
 }
+// named CTA barrier as a one-way hand-over: the producers' arrive (no wait) releases their shared-memory stores to the
+// consumers' sync; `n` counts the threads of both sides
+__device__ __forceinline__ void named_bar_arrive(unsigned bar, unsigned n) {
+    asm volatile("bar.arrive %0, %1;" ::"r"(bar), "r"(n) : "memory");
+}
+__device__ __forceinline__ void named_bar_sync(unsigned bar, unsigned n) {
+    asm volatile("bar.sync %0, %1;" ::"r"(bar), "r"(n) : "memory");
+}
 __device__ __forceinline__ float dsmem_ld_f(uint32_t addr) {
     float v;
     asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
@@ -172,8 +193,10 @@ __device__ __forceinline__ float warp_sum16_transposed(const float (&v)[16], int
 struct ThreadId {
     int t, warp, lane, m, wx, wy;
     bool worker;
-    __device__ __forceinline__ ThreadId() {
-        t = threadIdx.x;
+    __device__ __forceinline__ ThreadId() : ThreadId((int)threadIdx.x) {}
+    // thread tt of a 224-thread group (one image's threads)
+    __device__ __forceinline__ explicit ThreadId(int tt) {
+        t = tt;
         warp = t >> 5;
         lane = t & 31;
         worker = t < NWK;
@@ -200,32 +223,37 @@ struct Acc {
     }
 };
 
-template <typename InT> __device__ __forceinline__ void init_barriers(FusedSmem<InT> &S) {
+// H1: the second image's buffers of a two-image CTA, else null
+template <typename InT> __device__ __forceinline__ void init_barriers(FusedSmem<InT> &S, ImageSmem<InT> *H1 = nullptr) {
     if (threadIdx.x == 0) {
         mbar_init(&S.mbar[0], 1);
         mbar_init(&S.mbar[1], 1);
-        mbar_init(&S.mbar[2], 1);
-        mbar_init(&S.mbar[3], 1);
+        mbar_init(&S.params_bar, 1);
+        mbar_init(&S.grads_bar, 1);
+        if (H1) {
+            mbar_init(&H1->mbar[0], 1);
+            mbar_init(&H1->mbar[1], 1);
+        }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     // mnist.h:145 + Main.cpp:64: (float)((double)u / 255.0).  u / 255 has a period-8 binary expansion, so rounding the exact
     // quotient straight to fp32 equals rounding via double (checked for all 256 values in tests/); one table per CTA instead
     // of four IEEE divisions per thread and image
-    for (int u = threadIdx.x; u < 256; u += NT) S.lut[u] = __fdiv_rn((float)u, 255.0f);
+    for (int u = threadIdx.x; u < 256; u += blockDim.x) S.lut[u] = __fdiv_rn((float)u, 255.0f);
     __syncthreads();
 }
 
-// thread 0 only: start the bulk copy of one image into staging buffer `buf`
-template <typename InT> __device__ __forceinline__ void issue_image(FusedSmem<InT> &S, int buf, const InT *src) {
+// thread 0 of the image's threads only: start the bulk copy of one image into staging buffer `buf`
+template <typename InT> __device__ __forceinline__ void issue_image(ImageSmem<InT> &H, int buf, const InT *src) {
     constexpr bool IS_U8 = (sizeof(InT) == 1);
     constexpr unsigned IMG_BYTES = PCNN_IMG * sizeof(InT);
-    mbar_expect_tx(&S.mbar[buf], IMG_BYTES);
-    bulk_g2s(IS_U8 ? (void *)S.stage[buf] : (void *)S.imgf[buf], src, IMG_BYTES, &S.mbar[buf]);
+    mbar_expect_tx(&H.mbar[buf], IMG_BYTES);
+    bulk_g2s(IS_U8 ? (void *)H.stage[buf] : (void *)H.imgf[buf], src, IMG_BYTES, &H.mbar[buf]);
 }
 // thread 0 only: start the bulk copy of the packed parameters
 template <typename InT> __device__ __forceinline__ void issue_params(FusedSmem<InT> &S, const float *params) {
-    mbar_expect_tx(&S.mbar[2], NPACK * 4);
-    bulk_g2s(S.params, params, NPACK * 4, &S.mbar[2]);
+    mbar_expect_tx(&S.params_bar, NPACK * 4);
+    bulk_g2s(S.params, params, NPACK * 4, &S.params_bar);
 }
 
 // hook called by thread 0 right before it issues the bulk copy of a prefetched image (the persistent kernel gates on the
@@ -246,20 +274,21 @@ struct EvalOut {
 // parity before the first use of S.params (lets the parameter copy overlap the u8 -> fp32 conversion).
 // P0 of an image: wait until it has landed in staging buffer li & 1, convert it to fp32 (u8 path), fetch the label.  No
 // barrier: the caller's next block barrier (sync #1 of image_pass) publishes the results.
+// H: the image's buffers (S itself, or the second image's of a two-image CTA).
 template <typename InT>
-__device__ __forceinline__ void image_prepare(FusedSmem<InT> &S, const ThreadId &id, int li, const uint8_t *label_ptr) {
+__device__ __forceinline__ void image_prepare(FusedSmem<InT> &S, ImageSmem<InT> &H, const ThreadId &id, int li, const uint8_t *label_ptr) {
     constexpr bool IS_U8 = (sizeof(InT) == 1);
     const int t = id.t;
     const int buf = li & 1;
-    mbar_wait(&S.mbar[buf], (unsigned)(li >> 1) & 1u);
+    mbar_wait(&H.mbar[buf], (unsigned)(li >> 1) & 1u);
     if (IS_U8) {
         if (t < 196) {
-            uchar4 q = reinterpret_cast<const uchar4 *>(S.stage[buf])[t];
+            uchar4 q = reinterpret_cast<const uchar4 *>(H.stage[buf])[t];
             float4 f = make_float4(S.lut[q.x], S.lut[q.y], S.lut[q.z], S.lut[q.w]);
-            reinterpret_cast<float4 *>(S.imgf[buf])[t] = f;
+            reinterpret_cast<float4 *>(H.imgf[buf])[t] = f;
         }
     }
-    if (t == NWK && label_ptr) S.label[buf] = (int)*label_ptr;
+    if (t == NWK && label_ptr) H.label[buf] = (int)*label_ptr;
 }
 
 // `prepared`: image_prepare has already run for this image (the persistent kernel does it while it waits for the step's
@@ -271,8 +300,8 @@ __device__ __forceinline__ void image_pass(FusedSmem<InT> &S, const ThreadId &id
     const int t = id.t, warp = id.warp, lane = id.lane;
     const int buf = li & 1;
     // ---- P0: the image has landed; convert to fp32 (u8 path), fetch the label
-    if (!prepared) image_prepare(S, id, li, label_ptr);
-    if (params_parity >= 0) mbar_wait(&S.mbar[2], (unsigned)params_parity);
+    if (!prepared) image_prepare(S, S, id, li, label_ptr);
+    if (params_parity >= 0) mbar_wait(&S.params_bar, (unsigned)params_parity);
     __syncthreads();                                                         // sync #1
     if (t == 0 && next_src) {
         gate(next_src);
@@ -503,8 +532,15 @@ __device__ __forceinline__ void cta_epilogue(FusedSmem<InT> &S, const ThreadId &
 //     156 c1 entries.
 // `put(p, v)` consumes packed entry p (the persistent kernel pushes it to the cluster rank that owns it).  The image must
 // have been prepared (image_prepare) by the caller; `S.params` must be complete.  Same arithmetic as image_pass + cta_epilogue.
-template <typename InT, typename Sink>
-__device__ __forceinline__ void image_step_single(FusedSmem<InT> &S, const ThreadId &id, int li, bool has_image, const Sink &put) {
+//
+// IPC = 2: a 448-thread CTA trains two images side by side, threads half * 224 + id.t running image `half` out of its own
+// buffers H with the arithmetic above; both halves read the one S.params.  Half 1 hands its f-layer gradient, f bias / error
+// and end-of-pass sums to half 0 through X (named barriers 1 and 2, arrive / sync: half 1 never waits), and half 0 pushes
+// image 0 + image 1 of every packed entry, once per CTA.
+template <int IPC, typename InT, typename Sink>
+__device__ __forceinline__ void image_step_single(FusedSmem<InT> &S, ImageSmem<InT> &H, PairXchg *X, const ThreadId &id, int half, int li,
+                                                  bool has_image, const Sink &put) {
+    constexpr bool PAIR = IPC == 2;
     const int t = id.t, warp = id.warp, lane = id.lane;
     const int buf = li & 1;
     __syncthreads();                                                         // sync #1: image + parameters visible
@@ -518,7 +554,7 @@ __device__ __forceinline__ void image_step_single(FusedSmem<InT> &S, const Threa
     for (int q = 0; q < PCNN_F; ++q) fw[q] = 0.0f;
 #pragma unroll
     for (int p = 0; p < 16; ++p) o[p] = 0.0f;
-    const float *ip = S.imgf[buf] + (id.worker ? (4 * id.wx) * 28 + 4 * id.wy : 0);
+    const float *ip = H.imgf[buf] + (id.worker ? (4 * id.wx) * 28 + 4 * id.wy : 0);
     if (work) {
         float patch[8][8];
 #pragma unroll
@@ -559,7 +595,7 @@ __device__ __forceinline__ void image_step_single(FusedSmem<InT> &S, const Threa
     __syncwarp();
     {
         const float v = warp_sum16_transposed(fcp, lane);                    // lane 2q (and 2q + 1) holds output q's warp sum
-        if ((lane & 1) == 0 && (lane >> 1) < PCNN_F) S.fc_red[warp][lane >> 1] = v;
+        if ((lane & 1) == 0 && (lane >> 1) < PCNN_F) H.fc_red[warp][lane >> 1] = v;
     }
     __syncthreads();                                                         // sync #2
     // f output, makeError (layer.h:91-95), vectorNorm (Main.cpp:28-34): every warp for itself, d_preact broadcast by shuffle
@@ -568,20 +604,47 @@ __device__ __forceinline__ void image_step_single(FusedSmem<InT> &S, const Threa
     if (lane < PCNN_F && has_image) {
         float pre = 0.0f;
 #pragma unroll
-        for (int w = 0; w < NWARP; ++w) pre += S.fc_red[w][lane];
+        for (int w = 0; w < NWARP; ++w) pre += H.fc_red[w][lane];
         pre += S.params[OFF_FB + lane];                                      // fp_bias_f, layer.h:206-211
-        d = (lane == S.label[buf] ? 1.0f : 0.0f) - sigmoid_fast(pre);
+        d = (lane == H.label[buf] ? 1.0f : 0.0f) - sigmoid_fast(pre);
     }
     __syncwarp();
 #pragma unroll
     for (int q = 0; q < PCNN_F; ++q) dq[q] = __shfl_sync(0xffffffffu, d, q);
-    if (warp == 0) {
-        if (lane < PCNN_F) put(OFF_FB + lane, d);                            // bp_bias_f accumulator, layer.h:229-234
-        if (lane == 0) {
-            float ss = 0.0f;
+    float err = 0.0f;
+    if (!PAIR) {
+        if (warp == 0) {
+            if (lane < PCNN_F) put(OFF_FB + lane, d);                        // bp_bias_f accumulator, layer.h:229-234
+            if (lane == 0) {
+                float ss = 0.0f;
 #pragma unroll
-            for (int q = 0; q < PCNN_F; ++q) ss = fmaf(dq[q], dq[q], ss);
-            put(OFF_ERR, has_image ? sqrtf(ss) : 0.0f);
+                for (int q = 0; q < PCNN_F; ++q) ss = fmaf(dq[q], dq[q], ss);
+                put(OFF_ERR, has_image ? sqrtf(ss) : 0.0f);
+            }
+        }
+    } else if (warp == 0 && lane == 0) {
+        float ss = 0.0f;
+#pragma unroll
+        for (int q = 0; q < PCNN_F; ++q) ss = fmaf(dq[q], dq[q], ss);
+        err = has_image ? sqrtf(ss) : 0.0f;
+    }
+    if (PAIR && half == 1) {                                                  // image 1's f-layer entries go to half 0
+        if (warp == 0) {
+            if (lane < PCNN_F) X->fb[lane] = d;
+            if (lane == 0) X->fb[PCNN_F] = err;
+        }
+        if (id.worker) {
+#pragma unroll
+            for (int q = 0; q < PCNN_F; ++q) X->fw[q][t] = dq[q] * s1o;
+        }
+        __syncwarp();
+        named_bar_arrive(1, 2 * NT);
+    } else if (PAIR) {                                                       // image 0 + image 1, before the convolution
+        __syncwarp();
+        named_bar_sync(1, 2 * NT);
+        if (warp == 0) {
+            if (lane < PCNN_F) put(OFF_FB + lane, d + X->fb[lane]);
+            if (lane == 0) put(OFF_ERR, err + X->fb[PCNN_F]);
         }
     }
     __syncwarp();
@@ -596,7 +659,8 @@ __device__ __forceinline__ void image_step_single(FusedSmem<InT> &S, const Threa
         float dout_s1 = 0.0f;
 #pragma unroll
         for (int q = 0; q < PCNN_F; ++q) {
-            put(OFF_FW + q * PCNN_S1 + t, dq[q] * s1o);                      // bp_weight_f, layer.h:214-227: on its way already
+            if (!PAIR) put(OFF_FW + q * PCNN_S1 + t, dq[q] * s1o);           // bp_weight_f, layer.h:214-227: on its way already
+            else if (half == 0) put(OFF_FW + q * PCNN_S1 + t, __fmul_rn(dq[q], s1o) + X->fw[q][t]);
             dout_s1 = fmaf(fw[q], dq[q], dout_s1);                           // bp_output_s1, layer.h:237-257
         }
         const float dpre_s1 = dout_s1 * s1o * (1.0f - s1o);                  // bp_preact_s1, layer.h:260-270
@@ -615,9 +679,9 @@ __device__ __forceinline__ void image_step_single(FusedSmem<InT> &S, const Threa
 #pragma unroll
         for (int p = 0; p < 16; ++p) d16[p] = dws[p];
         const float v = warp_sum16_transposed(d16, lane);
-        if ((lane & 1) == 0) S.red_s1[warp][lane >> 1] = v;
+        if ((lane & 1) == 0) H.red_s1[warp][lane >> 1] = v;
         const float vb = warp_sum(dws[16]);
-        if (lane == 0) S.red_s1[warp][16] = vb;
+        if (lane == 0) H.red_s1[warp][16] = vb;
     }
     if (id.worker) {
         // bp_weight_c1, layer.h:371-395 (the /576 is applied once, below): the patch comes back from shared memory in one go
@@ -630,7 +694,7 @@ __device__ __forceinline__ void image_step_single(FusedSmem<InT> &S, const Threa
             patch[r][0] = lo.x; patch[r][1] = lo.y; patch[r][2] = lo.z; patch[r][3] = lo.w;
             patch[r][4] = hi.x; patch[r][5] = hi.y; patch[r][6] = hi.z; patch[r][7] = hi.w;
         }
-        float *row = S.red + t * RED_STRIDE;
+        float *row = H.red + t * RED_STRIDE;
 #pragma unroll
         for (int i = 0; i < 5; ++i)
 #pragma unroll
@@ -644,11 +708,38 @@ __device__ __forceinline__ void image_step_single(FusedSmem<InT> &S, const Threa
             }
         row[25] = bsum_c1;
     }
-    __syncthreads();                                                         // sync #3: S.red, S.red_s1 complete
-    if (t < 156) {                       // 150 c1 taps + 6 c1 bias sums: sum over the 36 windows of a map, 4 chains
+    __syncthreads();                                                         // sync #3: H.red, H.red_s1 complete
+    if (!PAIR) {
+        if (t < 156) {                   // 150 c1 taps + 6 c1 bias sums: sum over the 36 windows of a map, 4 chains
+            const int mm = t < 150 ? t / 25 : t - 150;
+            const int col = t < 150 ? t % 25 : 25;
+            const float *r = H.red + (mm * 36) * RED_STRIDE + col;
+            float s0 = 0.0f, s1 = 0.0f, s2 = 0.0f, s3 = 0.0f;
+#pragma unroll
+            for (int w = 0; w < 36; w += 4) {
+                s0 += r[(w + 0) * RED_STRIDE];
+                s1 += r[(w + 1) * RED_STRIDE];
+                s2 += r[(w + 2) * RED_STRIDE];
+                s3 += r[(w + 3) * RED_STRIDE];
+            }
+            const float ssum = (s0 + s1) + (s2 + s3);
+            if (t < 150) put(OFF_C1W + t, ssum * (1.0f / 576.0f));
+            else put(OFF_C1B + mm, ssum);
+        } else if (t < 173) {            // s1 taps and s1 bias sum
+            const int p = t - 156;
+            float ssum = 0.0f;
+#pragma unroll
+            for (int w = 0; w < NWARP; ++w) ssum += H.red_s1[w][p];
+            put(OFF_S1W + p, ssum);      // p == 16 lands on OFF_S1B
+        }
+        return;
+    }
+    // the same sums of both images: image 0 + image 1
+    float ssum = 0.0f;
+    if (t < 156) {
         const int mm = t < 150 ? t / 25 : t - 150;
         const int col = t < 150 ? t % 25 : 25;
-        const float *r = S.red + (mm * 36) * RED_STRIDE + col;
+        const float *r = H.red + (mm * 36) * RED_STRIDE + col;
         float s0 = 0.0f, s1 = 0.0f, s2 = 0.0f, s3 = 0.0f;
 #pragma unroll
         for (int w = 0; w < 36; w += 4) {
@@ -657,16 +748,23 @@ __device__ __forceinline__ void image_step_single(FusedSmem<InT> &S, const Threa
             s2 += r[(w + 2) * RED_STRIDE];
             s3 += r[(w + 3) * RED_STRIDE];
         }
-        const float ssum = (s0 + s1) + (s2 + s3);
-        if (t < 150) put(OFF_C1W + t, ssum * (1.0f / 576.0f));
-        else put(OFF_C1B + mm, ssum);
-    } else if (t < 173) {                // s1 taps and s1 bias sum
-        const int p = t - 156;
-        float ssum = 0.0f;
+        ssum = (s0 + s1) + (s2 + s3);
+    } else if (t < 173) {
 #pragma unroll
-        for (int w = 0; w < NWARP; ++w) ssum += S.red_s1[w][p];
-        put(OFF_S1W + p, ssum);          // p == 16 lands on OFF_S1B
+        for (int w = 0; w < NWARP; ++w) ssum += H.red_s1[w][t - 156];
     }
+    if (half == 1) {
+        if (t < 173) X->tail[t] = ssum;
+        __syncwarp();
+        named_bar_arrive(2, 2 * NT);
+        return;
+    }
+    __syncwarp();
+    named_bar_sync(2, 2 * NT);                                               // the 72 windows / 14 warps of the pair
+    if (t < 173) ssum += X->tail[t];
+    if (t < 150) put(OFF_C1W + t, ssum * (1.0f / 576.0f));
+    else if (t < 156) put(OFF_C1B + t - 150, ssum);
+    else if (t < 173) put(OFF_S1W + t - 156, ssum);                          // t == 172 lands on OFF_S1B
 }
 
 // Several images per CTA and step (batch > grid): the same structure as image_step_single -- whole patch in registers per
@@ -689,7 +787,7 @@ __device__ __forceinline__ int image_steps_multi(FusedSmem<InT> &S, const Thread
     const float *ip_off = nullptr;
     for (int b = c; b < nb; b += G, ++li) {
         const int buf = li & 1;
-        if (b != c) image_prepare(S, id, li, lab_base + b);
+        if (b != c) image_prepare(S, S, id, li, lab_base + b);
         __syncthreads();                                                     // sync #1: image (+ parameters) visible
         const int bn = b + G;
         if (t == 0 && bn < nb) {

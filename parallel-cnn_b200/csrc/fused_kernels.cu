@@ -75,10 +75,10 @@ __global__ void __launch_bounds__(NT, FUSED_CTAS_PER_SM) k_fused(const FusedArgs
     }
     if (!TRAIN) {
         if (id.t == 0 && a.wrong && A.wrong) atomicAdd(a.wrong, A.wrong);
-        if (li == 0) mbar_wait(&S.mbar[2], 0);   // never exit with the parameter copy still in flight
+        if (li == 0) mbar_wait(&S.params_bar, 0);   // never exit with the parameter copy still in flight
         return;
     }
-    if (li == 0) mbar_wait(&S.mbar[2], 0);
+    if (li == 0) mbar_wait(&S.params_bar, 0);
     cta_epilogue(S, id, A, FloatSink{a.slots + (long long)blockIdx.x * NPACK});
 }
 // ---- second kernel: fixed-order reduction of the per-CTA slots, optional update ------------------------------

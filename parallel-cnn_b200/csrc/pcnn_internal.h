@@ -117,6 +117,8 @@ struct pcnn_ctx {
     bool persist_no_coop = false;           // the driver refused cooperative + cluster launches
     int persist_force_cluster = 0;          // > 0: cap the cluster size (A/B measurements through pcnn_persist_tune)
     int persist_last_cluster = 0, persist_last_grid = 0, persist_last_direct = 0;
+    int persist_pair_cap[2] = {0, 0};       // co-resident two-image CTAs (448 threads) in clusters of 4 / of 2
+    int persist_last_ipc = 0;               // images per CTA of the most recent launch
     bool persist_no_direct = false;         // measurement knob: keep the two-stage exchange on 2..4 GPUs
     int *d_abort = nullptr;                 // set by a spin loop that ran out of budget
     long long *d_trace = nullptr;           // optional phase timestamps of the persistent kernel (pcnn_persist_trace)

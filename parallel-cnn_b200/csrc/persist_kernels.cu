@@ -165,13 +165,13 @@ template <int CS> struct Share {
 
 // Step 1: poll this rank's share of the tagged parameters and push every pair into S.params of ALL CTAs of the cluster;
 // then wait until this CTA's own S.params has received all NPACK floats (thread 0 armed the mbarrier for them).
-template <typename InT, int CS>
+template <typename InT, int CS, int NTH>
 __device__ __forceinline__ void fetch_params_cluster(FusedSmem<InT> &S, const llword *pll, unsigned tag, unsigned crank, unsigned parity,
                                                      int *abort_flag) {
     static_assert(NPACK % 2 == 0, "pairs");
     const int sb = (int)crank * Share<CS>::SH, sl = Share<CS>::len(crank);
     PollGuard guard(abort_flag, &S.aborted);
-    for (int i = threadIdx.x; i < sl / 2; i += NT) {
+    for (int i = threadIdx.x; i < sl / 2; i += NTH) {
         float v0, v1;
         unsigned g0, g1;
         for (;;) {
@@ -183,10 +183,10 @@ __device__ __forceinline__ void fetch_params_cluster(FusedSmem<InT> &S, const ll
             *reinterpret_cast<float2 *>(dst) = make_float2(v0, v1);       // published by the image pass's first block barrier
         } else {
 #pragma unroll
-            for (unsigned q = 0; q < (unsigned)CS; ++q) dsmem_st_async_f2(dsmem_addr(dst, q), v0, v1, dsmem_addr(&S.mbar[2], q));
+            for (unsigned q = 0; q < (unsigned)CS; ++q) dsmem_st_async_f2(dsmem_addr(dst, q), v0, v1, dsmem_addr(&S.params_bar, q));
         }
     }
-    if (CS > 1) mbar_wait_guarded(&S.mbar[2], parity, guard);
+    if (CS > 1) mbar_wait_guarded(&S.params_bar, parity, guard);
 }
 
 // gradient piece sink of the CTA epilogue: entry p goes to the cluster rank that owns its share
@@ -200,7 +200,7 @@ template <typename InT, int CS> struct PushSink {
         }
         const unsigned q = (unsigned)p / (unsigned)Share<CS>::SH;
         const int i = p - (int)q * Share<CS>::SH;
-        dsmem_st_async_f32(dsmem_addr(S->recv + (int)crank * Share<CS>::SH + i, q), v, dsmem_addr(&S->mbar[3], q));
+        dsmem_st_async_f32(dsmem_addr(S->recv + (int)crank * Share<CS>::SH + i, q), v, dsmem_addr(&S->grads_bar, q));
     }
 };
 
@@ -221,22 +221,25 @@ template <typename InT> struct ChunkGate {
     }
 };
 
-// Steps 2 and 3 of a step: forward + backward over this CTA's images b = c, c + G, ... < nb, then the CTA reduction whose
-// results are pushed piece-wise to the cluster ranks.  Returns the advanced CTA-local image counter.
-template <typename InT, int CS>
-__device__ __forceinline__ int step_images(FusedSmem<InT> &S, const ThreadId &id, const InT *img_base, const uint8_t *lab_base, int c, int G,
-                                           int nb, int li, unsigned crank, long long *trace_row, long long *trace_row2) {
+// Steps 2 and 3 of a step: forward + backward over this CTA's images b = c, c + G, ... < nb (IPC = 2: image 2c + half of
+// each half), then the CTA reduction whose results are pushed piece-wise to the cluster ranks.  Returns the advanced
+// image counter of this thread's half.
+template <typename InT, int CS, int IPC>
+__device__ __forceinline__ int step_images(FusedSmem<InT> &S, ImageSmem<InT> &H, PairXchg *X, const ThreadId &id, int half,
+                                           const InT *img_base, const uint8_t *lab_base, int c, int G, int nb, int li, unsigned crank,
+                                           long long *trace_row, long long *trace_row2) {
     const ChunkGate<InT> gate{&S};
-    if (nb <= G) {
-        // at most one image per CTA (batch <= grid, the usual case): the specialised single-image step; the image was
-        // prepared (landed + converted) while the CTA was waiting for the parameters
-        image_step_single(S, id, li, c < nb, PushSink<InT, CS>{&S, crank});
-        if (id.t == 0 && (trace_row || trace_row2)) {
+    if (IPC == 2 || nb <= G) {
+        // at most one image per CTA half (batch <= images the grid holds side by side, the usual case): the specialised
+        // single-image step; the image was prepared (landed + converted) while the CTA was waiting for the parameters
+        const int ci = c * IPC + half;
+        image_step_single<IPC>(S, H, X, id, half, li, ci < nb, PushSink<InT, CS>{&S, crank});
+        if (threadIdx.x == 0 && (trace_row || trace_row2)) {
             const long long now = globaltimer_ns();
             if (trace_row) trace_row[2] = now;
             if (trace_row2) trace_row2[2] = now;
         }
-        return c < nb ? li + 1 : li;
+        return ci < nb ? li + 1 : li;
     }
     li = image_steps_multi(S, id, img_base, lab_base, c, G, nb, li, gate, PushSink<InT, CS>{&S, crank});
     if (id.t == 0 && (trace_row || trace_row2)) {
@@ -247,15 +250,34 @@ __device__ __forceinline__ int step_images(FusedSmem<InT> &S, const ThreadId &id
     return li;
 }
 
+// two-image CTA (IPC = 2): image 0's buffers and everything the CTA shares, image 1's buffers, the hand-over area
+template <typename InT> struct PairSmem {
+    FusedSmem<InT> s;
+    ImageSmem<InT> h1;
+    PairXchg x;
+};
+template <typename InT, int IPC> constexpr size_t persist_smem_bytes() {
+    return IPC == 1 ? sizeof(FusedSmem<InT>) : sizeof(PairSmem<InT>);
+}
+
 // DIRECT (2 GPUs, see PersistArgs::xslots) is compile-time: as a run-time flag the generalised slot addressing of the owner gather
 // is paid by every configuration, one GPU included (compare builds with scripts/step_ab_raw.py).
-template <typename InT, int CS, bool DIRECT>
-__global__ void __launch_bounds__(NT, FUSED_CTAS_PER_SM) k_train_persist(const PersistArgs a) {
+// IPC: images per CTA trained side by side.  1: one 224-thread CTA per image, two CTAs per SM.  2: one 448-thread CTA per SM
+// whose halves (threads half * 224 ...) train images 2c and 2c + 1; the CTA's once-per-step work (parameter fetch, gradient
+// pushes, cluster slot, barriers) is then done once per SM instead of twice (image_step_single).
+template <typename InT, int CS, bool DIRECT, int IPC>
+__global__ void __launch_bounds__(NT * IPC, IPC == 1 ? FUSED_CTAS_PER_SM : 1) k_train_persist(const PersistArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
+    constexpr int NTH = NT * IPC;
     FusedSmem<InT> &S = *reinterpret_cast<FusedSmem<InT> *>(smem_raw);
-    const ThreadId id;
-    const int t = id.t;
+    PairSmem<InT> &PS = *reinterpret_cast<PairSmem<InT> *>(smem_raw);      // IPC = 2 only
+    const int half = IPC == 1 ? 0 : (int)threadIdx.x / NT;
+    ImageSmem<InT> &H = half == 0 ? static_cast<ImageSmem<InT> &>(S) : PS.h1;
+    PairXchg *X = IPC == 1 ? nullptr : &PS.x;
+    const ThreadId id((int)threadIdx.x - half * NT);                         // thread within its image's 224
+    const int t = threadIdx.x;
     const int G = gridDim.x, c = blockIdx.x;
+    const int ci = c * IPC + half;                                           // this half's image of the batch
     const InT *images = reinterpret_cast<const InT *>(a.images);
     const ChunkGate<InT> gate{&S};
     if (t == 0) {
@@ -272,7 +294,7 @@ __global__ void __launch_bounds__(NT, FUSED_CTAS_PER_SM) k_train_persist(const P
     const int NC = G / CS;                                // clusters = slots
     const int my_sb = (int)crank * Share<CS>::SH, my_sl = Share<CS>::len(crank);
     llword *cslot = a.slots_ll + (long long)(CS == 1 ? (unsigned)c : cluster_idx()) * NPACK;
-    // owner geometry: this CTA owns packed entries [e0, e0 + cnt); thread t owns entry e0 + t (wide chunks: + i * NT)
+    // owner geometry: this CTA owns packed entries [e0, e0 + cnt); thread t owns entry e0 + t (wide chunks: + i * NTH)
     const int chunk = (NPACK + G - 1) / G;
     const int e0 = c * chunk;
     const int cnt = e0 >= NPACK ? 0 : (e0 + chunk > NPACK ? NPACK - e0 : chunk);
@@ -299,13 +321,13 @@ __global__ void __launch_bounds__(NT, FUSED_CTAS_PER_SM) k_train_persist(const P
         if (t == 0) *(volatile int *)a.abort_flag = 4;
         return;
     }
-    init_barriers(S);
+    init_barriers(S, IPC == 1 ? nullptr : &PS.h1);
     if (CS > 1) cluster_sync_all();   // every CTA's mbarriers are initialised before a peer may signal them
-    int li = 0;                 // CTA-local running image counter (staging buffer + mbarrier phase)
-    if (t == 0 && c < nb) {
-        const InT *src = images + (base + c) * PCNN_IMG;
+    int li = 0;                 // running image counter of this half (staging buffer + mbarrier phase)
+    if (id.t == 0 && ci < nb) {
+        const InT *src = images + (base + ci) * PCNN_IMG;
         gate(src);
-        issue_image(S, 0, src);
+        issue_image(H, 0, src);
     }
     __syncwarp();   // lane 0 rejoins its warp (see image_pass)
 
@@ -313,7 +335,7 @@ __global__ void __launch_bounds__(NT, FUSED_CTAS_PER_SM) k_train_persist(const P
     // the first step
     float w0 = 0.0f;            // chunk < NT (the usual case): the one parameter this thread owns
 #pragma unroll 1
-    for (int e = t; e < cnt; e += NT) {
+    for (int e = t; e < cnt; e += NTH) {
         const int p = e0 + e;
         const float w = p < NPARAM ? __ldcg(a.params + p) : 0.0f;
         if (e == t) w0 = w;
@@ -333,39 +355,39 @@ __global__ void __launch_bounds__(NT, FUSED_CTAS_PER_SM) k_train_persist(const P
         // ---- 1. this step's parameters: my share L2 -> shared memory of the whole cluster.  Thread 0 arms both
         //         mbarriers of the step: all NPACK parameters, and CS pieces of my gradient share
         if (CS > 1 && t == 0) {
-            mbar_expect_tx(&S.mbar[2], NPACK * 4);
-            mbar_expect_tx(&S.mbar[3], (unsigned)(CS * my_sl * 4));
+            mbar_expect_tx(&S.params_bar, NPACK * 4);
+            mbar_expect_tx(&S.grads_bar, (unsigned)(CS * my_sl * 4));
         }
         __syncwarp();
         // the step's first image has been in flight since the previous step: land + convert it while the owners publish
-        if (c < nb) image_prepare(S, id, li, a.labels + base + c);
-        fetch_params_cluster<InT, CS>(S, a.params_ll, tag, crank, (unsigned)s & 1u, a.abort_flag);
+        if (ci < nb) image_prepare(S, H, id, li, a.labels + base + ci);
+        fetch_params_cluster<InT, CS, NTH>(S, a.params_ll, tag, crank, (unsigned)s & 1u, a.abort_flag);
         PCNN_TRACE2(1);
 
         // Images in pinned HOST memory (pcnn_learn_host): the NEXT step's first image is requested now, a whole step ahead, so that
-        // the PCIe latency disappears behind the step; the other staging buffer is free (one image per CTA and step;
+        // the PCIe latency disappears behind the step; the other staging buffer is free (one image per CTA half and step;
         // with more, the in-step prefetch chain owns it).  Device-resident data keep the late request (no PCIe latency to hide).
-        const bool early_issue = a.early != 0 && nb <= G;
-        if (early_issue && t == 0 && s + 1 < a.nsteps) {
+        const bool early_issue = a.early != 0 && nb <= G * IPC;
+        if (early_issue && id.t == 0 && s + 1 < a.nsteps) {
             long long ecur = cursor + stride;
             if (ecur >= a.n_total) ecur = 0;
             long long ebase;
             int enb;
             shard(ecur, ebase, enb);
-            if (c < enb) issue_image(S, (c < nb ? li + 1 : li) & 1, images + (ebase + c) * PCNN_IMG);
+            if (ci < enb) issue_image(H, (ci < nb ? li + 1 : li) & 1, images + (ebase + ci) * PCNN_IMG);
         }
         __syncwarp();
 
         // ---- 2. forward + backward over this CTA's images, 3. CTA reduction, pieces pushed to the cluster ranks
-        li = step_images<InT, CS>(S, id, images + base * PCNN_IMG, a.labels + base, c, G, nb, li, crank,
-                                  tr0, tr1);
+        li = step_images<InT, CS, IPC>(S, H, X, id, half, images + base * PCNN_IMG, a.labels + base, c, G, nb, li, crank,
+                                       tr0, tr1);
 
         // ---- 4. my share: the CS pieces (rank order) -> tagged cluster slot
         {
             PollGuard guard(a.abort_flag, &S.aborted);
-            if (CS > 1) mbar_wait_guarded(&S.mbar[3], (unsigned)s & 1u, guard);
+            if (CS > 1) mbar_wait_guarded(&S.grads_bar, (unsigned)s & 1u, guard);
             else __syncthreads();
-            for (int i = t; i < my_sl; i += NT) {
+            for (int i = t; i < my_sl; i += NTH) {
                 float g = 0.0f;
 #pragma unroll
                 for (int q = 0; q < CS; ++q) g += S.recv[q * Share<CS>::SH + i];
@@ -387,10 +409,10 @@ __global__ void __launch_bounds__(NT, FUSED_CTAS_PER_SM) k_train_persist(const P
         int nnb;
         shard(ncur, nbase, nnb);
         const bool more = s + 1 < a.nsteps;
-        if (t == 0 && more && c < nnb && !early_issue) {
-            const InT *src = images + (nbase + c) * PCNN_IMG;
+        if (id.t == 0 && more && ci < nnb && !early_issue) {
+            const InT *src = images + (nbase + ci) * PCNN_IMG;
             gate(src);
-            issue_image(S, li & 1, src);
+            issue_image(H, li & 1, src);
         }
         __syncwarp();
 
@@ -524,7 +546,7 @@ __global__ void __launch_bounds__(NT, FUSED_CTAS_PER_SM) k_train_persist(const P
         } else {                                                               // G <= 10: a thread owns several entries
             PCNN_TRACE2(4);
 #pragma unroll 1
-            for (int e = t; e < cnt; e += NT) {
+            for (int e = t; e < cnt; e += NTH) {
                 const int p = e0 + e;
                 const llword *sp = a.slots_ll + p;
                 PollGuard guard(a.abort_flag, &S.aborted);
@@ -556,11 +578,15 @@ __global__ void __launch_bounds__(NT, FUSED_CTAS_PER_SM) k_train_persist(const P
 }
 
 constexpr int PERSIST_CS = 8;            // cluster size of the dataflow kernel (1 = fallback without clusters)
+// cluster sizes of the two-image kernel, preferred first: at one CTA per SM a cluster needs that many SMs of one GPC.  An
+// H100 80GB HBM3 keeps 120 such CTAs co-resident in clusters of 4 (or 8) -- up to 240 images -- and 128 and more in clusters
+// of 2 (a batch of 256).  Where both fit, clusters of 4 are faster (fewer cluster slots to gather).
+constexpr int PAIR_CS[2] = {4, 2};
 
 template <typename InT> int persist_cap(int *out) {
     int m = 1 << 30;
-    const void *fns[3] = {(const void *)k_train_persist<InT, PERSIST_CS, false>, (const void *)k_train_persist<InT, PERSIST_CS, true>,
-                          (const void *)k_train_persist<InT, 1, false>};
+    const void *fns[3] = {(const void *)k_train_persist<InT, PERSIST_CS, false, 1>, (const void *)k_train_persist<InT, PERSIST_CS, true, 1>,
+                          (const void *)k_train_persist<InT, 1, false, 1>};
     for (const void *fn : fns) {
         int per_sm = 0;
         cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem<InT>));
@@ -572,25 +598,44 @@ template <typename InT> int persist_cap(int *out) {
     return PCNN_OK;
 }
 
-// CTAs that can be co-resident when the grid is launched as clusters of PERSIST_CS (0 when they cannot be scheduled)
-template <typename InT> int cluster_cap(int sm_count) {
+// CTAs of IPC images each that can be co-resident when the grid is launched as clusters of CSZ (0 when they cannot be
+// scheduled)
+template <typename InT, int IPC, int CSZ> int cluster_cap(int sm_count) {
+    if constexpr (IPC == 2) {      // the single-image variants are set up by persist_cap
+        const void *fns[2] = {(const void *)k_train_persist<InT, CSZ, false, 2>, (const void *)k_train_persist<InT, CSZ, true, 2>};
+        for (const void *fn : fns)
+            if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)persist_smem_bytes<InT, 2>()) != cudaSuccess) {
+                cudaGetLastError();
+                return 0;
+            }
+    }
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)(PERSIST_CS * sm_count));     // any multiple of the cluster size
-    cfg.blockDim = dim3(NT);
-    cfg.dynamicSmemBytes = sizeof(FusedSmem<InT>);
+    cfg.gridDim = dim3((unsigned)(CSZ * sm_count));            // any multiple of the cluster size
+    cfg.blockDim = dim3(NT * IPC);
+    cfg.dynamicSmemBytes = persist_smem_bytes<InT, IPC>();
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = PERSIST_CS;
+    at[0].val.clusterDim.x = CSZ;
     at[0].val.clusterDim.y = 1;
     at[0].val.clusterDim.z = 1;
     cfg.attrs = at;
     cfg.numAttrs = 1;
     int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, k_train_persist<InT, PERSIST_CS, false>, &cfg) != cudaSuccess) {
+    if (cudaOccupancyMaxActiveClusters(&n, k_train_persist<InT, CSZ, false, IPC>, &cfg) != cudaSuccess) {
         cudaGetLastError();
         return 0;
     }
-    return n * PERSIST_CS;
+    return n * CSZ;
+}
+
+template <typename InT> const void *persist_fn(int cs, bool direct, int ipc) {
+    if (ipc == 2 && cs == PAIR_CS[0])
+        return direct ? (const void *)k_train_persist<InT, PAIR_CS[0], true, 2> : (const void *)k_train_persist<InT, PAIR_CS[0], false, 2>;
+    if (ipc == 2)
+        return direct ? (const void *)k_train_persist<InT, PAIR_CS[1], true, 2> : (const void *)k_train_persist<InT, PAIR_CS[1], false, 2>;
+    if (cs > 1)
+        return direct ? (const void *)k_train_persist<InT, PERSIST_CS, true, 1> : (const void *)k_train_persist<InT, PERSIST_CS, false, 1>;
+    return (const void *)k_train_persist<InT, 1, false, 1>;
 }
 
 }  // namespace
@@ -604,10 +649,20 @@ int pcnn_persist_configure(pcnn_ctx *ctx) {
     ctx->persist_cap = per_sm * ctx->sm_count;
     if (ctx->persist_cap > MAX_SLOTS) ctx->persist_cap = MAX_SLOTS;
     {
-        const int u = cluster_cap<uint8_t>(ctx->sm_count), f = cluster_cap<float>(ctx->sm_count);
+        const int u = cluster_cap<uint8_t, 1, PERSIST_CS>(ctx->sm_count), f = cluster_cap<float, 1, PERSIST_CS>(ctx->sm_count);
         int cap = u < f ? u : f;
         if (cap > ctx->persist_cap) cap = ctx->persist_cap;
         ctx->persist_cluster_cap = cap - cap % PERSIST_CS;
+    }
+    {
+        const int u = cluster_cap<uint8_t, 2, PAIR_CS[0]>(ctx->sm_count), f = cluster_cap<float, 2, PAIR_CS[0]>(ctx->sm_count);
+        const int cap = u < f ? u : f;
+        ctx->persist_pair_cap[0] = cap - cap % PAIR_CS[0];
+    }
+    {
+        const int u = cluster_cap<uint8_t, 2, PAIR_CS[1]>(ctx->sm_count), f = cluster_cap<float, 2, PAIR_CS[1]>(ctx->sm_count);
+        const int cap = u < f ? u : f;
+        ctx->persist_pair_cap[1] = cap - cap % PAIR_CS[1];
     }
     PCNN_CUDA(cudaMalloc((void **)&ctx->d_slots_ll, (size_t)MAX_SLOTS * NPACK * sizeof(llword)));
     PCNN_CUDA(cudaMalloc((void **)&ctx->d_params_ll, (size_t)NPACK * sizeof(llword)));
@@ -616,12 +671,22 @@ int pcnn_persist_configure(pcnn_ctx *ctx) {
     return PCNN_OK;
 }
 
-// Grid and cluster size of the dataflow kernel for a per-rank batch of B: one image per CTA while the device can hold them,
-// rounded up to whole clusters (CTAs without an image still take part in the reduction); clusters of PERSIST_CS whenever the
-// device can keep that grid co-resident, otherwise single CTAs.
-static void persist_geometry(const pcnn_ctx *ctx, int B, int *grid, int *cs) {
-    const int want = B < ctx->persist_cap ? B : ctx->persist_cap;
+// Grid, cluster size and images per CTA of the dataflow kernel for a per-rank batch of B.  When the batch outnumbers the
+// SMs, single-image CTAs would share SMs and do their once-per-step work (parameter fetch, gradient pushes, cluster slot,
+// barriers) twice per SM: then one two-image CTA per SM, ceil(B / 2) of them rounded up to whole clusters, in the first of
+// the PAIR_CS cluster sizes at which the device keeps that grid co-resident.  Otherwise one image per CTA while the device can hold them, rounded up to whole clusters
+// (CTAs without an image still take part in the reduction); clusters of PERSIST_CS whenever the device can keep that grid
+// co-resident, otherwise single CTAs.
+static void persist_geometry(const pcnn_ctx *ctx, int B, int *grid, int *cs, int *ipc) {
     const int capc = ctx->persist_force_cluster == 1 ? 0 : ctx->persist_cluster_cap;
+    *ipc = 1;
+    if (B > ctx->sm_count && ctx->persist_force_cluster != 1) {
+        for (int k = 0; k < 2; ++k) {
+            const int g = ((B + 1) / 2 + PAIR_CS[k] - 1) / PAIR_CS[k] * PAIR_CS[k];
+            if (g <= ctx->persist_pair_cap[k]) { *grid = g; *cs = PAIR_CS[k]; *ipc = 2; return; }
+        }
+    }
+    const int want = B < ctx->persist_cap ? B : ctx->persist_cap;
     if (capc >= PERSIST_CS) {
         int g = ((want + PERSIST_CS - 1) / PERSIST_CS) * PERSIST_CS;
         if (g > capc) g = capc;
@@ -695,27 +760,22 @@ int pcnn_persist_run(pcnn_ctx *ctx, const pcnn_split_binding &s, int B, long nst
             a.done_tag = done_tag;
         }
         void *args[] = {&a};
-        const size_t smem = s.pixel_type == PCNN_U8 ? sizeof(FusedSmem<uint8_t>) : sizeof(FusedSmem<float>);
         cudaError_t e;
         {
-            int grid = 0, cs = 1;
-            persist_geometry(ctx, B, &grid, &cs);
+            int grid = 0, cs = 1, ipc = 1;
+            persist_geometry(ctx, B, &grid, &cs, &ipc);
             // 2 GPUs: the cluster shares go straight into the peer's memory and the owners gather ranks x clusters slots (one
             // NVLink hop replaces an L2 hop + the separate exchange).  With more GPUs the per-step NVLink volume of that scheme
             // ((N - 1) x 0.6 MB per GPU) grows and the owners exchange their 9.4 KB of sums instead (PCNN_DIRECT_MAX_WORLD)
             a.direct = (ctx->world >= 2 && ctx->world <= PCNN_DIRECT_MAX_WORLD && cs > 1 && grid / cs <= XS_MAXC && grid > 16 &&
                         !ctx->persist_no_direct) ? 1 : 0;
-            const void *fn;
-            if (cs > 1 && a.direct)
-                fn = s.pixel_type == PCNN_U8 ? (const void *)k_train_persist<uint8_t, PERSIST_CS, true> : (const void *)k_train_persist<float, PERSIST_CS, true>;
-            else if (cs > 1)
-                fn = s.pixel_type == PCNN_U8 ? (const void *)k_train_persist<uint8_t, PERSIST_CS, false> : (const void *)k_train_persist<float, PERSIST_CS, false>;
-            else
-                fn = s.pixel_type == PCNN_U8 ? (const void *)k_train_persist<uint8_t, 1, false> : (const void *)k_train_persist<float, 1, false>;
+            const bool u8 = s.pixel_type == PCNN_U8;
+            const void *fn = u8 ? persist_fn<uint8_t>(cs, a.direct != 0, ipc) : persist_fn<float>(cs, a.direct != 0, ipc);
             cudaLaunchConfig_t cfg = {};
             cfg.gridDim = dim3((unsigned)grid);
-            cfg.blockDim = dim3(NT);
-            cfg.dynamicSmemBytes = smem;
+            cfg.blockDim = dim3((unsigned)(NT * ipc));
+            cfg.dynamicSmemBytes = ipc == 2 ? (u8 ? persist_smem_bytes<uint8_t, 2>() : persist_smem_bytes<float, 2>())
+                                            : (u8 ? persist_smem_bytes<uint8_t, 1>() : persist_smem_bytes<float, 1>());
             cfg.stream = ctx->stream;
             cudaLaunchAttribute at[2];
             int na = 0;
@@ -748,6 +808,7 @@ int pcnn_persist_run(pcnn_ctx *ctx, const pcnn_split_binding &s, int B, long nst
             ctx->persist_last_cluster = cs;
             ctx->persist_last_grid = grid;
             ctx->persist_last_direct = a.direct;
+            ctx->persist_last_ipc = ipc;
         }
         if (e != cudaSuccess) return pcnn_fail_cuda(e, "launch of k_train_persist", __FILE__, __LINE__);
         ctx->launches += 1;
@@ -875,7 +936,7 @@ extern "C" int pcnn_persist_info(pcnn_ctx *ctx, int *out6) {
     out6[2] = ctx->persist_cap;
     out6[3] = ctx->persist_cluster_cap;
     out6[4] = PERSIST_CS;
-    out6[5] = (ctx->persist_no_coop ? 0 : 1) | (ctx->persist_last_direct ? 2 : 0);
+    out6[5] = (ctx->persist_no_coop ? 0 : 1) | (ctx->persist_last_direct ? 2 : 0) | (ctx->persist_last_ipc == 2 ? 4 : 0);
     return PCNN_OK;
 }
 

@@ -341,7 +341,8 @@ class Engine:
         out = np.zeros(6, np.int32)
         self._call("pcnn_persist_info", out.ctypes.data)
         return {"grid": int(out[0]), "cluster": int(out[1]), "cta_capacity": int(out[2]), "cta_capacity_clustered": int(out[3]),
-                "cluster_size_used_when_possible": int(out[4]), "cooperative": bool(out[5] & 1), "direct_exchange": bool(out[5] & 2)}
+                "cluster_size_used_when_possible": int(out[4]), "cooperative": bool(out[5] & 1), "direct_exchange": bool(out[5] & 2),
+                "images_per_cta": 2 if out[5] & 4 else 1}
 
     def persist_tune(self, max_cluster=0):
         self._call("pcnn_persist_tune", int(max_cluster))
