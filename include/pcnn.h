@@ -320,6 +320,35 @@ int pcnn_conv_wide_dgrad(pcnn_ctx *ctx, const void *dy_bf16_dev, const float *fi
  *           range (the fewest; the forward's Pt x Qt blocks), stages, work units (row-block pairs x ranges);
  *           input gradient: Pt, Qt of its pixel block of one phase's grid, channel groups, stages, tiles } */
 int pcnn_conv_wide_bwd_info(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows, int *out10);
+/* The same five with a symmetric zero padding of pad_h rows and pad_w columns, as torch.nn.functional.conv2d(padding=(pad_h, pad_w)):
+ * with x~ = x inside the H x W image and 0 outside it,
+ *     P = (H + 2 pad_h - R) / stride + 1,   Q = (W + 2 pad_w - S) / stride + 1
+ *     y[n][p][q][k]  = b[k] + sum_{r,s,c} x~[n][p*stride + r - pad_h][q*stride + s - pad_w][c] * f[k][r][s][c]   (then sigmoid if act)
+ *     dw[k][r][s][c] = sum_{n,p,q} dy[n][p][q][k] * x~[n][p*stride + r - pad_h][q*stride + s - pad_w][c]
+ *     dx[n][h][w][c] = sum_{k,r,s} dy[n][(h + pad_h - r)/stride][(w + pad_w - s)/stride][k] * f[k][r][s][c]
+ *                      over the (r, s) that divide exactly and give a dy pixel inside P x Q:
+ * exactly pcnn_pad_nhwc_bf16 into a zeroed canvas followed by the unpadded pass, with dx cropped from the canvas's gradient, but
+ * with no canvas: the kernels read x and dy at shifted box coordinates and TMA zero-fills what lies outside.  dy is dense
+ * [N][P][Q][K]; out8 / out10 and every other part of the contract are the unpadded calls' (every element of dx's H x W x C image
+ * is written, its pad never; the pad columns and rows of x's layout are not the zero padding and are never read, NaN included;
+ * reruns are bit-identical).  The domain is the unpadded one with, in addition,
+ *   - 0 <= pad_h <= R - 1 and 0 <= pad_w <= S - 1 ("same" is R/2, "full" is R - 1);
+ *   - H + 2 pad_h >= R and W + 2 pad_w >= S in place of H >= R and W >= S;
+ *   - H >= stride if pad_h > 0 and W >= stride if pad_w > 0 (every phase of x must have a row / pixel inside the image).
+ * At padding (0, 0) each is exactly its unpadded call, refusals included (a shape the row-Toeplitz plan takes is refused).
+ * A padded shape is never refused for that: the row-Toeplitz plan has no padding, so no shape has two forward kernels.
+ * Refusals name the called function (pcnn_conv_wide_plan_create_padded for both forward calls). */
+int pcnn_conv_wide_plan_create_padded(pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w,
+                                      int row_pitch, int image_rows, int act, const float *filt_host, const float *bias_host,
+                                      pcnn_conv_plan **plan_out);
+int pcnn_conv_wide_plan_info_padded(int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch,
+                                    int image_rows, int *out8);
+int pcnn_conv_wide_wgrad_padded(pcnn_ctx *ctx, const void *x_bf16_dev, const void *dy_bf16_dev, float *dw_f32_dev, int N, int H, int W,
+                                int C, int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch, int image_rows);
+int pcnn_conv_wide_dgrad_padded(pcnn_ctx *ctx, const void *dy_bf16_dev, const float *filt_f32_dev, void *dx_bf16_dev, int N, int H,
+                                int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch, int image_rows);
+int pcnn_conv_wide_bwd_info_padded(int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch,
+                                   int image_rows, int *out10);
 /* Backward passes of the same convolution (bf16 operands, fp32 accumulation, deterministic; wgmma kernels, see
  * pcnn_conv_bwd_select): weight gradient fp32 KRSC [ref: layer.h:371-395 bp_weight_c1, without its /576] and input gradient
  * bf16 NHWC in x's layout.  row_pitch / image_rows as for the forward plan (0 = dense). */
@@ -358,7 +387,8 @@ int pcnn_conv_bwd_plan_info_strided(int N, int H, int W, int C, int K, int R, in
 /* Zero padding for the valid-padding kernels above (SURVEY.md 8f row 4): pcnn_pad_nhwc_bf16 embeds dense [N][H][W][C] images into
  * a zeroed canvas [N][dst_image_rows][dst_row_pitch] at row offset pad_h, pixel offset pad_w (0 = the tight canvas
  * [H + 2 pad_h][(W + 2 pad_w) * C]); a "same" convolution is pad -> pcnn_conv_tc_fwd, its input gradient is
- * pcnn_conv_dgrad into a padded canvas -> pcnn_crop_nhwc_bf16, its weight gradient is pcnn_conv_wgrad on the padded x. */
+ * pcnn_conv_dgrad into a padded canvas -> pcnn_crop_nhwc_bf16, its weight gradient is pcnn_conv_wgrad on the padded x.  The wide
+ * family pads without a canvas: pcnn_conv_wide_plan_create_padded / pcnn_conv_wide_wgrad_padded / pcnn_conv_wide_dgrad_padded. */
 int pcnn_pad_nhwc_bf16(pcnn_ctx *ctx, const void *src_bf16_dev, void *dst_bf16_dev, int N, int H, int W, int C, int pad_h, int pad_w,
                        int dst_row_pitch, int dst_image_rows);
 int pcnn_crop_nhwc_bf16(pcnn_ctx *ctx, const void *src_bf16_dev, void *dst_bf16_dev, int N, int H, int W, int C, int pad_h, int pad_w,

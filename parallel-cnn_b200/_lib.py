@@ -121,6 +121,11 @@ _SIG = {
     "pcnn_conv_wide_wgrad": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
     "pcnn_conv_wide_dgrad": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
     "pcnn_conv_wide_bwd_info": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
+    "pcnn_conv_wide_plan_create_padded": [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _pvp],
+    "pcnn_conv_wide_plan_info_padded": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
+    "pcnn_conv_wide_wgrad_padded": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
+    "pcnn_conv_wide_dgrad_padded": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
+    "pcnn_conv_wide_bwd_info_padded": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_f32_to_bf16_rows": [_vp, _vp, _vp, _l, _i, _i],
     "pcnn_conv_bwd_plan_info": [_i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_pad_nhwc_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i],
@@ -180,23 +185,35 @@ def conv_tc_plan_info(N, H, W, C, K, R, S, stride=1, row_pitch=None, image_rows=
     return dict(Qt=out[0], V=out[1], stages=out[2], n_mtiles=out[3], n_qtiles=out[4], tiles=out[3] * out[4])
 
 
-def conv_wide_plan_info(N, H, W, C, K, R, S, stride=1, row_pitch=None, image_rows=0):
-    """How the wide-channel forward plan tiles a shape (pcnn_conv_wide_plan_info; host only, no GPU).  row_pitch None = W*C
-    rounded up to 8 elements, as WideConvPlan.  issued_pixels / useful_pixels: output pixels the tiles cover / compute."""
+def conv_wide_plan_info(N, H, W, C, K, R, S, stride=1, row_pitch=None, image_rows=0, padding=(0, 0)):
+    """How the wide-channel forward plan tiles a shape (pcnn_conv_wide_plan_info, or pcnn_conv_wide_plan_info_padded for a
+    padding (pad_h, pad_w) other than (0, 0); host only, no GPU).  row_pitch None = W*C rounded up to 8 elements, as
+    WideConvPlan.  issued_pixels / useful_pixels: output pixels the tiles cover / compute."""
     pitch = (W * C + 7) // 8 * 8 if row_pitch is None else row_pitch
+    ph, pw = (int(v) for v in padding)
     out = (_i * 8)()
-    check("pcnn_conv_wide_plan_info", lib().pcnn_conv_wide_plan_info(N, H, W, C, K, R, S, int(stride), int(pitch), int(image_rows), out))
-    P, Q = (H - R) // stride + 1, (W - S) // stride + 1
+    if (ph, pw) == (0, 0):
+        check("pcnn_conv_wide_plan_info", lib().pcnn_conv_wide_plan_info(N, H, W, C, K, R, S, int(stride), int(pitch), int(image_rows), out))
+    else:
+        check("pcnn_conv_wide_plan_info_padded",
+              lib().pcnn_conv_wide_plan_info_padded(N, H, W, C, K, R, S, int(stride), ph, pw, int(pitch), int(image_rows), out))
+    P, Q = (H + 2 * ph - R) // stride + 1, (W + 2 * pw - S) // stride + 1
     return dict(Pt=out[0], Qt=out[1], chunks=out[2], stages=out[3], tiles=out[4], n_pb=out[5], n_qb=out[6], npad=out[7],
                 issued_pixels=out[4] * out[0] * out[1], useful_pixels=N * P * Q)
 
 
-def conv_wide_bwd_info(N, H, W, C, K, R, S, stride=1, row_pitch=None, image_rows=0):
-    """How the wide-channel gradients tile a shape (pcnn_conv_wide_bwd_info; host only, no GPU).  row_pitch None = W*C rounded
-    up to 8 elements, as WideConvPlan.  wgrad_units = row-block pairs x pixel ranges; wgrad_blocks_per_split is the fewest."""
+def conv_wide_bwd_info(N, H, W, C, K, R, S, stride=1, row_pitch=None, image_rows=0, padding=(0, 0)):
+    """How the wide-channel gradients tile a shape (pcnn_conv_wide_bwd_info, or pcnn_conv_wide_bwd_info_padded for a padding
+    (pad_h, pad_w) other than (0, 0); host only, no GPU).  row_pitch None = W*C rounded up to 8 elements, as WideConvPlan.
+    wgrad_units = row-block pairs x pixel ranges; wgrad_blocks_per_split is the fewest."""
     pitch = (W * C + 7) // 8 * 8 if row_pitch is None else row_pitch
+    ph, pw = (int(v) for v in padding)
     out = (_i * 10)()
-    check("pcnn_conv_wide_bwd_info", lib().pcnn_conv_wide_bwd_info(N, H, W, C, K, R, S, int(stride), int(pitch), int(image_rows), out))
+    if (ph, pw) == (0, 0):
+        check("pcnn_conv_wide_bwd_info", lib().pcnn_conv_wide_bwd_info(N, H, W, C, K, R, S, int(stride), int(pitch), int(image_rows), out))
+    else:
+        check("pcnn_conv_wide_bwd_info_padded",
+              lib().pcnn_conv_wide_bwd_info_padded(N, H, W, C, K, R, S, int(stride), ph, pw, int(pitch), int(image_rows), out))
     return dict(wgrad_row_blocks=out[0], wgrad_splits=out[1], wgrad_blocks_per_split=out[2], wgrad_stages=out[3], wgrad_units=out[4],
                 dgrad_Pt=out[5], dgrad_Qt=out[6], dgrad_groups=out[7], dgrad_stages=out[8], dgrad_tiles=out[9])
 

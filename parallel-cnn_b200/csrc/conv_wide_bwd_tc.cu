@@ -27,6 +27,11 @@
 //     stores clip there, so pad and the other phases are never written; rows and columns no window covers come out as
 //     written zeros.  A phase without taps (st > R or st > S) writes its tiles from accumulators zeroed explicitly.
 //
+// Zero padding (the _padded entry points) changes box coordinates only.  Weight gradient: x through the forward's per-tap phase
+// and offset (ConvWideTaps).  Input gradient: the tiles and dx maps stay those of the unpadded phases (a, b) of dx; with
+// a + pad_h = st * off_h + rho_h, phase a takes the taps r = rho_h + st*i (none when rho_h >= R) and reads dy at row u - i + off_h,
+// columns the same with pad_w.  At pad 0, rho_h = a and off_h = 0.
+//
 // Warp roles (288 threads, 1 CTA/SM, persistent): warps 0-7 = two consumer warpgroups, warp 8 = TMA producer.
 #include "tc_common.cuh"
 
@@ -62,6 +67,7 @@ struct WideWgradParams {
     int blocks, splits, units;       // pixel blocks N*n_pb*n_qb, pixel ranges, pairs * splits
     int stages;
     float *slots;                    // [splits][K][R][S][C]
+    ConvWideTaps taps;               // the forward's x phase and box offset of every tap row / column
 };
 
 struct WideWgradMaps {
@@ -107,8 +113,8 @@ k_conv_wide_wgrad(const __grid_constant__ WideWgradMaps m, const WideWgradParams
                     bar_expect_tx(&S.full[stage], (unsigned)((nx + NB) * WB_BOX_BYTES));
                     for (int w = 0; w < nx; ++w) {
                         const int rb = 2 * pair + w, t = rb / p.nch, ch = rb % p.nch, r = t / p.S, s = t % p.S;
-                        tma_load_4d(sp + w * WB_BOX_BYTES, &m.x[(r % st) * st + s % st], ch * WB_KC, q0 + s / st, p0 + r / st, n,
-                                    &S.full[stage]);
+                        tma_load_4d(sp + w * WB_BOX_BYTES, &m.x[p.taps.rph[r] * st + p.taps.sph[s]], ch * WB_KC, q0 + p.taps.soff[s],
+                                    p0 + p.taps.roff[r], n, &S.full[stage]);
                     }
                     for (int g = 0; g < NB; ++g)
                         tma_load_4d(sp + (2 + g) * WB_BOX_BYTES, &m.dy, g * 64, q0, p0, n, &S.full[stage]);
@@ -169,6 +175,8 @@ struct WideDgradParams {
     int tile0[17];                   // first tile of phase a * st + b; tile0[st * st] = all tiles
     int n_ub[16], n_vb[16];          // pixel blocks down / along the phase's grid
     int Ri[16], Sj[16];              // taps of the phase in each direction
+    int rho_h[4], off_h[4];          // row phase a: taps r = rho_h[a] + st*i, dy row u - i + off_h[a] (a + pad_h = st*off_h + rho_h)
+    int rho_w[4], off_w[4];          // column phase b: the same with pad_w
 };
 
 struct WideDgradMaps {
@@ -222,13 +230,14 @@ k_conv_wide_dgrad(const __grid_constant__ WideDgradMaps m, const WideDgradParams
                 const int a = d.ph / st, b = d.ph % st;
                 for (int i = 0; i < p.Ri[d.ph]; ++i)
                     for (int j = 0; j < p.Sj[d.ph]; ++j) {
-                        const int t = (a + st * i) * p.S + b + st * j;
+                        const int t = (p.rho_h[a] + st * i) * p.S + p.rho_w[b] + st * j;
+                        const int bv = d.v0 - j + p.off_w[b], bu = d.u0 - i + p.off_h[a];
                         for (int kc = 0; kc < p.nkc; ++kc, ++it) {
                             const int stage = it % NST;
                             bar_wait_relaxed(&S.empty[stage], ((unsigned)(it / NST) & 1u) ^ 1u, 32);
                             unsigned char *sa = ring + (size_t)stage * (A_BYTES + B_BYTES);
                             bar_expect_tx(&S.full[stage], (unsigned)(A_BYTES + B_BYTES));
-                            tma_load_4d(sa, &m.dy, kc * WB_KC, d.v0 - j, d.u0 - i, d.n, &S.full[stage]);
+                            tma_load_4d(sa, &m.dy, kc * WB_KC, bv, bu, d.n, &S.full[stage]);
                             tma_load_3d(sa + A_BYTES, &m.f, kc * WB_KC, d.g * p.G, t, &S.full[stage]);
                         }
                     }
@@ -323,14 +332,16 @@ struct WideBwdPlan {
     int dn, d_tiles;                  // input-gradient accumulator columns, tiles
 };
 
-int wide_bwd_plan(const char *fn, int N, int H, int W, int C, int K, int R, int S, int st, int row_pitch, int image_rows, WideBwdPlan *pl) {
+int wide_bwd_plan(const char *fn, int N, int H, int W, int C, int K, int R, int S, int st, int pad_h, int pad_w, int row_pitch,
+                  int image_rows, WideBwdPlan *pl) {
     memset(pl, 0, sizeof(*pl));
-    int rc = conv_wide_shape(fn, N, H, W, C, K, R, S, st, row_pitch, image_rows, &pl->sh);
+    int rc = conv_wide_shape(fn, N, H, W, C, K, R, S, st, pad_h, pad_w, row_pitch, image_rows, &pl->sh);
     if (rc) return rc;
     const ConvWideShape &sh = pl->sh;
     WideWgradParams &w = pl->w;
     w.Pt = sh.Pt; w.Qt = sh.Qt; w.n_pb = sh.n_pb; w.n_qb = sh.n_qb;
     w.R = R; w.S = S; w.stride = st; w.nch = sh.nch; w.C = C; w.K = K;
+    w.taps = sh.taps;
     w.rows = R * S * sh.nch;
     w.pairs = (w.rows + 1) / 2;
     w.blocks = sh.tiles;
@@ -349,6 +360,10 @@ int wide_bwd_plan(const char *fn, int N, int H, int W, int C, int K, int R, int 
     d.G = d.ngroups == 1 ? C : ((C + d.ngroups - 1) / d.ngroups + 63) / 64 * 64;
     pl->dn = (d.G + 15) / 16 * 16;
     conv_wide_pixel_block((H + st - 1) / st, (W + st - 1) / st, &d.Pt, &d.Qt);    // phase (0, 0) has the largest grid
+    for (int a = 0; a < st; ++a) {
+        d.rho_h[a] = (a + pad_h) % st; d.off_h[a] = (a + pad_h) / st;
+        d.rho_w[a] = (a + pad_w) % st; d.off_w[a] = (a + pad_w) / st;
+    }
     long long tiles = 0;
     for (int a = 0; a < st; ++a)
         for (int b = 0; b < st; ++b) {
@@ -356,8 +371,8 @@ int wide_bwd_plan(const char *fn, int N, int H, int W, int C, int K, int R, int 
             d.tile0[ph] = (int)tiles;
             d.n_ub[ph] = U > 0 ? (U + d.Pt - 1) / d.Pt : 0;
             d.n_vb[ph] = V > 0 ? (V + d.Qt - 1) / d.Qt : 0;
-            d.Ri[ph] = R > a ? (R - a + st - 1) / st : 0;
-            d.Sj[ph] = S > b ? (S - b + st - 1) / st : 0;
+            d.Ri[ph] = R > d.rho_h[a] ? (R - d.rho_h[a] + st - 1) / st : 0;
+            d.Sj[ph] = S > d.rho_w[b] ? (S - d.rho_w[b] + st - 1) / st : 0;
             tiles += (long long)N * d.n_ub[ph] * d.n_vb[ph] * d.ngroups;
             PCNN_REQUIRE(tiles < (1LL << 31), PCNN_ERR_ARG, "%s: %lld input-gradient tiles exceed the int range", fn, tiles);
         }
@@ -403,25 +418,27 @@ int configure(pcnn_ctx *ctx) {
 
 }  // namespace
 
-extern "C" int pcnn_conv_wide_bwd_info(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows,
-                                       int *out10) {
-    PCNN_REQUIRE(out10, PCNN_ERR_ARG, "pcnn_conv_wide_bwd_info: NULL argument");
+// The three passes below are each entry point's body, with its name for the messages; the unpadded entry points run them at
+// padding (0, 0).
+static int wide_bwd_info(const char *fn, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w,
+                         int row_pitch, int image_rows, int *out10) {
+    PCNN_REQUIRE(out10, PCNN_ERR_ARG, "%s: NULL argument", fn);
     WideBwdPlan pl;
-    int rc = wide_bwd_plan("pcnn_conv_wide_bwd_info", N, H, W, C, K, R, S, stride, row_pitch, image_rows, &pl);
+    int rc = wide_bwd_plan(fn, N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows, &pl);
     if (rc) return rc;
     out10[0] = pl.w.rows; out10[1] = pl.w.splits; out10[2] = pl.w.blocks / pl.w.splits; out10[3] = pl.w.stages; out10[4] = pl.w.units;
     out10[5] = pl.d.Pt; out10[6] = pl.d.Qt; out10[7] = pl.d.ngroups; out10[8] = pl.d.stages; out10[9] = pl.d_tiles;
     return PCNN_OK;
 }
 
-extern "C" int pcnn_conv_wide_wgrad(pcnn_ctx *ctx, const void *x_bf16, const void *dy_bf16, float *dw_f32, int N, int H, int W, int C,
-                                    int K, int R, int S, int stride, int row_pitch, int image_rows) {
-    PCNN_REQUIRE(ctx && x_bf16 && dy_bf16 && dw_f32, PCNN_ERR_ARG, "pcnn_conv_wide_wgrad: NULL argument");
+static int wide_wgrad(const char *fn, pcnn_ctx *ctx, const void *x_bf16, const void *dy_bf16, float *dw_f32, int N, int H, int W, int C,
+                      int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch, int image_rows) {
+    PCNN_REQUIRE(ctx && x_bf16 && dy_bf16 && dw_f32, PCNN_ERR_ARG, "%s: NULL argument", fn);
     WideBwdPlan pl;
-    int rc = wide_bwd_plan("pcnn_conv_wide_wgrad", N, H, W, C, K, R, S, stride, row_pitch, image_rows, &pl);
+    int rc = wide_bwd_plan(fn, N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows, &pl);
     if (rc) return rc;
     PCNN_REQUIRE(((uintptr_t)x_bf16 & 15) == 0 && ((uintptr_t)dy_bf16 & 15) == 0, PCNN_ERR_ARG,
-                 "pcnn_conv_wide_wgrad: x and dy must be 16-byte aligned (TMA)");
+                 "%s: x and dy must be 16-byte aligned (TMA)", fn);
     pcnn_device_guard g(ctx->device);
     if ((rc = configure(ctx))) return rc;
     WideWgradParams p = pl.w;
@@ -429,7 +446,8 @@ extern "C" int pcnn_conv_wide_wgrad(pcnn_ctx *ctx, const void *x_bf16, const voi
     if ((rc = pcnn_scratch(ctx, (size_t)p.splits * nout * sizeof(float), (void **)&p.slots))) return rc;
     WideWgradMaps m;
     memset(&m, 0, sizeof(m));
-    if ((rc = conv_wide_x_maps(m.x, x_bf16, N, H, W, C, R, S, stride, row_pitch, image_rows > 0 ? image_rows : H, p.Pt, p.Qt))) return rc;
+    if ((rc = conv_wide_x_maps(m.x, x_bf16, N, H, W, C, R, S, stride, p.taps, row_pitch, image_rows > 0 ? image_rows : H, p.Pt, p.Qt)))
+        return rc;
     if ((rc = dense_dy_map(&m.dy, dy_bf16, N, pl.sh.P, pl.sh.Q, K, p.Pt, p.Qt))) return rc;
     const int grid = p.units < ctx->sm_count ? p.units : ctx->sm_count;
     void *args[] = {&m, &p};
@@ -439,14 +457,14 @@ extern "C" int pcnn_conv_wide_wgrad(pcnn_ctx *ctx, const void *x_bf16, const voi
     return pcnn_conv_wgrad_reduce_slots(ctx, p.slots, dw_f32, p.splits, nout);
 }
 
-extern "C" int pcnn_conv_wide_dgrad(pcnn_ctx *ctx, const void *dy_bf16, const float *filt_f32_dev, void *dx_bf16, int N, int H, int W,
-                                    int C, int K, int R, int S, int stride, int row_pitch, int image_rows) {
-    PCNN_REQUIRE(ctx && dy_bf16 && filt_f32_dev && dx_bf16, PCNN_ERR_ARG, "pcnn_conv_wide_dgrad: NULL argument");
+static int wide_dgrad(const char *fn, pcnn_ctx *ctx, const void *dy_bf16, const float *filt_f32_dev, void *dx_bf16, int N, int H, int W,
+                      int C, int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch, int image_rows) {
+    PCNN_REQUIRE(ctx && dy_bf16 && filt_f32_dev && dx_bf16, PCNN_ERR_ARG, "%s: NULL argument", fn);
     WideBwdPlan pl;
-    int rc = wide_bwd_plan("pcnn_conv_wide_dgrad", N, H, W, C, K, R, S, stride, row_pitch, image_rows, &pl);
+    int rc = wide_bwd_plan(fn, N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows, &pl);
     if (rc) return rc;
     PCNN_REQUIRE(((uintptr_t)dy_bf16 & 15) == 0 && ((uintptr_t)dx_bf16 & 15) == 0, PCNN_ERR_ARG,
-                 "pcnn_conv_wide_dgrad: dy and dx must be 16-byte aligned (TMA)");
+                 "%s: dy and dx must be 16-byte aligned (TMA)", fn);
     pcnn_device_guard g(ctx->device);
     if ((rc = configure(ctx))) return rc;
     if (image_rows <= 0) image_rows = H;
@@ -488,4 +506,38 @@ extern "C" int pcnn_conv_wide_dgrad(pcnn_ctx *ctx, const void *dy_bf16, const fl
                                dgrad_staging_bytes(pl.dn) + (size_t)pp.stages * dgrad_stage_bytes(pl.dn) + sizeof(WideCtl) + 1024, ctx->stream));
     PCNN_CHECK_LAUNCH(ctx);
     return PCNN_OK;
+}
+
+extern "C" int pcnn_conv_wide_bwd_info(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows,
+                                       int *out10) {
+    return wide_bwd_info("pcnn_conv_wide_bwd_info", N, H, W, C, K, R, S, stride, 0, 0, row_pitch, image_rows, out10);
+}
+
+extern "C" int pcnn_conv_wide_bwd_info_padded(int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w,
+                                              int row_pitch, int image_rows, int *out10) {
+    return wide_bwd_info("pcnn_conv_wide_bwd_info_padded", N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows, out10);
+}
+
+extern "C" int pcnn_conv_wide_wgrad(pcnn_ctx *ctx, const void *x_bf16, const void *dy_bf16, float *dw_f32, int N, int H, int W, int C,
+                                    int K, int R, int S, int stride, int row_pitch, int image_rows) {
+    return wide_wgrad("pcnn_conv_wide_wgrad", ctx, x_bf16, dy_bf16, dw_f32, N, H, W, C, K, R, S, stride, 0, 0, row_pitch, image_rows);
+}
+
+extern "C" int pcnn_conv_wide_wgrad_padded(pcnn_ctx *ctx, const void *x_bf16, const void *dy_bf16, float *dw_f32, int N, int H, int W,
+                                           int C, int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch, int image_rows) {
+    return wide_wgrad("pcnn_conv_wide_wgrad_padded", ctx, x_bf16, dy_bf16, dw_f32, N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch,
+                      image_rows);
+}
+
+extern "C" int pcnn_conv_wide_dgrad(pcnn_ctx *ctx, const void *dy_bf16, const float *filt_f32_dev, void *dx_bf16, int N, int H, int W,
+                                    int C, int K, int R, int S, int stride, int row_pitch, int image_rows) {
+    return wide_dgrad("pcnn_conv_wide_dgrad", ctx, dy_bf16, filt_f32_dev, dx_bf16, N, H, W, C, K, R, S, stride, 0, 0, row_pitch,
+                      image_rows);
+}
+
+extern "C" int pcnn_conv_wide_dgrad_padded(pcnn_ctx *ctx, const void *dy_bf16, const float *filt_f32_dev, void *dx_bf16, int N, int H,
+                                           int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch,
+                                           int image_rows) {
+    return wide_dgrad("pcnn_conv_wide_dgrad_padded", ctx, dy_bf16, filt_f32_dev, dx_bf16, N, H, W, C, K, R, S, stride, pad_h, pad_w,
+                      row_pitch, image_rows);
 }

@@ -19,6 +19,10 @@
 //     drains while the warpgroup already runs the next tile's MMAs; the staging tile is reused once its store has been read.
 // Pixel blocks on small images issue more pixels than they compute: pcnn_conv_wide_plan_info reports both.
 //
+// Zero padding (pcnn_conv_wide_plan_create_padded) moves the box coordinates only: with r - pad_h = st * a_r + rho_r (floor
+// division, 0 <= rho_r < st) tap r reads phase map rho_r at box row p0 + a_r, and columns the same (ConvWideTaps).  A box row
+// or column before the image (a_r < 0) or past it is zero-filled by TMA like the channels >= C; nothing else changes.
+//
 // Warp roles (288 threads, 1 CTA/SM, persistent over tiles): warps 0-7 = two consumer warpgroups, warp 8 = TMA producer.
 #include "tc_common.cuh"
 
@@ -44,10 +48,11 @@ struct ConvWideParams {
     int R, S, stride, nch;       // taps, window step, 64-channel chunks per tap
     int stages, K;
     const float *bias;           // [K] or null
+    ConvWideTaps taps;           // x phase and box offset of every tap row / column
 };
 
 struct ConvWideMaps {
-    CUtensorMap x[16];           // phase (r % st, s % st) at index (r % st) * st + s % st
+    CUtensorMap x[16];           // phase (rph[r], sph[s]) at index rph[r] * st + sph[s]
     CUtensorMap w;               // filters {C, R*S, K}
     CUtensorMap y;               // output {K, Q, P, N}
 };
@@ -94,14 +99,15 @@ k_conv_wide_fwd(const __grid_constant__ ConvWideMaps m, const ConvWideParams p) 
                 const int p0 = (rem / p.n_qb) * p.Pt, q0 = (rem % p.n_qb) * p.Qt;
                 for (int r = 0; r < p.R; ++r)
                     for (int s = 0; s < p.S; ++s) {
-                        const CUtensorMap *mx = &m.x[(r % p.stride) * p.stride + s % p.stride];
+                        const CUtensorMap *mx = &m.x[p.taps.rph[r] * p.stride + p.taps.sph[s]];
+                        const int bq = q0 + p.taps.soff[s], bp = p0 + p.taps.roff[r];
                         for (int ch = 0; ch < p.nch; ++ch, ++it) {
                             const int stage = it % NST;
                             const unsigned ph = (unsigned)(it / NST) & 1u;
                             bar_wait_relaxed(&S.empty[stage], ph ^ 1u, 32);
                             unsigned char *a = ring + (size_t)stage * (WD_A_BYTES + B_BYTES);
                             bar_expect_tx(&S.full[stage], (unsigned)(WD_A_BYTES + B_BYTES));
-                            tma_load_4d(a, mx, ch * WD_KC, q0 + s / p.stride, p0 + r / p.stride, n, &S.full[stage]);
+                            tma_load_4d(a, mx, ch * WD_KC, bq, bp, n, &S.full[stage]);
                             tma_load_3d(a + WD_A_BYTES, &m.w, ch * WD_KC, r * p.S + s, 0, &S.full[stage]);
                         }
                     }
@@ -199,13 +205,34 @@ long long conv_wide_pixel_block(int P, int Q, int *Pt, int *Qt) {
     return best;
 }
 
-int conv_wide_shape(const char *fn, int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows,
-                    ConvWideShape *out) {
+// r - pad = st * off[r] + ph[r], 0 <= ph[r] < st, for the taps r < R (pad <= R - 1 < 7, so r - pad + 8 * st > 0)
+static void wide_tap_table(int R, int pad, int st, int *ph, int *off) {
+    for (int r = 0; r < R; ++r) {
+        const int t = r - pad + 8 * st;
+        ph[r] = t % st;
+        off[r] = t / st - 8;
+    }
+}
+
+int conv_wide_shape(const char *fn, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch,
+                    int image_rows, ConvWideShape *out) {
     PCNN_REQUIRE(stride >= 1 && stride <= 4, PCNN_ERR_ARG, "%s: stride %d outside 1..4", fn, stride);
     PCNN_REQUIRE(R >= 1 && R <= WD_MAX_RS && S >= 1 && S <= WD_MAX_RS, PCNN_ERR_ARG,
                  "%s: R = %d, S = %d: taps must be 1..7 in each direction", fn, R, S);
-    PCNN_REQUIRE(N > 0 && H >= R && W >= S && C > 0 && K > 0, PCNN_ERR_ARG,
-                 "%s: bad shape N=%d H=%d W=%d C=%d K=%d R=%d S=%d", fn, N, H, W, C, K, R, S);
+    PCNN_REQUIRE(pad_h >= 0 && pad_h < R && pad_w >= 0 && pad_w < S, PCNN_ERR_ARG,
+                 "%s: padding (%d, %d) with R = %d, S = %d taps: 0 <= pad_h <= R - 1 and 0 <= pad_w <= S - 1 are required", fn, pad_h,
+                 pad_w, R, S);
+    const bool padded = pad_h > 0 || pad_w > 0;
+    if (!padded)
+        PCNN_REQUIRE(N > 0 && H >= R && W >= S && C > 0 && K > 0, PCNN_ERR_ARG,
+                     "%s: bad shape N=%d H=%d W=%d C=%d K=%d R=%d S=%d", fn, N, H, W, C, K, R, S);
+    else
+        PCNN_REQUIRE(N > 0 && H >= R - 2 * pad_h && W >= S - 2 * pad_w && C > 0 && K > 0, PCNN_ERR_ARG,
+                     "%s: bad shape N=%d H=%d W=%d C=%d K=%d R=%d S=%d padding (%d, %d): H + 2*pad_h >= R and W + 2*pad_w >= S are "
+                     "required", fn, N, H, W, C, K, R, S, pad_h, pad_w);
+    PCNN_REQUIRE((pad_h == 0 || H >= stride) && (pad_w == 0 || W >= stride), PCNN_ERR_ARG,
+                 "%s: H = %d, W = %d with padding (%d, %d) at stride %d: a padded direction needs at least stride rows / pixels, "
+                 "so that every phase of x has one inside the image", fn, H, W, pad_h, pad_w, stride);
     PCNN_REQUIRE(K % 8 == 0 && K <= 256, PCNN_ERR_ARG,
                  "%s: K = %d filters: K %% 8 == 0 and K <= 256 are required", fn, K);
     PCNN_REQUIRE(C % 8 == 0, PCNN_ERR_ARG,
@@ -214,10 +241,10 @@ int conv_wide_shape(const char *fn, int N, int H, int W, int C, int K, int R, in
                  "%s: row pitch %d must be >= W*C and a multiple of 8 elements (TMA 16-byte strides)", fn, row_pitch);
     if (image_rows <= 0) image_rows = H;
     PCNN_REQUIRE(image_rows >= H, PCNN_ERR_ARG, "%s: image pitch of %d rows is smaller than H = %d", fn, image_rows, H);
-    int tc[5];
-    PCNN_REQUIRE(pcnn_conv_tc_plan_info(N, H, W, C, K, R, S, stride, row_pitch, image_rows, tc) != PCNN_OK, PCNN_ERR_ARG,
+    int tc[5];                              // the row-Toeplitz plan has no padding: a padded shape is this plan's alone
+    PCNN_REQUIRE(padded || pcnn_conv_tc_plan_info(N, H, W, C, K, R, S, stride, row_pitch, image_rows, tc) != PCNN_OK, PCNN_ERR_ARG,
                  "%s: this shape is served by the row-Toeplitz forward: use pcnn_conv_tc_plan_create", fn);
-    const int P = (H - R) / stride + 1, Q = (W - S) / stride + 1;
+    const int P = (H + 2 * pad_h - R) / stride + 1, Q = (W + 2 * pad_w - S) / stride + 1;
     const long long best = conv_wide_pixel_block(P, Q, &out->Pt, &out->Qt);
     out->n_pb = (P + out->Pt - 1) / out->Pt;
     out->n_qb = (Q + out->Qt - 1) / out->Qt;
@@ -229,15 +256,23 @@ int conv_wide_shape(const char *fn, int N, int H, int W, int C, int K, int R, in
     int st = (int)(((size_t)WD_SMEM_BUDGET - fixed) / wide_stage_bytes(out->npad));
     out->stages = st > WD_MAX_STAGES ? WD_MAX_STAGES : st;
     out->P = P; out->Q = Q;
+    wide_tap_table(R, pad_h, stride, out->taps.rph, out->taps.roff);
+    wide_tap_table(S, pad_w, stride, out->taps.sph, out->taps.soff);
     return PCNN_OK;
 }
 
 // x phase (rb, sb) of the window step: input rows rb, rb + st, ... and pixels sb, sb + st, ... of every image; the extents end at
-// the image's last row and pixel, so a box never reads pad rows, pad columns or the next image
-int conv_wide_x_maps(CUtensorMap *maps, const void *x_bf16, int N, int H, int W, int C, int R, int S, int st, int row_pitch,
-                     int image_rows, int Pt, int Qt) {
-    for (int rb = 0; rb < st && rb < R; ++rb)
-        for (int sb = 0; sb < st && sb < S; ++sb) {
+// the image's last row and pixel, so a box never reads pad rows, pad columns or the next image.  Only the phases some tap reads
+// are encoded (rb < min(st, R) at pad 0; with padding they need not be a prefix); each has a row and a pixel inside the image
+// (H >= R at pad 0, H >= st when padded, and the same for W).
+int conv_wide_x_maps(CUtensorMap *maps, const void *x_bf16, int N, int H, int W, int C, int R, int S, int st, const ConvWideTaps &taps,
+                     int row_pitch, int image_rows, int Pt, int Qt) {
+    bool row_used[4] = {}, col_used[4] = {};
+    for (int r = 0; r < R; ++r) row_used[taps.rph[r]] = true;
+    for (int s = 0; s < S; ++s) col_used[taps.sph[s]] = true;
+    for (int rb = 0; rb < st; ++rb)
+        for (int sb = 0; sb < st; ++sb) {
+            if (!row_used[rb] || !col_used[sb]) continue;
             const uint64_t dims[4] = {(uint64_t)C, (uint64_t)((W - sb + st - 1) / st), (uint64_t)((H - rb + st - 1) / st), (uint64_t)N};
             const uint64_t str[3] = {(uint64_t)st * C * 2, (uint64_t)st * row_pitch * 2, (uint64_t)image_rows * row_pitch * 2};
             const uint32_t box[4] = {WD_KC, (uint32_t)Qt, (uint32_t)Pt, 1};
@@ -264,24 +299,36 @@ void conv_wide_free(ConvWidePlan *w) {
     delete w;
 }
 
-extern "C" int pcnn_conv_wide_plan_info(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows,
-                                        int *out8) {
-    PCNN_REQUIRE(out8, PCNN_ERR_ARG, "pcnn_conv_wide_plan_info: NULL argument");
+// the query of the create call `fn` (its refusals name that call)
+static int wide_plan_info(const char *fn, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w,
+                          int row_pitch, int image_rows, int *out8) {
     ConvWideShape sh;
-    int rc = conv_wide_shape("pcnn_conv_wide_plan_create", N, H, W, C, K, R, S, stride, row_pitch, image_rows, &sh);
+    int rc = conv_wide_shape(fn, N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows, &sh);
     if (rc) return rc;
     out8[0] = sh.Pt; out8[1] = sh.Qt; out8[2] = sh.nch; out8[3] = sh.stages;
     out8[4] = sh.tiles; out8[5] = sh.n_pb; out8[6] = sh.n_qb; out8[7] = sh.npad;
     return PCNN_OK;
 }
 
-extern "C" int pcnn_conv_wide_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch,
-                                          int image_rows, int act, const float *filt_host, const float *bias_host,
-                                          pcnn_conv_plan **out) {
-    PCNN_REQUIRE(ctx && filt_host && out, PCNN_ERR_ARG, "pcnn_conv_wide_plan_create: NULL argument");
-    PCNN_REQUIRE(act == 0 || act == 1, PCNN_ERR_ARG, "pcnn_conv_wide_plan_create: act %d is not 0 (none) or 1 (sigmoid)", act);
+extern "C" int pcnn_conv_wide_plan_info(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows,
+                                        int *out8) {
+    PCNN_REQUIRE(out8, PCNN_ERR_ARG, "pcnn_conv_wide_plan_info: NULL argument");
+    return wide_plan_info("pcnn_conv_wide_plan_create", N, H, W, C, K, R, S, stride, 0, 0, row_pitch, image_rows, out8);
+}
+
+extern "C" int pcnn_conv_wide_plan_info_padded(int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w,
+                                               int row_pitch, int image_rows, int *out8) {
+    PCNN_REQUIRE(out8, PCNN_ERR_ARG, "pcnn_conv_wide_plan_info_padded: NULL argument");
+    return wide_plan_info("pcnn_conv_wide_plan_create_padded", N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows, out8);
+}
+
+static int wide_plan_create(const char *fn, pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h,
+                            int pad_w, int row_pitch, int image_rows, int act, const float *filt_host, const float *bias_host,
+                            pcnn_conv_plan **out) {
+    PCNN_REQUIRE(ctx && filt_host && out, PCNN_ERR_ARG, "%s: NULL argument", fn);
+    PCNN_REQUIRE(act == 0 || act == 1, PCNN_ERR_ARG, "%s: act %d is not 0 (none) or 1 (sigmoid)", fn, act);
     ConvWideShape sh;
-    int rc = conv_wide_shape("pcnn_conv_wide_plan_create", N, H, W, C, K, R, S, stride, row_pitch, image_rows, &sh);
+    int rc = conv_wide_shape(fn, N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows, &sh);
     if (rc) return rc;
     pcnn_device_guard g(ctx->device);
     struct PlanGuard {                       // frees a half-built plan on every early return below
@@ -295,6 +342,7 @@ extern "C" int pcnn_conv_wide_plan_create(pcnn_ctx *ctx, int N, int H, int W, in
     ConvWideParams &p = pl->p;
     p.Pt = sh.Pt; p.Qt = sh.Qt; p.n_pb = sh.n_pb; p.n_qb = sh.n_qb; p.tiles = sh.tiles;
     p.R = R; p.S = S; p.stride = stride; p.nch = sh.nch; p.stages = sh.stages; p.K = K;
+    p.taps = sh.taps;
     const size_t nf = (size_t)K * R * S * C;
     std::vector<uint16_t> fb(nf);
     for (size_t i = 0; i < nf; ++i) fb[i] = f32_to_bf16_bits(filt_host[i]);
@@ -324,6 +372,20 @@ extern "C" int pcnn_conv_wide_plan_create(pcnn_ctx *ctx, int N, int H, int W, in
     return PCNN_OK;
 }
 
+extern "C" int pcnn_conv_wide_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch,
+                                          int image_rows, int act, const float *filt_host, const float *bias_host,
+                                          pcnn_conv_plan **out) {
+    return wide_plan_create("pcnn_conv_wide_plan_create", ctx, N, H, W, C, K, R, S, stride, 0, 0, row_pitch, image_rows, act, filt_host,
+                            bias_host, out);
+}
+
+extern "C" int pcnn_conv_wide_plan_create_padded(pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h,
+                                                 int pad_w, int row_pitch, int image_rows, int act, const float *filt_host,
+                                                 const float *bias_host, pcnn_conv_plan **out) {
+    return wide_plan_create("pcnn_conv_wide_plan_create_padded", ctx, N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows,
+                            act, filt_host, bias_host, out);
+}
+
 int conv_wide_fwd(pcnn_ctx *ctx, const ConvWidePlan *pl, const void *x_bf16, void *y_bf16) {
     PCNN_REQUIRE(((uintptr_t)y_bf16 & 15) == 0, PCNN_ERR_ARG, "pcnn_conv_tc_fwd: the output must be 16-byte aligned (TMA stores)");
     const ConvWideShape &sh = pl->sh;
@@ -331,7 +393,8 @@ int conv_wide_fwd(pcnn_ctx *ctx, const ConvWidePlan *pl, const void *x_bf16, voi
     ConvWideMaps m;
     memset(&m, 0, sizeof(m));
     m.w = pl->map_w;
-    int rc = conv_wide_x_maps(m.x, x_bf16, pl->N, pl->H, pl->W, C, pl->p.R, pl->p.S, st, pl->row_pitch, pl->image_rows, sh.Pt, sh.Qt);
+    int rc = conv_wide_x_maps(m.x, x_bf16, pl->N, pl->H, pl->W, C, pl->p.R, pl->p.S, st, sh.taps, pl->row_pitch, pl->image_rows, sh.Pt,
+                              sh.Qt);
     if (rc) return rc;
     {
         const uint64_t dims[4] = {(uint64_t)K, (uint64_t)sh.Q, (uint64_t)sh.P, (uint64_t)pl->N};

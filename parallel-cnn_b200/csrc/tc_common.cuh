@@ -286,7 +286,8 @@ static inline uint16_t f32_to_bf16_bits(float f) {   // round to nearest even, a
 
 }  // namespace pcnn_tc
 
-// conv_wide_tc.cu: the maps of x of the wide forward, one per phase (r % st, s % st) at index (r % st) * st + s % st, box
-// {64 channels, Qt, Pt, 1} landing K-major with SWIZZLE_128B; also the x operand of the wide weight gradient
-int conv_wide_x_maps(CUtensorMap *maps, const void *x_bf16, int N, int H, int W, int C, int R, int S, int st, int row_pitch,
-                     int image_rows, int Pt, int Qt);
+// conv_wide_tc.cu: the maps of x of the wide forward, one per phase (rph[r], sph[s]) the taps read, at index
+// rph[r] * st + sph[s], box {64 channels, Qt, Pt, 1} landing K-major with SWIZZLE_128B; also the x operand of the wide weight
+// gradient
+int conv_wide_x_maps(CUtensorMap *maps, const void *x_bf16, int N, int H, int W, int C, int R, int S, int st, const ConvWideTaps &taps,
+                     int row_pitch, int image_rows, int Pt, int Qt);

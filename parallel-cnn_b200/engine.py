@@ -384,17 +384,29 @@ class Engine:
         self._call("pcnn_conv_dgrad_strided", _p(dy_bf16), _p(filt_f32), _p(dx_bf16), N, H, W, Cin, K, R, S, int(stride), int(row_pitch),
                    int(image_rows))
 
-    def conv_wide_wgrad(self, x_bf16, dy_bf16, dw_f32, N, H, W, Cin, K, R, S, row_pitch=None, image_rows=0, stride=1):
-        """weight gradient of WideConvPlan's forward (pcnn_conv_wide_wgrad); row_pitch None = W*Cin rounded up to 8, as the plan"""
+    def conv_wide_wgrad(self, x_bf16, dy_bf16, dw_f32, N, H, W, Cin, K, R, S, row_pitch=None, image_rows=0, stride=1, padding=(0, 0)):
+        """weight gradient of WideConvPlan's forward (pcnn_conv_wide_wgrad, or pcnn_conv_wide_wgrad_padded for a zero padding
+        (pad_h, pad_w) other than (0, 0)); row_pitch None = W*Cin rounded up to 8, as the plan"""
         pitch = (W * Cin + 7) // 8 * 8 if row_pitch is None else row_pitch
-        self._call("pcnn_conv_wide_wgrad", _p(x_bf16), _p(dy_bf16), _p(dw_f32), N, H, W, Cin, K, R, S, int(stride), int(pitch),
-                   int(image_rows))
+        ph, pw = (int(v) for v in padding)
+        if (ph, pw) == (0, 0):
+            self._call("pcnn_conv_wide_wgrad", _p(x_bf16), _p(dy_bf16), _p(dw_f32), N, H, W, Cin, K, R, S, int(stride), int(pitch),
+                       int(image_rows))
+        else:
+            self._call("pcnn_conv_wide_wgrad_padded", _p(x_bf16), _p(dy_bf16), _p(dw_f32), N, H, W, Cin, K, R, S, int(stride), ph, pw,
+                       int(pitch), int(image_rows))
 
-    def conv_wide_dgrad(self, dy_bf16, filt_f32, dx_bf16, N, H, W, Cin, K, R, S, row_pitch=None, image_rows=0, stride=1):
-        """input gradient of WideConvPlan's forward (pcnn_conv_wide_dgrad) into dx in x's layout"""
+    def conv_wide_dgrad(self, dy_bf16, filt_f32, dx_bf16, N, H, W, Cin, K, R, S, row_pitch=None, image_rows=0, stride=1, padding=(0, 0)):
+        """input gradient of WideConvPlan's forward (pcnn_conv_wide_dgrad, or pcnn_conv_wide_dgrad_padded for a zero padding
+        (pad_h, pad_w) other than (0, 0)) into dx in x's layout"""
         pitch = (W * Cin + 7) // 8 * 8 if row_pitch is None else row_pitch
-        self._call("pcnn_conv_wide_dgrad", _p(dy_bf16), _p(filt_f32), _p(dx_bf16), N, H, W, Cin, K, R, S, int(stride), int(pitch),
-                   int(image_rows))
+        ph, pw = (int(v) for v in padding)
+        if (ph, pw) == (0, 0):
+            self._call("pcnn_conv_wide_dgrad", _p(dy_bf16), _p(filt_f32), _p(dx_bf16), N, H, W, Cin, K, R, S, int(stride), int(pitch),
+                       int(image_rows))
+        else:
+            self._call("pcnn_conv_wide_dgrad_padded", _p(dy_bf16), _p(filt_f32), _p(dx_bf16), N, H, W, Cin, K, R, S, int(stride), ph, pw,
+                       int(pitch), int(image_rows))
 
     def pad_nhwc(self, src_bf16, dst_bf16, N, H, W, Cin, pad_h, pad_w, dst_row_pitch=0, dst_image_rows=0):
         self._call("pcnn_pad_nhwc_bf16", _p(src_bf16), _p(dst_bf16), N, H, W, Cin, int(pad_h), int(pad_w), int(dst_row_pitch), int(dst_image_rows))
@@ -440,9 +452,10 @@ class ConvPlan:
 
 class WideConvPlan(ConvPlan):
     """The wide-channel forward (pcnn_conv_wide_plan_create): the shapes ConvPlan refuses, C % 8 == 0, K % 8 == 0, K <= 256.
+    padding=(pad_h, pad_w) other than (0, 0) zero-pads x as conv2d(padding=...) does (pcnn_conv_wide_plan_create_padded).
     Run and closed like ConvPlan."""
 
-    def __init__(self, engine, N, H, W, C, K, R, S, filt, bias=None, act=0, row_pitch=None, image_rows=0, stride=1):
+    def __init__(self, engine, N, H, W, C, K, R, S, filt, bias=None, act=0, row_pitch=None, image_rows=0, stride=1, padding=(0, 0)):
         self.engine = engine
         self.shape = (N, H, W, C, K, R, S)
         self.row_pitch = int(row_pitch if row_pitch is not None else (W * C + 7) // 8 * 8)
@@ -450,11 +463,18 @@ class WideConvPlan(ConvPlan):
         assert filt.size == K * R * S * C
         b = None if bias is None else np.ascontiguousarray(bias, np.float32)
         plan = C_.c_void_p()
-        check("pcnn_conv_wide_plan_create",
-              lib().pcnn_conv_wide_plan_create(engine.ctx, N, H, W, C, K, R, S, int(stride), self.row_pitch, int(image_rows), int(act),
-                                               filt.ctypes.data, None if b is None else b.ctypes.data, C_.byref(plan)))
+        ph, pw = (int(v) for v in padding)
+        if (ph, pw) == (0, 0):
+            check("pcnn_conv_wide_plan_create",
+                  lib().pcnn_conv_wide_plan_create(engine.ctx, N, H, W, C, K, R, S, int(stride), self.row_pitch, int(image_rows), int(act),
+                                                   filt.ctypes.data, None if b is None else b.ctypes.data, C_.byref(plan)))
+        else:
+            check("pcnn_conv_wide_plan_create_padded",
+                  lib().pcnn_conv_wide_plan_create_padded(engine.ctx, N, H, W, C, K, R, S, int(stride), ph, pw, self.row_pitch,
+                                                          int(image_rows), int(act), filt.ctypes.data,
+                                                          None if b is None else b.ctypes.data, C_.byref(plan)))
         self.plan = plan
-        self.out_shape = (N, (H - R) // stride + 1, (W - S) // stride + 1, K)
+        self.out_shape = (N, (H + 2 * ph - R) // stride + 1, (W + 2 * pw - S) // stride + 1, K)
 
 
 def f32_to_bf16_bits(a):

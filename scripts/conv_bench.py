@@ -183,6 +183,80 @@ def run_wide_bwd(name, N, H, W, C, K, R, S, stride, iters):
     del x, dy, dx, xt, dyt
 
 
+def run_wide_same(name, N, H, W, C, K, R, S, stride, pad, iters):
+    """a "same" layer three ways, per pass: the built-in padding of the wide kernels (padding=(pad, pad)); the pad-copy route,
+    each step timed alone (pcnn_pad_nhwc_bf16 into the canvas, the unpadded wide pass on the canvas, and pcnn_crop_nhwc_bf16 for
+    dx); cuDNN with padding=pad on the same bf16 channels-last tensors.  Bound as in run_wide on the unpadded tensors:
+    bytes = N * (H*W*C + P*Q*K) * 2, flops = 2 * N * P*Q*K * R*S*C."""
+    Hc, Wc = H + 2 * pad, W + 2 * pad
+    P, Q = (Hc - R) // stride + 1, (Wc - S) // stride + 1
+    f = rng.uniform(-0.5, 0.5, (K, R, S, C)).astype(np.float32)
+    b = rng.uniform(-0.5, 0.5, K).astype(np.float32)
+    plan = pkg.WideConvPlan(eng, N, H, W, C, K, R, S, f, b, stride=stride, padding=(pad, pad))
+    plan_c = pkg.WideConvPlan(eng, N, Hc, Wc, C, K, R, S, f, b, stride=stride)
+    x = torch.randint(0, 0x3F80, (N, H, W, C), dtype=torch.int16, device="cuda")   # positive bf16 bit patterns < 1.0
+    xc = torch.empty((N, Hc, Wc, C), dtype=torch.int16, device="cuda")
+    y = torch.empty((N, P, Q, K), dtype=torch.int16, device="cuda")
+    dy = torch.randint(0, 0x3F80, (N, P, Q, K), dtype=torch.int16, device="cuda")
+    dy ^= (torch.randint(0, 2, (N, P, Q, K), dtype=torch.int16, device="cuda") << 15)   # random signs
+    fd = torch.from_numpy(f).to("cuda")
+    dw = torch.empty((K, R, S, C), dtype=torch.float32, device="cuda")
+    dx = torch.empty((N, H, W, C), dtype=torch.int16, device="cuda")
+    dxc = torch.empty((N, Hc, Wc, C), dtype=torch.int16, device="cuda")
+    xt, dyt = x.view(torch.bfloat16).permute(0, 3, 1, 2), dy.view(torch.bfloat16).permute(0, 3, 1, 2)   # channels-last views
+    wt = fd.permute(0, 3, 1, 2).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+    bt = torch.from_numpy(b).to("cuda", torch.bfloat16)
+    alg = N * (H * W * C + P * Q * K) * 2
+    flops = 2.0 * N * P * Q * K * R * S * C
+    t_bound = max(flops / 989e12, alg / 3.35e12)
+    gpu, power = card()
+
+    def timeit(fn):
+        for _ in range(5):
+            fn()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        for _ in range(iters):
+            fn()
+        e1.record(stream)
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / iters
+
+    def cudnn_bwd(mask):
+        return torch.ops.aten.convolution_backward(dyt, xt, wt, None, [stride, stride], [pad, pad], [1, 1], False, [0, 0], 1, mask)
+
+    pad_ms = timeit(lambda: eng.pad_nhwc(x, xc, N, H, W, C, pad, pad))
+    crop_ms = timeit(lambda: eng.crop_nhwc(dxc, dx, N, H, W, C, pad, pad))
+    passes = (
+        ("fwd", lambda: plan.fwd(x, y), [("pad", pad_ms), ("valid", timeit(lambda: plan_c.fwd(xc, y)))],
+         lambda: torch.nn.functional.conv2d(xt, wt, bt, stride=stride, padding=pad)),
+        ("wgrad", lambda: eng.conv_wide_wgrad(x, dy, dw, N, H, W, C, K, R, S, stride=stride, padding=(pad, pad)),
+         [("pad", pad_ms), ("valid", timeit(lambda: eng.conv_wide_wgrad(xc, dy, dw, N, Hc, Wc, C, K, R, S, stride=stride)))],
+         lambda: cudnn_bwd([False, True, False])),
+        ("dgrad", lambda: eng.conv_wide_dgrad(dy, fd, dx, N, H, W, C, K, R, S, stride=stride, padding=(pad, pad)),
+         [("valid", timeit(lambda: eng.conv_wide_dgrad(dy, fd, dxc, N, Hc, Wc, C, K, R, S, stride=stride))), ("crop", crop_ms)],
+         lambda: cudnn_bwd([True, False, False])),
+    )
+    for what, fn, route, cudnn in passes:
+        ms = timeit(fn)
+        ms_cudnn = timeit(cudnn)
+        route_ms = sum(t for _, t in route)
+        print(json.dumps({"case": f"{name} {what}", "N": N, "ms": ms, "bound": "tensor" if flops / 989e12 >= alg / 3.35e12 else "hbm",
+                          "bound_frac": t_bound / (ms * 1e-3), "route_ms": {k: t for k, t in route}, "route_total_ms": route_ms,
+                          "route_over_builtin": route_ms / ms, "canvas_valid_over_builtin": dict(route)["valid"] / ms,
+                          "cudnn_ms": ms_cudnn, "cudnn_bound_frac": t_bound / (ms_cudnn * 1e-3), "gpu": gpu, "power_limit": power}),
+              flush=True)
+    plan.close()
+    plan_c.close()
+    del x, xc, y, dy, dx, dxc, xt, dyt
+
+
+if only == "widesame":                                                 # "same" layers: built-in padding, pad-copy route, cuDNN
+    run_wide_same("56x56x64->64 3x3 pad 1", 128, 56, 56, 64, 64, 3, 3, 1, 1, 20)
+    run_wide_same("28x28x128->128 3x3 pad 1", 128, 28, 28, 128, 128, 3, 3, 1, 1, 20)
+    run_wide_same("14x14x256->256 3x3 pad 1", 128, 14, 14, 256, 256, 3, 3, 1, 1, 20)
+    run_wide_same("56x56x64->128 3x3 stride 2 pad 1", 128, 56, 56, 64, 128, 3, 3, 2, 1, 20)
 if only == "wide":                                                     # wide channel counts (WideConvPlan), cuDNN beside them
     run_wide("56x56x64->64 3x3", 128, 56, 56, 64, 64, 3, 3, 1, 20)
     run_wide("28x28x128->128 3x3", 128, 28, 28, 128, 128, 3, 3, 1, 20)
