@@ -225,6 +225,8 @@ int pcnn_set_step_mode(pcnn_ctx *ctx, int mode);
  * kernel-replay profilers; CUDA_LAUNCH_BLOCKING=1 is detected by itself); bit 3 keeps the two-stage gradient exchange on 2
  * GPUs (default there: cluster shares stored straight into the peer's memory); bit 4 sends pinned host images of
  * pcnn_learn_host through the staged copy stream instead of letting the kernel pull them.  Measurement knobs for A/B runs.
+ * Each call sets every knob from its mask, so pcnn_persist_tune(ctx, 0) restores the defaults; a driver that refused a
+ * cooperative cluster launch and CUDA_LAUNCH_BLOCKING=1 still keep bits 1 and 2 on, as they do without any tune call.
  * out6[5] of pcnn_persist_info: bit 0 = cooperative launch, bit 1 = direct exchange used, bit 2 = two images per CTA (one
  * 448-thread CTA per SM, chosen when the batch outnumbers the SMs and ceil(B / 2) such CTAs fit as clusters). */
 int pcnn_persist_info(pcnn_ctx *ctx, int *out6);

@@ -88,7 +88,8 @@ extern "C" int pcnn_create(pcnn_ctx **out, int device, void *stream) {
     }
     {   // a CUDA runtime setting, not a knob of this library: blocking launches change the order pcnn_learn_host must enqueue in
         const char *lb = getenv("CUDA_LAUNCH_BLOCKING");
-        c->hs_copies_first = lb && lb[0] == '1';
+        c->launch_blocking_env = lb && lb[0] == '1';
+        c->hs_copies_first = c->launch_blocking_env;
     }
     // default parameters = the reference's static-constructor state
     float init[NPARAM];

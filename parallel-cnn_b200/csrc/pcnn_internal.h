@@ -98,6 +98,7 @@ struct pcnn_ctx {
     long hs_label_cap = 0, hs_ready_cap = 0;
     unsigned hs_serial = 0;
     bool hs_copies_first = false;           // launches block the host thread (CUDA_LAUNCH_BLOCKING, kernel-replay profilers)
+    bool launch_blocking_env = false;       // CUDA_LAUNCH_BLOCKING=1 at context creation (keeps hs_copies_first across pcnn_persist_tune)
     bool hs_no_pull = false;          // pcnn_persist_tune bit 4: pinned host images go through the staged stream too (A/B)
     double *h_hs_done = nullptr;            // pinned {double error sum, unsigned tag} written by the kernel after its last step
     cudaStream_t copy_stream = nullptr;
@@ -114,7 +115,8 @@ struct pcnn_ctx {
     int persist_cap = 0;                    // co-resident CTAs of k_train_persist on this device
     bool persist_used = false;
     int persist_cluster_cap = 0;            // co-resident CTAs when launched as clusters of 8
-    bool persist_no_coop = false;           // the driver refused cooperative + cluster launches
+    bool persist_no_coop = false;           // launch without the cooperative attribute (driver refusal or pcnn_persist_tune bit 1)
+    bool persist_coop_refused = false;      // the driver refused a cooperative + cluster launch (keeps persist_no_coop across tunes)
     int persist_force_cluster = 0;          // > 0: cap the cluster size (A/B measurements through pcnn_persist_tune)
     int persist_last_cluster = 0, persist_last_grid = 0, persist_last_direct = 0;
     int persist_pair_cap[2] = {0, 0};       // co-resident two-image CTAs (448 threads) in clusters of 4 / of 2

@@ -250,6 +250,15 @@ __device__ __forceinline__ int step_images(FusedSmem<InT> &S, ImageSmem<InT> &H,
     return li;
 }
 
+// The fp32 staging buffers of a CTA half start as zeros.  A half without an image still reads its buffer in the c1 weight
+// gradient of image_step_single (as a product with dpc = 0), and leftover shared memory may hold NaN (0 x NaN = NaN).  From
+// then on only bulk copies of pixels and the u8 conversion write them.  The fence orders these stores before the bulk copies.
+// Not inlined: the launch prologue then leaves the register allocation of the step loop alone.
+__device__ __noinline__ void zero_staging(float *imgf, int t) {
+    for (int i = t; i < 2 * PCNN_IMG; i += NT) imgf[i] = 0.0f;
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+
 // two-image CTA (IPC = 2): image 0's buffers and everything the CTA shares, image 1's buffers, the hand-over area
 template <typename InT> struct PairSmem {
     FusedSmem<InT> s;
@@ -321,6 +330,7 @@ __global__ void __launch_bounds__(NT * IPC, IPC == 1 ? FUSED_CTAS_PER_SM : 1) k_
         if (t == 0) *(volatile int *)a.abort_flag = 4;
         return;
     }
+    zero_staging(&H.imgf[0][0], id.t);      // ordered before the first bulk copy by the barrier that ends init_barriers
     init_barriers(S, IPC == 1 ? nullptr : &PS.h1);
     if (CS > 1) cluster_sync_all();   // every CTA's mbarriers are initialised before a peer may signal them
     int li = 0;                 // running image counter of this half (staging buffer + mbarrier phase)
@@ -800,6 +810,7 @@ int pcnn_persist_run(pcnn_ctx *ctx, const pcnn_split_binding &s, int B, long nst
                 // a driver that refuses cooperative + cluster launches: the grid was sized by cudaOccupancyMaxActiveClusters,
                 // so it is co-resident on an otherwise idle device; remember the choice
                 cudaGetLastError();
+                ctx->persist_coop_refused = true;
                 ctx->persist_no_coop = true;
                 cfg.attrs = at + 1;
                 cfg.numAttrs = 1;
@@ -947,8 +958,9 @@ extern "C" int pcnn_persist_tune(pcnn_ctx *ctx, int max_cluster) {
                  "launch), 8 (two-stage exchange also on 2 GPUs), 16 (pinned host images are staged, not pulled by the kernel)");
     ctx->persist_no_direct = (max_cluster & 8) != 0;
     ctx->persist_force_cluster = (max_cluster & 1) ? 1 : 0;
-    if (max_cluster & 2) ctx->persist_no_coop = true;
-    if (max_cluster & 4) ctx->hs_copies_first = true;
+    // the mask is the whole state of the knobs (tune(0) restores the defaults); the automatic causes are kept on their own
+    ctx->persist_no_coop = (max_cluster & 2) != 0 || ctx->persist_coop_refused;
+    ctx->hs_copies_first = (max_cluster & 4) != 0 || ctx->launch_blocking_env;
     ctx->hs_no_pull = (max_cluster & 16) != 0;
     return PCNN_OK;
 }
