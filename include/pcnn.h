@@ -267,7 +267,7 @@ int pcnn_l5_forward(pcnn_ctx *ctx, const float *params_dev, const void *images_d
  * The reference's conv semantics (valid, stride 1, cross-correlation, layer.h:118-130) generalised to C input channels,
  * K filters of R x S taps, on the wgmma tensor cores with register accumulators and TMA-fed operands (csrc/conv_tc.cu).
  * Activations are NHWC bf16 with a row pitch of `row_pitch` elements (>= W*C, multiple of 8); filters fp32 KRSC on the
- * host (rounded to bf16 once, at plan creation); output NHWC bf16 [N][H-R+1][W-S+1][K], bias and optional sigmoid fused.
+ * host (rounded to bf16 on the device at plan creation, refreshed from device memory by pcnn_conv_plan_set_params); output NHWC bf16 [N][H-R+1][W-S+1][K], bias and optional sigmoid fused.
  * Pad contents are ignored by the forward, the weight gradient and the input gradient alike: the pad columns W*C ..
  * row_pitch-1 and the pad rows H .. image_rows-1 of x may hold anything, NaN included, without changing a result bit.
  * Constraint of this round: some pixel block Qt with (Qt+S-1)*C <= 32, Qt*K <= 256 and Qt*K % 16 == 0 must exist
@@ -291,7 +291,7 @@ int pcnn_conv_tc_plan_destroy(pcnn_ctx *ctx, pcnn_conv_plan *plan);
 int pcnn_conv_tc_plan_info(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows, int *out5);
 int pcnn_conv_tc_fwd(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *x_bf16_dev, void *y_bf16_dev);
 /* Forward for wide channel counts (csrc/conv_wide_tc.cu): the same contract as pcnn_conv_tc_plan_create_strided (x NHWC bf16 with
- * row_pitch and image_rows, filters fp32 KRSC rounded to bf16 once here, optional bias, act 0 none / 1 sigmoid, y dense NHWC bf16
+ * row_pitch and image_rows, filters fp32 KRSC rounded to bf16 here or by pcnn_conv_plan_set_params, optional bias, act 0 none / 1 sigmoid, y dense NHWC bf16
  * [N][(H-R)/stride+1][(W-S)/stride+1][K], pad columns and pad rows of x ignored, NaN included), computed as a tap-major implicit
  * GEMM on wgmma with the channels as the reduction.  The plan is run by pcnn_conv_tc_fwd (which then also needs y 16-byte aligned)
  * and freed by pcnn_conv_tc_plan_destroy.  Its domain is exactly the shapes that
@@ -397,6 +397,28 @@ int pcnn_crop_nhwc_bf16(pcnn_ctx *ctx, const void *src_bf16_dev, void *dst_bf16_
                         int src_row_pitch, int src_image_rows);
 /* fp32 [rows][w] -> bf16 [rows][pitch] with zero padding (builds the padded activation rows the TMA descriptor needs) */
 int pcnn_f32_to_bf16_rows(pcnn_ctx *ctx, const float *src_dev, void *dst_bf16_dev, long rows, int w, int pitch);
+/* ------------------------------------------------------------------ training a convolution layer on the device
+ * Refresh the parameters of a plan of any kind (pcnn_conv_tc_plan_create[_strided], pcnn_conv_wide_plan_create[_padded]) from
+ * device memory: filt_f32_dev fp32 KRSC [K][R][S][C] as the create calls take them from the host, bias_f32_dev fp32 [K].  Either
+ * may be NULL ("unchanged"); both NULL is PCNN_ERR_ARG, and so is a bias for a plan created without one.  Enqueued on the
+ * context's stream with no host synchronisation and no allocation: a pcnn_conv_tc_fwd enqueued before it reads the old
+ * parameters, one enqueued after it the new ones.  The plan's buffers and tensor maps stay; only their contents change.
+ * The filters are rounded to bf16 (round to nearest even) on the device, by the same kernels the create calls use for their host
+ * filters (uploaded to a temporary device buffer first): a plan refreshed with f holds the same operand bits as a plan created
+ * from f.  A NaN filter stays a NaN; its payload is whatever __float2bfloat16_rn makes of it. */
+int pcnn_conv_plan_set_params(pcnn_ctx *ctx, pcnn_conv_plan *plan, const float *filt_f32_dev, const float *bias_f32_dev);
+/* The sigmoid derivative and the bias gradient of a convolution layer in one pass over dy.  y, dy and dpre are dense bf16
+ * [pixels][K] (pixels = N * P * Q, the layout both forwards write and the gradients read as dy).
+ *   act 1: dpre = bf16_rn(float(dy) * (float(y) * (1 - float(y)))), in exactly this order, fp32 round to nearest with no
+ *          contraction: the derivative at the pre-activation whose sigmoid the forward stored.  y and dpre must not be NULL.
+ *   act 0: dpre must be NULL and y is not read; only db is computed, over dy.
+ *   db[k] = sum over the pixels of float(dpre[pixel][k]) (of dy at act 0): the bf16 values the weight and input gradients consume,
+ *          accumulated in fp32 in a fixed order (per-CTA partials over pixel ranges that depend only on pixels and K, then a
+ *          fixed-order pass over them, no atomics): reruns and every H100 give the same bits.  db may be NULL at act 1 (no bias).
+ * dpre == dy (in place) is allowed; no other overlap is.  Domain: 1 <= K <= 256, pixels >= 1, act 0 or 1, every pointer 16-byte
+ * aligned; anything else is PCNN_ERR_ARG with the rule in the message.  Elements past pixels * K are never written. */
+int pcnn_conv_bias_act_bwd(pcnn_ctx *ctx, const void *y_bf16_dev, const void *dy_bf16_dev, void *dpre_bf16_dev, float *db_f32_dev,
+                           long pixels, int K, int act);
 
 #ifdef __cplusplus
 }

@@ -127,6 +127,8 @@ _SIG = {
     "pcnn_conv_wide_dgrad_padded": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
     "pcnn_conv_wide_bwd_info_padded": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_f32_to_bf16_rows": [_vp, _vp, _vp, _l, _i, _i],
+    "pcnn_conv_plan_set_params": [_vp, _vp, _vp, _vp],
+    "pcnn_conv_bias_act_bwd": [_vp, _vp, _vp, _vp, _vp, _l, _i, _i],
     "pcnn_conv_bwd_plan_info": [_i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_pad_nhwc_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i],
     "pcnn_crop_nhwc_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i],
@@ -216,6 +218,34 @@ def conv_wide_bwd_info(N, H, W, C, K, R, S, stride=1, row_pitch=None, image_rows
               lib().pcnn_conv_wide_bwd_info_padded(N, H, W, C, K, R, S, int(stride), ph, pw, int(pitch), int(image_rows), out))
     return dict(wgrad_row_blocks=out[0], wgrad_splits=out[1], wgrad_blocks_per_split=out[2], wgrad_stages=out[3], wgrad_units=out[4],
                 dgrad_Pt=out[5], dgrad_Qt=out[6], dgrad_groups=out[7], dgrad_stages=out[8], dgrad_tiles=out[9])
+
+
+def conv_layer_family(N, H, W, C, K, R, S, stride=1, padding=(0, 0), row_pitch=None, image_rows=0):
+    """Which forward plan serves a convolution layer (host only, no GPU): "narrow" (the row-Toeplitz plan,
+    pcnn_conv_tc_plan_create_strided) when pcnn_conv_tc_plan_info accepts the shape and there is no padding, otherwise "wide"
+    (pcnn_conv_wide_plan_create[_padded]).  The two domains do not overlap, so there is nothing to choose.  A padded shape the
+    wide plan refuses but the row-Toeplitz plan takes unpadded (a narrow shape: few channels) has no padded kernel: it is
+    refused with a PcnnError naming pcnn_pad_nhwc_bf16.  Any other shape neither plan takes gets the refusal of the plan its
+    padding points to."""
+    ph, pw = (int(v) for v in padding)
+    if (ph, pw) == (0, 0):
+        try:
+            conv_tc_plan_info(N, H, W, C, K, R, S, stride, row_pitch, image_rows)
+            return "narrow"
+        except PcnnError:
+            conv_wide_plan_info(N, H, W, C, K, R, S, stride, row_pitch, image_rows)
+            return "wide"
+    try:
+        conv_wide_plan_info(N, H, W, C, K, R, S, stride, row_pitch, image_rows, padding=(ph, pw))
+        return "wide"
+    except PcnnError as wide_refusal:
+        try:
+            conv_tc_plan_info(N, H, W, C, K, R, S, stride, row_pitch, image_rows)
+        except PcnnError:
+            raise wide_refusal
+    raise PcnnError("conv_layer_family", -1,
+                    f"padding ({ph}, {pw}) for a narrow shape (C = {C}, K = {K}, {R}x{S} taps) of the row-Toeplitz plan, which has no "
+                    "padding: pad x into a zeroed canvas with pcnn_pad_nhwc_bf16 and build the layer on the canvas")
 
 
 def conv_bwd_plan_info(N, H, W, C, K, R, S, stride=1):

@@ -12,7 +12,8 @@
 //     the view is 3-D for window steps > 1, see pcnn_conv_tc_fwd)
 //     (row r of the filter = the same box shifted down by r rows): zero im2col traffic, the 16x..25x expansion of
 //     im2col never exists anywhere, not even in shared memory;
-//   * B = R matrices [Qt*K x 32] (<= 48 KB) built once on the host from the filter bank, resident in shared memory;
+//   * B = R matrices [Qt*K x 32] (<= 48 KB) built on the device from the filter bank (k_conv_tc_toeplitz, at creation and by
+//     pcnn_conv_plan_set_params), resident in shared memory;
 //   * D = [128 x Qt*K] fp32 in the registers of two warpgroups (64 rows each, N = Qt*K rounded up to 32 <= 256);
 //   * per tile and warpgroup 2*R wgmma (M=64, N, K=16), then the epilogue (bias, optional sigmoid, bf16 pack, store)
 //     straight from the accumulator registers while the producer warp already stages the next tiles.
@@ -25,8 +26,6 @@
 // Warp roles (288 threads, 1 CTA/SM, persistent over tiles): warps 0-7 = two consumer warpgroups (MMA + epilogue, output rows
 // 0-63 and 64-127 of a tile), warp 8 = TMA producer.
 #include "tc_common.cuh"
-
-#include <vector>
 
 using namespace pcnn_tc;
 
@@ -184,6 +183,26 @@ static const void *conv_tc_fwd_variant(bool sigmoid, int npad) {
 #undef PCNN_FWD_ROW
 
 
+// The Toeplitz operand [V][R][npad][32] from fp32 KRSC filters in device memory, one thread per element: a gather that writes
+// every element, so the buffer needs no clearing.  Row ql * K + k < ncols of variant v and filter row r holds f[k][r][s][c] at
+// kk = delta_v + ql * stride * C + s * C + c with delta_v = (v * Qt * stride * C) % 8; everything else is 0.
+__global__ void k_conv_tc_toeplitz(const float *__restrict__ f, __nv_bfloat16 *__restrict__ t, const ConvTcParams p, int S) {
+    const long total = (long)p.V * p.R * p.npad * TC_KCHUNK;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+        const int kk = (int)(i % TC_KCHUNK);
+        const long vrow = i / TC_KCHUNK;
+        const int row = (int)(vrow % p.npad), vr = (int)(vrow / p.npad);
+        const int r = vr % p.R, v = vr / p.R;
+        float val = 0.0f;
+        if (row < p.ncols) {
+            const int ql = row / p.K, k = row % p.K;
+            const int e = kk - (v * p.Qt * p.stride * p.C) % 8 - ql * p.stride * p.C;
+            if (e >= 0 && e < S * p.C) val = f[(((long)k * p.R + r) * S + e / p.C) * p.C + e % p.C];
+        }
+        t[i] = __float2bfloat16_rn(val);
+    }
+}
+
 // fp32 [rows][w] -> bf16 [rows][pitch] (zero padded), for building the padded NHWC activations the TMA map needs
 __global__ void k_f32_to_bf16_rows(const float *__restrict__ src, __nv_bfloat16 *__restrict__ dst, long rows, int w, int pitch) {
     const long total = rows * pitch;
@@ -217,7 +236,7 @@ int make_map_2d(CUtensorMap *map, void *base, uint64_t inner, uint64_t outer, ui
 struct pcnn_conv_plan {
     ConvTcParams p;
     int W, S, row_pitch, stride, in_image_rows;
-    void *d_toeplitz = nullptr;     // [R][ncols][32] bf16
+    void *d_toeplitz = nullptr;     // [V][R][npad][32] bf16
     float *d_bias = nullptr;
     CUtensorMap map_b;
     ConvWidePlan *wide = nullptr;   // non-null: a plan of pcnn_conv_wide_plan_create (conv_wide_tc.cu), nothing above is used
@@ -227,6 +246,15 @@ pcnn_conv_plan *conv_plan_wrap_wide(ConvWidePlan *w) {
     pcnn_conv_plan *pl = new pcnn_conv_plan();
     pl->wide = w;
     return pl;
+}
+
+// the Toeplitz operand of the plan from fp32 KRSC filters in device memory, enqueued on the context's stream
+static int conv_tc_load_filters(pcnn_ctx *ctx, pcnn_conv_plan *pl, const float *filt_dev) {
+    const long total = (long)pl->p.V * pl->p.R * pl->p.npad * TC_KCHUNK;
+    k_conv_tc_toeplitz<<<(int)((total + 255) / 256), 256, 0, ctx->stream>>>(filt_dev, reinterpret_cast<__nv_bfloat16 *>(pl->d_toeplitz),
+                                                                             pl->p, pl->S);
+    PCNN_CHECK_LAUNCH(ctx);
+    return PCNN_OK;
 }
 
 static void free_plan(pcnn_conv_plan *plan) {
@@ -318,20 +346,16 @@ extern "C" int pcnn_conv_tc_plan_create_strided(pcnn_ctx *ctx, int N, int H, int
     p.n_mtiles = sh.n_mtiles; p.n_qtiles = sh.n_qtiles;
     p.act = act;
     p.y_row_elems = (long long)sh.Q * K;
-    // Toeplitz operands: T_{v,r}[(ql, k)][kk] = f[k][r][s][c] where kk = delta_v + (ql + s) * C + c; rows ncols..npad-1 stay zero
-    std::vector<uint16_t> t((size_t)V * R * p.npad * TC_KCHUNK, 0);
-    for (int v = 0; v < V; ++v) {
-        const int delta = (v * Qt * stride * C) % 8;
-        for (int r = 0; r < R; ++r)
-            for (int ql = 0; ql < Qt; ++ql)
-                for (int k = 0; k < K; ++k)
-                    for (int s = 0; s < S; ++s)
-                        for (int c = 0; c < C; ++c)
-                            t[(((size_t)v * R + r) * p.npad + ql * K + k) * TC_KCHUNK + delta + (ql * stride + s) * C + c] =
-                                f32_to_bf16_bits(filt_host[(((size_t)k * R + r) * S + s) * C + c]);
+    // Toeplitz operands: the same device conversion as pcnn_conv_plan_set_params, from a temporary copy of the host filters
+    PCNN_CUDA(cudaMalloc(&pl->d_toeplitz, (size_t)V * R * p.npad * TC_KCHUNK * 2));
+    {
+        const size_t nf = (size_t)K * R * S * C;
+        pcnn_dev_temp tf;
+        PCNN_CUDA(cudaMalloc((void **)&tf.p, nf * sizeof(float)));
+        PCNN_CUDA(cudaMemcpyAsync(tf.p, filt_host, nf * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+        if ((rc = conv_tc_load_filters(ctx, pl, tf.p))) return rc;
+        PCNN_CUDA(cudaStreamSynchronize(ctx->stream));
     }
-    PCNN_CUDA(cudaMalloc(&pl->d_toeplitz, t.size() * 2));
-    PCNN_CUDA(cudaMemcpy(pl->d_toeplitz, t.data(), t.size() * 2, cudaMemcpyHostToDevice));
     if (bias_host) {
         PCNN_CUDA(cudaMalloc((void **)&pl->d_bias, K * sizeof(float)));
         PCNN_CUDA(cudaMemcpy(pl->d_bias, bias_host, K * sizeof(float), cudaMemcpyHostToDevice));
@@ -357,6 +381,25 @@ extern "C" int pcnn_conv_tc_plan_destroy(pcnn_ctx *ctx, pcnn_conv_plan *plan) {
     pcnn_device_guard g(ctx->device);
     cudaStreamSynchronize(ctx->stream);
     free_plan(plan);
+    return PCNN_OK;
+}
+
+extern "C" int pcnn_conv_plan_set_params(pcnn_ctx *ctx, pcnn_conv_plan *plan, const float *filt_f32_dev, const float *bias_f32_dev) {
+    PCNN_REQUIRE(ctx && plan, PCNN_ERR_ARG, "pcnn_conv_plan_set_params: NULL context or plan");
+    PCNN_REQUIRE(filt_f32_dev || bias_f32_dev, PCNN_ERR_ARG,
+                 "pcnn_conv_plan_set_params: filters and bias are both NULL (at least one must be given)");
+    int K = plan->p.K;
+    float *d_bias = plan->d_bias;
+    if (plan->wide) d_bias = conv_wide_bias(plan->wide, &K);
+    PCNN_REQUIRE(!bias_f32_dev || d_bias, PCNN_ERR_ARG,
+                 "pcnn_conv_plan_set_params: a bias for a plan created without one (bias_host NULL): only a plan with a bias can "
+                 "refresh it");
+    pcnn_device_guard g(ctx->device);
+    if (filt_f32_dev) {
+        const int rc = plan->wide ? conv_wide_load_filters(ctx, plan->wide, filt_f32_dev) : conv_tc_load_filters(ctx, plan, filt_f32_dev);
+        if (rc) return rc;
+    }
+    if (bias_f32_dev) PCNN_CUDA(cudaMemcpyAsync(d_bias, bias_f32_dev, (size_t)K * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
     return PCNN_OK;
 }
 

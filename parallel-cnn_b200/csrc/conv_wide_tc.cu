@@ -11,7 +11,7 @@
 //     pixels (one map per such phase, at most st^2 = 16): box coordinate (q0 + s / st, p0 + r / st) is then input pixel
 //     ((p0 + pp) * st + r, (q0 + qq) * st + s) for the block's pixel (pp, qq).  The map extents stop at the last row / pixel of
 //     the image and at channel C: everything outside is zero-filled, pad rows and columns of x are never read.
-//   * B: the filters rounded to bf16 once, KRSC on the device, viewed as {C, R*S, K}: a box {64, 1, Npad} is the K-major
+//   * B: the filters rounded to bf16 on the device (at creation and by pcnn_conv_plan_set_params), KRSC, viewed as {C, R*S, K}: a box {64, 1, Npad} is the K-major
 //     operand of one step; channels >= C and filters >= K are zero-filled by TMA, and a box never reaches the next tap.
 //   * D: [128 x Npad] fp32 in the registers of two warpgroups (rows 0-63 / 64-127 of the block), Npad = K rounded up to 16.
 //   * Epilogue: bias, optional sigmoid, bf16, written to a shared staging tile per warpgroup (SWIZZLE_128B, conflict-free),
@@ -25,8 +25,6 @@
 //
 // Warp roles (288 threads, 1 CTA/SM, persistent over tiles): warps 0-7 = two consumer warpgroups, warp 8 = TMA producer.
 #include "tc_common.cuh"
-
-#include <vector>
 
 using namespace pcnn_tc;
 
@@ -299,6 +297,17 @@ void conv_wide_free(ConvWidePlan *w) {
     delete w;
 }
 
+float *conv_wide_bias(ConvWidePlan *w, int *K) {
+    *K = w->p.K;
+    return w->d_bias;
+}
+
+// fp32 KRSC filters in device memory -> d_filt [K][R*S][C] bf16 (the same order), enqueued on the context's stream
+int conv_wide_load_filters(pcnn_ctx *ctx, ConvWidePlan *w, const float *filt_dev) {
+    const int rsc = w->p.R * w->p.S * w->C;
+    return pcnn_f32_to_bf16_rows(ctx, filt_dev, w->d_filt, w->p.K, rsc, rsc);
+}
+
 // the query of the create call `fn` (its refusals name that call)
 static int wide_plan_info(const char *fn, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w,
                           int row_pitch, int image_rows, int *out8) {
@@ -344,10 +353,14 @@ static int wide_plan_create(const char *fn, pcnn_ctx *ctx, int N, int H, int W, 
     p.R = R; p.S = S; p.stride = stride; p.nch = sh.nch; p.stages = sh.stages; p.K = K;
     p.taps = sh.taps;
     const size_t nf = (size_t)K * R * S * C;
-    std::vector<uint16_t> fb(nf);
-    for (size_t i = 0; i < nf; ++i) fb[i] = f32_to_bf16_bits(filt_host[i]);
     PCNN_CUDA(cudaMalloc(&pl->d_filt, nf * 2));
-    PCNN_CUDA(cudaMemcpy(pl->d_filt, fb.data(), nf * 2, cudaMemcpyHostToDevice));
+    {                                        // the same device conversion as pcnn_conv_plan_set_params
+        pcnn_dev_temp tf;
+        PCNN_CUDA(cudaMalloc((void **)&tf.p, nf * sizeof(float)));
+        PCNN_CUDA(cudaMemcpyAsync(tf.p, filt_host, nf * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+        if ((rc = conv_wide_load_filters(ctx, pl, tf.p))) return rc;
+        PCNN_CUDA(cudaStreamSynchronize(ctx->stream));
+    }
     if (bias_host) {
         PCNN_CUDA(cudaMalloc((void **)&pl->d_bias, K * sizeof(float)));
         PCNN_CUDA(cudaMemcpy(pl->d_bias, bias_host, K * sizeof(float), cudaMemcpyHostToDevice));

@@ -225,6 +225,15 @@ struct ConvWidePlan;
 int conv_wide_fwd(pcnn_ctx *ctx, const ConvWidePlan *w, const void *x_bf16, void *y_bf16);
 void conv_wide_free(ConvWidePlan *w);
 pcnn_conv_plan *conv_plan_wrap_wide(ConvWidePlan *w);   // conv_tc.cu; takes ownership
+// the plan's bias buffer (null for a plan without bias) and its filter count; the filters from fp32 KRSC in device memory,
+// rounded to bf16 on the context's stream (pcnn_conv_plan_set_params and the create calls)
+float *conv_wide_bias(ConvWidePlan *w, int *K);
+int conv_wide_load_filters(pcnn_ctx *ctx, ConvWidePlan *w, const float *filt_dev);
+// a temporary device copy of host data (the create calls upload their filters through one); freed when it goes out of scope
+struct pcnn_dev_temp {
+    float *p = nullptr;
+    ~pcnn_dev_temp() { if (p) cudaFree(p); }
+};
 // The domain and tiling of the wide forward, which its gradients (conv_wide_bwd_tc.cu) share: one rule, refused with
 // PCNN_ERR_ARG and a message that names `fn`, the caller's entry point.  conv_wide_pixel_block picks the Pt x Qt = 128 block
 // of a P x Q image and returns the blocks per image.

@@ -276,14 +276,6 @@ static inline int make_map_bf16(CUtensorMap *map, void *base, int rank, const ui
     return PCNN_OK;
 }
 
-static inline uint16_t f32_to_bf16_bits(float f) {   // round to nearest even, as __float2bfloat16_rn
-    uint32_t u;
-    memcpy(&u, &f, 4);
-    if ((u & 0x7fffffffu) > 0x7f800000u) return 0x7fc0;
-    u += 0x7fffu + ((u >> 16) & 1u);
-    return (uint16_t)(u >> 16);
-}
-
 }  // namespace pcnn_tc
 
 // conv_wide_tc.cu: the maps of x of the wide forward, one per phase (rph[r], sph[s]) the taps read, at index

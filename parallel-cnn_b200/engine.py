@@ -4,7 +4,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import F32, NPARAM, TEST_SET, TRAIN_SET, U8, PcnnError, check, lib
+from ._lib import F32, NPARAM, TEST_SET, TRAIN_SET, U8, PcnnError, check, conv_layer_family, lib
 
 
 def _pixel_type(arr_or_dtype):
@@ -165,6 +165,10 @@ class Engine:
 
     def apply_grad(self, w, g, n):
         self._call("pcnn_apply_grad", _p(w), _p(g), int(n))
+
+    def apply_grad_scaled(self, w, g, n, step):
+        """w += step * g over n fp32 elements (__fmul_rn, then __fadd_rn)"""
+        self._call("pcnn_apply_grad_scaled", _p(w), _p(g), int(n), float(step))
 
     def vectorNorm(self, v, n, B, norms):
         self._call("pcnn_vector_norm", _p(v), int(n), int(B), _p(norms))
@@ -408,6 +412,11 @@ class Engine:
             self._call("pcnn_conv_wide_dgrad_padded", _p(dy_bf16), _p(filt_f32), _p(dx_bf16), N, H, W, Cin, K, R, S, int(stride), ph, pw,
                        int(pitch), int(image_rows))
 
+    def conv_bias_act_bwd(self, y, dy, dpre, db, pixels, K, act):
+        """pcnn_conv_bias_act_bwd: dpre = bf16(dy * y * (1 - y)) at act 1 (dpre may be dy itself), db[k] = sum of dpre (of dy at
+        act 0) over the pixels; dpre None at act 0, db None for a layer without bias"""
+        self._call("pcnn_conv_bias_act_bwd", _p(y), _p(dy), _p(dpre), _p(db), int(pixels), int(K), int(act))
+
     def pad_nhwc(self, src_bf16, dst_bf16, N, H, W, Cin, pad_h, pad_w, dst_row_pitch=0, dst_image_rows=0):
         self._call("pcnn_pad_nhwc_bf16", _p(src_bf16), _p(dst_bf16), N, H, W, Cin, int(pad_h), int(pad_w), int(dst_row_pitch), int(dst_image_rows))
 
@@ -437,6 +446,11 @@ class ConvPlan:
 
     def fwd(self, x_bf16_dev, y_bf16_dev):
         check("pcnn_conv_tc_fwd", lib().pcnn_conv_tc_fwd(self.engine.ctx, self.plan, _p(x_bf16_dev), _p(y_bf16_dev)))
+
+    def set_params(self, filt_dev, bias_dev=None):
+        """new filters (fp32 KRSC) and / or bias (fp32 [K]) from device memory, enqueued on the engine's stream
+        (pcnn_conv_plan_set_params); None leaves that part unchanged"""
+        check("pcnn_conv_plan_set_params", lib().pcnn_conv_plan_set_params(self.engine.ctx, self.plan, _p(filt_dev), _p(bias_dev)))
 
     def close(self):
         if self.plan and self.engine.ctx:
@@ -477,6 +491,79 @@ class WideConvPlan(ConvPlan):
         self.out_shape = (N, (H + 2 * ph - R) // stride + 1, (W + 2 * pw - S) // stride + 1, K)
 
 
+class ConvLayer:
+    """One bf16 convolution layer trained on the device: forward, backward and an SGD step with no host round trip.
+
+    It owns fp32 master filters (KRSC) and bias, their gradients dw and db, all in DeviceArrays, and a forward plan of the family
+    that serves the shape (conv_layer_family: the row-Toeplitz plan for few channels without padding, the wide plan otherwise).
+    Activations are NHWC bf16: x with row_pitch (None = W*C rounded up to 8) and image_rows (0 = H), y and dy dense
+    [N][P][Q][K], dx in x's layout.  act 1 is a sigmoid after the bias."""
+
+    def __init__(self, engine, N, H, W, C, K, R, S, filt, bias=None, act=0, stride=1, padding=(0, 0), row_pitch=None, image_rows=0):
+        self.engine = engine
+        self.shape = (N, H, W, C, K, R, S)
+        self.act, self.stride = int(act), int(stride)
+        self.padding = tuple(int(v) for v in padding)
+        self.row_pitch = int(row_pitch if row_pitch is not None else (W * C + 7) // 8 * 8)
+        self.image_rows = int(image_rows)
+        self.family = conv_layer_family(N, H, W, C, K, R, S, self.stride, self.padding, self.row_pitch, self.image_rows)
+        filt = np.ascontiguousarray(filt, np.float32).reshape(K, R, S, C)
+        bias = None if bias is None else np.ascontiguousarray(bias, np.float32).reshape(K)
+        if self.family == "narrow":
+            self.plan = ConvPlan(engine, N, H, W, C, K, R, S, filt, bias, act=act, row_pitch=self.row_pitch, image_rows=self.image_rows,
+                                 stride=self.stride)
+        else:
+            self.plan = WideConvPlan(engine, N, H, W, C, K, R, S, filt, bias, act=act, row_pitch=self.row_pitch,
+                                     image_rows=self.image_rows, stride=self.stride, padding=self.padding)
+        self.out_shape = self.plan.out_shape
+        self.pixels = int(np.prod(self.out_shape[:3]))
+        self.filt = DeviceArray.from_host(engine, filt)
+        self.bias = None if bias is None else DeviceArray.from_host(engine, bias)
+        self.dw = engine.array((K, R, S, C))
+        self.db = None if bias is None else engine.array(K)
+        self._x = None
+
+    def forward(self, x, y):
+        """y = act(conv(x) + bias) with the plan's bf16 filters.  The layer keeps x: backward's weight gradient reads it."""
+        self.plan.fwd(x, y)
+        self._x = x
+
+    def backward(self, y, dy, dx=None):
+        """Gradients of the most recent forward, whose output y was: dw, db (with a bias) and dx (when given; a first layer
+        passes None).  dy is CONSUMED: with a sigmoid it is overwritten in place by the gradient at the pre-activation, which
+        the weight and input gradients then read (pcnn_conv_bias_act_bwd, skipped without sigmoid and bias)."""
+        N, H, W, C, K, R, S = self.shape
+        e = self.engine
+        if self.act or self.bias is not None:
+            e.conv_bias_act_bwd(y if self.act else None, dy, dy if self.act else None, self.db, self.pixels, K, self.act)
+        if self.family == "narrow":
+            e.conv_wgrad(self._x, dy, self.dw, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride)
+            if dx is not None:
+                e.conv_dgrad(dy, self.filt, dx, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride)
+        else:
+            e.conv_wide_wgrad(self._x, dy, self.dw, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride, self.padding)
+            if dx is not None:
+                e.conv_wide_dgrad(dy, self.filt, dx, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride, self.padding)
+
+    def sgd(self, lr):
+        """w += (-lr) * dw and b += (-lr) * db in fp32 on the masters, then the plan refreshed from them, all on the engine's stream"""
+        n = int(np.prod(self.shape[4:])) * self.shape[3]
+        self.engine.apply_grad_scaled(self.filt, self.dw, n, -lr)
+        if self.bias is not None:
+            self.engine.apply_grad_scaled(self.bias, self.db, self.shape[4], -lr)
+        self.plan.set_params(self.filt, self.bias)
+
+    def params(self):
+        """host copies (filters [K][R][S][C], bias [K] or None) of the fp32 masters"""
+        return self.filt.to_host(), None if self.bias is None else self.bias.to_host()
+
+    def close(self):
+        self.plan.close()
+        for a in (self.filt, self.bias, self.dw, self.db):
+            if a is not None:
+                a.free()
+
+
 def f32_to_bf16_bits(a):
     """numpy float32 -> uint16 bf16 bit patterns (round to nearest even), the rounding the kernels use; NaN -> the quiet NaN
     0x7FC0 (rounding the payload could carry into the exponent and the sign: 0x7FFFFFFF would become -0)"""
@@ -491,4 +578,4 @@ def bf16_bits_to_f32(b):
 
 
 C_ = C
-__all__ = ["Engine", "DeviceArray", "ConvPlan", "WideConvPlan", "f32_to_bf16_bits", "bf16_bits_to_f32", "TRAIN_SET", "TEST_SET", "U8", "F32"]
+__all__ = ["Engine", "DeviceArray", "ConvPlan", "WideConvPlan", "ConvLayer", "f32_to_bf16_bits", "bf16_bits_to_f32", "TRAIN_SET", "TEST_SET", "U8", "F32"]

@@ -252,6 +252,98 @@ def run_wide_same(name, N, H, W, C, K, R, S, stride, pad, iters):
     del x, xc, y, dy, dx, dxc, xt, dyt
 
 
+def run_train(name, N, H, W, C, K, R, S, stride, pad, iters, with_dx=True):
+    """one training step of a ConvLayer (bias, sigmoid), pass by pass: forward, pcnn_conv_bias_act_bwd (out of place, so that every
+    launch sees the same dy), the family's weight and input gradients, sgd (two fp32 updates and pcnn_conv_plan_set_params), and
+    the whole ConvLayer step (forward, backward in place over dy, sgd).  bias_act_bwd moves 3 * pixels * K * 2 bytes (read y and
+    dy, write dpre), compared with 3.35 TB/s.  Next to it the torch eager step on bf16 channels-last tensors of the same shapes:
+    conv2d with bias, sigmoid, autograd backward with dy, then w -= lr * grad on fp32 masters and the re-cast to bf16."""
+    Hc, Wc = H + 2 * pad, W + 2 * pad
+    P, Q = (Hc - R) // stride + 1, (Wc - S) // stride + 1
+    f = rng.uniform(-0.5, 0.5, (K, R, S, C)).astype(np.float32)
+    b = rng.uniform(-0.5, 0.5, K).astype(np.float32)
+    layer = pkg.ConvLayer(eng, N, H, W, C, K, R, S, f, b, act=1, stride=stride, padding=(pad, pad))
+    pitch = layer.row_pitch
+    x = torch.randint(0, 0x3F80, (N * H, pitch), dtype=torch.int16, device="cuda")   # positive bf16 bit patterns < 1.0
+    y = torch.empty((N, P, Q, K), dtype=torch.int16, device="cuda")
+    dy = torch.randint(0, 0x3F80, (N, P, Q, K), dtype=torch.int16, device="cuda")
+    dy ^= (torch.randint(0, 2, (N, P, Q, K), dtype=torch.int16, device="cuda") << 15)   # random signs
+    dpre, dy_step = torch.empty_like(dy), torch.empty_like(dy)
+    dx = torch.empty_like(x) if with_dx else None
+    pixels, lr = N * P * Q, 1e-6
+    gpu, power = card()
+
+    def timeit(fn):
+        for _ in range(5):
+            fn()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        for _ in range(iters):
+            fn()
+        e1.record(stream)
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / iters
+
+    args = (N, H, W, C, K, R, S)
+    if layer.family == "narrow":
+        wgrad = lambda: eng.conv_wgrad(x, dpre, layer.dw, *args, pitch, 0, stride)
+        dgrad = lambda: eng.conv_dgrad(dpre, layer.filt, dx, *args, pitch, 0, stride)
+    else:
+        wgrad = lambda: eng.conv_wide_wgrad(x, dpre, layer.dw, *args, pitch, 0, stride, (pad, pad))
+        dgrad = lambda: eng.conv_wide_dgrad(dpre, layer.filt, dx, *args, pitch, 0, stride, (pad, pad))
+
+    def step():
+        dy_step.copy_(dy)                          # backward consumes dy; the copy is timed on its own below
+        layer.forward(x, y)
+        layer.backward(y, dy_step, dx)
+        layer.sgd(lr)
+
+    ms = {"fwd": timeit(lambda: layer.forward(x, y)),
+          "bias_act_bwd": timeit(lambda: eng.conv_bias_act_bwd(y, dy, dpre, layer.db, pixels, K, 1)),
+          "wgrad": timeit(wgrad)}
+    if with_dx:
+        ms["dgrad"] = timeit(dgrad)
+    ms["sgd_set_params"] = timeit(lambda: layer.sgd(lr))
+    ms["dy_copy"] = timeit(lambda: dy_step.copy_(dy))
+    ms["layer_step_minus_dy_copy"] = timeit(step) - ms["dy_copy"]
+
+    # torch eager step on the same shapes (fresh random x: the values do not change the work)
+    xt = x[:, :W * C].reshape(N, H, W, C).view(torch.bfloat16).permute(0, 3, 1, 2).detach().requires_grad_(with_dx)
+    dyt = dy.view(torch.bfloat16).permute(0, 3, 1, 2)
+    w32 = torch.from_numpy(f).permute(0, 3, 1, 2).to("cuda").contiguous(memory_format=torch.channels_last)
+    b32 = torch.from_numpy(b).to("cuda")
+    wb, bb = w32.to(torch.bfloat16).requires_grad_(True), b32.to(torch.bfloat16).requires_grad_(True)
+
+    def torch_step():
+        wb.grad = bb.grad = None
+        if with_dx:
+            xt.grad = None
+        out = torch.sigmoid(torch.nn.functional.conv2d(xt, wb, bb, stride=stride, padding=pad))
+        out.backward(dyt)
+        with torch.no_grad():
+            w32.add_(wb.grad.float(), alpha=-lr)
+            b32.add_(bb.grad.float(), alpha=-lr)
+            wb.copy_(w32)
+            bb.copy_(b32)
+
+    ms["torch_eager_step"] = timeit(torch_step)
+    ba_bytes = 3 * pixels * K * 2
+    print(json.dumps({"case": name, "N": N, "family": layer.family, "dx": with_dx, "ms": ms,
+                      "bias_act_GBps": ba_bytes / (ms["bias_act_bwd"] * 1e-3) / 1e9,
+                      "bias_act_hbm_frac": ba_bytes / (ms["bias_act_bwd"] * 1e-3) / 1e9 / HBM,
+                      "layer_over_torch": ms["layer_step_minus_dy_copy"] / ms["torch_eager_step"], "gpu": gpu, "power_limit": power}),
+          flush=True)
+    layer.close()
+    del x, y, dy, dpre, dy_step, dx, xt
+
+
+if only == "train":                                                    # a ConvLayer training step, pass by pass, and torch eager
+    run_train("56x56x64->64 3x3 pad 1", 128, 56, 56, 64, 64, 3, 3, 1, 1, 20)
+    run_train("28x28x128->128 3x3 pad 1", 128, 28, 28, 128, 128, 3, 3, 1, 1, 20)
+    run_train("14x14x256->256 3x3 pad 1", 128, 14, 14, 256, 256, 3, 3, 1, 1, 20)
+    run_train("56x56x64->128 3x3 stride 2 pad 1", 128, 56, 56, 64, 128, 3, 3, 2, 1, 20)
+    run_train("LeNet c1 28x28x1->6 5x5", 1024, 28, 28, 1, 6, 5, 5, 1, 0, 20, with_dx=False)
 if only == "widesame":                                                 # "same" layers: built-in padding, pad-copy route, cuDNN
     run_wide_same("56x56x64->64 3x3 pad 1", 128, 56, 56, 64, 64, 3, 3, 1, 1, 20)
     run_wide_same("28x28x128->128 3x3 pad 1", 128, 28, 28, 128, 128, 3, 3, 1, 1, 20)
