@@ -419,6 +419,39 @@ int pcnn_conv_plan_set_params(pcnn_ctx *ctx, pcnn_conv_plan *plan, const float *
  * aligned; anything else is PCNN_ERR_ARG with the rule in the message.  Elements past pixels * K are never written. */
 int pcnn_conv_bias_act_bwd(pcnn_ctx *ctx, const void *y_bf16_dev, const void *dy_bf16_dev, void *dpre_bf16_dev, float *db_f32_dev,
                            long pixels, int K, int act);
+/* Max pooling between convolution layers (csrc/pool_nhwc.cu), as torch.nn.functional.max_pool2d with ceil_mode=False and
+ * dilation 1, in the layouts of the layers around it:
+ *   - x is dense bf16 [N][H][W][C], exactly what both forwards write as y;
+ *   - y and dy are [N][image_rows][row_pitch] with P x Q pixels of C channels per image: the layout a plan reads as x;
+ *   - dx is dense [N][H][W][C], exactly what pcnn_conv_bias_act_bwd and the weight gradients read as dy;
+ *   - argmax is uint8 dense [N][P][Q][C].
+ *     P = (H + 2 pad_h - R) / stride + 1,   Q = (W + 2 pad_w - S) / stride + 1.
+ * Forward: the window of output (p, q) starts at (h0, w0) = (p stride - pad_h, q stride - pad_w).  Over its positions inside the
+ * image only (padding is never a candidate), r = 0..R-1 then s = 0..S-1, starting from m = -Inf and a = the first in-image
+ * position, a position is taken when float(v) > m or v is NaN.  So the first maximum wins a tie (-0 and +0 included), the last
+ * NaN in the window wins if there is one, and a window of all -Inf gives its first in-image element.  y[n][p][q][c] is the bits
+ * of x at the winner, argmax[n][p][q][c] the byte r S + s (< 49).  argmax may be NULL (inference).
+ * Backward: dx[n][h][w][c] sums float(dy[n][p][q][c]) over the windows (p, q) that contain (h, w) and whose argmax points at it,
+ * in ascending p, then ascending q, in fp32 starting from the first term, rounded to bf16 once (a sum with a NaN term and two or
+ * more terms is a NaN whose payload is the conversion's).  With one term dx is dy's bits; with none it is +0.  Every element of
+ * the H x W x C image of dx is written, rows and columns no window covers included; there is no memset pass and no atomics.  When
+ * stride >= R and stride >= S no element has more than one term.
+ * The pad columns and pad rows of y's layout are never written; those of dy are never read (NaN there changes no bit).
+ * Domain (anything else is PCNN_ERR_ARG with the function and the rule in the message):
+ *   - N, H, W, C >= 1; 1 <= R, S <= 7; stride 1..7 (larger than the window is allowed: the gaps get zero gradient);
+ *   - 0 <= pad_h <= R/2 and 0 <= pad_w <= S/2 (every window then holds an image element); H + 2 pad_h >= R, W + 2 pad_w >= S;
+ *   - row_pitch 0 = Q C rounded up to a multiple of 8, otherwise >= Q C and a multiple of 8; image_rows 0 = P, otherwise >= P;
+ *   - H W C, P Q C and Q C within the 32-bit index range of one image;
+ *   - every pointer 16-byte aligned; x, y and argmax pairwise disjoint; dy and argmax disjoint from dx.
+ * Both calls are stream-ordered on the context's stream, allocate nothing, and give the same bits on every run and SM count.
+ * pcnn_maxpool_nhwc_info: host only (no GPU, no context), refusals as the two calls.  out5 = { P, Q, row pitch used, channels per
+ * thread (8 when C % 8 == 0: 16-byte vectors, else 1), most windows over one input pixel }. */
+int pcnn_maxpool_nhwc_bf16_fwd(pcnn_ctx *ctx, const void *x_bf16_dev, void *y_bf16_dev, uint8_t *argmax_dev, int N, int H, int W, int C,
+                               int R, int S, int stride, int pad_h, int pad_w, int y_row_pitch, int y_image_rows);
+int pcnn_maxpool_nhwc_bf16_bwd(pcnn_ctx *ctx, const void *dy_bf16_dev, const uint8_t *argmax_dev, void *dx_bf16_dev, int N, int H, int W,
+                               int C, int R, int S, int stride, int pad_h, int pad_w, int dy_row_pitch, int dy_image_rows);
+int pcnn_maxpool_nhwc_info(int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int row_pitch, int image_rows,
+                           int *out5);
 
 #ifdef __cplusplus
 }

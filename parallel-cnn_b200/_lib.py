@@ -129,6 +129,9 @@ _SIG = {
     "pcnn_f32_to_bf16_rows": [_vp, _vp, _vp, _l, _i, _i],
     "pcnn_conv_plan_set_params": [_vp, _vp, _vp, _vp],
     "pcnn_conv_bias_act_bwd": [_vp, _vp, _vp, _vp, _vp, _l, _i, _i],
+    "pcnn_maxpool_nhwc_bf16_fwd": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
+    "pcnn_maxpool_nhwc_bf16_bwd": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
+    "pcnn_maxpool_nhwc_info": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_conv_bwd_plan_info": [_i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_pad_nhwc_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i],
     "pcnn_crop_nhwc_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i],
@@ -246,6 +249,16 @@ def conv_layer_family(N, H, W, C, K, R, S, stride=1, padding=(0, 0), row_pitch=N
     raise PcnnError("conv_layer_family", -1,
                     f"padding ({ph}, {pw}) for a narrow shape (C = {C}, K = {K}, {R}x{S} taps) of the row-Toeplitz plan, which has no "
                     "padding: pad x into a zeroed canvas with pcnn_pad_nhwc_bf16 and build the layer on the canvas")
+
+
+def maxpool_nhwc_info(N, H, W, C, R, S, stride, padding=(0, 0), row_pitch=0, image_rows=0):
+    """The output size and layout of the NHWC max pool (pcnn_maxpool_nhwc_info; host only, no GPU).  row_pitch 0 = Q*C rounded up
+    to 8 elements, image_rows 0 = P.  vec: channels per thread (8 or 1); cover: most windows over one input pixel."""
+    ph, pw = (int(v) for v in padding)
+    out = (_i * 5)()
+    check("pcnn_maxpool_nhwc_info", lib().pcnn_maxpool_nhwc_info(int(N), int(H), int(W), int(C), int(R), int(S), int(stride), ph, pw,
+                                                                 int(row_pitch), int(image_rows), out))
+    return dict(P=out[0], Q=out[1], row_pitch=out[2], vec=out[3], cover=out[4])
 
 
 def conv_bwd_plan_info(N, H, W, C, K, R, S, stride=1):

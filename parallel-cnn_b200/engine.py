@@ -4,7 +4,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import F32, NPARAM, TEST_SET, TRAIN_SET, U8, PcnnError, check, conv_layer_family, lib
+from ._lib import F32, NPARAM, TEST_SET, TRAIN_SET, U8, PcnnError, check, conv_layer_family, lib, maxpool_nhwc_info
 
 
 def _pixel_type(arr_or_dtype):
@@ -417,6 +417,19 @@ class Engine:
         act 0) over the pixels; dpre None at act 0, db None for a layer without bias"""
         self._call("pcnn_conv_bias_act_bwd", _p(y), _p(dy), _p(dpre), _p(db), int(pixels), int(K), int(act))
 
+    def maxpool_nhwc_fwd(self, x, y, argmax, N, H, W, Cin, R, S, stride, padding=(0, 0), row_pitch=None, image_rows=0):
+        """pcnn_maxpool_nhwc_bf16_fwd: x dense bf16 [N][H][W][C] -> y [N][image_rows][row_pitch] (P x Q pixels of C channels per
+        image) and the uint8 argmax r*S + s [N][P][Q][C] (None for inference); row_pitch None = Q*C rounded up to 8, image_rows 0 = P"""
+        ph, pw = (int(v) for v in padding)
+        self._call("pcnn_maxpool_nhwc_bf16_fwd", _p(x), _p(y), _p(argmax), int(N), int(H), int(W), int(Cin), int(R), int(S), int(stride),
+                   ph, pw, int(row_pitch or 0), int(image_rows))
+
+    def maxpool_nhwc_bwd(self, dy, argmax, dx, N, H, W, Cin, R, S, stride, padding=(0, 0), row_pitch=None, image_rows=0):
+        """pcnn_maxpool_nhwc_bf16_bwd: dy in y's layout and the forward's argmax -> dx dense bf16 [N][H][W][C], every element written"""
+        ph, pw = (int(v) for v in padding)
+        self._call("pcnn_maxpool_nhwc_bf16_bwd", _p(dy), _p(argmax), _p(dx), int(N), int(H), int(W), int(Cin), int(R), int(S), int(stride),
+                   ph, pw, int(row_pitch or 0), int(image_rows))
+
     def pad_nhwc(self, src_bf16, dst_bf16, N, H, W, Cin, pad_h, pad_w, dst_row_pitch=0, dst_image_rows=0):
         self._call("pcnn_pad_nhwc_bf16", _p(src_bf16), _p(dst_bf16), N, H, W, Cin, int(pad_h), int(pad_w), int(dst_row_pitch), int(dst_image_rows))
 
@@ -564,6 +577,43 @@ class ConvLayer:
                 a.free()
 
 
+class MaxPoolLayer:
+    """Max pooling between two ConvLayers (pcnn_maxpool_nhwc_bf16_fwd / _bwd), as max_pool2d(kernel (R, S), stride, padding): S
+    defaults to R and stride to R, as torch does.  It owns the uint8 argmax [N][P][Q][C] the backward reads.
+
+    x is what a ConvLayer's forward writes as y (dense [N][H][W][C]); y is written in the layout the next layer reads as x
+    (row_pitch None = Q*C rounded up to 8, image_rows 0 = P: pass that layer's row_pitch and image_rows); dx is what the
+    previous layer's backward reads as dy.  A stack runs with no copies:
+
+        conv1.forward(x, y1);  pool.forward(y1, x2);  conv2.forward(x2, y2)
+        conv2.backward(y2, dy2, dx2);  pool.backward(dx2, dy1);  conv1.backward(y1, dy1, None)
+
+    with x2 and dx2 in conv2's x layout and y1 and dy1 dense [N][H][W][C]."""
+
+    def __init__(self, engine, N, H, W, C, R, S=None, stride=None, padding=(0, 0), row_pitch=None, image_rows=0):
+        self.engine = engine
+        S = R if S is None else S
+        stride = R if stride is None else stride
+        self.shape = (N, H, W, C, R, S)
+        self.stride = int(stride)
+        self.padding = tuple(int(v) for v in padding)
+        info = maxpool_nhwc_info(N, H, W, C, R, S, self.stride, self.padding, row_pitch or 0, image_rows)
+        self.row_pitch, self.image_rows = info["row_pitch"], int(image_rows)
+        self.out_shape = (N, info["P"], info["Q"], C)
+        self.argmax = engine.array(self.out_shape, np.uint8)
+
+    def forward(self, x, y):
+        """y = max over each window of x, and the argmax the backward reads"""
+        self.engine.maxpool_nhwc_fwd(x, y, self.argmax, *self.shape, self.stride, self.padding, self.row_pitch, self.image_rows)
+
+    def backward(self, dy, dx):
+        """dx (dense, every element written) from dy (in y's layout) through the argmax of the most recent forward"""
+        self.engine.maxpool_nhwc_bwd(dy, self.argmax, dx, *self.shape, self.stride, self.padding, self.row_pitch, self.image_rows)
+
+    def close(self):
+        self.argmax.free()
+
+
 def f32_to_bf16_bits(a):
     """numpy float32 -> uint16 bf16 bit patterns (round to nearest even), the rounding the kernels use; NaN -> the quiet NaN
     0x7FC0 (rounding the payload could carry into the exponent and the sign: 0x7FFFFFFF would become -0)"""
@@ -578,4 +628,4 @@ def bf16_bits_to_f32(b):
 
 
 C_ = C
-__all__ = ["Engine", "DeviceArray", "ConvPlan", "WideConvPlan", "ConvLayer", "f32_to_bf16_bits", "bf16_bits_to_f32", "TRAIN_SET", "TEST_SET", "U8", "F32"]
+__all__ = ["Engine", "DeviceArray", "ConvPlan", "WideConvPlan", "ConvLayer", "MaxPoolLayer", "f32_to_bf16_bits", "bf16_bits_to_f32", "TRAIN_SET", "TEST_SET", "U8", "F32"]

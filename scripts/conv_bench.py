@@ -338,6 +338,57 @@ def run_train(name, N, H, W, C, K, R, S, stride, pad, iters, with_dx=True):
     del x, y, dy, dpre, dy_step, dx, xt
 
 
+def run_pool(name, N, H, W, C, R, stride, pad, iters):
+    """the NHWC max pool (pcnn_maxpool_nhwc_bf16_fwd / _bwd) next to torch's max_pool2d(return_indices=True) and
+    max_pool2d_with_indices_backward on the same channels-last bf16 tensors.  Bytes: forward N*H*W*C*2 + N*P*Q*C*3 (read x, write
+    y and the one-byte argmax), backward N*P*Q*C*3 + N*H*W*C*2 (read dy and argmax, write dx); re-reads of x by overlapping
+    windows come from L2 and are not counted.  Torch's forward writes 8-byte indices: N*P*Q*C*10 bytes on its output side."""
+    P, Q = (H + 2 * pad - R) // stride + 1, (W + 2 * pad - R) // stride + 1
+    x = torch.randint(0, 0x3F80, (N, H, W, C), dtype=torch.int16, device="cuda")   # positive bf16 bit patterns < 1.0
+    x ^= (torch.randint(0, 2, (N, H, W, C), dtype=torch.int16, device="cuda") << 15)   # random signs
+    y = torch.empty((N, P, Q, C), dtype=torch.int16, device="cuda")
+    am = torch.empty((N, P, Q, C), dtype=torch.uint8, device="cuda")
+    dy = torch.randint(0, 0x3F80, (N, P, Q, C), dtype=torch.int16, device="cuda")
+    dy ^= (torch.randint(0, 2, (N, P, Q, C), dtype=torch.int16, device="cuda") << 15)
+    dx = torch.empty((N, H, W, C), dtype=torch.int16, device="cuda")
+    xt, dyt = x.view(torch.bfloat16).permute(0, 3, 1, 2), dy.view(torch.bfloat16).permute(0, 3, 1, 2)   # channels-last views
+    _, idx = torch.nn.functional.max_pool2d(xt, R, stride, pad, return_indices=True)
+    gpu, power = card()
+
+    def timeit(fn):
+        for _ in range(5):
+            fn()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        for _ in range(iters):
+            fn()
+        e1.record(stream)
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / iters
+
+    big, small = N * H * W * C, N * P * Q * C
+    args = (N, H, W, C, R, R, stride, (pad, pad))
+    eng.maxpool_nhwc_fwd(x, y, am, *args)                          # the backward reads this argmax
+    for what, fn, tfn, nbytes in (
+            ("fwd", lambda: eng.maxpool_nhwc_fwd(x, y, am, *args),
+             lambda: torch.nn.functional.max_pool2d(xt, R, stride, pad, return_indices=True), big * 2 + small * 3),
+            ("bwd", lambda: eng.maxpool_nhwc_bwd(dy, am, dx, *args),
+             lambda: torch.ops.aten.max_pool2d_with_indices_backward(dyt, xt, [R, R], [stride, stride], [pad, pad], [1, 1], False, idx),
+             small * 3 + big * 2)):
+        ms, ms_torch = timeit(fn), timeit(tfn)
+        print(json.dumps({"case": f"{name} {what}", "N": N, "ms": ms, "GBps": nbytes / (ms * 1e-3) / 1e9,
+                          "hbm_frac": nbytes / (ms * 1e-3) / 1e9 / HBM, "torch_ms": ms_torch, "torch_over_ours": ms_torch / ms,
+                          "vec": pkg.maxpool_nhwc_info(*args[:7], args[7])["vec"], "gpu": gpu, "power_limit": power}), flush=True)
+    del x, y, am, dy, dx, xt, dyt, idx
+
+
+if only == "pool":                                                     # max pooling between conv layers, torch beside it
+    run_pool("LeNet c1 output 24x24x6, 2x2/2", 1024, 24, 24, 6, 2, 2, 0, 20)
+    run_pool("112x112x64, 2x2/2", 128, 112, 112, 64, 2, 2, 0, 20)
+    run_pool("112x112x64, 3x3/2 pad 1", 128, 112, 112, 64, 3, 2, 1, 20)
+    run_pool("56x56x128, 2x2/2", 128, 56, 56, 128, 2, 2, 0, 20)
+    run_pool("28x28x256, 2x2/2", 128, 28, 28, 256, 2, 2, 0, 20)
 if only == "train":                                                    # a ConvLayer training step, pass by pass, and torch eager
     run_train("56x56x64->64 3x3 pad 1", 128, 56, 56, 64, 64, 3, 3, 1, 1, 20)
     run_train("28x28x128->128 3x3 pad 1", 128, 28, 28, 128, 128, 3, 3, 1, 1, 20)
