@@ -452,6 +452,44 @@ int pcnn_maxpool_nhwc_bf16_bwd(pcnn_ctx *ctx, const void *dy_bf16_dev, const uin
                                int C, int R, int S, int stride, int pad_h, int pad_w, int dy_row_pitch, int dy_image_rows);
 int pcnn_maxpool_nhwc_info(int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int row_pitch, int image_rows,
                            int *out5);
+/* Fully connected layers (csrc/linear_tc.cu), bf16 on the tensor cores with fp32 accumulation:
+ *   - x is [N][image_rows][row_pitch] bf16 with P x Q pixels of C channels per image: the layout a plan reads as x and the NHWC
+ *     pool writes as y.  A previous linear layer's y is the same with P = Q = 1, C = its O, row_pitch = O, image_rows 1.
+ *   - F = P Q C features in NHWC order; W fp32 [O][P][Q][C] (KRSC with K = O, R = P, S = Q), b fp32 [O];
+ *   - y, dy are dense bf16 [N][O]; dW is fp32 [O][P][Q][C].
+ * pcnn_linear_plan_create returns a pcnn_conv_plan: pcnn_conv_tc_fwd runs it, y[n][o] = act(b[o] + sum_f x[n][f] W[o][f]) (act 1 is
+ * the sigmoid of the conv forwards), pcnn_conv_plan_set_params refreshes W (fp32 [O][P][Q][C]) and b from device memory, and
+ * pcnn_conv_tc_plan_destroy frees it.  The plan holds W rounded to bf16 (round to nearest even, on the device).
+ * pcnn_linear_wgrad: dW[o][f] = sum_n dy[n][o] x[n][f], fp32.  pcnn_linear_dgrad: dx[n][f] = sum_o dy[n][o] Wbf16[o][f], rounded to
+ * bf16 once, written in x's layout: exactly the dy pcnn_maxpool_nhwc_bf16_bwd reads, or a previous linear layer's dy.  dx uses the
+ * plan's bf16 weights, the bits the forward multiplied: call it before pcnn_conv_plan_set_params.  Both take the shape from the
+ * plan; a plan not made by pcnn_linear_plan_create is PCNN_ERR_ARG.
+ * Pad columns and pad rows of x are never read (NaN there changes no bit); those of dx are never written; y and dx rows of
+ * every image are fully written.  Reductions may be split into ranges whose fp32 partials are added in a fixed order; the
+ * split depends on the shape only, so reruns and every H100 give the same bits.  All calls are stream-ordered.
+ * Domain (anything else is PCNN_ERR_ARG with the rule in the message, the same for the create call and the query):
+ *   - N, P, Q, C >= 1, 1 <= O <= 256 (the limit of pcnn_conv_bias_act_bwd, which serves as the layer's bias / sigmoid backward);
+ *   - F <= 2^24;
+ *   - row_pitch 0 = Q C rounded up to a multiple of 8, otherwise >= Q C and a multiple of 8 (so a hidden width that feeds another
+ *     linear layer must be a multiple of 8); image_rows 0 = P, otherwise >= P;  act 0 (none) or 1 (sigmoid);
+ *   - every device pointer 16-byte aligned.
+ * pcnn_linear_info: host only (no GPU, no context).  out12 = { row pitch used, 128-image tiles, forward reduction steps (64-feature
+ * chunks), forward splits, forward stages, weight-gradient chunk pairs, weight-gradient splits (image ranges), weight-gradient
+ * stages, input-gradient tiles, chunks per input-gradient tile, input-gradient stages, forward MMA width (O rounded up to 16) }. */
+int pcnn_linear_plan_create(pcnn_ctx *ctx, int N, int P, int Q, int C, int O, int row_pitch, int image_rows, int act,
+                            const float *w_host, const float *b_host, pcnn_conv_plan **out);
+int pcnn_linear_wgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *x_bf16_dev, const void *dy_bf16_dev, float *dw_f32_dev);
+int pcnn_linear_dgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *dy_bf16_dev, void *dx_bf16_dev);
+int pcnn_linear_info(int N, int P, int Q, int C, int O, int row_pitch, int image_rows, int *out12);
+/* Softmax cross-entropy on bf16 logits [N][O], 1 <= O <= 256, labels uint8 [N]:
+ *   p = softmax(row) evaluated in double: m = max, den = sum exp(z - m), p_t = exp(z_t - m) / den;
+ *   dlogits[n][t] = bf16_rn(float_rn((p_t - [t == label]) * scale)), double -> fp32 -> bf16, each round to nearest even: the
+ *     gradient of scale * sum_n CE_n, so scale = 1/N descends the mean loss;
+ *   loss[n] = -((z_label - m) - log den) as fp32 (may be NULL);  pred[n] = the first index of the largest logit (may be NULL).
+ * A row holding a NaN gets pred -1, a NaN loss and NaN dlogits.  A label >= O gives that row a NaN loss and NaN dlogits (pred is
+ * still the argmax).  dlogits == logits (in place) is allowed, any other overlap is not. */
+int pcnn_softmax_ce_bf16(pcnn_ctx *ctx, const void *logits_bf16_dev, const uint8_t *labels_dev, int N, int O, float scale,
+                         void *dlogits_bf16_dev, float *loss_f32_dev, int *pred_i32_dev);
 
 #ifdef __cplusplus
 }

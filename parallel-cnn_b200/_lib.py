@@ -140,6 +140,11 @@ _SIG = {
     "pcnn_conv_wgrad_strided": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
     "pcnn_conv_dgrad_strided": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
     "pcnn_conv_bwd_plan_info_strided": [_i, _i, _i, _i, _i, _i, _i, _i, _vp],
+    "pcnn_linear_plan_create": [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _pvp],
+    "pcnn_linear_wgrad": [_vp, _vp, _vp, _vp, _vp],
+    "pcnn_linear_dgrad": [_vp, _vp, _vp, _vp],
+    "pcnn_linear_info": [_i, _i, _i, _i, _i, _i, _i, _vp],
+    "pcnn_softmax_ce_bf16": [_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp],
 }
 _RESTYPE = {"pcnn_last_error_string": C.c_char_p, "pcnn_mnist_free": None}
 
@@ -259,6 +264,15 @@ def maxpool_nhwc_info(N, H, W, C, R, S, stride, padding=(0, 0), row_pitch=0, ima
     check("pcnn_maxpool_nhwc_info", lib().pcnn_maxpool_nhwc_info(int(N), int(H), int(W), int(C), int(R), int(S), int(stride), ph, pw,
                                                                  int(row_pitch), int(image_rows), out))
     return dict(P=out[0], Q=out[1], row_pitch=out[2], vec=out[3], cover=out[4])
+
+
+def linear_info(N, P, Q, C, O, row_pitch=0, image_rows=0):
+    """How the fully connected layer tiles a shape (pcnn_linear_info; host only, no GPU).  row_pitch 0 = Q*C rounded up to 8
+    elements, image_rows 0 = P.  Each pass splits its reduction as a function of the shape alone."""
+    out = (_i * 12)()
+    check("pcnn_linear_info", lib().pcnn_linear_info(int(N), int(P), int(Q), int(C), int(O), int(row_pitch), int(image_rows), out))
+    return dict(row_pitch=out[0], image_tiles=out[1], fwd_steps=out[2], fwd_splits=out[3], fwd_stages=out[4], wgrad_pairs=out[5],
+                wgrad_splits=out[6], wgrad_stages=out[7], dgrad_tiles=out[8], dgrad_chunks=out[9], dgrad_stages=out[10], npad=out[11])
 
 
 def conv_bwd_plan_info(N, H, W, C, K, R, S, stride=1):

@@ -240,6 +240,7 @@ struct pcnn_conv_plan {
     float *d_bias = nullptr;
     CUtensorMap map_b;
     ConvWidePlan *wide = nullptr;   // non-null: a plan of pcnn_conv_wide_plan_create (conv_wide_tc.cu), nothing above is used
+    LinearPlan *linear = nullptr;   // non-null: a plan of pcnn_linear_plan_create (linear_tc.cu), nothing above is used
 };
 
 pcnn_conv_plan *conv_plan_wrap_wide(ConvWidePlan *w) {
@@ -247,6 +248,14 @@ pcnn_conv_plan *conv_plan_wrap_wide(ConvWidePlan *w) {
     pl->wide = w;
     return pl;
 }
+
+pcnn_conv_plan *conv_plan_wrap_linear(LinearPlan *l) {
+    pcnn_conv_plan *pl = new pcnn_conv_plan();
+    pl->linear = l;
+    return pl;
+}
+
+LinearPlan *conv_plan_linear(pcnn_conv_plan *plan) { return plan->linear; }
 
 // the Toeplitz operand of the plan from fp32 KRSC filters in device memory, enqueued on the context's stream
 static int conv_tc_load_filters(pcnn_ctx *ctx, pcnn_conv_plan *pl, const float *filt_dev) {
@@ -260,6 +269,7 @@ static int conv_tc_load_filters(pcnn_ctx *ctx, pcnn_conv_plan *pl, const float *
 static void free_plan(pcnn_conv_plan *plan) {
     if (!plan) return;
     if (plan->wide) conv_wide_free(plan->wide);
+    if (plan->linear) linear_free(plan->linear);
     if (plan->d_toeplitz) cudaFree(plan->d_toeplitz);
     if (plan->d_bias) cudaFree(plan->d_bias);
     delete plan;
@@ -391,12 +401,15 @@ extern "C" int pcnn_conv_plan_set_params(pcnn_ctx *ctx, pcnn_conv_plan *plan, co
     int K = plan->p.K;
     float *d_bias = plan->d_bias;
     if (plan->wide) d_bias = conv_wide_bias(plan->wide, &K);
+    if (plan->linear) d_bias = linear_bias(plan->linear, &K);
     PCNN_REQUIRE(!bias_f32_dev || d_bias, PCNN_ERR_ARG,
                  "pcnn_conv_plan_set_params: a bias for a plan created without one (bias_host NULL): only a plan with a bias can "
                  "refresh it");
     pcnn_device_guard g(ctx->device);
     if (filt_f32_dev) {
-        const int rc = plan->wide ? conv_wide_load_filters(ctx, plan->wide, filt_f32_dev) : conv_tc_load_filters(ctx, plan, filt_f32_dev);
+        const int rc = plan->wide     ? conv_wide_load_filters(ctx, plan->wide, filt_f32_dev)
+                       : plan->linear ? linear_load_weights(ctx, plan->linear, filt_f32_dev)
+                                      : conv_tc_load_filters(ctx, plan, filt_f32_dev);
         if (rc) return rc;
     }
     if (bias_f32_dev) PCNN_CUDA(cudaMemcpyAsync(d_bias, bias_f32_dev, (size_t)K * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
@@ -408,6 +421,7 @@ extern "C" int pcnn_conv_tc_fwd(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void 
     PCNN_REQUIRE(((uintptr_t)x_bf16 & 15) == 0, PCNN_ERR_ARG, "pcnn_conv_tc_fwd: activations must be 16-byte aligned");
     pcnn_device_guard g(ctx->device);
     if (plan->wide) return conv_wide_fwd(ctx, plan->wide, x_bf16, y_bf16);
+    if (plan->linear) return linear_fwd(ctx, plan->linear, x_bf16, y_bf16);
     ConvTcParams p = plan->p;
     p.y = reinterpret_cast<__nv_bfloat16 *>(y_bf16);
     CUtensorMap map_x;

@@ -229,6 +229,15 @@ pcnn_conv_plan *conv_plan_wrap_wide(ConvWidePlan *w);   // conv_tc.cu; takes own
 // rounded to bf16 on the context's stream (pcnn_conv_plan_set_params and the create calls)
 float *conv_wide_bias(ConvWidePlan *w, int *K);
 int conv_wide_load_filters(pcnn_ctx *ctx, ConvWidePlan *w, const float *filt_dev);
+// linear_tc.cu: a plan of pcnn_linear_plan_create is a pcnn_conv_plan holding a LinearPlan, run, refreshed and freed like the
+// wide one; conv_plan_linear is null for a convolution plan
+struct LinearPlan;
+int linear_fwd(pcnn_ctx *ctx, const LinearPlan *l, const void *x_bf16, void *y_bf16);
+void linear_free(LinearPlan *l);
+float *linear_bias(LinearPlan *l, int *O);
+int linear_load_weights(pcnn_ctx *ctx, LinearPlan *l, const float *w_dev);
+pcnn_conv_plan *conv_plan_wrap_linear(LinearPlan *l);   // conv_tc.cu; takes ownership
+LinearPlan *conv_plan_linear(pcnn_conv_plan *plan);
 // a temporary device copy of host data (the create calls upload their filters through one); freed when it goes out of scope
 struct pcnn_dev_temp {
     float *p = nullptr;

@@ -4,7 +4,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import F32, NPARAM, TEST_SET, TRAIN_SET, U8, PcnnError, check, conv_layer_family, lib, maxpool_nhwc_info
+from ._lib import F32, NPARAM, TEST_SET, TRAIN_SET, U8, PcnnError, check, conv_layer_family, lib, linear_info, maxpool_nhwc_info
 
 
 def _pixel_type(arr_or_dtype):
@@ -439,6 +439,19 @@ class Engine:
     def softmax_ce(self, logits, labels, B, n, prob=None, d=None, loss=None):
         self._call("pcnn_softmax_ce", _p(logits), _p(labels), int(B), int(n), _p(prob), _p(d), _p(loss))
 
+    def softmax_ce_bf16(self, logits, labels, N, O, scale, dlogits, loss=None, pred=None):
+        """pcnn_softmax_ce_bf16: bf16 logits [N][O] and uint8 labels -> dlogits = bf16((softmax - onehot) * scale) (may be logits
+        itself), fp32 loss [N] and int32 pred [N] (each None to skip)"""
+        self._call("pcnn_softmax_ce_bf16", _p(logits), _p(labels), int(N), int(O), float(scale), _p(dlogits), _p(loss), _p(pred))
+
+    def linear_wgrad(self, plan, x, dy, dw):
+        """pcnn_linear_wgrad: dW fp32 [O][P][Q][C] = dy^T x, the shape from the LinearPlan"""
+        self._call("pcnn_linear_wgrad", plan.plan, _p(x), _p(dy), _p(dw))
+
+    def linear_dgrad(self, plan, dy, dx):
+        """pcnn_linear_dgrad: dx = dy W with the plan's bf16 weights, written in x's layout (pad untouched)"""
+        self._call("pcnn_linear_dgrad", plan.plan, _p(dy), _p(dx))
+
 
 class ConvPlan:
     """bf16 tensor-core convolution plan (pcnn_conv_tc_*): filters fp32 KRSC on the host, activations NHWC bf16."""
@@ -502,6 +515,26 @@ class WideConvPlan(ConvPlan):
                                                           None if b is None else b.ctypes.data, C_.byref(plan)))
         self.plan = plan
         self.out_shape = (N, (H + 2 * ph - R) // stride + 1, (W + 2 * pw - S) // stride + 1, K)
+
+
+class LinearPlan(ConvPlan):
+    """A fully connected layer's plan (pcnn_linear_plan_create): x [N][image_rows][row_pitch] bf16 holding P x Q pixels of C
+    channels per image, w fp32 [O][P][Q][C], y dense bf16 [N][O], 1 <= O <= 256.  row_pitch None or 0 = Q*C rounded up to 8.  Run,
+    refreshed and closed like ConvPlan; its gradients are Engine.linear_wgrad / linear_dgrad."""
+
+    def __init__(self, engine, N, P, Q, C, O, w, bias=None, act=0, row_pitch=None, image_rows=0):
+        self.engine = engine
+        self.shape = (N, P, Q, C, O)
+        self.row_pitch = int(row_pitch or (Q * C + 7) // 8 * 8)
+        w = np.ascontiguousarray(w, np.float32)
+        assert w.size == O * P * Q * C
+        b = None if bias is None else np.ascontiguousarray(bias, np.float32)
+        plan = C_.c_void_p()
+        check("pcnn_linear_plan_create",
+              lib().pcnn_linear_plan_create(engine.ctx, N, P, Q, C, O, self.row_pitch, int(image_rows), int(act), w.ctypes.data,
+                                            None if b is None else b.ctypes.data, C_.byref(plan)))
+        self.plan = plan
+        self.out_shape = (N, O)
 
 
 class ConvLayer:
@@ -577,6 +610,75 @@ class ConvLayer:
                 a.free()
 
 
+class LinearLayer:
+    """A fully connected layer trained on the device, with ConvLayer's interface: fp32 masters w [O][P][Q][C] and bias [O], their
+    gradients dw and db, and a LinearPlan holding w in bf16.
+
+    x is [N][image_rows][row_pitch] bf16 with P x Q pixels of C channels per image, which is what MaxPoolLayer writes as y (pass
+    its row_pitch and image_rows) or, with P = Q = 1 and C = the previous O, what a LinearLayer writes (row_pitch = that O, a
+    multiple of 8).  y and dy are dense [N][O]; dx is written in x's layout.  act 1 is a sigmoid after the bias.  A LeNet-style
+    classifier runs every pass on the engine's stream:
+
+        conv1.forward(x, y1);  pool1.forward(y1, x2);  conv2.forward(x2, y2);  pool2.forward(y2, x3)
+        fc1.forward(x3, y3);  fc2.forward(y3, z)
+        engine.softmax_ce_bf16(z, labels, N, 10, 1 / N, dz, loss, pred)
+        fc2.backward(z, dz, dy3);  fc1.backward(y3, dy3, dx3);  pool2.backward(dx3, dy2)
+        conv2.backward(y2, dy2, dx2);  pool1.backward(dx2, dy1);  conv1.backward(y1, dy1, None)
+        for layer in (conv1, conv2, fc1, fc2): layer.sgd(lr)"""
+
+    def __init__(self, engine, N, P, Q, C, O, w, bias=None, act=0, row_pitch=None, image_rows=0):
+        self.engine = engine
+        self.shape = (N, P, Q, C, O)
+        self.act = int(act)
+        self.row_pitch = int(row_pitch or (Q * C + 7) // 8 * 8)
+        self.image_rows = int(image_rows)
+        self.info = linear_info(N, P, Q, C, O, self.row_pitch, self.image_rows)
+        w = np.ascontiguousarray(w, np.float32).reshape(O, P, Q, C)
+        bias = None if bias is None else np.ascontiguousarray(bias, np.float32).reshape(O)
+        self.plan = LinearPlan(engine, N, P, Q, C, O, w, bias, act=act, row_pitch=self.row_pitch, image_rows=self.image_rows)
+        self.out_shape = (N, O)
+        self.w = DeviceArray.from_host(engine, w)
+        self.bias = None if bias is None else DeviceArray.from_host(engine, bias)
+        self.dw = engine.array((O, P, Q, C))
+        self.db = None if bias is None else engine.array(O)
+        self._x = None
+
+    def forward(self, x, y):
+        """y = act(x W^T + bias) with the plan's bf16 weights.  The layer keeps x: backward's weight gradient reads it."""
+        self.plan.fwd(x, y)
+        self._x = x
+
+    def backward(self, y, dy, dx=None):
+        """Gradients of the most recent forward, whose output y was: dw, db (with a bias) and dx (when given).  dy is CONSUMED:
+        with a sigmoid it is overwritten in place by the gradient at the pre-activation (pcnn_conv_bias_act_bwd with pixels = N,
+        K = O; skipped without sigmoid and bias).  dx uses the plan's bf16 weights, so call it before sgd."""
+        N, P, Q, C, O = self.shape
+        e = self.engine
+        if self.act or self.bias is not None:
+            e.conv_bias_act_bwd(y if self.act else None, dy, dy if self.act else None, self.db, N, O, self.act)
+        e.linear_wgrad(self.plan, self._x, dy, self.dw)
+        if dx is not None:
+            e.linear_dgrad(self.plan, dy, dx)
+
+    def sgd(self, lr):
+        """w += (-lr) * dw and b += (-lr) * db in fp32 on the masters, then the plan refreshed from them, all on the engine's stream"""
+        N, P, Q, C, O = self.shape
+        self.engine.apply_grad_scaled(self.w, self.dw, O * P * Q * C, -lr)
+        if self.bias is not None:
+            self.engine.apply_grad_scaled(self.bias, self.db, O, -lr)
+        self.plan.set_params(self.w, self.bias)
+
+    def params(self):
+        """host copies (w [O][P][Q][C], bias [O] or None) of the fp32 masters"""
+        return self.w.to_host(), None if self.bias is None else self.bias.to_host()
+
+    def close(self):
+        self.plan.close()
+        for a in (self.w, self.bias, self.dw, self.db):
+            if a is not None:
+                a.free()
+
+
 class MaxPoolLayer:
     """Max pooling between two ConvLayers (pcnn_maxpool_nhwc_bf16_fwd / _bwd), as max_pool2d(kernel (R, S), stride, padding): S
     defaults to R and stride to R, as torch does.  It owns the uint8 argmax [N][P][Q][C] the backward reads.
@@ -628,4 +730,4 @@ def bf16_bits_to_f32(b):
 
 
 C_ = C
-__all__ = ["Engine", "DeviceArray", "ConvPlan", "WideConvPlan", "ConvLayer", "MaxPoolLayer", "f32_to_bf16_bits", "bf16_bits_to_f32", "TRAIN_SET", "TEST_SET", "U8", "F32"]
+__all__ = ["Engine", "DeviceArray", "ConvPlan", "WideConvPlan", "LinearPlan", "ConvLayer", "LinearLayer", "MaxPoolLayer", "f32_to_bf16_bits", "bf16_bits_to_f32", "TRAIN_SET", "TEST_SET", "U8", "F32"]

@@ -383,6 +383,125 @@ def run_pool(name, N, H, W, C, R, stride, pad, iters):
     del x, y, am, dy, dx, xt, dyt, idx
 
 
+def timed(fn, iters):
+    for _ in range(5):
+        fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(stream)
+    for _ in range(iters):
+        fn()
+    e1.record(stream)
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / iters
+
+
+def run_linear(name, N, P, Q, C, O, act, iters):
+    """the three passes of a LinearPlan (pcnn_conv_tc_fwd on a linear plan, pcnn_linear_wgrad, pcnn_linear_dgrad) next to
+    torch.nn.functional.linear and its two backward matmuls on the same bf16 tensors.  Bound: the larger of 2 N F O / 989 TFLOP/s
+    and the bytes of each operand crossing HBM once / 3.35 TB/s.  Forward: x, W bf16, y; weight gradient: x, dy, dW fp32; input
+    gradient: dy, W, dx.  The fp32 slots of a split reduction (written and read once each) are reported apart: the bound omits them."""
+    F_ = P * Q * C
+    w = rng.uniform(-1, 1, (O, P, Q, C)).astype(np.float32) / np.float32(np.sqrt(F_))
+    b = rng.uniform(-0.5, 0.5, O).astype(np.float32)
+    plan = pkg.LinearPlan(eng, N, P, Q, C, O, w, b, act=act)
+    info = pkg.linear_info(N, P, Q, C, O)
+    pitch = info["row_pitch"]
+    x = torch.randint(0, 0x3F80, (N, P, pitch), dtype=torch.int16, device="cuda")
+    y = torch.empty((N, O), dtype=torch.int16, device="cuda")
+    dy = torch.randint(0, 0x3F80, (N, O), dtype=torch.int16, device="cuda")
+    dx = torch.empty_like(x)
+    dw = eng.array((O, P, Q, C))
+    gpu, power = card()
+    xt = x.view(torch.bfloat16)[:, :, :Q * C].reshape(N, F_)
+    wt = torch.from_numpy(w).reshape(O, F_).to("cuda").to(torch.bfloat16)
+    bt = torch.from_numpy(b).to("cuda").to(torch.bfloat16)
+    dyt = dy.view(torch.bfloat16)
+    flops = 2.0 * N * F_ * O
+    passes = (("fwd", lambda: plan.fwd(x, y), lambda: torch.nn.functional.linear(xt, wt, bt), N * F_ * 2 + O * F_ * 2 + N * O * 2,
+               info["fwd_splits"], 2 * info["fwd_splits"] * N * O * 4 if info["fwd_splits"] > 1 else 0),
+              ("wgrad", lambda: eng.linear_wgrad(plan, x, dy, dw), lambda: dyt.t() @ xt, N * F_ * 2 + N * O * 2 + O * F_ * 4,
+               info["wgrad_splits"], 2 * info["wgrad_splits"] * O * F_ * 4 if info["wgrad_splits"] > 1 else 0),
+              ("dgrad", lambda: eng.linear_dgrad(plan, dy, dx), lambda: dyt @ wt, N * O * 2 + O * F_ * 2 + N * F_ * 2, 1, 0))
+    for what, fn, tfn, nbytes, splits, slot_bytes in passes:
+        ms, ms_torch = timed(fn, iters), timed(tfn, iters)
+        t_bound = max(flops / 989e12, nbytes / (HBM * 1e9))
+        print(json.dumps({"case": f"{name} {what}", "N": N, "F": F_, "O": O, "us": ms * 1e3, "bound_us": t_bound * 1e6,
+                          "bound_frac": t_bound / (ms * 1e-3), "bound_by": "flops" if flops / 989e12 > nbytes / (HBM * 1e9) else "HBM",
+                          "MB": nbytes / 1e6, "splits": splits, "slot_MB": slot_bytes / 1e6, "torch_us": ms_torch * 1e3,
+                          "torch_over_ours": ms_torch / ms, "gpu": gpu, "power_limit": power}), flush=True)
+    plan.close()
+    dw.free()
+    del x, y, dy, dx
+
+
+def run_classifier(N, iters):
+    """one training step of conv 8@5x5 sigmoid -> pool 2 -> conv 16@3x3 pad 1 -> pool 2 -> fc 576->128 sigmoid -> fc 128->10 ->
+    softmax cross-entropy (pcnn_softmax_ce_bf16, scale 1/N) -> backward -> sgd of all four layers, on the engine's stream; next to it
+    the torch eager step of the same layers on bf16 channels-last tensors (fp32 masters, w -= lr * grad, re-cast to bf16)"""
+    r = np.random.default_rng(5)
+    u = lambda shape, fan: r.uniform(-1, 1, shape).astype(np.float32) / np.float32(np.sqrt(fan))
+    p = dict(f1=u((8, 5, 5, 1), 25), b1=u(8, 25), f2=u((16, 3, 3, 8), 72), b2=u(16, 72), w3=u((128, 6, 6, 16), 576),
+             b3=u(128, 576), w4=u((10, 1, 1, 128), 128), b4=u(10, 128))
+    c1 = pkg.ConvLayer(eng, N, 28, 28, 1, 8, 5, 5, p["f1"], p["b1"], act=1)
+    c2 = pkg.ConvLayer(eng, N, 12, 12, 8, 16, 3, 3, p["f2"], p["b2"], act=0, padding=(1, 1))
+    fc1 = pkg.LinearLayer(eng, N, 6, 6, 16, 128, p["w3"], p["b3"], act=1)
+    fc2 = pkg.LinearLayer(eng, N, 1, 1, 128, 10, p["w4"], p["b4"], act=0, row_pitch=128)
+    p1 = pkg.MaxPoolLayer(eng, N, 24, 24, 8, 2, row_pitch=c2.row_pitch, image_rows=c2.image_rows)
+    p2 = pkg.MaxPoolLayer(eng, N, 12, 12, 16, 2, row_pitch=fc1.row_pitch, image_rows=fc1.image_rows)
+    e = lambda *s: torch.empty(s, dtype=torch.int16, device="cuda")
+    x = torch.randint(0, 0x3F80, (N * 28, 32), dtype=torch.int16, device="cuda")
+    labels = torch.randint(0, 10, (N,), dtype=torch.uint8, device="cuda")
+    y1, dy1, x2, dx2, y2, dy2 = e(N, 24, 24, 8), e(N, 24, 24, 8), e(N, 12, 96), e(N, 12, 96), e(N, 12, 12, 16), e(N, 12, 12, 16)
+    x3, dx3, y3, dy3, z, dz = e(N, 6, 96), e(N, 6, 96), e(N, 128), e(N, 128), e(N, 10), e(N, 10)
+    loss = torch.empty(N, dtype=torch.float32, device="cuda")
+    lr = 0.3
+    gpu, power = card()
+
+    def step():
+        c1.forward(x, y1); p1.forward(y1, x2); c2.forward(x2, y2); p2.forward(y2, x3); fc1.forward(x3, y3); fc2.forward(y3, z)
+        eng.softmax_ce_bf16(z, labels, N, 10, 1.0 / N, dz, loss)
+        fc2.backward(z, dz, dy3); fc1.backward(y3, dy3, dx3); p2.backward(dx3, dy2); c2.backward(y2, dy2, dx2)
+        p1.backward(dx2, dy1); c1.backward(y1, dy1, None)
+        for layer in (c1, c2, fc1, fc2):
+            layer.sgd(lr)
+
+    ms = timed(step, iters)
+    F = torch.nn.functional
+    xt = x[:, :28].reshape(N, 28, 28, 1).view(torch.bfloat16).permute(0, 3, 1, 2)
+    lt = labels.long()
+    m32 = {k: torch.from_numpy(v).to("cuda") for k, v in p.items()}
+    m32["f1"] = m32["f1"].permute(0, 3, 1, 2).contiguous(memory_format=torch.channels_last)
+    m32["f2"] = m32["f2"].permute(0, 3, 1, 2).contiguous(memory_format=torch.channels_last)
+    m32["w3"], m32["w4"] = m32["w3"].reshape(128, -1), m32["w4"].reshape(10, -1)
+    mb = {k: v.to(torch.bfloat16).requires_grad_(True) for k, v in m32.items()}
+
+    def torch_step():
+        for v in mb.values():
+            v.grad = None
+        h = F.max_pool2d(torch.sigmoid(F.conv2d(xt, mb["f1"], mb["b1"])), 2)
+        h = F.max_pool2d(F.conv2d(h, mb["f2"], mb["b2"], padding=1), 2)
+        h = torch.sigmoid(F.linear(h.permute(0, 2, 3, 1).reshape(N, -1), mb["w3"], mb["b3"]))
+        F.cross_entropy(F.linear(h, mb["w4"], mb["b4"]), lt).backward()
+        with torch.no_grad():
+            for k in m32:
+                m32[k].add_(mb[k].grad.float(), alpha=-lr)
+                mb[k].copy_(m32[k])
+
+    ms_torch = timed(torch_step, iters)
+    print(json.dumps({"case": f"classifier training step N={N}", "ms": ms, "torch_eager_ms": ms_torch, "ours_over_torch": ms / ms_torch,
+                      "gpu": gpu, "power_limit": power}), flush=True)
+    for layer in (c1, c2, fc1, fc2, p1, p2):
+        layer.close()
+
+
+if only == "linear":                                                   # fully connected passes, torch.nn.functional.linear beside them
+    run_linear("7x7x256 -> 256", 1024, 7, 7, 256, 256, 0, 50)
+    run_linear("1x1x2048 -> 256", 4096, 1, 1, 2048, 256, 0, 50)
+    run_linear("6x6x16 -> 128 sigmoid (fc1)", 1024, 6, 6, 16, 128, 1, 50)
+    run_linear("128 -> 10 (fc2)", 1024, 1, 1, 128, 10, 0, 50)
+if only == "classifier":                                               # one step of the LeNet-style classifier, torch eager beside it
+    run_classifier(1024, 50)
 if only == "pool":                                                     # max pooling between conv layers, torch beside it
     run_pool("LeNet c1 output 24x24x6, 2x2/2", 1024, 24, 24, 6, 2, 2, 0, 20)
     run_pool("112x112x64, 2x2/2", 128, 112, 112, 64, 2, 2, 0, 20)
