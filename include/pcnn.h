@@ -267,12 +267,26 @@ int pcnn_l5_forward(pcnn_ctx *ctx, const float *params_dev, const void *images_d
  * The reference's conv semantics (valid, stride 1, cross-correlation, layer.h:118-130) generalised to C input channels,
  * K filters of R x S taps, on the wgmma tensor cores with register accumulators and TMA-fed operands (csrc/conv_tc.cu).
  * Activations are NHWC bf16 with a row pitch of `row_pitch` elements (>= W*C, multiple of 8); filters fp32 KRSC on the
- * host (rounded to bf16 on the device at plan creation, refreshed from device memory by pcnn_conv_plan_set_params); output NHWC bf16 [N][H-R+1][W-S+1][K], bias and optional sigmoid fused.
+ * host (rounded to bf16 on the device at plan creation, refreshed from device memory by pcnn_conv_plan_set_params); output NHWC bf16 [N][H-R+1][W-S+1][K], bias and activation
+ * (act 0 none, 1 sigmoid, 3 ReLU: PCNN_ACT_* below) fused.
  * Pad contents are ignored by the forward, the weight gradient and the input gradient alike: the pad columns W*C ..
  * row_pitch-1 and the pad rows H .. image_rows-1 of x may hold anything, NaN included, without changing a result bit.
  * Constraint of this round: some pixel block Qt with (Qt+S-1)*C <= 32, Qt*K <= 256 and Qt*K % 16 == 0 must exist
  * (LeNet c1: Qt = 24; 224x224x3 -> 64 x 3x3: Qt = 4).  PARITY UNPINNED by the reference (it has no bf16 path): the
  * checker is orc_conv_fwd_nhwc in oracle/lenet_oracle.c on the bf16-rounded operands. */
+/* Activation codes (`act`) of the device-trained layers: every create call below (row-Toeplitz, wide, padded wide, linear) and
+ * pcnn_conv_bias_act_bwd take one of these three; any other value, 2 included, is PCNN_ERR_ARG with the message
+ * "<function>: act <n> is not 0 (none), 1 (sigmoid) or 3 (ReLU)".  The forward epilogue first forms v = fp32 accumulator + bias,
+ * then
+ *   PCNN_ACT_NONE:    y = bf16_rn(v);
+ *   PCNN_ACT_SIGMOID: y = bf16_rn(sigmoid(v)) (the reference's activation, layer.h:81-83);
+ *   PCNN_ACT_RELU:    y = bf16_rn(v < 0 ? +0 : v), applied once in fp32 before the one rounding.  NaN and -0 pass unchanged, as
+ *                     in torch.relu / clamp_min(0) (not fmaxf, which turns NaN into 0): +Inf stays +Inf, -Inf gives +0, a
+ *                     negative v gives +0 and a positive v too small for bf16 rounds to +0.
+ * The backward of each is pcnn_conv_bias_act_bwd with the same code. */
+#define PCNN_ACT_NONE 0
+#define PCNN_ACT_SIGMOID 1
+#define PCNN_ACT_RELU 3
 typedef struct pcnn_conv_plan pcnn_conv_plan;
 int pcnn_conv_tc_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int row_pitch,
                              int image_rows /* rows between consecutive images in memory, >= H; 0 = H */,
@@ -291,7 +305,7 @@ int pcnn_conv_tc_plan_destroy(pcnn_ctx *ctx, pcnn_conv_plan *plan);
 int pcnn_conv_tc_plan_info(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows, int *out5);
 int pcnn_conv_tc_fwd(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *x_bf16_dev, void *y_bf16_dev);
 /* Forward for wide channel counts (csrc/conv_wide_tc.cu): the same contract as pcnn_conv_tc_plan_create_strided (x NHWC bf16 with
- * row_pitch and image_rows, filters fp32 KRSC rounded to bf16 here or by pcnn_conv_plan_set_params, optional bias, act 0 none / 1 sigmoid, y dense NHWC bf16
+ * row_pitch and image_rows, filters fp32 KRSC rounded to bf16 here or by pcnn_conv_plan_set_params, optional bias, act 0 none / 1 sigmoid / 3 ReLU, y dense NHWC bf16
  * [N][(H-R)/stride+1][(W-S)/stride+1][K], pad columns and pad rows of x ignored, NaN included), computed as a tap-major implicit
  * GEMM on wgmma with the channels as the reduction.  The plan is run by pcnn_conv_tc_fwd (which then also needs y 16-byte aligned)
  * and freed by pcnn_conv_tc_plan_destroy.  Its domain is exactly the shapes that
@@ -325,7 +339,7 @@ int pcnn_conv_wide_bwd_info(int N, int H, int W, int C, int K, int R, int S, int
 /* The same five with a symmetric zero padding of pad_h rows and pad_w columns, as torch.nn.functional.conv2d(padding=(pad_h, pad_w)):
  * with x~ = x inside the H x W image and 0 outside it,
  *     P = (H + 2 pad_h - R) / stride + 1,   Q = (W + 2 pad_w - S) / stride + 1
- *     y[n][p][q][k]  = b[k] + sum_{r,s,c} x~[n][p*stride + r - pad_h][q*stride + s - pad_w][c] * f[k][r][s][c]   (then sigmoid if act)
+ *     y[n][p][q][k]  = b[k] + sum_{r,s,c} x~[n][p*stride + r - pad_h][q*stride + s - pad_w][c] * f[k][r][s][c]   (then act)
  *     dw[k][r][s][c] = sum_{n,p,q} dy[n][p][q][k] * x~[n][p*stride + r - pad_h][q*stride + s - pad_w][c]
  *     dx[n][h][w][c] = sum_{k,r,s} dy[n][(h + pad_h - r)/stride][(w + pad_w - s)/stride][k] * f[k][r][s][c]
  *                      over the (r, s) that divide exactly and give a dy pixel inside P x Q:
@@ -407,16 +421,21 @@ int pcnn_f32_to_bf16_rows(pcnn_ctx *ctx, const float *src_dev, void *dst_bf16_de
  * filters (uploaded to a temporary device buffer first): a plan refreshed with f holds the same operand bits as a plan created
  * from f.  A NaN filter stays a NaN; its payload is whatever __float2bfloat16_rn makes of it. */
 int pcnn_conv_plan_set_params(pcnn_ctx *ctx, pcnn_conv_plan *plan, const float *filt_f32_dev, const float *bias_f32_dev);
-/* The sigmoid derivative and the bias gradient of a convolution layer in one pass over dy.  y, dy and dpre are dense bf16
- * [pixels][K] (pixels = N * P * Q, the layout both forwards write and the gradients read as dy).
+/* The activation derivative and the bias gradient of a convolution or linear layer in one pass over dy.  y, dy and dpre are
+ * dense bf16 [pixels][K] (pixels = N * P * Q, the layout both forwards write and the gradients read as dy).
  *   act 1: dpre = bf16_rn(float(dy) * (float(y) * (1 - float(y)))), in exactly this order, fp32 round to nearest with no
  *          contraction: the derivative at the pre-activation whose sigmoid the forward stored.  y and dpre must not be NULL.
+ *   act 3: dpre = float(y) <= 0 ? +0 : dy, dy's bits passed through with no arithmetic: the ReLU derivative on the output the
+ *          forward stored, as torch's threshold_backward(dy, y, 0) (a NaN y passes dy; y = +-0 gives +0).  y and dpre must
+ *          not be NULL.
  *   act 0: dpre must be NULL and y is not read; only db is computed, over dy.
  *   db[k] = sum over the pixels of float(dpre[pixel][k]) (of dy at act 0): the bf16 values the weight and input gradients consume,
  *          accumulated in fp32 in a fixed order (per-CTA partials over pixel ranges that depend only on pixels and K, then a
- *          fixed-order pass over them, no atomics): reruns and every H100 give the same bits.  db may be NULL at act 1 (no bias).
- * dpre == dy (in place) is allowed; no other overlap is.  Domain: 1 <= K <= 256, pixels >= 1, act 0 or 1, every pointer 16-byte
- * aligned; anything else is PCNN_ERR_ARG with the rule in the message.  Elements past pixels * K are never written. */
+ *          fixed-order pass over them, no atomics): reruns and every H100 give the same bits.  db may be NULL at act 1 and 3
+ *          (no bias).
+ * dpre == dy (in place) is allowed; no other overlap is.  Domain: 1 <= K <= 256, pixels >= 1, act 0, 1 or 3 (PCNN_ACT_*), every
+ * pointer 16-byte aligned; anything else is PCNN_ERR_ARG with the rule in the message.  Elements past pixels * K are never
+ * written. */
 int pcnn_conv_bias_act_bwd(pcnn_ctx *ctx, const void *y_bf16_dev, const void *dy_bf16_dev, void *dpre_bf16_dev, float *db_f32_dev,
                            long pixels, int K, int act);
 /* Max pooling between convolution layers (csrc/pool_nhwc.cu), as torch.nn.functional.max_pool2d with ceil_mode=False and
@@ -457,8 +476,8 @@ int pcnn_maxpool_nhwc_info(int N, int H, int W, int C, int R, int S, int stride,
  *     pool writes as y.  A previous linear layer's y is the same with P = Q = 1, C = its O, row_pitch = O, image_rows 1.
  *   - F = P Q C features in NHWC order; W fp32 [O][P][Q][C] (KRSC with K = O, R = P, S = Q), b fp32 [O];
  *   - y, dy are dense bf16 [N][O]; dW is fp32 [O][P][Q][C].
- * pcnn_linear_plan_create returns a pcnn_conv_plan: pcnn_conv_tc_fwd runs it, y[n][o] = act(b[o] + sum_f x[n][f] W[o][f]) (act 1 is
- * the sigmoid of the conv forwards), pcnn_conv_plan_set_params refreshes W (fp32 [O][P][Q][C]) and b from device memory, and
+ * pcnn_linear_plan_create returns a pcnn_conv_plan: pcnn_conv_tc_fwd runs it, y[n][o] = act(b[o] + sum_f x[n][f] W[o][f]) (the
+ * activations of the conv forwards, PCNN_ACT_*), pcnn_conv_plan_set_params refreshes W (fp32 [O][P][Q][C]) and b from device memory, and
  * pcnn_conv_tc_plan_destroy frees it.  The plan holds W rounded to bf16 (round to nearest even, on the device).
  * pcnn_linear_wgrad: dW[o][f] = sum_n dy[n][o] x[n][f], fp32.  pcnn_linear_dgrad: dx[n][f] = sum_o dy[n][o] Wbf16[o][f], rounded to
  * bf16 once, written in x's layout: exactly the dy pcnn_maxpool_nhwc_bf16_bwd reads, or a previous linear layer's dy.  dx uses the
@@ -468,10 +487,10 @@ int pcnn_maxpool_nhwc_info(int N, int H, int W, int C, int R, int S, int stride,
  * every image are fully written.  Reductions may be split into ranges whose fp32 partials are added in a fixed order; the
  * split depends on the shape only, so reruns and every H100 give the same bits.  All calls are stream-ordered.
  * Domain (anything else is PCNN_ERR_ARG with the rule in the message, the same for the create call and the query):
- *   - N, P, Q, C >= 1, 1 <= O <= 256 (the limit of pcnn_conv_bias_act_bwd, which serves as the layer's bias / sigmoid backward);
+ *   - N, P, Q, C >= 1, 1 <= O <= 256 (the limit of pcnn_conv_bias_act_bwd, which serves as the layer's bias / activation backward);
  *   - F <= 2^24;
  *   - row_pitch 0 = Q C rounded up to a multiple of 8, otherwise >= Q C and a multiple of 8 (so a hidden width that feeds another
- *     linear layer must be a multiple of 8); image_rows 0 = P, otherwise >= P;  act 0 (none) or 1 (sigmoid);
+ *     linear layer must be a multiple of 8); image_rows 0 = P, otherwise >= P;  act 0 (none), 1 (sigmoid) or 3 (ReLU);
  *   - every device pointer 16-byte aligned.
  * pcnn_linear_info: host only (no GPU, no context).  out12 = { row pitch used, 128-image tiles, forward reduction steps (64-feature
  * chunks), forward splits, forward stages, weight-gradient chunk pairs, weight-gradient splits (image ranges), weight-gradient

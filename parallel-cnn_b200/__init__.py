@@ -9,7 +9,7 @@ The directory name contains a hyphen, so import it through ``pcnn_loader.load()`
 it as the module ``parallel_cnn_b200``).
 """
 from ._lib import (  # noqa: F401
-    LIB_PATH, NPARAM, OFF, PcnnError, U8, F32, TRAIN_SET, TEST_SET, MODE_AUTO, MODE_GRAPH, MODE_PERSISTENT,
+    LIB_PATH, NPARAM, OFF, PcnnError, U8, F32, TRAIN_SET, TEST_SET, MODE_AUTO, MODE_GRAPH, MODE_PERSISTENT, ACT_NONE, ACT_SIGMOID, ACT_RELU,
     lib, declared_symbols, init_params_reference, mnist_load_u8, conv_tc_plan_info, conv_wide_plan_info, conv_wide_bwd_info,
     conv_bwd_plan_info, conv_layer_family, maxpool_nhwc_info, linear_info,
 )
@@ -17,4 +17,4 @@ from .engine import ConvLayer, ConvPlan, LinearLayer, LinearPlan, MaxPoolLayer, 
 
 __all__ = ["Engine", "DeviceArray", "PcnnError", "lib", "declared_symbols", "init_params_reference",
            "mnist_load_u8", "conv_tc_plan_info", "conv_wide_plan_info", "conv_wide_bwd_info", "conv_bwd_plan_info", "conv_layer_family", "maxpool_nhwc_info", "linear_info", "ConvLayer", "MaxPoolLayer", "LinearLayer", "ConvPlan", "LinearPlan",
-           "WideConvPlan", "NPARAM", "OFF", "U8", "F32", "TRAIN_SET", "TEST_SET", "LIB_PATH"]
+           "WideConvPlan", "NPARAM", "OFF", "U8", "F32", "TRAIN_SET", "TEST_SET", "LIB_PATH", "ACT_NONE", "ACT_SIGMOID", "ACT_RELU"]

@@ -15,6 +15,7 @@ OFF = dict(c1w=(0, 150), c1b=(150, 156), s1w=(156, 172), s1b=(172, 173), fw=(173
 U8, F32 = 0, 1
 MODE_AUTO, MODE_GRAPH, MODE_PERSISTENT = 0, 1, 2
 TRAIN_SET, TEST_SET = 0, 1
+ACT_NONE, ACT_SIGMOID, ACT_RELU = 0, 1, 3     # PCNN_ACT_*: the `act` of the device-trained layers (2 is not a code)
 
 
 class PcnnError(RuntimeError):

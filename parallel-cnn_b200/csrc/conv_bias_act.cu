@@ -1,12 +1,13 @@
-// parallel-cnn_b200/csrc/conv_bias_act.cu -- the gradient at the pre-activation and the bias gradient of a convolution layer
-// (pcnn_conv_bias_act_bwd), in one pass over dy:
+// parallel-cnn_b200/csrc/conv_bias_act.cu -- the gradient at the pre-activation and the bias gradient of a convolution or linear
+// layer (pcnn_conv_bias_act_bwd), in one pass over dy:
 //     dpre = bf16_rn(dy * (y * (1 - y)))      (act 1: y is the sigmoid output the forward stored; fp32, no contraction)
+//     dpre = float(y) <= 0 ? +0 : dy          (act 3: y is the ReLU output; dy's bits pass through, a NaN y passes dy)
 //     db[k] = sum over pixels of float(dpre[pixel][k])      (of dy at act 0)
 // so db sums exactly the bf16 values the weight and input gradients consume.
 //
-// The pass is HBM-bound (read y and dy, write dpre).  With K % 8 == 0 a thread moves 16-byte vectors of 8 channels of one
-// pixel, otherwise single elements.  A CTA owns the fixed pixel range [b * BA_ITERS * lanes, (b + 1) * BA_ITERS * lanes):
-// thread t keeps channel group g = t % G of pixel lane t / G (G = K / VEC groups, lanes = 256 / G), so its VEC accumulators
+// The pass is HBM-bound (read y and dy, write dpre: the same bytes at act 1 and 3).  With K % 8 == 0 a thread moves 16-byte
+// vectors of 8 channels of one pixel, otherwise single elements.  A CTA owns the fixed pixel range
+// [b * BA_ITERS * lanes, (b + 1) * BA_ITERS * lanes): thread t keeps channel group g = t % G of pixel lane t / G (G = K / VEC groups, lanes = 256 / G), so its VEC accumulators
 // stay on the same channels over its BA_ITERS pixels, which are loaded before any is stored (in place, dpre == dy, each element
 // is read and written by one thread).  The lanes' sums go through shared memory into the CTA's slot [b][K] in lane order, and
 // pcnn_conv_wgrad_reduce_slots adds the slots in a fixed order.  Nothing depends on the SM count: the bits of db are the same
@@ -54,8 +55,13 @@ __global__ void __launch_bounds__(BA_THREADS) k_conv_bias_act_bwd(const __nv_bfl
                 if (ACT) {
 #pragma unroll
                     for (int i = 0; i < VEC; ++i) {
-                        const float yf = __bfloat162float(yv[j].h[i]), gf = __bfloat162float(gv[j].h[i]);
-                        d.h[i] = __float2bfloat16_rn(__fmul_rn(gf, __fmul_rn(yf, __fsub_rn(1.0f, yf))));
+                        const float yf = __bfloat162float(yv[j].h[i]);
+                        if (ACT == PCNN_ACT_SIGMOID) {
+                            const float gf = __bfloat162float(gv[j].h[i]);
+                            d.h[i] = __float2bfloat16_rn(__fmul_rn(gf, __fmul_rn(yf, __fsub_rn(1.0f, yf))));
+                        }
+                        else if (yf <= 0.0f)                     // ReLU: d keeps dy's bits where y > 0 or NaN
+                            d.h[i] = __ushort_as_bfloat16((unsigned short)0);
                     }
                     *reinterpret_cast<BfVec<VEC> *>(dpre + px * K + g * VEC) = d;
                 }
@@ -90,19 +96,20 @@ extern "C" int pcnn_conv_bias_act_bwd(pcnn_ctx *ctx, const void *y_bf16, const v
                                       int K, int act) {
     const char *fn = "pcnn_conv_bias_act_bwd";
     PCNN_REQUIRE(ctx && dy_bf16, PCNN_ERR_ARG, "%s: NULL context or dy", fn);
-    PCNN_REQUIRE(act == 0 || act == 1, PCNN_ERR_ARG, "%s: act %d is not 0 (none) or 1 (sigmoid)", fn, act);
+    PCNN_REQUIRE_ACT(fn, act);
     PCNN_REQUIRE(K >= 1 && K <= 256, PCNN_ERR_ARG, "%s: K = %d filters: 1 <= K <= 256 is required", fn, K);
     PCNN_REQUIRE(pixels >= 1, PCNN_ERR_ARG, "%s: pixels = %ld: at least one pixel (N * P * Q) is required", fn, pixels);
-    if (act == 1)
-        PCNN_REQUIRE(y_bf16 && dpre_bf16, PCNN_ERR_ARG, "%s: act 1 (sigmoid) needs y, the forward's output, and dpre (NULL given)", fn);
+    if (act != PCNN_ACT_NONE)
+        PCNN_REQUIRE(y_bf16 && dpre_bf16, PCNN_ERR_ARG, "%s: act %d (%s) needs y, the forward's output, and dpre (NULL given)", fn,
+                     act, act == PCNN_ACT_SIGMOID ? "sigmoid" : "ReLU");
     else
         PCNN_REQUIRE(!dpre_bf16 && db_f32, PCNN_ERR_ARG,
                      "%s: act 0 writes no dpre (it must be NULL) and computes db only (it must not be NULL)", fn);
-    const void *ptrs[4] = {act == 1 ? y_bf16 : nullptr, dy_bf16, dpre_bf16, db_f32};
+    const void *y = act != PCNN_ACT_NONE ? y_bf16 : nullptr;
+    const void *ptrs[4] = {y, dy_bf16, dpre_bf16, db_f32};
     for (const void *q : ptrs)
         PCNN_REQUIRE(((uintptr_t)q & 15) == 0, PCNN_ERR_ARG, "%s: y, dy, dpre and db must be 16-byte aligned", fn);
     const size_t bytes = (size_t)pixels * K * 2, db_bytes = (size_t)K * sizeof(float);
-    const void *y = act == 1 ? y_bf16 : nullptr;
     PCNN_REQUIRE((dpre_bf16 == dy_bf16 || !overlap(dpre_bf16, bytes, dy_bf16, bytes)) && !overlap(dpre_bf16, bytes, y, bytes) &&
                      !overlap(db_f32, db_bytes, y, bytes) && !overlap(db_f32, db_bytes, dy_bf16, bytes) &&
                      !overlap(db_f32, db_bytes, dpre_bf16, bytes),
@@ -118,9 +125,10 @@ extern "C" int pcnn_conv_bias_act_bwd(pcnn_ctx *ctx, const void *y_bf16, const v
         int rc = pcnn_scratch(ctx, (size_t)ctas * K * sizeof(float), (void **)&slots);
         if (rc) return rc;
     }
-    static const bias_act_fn table[2][2] = {{k_conv_bias_act_bwd<1, 0>, k_conv_bias_act_bwd<1, 1>},
-                                            {k_conv_bias_act_bwd<8, 0>, k_conv_bias_act_bwd<8, 1>}};
-    table[vec ? 1 : 0][act]<<<(unsigned)ctas, BA_THREADS, 0, ctx->stream>>>(
+    static const bias_act_fn table[2][3] = {
+        {k_conv_bias_act_bwd<1, PCNN_ACT_NONE>, k_conv_bias_act_bwd<1, PCNN_ACT_SIGMOID>, k_conv_bias_act_bwd<1, PCNN_ACT_RELU>},
+        {k_conv_bias_act_bwd<8, PCNN_ACT_NONE>, k_conv_bias_act_bwd<8, PCNN_ACT_SIGMOID>, k_conv_bias_act_bwd<8, PCNN_ACT_RELU>}};
+    table[vec ? 1 : 0][pcnn_act_col(act)]<<<(unsigned)ctas, BA_THREADS, 0, ctx->stream>>>(
         static_cast<const __nv_bfloat16 *>(y), static_cast<const __nv_bfloat16 *>(dy_bf16), static_cast<__nv_bfloat16 *>(dpre_bf16),
         slots, pixels, K);
     PCNN_CHECK_LAUNCH(ctx);

@@ -15,7 +15,7 @@
 //   * B = R matrices [Qt*K x 32] (<= 48 KB) built on the device from the filter bank (k_conv_tc_toeplitz, at creation and by
 //     pcnn_conv_plan_set_params), resident in shared memory;
 //   * D = [128 x Qt*K] fp32 in the registers of two warpgroups (64 rows each, N = Qt*K rounded up to 32 <= 256);
-//   * per tile and warpgroup 2*R wgmma (M=64, N, K=16), then the epilogue (bias, optional sigmoid, bf16 pack, store)
+//   * per tile and warpgroup 2*R wgmma (M=64, N, K=16), then the epilogue (bias, activation, bf16 pack, store)
 //     straight from the accumulator registers while the producer warp already stages the next tiles.
 // Density: LeNet c1 (C=1, K=6, 5x5, Qt=24): 25/32 of K and 6*24/144 of N are useful but the band itself is sparse
 // (17 % of the issued MACs are useful); config 5 (C=3, K=64, 3x3, Qt=4): 28 %.  The tensor pipe has > 10x headroom over
@@ -51,7 +51,7 @@ struct ConvTcParams {
                                    // requirement on the global address), the remainder (q0*C) % 8 selects the variant
     int stages;                    // activation stages that fit next to the V * R Toeplitz matrices
     int n_mtiles, n_qtiles;
-    int act;                       // 0: none, 1: sigmoid (the reference's activation, layer.h:81-83)
+    int act;                       // PCNN_ACT_*: 0 none, 1 sigmoid (the reference's activation, layer.h:81-83), 3 ReLU
     long long y_row_elems;         // Q * K
     __nv_bfloat16 *y;
     const float *bias;             // [K] or null
@@ -77,7 +77,8 @@ static size_t conv_tc_smem_bytes(int V, int R, int npad, int stages) {
     return (size_t)V * R * npad * TC_KCHUNK * 2 + (size_t)stages * R * A_TILE_BYTES + sizeof(ConvTcCtl) + 1024;
 }
 
-// ACT (0 none, 1 sigmoid) and the MMA width N are compile-time; a missing bias reads as zeros from the shared bias table
+// ACT (PCNN_ACT_*: 0 none, 1 sigmoid, 3 ReLU) and the MMA width N are compile-time; a missing bias reads as zeros from the
+// shared bias table
 template <int ACT, int N>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_conv_tc_fwd(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_b, const ConvTcParams p) {
@@ -161,7 +162,7 @@ k_conv_tc_fwd(const __grid_constant__ CUtensorMap map_x, const __grid_constant__
                 float2 bb;
                 asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(bb.x), "=f"(bb.y) : "r"(bias_s + (uint32_t)c * 4u));
                 f0 += bb.x; f1 += bb.y;
-                if (ACT == 1) { f0 = sigmoid_bf16(f0); f1 = sigmoid_bf16(f1); }
+                f0 = apply_act<ACT>(f0); f1 = apply_act<ACT>(f1);
                 if (c + 1 < valid_cols && ((reinterpret_cast<uintptr_t>(yrow + c) & 3) == 0)) {
                     *reinterpret_cast<__nv_bfloat162 *>(yrow + c) = __floats2bfloat162_rn(f0, f1);
                 } else {
@@ -174,11 +175,11 @@ k_conv_tc_fwd(const __grid_constant__ CUtensorMap map_x, const __grid_constant__
 }
 
 typedef void (*conv_tc_fwd_fn)(const CUtensorMap, const CUtensorMap, const ConvTcParams);
-#define PCNN_FWD_ROW(N) {k_conv_tc_fwd<0, N>, k_conv_tc_fwd<1, N>}
-static const void *conv_tc_fwd_variant(bool sigmoid, int npad) {
-    static const conv_tc_fwd_fn table[8][2] = {PCNN_FWD_ROW(32),  PCNN_FWD_ROW(64),  PCNN_FWD_ROW(96),  PCNN_FWD_ROW(128),
+#define PCNN_FWD_ROW(N) {k_conv_tc_fwd<PCNN_ACT_NONE, N>, k_conv_tc_fwd<PCNN_ACT_SIGMOID, N>, k_conv_tc_fwd<PCNN_ACT_RELU, N>}
+static const void *conv_tc_fwd_variant(int act, int npad) {
+    static const conv_tc_fwd_fn table[8][3] = {PCNN_FWD_ROW(32),  PCNN_FWD_ROW(64),  PCNN_FWD_ROW(96),  PCNN_FWD_ROW(128),
                                                PCNN_FWD_ROW(160), PCNN_FWD_ROW(192), PCNN_FWD_ROW(224), PCNN_FWD_ROW(256)};
-    return reinterpret_cast<const void *>(table[npad / 32 - 1][sigmoid ? 1 : 0]);
+    return reinterpret_cast<const void *>(table[npad / 32 - 1][pcnn_act_col(act)]);
 }
 #undef PCNN_FWD_ROW
 
@@ -337,6 +338,7 @@ extern "C" int pcnn_conv_tc_plan_create_strided(pcnn_ctx *ctx, int N, int H, int
                                                 int image_rows, int act, const float *filt_host, const float *bias_host,
                                                 pcnn_conv_plan **out) {
     PCNN_REQUIRE(ctx && filt_host && out, PCNN_ERR_ARG, "pcnn_conv_tc_plan_create: NULL argument");
+    PCNN_REQUIRE_ACT("pcnn_conv_tc_plan_create", act);
     ConvTcShape sh;
     int rc = conv_tc_shape(N, H, W, C, K, R, S, stride, row_pitch, image_rows, &sh);
     if (rc) return rc;
@@ -375,9 +377,10 @@ extern "C" int pcnn_conv_tc_plan_create_strided(pcnn_ctx *ctx, int N, int H, int
     if (rc) return rc;
     static bool configured[64] = {};        // function attributes are per device
     if (!configured[ctx->device & 63]) {
-        for (int v = 0; v < 16; ++v)
-            PCNN_CUDA(cudaFuncSetAttribute(conv_tc_fwd_variant(v & 1, 32 * (v / 2 + 1)), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           TC_SMEM_BUDGET + 2048));
+        for (int npad = 32; npad <= 256; npad += 32)
+            for (int a : {PCNN_ACT_NONE, PCNN_ACT_SIGMOID, PCNN_ACT_RELU})
+                PCNN_CUDA(cudaFuncSetAttribute(conv_tc_fwd_variant(a, npad), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               TC_SMEM_BUDGET + 2048));
         configured[ctx->device & 63] = true;
     }
     guard.p = nullptr;
@@ -440,7 +443,7 @@ extern "C" int pcnn_conv_tc_fwd(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void 
     const int ntiles = p.n_mtiles * p.n_qtiles;
     const int grid = ntiles < ctx->sm_count ? ntiles : ctx->sm_count;
     void *args[] = {&map_x, &plan->map_b, &p};
-    PCNN_CUDA(cudaLaunchKernel(conv_tc_fwd_variant(p.act == 1, p.npad), dim3((unsigned)grid), dim3(TC_THREADS), args,
+    PCNN_CUDA(cudaLaunchKernel(conv_tc_fwd_variant(p.act, p.npad), dim3((unsigned)grid), dim3(TC_THREADS), args,
                                conv_tc_smem_bytes(p.V, p.R, p.npad, p.stages), ctx->stream));
     PCNN_CHECK_LAUNCH(ctx);
     return PCNN_OK;

@@ -14,8 +14,8 @@
 //   * B: the filters rounded to bf16 on the device (at creation and by pcnn_conv_plan_set_params), KRSC, viewed as {C, R*S, K}: a box {64, 1, Npad} is the K-major
 //     operand of one step; channels >= C and filters >= K are zero-filled by TMA, and a box never reaches the next tap.
 //   * D: [128 x Npad] fp32 in the registers of two warpgroups (rows 0-63 / 64-127 of the block), Npad = K rounded up to 16.
-//   * Epilogue: bias, optional sigmoid, bf16, written to a shared staging tile per warpgroup (SWIZZLE_128B, conflict-free),
-//     then stored by TMA through a map of y {K, Q, P, N} that clips pixels outside the image and channels >= K.  The store
+//   * Epilogue: bias, activation (none, sigmoid or ReLU), bf16, written to a shared staging tile per warpgroup (SWIZZLE_128B,
+//     conflict-free), then stored by TMA through a map of y {K, Q, P, N} that clips pixels outside the image and channels >= K.  The store
 //     drains while the warpgroup already runs the next tile's MMAs; the staging tile is reused once its store has been read.
 // Pixel blocks on small images issue more pixels than they compute: pcnn_conv_wide_plan_info reports both.
 //
@@ -158,7 +158,7 @@ k_conv_wide_fwd(const __grid_constant__ ConvWideMaps m, const ConvWideParams p) 
                 float2 bb;
                 asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(bb.x), "=f"(bb.y) : "r"(bias_s + (uint32_t)c * 4u));
                 f0 += bb.x; f1 += bb.y;
-                if (ACT == 1) { f0 = sigmoid_bf16(f0); f1 = sigmoid_bf16(f1); }
+                f0 = apply_act<ACT>(f0); f1 = apply_act<ACT>(f1);
                 __nv_bfloat162 v = __floats2bfloat162_rn(f0, f1);
                 // sub-tile j / 8 holds channels 64 (j / 8) ..; 16-byte chunk j % 8 of the row, XOR-swizzled by row % 8 (SWIZZLE_128B)
                 const uint32_t addr = stg_s + (uint32_t)((j / 8) * WD_STG_BYTES + row * 128 + (((j % 8) ^ (row & 7)) << 4) + (lane & 3) * 4);
@@ -179,13 +179,14 @@ k_conv_wide_fwd(const __grid_constant__ ConvWideMaps m, const ConvWideParams p) 
 }
 
 typedef void (*conv_wide_fn)(const ConvWideMaps, const ConvWideParams);
-#define PCNN_WIDE_ROW(N) {k_conv_wide_fwd<0, N>, k_conv_wide_fwd<1, N>}
-static const void *conv_wide_variant(bool sigmoid, int npad) {
-    static const conv_wide_fn table[16][2] = {
+#define PCNN_WIDE_ROW(N) \
+    {k_conv_wide_fwd<PCNN_ACT_NONE, N>, k_conv_wide_fwd<PCNN_ACT_SIGMOID, N>, k_conv_wide_fwd<PCNN_ACT_RELU, N>}
+static const void *conv_wide_variant(int act, int npad) {
+    static const conv_wide_fn table[16][3] = {
         PCNN_WIDE_ROW(16),  PCNN_WIDE_ROW(32),  PCNN_WIDE_ROW(48),  PCNN_WIDE_ROW(64),  PCNN_WIDE_ROW(80),  PCNN_WIDE_ROW(96),
         PCNN_WIDE_ROW(112), PCNN_WIDE_ROW(128), PCNN_WIDE_ROW(144), PCNN_WIDE_ROW(160), PCNN_WIDE_ROW(176), PCNN_WIDE_ROW(192),
         PCNN_WIDE_ROW(208), PCNN_WIDE_ROW(224), PCNN_WIDE_ROW(240), PCNN_WIDE_ROW(256)};
-    return reinterpret_cast<const void *>(table[npad / 16 - 1][sigmoid ? 1 : 0]);
+    return reinterpret_cast<const void *>(table[npad / 16 - 1][pcnn_act_col(act)]);
 }
 #undef PCNN_WIDE_ROW
 
@@ -335,7 +336,7 @@ static int wide_plan_create(const char *fn, pcnn_ctx *ctx, int N, int H, int W, 
                             int pad_w, int row_pitch, int image_rows, int act, const float *filt_host, const float *bias_host,
                             pcnn_conv_plan **out) {
     PCNN_REQUIRE(ctx && filt_host && out, PCNN_ERR_ARG, "%s: NULL argument", fn);
-    PCNN_REQUIRE(act == 0 || act == 1, PCNN_ERR_ARG, "%s: act %d is not 0 (none) or 1 (sigmoid)", fn, act);
+    PCNN_REQUIRE_ACT(fn, act);
     ConvWideShape sh;
     int rc = conv_wide_shape(fn, N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows, &sh);
     if (rc) return rc;
@@ -375,9 +376,10 @@ static int wide_plan_create(const char *fn, pcnn_ctx *ctx, int N, int H, int W, 
     }
     static bool configured[64] = {};        // function attributes are per device
     if (!configured[ctx->device & 63]) {
-        for (int v = 0; v < 32; ++v)
-            PCNN_CUDA(cudaFuncSetAttribute(conv_wide_variant(v & 1, 16 * (v / 2 + 1)), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           WD_SMEM_BUDGET + 2048));
+        for (int npad = 16; npad <= 256; npad += 16)
+            for (int a : {PCNN_ACT_NONE, PCNN_ACT_SIGMOID, PCNN_ACT_RELU})
+                PCNN_CUDA(cudaFuncSetAttribute(conv_wide_variant(a, npad), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               WD_SMEM_BUDGET + 2048));
         configured[ctx->device & 63] = true;
     }
     *out = conv_plan_wrap_wide(pl);
@@ -419,7 +421,7 @@ int conv_wide_fwd(pcnn_ctx *ctx, const ConvWidePlan *pl, const void *x_bf16, voi
     ConvWideParams p = pl->p;
     const int grid = p.tiles < ctx->sm_count ? p.tiles : ctx->sm_count;
     void *args[] = {&m, &p};
-    PCNN_CUDA(cudaLaunchKernel(conv_wide_variant(pl->act == 1, sh.npad), dim3((unsigned)grid), dim3(WD_THREADS), args,
+    PCNN_CUDA(cudaLaunchKernel(conv_wide_variant(pl->act, sh.npad), dim3((unsigned)grid), dim3(WD_THREADS), args,
                                wide_smem_bytes(sh.npad, p.stages), ctx->stream));
     PCNN_CHECK_LAUNCH(ctx);
     return PCNN_OK;

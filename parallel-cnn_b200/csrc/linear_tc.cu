@@ -12,7 +12,8 @@
 //     inner extent is Q*C, not the pitch, so pad columns and pad rows are never read.  B: a box {64, 1, Npad} of the bf16
 //     weights viewed as {Q*C, P, O}, K-major.  Both SWIZZLE_128B.  Split: the chunks are cut into `splits` ranges, each unit
 //     (image tile, range) writes fp32 partials into slot [range][N][O] and k_linear_fwd_reduce adds them in range order, then
-//     applies bias and activation.  Unsplit, the epilogue does that from the registers.  y is written with masked stores.
+//     applies bias and activation (none, sigmoid or ReLU: a run-time branch, no extra instantiation).  Unsplit, the epilogue
+//     does that from the registers.  y is written with masked stores.
 //   * Weight gradient  dW[o][f] = sum_n dy[n][o] x[n][f]:  M = 64 features of one chunk per warpgroup, N = O rounded up to 64,
 //     reduction over images, 16 per m64nNk16.  A: the forward's x box (128 image rows of 64 features, MN-major).  B: boxes
 //     {64 outputs, 128 images} of dy, MN-major.  A unit is a pair of chunks and a range of 128-image blocks; ranges > 1 write
@@ -138,7 +139,8 @@ k_linear_fwd(const __grid_constant__ LinearMaps m, const LinearFwdParams p) {
                 p.slots[((size_t)sp * p.N + n) * p.O + o] = acc[i];
             } else {
                 float v = p.bias ? __fadd_rn(acc[i], p.bias[o]) : acc[i];
-                if (p.act == 1) v = sigmoid_bf16(v);
+                if (p.act == PCNN_ACT_SIGMOID) v = sigmoid_bf16(v);
+                else if (p.act == PCNN_ACT_RELU) v = relu_f32(v);
                 p.y[(size_t)n * p.O + o] = __float2bfloat16_rn(v);
             }
         }
@@ -152,7 +154,8 @@ __global__ void __launch_bounds__(256) k_linear_fwd_reduce(const float *__restri
         float v = slots[i];
         for (int s = 1; s < splits; ++s) v = __fadd_rn(v, slots[(size_t)s * total + i]);
         if (bias) v = __fadd_rn(v, bias[i % O]);
-        if (act == 1) v = sigmoid_bf16(v);
+        if (act == PCNN_ACT_SIGMOID) v = sigmoid_bf16(v);
+        else if (act == PCNN_ACT_RELU) v = relu_f32(v);
         y[i] = __float2bfloat16_rn(v);
     }
 }
@@ -564,7 +567,7 @@ extern "C" int pcnn_linear_plan_create(pcnn_ctx *ctx, int N, int P, int Q, int C
                                        const float *w_host, const float *b_host, pcnn_conv_plan **out) {
     const char *fn = "pcnn_linear_plan_create";
     PCNN_REQUIRE(ctx && w_host && out, PCNN_ERR_ARG, "%s: NULL argument", fn);
-    PCNN_REQUIRE(act == 0 || act == 1, PCNN_ERR_ARG, "%s: act %d is not 0 (none) or 1 (sigmoid)", fn, act);
+    PCNN_REQUIRE_ACT(fn, act);
     LinearShape s;
     int rc = linear_shape(N, P, Q, C, O, row_pitch, image_rows, &s);
     if (rc) return rc;

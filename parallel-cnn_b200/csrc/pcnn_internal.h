@@ -164,6 +164,13 @@ int pcnn_fail_cuda(cudaError_t e, const char *what, const char *file, int line);
     do {                                                                         \
         if (!(cond)) { pcnn_set_error(__VA_ARGS__); return (code); }             \
     } while (0)
+// the activation codes (PCNN_ACT_* of pcnn.h) every create call and pcnn_conv_bias_act_bwd take; any other is refused with
+// this message, `fn` naming the called function
+#define PCNN_REQUIRE_ACT(fn, act)                                                                                              \
+    PCNN_REQUIRE((act) == PCNN_ACT_NONE || (act) == PCNN_ACT_SIGMOID || (act) == PCNN_ACT_RELU, PCNN_ERR_ARG,                 \
+                 "%s: act %d is not 0 (none), 1 (sigmoid) or 3 (ReLU)", fn, act)
+// column of a kernel table with one instantiation per activation: none, sigmoid, ReLU
+inline int pcnn_act_col(int act) { return act == PCNN_ACT_RELU ? 2 : act; }
 #define PCNN_CHECK_LAUNCH(ctx)                                                   \
     do {                                                                         \
         (ctx)->launches++;                                                       \

@@ -97,6 +97,18 @@ __device__ __forceinline__ float sigmoid_bf16(float x) {
     return fmaf(t, 0.5f, 0.5f);
 }
 
+// ReLU in fp32 before the one bf16 rounding: x < 0 ? +0 : x, so NaN and -0 pass unchanged as in torch.relu (fmaxf would turn
+// NaN into 0 and leaves the sign of a zero unspecified)
+__device__ __forceinline__ float relu_f32(float x) { return x < 0.0f ? 0.0f : x; }
+
+// the forward epilogues' activation (PCNN_ACT_*), applied to v = accumulator + bias before the bf16 rounding
+template <int ACT>
+__device__ __forceinline__ float apply_act(float v) {
+    if (ACT == PCNN_ACT_SIGMOID) return sigmoid_bf16(v);
+    if (ACT == PCNN_ACT_RELU) return relu_f32(v);
+    return v;
+}
+
 
 // ---- wgmma (Hopper warpgroup MMA: D[64 x N] fp32 in registers += A[64 x 16] * B[16 x N], operands in shared memory) ----------
 // Register layout of the accumulator float d[N / 2] of thread t of the warpgroup (warp w = t / 32, lane l = t % 32):

@@ -413,8 +413,9 @@ class Engine:
                        int(pitch), int(image_rows))
 
     def conv_bias_act_bwd(self, y, dy, dpre, db, pixels, K, act):
-        """pcnn_conv_bias_act_bwd: dpre = bf16(dy * y * (1 - y)) at act 1 (dpre may be dy itself), db[k] = sum of dpre (of dy at
-        act 0) over the pixels; dpre None at act 0, db None for a layer without bias"""
+        """pcnn_conv_bias_act_bwd: dpre = bf16(dy * y * (1 - y)) at act 1 (ACT_SIGMOID), dpre = (y <= 0 ? +0 : dy) at act 3
+        (ACT_RELU; dy's bits pass through, a NaN y passes dy); dpre may be dy itself.  db[k] = sum of dpre (of dy at act 0) over the
+        pixels; dpre None at act 0, db None for a layer without bias"""
         self._call("pcnn_conv_bias_act_bwd", _p(y), _p(dy), _p(dpre), _p(db), int(pixels), int(K), int(act))
 
     def maxpool_nhwc_fwd(self, x, y, argmax, N, H, W, Cin, R, S, stride, padding=(0, 0), row_pitch=None, image_rows=0):
@@ -454,7 +455,8 @@ class Engine:
 
 
 class ConvPlan:
-    """bf16 tensor-core convolution plan (pcnn_conv_tc_*): filters fp32 KRSC on the host, activations NHWC bf16."""
+    """bf16 tensor-core convolution plan (pcnn_conv_tc_*): filters fp32 KRSC on the host, activations NHWC bf16.  act is
+    ACT_NONE (0), ACT_SIGMOID (1) or ACT_RELU (3), fused after the bias; any other value is refused."""
 
     def __init__(self, engine, N, H, W, C, K, R, S, filt, bias=None, act=0, row_pitch=None, image_rows=0, stride=1):
         self.engine = engine
@@ -543,7 +545,7 @@ class ConvLayer:
     It owns fp32 master filters (KRSC) and bias, their gradients dw and db, all in DeviceArrays, and a forward plan of the family
     that serves the shape (conv_layer_family: the row-Toeplitz plan for few channels without padding, the wide plan otherwise).
     Activations are NHWC bf16: x with row_pitch (None = W*C rounded up to 8) and image_rows (0 = H), y and dy dense
-    [N][P][Q][K], dx in x's layout.  act 1 is a sigmoid after the bias."""
+    [N][P][Q][K], dx in x's layout.  act ACT_SIGMOID (1) is a sigmoid after the bias, ACT_RELU (3) a ReLU, ACT_NONE (0) none."""
 
     def __init__(self, engine, N, H, W, C, K, R, S, filt, bias=None, act=0, stride=1, padding=(0, 0), row_pitch=None, image_rows=0):
         self.engine = engine
@@ -576,8 +578,8 @@ class ConvLayer:
 
     def backward(self, y, dy, dx=None):
         """Gradients of the most recent forward, whose output y was: dw, db (with a bias) and dx (when given; a first layer
-        passes None).  dy is CONSUMED: with a sigmoid it is overwritten in place by the gradient at the pre-activation, which
-        the weight and input gradients then read (pcnn_conv_bias_act_bwd, skipped without sigmoid and bias)."""
+        passes None).  dy is CONSUMED: with a sigmoid or a ReLU it is overwritten in place by the gradient at the pre-activation,
+        which the weight and input gradients then read (pcnn_conv_bias_act_bwd, skipped without activation and bias)."""
         N, H, W, C, K, R, S = self.shape
         e = self.engine
         if self.act or self.bias is not None:
@@ -616,7 +618,8 @@ class LinearLayer:
 
     x is [N][image_rows][row_pitch] bf16 with P x Q pixels of C channels per image, which is what MaxPoolLayer writes as y (pass
     its row_pitch and image_rows) or, with P = Q = 1 and C = the previous O, what a LinearLayer writes (row_pitch = that O, a
-    multiple of 8).  y and dy are dense [N][O]; dx is written in x's layout.  act 1 is a sigmoid after the bias.  A LeNet-style
+    multiple of 8).  y and dy are dense [N][O]; dx is written in x's layout.  act ACT_SIGMOID (1) is a sigmoid after the bias,
+    ACT_RELU (3) a ReLU, ACT_NONE (0) none.  A LeNet-style
     classifier runs every pass on the engine's stream:
 
         conv1.forward(x, y1);  pool1.forward(y1, x2);  conv2.forward(x2, y2);  pool2.forward(y2, x3)
@@ -650,8 +653,8 @@ class LinearLayer:
 
     def backward(self, y, dy, dx=None):
         """Gradients of the most recent forward, whose output y was: dw, db (with a bias) and dx (when given).  dy is CONSUMED:
-        with a sigmoid it is overwritten in place by the gradient at the pre-activation (pcnn_conv_bias_act_bwd with pixels = N,
-        K = O; skipped without sigmoid and bias).  dx uses the plan's bf16 weights, so call it before sgd."""
+        with a sigmoid or a ReLU it is overwritten in place by the gradient at the pre-activation (pcnn_conv_bias_act_bwd with
+        pixels = N, K = O; skipped without activation and bias).  dx uses the plan's bf16 weights, so call it before sgd."""
         N, P, Q, C, O = self.shape
         e = self.engine
         if self.act or self.bias is not None:

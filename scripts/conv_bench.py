@@ -252,19 +252,23 @@ def run_wide_same(name, N, H, W, C, K, R, S, stride, pad, iters):
     del x, xc, y, dy, dx, dxc, xt, dyt
 
 
-def run_train(name, N, H, W, C, K, R, S, stride, pad, iters, with_dx=True):
-    """one training step of a ConvLayer (bias, sigmoid), pass by pass: forward, pcnn_conv_bias_act_bwd (out of place, so that every
-    launch sees the same dy), the family's weight and input gradients, sgd (two fp32 updates and pcnn_conv_plan_set_params), and
-    the whole ConvLayer step (forward, backward in place over dy, sgd).  bias_act_bwd moves 3 * pixels * K * 2 bytes (read y and
-    dy, write dpre), compared with 3.35 TB/s.  Next to it the torch eager step on bf16 channels-last tensors of the same shapes:
-    conv2d with bias, sigmoid, autograd backward with dy, then w -= lr * grad on fp32 masters and the re-cast to bf16."""
+def run_train(name, N, H, W, C, K, R, S, stride, pad, iters, with_dx=True, act=1):
+    """one training step of a ConvLayer (bias, sigmoid at act 1, ReLU at act 3), pass by pass: forward, pcnn_conv_bias_act_bwd (out
+    of place, so that every launch sees the same dy), the family's weight and input gradients, sgd (two fp32 updates and
+    pcnn_conv_plan_set_params), and the whole ConvLayer step (forward, backward in place over dy, sgd).  bias_act_bwd moves
+    3 * pixels * K * 2 bytes (read y and dy, write dpre), compared with 3.35 TB/s.  Next to it the torch eager step on bf16
+    channels-last tensors of the same shapes: conv2d with bias, the activation, autograd backward with dy, then w -= lr * grad on
+    fp32 masters and the re-cast to bf16.  At act 3 the forward of the same layer is also timed at act 0, 1 and 3, alternating
+    plans of the three codes (fwd_by_act: two rounds each)."""
     Hc, Wc = H + 2 * pad, W + 2 * pad
     P, Q = (Hc - R) // stride + 1, (Wc - S) // stride + 1
     f = rng.uniform(-0.5, 0.5, (K, R, S, C)).astype(np.float32)
     b = rng.uniform(-0.5, 0.5, K).astype(np.float32)
-    layer = pkg.ConvLayer(eng, N, H, W, C, K, R, S, f, b, act=1, stride=stride, padding=(pad, pad))
+    layer = pkg.ConvLayer(eng, N, H, W, C, K, R, S, f, b, act=act, stride=stride, padding=(pad, pad))
     pitch = layer.row_pitch
     x = torch.randint(0, 0x3F80, (N * H, pitch), dtype=torch.int16, device="cuda")   # positive bf16 bit patterns < 1.0
+    if act == pkg.ACT_RELU:                                                           # signed x: about half the outputs < 0
+        x ^= (torch.randint(0, 2, (N * H, pitch), dtype=torch.int16, device="cuda") << 15)
     y = torch.empty((N, P, Q, K), dtype=torch.int16, device="cuda")
     dy = torch.randint(0, 0x3F80, (N, P, Q, K), dtype=torch.int16, device="cuda")
     dy ^= (torch.randint(0, 2, (N, P, Q, K), dtype=torch.int16, device="cuda") << 15)   # random signs
@@ -300,13 +304,21 @@ def run_train(name, N, H, W, C, K, R, S, stride, pad, iters, with_dx=True):
         layer.sgd(lr)
 
     ms = {"fwd": timeit(lambda: layer.forward(x, y)),
-          "bias_act_bwd": timeit(lambda: eng.conv_bias_act_bwd(y, dy, dpre, layer.db, pixels, K, 1)),
+          "bias_act_bwd": timeit(lambda: eng.conv_bias_act_bwd(y, dy, dpre, layer.db, pixels, K, act)),
           "wgrad": timeit(wgrad)}
     if with_dx:
         ms["dgrad"] = timeit(dgrad)
     ms["sgd_set_params"] = timeit(lambda: layer.sgd(lr))
     ms["dy_copy"] = timeit(lambda: dy_step.copy_(dy))
     ms["layer_step_minus_dy_copy"] = timeit(step) - ms["dy_copy"]
+    fwd_by_act = {}
+    if act == pkg.ACT_RELU:
+        layers = {a: pkg.ConvLayer(eng, N, H, W, C, K, R, S, f, b, act=a, stride=stride, padding=(pad, pad)) for a in (0, 1, 3)}
+        for _ in range(2):
+            for a, lay in layers.items():
+                fwd_by_act.setdefault(f"act{a}", []).append(timeit(lambda: lay.forward(x, y)))
+        for lay in layers.values():
+            lay.close()
 
     # torch eager step on the same shapes (fresh random x: the values do not change the work)
     xt = x[:, :W * C].reshape(N, H, W, C).view(torch.bfloat16).permute(0, 3, 1, 2).detach().requires_grad_(with_dx)
@@ -319,7 +331,8 @@ def run_train(name, N, H, W, C, K, R, S, stride, pad, iters, with_dx=True):
         wb.grad = bb.grad = None
         if with_dx:
             xt.grad = None
-        out = torch.sigmoid(torch.nn.functional.conv2d(xt, wb, bb, stride=stride, padding=pad))
+        out = torch.nn.functional.conv2d(xt, wb, bb, stride=stride, padding=pad)
+        out = torch.relu(out) if act == pkg.ACT_RELU else torch.sigmoid(out)
         out.backward(dyt)
         with torch.no_grad():
             w32.add_(wb.grad.float(), alpha=-lr)
@@ -329,7 +342,7 @@ def run_train(name, N, H, W, C, K, R, S, stride, pad, iters, with_dx=True):
 
     ms["torch_eager_step"] = timeit(torch_step)
     ba_bytes = 3 * pixels * K * 2
-    print(json.dumps({"case": name, "N": N, "family": layer.family, "dx": with_dx, "ms": ms,
+    print(json.dumps({"case": name, "act": act, "N": N, "family": layer.family, "dx": with_dx, "ms": ms, "fwd_by_act_ms": fwd_by_act,
                       "bias_act_GBps": ba_bytes / (ms["bias_act_bwd"] * 1e-3) / 1e9,
                       "bias_act_hbm_frac": ba_bytes / (ms["bias_act_bwd"] * 1e-3) / 1e9 / HBM,
                       "layer_over_torch": ms["layer_step_minus_dy_copy"] / ms["torch_eager_step"], "gpu": gpu, "power_limit": power}),
@@ -435,17 +448,19 @@ def run_linear(name, N, P, Q, C, O, act, iters):
     del x, y, dy, dx
 
 
-def run_classifier(N, iters):
+def run_classifier(N, iters, relu=False):
     """one training step of conv 8@5x5 sigmoid -> pool 2 -> conv 16@3x3 pad 1 -> pool 2 -> fc 576->128 sigmoid -> fc 128->10 ->
     softmax cross-entropy (pcnn_softmax_ce_bf16, scale 1/N) -> backward -> sgd of all four layers, on the engine's stream; next to it
-    the torch eager step of the same layers on bf16 channels-last tensors (fp32 masters, w -= lr * grad, re-cast to bf16)"""
+    the torch eager step of the same layers on bf16 channels-last tensors (fp32 masters, w -= lr * grad, re-cast to bf16).
+    relu=True: ReLU after conv 1, conv 2 and fc 1 (step 0.05)."""
     r = np.random.default_rng(5)
     u = lambda shape, fan: r.uniform(-1, 1, shape).astype(np.float32) / np.float32(np.sqrt(fan))
     p = dict(f1=u((8, 5, 5, 1), 25), b1=u(8, 25), f2=u((16, 3, 3, 8), 72), b2=u(16, 72), w3=u((128, 6, 6, 16), 576),
              b3=u(128, 576), w4=u((10, 1, 1, 128), 128), b4=u(10, 128))
-    c1 = pkg.ConvLayer(eng, N, 28, 28, 1, 8, 5, 5, p["f1"], p["b1"], act=1)
-    c2 = pkg.ConvLayer(eng, N, 12, 12, 8, 16, 3, 3, p["f2"], p["b2"], act=0, padding=(1, 1))
-    fc1 = pkg.LinearLayer(eng, N, 6, 6, 16, 128, p["w3"], p["b3"], act=1)
+    a1, a2 = (pkg.ACT_RELU, pkg.ACT_RELU) if relu else (pkg.ACT_SIGMOID, pkg.ACT_NONE)
+    c1 = pkg.ConvLayer(eng, N, 28, 28, 1, 8, 5, 5, p["f1"], p["b1"], act=a1)
+    c2 = pkg.ConvLayer(eng, N, 12, 12, 8, 16, 3, 3, p["f2"], p["b2"], act=a2, padding=(1, 1))
+    fc1 = pkg.LinearLayer(eng, N, 6, 6, 16, 128, p["w3"], p["b3"], act=a1)
     fc2 = pkg.LinearLayer(eng, N, 1, 1, 128, 10, p["w4"], p["b4"], act=0, row_pitch=128)
     p1 = pkg.MaxPoolLayer(eng, N, 24, 24, 8, 2, row_pitch=c2.row_pitch, image_rows=c2.image_rows)
     p2 = pkg.MaxPoolLayer(eng, N, 12, 12, 16, 2, row_pitch=fc1.row_pitch, image_rows=fc1.image_rows)
@@ -455,7 +470,7 @@ def run_classifier(N, iters):
     y1, dy1, x2, dx2, y2, dy2 = e(N, 24, 24, 8), e(N, 24, 24, 8), e(N, 12, 96), e(N, 12, 96), e(N, 12, 12, 16), e(N, 12, 12, 16)
     x3, dx3, y3, dy3, z, dz = e(N, 6, 96), e(N, 6, 96), e(N, 128), e(N, 128), e(N, 10), e(N, 10)
     loss = torch.empty(N, dtype=torch.float32, device="cuda")
-    lr = 0.3
+    lr = 0.05 if relu else 0.3
     gpu, power = card()
 
     def step():
@@ -479,9 +494,10 @@ def run_classifier(N, iters):
     def torch_step():
         for v in mb.values():
             v.grad = None
-        h = F.max_pool2d(torch.sigmoid(F.conv2d(xt, mb["f1"], mb["b1"])), 2)
-        h = F.max_pool2d(F.conv2d(h, mb["f2"], mb["b2"], padding=1), 2)
-        h = torch.sigmoid(F.linear(h.permute(0, 2, 3, 1).reshape(N, -1), mb["w3"], mb["b3"]))
+        act1, act2 = (torch.relu, torch.relu) if relu else (torch.sigmoid, lambda t: t)
+        h = F.max_pool2d(act1(F.conv2d(xt, mb["f1"], mb["b1"])), 2)
+        h = F.max_pool2d(act2(F.conv2d(h, mb["f2"], mb["b2"], padding=1)), 2)
+        h = act1(F.linear(h.permute(0, 2, 3, 1).reshape(N, -1), mb["w3"], mb["b3"]))
         F.cross_entropy(F.linear(h, mb["w4"], mb["b4"]), lt).backward()
         with torch.no_grad():
             for k in m32:
@@ -489,7 +505,7 @@ def run_classifier(N, iters):
                 mb[k].copy_(m32[k])
 
     ms_torch = timed(torch_step, iters)
-    print(json.dumps({"case": f"classifier training step N={N}", "ms": ms, "torch_eager_ms": ms_torch, "ours_over_torch": ms / ms_torch,
+    print(json.dumps({"case": f"classifier training step N={N}" + (" ReLU" if relu else ""), "ms": ms, "torch_eager_ms": ms_torch, "ours_over_torch": ms / ms_torch,
                       "gpu": gpu, "power_limit": power}), flush=True)
     for layer in (c1, c2, fc1, fc2, p1, p2):
         layer.close()
@@ -502,6 +518,7 @@ if only == "linear":                                                   # fully c
     run_linear("128 -> 10 (fc2)", 1024, 1, 1, 128, 10, 0, 50)
 if only == "classifier":                                               # one step of the LeNet-style classifier, torch eager beside it
     run_classifier(1024, 50)
+    run_classifier(1024, 50, relu=True)
 if only == "pool":                                                     # max pooling between conv layers, torch beside it
     run_pool("LeNet c1 output 24x24x6, 2x2/2", 1024, 24, 24, 6, 2, 2, 0, 20)
     run_pool("112x112x64, 2x2/2", 128, 112, 112, 64, 2, 2, 0, 20)
@@ -514,6 +531,11 @@ if only == "train":                                                    # a ConvL
     run_train("14x14x256->256 3x3 pad 1", 128, 14, 14, 256, 256, 3, 3, 1, 1, 20)
     run_train("56x56x64->128 3x3 stride 2 pad 1", 128, 56, 56, 64, 128, 3, 3, 2, 1, 20)
     run_train("LeNet c1 28x28x1->6 5x5", 1024, 28, 28, 1, 6, 5, 5, 1, 0, 20, with_dx=False)
+    run_train("56x56x64->64 3x3 pad 1", 128, 56, 56, 64, 64, 3, 3, 1, 1, 20, act=3)            # the same layers with ReLU
+    run_train("28x28x128->128 3x3 pad 1", 128, 28, 28, 128, 128, 3, 3, 1, 1, 20, act=3)
+    run_train("14x14x256->256 3x3 pad 1", 128, 14, 14, 256, 256, 3, 3, 1, 1, 20, act=3)
+    run_train("56x56x64->128 3x3 stride 2 pad 1", 128, 56, 56, 64, 128, 3, 3, 2, 1, 20, act=3)
+    run_train("LeNet c1 28x28x1->6 5x5", 1024, 28, 28, 1, 6, 5, 5, 1, 0, 20, with_dx=False, act=3)
 if only == "widesame":                                                 # "same" layers: built-in padding, pad-copy route, cuDNN
     run_wide_same("56x56x64->64 3x3 pad 1", 128, 56, 56, 64, 64, 3, 3, 1, 1, 20)
     run_wide_same("28x28x128->128 3x3 pad 1", 128, 28, 28, 128, 128, 3, 3, 1, 1, 20)
