@@ -471,6 +471,50 @@ int pcnn_maxpool_nhwc_bf16_bwd(pcnn_ctx *ctx, const void *dy_bf16_dev, const uin
                                int C, int R, int S, int stride, int pad_h, int pad_w, int dy_row_pitch, int dy_image_rows);
 int pcnn_maxpool_nhwc_info(int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int row_pitch, int image_rows,
                            int *out5);
+/* Batch normalization between convolution layers (csrc/batchnorm_nhwc.cu), as torch.nn.functional.batch_norm with affine
+ * parameters, followed by an optional residual add and ReLU.  x, r, y, dy, dy2, dx and dr are dense bf16 [pixels][C] (pixels =
+ * N H W: the layout both conv forwards write as y and the gradients read as dy); gamma, beta, the running and the saved
+ * statistics, dgamma and dbeta are fp32 [C].  M = pixels.  Every fp32 operation below rounds to nearest with no contraction.
+ * Forward, training = 1:
+ *   - mean and the biased variance var of float(x) over the M pixels of each channel, accumulated so that a mean large next to
+ *     the spread does not cancel (per-CTA sums of x - k in fp32, k the CTA's first pixel, merged in double in a fixed order;
+ *     not E[x^2] - E[x]^2): save_mean = float(mean), save_rstd = float(1 / sqrt(var + double(eps))) in double;
+ *   - when running_mean and running_var are given (both or neither): with keep = 1 - momentum in fp32,
+ *       running_mean = keep * running_mean + momentum * save_mean
+ *       running_var  = keep * running_var + momentum * float(var * M / (M - 1))   (the unbiased variance, as torch)
+ *     each product rounded, then the sum.
+ * Forward, training = 0: mean = running_mean and rstd = float(1 / sqrt(double(running_var) + double(eps))) in double; nothing
+ * but y is written (save_mean, save_rstd and momentum are not used).
+ * Then per element, with mean and rstd those of the channel:
+ *   xhat = (float(x) - mean) * rstd;  v = xhat * gamma + beta;  v = v + float(r) when r is given;
+ *   y = bf16_rn(act(v)), act 0 none or 3 the ReLU of the conv epilogues (v < 0 ? +0 : v, NaN and -0 unchanged).
+ * Act 1 is refused: the sigmoid of the conv epilogues uses tanh.approx, which no reference can replay bit for bit.
+ * Backward (of a training forward; save_mean and save_rstd are what it wrote, y its output):
+ *   t = float(dy), or float(dy) + float(dy2) when dy2 (a second gradient arriving at a residual join) is given;
+ *   g = bf16_rn(act'(t)): at act 3 float(y) <= 0 gives +0 (a NaN y passes t), as threshold_backward; without dy2 dy's bits pass;
+ *   dbeta = sum over pixels of float(g), dgamma = sum of float(g) * xhat (xhat exactly as in the forward), in fp32 per-CTA
+ *     partials over pixel ranges that depend only on (pixels, C), then a fixed-order pass over them;
+ *   dx = bf16_rn(((float(g) - dbeta / Mf) - xhat * (dgamma / Mf)) * (gamma * rstd)), Mf = float(M), the two quotients and
+ *     gamma * rstd formed once per channel from the dgamma and dbeta just written;
+ *   dr = g when dr is given: the gradient of the residual input r.
+ * dx == dy (in place) is allowed; no other two buffers may overlap.  Domain (anything else is PCNN_ERR_ARG with the function and
+ * the rule in the message; the shape rules read the same in pcnn_batchnorm_nhwc_info):
+ *   - 1 <= C <= 256; training 0 or 1; M >= 2 when training and for the backward, M >= 1 in eval;
+ *   - eps finite and >= 0; 0 <= momentum <= 1; act 0 or 3;
+ *   - every pointer 16-byte aligned; x, y, gamma, beta not NULL; save_mean and save_rstd not NULL when training; running_mean
+ *     and running_var not NULL in eval; x, y, dy, gamma, the saved statistics, dx, dgamma and dbeta not NULL in the backward.
+ * With C % 8 == 0 the passes move 16-byte vectors of 8 channels, otherwise single elements.  No atomics: reruns and every H100
+ * give the same bits.  Elements past pixels * C are never written.  All calls are stream-ordered and use the context's one
+ * scratch block for their per-CTA partials.
+ * pcnn_batchnorm_nhwc_info: host only (no GPU, no context).  out5 = { channels per thread (8 or 1), pixel lanes per CTA, pixels
+ * per CTA, slots of the statistics pass (0 when training = 0), slots of the gradient pass }. */
+int pcnn_batchnorm_nhwc_bf16_fwd(pcnn_ctx *ctx, const void *x_bf16_dev, const void *r_bf16_dev, void *y_bf16_dev, long pixels, int C,
+                                 int act, int training, float eps, float momentum, const float *gamma_dev, const float *beta_dev,
+                                 float *running_mean_dev, float *running_var_dev, float *save_mean_dev, float *save_rstd_dev);
+int pcnn_batchnorm_nhwc_bf16_bwd(pcnn_ctx *ctx, const void *x_bf16_dev, const void *y_bf16_dev, const void *dy_bf16_dev,
+                                 const void *dy2_bf16_dev, const float *gamma_dev, const float *save_mean_dev, const float *save_rstd_dev,
+                                 void *dx_bf16_dev, void *dr_bf16_dev, float *dgamma_dev, float *dbeta_dev, long pixels, int C, int act);
+int pcnn_batchnorm_nhwc_info(long pixels, int C, int training, int *out5);
 /* Fully connected layers (csrc/linear_tc.cu), bf16 on the tensor cores with fp32 accumulation:
  *   - x is [N][image_rows][row_pitch] bf16 with P x Q pixels of C channels per image: the layout a plan reads as x and the NHWC
  *     pool writes as y.  A previous linear layer's y is the same with P = Q = 1, C = its O, row_pitch = O, image_rows 1.

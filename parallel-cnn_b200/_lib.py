@@ -133,6 +133,9 @@ _SIG = {
     "pcnn_maxpool_nhwc_bf16_fwd": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
     "pcnn_maxpool_nhwc_bf16_bwd": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
     "pcnn_maxpool_nhwc_info": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
+    "pcnn_batchnorm_nhwc_bf16_fwd": [_vp, _vp, _vp, _vp, _l, _i, _i, _i, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp],
+    "pcnn_batchnorm_nhwc_bf16_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _l, _i, _i],
+    "pcnn_batchnorm_nhwc_info": [_l, _i, _i, _vp],
     "pcnn_conv_bwd_plan_info": [_i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_pad_nhwc_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i],
     "pcnn_crop_nhwc_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i],
@@ -265,6 +268,15 @@ def maxpool_nhwc_info(N, H, W, C, R, S, stride, padding=(0, 0), row_pitch=0, ima
     check("pcnn_maxpool_nhwc_info", lib().pcnn_maxpool_nhwc_info(int(N), int(H), int(W), int(C), int(R), int(S), int(stride), ph, pw,
                                                                  int(row_pitch), int(image_rows), out))
     return dict(P=out[0], Q=out[1], row_pitch=out[2], vec=out[3], cover=out[4])
+
+
+def batchnorm_nhwc_info(pixels, C, training=True):
+    """How batch normalization partitions dense [pixels][C] activations (pcnn_batchnorm_nhwc_info; host only, no GPU).  vec:
+    channels per thread (8 or 1); lanes: pixels a CTA works on side by side; stat_slots (0 in eval) and grad_slots: per-CTA
+    partials of the statistics and of the gradient pass, a function of (pixels, C) alone."""
+    out = (_i * 5)()
+    check("pcnn_batchnorm_nhwc_info", lib().pcnn_batchnorm_nhwc_info(int(pixels), int(C), 1 if training else 0, out))
+    return dict(vec=out[0], lanes=out[1], pixels_per_cta=out[2], stat_slots=out[3], grad_slots=out[4])
 
 
 def linear_info(N, P, Q, C, O, row_pitch=0, image_rows=0):

@@ -4,7 +4,8 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import F32, NPARAM, TEST_SET, TRAIN_SET, U8, PcnnError, check, conv_layer_family, lib, linear_info, maxpool_nhwc_info
+from ._lib import (F32, NPARAM, TEST_SET, TRAIN_SET, U8, PcnnError, batchnorm_nhwc_info, check, conv_layer_family, lib, linear_info,
+                   maxpool_nhwc_info)
 
 
 def _pixel_type(arr_or_dtype):
@@ -431,6 +432,20 @@ class Engine:
         self._call("pcnn_maxpool_nhwc_bf16_bwd", _p(dy), _p(argmax), _p(dx), int(N), int(H), int(W), int(Cin), int(R), int(S), int(stride),
                    ph, pw, int(row_pitch or 0), int(image_rows))
 
+    def batchnorm_fwd(self, x, y, pixels, C, gamma, beta, running_mean=None, running_var=None, save_mean=None, save_rstd=None, r=None,
+                      act=0, training=True, eps=1e-5, momentum=0.1):
+        """pcnn_batchnorm_nhwc_bf16_fwd: y = bf16(act((x - mean) * rstd * gamma + beta (+ r))) over dense bf16 [pixels][C].
+        training: batch statistics into save_mean / save_rstd and, when given, the running statistics updated with momentum;
+        eval: the running statistics.  act ACT_NONE or ACT_RELU"""
+        self._call("pcnn_batchnorm_nhwc_bf16_fwd", _p(x), _p(r), _p(y), int(pixels), int(C), int(act), 1 if training else 0, float(eps),
+                   float(momentum), _p(gamma), _p(beta), _p(running_mean), _p(running_var), _p(save_mean), _p(save_rstd))
+
+    def batchnorm_bwd(self, x, y, dy, gamma, save_mean, save_rstd, dx, dgamma, dbeta, pixels, C, act=0, dy2=None, dr=None):
+        """pcnn_batchnorm_nhwc_bf16_bwd of a training forward: g = bf16(act'(dy (+ dy2))), dbeta = sum g, dgamma = sum g * xhat,
+        dx (may be dy itself) and, when given, dr = g (the gradient of the forward's residual input)"""
+        self._call("pcnn_batchnorm_nhwc_bf16_bwd", _p(x), _p(y), _p(dy), _p(dy2), _p(gamma), _p(save_mean), _p(save_rstd), _p(dx), _p(dr),
+                   _p(dgamma), _p(dbeta), int(pixels), int(C), int(act))
+
     def pad_nhwc(self, src_bf16, dst_bf16, N, H, W, Cin, pad_h, pad_w, dst_row_pitch=0, dst_image_rows=0):
         self._call("pcnn_pad_nhwc_bf16", _p(src_bf16), _p(dst_bf16), N, H, W, Cin, int(pad_h), int(pad_w), int(dst_row_pitch), int(dst_image_rows))
 
@@ -612,6 +627,69 @@ class ConvLayer:
                 a.free()
 
 
+class BatchNormLayer:
+    """Batch normalization trained on the device (pcnn_batchnorm_nhwc_bf16_fwd / _bwd), as torch's BatchNorm2d with affine
+    parameters, with an optional residual add and ReLU after it.  It owns fp32 gamma (default ones) and beta (default zeros), their
+    gradients dgamma and dbeta, the running mean and variance (zeros and ones, updated with `momentum` by every training forward)
+    and the saved mean and rstd of the last training forward, all in DeviceArrays.
+
+    x, r, y, dy, dy2, dx and dr are dense bf16 [N][H][W][C]: what a ConvLayer writes as y and reads as dy.  act ACT_RELU (3) is
+    a ReLU after the add, ACT_NONE (0) none.  A ResNet basic block, x0 being a previous BatchNormLayer's output:
+
+        conv_a.forward(x0, ya); bn_a.forward(ya, za); conv_b.forward(za, yb); bn_b.forward(yb, out, r=x0)
+        bn_b.backward(out, dout, dyb, dr=dres); conv_b.backward(yb, dyb, dza); bn_a.backward(za, dza, dya)
+        conv_a.backward(ya, dya, dx0)
+
+    with bn_a at ACT_RELU, bn_b at ACT_RELU, conv_a and conv_b without bias; the BatchNormLayer that wrote x0 completes the join
+    with backward(..., dx0, dy2=dres)."""
+
+    def __init__(self, engine, N, H, W, C, act=0, eps=1e-5, momentum=0.1, gamma=None, beta=None):
+        self.engine = engine
+        self.shape = (N, H, W, C)
+        self.pixels = int(N) * int(H) * int(W)
+        self.act, self.eps, self.momentum = int(act), float(eps), float(momentum)
+        self.info = batchnorm_nhwc_info(self.pixels, C, True)
+        g = np.ones(C, np.float32) if gamma is None else np.ascontiguousarray(gamma, np.float32).reshape(C)
+        b = np.zeros(C, np.float32) if beta is None else np.ascontiguousarray(beta, np.float32).reshape(C)
+        self.gamma, self.beta = DeviceArray.from_host(engine, g), DeviceArray.from_host(engine, b)
+        self.dgamma, self.dbeta = engine.array(C), engine.array(C)
+        self.running_mean = DeviceArray.from_host(engine, np.zeros(C, np.float32))
+        self.running_var = DeviceArray.from_host(engine, np.ones(C, np.float32))
+        self.save_mean, self.save_rstd = engine.array(C), engine.array(C)
+        self._x = None
+
+    def forward(self, x, y, r=None, training=True):
+        """y = act(bn(x) + r).  training: batch statistics, saved for backward, and the running statistics updated; otherwise the
+        running statistics.  The layer keeps x: backward reads it."""
+        N, H, W, C = self.shape
+        self.engine.batchnorm_fwd(x, y, self.pixels, C, self.gamma, self.beta, self.running_mean, self.running_var, self.save_mean,
+                                  self.save_rstd, r=r, act=self.act, training=training, eps=self.eps, momentum=self.momentum)
+        if training:
+            self._x = x
+
+    def backward(self, y, dy, dx, dr=None, dy2=None):
+        """Gradients of the most recent training forward, whose output y was: dgamma, dbeta and dx (dx may be dy).  dy2 is a second
+        gradient added to dy before the activation (the other branch of a residual join); dr receives the gradient of the
+        forward's r."""
+        N, H, W, C = self.shape
+        self.engine.batchnorm_bwd(self._x, y, dy, self.gamma, self.save_mean, self.save_rstd, dx, self.dgamma, self.dbeta, self.pixels, C,
+                                  act=self.act, dy2=dy2, dr=dr)
+
+    def sgd(self, lr):
+        """gamma += (-lr) * dgamma and beta += (-lr) * dbeta in fp32, on the engine's stream"""
+        C = self.shape[3]
+        self.engine.apply_grad_scaled(self.gamma, self.dgamma, C, -lr)
+        self.engine.apply_grad_scaled(self.beta, self.dbeta, C, -lr)
+
+    def params(self):
+        """host copies of gamma, beta, the running mean and the running variance"""
+        return self.gamma.to_host(), self.beta.to_host(), self.running_mean.to_host(), self.running_var.to_host()
+
+    def close(self):
+        for a in (self.gamma, self.beta, self.dgamma, self.dbeta, self.running_mean, self.running_var, self.save_mean, self.save_rstd):
+            a.free()
+
+
 class LinearLayer:
     """A fully connected layer trained on the device, with ConvLayer's interface: fp32 masters w [O][P][Q][C] and bias [O], their
     gradients dw and db, and a LinearPlan holding w in bf16.
@@ -733,4 +811,4 @@ def bf16_bits_to_f32(b):
 
 
 C_ = C
-__all__ = ["Engine", "DeviceArray", "ConvPlan", "WideConvPlan", "LinearPlan", "ConvLayer", "LinearLayer", "MaxPoolLayer", "f32_to_bf16_bits", "bf16_bits_to_f32", "TRAIN_SET", "TEST_SET", "U8", "F32"]
+__all__ = ["Engine", "DeviceArray", "ConvPlan", "WideConvPlan", "LinearPlan", "ConvLayer", "LinearLayer", "MaxPoolLayer", "BatchNormLayer", "f32_to_bf16_bits", "bf16_bits_to_f32", "TRAIN_SET", "TEST_SET", "U8", "F32"]

@@ -511,6 +511,118 @@ def run_classifier(N, iters, relu=False):
         layer.close()
 
 
+def run_bn(name, N, H, W, C, iters):
+    """batch normalization with ReLU (pcnn_batchnorm_nhwc_bf16_fwd / _bwd), each pass with and without the residual r, next to
+    torch's F.batch_norm (+ add) + relu and its autograd backward on the same channels-last bf16 tensors.  Bytes, T = N*H*W*C*2:
+    training forward 3T (x read twice: once for the statistics, once for y; y written), eval forward 2T, + T for reading r;
+    backward 7T (x, y, dy read by the statistics pass; x, y, dy read and dx written by the second), + T for writing dr.  The
+    per-CTA slots (a few 100 kB) and the [C] vectors are not counted."""
+    M = N * H * W
+    T = M * C * 2
+    rnd = lambda: torch.randint(-0x4000, 0x4000, (M, C), dtype=torch.int16, device="cuda") & 0x3FFF | 0x3C00   # bf16 in [1, 2) * 2^k
+    x, r, dy = rnd(), rnd(), rnd()
+    r ^= torch.randint(0, 2, (M, C), dtype=torch.int16, device="cuda") << 15
+    dy ^= torch.randint(0, 2, (M, C), dtype=torch.int16, device="cuda") << 15
+    y, dx, dr = (torch.empty((M, C), dtype=torch.int16, device="cuda") for _ in range(3))
+    info = pkg.batchnorm_nhwc_info(M, C)
+    f = lambda v: eng.to_device(np.full(C, v, np.float32))
+    gamma, beta, rm, rv, sm, sr, dg, db = f(1), f(0), f(0), f(1), f(0), f(1), f(0), f(0)
+    gpu, power = card()
+    F = torch.nn.functional
+    bf = lambda t: t.view(torch.bfloat16).reshape(N, H, W, C).permute(0, 3, 1, 2)         # channels-last NCHW views
+    xt, rt, dyt = bf(x).detach().clone().requires_grad_(True), bf(r).detach().clone().requires_grad_(True), bf(dy)
+    gt, bt = torch.ones(C, device="cuda", requires_grad=True), torch.zeros(C, device="cuda", requires_grad=True)
+    rmt, rvt = torch.zeros(C, device="cuda"), torch.ones(C, device="cuda")
+
+    def torch_fwd(with_r, training):
+        v = F.batch_norm(xt, rmt, rvt, gt, bt, training=training, momentum=0.1, eps=1e-5)
+        return torch.relu(v + rt if with_r else v)
+
+    eng.batchnorm_fwd(x, y, M, C, gamma, beta, rm, rv, sm, sr, act=3)       # the statistics the backward reads
+    for with_r in (False, True):
+        rr, drr = (r, dr) if with_r else (None, None)
+        out = torch_fwd(with_r, True)
+        ins = [xt, gt, bt] + ([rt] if with_r else [])
+        passes = (("training fwd", lambda: eng.batchnorm_fwd(x, y, M, C, gamma, beta, rm, rv, sm, sr, r=rr, act=3),
+                   lambda: torch_fwd(with_r, True), 3 * T + (T if with_r else 0)),
+                  ("eval fwd", lambda: eng.batchnorm_fwd(x, y, M, C, gamma, beta, rm, rv, r=rr, act=3, training=False),
+                   lambda: torch_fwd(with_r, False), 2 * T + (T if with_r else 0)),
+                  ("bwd", lambda: eng.batchnorm_bwd(x, y, dy, gamma, sm, sr, dx, dg, db, M, C, act=3, dr=drr),
+                   lambda: torch.autograd.grad(out, ins, dyt, retain_graph=True), 7 * T + (T if with_r else 0)))
+        for what, fn, tfn, nbytes in passes:
+            ms, ms_torch = timed(fn, iters), timed(tfn, iters)
+            print(json.dumps({"case": f"{name} {what}" + (" + r" if with_r else ""), "N": N, "us": ms * 1e3, "MB": nbytes / 1e6,
+                              "hbm_frac": nbytes / (ms * 1e-3) / 1e9 / HBM, "torch_us": ms_torch * 1e3, "torch_over_ours": ms_torch / ms,
+                              "vec": info["vec"], "slots": info["grad_slots"], "gpu": gpu, "power_limit": power}), flush=True)
+    for a in (gamma, beta, rm, rv, sm, sr, dg, db):
+        a.free()
+    del x, r, dy, y, dx, dr, xt, rt
+
+
+def run_resblock(N, iters):
+    """one training step of a ResNet basic block, 56x56x64 at N = 128: conv_a 3x3 pad 1 (no bias) -> BN + ReLU -> conv_b -> BN + x0
+    -> ReLU, its backward (dx0 and the shortcut's gradient dres left apart: the BN that wrote x0 adds them as dy2) and the sgd of
+    the four layers, on the engine's stream.  Next to it the torch eager step of the same block on bf16 channels-last tensors (fp32
+    masters, w -= lr * grad, re-cast to bf16)."""
+    H = W = 56
+    C = 64
+    r = np.random.default_rng(11)
+    u = lambda shape, fan: r.uniform(-1, 1, shape).astype(np.float32) / np.float32(np.sqrt(fan))
+    fa, fb = u((C, 3, 3, C), 9 * C), u((C, 3, 3, C), 9 * C)
+    ca = pkg.ConvLayer(eng, N, H, W, C, C, 3, 3, fa, None, act=0, padding=(1, 1))
+    cb = pkg.ConvLayer(eng, N, H, W, C, C, 3, 3, fb, None, act=0, padding=(1, 1))
+    ba, bb = pkg.BatchNormLayer(eng, N, H, W, C, act=pkg.ACT_RELU), pkg.BatchNormLayer(eng, N, H, W, C, act=pkg.ACT_RELU)
+    e = lambda: torch.empty((N, H, W, C), dtype=torch.int16, device="cuda")
+    x0 = torch.randint(0, 0x3F80, (N, H, W, C), dtype=torch.int16, device="cuda")
+    dout = torch.randint(0, 0x3F80, (N, H, W, C), dtype=torch.int16, device="cuda")
+    dout ^= torch.randint(0, 2, (N, H, W, C), dtype=torch.int16, device="cuda") << 15
+    ya, za, yb, out, dyb, dres, dza, dya, dx0 = (e() for _ in range(9))
+    lr = 0.05
+    gpu, power = card()
+
+    def step():
+        ca.forward(x0, ya); ba.forward(ya, za); cb.forward(za, yb); bb.forward(yb, out, r=x0)
+        bb.backward(out, dout, dyb, dr=dres); cb.backward(yb, dyb, dza); ba.backward(za, dza, dya); ca.backward(ya, dya, dx0)
+        for layer in (ca, ba, cb, bb):
+            layer.sgd(lr)
+
+    ms = timed(step, iters)
+    F = torch.nn.functional
+    xt = x0.view(torch.bfloat16).permute(0, 3, 1, 2).detach().requires_grad_(True)
+    dt = dout.view(torch.bfloat16).permute(0, 3, 1, 2)
+    m32 = {k: torch.from_numpy(v).to("cuda").permute(0, 3, 1, 2).contiguous(memory_format=torch.channels_last) for k, v in
+           (("fa", fa), ("fb", fb))}
+    m32.update(ga=torch.ones(C, device="cuda"), ba=torch.zeros(C, device="cuda"), gb=torch.ones(C, device="cuda"), bb=torch.zeros(C, device="cuda"))
+    mb = {k: (v.to(torch.bfloat16) if k.startswith("f") else v.clone()).requires_grad_(True) for k, v in m32.items()}
+    stats = [torch.zeros(C, device="cuda"), torch.ones(C, device="cuda"), torch.zeros(C, device="cuda"), torch.ones(C, device="cuda")]
+
+    def torch_step():
+        for v in mb.values():
+            v.grad = None
+        xt.grad = None
+        h = torch.relu(F.batch_norm(F.conv2d(xt, mb["fa"], padding=1), stats[0], stats[1], mb["ga"], mb["ba"], training=True))
+        h = torch.relu(F.batch_norm(F.conv2d(h, mb["fb"], padding=1), stats[2], stats[3], mb["gb"], mb["bb"], training=True) + xt)
+        h.backward(dt)
+        with torch.no_grad():
+            for k in m32:
+                m32[k].add_(mb[k].grad.float(), alpha=-lr)
+                mb[k].copy_(m32[k])
+
+    ms_torch = timed(torch_step, iters)
+    print(json.dumps({"case": f"basic block 56x56x64 training step N={N}", "ms": ms, "torch_eager_ms": ms_torch, "ours_over_torch": ms / ms_torch,
+                      "gpu": gpu, "power_limit": power}), flush=True)
+    for layer in (ca, cb, ba, bb):
+        layer.close()
+
+
+if only == "bn":                                                       # batch normalization passes, torch beside them
+    run_bn("56x56x64", 128, 56, 56, 64, 50)
+    run_bn("28x28x128", 128, 28, 28, 128, 50)
+    run_bn("14x14x256", 128, 14, 14, 256, 50)
+    run_bn("7x7x256", 128, 7, 7, 256, 50)
+    run_bn("24x24x6 (scalar path)", 1024, 24, 24, 6, 50)
+if only == "resblock":                                                 # one step of a ResNet basic block, torch eager beside it
+    run_resblock(128, 20)
 if only == "linear":                                                   # fully connected passes, torch.nn.functional.linear beside them
     run_linear("7x7x256 -> 256", 1024, 7, 7, 256, 256, 0, 50)
     run_linear("1x1x2048 -> 256", 4096, 1, 1, 2048, 256, 0, 50)
