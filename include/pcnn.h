@@ -471,6 +471,44 @@ int pcnn_maxpool_nhwc_bf16_bwd(pcnn_ctx *ctx, const void *dy_bf16_dev, const uin
                                int C, int R, int S, int stride, int pad_h, int pad_w, int dy_row_pitch, int dy_image_rows);
 int pcnn_maxpool_nhwc_info(int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int row_pitch, int image_rows,
                            int *out5);
+/* Average pooling between convolution layers (csrc/pool_nhwc.cu), in the max pool's layouts, shapes and domain (the refusals read
+ * the same, with the function's name), as torch.nn.functional.avg_pool2d with ceil_mode=False and no divisor_override.  Every fp32
+ * operation below rounds to nearest with no contraction; "/" is an IEEE division, not a product with a reciprocal.
+ *   - count_include_pad must be 0 or 1.  cnt(p, q) = R S when it is 1, else the number of the window's in-image positions (>= 1:
+ *     with pad <= R/2 every window holds an image element).  With no ceil mode R S is also torch's divisor.
+ * Forward: s = the sum of float(x) over the in-image positions of the window of (p, q), r = 0..R-1 then s = 0..S-1, starting from
+ *   the first term (not from +0); y[n][p][q][c] = bf16_rn(s / float(cnt(p, q))).  NaN and +-Inf propagate as IEEE addition does.
+ * Backward: dx[n][h][w][c] = the sum of float(dy[n][p][q][c]) / float(cnt(p, q)) over the windows (p, q) that contain (h, w), in
+ *   ascending p, then ascending q, each quotient rounded, the sum starting from the first term and rounded to bf16 once; +0 with
+ *   no term.  Every element of dx is written, with no memset and no atomics.
+ * The pad columns and pad rows of y's layout are never written; those of dy are never read.  x and y disjoint, dy and dx
+ * disjoint, every pointer 16-byte aligned.  Stream-ordered, no allocation, the same bits on every run and SM count.
+ * pcnn_avgpool_nhwc_info: host only, out5 as pcnn_maxpool_nhwc_info. */
+int pcnn_avgpool_nhwc_bf16_fwd(pcnn_ctx *ctx, const void *x_bf16_dev, void *y_bf16_dev, int N, int H, int W, int C, int R, int S,
+                               int stride, int pad_h, int pad_w, int count_include_pad, int y_row_pitch, int y_image_rows);
+int pcnn_avgpool_nhwc_bf16_bwd(pcnn_ctx *ctx, const void *dy_bf16_dev, void *dx_bf16_dev, int N, int H, int W, int C, int R, int S,
+                               int stride, int pad_h, int pad_w, int count_include_pad, int dy_row_pitch, int dy_image_rows);
+int pcnn_avgpool_nhwc_info(int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int row_pitch, int image_rows,
+                           int *out5);
+/* Global average pooling (csrc/pool_nhwc.cu), as torch.nn.functional.adaptive_avg_pool2d(x, 1) or x.mean((2, 3)):
+ *   - x and dx are dense bf16 [N][H][W][C]: what a conv forward or a batch norm writes as y, and what their backward reads as dy;
+ *   - y and dy are [N][1][row_pitch], row_pitch 0 = C rounded up to 8, otherwise >= C and a multiple of 8: the x layout of a
+ *     LinearLayer with P = Q = 1, so the pool sits between a batch norm and a linear layer with no copy.
+ * Forward: s = the sum of float(x[n][h][w][c]) over the H W pixels in fp32, in the order of the partition pcnn_global_avgpool_nhwc_info
+ *   reports, which depends on (N, H, W, C) alone, never on the SM count: the pixels are cut into ranges of `pixels per CTA`; in a
+ *   range, lane l (0..lanes-1) sums the pixels l, l + lanes, ... from its first one; the lanes holding a pixel are added in lane
+ *   order; the ranges of an image are added in range order (through fp32 slots in the context's scratch block when there are
+ *   several).  y[n][c] = bf16_rn(s / float(H W)).  The pad columns of y are never written.
+ * Backward: dx[n][h][w][c] = bf16_rn(float(dy[n][c]) / float(H W)) for every pixel; the pad of dy is never read.
+ * Domain (anything else is PCNN_ERR_ARG with the function and the rule in the message): N, H, W, C >= 1; H W C within the 32-bit
+ * index range of one image; the row pitch above; every pointer 16-byte aligned; x and y, dy and dx disjoint.  Channel groups (8
+ * channels when C % 8 == 0, else 1) beyond 256 are sliced across CTAs.  Stream-ordered; the same bits on every run and SM count.
+ * pcnn_global_avgpool_nhwc_info: host only (no GPU, no context).  out8 = { row pitch used, channels per thread (8 or 1), channel
+ * groups per CTA, channel slices, pixel lanes per CTA, pixels per CTA (8 per lane), pixel ranges per image, CTAs of the forward }. */
+int pcnn_global_avgpool_nhwc_bf16_fwd(pcnn_ctx *ctx, const void *x_bf16_dev, void *y_bf16_dev, int N, int H, int W, int C, int y_row_pitch);
+int pcnn_global_avgpool_nhwc_bf16_bwd(pcnn_ctx *ctx, const void *dy_bf16_dev, void *dx_bf16_dev, int N, int H, int W, int C,
+                                      int dy_row_pitch);
+int pcnn_global_avgpool_nhwc_info(int N, int H, int W, int C, int row_pitch, int *out8);
 /* Batch normalization between convolution layers (csrc/batchnorm_nhwc.cu), as torch.nn.functional.batch_norm with affine
  * parameters, followed by an optional residual add and ReLU.  x, r, y, dy, dy2, dx and dr are dense bf16 [pixels][C] (pixels =
  * N H W: the layout both conv forwards write as y and the gradients read as dy); gamma, beta, the running and the saved

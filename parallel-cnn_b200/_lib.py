@@ -133,6 +133,12 @@ _SIG = {
     "pcnn_maxpool_nhwc_bf16_fwd": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
     "pcnn_maxpool_nhwc_bf16_bwd": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
     "pcnn_maxpool_nhwc_info": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
+    "pcnn_avgpool_nhwc_bf16_fwd": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
+    "pcnn_avgpool_nhwc_bf16_bwd": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
+    "pcnn_avgpool_nhwc_info": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
+    "pcnn_global_avgpool_nhwc_bf16_fwd": [_vp, _vp, _vp, _i, _i, _i, _i, _i],
+    "pcnn_global_avgpool_nhwc_bf16_bwd": [_vp, _vp, _vp, _i, _i, _i, _i, _i],
+    "pcnn_global_avgpool_nhwc_info": [_i, _i, _i, _i, _i, _vp],
     "pcnn_batchnorm_nhwc_bf16_fwd": [_vp, _vp, _vp, _vp, _l, _i, _i, _i, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp],
     "pcnn_batchnorm_nhwc_bf16_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _l, _i, _i],
     "pcnn_batchnorm_nhwc_info": [_l, _i, _i, _vp],
@@ -268,6 +274,25 @@ def maxpool_nhwc_info(N, H, W, C, R, S, stride, padding=(0, 0), row_pitch=0, ima
     check("pcnn_maxpool_nhwc_info", lib().pcnn_maxpool_nhwc_info(int(N), int(H), int(W), int(C), int(R), int(S), int(stride), ph, pw,
                                                                  int(row_pitch), int(image_rows), out))
     return dict(P=out[0], Q=out[1], row_pitch=out[2], vec=out[3], cover=out[4])
+
+
+def avgpool_nhwc_info(N, H, W, C, R, S, stride, padding=(0, 0), row_pitch=0, image_rows=0):
+    """The output size and layout of the NHWC average pool (pcnn_avgpool_nhwc_info; host only, no GPU): the max pool's domain and
+    keys (maxpool_nhwc_info)."""
+    ph, pw = (int(v) for v in padding)
+    out = (_i * 5)()
+    check("pcnn_avgpool_nhwc_info", lib().pcnn_avgpool_nhwc_info(int(N), int(H), int(W), int(C), int(R), int(S), int(stride), ph, pw,
+                                                                 int(row_pitch), int(image_rows), out))
+    return dict(P=out[0], Q=out[1], row_pitch=out[2], vec=out[3], cover=out[4])
+
+
+def global_avgpool_nhwc_info(N, H, W, C, row_pitch=0):
+    """How the global average pool partitions a shape (pcnn_global_avgpool_nhwc_info; host only, no GPU).  row_pitch 0 = C rounded
+    up to 8.  Lane l of a pixel range sums the pixels l, l + lanes, ... of it; the lanes, then the ranges, are added in order."""
+    out = (_i * 8)()
+    check("pcnn_global_avgpool_nhwc_info", lib().pcnn_global_avgpool_nhwc_info(int(N), int(H), int(W), int(C), int(row_pitch), out))
+    return dict(row_pitch=out[0], vec=out[1], groups_per_cta=out[2], slices=out[3], lanes=out[4], pixels_per_cta=out[5], ranges=out[6],
+                ctas=out[7])
 
 
 def batchnorm_nhwc_info(pixels, C, training=True):

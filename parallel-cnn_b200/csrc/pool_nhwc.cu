@@ -8,6 +8,10 @@
 // pixel in ascending (p, q), adds the dy of those whose argmax points at it in fp32 and writes dx once, so every element of
 // dx is written (0 where nothing points), with no memset and no atomics.  The work of a thread depends only on the shape: the
 // bits are the same on every run and every H100.
+//
+// Average pooling (pcnn_avgpool_nhwc_bf16_fwd / _bwd) is the same two passes with a sum in place of the compare and no argmax.
+// Global average pooling (pcnn_global_avgpool_nhwc_bf16_fwd / _bwd) writes y in the x layout of a LinearLayer with P = Q = 1:
+// its forward is a reduction over the pixels of an image (partition at k_gap_fwd), its backward a broadcast.
 #include "pcnn_internal.h"
 
 #include <cuda_bf16.h>
@@ -127,6 +131,181 @@ __global__ void __launch_bounds__(POOL_THREADS) k_maxpool_nhwc_bwd(const __nv_bf
     *reinterpret_cast<BfVec<VEC> *>(dx + (((long)n * a.H + h) * a.W + w) * a.C + g * VEC) = out;
 }
 
+// The IEEE quotient RN(a / b) for b >= 1 given rb = RN(1 / double(b)), with no out-of-line slow path: __fdiv_rn branches to one
+// for extreme exponents, and the call's register convention spills the sums held across it.  In double, a / b of a float a
+// neither overflows nor underflows, so two FMA remainder steps give RN_double(a / b) (Markstein: rb correctly rounded, the
+// second step starts from a faithful quotient); rounding that to float is RN(a / b) (53 >= 2 * 24 + 2 bits: double rounding is
+// innocuous for a quotient).  Zeros, infinities and NaN take a * rb, which keeps the sign of a zero and propagates the rest.
+__device__ __forceinline__ float div_rn(float a, double b, double rb) {
+    const double ad = a;
+    double q = ad * rb;
+    q = fma(fma(-b, q, ad), rb, q);
+    q = fma(fma(-b, q, ad), rb, q);
+    return a == 0.0f || !isfinite(a) ? a * (float)rb : __double2float_rn(q);
+}
+
+// RN(1 / k) for the window counts k = 1..49 (constant-folded in IEEE double)
+struct RcpTable {
+    double v[POOL_MAX_TAPS * POOL_MAX_TAPS + 1];
+};
+constexpr RcpTable make_rcp() {
+    RcpTable t{};
+    for (int k = 1; k <= POOL_MAX_TAPS * POOL_MAX_TAPS; ++k) t.v[k] = 1.0 / k;
+    return t;
+}
+__constant__ RcpTable k_rcp = make_rcp();
+
+// y = bf16_rn(s / cnt): s sums the window's in-image elements in (r, s) order starting from the first, cnt = R S with
+// count_include_pad, else the in-image positions (>= 1: pad <= R/2 puts an image element in every window)
+template <int VEC>
+__global__ void __launch_bounds__(POOL_THREADS) k_avgpool_nhwc_fwd(const __nv_bfloat16 *__restrict__ x, __nv_bfloat16 *__restrict__ y, PoolArgs a,
+                                                                   int include_pad) {
+    const int n = blockIdx.x / a.blocks;
+    const int i = (blockIdx.x - n * a.blocks) * POOL_THREADS + threadIdx.x;
+    if (i >= a.work) return;
+    const int g = i % a.G, pq = i / a.G, q = pq % a.Q, p = pq / a.Q;
+    const int h0 = p * a.stride - a.pad_h, w0 = q * a.stride - a.pad_w;
+    const int r0 = max(0, -h0), r1 = min(a.R, a.H - h0), s0 = max(0, -w0), s1 = min(a.S, a.W - w0);
+    const int cnt = include_pad ? a.R * a.S : (r1 - r0) * (s1 - s0);
+    const __nv_bfloat16 *xi = x + (long)n * a.H * a.W * a.C + g * VEC;
+    float acc[VEC];                                        // -0 + f == f for every f: the sum starts from the first term
+#pragma unroll
+    for (int c = 0; c < VEC; ++c) acc[c] = -0.0f;
+    for (int r = r0; r < r1; ++r) {
+        const __nv_bfloat16 *row = xi + (long)(h0 + r) * a.W * a.C;
+        for (int s = s0; s < s1; ++s) {
+            const BfVec<VEC> v = *reinterpret_cast<const BfVec<VEC> *>(row + (long)(w0 + s) * a.C);
+#pragma unroll
+            for (int c = 0; c < VEC; ++c) acc[c] = __fadd_rn(acc[c], __bfloat162float(v.h[c]));
+        }
+    }
+    BfVec<VEC> out;
+#pragma unroll
+    for (int c = 0; c < VEC; ++c) out.h[c] = __float2bfloat16_rn(div_rn(acc[c], (double)cnt, k_rcp.v[cnt]));
+    *reinterpret_cast<BfVec<VEC> *>(y + (long)n * a.rows * a.pitch + (long)p * a.pitch + q * a.C + g * VEC) = out;
+}
+
+// the gather of the forward: dx sums float(dy) / cnt over the windows that contain the pixel in ascending (p, q), each quotient
+// rounded, from the first term, rounded to bf16 once; +0 with no term
+template <int VEC>
+__global__ void __launch_bounds__(POOL_THREADS) k_avgpool_nhwc_bwd(const __nv_bfloat16 *__restrict__ dy, __nv_bfloat16 *__restrict__ dx, PoolArgs a,
+                                                                   int include_pad) {
+    const int n = blockIdx.x / a.blocks;
+    const int i = (blockIdx.x - n * a.blocks) * POOL_THREADS + threadIdx.x;
+    if (i >= a.work) return;
+    const int g = i % a.G, hw = i / a.G, w = hw % a.W, h = hw / a.W;
+    const int nh = h + a.pad_h - a.R + 1, nw = w + a.pad_w - a.S + 1;
+    const int p0 = nh <= 0 ? 0 : (nh + a.stride - 1) / a.stride, p1 = min(a.P - 1, (h + a.pad_h) / a.stride);
+    const int q0 = nw <= 0 ? 0 : (nw + a.stride - 1) / a.stride, q1 = min(a.Q - 1, (w + a.pad_w) / a.stride);
+    const __nv_bfloat16 *dyi = dy + (long)n * a.rows * a.pitch + g * VEC;
+    float acc[VEC];                                        // -0 + t == t for every t: the sum starts from the first term
+#pragma unroll
+    for (int c = 0; c < VEC; ++c) acc[c] = -0.0f;
+    for (int p = p0; p <= p1; ++p) {
+        const int hs = p * a.stride - a.pad_h;
+        const int rows = include_pad ? a.R : min(a.R, a.H - hs) - max(0, -hs);
+        for (int q = q0; q <= q1; ++q) {
+            const int ws = q * a.stride - a.pad_w;
+            const int cnt = include_pad ? a.R * a.S : rows * (min(a.S, a.W - ws) - max(0, -ws));
+            const double b = cnt, rb = k_rcp.v[cnt];
+            const BfVec<VEC> d = *reinterpret_cast<const BfVec<VEC> *>(dyi + (long)p * a.pitch + q * a.C);
+#pragma unroll
+            for (int c = 0; c < VEC; ++c) acc[c] = __fadd_rn(acc[c], div_rn(__bfloat162float(d.h[c]), b, rb));
+        }
+    }
+    const bool none = p0 > p1 || q0 > q1;
+    BfVec<VEC> out;
+#pragma unroll
+    for (int c = 0; c < VEC; ++c) out.h[c] = none ? __ushort_as_bfloat16(0) : __float2bfloat16_rn(acc[c]);
+    *reinterpret_cast<BfVec<VEC> *>(dx + (((long)n * a.H + h) * a.W + w) * a.C + g * VEC) = out;
+}
+
+// Global average pooling.  CTA (n, range, slice) owns the pixels [range * per_cta, (range + 1) * per_cta) of image n and the
+// channel groups [slice * Gc, (slice + 1) * Gc); thread t keeps group t % Gc of the pixels lane, lane + lanes, ... (lane = t / Gc,
+// lanes = 256 / Gc, GAP_ITERS pixels each), summed from the first; the lanes that hold a pixel are then added in lane order
+// through shared memory.  One range per image writes y; more write fp32 slots [n][range][C] that k_gap_finish adds in range order.
+constexpr int GAP_ITERS = 8;                               // pixels per thread
+constexpr int GAP_MAX_GROUPS = POOL_THREADS;               // channel groups per CTA: C up to 2048 in one slice on the 16-byte path
+
+struct GapArgs {
+    int HW, C, G;           // pixels per image, channels, channel groups of VEC
+    int Gc, slices;         // groups per CTA, channel slices
+    int lanes, per_cta, ranges;
+    int pitch;              // row pitch of y / dy
+    double hw, rhw;         // float(H W), the divisor, and RN(1 / double(float(H W))) for div_rn
+};
+
+template <int VEC>
+__global__ void __launch_bounds__(POOL_THREADS) k_gap_fwd(const __nv_bfloat16 *__restrict__ x, __nv_bfloat16 *__restrict__ y,
+                                                          float *__restrict__ slots, GapArgs a) {
+    __shared__ float part[POOL_THREADS * 8];               // [lanes][Gc * VEC]: lanes * Gc <= 256
+    constexpr int U = VEC == 8 ? 4 : 8;                    // pixels loaded before any is added
+    const int slice = blockIdx.x % a.slices, nr = blockIdx.x / a.slices, rg = nr % a.ranges, n = nr / a.ranges;
+    const int lane = threadIdx.x / a.Gc, gl = threadIdx.x % a.Gc, g = slice * a.Gc + gl;
+    const int width = a.Gc * VEC, p0 = rg * a.per_cta;
+    if (lane < a.lanes && g < a.G && p0 + lane < a.HW) {
+        const __nv_bfloat16 *xi = x + (long)n * a.HW * a.C + g * VEC;
+        float acc[VEC];
+        for (int j0 = 0; j0 < GAP_ITERS; j0 += U) {
+            BfVec<VEC> v[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                const int px = min(p0 + lane + (j0 + u) * a.lanes, a.HW - 1);     // past the image: a pixel loaded and not added
+                v[u] = *reinterpret_cast<const BfVec<VEC> *>(xi + (long)px * a.C);
+            }
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                if (p0 + lane + (j0 + u) * a.lanes >= a.HW) continue;
+#pragma unroll
+                for (int c = 0; c < VEC; ++c) {
+                    const float f = __bfloat162float(v[u].h[c]);
+                    acc[c] = j0 + u == 0 ? f : __fadd_rn(acc[c], f);
+                }
+            }
+        }
+#pragma unroll
+        for (int c = 0; c < VEC; ++c) part[lane * width + gl * VEC + c] = acc[c];
+    }
+    __syncthreads();
+    const int active = min(a.lanes, a.HW - p0);            // lanes holding at least one pixel
+    for (int t = threadIdx.x; t < width; t += POOL_THREADS) {
+        const int c = slice * width + t;
+        if (c >= a.C) break;
+        float s = part[t];
+        for (int l = 1; l < active; ++l) s = __fadd_rn(s, part[l * width + t]);
+        if (a.ranges == 1)
+            y[(long)n * a.pitch + c] = __float2bfloat16_rn(div_rn(s, a.hw, a.rhw));
+        else
+            slots[(long)nr * a.C + c] = s;
+    }
+}
+
+// one thread per (n, c): the slots of image n added in range order, then y = bf16_rn(s / float(H W))
+__global__ void __launch_bounds__(POOL_THREADS) k_gap_finish(const float *__restrict__ slots, __nv_bfloat16 *__restrict__ y, int N, GapArgs a) {
+    const long i = (long)blockIdx.x * POOL_THREADS + threadIdx.x;
+    if (i >= (long)N * a.C) return;
+    const int n = (int)(i / a.C), c = (int)(i - (long)n * a.C);
+    const float *sl = slots + (long)n * a.ranges * a.C + c;
+    float s = sl[0];
+    for (int r = 1; r < a.ranges; ++r) s = __fadd_rn(s, sl[(long)r * a.C]);
+    y[(long)n * a.pitch + c] = __float2bfloat16_rn(div_rn(s, a.hw, a.rhw));
+}
+
+// dx[n][pixel][c] = bf16_rn(float(dy[n][c]) / float(H W)): one 16-byte store per (pixel, channel group)
+template <int VEC>
+__global__ void __launch_bounds__(POOL_THREADS) k_gap_bwd(const __nv_bfloat16 *__restrict__ dy, __nv_bfloat16 *__restrict__ dx, GapArgs a,
+                                                          int blocks) {
+    const int n = blockIdx.x / blocks;
+    const int i = (blockIdx.x - n * blocks) * POOL_THREADS + threadIdx.x;
+    if (i >= a.HW * a.G) return;
+    const int g = i % a.G, px = i / a.G;
+    const BfVec<VEC> d = *reinterpret_cast<const BfVec<VEC> *>(dy + (long)n * a.pitch + g * VEC);
+    BfVec<VEC> out;
+#pragma unroll
+    for (int c = 0; c < VEC; ++c) out.h[c] = __float2bfloat16_rn(div_rn(__bfloat162float(d.h[c]), a.hw, a.rhw));
+    *reinterpret_cast<BfVec<VEC> *>(dx + ((long)n * a.HW + px) * a.C + g * VEC) = out;
+}
+
 struct PoolShape {
     PoolArgs args;
     int vec, cover;         // channels per thread; most windows over one input pixel
@@ -195,11 +374,9 @@ int pool_grid(const char *fn, int N, PoolArgs *a, int work, unsigned *grid) {
     return PCNN_OK;
 }
 
-}  // namespace
-
-extern "C" int pcnn_maxpool_nhwc_info(int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int row_pitch,
-                                      int image_rows, int *out5) {
-    const char *fn = "pcnn_maxpool_nhwc_info";
+// out5 of pcnn_maxpool_nhwc_info and pcnn_avgpool_nhwc_info
+int pool_info(const char *fn, int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int row_pitch, int image_rows,
+              int *out5) {
     PCNN_REQUIRE(out5, PCNN_ERR_ARG, "%s: NULL out5", fn);
     PoolShape sh;
     int rc = pool_shape(fn, N, H, W, C, R, S, stride, pad_h, pad_w, row_pitch, image_rows, &sh);
@@ -209,6 +386,168 @@ extern "C" int pcnn_maxpool_nhwc_info(int N, int H, int W, int C, int R, int S, 
     out5[2] = sh.args.pitch;
     out5[3] = sh.vec;
     out5[4] = sh.cover;
+    return PCNN_OK;
+}
+
+int include_pad_flag(const char *fn, int count_include_pad) {
+    PCNN_REQUIRE(count_include_pad == 0 || count_include_pad == 1, PCNN_ERR_ARG, "%s: count_include_pad = %d: 0 or 1 is required", fn,
+                 count_include_pad);
+    return PCNN_OK;
+}
+
+// the global pool's domain and partition, a function of (N, H, W, C) and the row pitch alone
+int gap_shape(const char *fn, int N, int H, int W, int C, int row_pitch, GapArgs *a) {
+    PCNN_REQUIRE(N >= 1 && H >= 1 && W >= 1 && C >= 1, PCNN_ERR_ARG, "%s: N = %d, H = %d, W = %d, C = %d: each must be >= 1", fn, N, H, W,
+                 C);
+    const int vec = C % 8 == 0 ? 8 : 1, G = C / vec;
+    PCNN_REQUIRE((long)H * W * C <= INT32_MAX - POOL_THREADS, PCNN_ERR_ARG,
+                 "%s: one %dx%dx%d image exceeds the 32-bit index range (H W C < 2^31 - 256 is required)", fn, H, W, C);
+    if (row_pitch == 0) row_pitch = (C + 7) / 8 * 8;
+    PCNN_REQUIRE(row_pitch >= C && row_pitch % 8 == 0, PCNN_ERR_ARG,
+                 "%s: row_pitch %d: 0 (C rounded up to 8) or a multiple of 8 that is >= C = %d is required", fn, row_pitch, C);
+    a->HW = H * W;
+    a->C = C;
+    a->G = G;
+    a->Gc = G < GAP_MAX_GROUPS ? G : GAP_MAX_GROUPS;
+    a->slices = (G + a->Gc - 1) / a->Gc;
+    a->lanes = POOL_THREADS / a->Gc;
+    a->per_cta = GAP_ITERS * a->lanes;
+    a->ranges = (a->HW + a->per_cta - 1) / a->per_cta;
+    a->pitch = row_pitch;
+    a->hw = (double)(float)a->HW;
+    a->rhw = 1.0 / a->hw;
+    PCNN_REQUIRE((long)N * a->ranges * a->slices <= INT32_MAX && (long)N * ((a->HW * G + POOL_THREADS - 1) / POOL_THREADS) <= INT32_MAX,
+                 PCNN_ERR_ARG, "%s: %d images of %dx%dx%d exceed the grid", fn, N, H, W, C);
+    return PCNN_OK;
+}
+
+}  // namespace
+
+extern "C" int pcnn_maxpool_nhwc_info(int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int row_pitch,
+                                      int image_rows, int *out5) {
+    return pool_info("pcnn_maxpool_nhwc_info", N, H, W, C, R, S, stride, pad_h, pad_w, row_pitch, image_rows, out5);
+}
+
+extern "C" int pcnn_avgpool_nhwc_info(int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int row_pitch,
+                                      int image_rows, int *out5) {
+    return pool_info("pcnn_avgpool_nhwc_info", N, H, W, C, R, S, stride, pad_h, pad_w, row_pitch, image_rows, out5);
+}
+
+extern "C" int pcnn_avgpool_nhwc_bf16_fwd(pcnn_ctx *ctx, const void *x_bf16_dev, void *y_bf16_dev, int N, int H, int W, int C, int R, int S,
+                                          int stride, int pad_h, int pad_w, int count_include_pad, int y_row_pitch, int y_image_rows) {
+    const char *fn = "pcnn_avgpool_nhwc_bf16_fwd";
+    PCNN_REQUIRE(ctx && x_bf16_dev && y_bf16_dev, PCNN_ERR_ARG, "%s: NULL context, x or y", fn);
+    int rc = include_pad_flag(fn, count_include_pad);
+    if (rc) return rc;
+    PoolShape sh;
+    if ((rc = pool_shape(fn, N, H, W, C, R, S, stride, pad_h, pad_w, y_row_pitch, y_image_rows, &sh))) return rc;
+    PoolArgs &a = sh.args;
+    PCNN_REQUIRE(aligned16(x_bf16_dev) && aligned16(y_bf16_dev), PCNN_ERR_ARG, "%s: x and y must be 16-byte aligned", fn);
+    const size_t xb = (size_t)N * H * W * C * 2, yb = (size_t)N * a.rows * a.pitch * 2;
+    PCNN_REQUIRE(!overlap(x_bf16_dev, xb, y_bf16_dev, yb), PCNN_ERR_ARG, "%s: overlapping buffers: x and y must not share memory", fn);
+    unsigned grid;
+    if ((rc = pool_grid(fn, N, &a, a.P * a.Q * a.G, &grid))) return rc;
+    pcnn_device_guard dg(ctx->device);
+    const auto *x = static_cast<const __nv_bfloat16 *>(x_bf16_dev);
+    auto *y = static_cast<__nv_bfloat16 *>(y_bf16_dev);
+    if (sh.vec == 8)
+        k_avgpool_nhwc_fwd<8><<<grid, POOL_THREADS, 0, ctx->stream>>>(x, y, a, count_include_pad);
+    else
+        k_avgpool_nhwc_fwd<1><<<grid, POOL_THREADS, 0, ctx->stream>>>(x, y, a, count_include_pad);
+    PCNN_CHECK_LAUNCH(ctx);
+    return PCNN_OK;
+}
+
+extern "C" int pcnn_avgpool_nhwc_bf16_bwd(pcnn_ctx *ctx, const void *dy_bf16_dev, void *dx_bf16_dev, int N, int H, int W, int C, int R, int S,
+                                          int stride, int pad_h, int pad_w, int count_include_pad, int dy_row_pitch, int dy_image_rows) {
+    const char *fn = "pcnn_avgpool_nhwc_bf16_bwd";
+    PCNN_REQUIRE(ctx && dy_bf16_dev && dx_bf16_dev, PCNN_ERR_ARG, "%s: NULL context, dy or dx", fn);
+    int rc = include_pad_flag(fn, count_include_pad);
+    if (rc) return rc;
+    PoolShape sh;
+    if ((rc = pool_shape(fn, N, H, W, C, R, S, stride, pad_h, pad_w, dy_row_pitch, dy_image_rows, &sh))) return rc;
+    PoolArgs &a = sh.args;
+    PCNN_REQUIRE(aligned16(dy_bf16_dev) && aligned16(dx_bf16_dev), PCNN_ERR_ARG, "%s: dy and dx must be 16-byte aligned", fn);
+    const size_t xb = (size_t)N * H * W * C * 2, yb = (size_t)N * a.rows * a.pitch * 2;
+    PCNN_REQUIRE(!overlap(dx_bf16_dev, xb, dy_bf16_dev, yb), PCNN_ERR_ARG, "%s: overlapping buffers: dy and dx must not share memory", fn);
+    unsigned grid;
+    if ((rc = pool_grid(fn, N, &a, H * W * a.G, &grid))) return rc;
+    pcnn_device_guard dg(ctx->device);
+    const auto *dy = static_cast<const __nv_bfloat16 *>(dy_bf16_dev);
+    auto *dx = static_cast<__nv_bfloat16 *>(dx_bf16_dev);
+    if (sh.vec == 8)
+        k_avgpool_nhwc_bwd<8><<<grid, POOL_THREADS, 0, ctx->stream>>>(dy, dx, a, count_include_pad);
+    else
+        k_avgpool_nhwc_bwd<1><<<grid, POOL_THREADS, 0, ctx->stream>>>(dy, dx, a, count_include_pad);
+    PCNN_CHECK_LAUNCH(ctx);
+    return PCNN_OK;
+}
+
+extern "C" int pcnn_global_avgpool_nhwc_info(int N, int H, int W, int C, int row_pitch, int *out8) {
+    const char *fn = "pcnn_global_avgpool_nhwc_info";
+    PCNN_REQUIRE(out8, PCNN_ERR_ARG, "%s: NULL out8", fn);
+    GapArgs a;
+    int rc = gap_shape(fn, N, H, W, C, row_pitch, &a);
+    if (rc) return rc;
+    out8[0] = a.pitch;
+    out8[1] = C / a.G;
+    out8[2] = a.Gc;
+    out8[3] = a.slices;
+    out8[4] = a.lanes;
+    out8[5] = a.per_cta;
+    out8[6] = a.ranges;
+    out8[7] = N * a.ranges * a.slices;
+    return PCNN_OK;
+}
+
+extern "C" int pcnn_global_avgpool_nhwc_bf16_fwd(pcnn_ctx *ctx, const void *x_bf16_dev, void *y_bf16_dev, int N, int H, int W, int C,
+                                                 int y_row_pitch) {
+    const char *fn = "pcnn_global_avgpool_nhwc_bf16_fwd";
+    PCNN_REQUIRE(ctx && x_bf16_dev && y_bf16_dev, PCNN_ERR_ARG, "%s: NULL context, x or y", fn);
+    GapArgs a;
+    int rc = gap_shape(fn, N, H, W, C, y_row_pitch, &a);
+    if (rc) return rc;
+    PCNN_REQUIRE(aligned16(x_bf16_dev) && aligned16(y_bf16_dev), PCNN_ERR_ARG, "%s: x and y must be 16-byte aligned", fn);
+    const size_t xb = (size_t)N * a.HW * C * 2, yb = (size_t)N * a.pitch * 2;
+    PCNN_REQUIRE(!overlap(x_bf16_dev, xb, y_bf16_dev, yb), PCNN_ERR_ARG, "%s: overlapping buffers: x and y must not share memory", fn);
+    pcnn_device_guard dg(ctx->device);
+    float *slots = nullptr;
+    if (a.ranges > 1 && (rc = pcnn_scratch(ctx, (size_t)N * a.ranges * C * sizeof(float), (void **)&slots))) return rc;
+    const auto *x = static_cast<const __nv_bfloat16 *>(x_bf16_dev);
+    auto *y = static_cast<__nv_bfloat16 *>(y_bf16_dev);
+    const unsigned grid = (unsigned)((long)N * a.ranges * a.slices);
+    if (C / a.G == 8)
+        k_gap_fwd<8><<<grid, POOL_THREADS, 0, ctx->stream>>>(x, y, slots, a);
+    else
+        k_gap_fwd<1><<<grid, POOL_THREADS, 0, ctx->stream>>>(x, y, slots, a);
+    PCNN_CHECK_LAUNCH(ctx);
+    if (a.ranges > 1) {
+        k_gap_finish<<<(unsigned)(((long)N * C + POOL_THREADS - 1) / POOL_THREADS), POOL_THREADS, 0, ctx->stream>>>(slots, y, N, a);
+        PCNN_CHECK_LAUNCH(ctx);
+    }
+    return PCNN_OK;
+}
+
+extern "C" int pcnn_global_avgpool_nhwc_bf16_bwd(pcnn_ctx *ctx, const void *dy_bf16_dev, void *dx_bf16_dev, int N, int H, int W, int C,
+                                                 int dy_row_pitch) {
+    const char *fn = "pcnn_global_avgpool_nhwc_bf16_bwd";
+    PCNN_REQUIRE(ctx && dy_bf16_dev && dx_bf16_dev, PCNN_ERR_ARG, "%s: NULL context, dy or dx", fn);
+    GapArgs a;
+    int rc = gap_shape(fn, N, H, W, C, dy_row_pitch, &a);
+    if (rc) return rc;
+    PCNN_REQUIRE(aligned16(dy_bf16_dev) && aligned16(dx_bf16_dev), PCNN_ERR_ARG, "%s: dy and dx must be 16-byte aligned", fn);
+    const size_t xb = (size_t)N * a.HW * C * 2, yb = (size_t)N * a.pitch * 2;
+    PCNN_REQUIRE(!overlap(dx_bf16_dev, xb, dy_bf16_dev, yb), PCNN_ERR_ARG, "%s: overlapping buffers: dy and dx must not share memory", fn);
+    pcnn_device_guard dg(ctx->device);
+    const int blocks = (a.HW * a.G + POOL_THREADS - 1) / POOL_THREADS;
+    const unsigned grid = (unsigned)((long)N * blocks);
+    const auto *dy = static_cast<const __nv_bfloat16 *>(dy_bf16_dev);
+    auto *dx = static_cast<__nv_bfloat16 *>(dx_bf16_dev);
+    if (C / a.G == 8)
+        k_gap_bwd<8><<<grid, POOL_THREADS, 0, ctx->stream>>>(dy, dx, a, blocks);
+    else
+        k_gap_bwd<1><<<grid, POOL_THREADS, 0, ctx->stream>>>(dy, dx, a, blocks);
+    PCNN_CHECK_LAUNCH(ctx);
     return PCNN_OK;
 }
 

@@ -4,8 +4,8 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import (F32, NPARAM, TEST_SET, TRAIN_SET, U8, PcnnError, batchnorm_nhwc_info, check, conv_layer_family, lib, linear_info,
-                   maxpool_nhwc_info)
+from ._lib import (F32, NPARAM, TEST_SET, TRAIN_SET, U8, PcnnError, avgpool_nhwc_info, batchnorm_nhwc_info, check, conv_layer_family,
+                   global_avgpool_nhwc_info, lib, linear_info, maxpool_nhwc_info)
 
 
 def _pixel_type(arr_or_dtype):
@@ -432,6 +432,28 @@ class Engine:
         self._call("pcnn_maxpool_nhwc_bf16_bwd", _p(dy), _p(argmax), _p(dx), int(N), int(H), int(W), int(Cin), int(R), int(S), int(stride),
                    ph, pw, int(row_pitch or 0), int(image_rows))
 
+    def avgpool_nhwc_fwd(self, x, y, N, H, W, Cin, R, S, stride, padding=(0, 0), count_include_pad=True, row_pitch=None, image_rows=0):
+        """pcnn_avgpool_nhwc_bf16_fwd: x dense bf16 [N][H][W][C] -> y [N][image_rows][row_pitch], each window's in-image sum over
+        R*S (count_include_pad) or over its in-image positions; row_pitch None = Q*C rounded up to 8, image_rows 0 = P"""
+        ph, pw = (int(v) for v in padding)
+        self._call("pcnn_avgpool_nhwc_bf16_fwd", _p(x), _p(y), int(N), int(H), int(W), int(Cin), int(R), int(S), int(stride), ph, pw,
+                   int(count_include_pad), int(row_pitch or 0), int(image_rows))
+
+    def avgpool_nhwc_bwd(self, dy, dx, N, H, W, Cin, R, S, stride, padding=(0, 0), count_include_pad=True, row_pitch=None, image_rows=0):
+        """pcnn_avgpool_nhwc_bf16_bwd: dy in y's layout -> dx dense bf16 [N][H][W][C], every element written"""
+        ph, pw = (int(v) for v in padding)
+        self._call("pcnn_avgpool_nhwc_bf16_bwd", _p(dy), _p(dx), int(N), int(H), int(W), int(Cin), int(R), int(S), int(stride), ph, pw,
+                   int(count_include_pad), int(row_pitch or 0), int(image_rows))
+
+    def global_avgpool_nhwc_fwd(self, x, y, N, H, W, Cin, row_pitch=None):
+        """pcnn_global_avgpool_nhwc_bf16_fwd: x dense bf16 [N][H][W][C] -> y [N][row_pitch], the mean over the H*W pixels;
+        row_pitch None = C rounded up to 8"""
+        self._call("pcnn_global_avgpool_nhwc_bf16_fwd", _p(x), _p(y), int(N), int(H), int(W), int(Cin), int(row_pitch or 0))
+
+    def global_avgpool_nhwc_bwd(self, dy, dx, N, H, W, Cin, row_pitch=None):
+        """pcnn_global_avgpool_nhwc_bf16_bwd: dy [N][row_pitch] -> dx dense bf16 [N][H][W][C] = dy / (H*W) at every pixel"""
+        self._call("pcnn_global_avgpool_nhwc_bf16_bwd", _p(dy), _p(dx), int(N), int(H), int(W), int(Cin), int(row_pitch or 0))
+
     def batchnorm_fwd(self, x, y, pixels, C, gamma, beta, running_mean=None, running_var=None, save_mean=None, save_rstd=None, r=None,
                       act=0, training=True, eps=1e-5, momentum=0.1):
         """pcnn_batchnorm_nhwc_bf16_fwd: y = bf16(act((x - mean) * rstd * gamma + beta (+ r))) over dense bf16 [pixels][C].
@@ -797,6 +819,69 @@ class MaxPoolLayer:
         self.argmax.free()
 
 
+class AvgPoolLayer:
+    """Average pooling between two layers (pcnn_avgpool_nhwc_bf16_fwd / _bwd), as avg_pool2d(kernel (R, S), stride, padding,
+    count_include_pad=count_include_pad): S defaults to R and stride to R, as torch does.  Layouts as MaxPoolLayer: x dense
+    [N][H][W][C], y in the layout the next layer reads as x (row_pitch None = Q*C rounded up to 8, image_rows 0 = P), dx dense.
+    It keeps no state: the backward reads dy alone."""
+
+    def __init__(self, engine, N, H, W, C, R, S=None, stride=None, padding=(0, 0), count_include_pad=True, row_pitch=None, image_rows=0):
+        self.engine = engine
+        S = R if S is None else S
+        stride = R if stride is None else stride
+        self.shape = (N, H, W, C, R, S)
+        self.stride = int(stride)
+        self.padding = tuple(int(v) for v in padding)
+        self.count_include_pad = bool(count_include_pad)
+        info = avgpool_nhwc_info(N, H, W, C, R, S, self.stride, self.padding, row_pitch or 0, image_rows)
+        self.row_pitch, self.image_rows = info["row_pitch"], int(image_rows)
+        self.out_shape = (N, info["P"], info["Q"], C)
+
+    def forward(self, x, y):
+        """y = the mean of each window of x"""
+        self.engine.avgpool_nhwc_fwd(x, y, *self.shape, self.stride, self.padding, self.count_include_pad, self.row_pitch, self.image_rows)
+
+    def backward(self, dy, dx):
+        """dx (dense, every element written) from dy (in y's layout)"""
+        self.engine.avgpool_nhwc_bwd(dy, dx, *self.shape, self.stride, self.padding, self.count_include_pad, self.row_pitch, self.image_rows)
+
+    def close(self):
+        pass
+
+
+class GlobalAvgPoolLayer:
+    """Global average pooling (pcnn_global_avgpool_nhwc_bf16_fwd / _bwd), as adaptive_avg_pool2d(x, 1): x and dx dense bf16
+    [N][H][W][C], y and dy [N][row_pitch] (row_pitch None = C rounded up to 8), the x layout of LinearLayer(engine, N, 1, 1, C, O).
+    It keeps no state; info is its partition (global_avgpool_nhwc_info)."""
+
+    def __init__(self, engine, N, H, W, C, row_pitch=None):
+        self.engine = engine
+        self.shape = (N, H, W, C)
+        self.info = global_avgpool_nhwc_info(N, H, W, C, row_pitch or 0)
+        self.row_pitch = self.info["row_pitch"]
+        self.out_shape = (N, C)
+
+    def forward(self, x, y):
+        """y[n][c] = the mean of x[n][:, :, c].  The head of a ResNet, z being a BatchNormLayer's output:
+
+            bn.forward(yc, z);  gap.forward(z, h);  fc.forward(h, logits)
+            engine.softmax_ce_bf16(logits, labels, N, O, 1 / N, dlogits)
+
+        with fc = LinearLayer(engine, N, 1, 1, C, O, w, b, row_pitch=gap.row_pitch) and h [N][gap.row_pitch]."""
+        self.engine.global_avgpool_nhwc_fwd(x, y, *self.shape, self.row_pitch)
+
+    def backward(self, dy, dx):
+        """dx = dy / (H*W) at every pixel: the chain of forward runs back as
+
+            fc.backward(logits, dlogits, dh);  gap.backward(dh, dz);  bn.backward(z, dz, dyc)
+
+        with dh in h's layout (its pad never read) and dz dense [N][H][W][C]."""
+        self.engine.global_avgpool_nhwc_bwd(dy, dx, *self.shape, self.row_pitch)
+
+    def close(self):
+        pass
+
+
 def f32_to_bf16_bits(a):
     """numpy float32 -> uint16 bf16 bit patterns (round to nearest even), the rounding the kernels use; NaN -> the quiet NaN
     0x7FC0 (rounding the payload could carry into the exponent and the sign: 0x7FFFFFFF would become -0)"""
@@ -811,4 +896,4 @@ def bf16_bits_to_f32(b):
 
 
 C_ = C
-__all__ = ["Engine", "DeviceArray", "ConvPlan", "WideConvPlan", "LinearPlan", "ConvLayer", "LinearLayer", "MaxPoolLayer", "BatchNormLayer", "f32_to_bf16_bits", "bf16_bits_to_f32", "TRAIN_SET", "TEST_SET", "U8", "F32"]
+__all__ = ["Engine", "DeviceArray", "ConvPlan", "WideConvPlan", "LinearPlan", "ConvLayer", "LinearLayer", "MaxPoolLayer", "AvgPoolLayer", "GlobalAvgPoolLayer", "BatchNormLayer", "f32_to_bf16_bits", "bf16_bits_to_f32", "TRAIN_SET", "TEST_SET", "U8", "F32"]

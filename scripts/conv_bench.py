@@ -615,6 +615,132 @@ def run_resblock(N, iters):
         layer.close()
 
 
+def run_avgpool(name, N, H, W, C, R, stride, pad, cip, iters):
+    """the NHWC average pool (pcnn_avgpool_nhwc_bf16_fwd / _bwd) next to torch's avg_pool2d and avg_pool2d_backward on the same
+    channels-last bf16 tensors.  Bytes: forward N*H*W*C*2 + N*P*Q*C*2 (read x, write y), backward the same (read dy, write dx);
+    re-reads of x or dy by overlapping windows come from L2 and are not counted."""
+    P, Q = (H + 2 * pad - R) // stride + 1, (W + 2 * pad - R) // stride + 1
+    x = torch.randint(0, 0x3F80, (N, H, W, C), dtype=torch.int16, device="cuda")
+    x ^= (torch.randint(0, 2, (N, H, W, C), dtype=torch.int16, device="cuda") << 15)
+    y = torch.empty((N, P, Q, C), dtype=torch.int16, device="cuda")
+    dy = torch.randint(0, 0x3F80, (N, P, Q, C), dtype=torch.int16, device="cuda")
+    dx = torch.empty((N, H, W, C), dtype=torch.int16, device="cuda")
+    xt, dyt = x.view(torch.bfloat16).permute(0, 3, 1, 2), dy.view(torch.bfloat16).permute(0, 3, 1, 2)   # channels-last views
+    gpu, power = card()
+    nbytes = (N * H * W * C + N * P * Q * C) * 2
+    args = (N, H, W, C, R, R, stride, (pad, pad), cip)
+    for what, fn, tfn in (
+            ("fwd", lambda: eng.avgpool_nhwc_fwd(x, y, *args),
+             lambda: torch.nn.functional.avg_pool2d(xt, R, stride, pad, count_include_pad=bool(cip))),
+            ("bwd", lambda: eng.avgpool_nhwc_bwd(dy, dx, *args),
+             lambda: torch.ops.aten.avg_pool2d_backward(dyt, xt, [R, R], [stride, stride], [pad, pad], False, bool(cip), None))):
+        ms, ms_torch = timed(fn, iters), timed(tfn, iters)
+        print(json.dumps({"case": f"{name} {what}", "N": N, "us": ms * 1e3, "MB": nbytes / 1e6, "hbm_frac": nbytes / (ms * 1e-3) / 1e9 / HBM,
+                          "torch_us": ms_torch * 1e3, "torch_over_ours": ms_torch / ms,
+                          "vec": pkg.avgpool_nhwc_info(*args[:7], args[7])["vec"], "gpu": gpu, "power_limit": power}), flush=True)
+    del x, y, dy, dx, xt, dyt
+
+
+def run_gap(name, N, H, W, C, iters):
+    """global average pooling (pcnn_global_avgpool_nhwc_bf16_fwd / _bwd) next to torch's x.mean((2, 3)), adaptive_avg_pool2d(x, 1)
+    and the autograd backward of the mean on the same channels-last bf16 tensors.  Bytes: forward N*H*W*C*2 + N*C*2 (read x, write
+    y), backward the same (read dy, write dx).  The forward's fp32 slots (written and read once, when an image has several pixel
+    ranges) are reported apart as slot_MB."""
+    info = pkg.global_avgpool_nhwc_info(N, H, W, C)
+    x = torch.randint(0, 0x3F80, (N, H, W, C), dtype=torch.int16, device="cuda")
+    y = torch.empty((N, info["row_pitch"]), dtype=torch.int16, device="cuda")
+    dy = torch.randint(0, 0x3F80, (N, info["row_pitch"]), dtype=torch.int16, device="cuda")
+    dx = torch.empty((N, H, W, C), dtype=torch.int16, device="cuda")
+    xt = x.view(torch.bfloat16).permute(0, 3, 1, 2)
+    xg = xt.detach().clone().requires_grad_(True)
+    mean = xg.mean((2, 3))
+    dyt = dy.view(torch.bfloat16)[:, :C]
+    gpu, power = card()
+    nbytes = (N * H * W * C + N * C) * 2
+    slot_bytes = 2 * N * info["ranges"] * C * 4 if info["ranges"] > 1 else 0
+    for what, fn, tfn, tname in (
+            ("fwd", lambda: eng.global_avgpool_nhwc_fwd(x, y, N, H, W, C), lambda: xt.mean((2, 3)), "mean"),
+            ("fwd", lambda: eng.global_avgpool_nhwc_fwd(x, y, N, H, W, C), lambda: torch.nn.functional.adaptive_avg_pool2d(xt, 1),
+             "adaptive_avg_pool2d"),
+            ("bwd", lambda: eng.global_avgpool_nhwc_bwd(dy, dx, N, H, W, C), lambda: torch.autograd.grad(mean, xg, dyt, retain_graph=True),
+             "mean autograd")):
+        ms, ms_torch = timed(fn, iters), timed(tfn, iters)
+        print(json.dumps({"case": f"{name} {what}", "N": N, "us": ms * 1e3, "MB": nbytes / 1e6, "hbm_frac": nbytes / (ms * 1e-3) / 1e9 / HBM,
+                          "slot_MB": slot_bytes / 1e6 if what == "fwd" else 0, "ranges": info["ranges"], "ctas": info["ctas"],
+                          "torch": tname, "torch_us": ms_torch * 1e3, "torch_over_ours": ms_torch / ms, "vec": info["vec"], "gpu": gpu,
+                          "power_limit": power}), flush=True)
+    del x, y, dy, dx, xt, xg, mean
+
+
+def run_resnetgap(N, iters):
+    """one training step of the GAP ResNet of tests/test_avgpool_nhwc_gpu.py (test_resnet_gap_mnist) at batch N: forward, softmax
+    cross-entropy, backward and the sgd of every layer on the engine's stream; next to it the torch eager step of the same layers on
+    bf16 channels-last tensors (fp32 masters, w -= lr * grad, re-cast to bf16)."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import test_avgpool_nhwc_gpu as T
+    assert N == T.NB
+    p = T.init_params()
+    net = T.ResNetGAP(eng, pkg, p)
+    xl = torch.randint(0, 0x3F80, (N * 28, 32), dtype=torch.int16, device="cuda")
+    labels = torch.randint(0, 10, (N,), dtype=torch.uint8, device="cuda")
+    lr = T.LR_STEP
+    gpu, power = card()
+
+    def step():
+        net.forward(xl.data_ptr(), labels)
+        net.backward()
+        net.sgd(lr)
+
+    ms = timed(step, iters)
+    net.close()
+    F = torch.nn.functional
+    xt = xl[:, :28].reshape(N, 28, 28, 1).view(torch.bfloat16).permute(0, 3, 1, 2)
+    lt = labels.long()
+    m32 = {k: torch.from_numpy(v).to("cuda") for k, v in p.items()}
+    for k in [k for k in m32 if k.startswith("f")]:
+        m32[k] = m32[k].permute(0, 3, 1, 2).contiguous(memory_format=torch.channels_last)
+    m32["w8"] = m32["w8"].reshape(10, -1)
+    for i, c in enumerate((8, 16, 16, 16, 32, 32, 32)):
+        m32[f"g{i}"], m32[f"b{i}"] = torch.ones(c, device="cuda"), torch.zeros(c, device="cuda")
+    mb = {k: (v.to(torch.bfloat16) if k[0] == "f" or k in ("w8", "b8") else v.clone()).requires_grad_(True) for k, v in m32.items()}
+    stats = [(torch.zeros(c, device="cuda"), torch.ones(c, device="cuda")) for c in (8, 16, 16, 16, 32, 32, 32)]
+    bn = lambda i, v: F.batch_norm(v, *stats[i], mb[f"g{i}"], mb[f"b{i}"], training=True)
+
+    def torch_step():
+        for v in mb.values():
+            v.grad = None
+        h = F.avg_pool2d(F.relu(bn(0, F.conv2d(xt, mb["f1"]))), 2)
+        x0 = F.relu(bn(1, F.conv2d(h, mb["f2"], padding=1)))
+        h = F.relu(bn(2, F.conv2d(x0, mb["f3"], padding=1)))
+        x1 = F.relu(bn(3, F.conv2d(h, mb["f4"], padding=1)) + x0)
+        h = F.relu(bn(4, F.conv2d(x1, mb["f5"], padding=1, stride=2)))
+        s = bn(6, F.conv2d(x1, mb["f7"], padding=1, stride=2))
+        h = F.relu(bn(5, F.conv2d(h, mb["f6"], padding=1)) + s)
+        F.cross_entropy(F.linear(F.adaptive_avg_pool2d(h, 1).flatten(1).to(torch.bfloat16), mb["w8"], mb["b8"]), lt).backward()
+        with torch.no_grad():
+            for k in m32:
+                m32[k].add_(mb[k].grad.float(), alpha=-lr)
+                mb[k].copy_(m32[k])
+
+    ms_torch = timed(torch_step, iters)
+    print(json.dumps({"case": f"GAP ResNet training step N={N}", "ms": ms, "torch_eager_ms": ms_torch, "ours_over_torch": ms / ms_torch,
+                      "gpu": gpu, "power_limit": power}), flush=True)
+
+
+if only == "avgpool":                                                  # average pooling between layers, torch beside it
+    run_avgpool("112x112x64, 2x2/2", 128, 112, 112, 64, 2, 2, 0, 1, 20)
+    run_avgpool("56x56x128, 2x2/2", 128, 56, 56, 128, 2, 2, 0, 1, 20)
+    run_avgpool("28x28x256, 3x3/1 pad 1, count_include_pad", 128, 28, 28, 256, 3, 1, 1, 1, 20)
+    run_avgpool("28x28x256, 3x3/1 pad 1, in-image count", 128, 28, 28, 256, 3, 1, 1, 0, 20)
+    run_avgpool("LeNet 24x24x6, 2x2/2 (scalar path)", 1024, 24, 24, 6, 2, 2, 0, 1, 20)
+if only == "gap":                                                      # global average pooling, torch beside it
+    run_gap("7x7x512", 128, 7, 7, 512, 50)
+    run_gap("7x7x2048", 128, 7, 7, 2048, 50)
+    run_gap("14x14x256", 128, 14, 14, 256, 50)
+    run_gap("56x56x64", 128, 56, 56, 64, 50)
+    run_gap("56x56x256 (split path)", 8, 56, 56, 256, 50)
+if only == "resnetgap":                                                # one step of the GAP ResNet, torch eager beside it
+    run_resnetgap(128, 20)
 if only == "bn":                                                       # batch normalization passes, torch beside them
     run_bn("56x56x64", 128, 56, 56, 64, 50)
     run_bn("28x28x128", 128, 28, 28, 128, 50)

@@ -1,0 +1,61 @@
+#!/usr/bin/env python
+"""scripts/resnetgap_replica.py -- float32 torch CPU replica of the GAP ResNet of tests/test_avgpool_nhwc_gpu.py
+(test_resnet_gap_mnist): the same layers, initialisation, batch order (8 batches of 128 over the 1024 golden training digits per
+epoch), softmax cross-entropy over the batch and plain SGD, evaluated on the 256 golden test digits with the running statistics.
+Its accuracy sets the test's threshold.  Usage: resnetgap_replica.py [step ...]"""
+import os
+import sys
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+from test_avgpool_nhwc_gpu import EPOCHS, NB, init_params  # noqa: E402
+
+F = torch.nn.functional
+
+
+def run(lr):
+    torch.manual_seed(0)
+    g = np.load(os.path.join(ROOT, "tests", "golden", "mnist_subset.npz"))
+    img = lambda u8: torch.from_numpy(u8.reshape(-1, 1, 28, 28).astype(np.float32) / 255.0).bfloat16().float()   # the device's bf16 input
+    xs, ys, xt, yt = img(g["train_u8"]), torch.from_numpy(g["train_labels"]).long(), img(g["test_u8"]), torch.from_numpy(g["test_labels"]).long()
+    p = {k: torch.from_numpy(v) for k, v in init_params().items()}
+    w = {k: (p[k].permute(0, 3, 1, 2).contiguous() if k.startswith("f") else p[k].reshape(10, -1) if k == "w8" else p[k]).requires_grad_(True)
+         for k in p}
+    bn = [(torch.ones(c, requires_grad=True), torch.zeros(c, requires_grad=True), torch.zeros(c), torch.ones(c)) for c in (8, 16, 16, 16, 32, 32, 32)]
+
+    def b(i, v, training):
+        ga, be, rm, rv = bn[i]
+        return F.batch_norm(v, rm, rv, ga, be, training=training, momentum=0.1, eps=1e-5)
+
+    def net(x, training):
+        h = F.avg_pool2d(F.relu(b(0, F.conv2d(x, w["f1"]), training)), 2)
+        x0 = F.relu(b(1, F.conv2d(h, w["f2"], padding=1), training))
+        h = F.relu(b(2, F.conv2d(x0, w["f3"], padding=1), training))
+        x1 = F.relu(b(3, F.conv2d(h, w["f4"], padding=1), training) + x0)
+        h = F.relu(b(4, F.conv2d(x1, w["f5"], padding=1, stride=2), training))
+        s = b(6, F.conv2d(x1, w["f7"], padding=1, stride=2), training)
+        h = F.relu(b(5, F.conv2d(h, w["f6"], padding=1), training) + s)
+        return F.linear(F.adaptive_avg_pool2d(h, 1).flatten(1), w["w8"], w["b8"])
+
+    params = list(w.values()) + [t for ga, be, _, _ in bn for t in (ga, be)]
+    losses = []
+    for ep in range(EPOCHS):
+        for s in range(1024 // NB):
+            loss = F.cross_entropy(net(xs[s * NB:(s + 1) * NB], True), ys[s * NB:(s + 1) * NB])
+            for t in params:
+                t.grad = None
+            loss.backward()
+            with torch.no_grad():
+                for t in params:
+                    t.add_(t.grad, alpha=-lr)
+            losses.append(float(loss))
+    with torch.no_grad():
+        acc = float((net(xt, False).argmax(1) == yt).float().mean())
+    print(f"step {lr}: mean loss epoch 1 {np.mean(losses[:8]):.4f} -> epoch {EPOCHS} {np.mean(losses[-8:]):.4f}; test accuracy {acc:.4f}", flush=True)
+
+
+for lr in [float(a) for a in sys.argv[1:]] or [0.1]:
+    run(lr)

@@ -1,0 +1,419 @@
+"""The NHWC average pools on the device (pcnn_avgpool_nhwc_bf16_fwd / _bwd, pcnn_global_avgpool_nhwc_bf16_fwd / _bwd, AvgPoolLayer,
+GlobalAvgPoolLayer): windowed y and dx and global dx bit-identical to the float32 replays of tests/avgpool_ref.py (pinned to
+torch's CPU float64 pools by test_avgpool_nhwc_cpu.py), global y exact on integer operands and within an error model on random
+ones, torch's CUDA pools on the same channels-last bf16 tensors recorded, every refusal, and a ResNet with a projection block and a
+global-average-pool head trained on MNIST digits.
+
+Error model of the global forward (random operands).  With n_acc = (pixels per lane - 1) + (lanes - 1) + (ranges - 1) additions on
+the longest path of the partition global_avgpool_nhwc_info reports, u = 2^-24, gamma = n_acc u / (1 - n_acc u), S the exact sum of
+an image's channel and A the sum of its absolute values: |s - S| <= gamma A, and the quotient q = fl(s / HW) satisfies
+|q - S / HW| <= E = (gamma A + u (|S| + gamma A)) / HW.  bf16 rounding is monotonic, so y lies between bf16_rn(S/HW - E) and
+bf16_rn(S/HW + E)."""
+import numpy as np
+import pytest
+import torch
+
+import avgpool_ref as AR
+import maxpool_ref as MR
+
+pytestmark = pytest.mark.gpu
+
+DEV = torch.device("cuda", 0)
+NAN_BF16 = 0x7FC0
+U = 2.0 ** -24
+
+CASES = [  # id, N, H, W, C, R, S, stride, pad_h, pad_w, row_pitch (0 = Q*C rounded up to 8), image_rows (0 = P)
+    ("c1-2x2s2", 2, 10, 9, 1, 2, 2, 2, 0, 0, 0, 0),
+    ("c3-2x2s2", 2, 10, 9, 3, 2, 2, 2, 0, 0, 0, 0),
+    ("c6-2x2s2-pitched", 3, 24, 24, 6, 2, 2, 2, 0, 0, 80, 14),
+    ("c16-2x2s2", 2, 10, 9, 16, 2, 2, 2, 0, 0, 0, 0),
+    ("c64-3x3s1p1", 2, 9, 11, 64, 3, 3, 1, 1, 1, 0, 0),
+    ("c256-2x2s2", 2, 10, 9, 256, 2, 2, 2, 0, 0, 0, 0),
+    ("c320-3x3s2p1-odd", 2, 9, 7, 320, 3, 3, 2, 1, 1, 0, 0),
+    ("c16-3x3s2p1-odd", 2, 13, 11, 16, 3, 3, 2, 1, 1, 0, 0),
+    ("c6-3x3s2p1-odd", 3, 9, 7, 6, 3, 3, 2, 1, 1, 0, 0),
+    ("c3-3x3s1p1-odd", 2, 7, 9, 3, 3, 3, 1, 1, 1, 0, 0),
+    ("c8-3x2s3-gaps", 2, 11, 10, 8, 3, 2, 3, 0, 0, 0, 0),
+    ("c6-3x2s3-gaps-pad", 2, 11, 10, 6, 3, 2, 3, 1, 1, 0, 0),
+    ("c16-7x7s7", 2, 15, 14, 16, 7, 7, 7, 0, 0, 0, 0),
+    ("c3-7x7s7p3", 1, 14, 16, 3, 7, 7, 7, 3, 3, 0, 0),
+    ("c1-1row-1x3s1p1", 3, 1, 9, 1, 1, 3, 1, 0, 1, 0, 0),
+    ("c16-pitched-3x3s2p1", 2, 12, 12, 16, 3, 3, 2, 1, 1, 104, 9),
+    ("many-ctas-128x56x56x64", 128, 56, 56, 64, 2, 2, 2, 0, 0, 0, 0),
+]
+
+
+def same_or_nan(got, want):
+    """bf16 bits: identical where want is a number; NaN (any payload) where want is NaN"""
+    nan, gnan = (want & 0x7FFF) > 0x7F80, (got & 0x7FFF) > 0x7F80
+    return np.array_equal(gnan, nan) and np.array_equal(got[~nan], want[~nan])
+
+
+def special_x(rng, shape):
+    """normal values with NaN, +-Inf and +-0 sprinkled in, and rows of -0"""
+    x = rng.standard_normal(shape).astype(np.float32)
+    flat = x.reshape(-1)
+    for v, frac in ((np.nan, 0.01), (np.inf, 0.01), (-np.inf, 0.01), (0.0, 0.05), (-0.0, 0.05)):
+        flat[rng.choice(flat.size, max(1, int(frac * flat.size)), replace=False)] = v
+    x[:, ::4] = -0.0
+    return x
+
+
+def layout(case):
+    _, N, H, W, C, R, S, st, ph, pw, pitch, rows = case
+    P, Q = MR.out_size(H, W, R, S, st, ph, pw)
+    return P, Q, (pitch or (Q * C + 7) // 8 * 8), (rows or P)
+
+
+def run_fwd(eng, case, cip, x_bits):
+    _, N, H, W, C, R, S, st, ph, pw, pitch, rows = case
+    P, Q, pitch_u, rows_u = layout(case)
+    y = eng.to_device(np.full((N, rows_u, pitch_u), NAN_BF16, np.uint16))
+    eng.avgpool_nhwc_fwd(eng.to_device(x_bits), y, N, H, W, C, R, S, st, (ph, pw), cip, pitch, rows)
+    eng.sync()
+    return y.to_host()
+
+
+def run_bwd(eng, case, cip, dy_img, pad_value=NAN_BF16):
+    _, N, H, W, C, R, S, st, ph, pw, pitch, rows = case
+    P, Q, pitch_u, rows_u = layout(case)
+    dy = np.full((N, rows_u, pitch_u), pad_value, np.uint16)
+    dy[:, :P, :Q * C] = dy_img.reshape(N, P, Q * C)
+    dx = eng.to_device(np.full((N, H, W, C), NAN_BF16, np.uint16))
+    eng.avgpool_nhwc_bwd(eng.to_device(dy), dx, N, H, W, C, R, S, st, (ph, pw), cip, pitch, rows)
+    eng.sync()
+    return dx.to_host()
+
+
+def cuda_bf16(bits):
+    return torch.from_numpy(np.ascontiguousarray(bits).view(np.int16)).to(DEV).view(torch.bfloat16).permute(0, 3, 1, 2)
+
+
+def host_bits(t):
+    return t.permute(0, 2, 3, 1).contiguous().view(torch.int16).cpu().numpy().view(np.uint16)
+
+
+@pytest.mark.parametrize("cip", [0, 1])
+@pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
+def test_windowed(eng, pkg, case, cip):
+    _, N, H, W, C, R, S, st, ph, pw, pitch, rows = case
+    P, Q, pitch_u, rows_u = layout(case)
+    assert pkg.avgpool_nhwc_info(N, H, W, C, R, S, st, (ph, pw), pitch, rows)["row_pitch"] == pitch_u
+    rng = np.random.default_rng(sum(case[1:]) + cip)
+    bf, f32 = pkg.f32_to_bf16_bits, pkg.bf16_bits_to_f32
+    img = lambda y: y[:, :P, :Q * C].reshape(N, P, Q, C)
+    cnt = AR.counts(H, W, R, S, st, ph, pw, cip)
+    pow2 = bool(np.all((cnt & (cnt - 1)) == 0))
+    for kind, x_bits in (("random", bf(rng.standard_normal((N, H, W, C)).astype(np.float32))), ("special", bf(special_x(rng, (N, H, W, C)))),
+                         ("integer", bf(rng.integers(-4, 5, (N, H, W, C)).astype(np.float32)))):
+        y = run_fwd(eng, case, cip, x_bits)
+        want = bf(AR.fwd(f32(x_bits), R, S, st, ph, pw, cip))
+        assert same_or_nan(img(y), want), (kind, int(np.sum(img(y) != want)))
+        assert np.all(y[:, :P, Q * C:] == NAN_BF16) and np.all(y[:, P:, :] == NAN_BF16)          # pad untouched
+        assert np.array_equal(run_fwd(eng, case, cip, x_bits), y)                               # rerun
+        if kind == "special":
+            continue
+        dy = bf(rng.integers(-3, 4, (N, P, Q, C)).astype(np.float32) if kind == "integer" else rng.standard_normal((N, P, Q, C)).astype(np.float32))
+        dx = run_bwd(eng, case, cip, dy)
+        want_dx, terms = AR.bwd(f32(dy), H, W, R, S, st, ph, pw, cip)
+        assert np.array_equal(dx, bf(want_dx)), (kind, int(np.sum(dx != bf(want_dx))))
+        assert np.all(dx[:, terms == 0] == 0)                                                   # +0 with no term
+        assert np.array_equal(run_bwd(eng, case, cip, dy, pad_value=0), dx)                     # NaN in dy's pad changes no bit
+        assert np.array_equal(run_bwd(eng, case, cip, dy), dx)                                  # rerun
+        if kind == "integer" and pow2:                                                          # exact adjoint: <y, dy> = <x, dx>
+            lhs = np.sum(f32(dy).astype(np.float64) * f32(img(y)))
+            rhs = np.sum(f32(dx).astype(np.float64) * f32(x_bits))
+            assert lhs == rhs
+        if kind == "random":                                                                    # torch CUDA, recorded
+            xt = cuda_bf16(x_bits).requires_grad_(True)
+            ty = torch.nn.functional.avg_pool2d(xt, (R, S), st, (ph, pw), count_include_pad=bool(cip))
+            ty.backward(cuda_bf16(dy))
+            print(f"{case[0]} cip={cip} vs torch CUDA: y bits differ on {int(np.sum(host_bits(ty.detach()) != img(y)))} of {img(y).size}, "
+                  f"dx on {int(np.sum(host_bits(xt.grad) != dx))} of {dx.size}")
+    # the layer drives the same calls
+    layer = pkg.AvgPoolLayer(eng, N, H, W, C, R, S, st, (ph, pw), bool(cip), pitch or None, rows)
+    assert layer.out_shape == (N, P, Q, C) and layer.row_pitch == pitch_u
+
+
+GSHAPES = [(3, H, W, C) for C in (1, 6, 8, 300, 2048) for H, W in ((1, 1), (7, 7), (56, 56))] + [(8, 56, 56, 256)]
+
+
+def gap_bound(pkg, xf, info):
+    """[lo, hi] of the error model (module docstring) for every y, as float32 values"""
+    N, H, W, C = xf.shape
+    n_acc = (info["pixels_per_cta"] // info["lanes"] - 1) + (info["lanes"] - 1) + (info["ranges"] - 1)
+    gamma = n_acc * U / (1 - n_acc * U)
+    x64 = xf.astype(np.float64)
+    S, A = x64.sum(axis=(1, 2)), np.abs(x64).sum(axis=(1, 2))
+    m, E = S / (H * W), (gamma * A + U * (np.abs(S) + gamma * A)) / (H * W)
+    bf, f32 = pkg.f32_to_bf16_bits, pkg.bf16_bits_to_f32
+    return m, E, f32(bf((m - E).astype(np.float32))), f32(bf((m + E).astype(np.float32)))
+
+
+@pytest.mark.parametrize("shape", GSHAPES, ids=["x".join(map(str, s)) for s in GSHAPES])
+def test_global(eng, pkg, shape):
+    N, H, W, C = shape
+    rng = np.random.default_rng(sum(shape))
+    bf, f32 = pkg.f32_to_bf16_bits, pkg.bf16_bits_to_f32
+    for pitch in (0, (C + 7) // 8 * 8 + 8):
+        info = pkg.global_avgpool_nhwc_info(N, H, W, C, pitch)
+        pu = info["row_pitch"]
+        layer = pkg.GlobalAvgPoolLayer(eng, N, H, W, C, pitch or None)
+        assert layer.info == info
+
+        def fwd(x_bits):
+            y = eng.to_device(np.full((N, pu), NAN_BF16, np.uint16))
+            layer.forward(eng.to_device(x_bits), y)
+            eng.sync()
+            return y.to_host()
+
+        x_int = bf(rng.integers(-8, 9, shape).astype(np.float32))
+        y = fwd(x_int)
+        assert np.array_equal(y[:, :C], bf(AR.global_fwd(f32(x_int), info)))                   # exact sums
+        assert np.all(y[:, C:] == NAN_BF16)
+        x_rnd = bf((rng.standard_normal(shape) + 0.5).astype(np.float32))
+        y = fwd(x_rnd)
+        m, E, lo, hi = gap_bound(pkg, f32(x_rnd), info)
+        yf = f32(y[:, :C])
+        assert np.all((yf >= lo) & (yf <= hi))
+        ulp = np.maximum(np.abs(m), 2.0 ** -126) * 2.0 ** -8
+        ratio = float(np.max(np.abs(yf - m) / (E + ulp / 2)))
+        diff = int(np.sum(y[:, :C] != bf(AR.global_fwd(f32(x_rnd), info))))
+        print(f"GAP {shape} pitch {pu}: {info['ranges']} ranges, {info['ctas']} CTAs; worst |y - mean| / (E + half bf16 ulp) {ratio:.3f}; "
+              f"bits differing from the ordered float32 replay {diff}")
+        assert np.array_equal(fwd(x_rnd), y)                                                    # rerun
+        dy_img = bf(rng.standard_normal((N, C)).astype(np.float32))
+        dy = np.full((N, pu), NAN_BF16, np.uint16)
+        dy[:, :C] = dy_img
+        dx = eng.to_device(np.full((N, H, W, C), NAN_BF16, np.uint16))
+        layer.backward(eng.to_device(dy), dx)
+        eng.sync()
+        assert np.array_equal(dx.to_host(), bf(AR.global_bwd(f32(dy_img), H, W)))             # every pixel written, pad never read
+        if pitch == 0 and N * H * W * C < 1 << 24:                                              # torch CUDA, recorded
+            xt = cuda_bf16(x_rnd.reshape(shape))
+            ty = xt.mean((2, 3)).contiguous().view(torch.int16).cpu().numpy().view(np.uint16)
+            ta = torch.nn.functional.adaptive_avg_pool2d(xt, 1)[:, :, 0, 0].contiguous().view(torch.int16).cpu().numpy().view(np.uint16)
+            print(f"GAP {shape} vs torch CUDA: mean differs on {int(np.sum(ty != y[:, :C]))}, adaptive_avg_pool2d on "
+                  f"{int(np.sum(ta != y[:, :C]))} of {N * C}")
+
+
+def test_refusals(eng, pkg):
+    N, H, W, C = 2, 8, 8, 16
+    x = eng.array((N, H, W, C + 8), np.uint16)
+    y = eng.array((N, 4, 4 * C + 8), np.uint16)
+    dx = eng.array((N, H, W, C + 8), np.uint16)
+    fwd, bwd = eng.avgpool_nhwc_fwd, eng.avgpool_nhwc_bwd
+    gf, gb = eng.global_avgpool_nhwc_fwd, eng.global_avgpool_nhwc_bwd
+    shape = (N, H, W, C, 2, 2, 2)
+    cases = [
+        (lambda: fwd(x, y, N, H, W, C, 8, 2, 2), "pcnn_avgpool_nhwc_bf16_fwd: 8x2 window: 1 <= R, S <= 7"),
+        (lambda: fwd(x, y, 0, H, W, C, 2, 2, 2), "each must be >= 1"),
+        (lambda: fwd(x, y, N, H, W, C, 2, 2, 8), "1 <= stride <= 7"),
+        (lambda: fwd(x, y, N, H, W, C, 3, 3, 2, (2, 0)), "pad_h <= R/2"),
+        (lambda: fwd(x, y, N, 1, W, C, 7, 2, 2, (2, 0)), "H \\+ 2 pad_h >= R"),
+        (lambda: fwd(x, y, *shape, row_pitch=60), "row_pitch 60"),
+        (lambda: fwd(x, y, *shape, image_rows=3), "image_rows 3"),
+        (lambda: fwd(x, y, *shape, count_include_pad=2), "pcnn_avgpool_nhwc_bf16_fwd: count_include_pad = 2: 0 or 1"),
+        (lambda: bwd(y, dx, *shape, count_include_pad=-1), "pcnn_avgpool_nhwc_bf16_bwd: count_include_pad = -1: 0 or 1"),
+        (lambda: bwd(y, dx, N, H, W, C, 2, 2, 2, (0, 2)), "pcnn_avgpool_nhwc_bf16_bwd: padding \\(0, 2\\)"),
+        (lambda: bwd(y, dx, *shape, row_pitch=68), "multiple of 8"),
+        (lambda: fwd(None, y, *shape), "NULL context, x or y"),
+        (lambda: fwd(x, None, *shape), "NULL context, x or y"),
+        (lambda: bwd(None, dx, *shape), "NULL context, dy or dx"),
+        (lambda: bwd(y, None, *shape), "NULL context, dy or dx"),
+        (lambda: fwd(x.ptr + 2, y, *shape), "16-byte aligned"),
+        (lambda: fwd(x, y.ptr + 8, *shape), "16-byte aligned"),
+        (lambda: bwd(y.ptr + 4, dx, *shape), "16-byte aligned"),
+        (lambda: bwd(y, dx.ptr + 2, *shape), "16-byte aligned"),
+        (lambda: fwd(x, x.ptr + 64, *shape), "overlapping buffers"),
+        (lambda: bwd(y, y, *shape), "overlapping buffers"),
+        (lambda: gf(x, y, 0, H, W, C), "pcnn_global_avgpool_nhwc_bf16_fwd: N = 0, H = 8, W = 8, C = 16: each must be >= 1"),
+        (lambda: gb(y, dx, N, H, 0, C), "pcnn_global_avgpool_nhwc_bf16_bwd: .* each must be >= 1"),
+        (lambda: gf(x, y, N, 46341, 46341, 1), "32-bit index range"),
+        (lambda: gf(x, y, N, H, W, C, row_pitch=12), "row_pitch 12: 0 \\(C rounded up to 8\\) or a multiple of 8"),
+        (lambda: gb(y, dx, N, H, W, C, row_pitch=8), "row_pitch 8"),
+        (lambda: gf(None, y, N, H, W, C), "NULL context, x or y"),
+        (lambda: gb(y, None, N, H, W, C), "NULL context, dy or dx"),
+        (lambda: gf(x.ptr + 2, y, N, H, W, C), "16-byte aligned"),
+        (lambda: gb(y, dx.ptr + 8, N, H, W, C), "16-byte aligned"),
+        (lambda: gf(x, x.ptr + 32, N, H, W, C), "overlapping buffers"),
+        (lambda: gb(dx.ptr + 64, dx, N, H, W, C), "overlapping buffers"),
+    ]
+    for fn, msg in cases:
+        with pytest.raises(pkg.PcnnError, match=msg):
+            fn()
+    fwd(x, y, *shape)
+    gf(x, y, N, H, W, C)
+    eng.sync()
+
+
+# ------------------------------------------------------------------------------------------------ end to end
+NB = 128
+LR_STEP = 0.2
+EPOCHS = 40
+ACC_MIN = 0.88          # a float32 torch CPU replica of this network, initialisation and step reaches 0.949 (DESIGN 3.16)
+
+
+def init_params(seed=9):
+    rng = np.random.default_rng(seed)
+    u = lambda shape, fan: rng.uniform(-1, 1, shape).astype(np.float32) / np.float32(np.sqrt(fan))
+    return dict(f1=u((8, 5, 5, 1), 25), f2=u((16, 3, 3, 8), 72), f3=u((16, 3, 3, 16), 144), f4=u((16, 3, 3, 16), 144),
+                f5=u((32, 3, 3, 16), 144), f6=u((32, 3, 3, 32), 288), f7=u((32, 3, 3, 16), 144), w8=u((10, 1, 1, 32), 32), b8=u(10, 32))
+
+
+class ResNetGAP:
+    """conv 8@5x5 -> BN+ReLU -> avg pool 2 -> conv 16@3x3 pad 1 -> BN+ReLU (x0) -> [conv 16@3x3 pad 1 -> BN+ReLU -> conv 16@3x3
+    pad 1 -> BN + x0 -> ReLU] (x1) -> [conv 32@3x3 stride 2 pad 1 -> BN+ReLU -> conv 32@3x3 pad 1 -> BN + s -> ReLU, s = BN(conv
+    32@3x3 stride 2 pad 1 (x1))] -> GAP -> fc 32->10 -> softmax CE (1/B).  The convs have no bias.  The projection is 3x3 rather
+    than ResNet's 1x1: a 1x1 stride-2 conv over 16 channels is a row-Toeplitz layer, whose input gradient has no 1x1 kernel."""
+
+    def __init__(self, eng, pkg, p):
+        self.eng = eng
+        relu, none = pkg.ACT_RELU, pkg.ACT_NONE
+        B = NB
+        conv = lambda H, C, K, R, f, **k: pkg.ConvLayer(eng, B, H, H, C, K, R, R, p[f], None, act=none, **k)
+        self.c1 = conv(28, 1, 8, 5, "f1")
+        self.c2 = conv(12, 8, 16, 3, "f2", padding=(1, 1))
+        self.c3, self.c4 = conv(12, 16, 16, 3, "f3", padding=(1, 1)), conv(12, 16, 16, 3, "f4", padding=(1, 1))
+        self.c5 = conv(12, 16, 32, 3, "f5", padding=(1, 1), stride=2)
+        self.c6 = conv(6, 32, 32, 3, "f6", padding=(1, 1))
+        self.c7 = conv(12, 16, 32, 3, "f7", padding=(1, 1), stride=2)
+        assert self.c5.out_shape == self.c7.out_shape == (B, 6, 6, 32)
+        BN = lambda H, C, act: pkg.BatchNormLayer(eng, B, H, H, C, act=act)
+        self.bn = [BN(24, 8, relu), BN(12, 16, relu), BN(12, 16, relu), BN(12, 16, relu), BN(6, 32, relu), BN(6, 32, relu), BN(6, 32, none)]
+        self.pool = pkg.AvgPoolLayer(eng, B, 24, 24, 8, 2, row_pitch=self.c2.row_pitch, image_rows=self.c2.image_rows)
+        self.gap = pkg.GlobalAvgPoolLayer(eng, B, 6, 6, 32)
+        self.fc = pkg.LinearLayer(eng, B, 1, 1, 32, 10, p["w8"], p["b8"], act=none, row_pitch=self.gap.row_pitch)
+        buf = lambda *shape: torch.full(shape, NAN_BF16, dtype=torch.int16, device=DEV)
+        self.y1, self.z1, self.dz1, self.dy1 = (buf(B, 24, 24, 8) for _ in range(4))
+        self.x2, self.dx2 = buf(B, 12, self.c2.row_pitch), buf(B, 12, self.c2.row_pitch)
+        (self.y2, self.x0, self.y3, self.z3, self.y4, self.x1, self.dx1, self.dx1p, self.dy4, self.dres, self.dz3, self.dy3, self.dx0,
+         self.dy2) = (buf(B, 12, 12, 16) for _ in range(14))
+        (self.y5, self.z5, self.y6, self.out, self.y7, self.s, self.dout, self.dy6, self.ds, self.dy7, self.dz5,
+         self.dy5) = (buf(B, 6, 6, 32) for _ in range(12))
+        self.h, self.dh = buf(B, self.gap.row_pitch), buf(B, self.gap.row_pitch)
+        self.z, self.dz = buf(B, 10), buf(B, 10)
+        self.loss = torch.zeros(B, dtype=torch.float32, device=DEV)
+        self.pred = torch.zeros(B, dtype=torch.int32, device=DEV)
+
+    def forward(self, x, labels, training=True):
+        b1, b2, b3, b4, b5, b6, b7 = self.bn
+        self.c1.forward(x, self.y1)
+        b1.forward(self.y1, self.z1, training=training)
+        self.pool.forward(self.z1, self.x2)
+        self.c2.forward(self.x2, self.y2)
+        b2.forward(self.y2, self.x0, training=training)
+        self.c3.forward(self.x0, self.y3)
+        b3.forward(self.y3, self.z3, training=training)
+        self.c4.forward(self.z3, self.y4)
+        b4.forward(self.y4, self.x1, r=self.x0, training=training)
+        self.c5.forward(self.x1, self.y5)
+        b5.forward(self.y5, self.z5, training=training)
+        self.c6.forward(self.z5, self.y6)
+        self.c7.forward(self.x1, self.y7)
+        b7.forward(self.y7, self.s, training=training)
+        b6.forward(self.y6, self.out, r=self.s, training=training)
+        self.gap.forward(self.out, self.h)
+        self.fc.forward(self.h, self.z)
+        self.eng.softmax_ce_bf16(self.z, labels, NB, 10, 1.0 / NB, self.dz, self.loss, self.pred)
+
+    def backward(self):
+        b1, b2, b3, b4, b5, b6, b7 = self.bn
+        self.fc.backward(self.z, self.dz, self.dh)
+        self.gap.backward(self.dh, self.dout)
+        b6.backward(self.out, self.dout, self.dy6, dr=self.ds)
+        self.c6.backward(self.y6, self.dy6, self.dz5)
+        b5.backward(self.z5, self.dz5, self.dy5)
+        self.c5.backward(self.y5, self.dy5, self.dx1)
+        b7.backward(self.s, self.ds, self.dy7)
+        self.c7.backward(self.y7, self.dy7, self.dx1p)
+        b4.backward(self.x1, self.dx1, self.dy4, dr=self.dres, dy2=self.dx1p)      # main path and projection meet at x1
+        self.c4.backward(self.y4, self.dy4, self.dz3)
+        b3.backward(self.z3, self.dz3, self.dy3)
+        self.c3.backward(self.y3, self.dy3, self.dx0)
+        b2.backward(self.x0, self.dx0, self.dy2, dy2=self.dres)
+        self.c2.backward(self.y2, self.dy2, self.dx2)
+        self.pool.backward(self.dx2, self.dz1)
+        b1.backward(self.z1, self.dz1, self.dy1)
+        self.c1.backward(self.y1, self.dy1, None)
+
+    def layers(self):
+        return (self.c1, self.c2, self.c3, self.c4, self.c5, self.c6, self.c7, self.fc, *self.bn)
+
+    def sgd(self, lr):
+        for layer in self.layers():
+            layer.sgd(lr)
+
+    def params(self):
+        return [a for layer in self.layers() for a in layer.params() if a is not None]
+
+    def close(self):
+        for layer in (*self.layers(), self.pool, self.gap):
+            layer.close()
+
+
+def mnist_device(pkg, u8):
+    n = u8.shape[0]
+    xl = np.zeros((n * 28, 32), np.uint16)
+    xl[:, :28] = pkg.f32_to_bf16_bits(u8.reshape(n, 28, 28).astype(np.float32) / 255.0).reshape(n * 28, 28)
+    return torch.from_numpy(xl.view(np.int16)).to(DEV)
+
+
+def host(t):
+    return t.cpu().numpy().view(np.uint16)
+
+
+def test_resnet_gap_mnist(eng, pkg, golden):
+    """In each of the first 5 steps the avg pool's y and dx and GAP's dx are bit-exact against the replays on the device's own
+    tensors, and GAP's y lies within its error model.  A fresh run reproduces the parameters after 5 steps bit for bit.  After
+    EPOCHS epochs over the 1024 training digits the mean loss has fallen, and test accuracy on the 256 test digits, evaluated with
+    the running statistics, exceeds ACC_MIN."""
+    xs, ys = mnist_device(pkg, golden["train_u8"]), torch.from_numpy(golden["train_labels"]).to(DEV)
+    xt, yt = mnist_device(pkg, golden["test_u8"]), torch.from_numpy(golden["test_labels"]).to(DEV)
+    row_bytes = 28 * 32 * 2
+    batch = lambda s, xs=xs, ys=ys: (xs.data_ptr() + s * NB * row_bytes, ys[s * NB:(s + 1) * NB])
+    bf, f32 = pkg.f32_to_bf16_bits, pkg.bf16_bits_to_f32
+
+    net = ResNetGAP(eng, pkg, init_params())
+    for it in range(5):
+        net.forward(*batch(it))
+        eng.sync()
+        z1, x2, out, h = host(net.z1), host(net.x2), host(net.out), host(net.h)
+        net.backward()
+        eng.sync()
+        assert np.array_equal(x2[:, :, :96].reshape(NB, 12, 12, 8), bf(AR.fwd(f32(z1), 2, 2, 2, 0, 0, 1))), it
+        dx2 = host(net.dx2)[:, :, :96].reshape(NB, 12, 12, 8)
+        assert np.array_equal(host(net.dz1), bf(AR.bwd(f32(dx2), 24, 24, 2, 2, 2, 0, 0, 1)[0])), it
+        assert np.array_equal(host(net.dout), bf(AR.global_bwd(f32(host(net.dh)[:, :32]), 6, 6))), it
+        _, _, lo, hi = gap_bound(pkg, f32(out).reshape(NB, 6, 6, 32), net.gap.info)
+        yf = f32(h[:, :32])
+        assert np.all((yf >= lo) & (yf <= hi)), it
+        net.sgd(LR_STEP)
+        eng.sync()
+    after5 = net.params()
+    net.close()
+
+    net = ResNetGAP(eng, pkg, init_params())
+    losses = []
+    for ep in range(EPOCHS):
+        for s in range(1024 // NB):
+            net.forward(*batch(s))
+            net.backward()
+            net.sgd(LR_STEP)
+            losses.append(net.loss)
+            net.loss = torch.zeros(NB, dtype=torch.float32, device=DEV)
+            if ep == 0 and s == 4:
+                eng.sync()
+                assert all(np.array_equal(a.view(np.uint32), b_.view(np.uint32)) for a, b_ in zip(net.params(), after5))
+    eng.sync()
+    ep_loss = [float(torch.stack(losses[e * 8:(e + 1) * 8]).double().mean()) for e in range(EPOCHS)]
+    right = 0
+    for s in range(2):
+        net.forward(*batch(s, xt, yt), training=False)
+        eng.sync()
+        right += int((net.pred.cpu().numpy() == golden["test_labels"][s * NB:(s + 1) * NB]).sum())
+    acc = right / 256
+    net.close()
+    print(f"GAP ResNet: mean loss by epoch {ep_loss[0]:.4f} -> {ep_loss[-1]:.4f}; test accuracy {acc:.4f} (threshold {ACC_MIN})")
+    assert np.isfinite(ep_loss).all() and ep_loss[-1] < ep_loss[0]
+    assert acc > ACC_MIN
