@@ -591,6 +591,73 @@ int pcnn_linear_info(int N, int P, int Q, int C, int O, int row_pitch, int image
  * still the argmax).  dlogits == logits (in place) is allowed, any other overlap is not. */
 int pcnn_softmax_ce_bf16(pcnn_ctx *ctx, const void *logits_bf16_dev, const uint8_t *labels_dev, int N, int O, float scale,
                          void *dlogits_bf16_dev, float *loss_f32_dev, int *pred_i32_dev);
+/* Optimizers for device-trained layers (csrc/optim.cu): one fused update of every parameter tensor of a network per step, as
+ * torch.optim.SGD and torch.optim.AdamW (decoupled weight decay) in their single-tensor form, with the bf16 operands of the plans
+ * the parameters belong to refreshed in the same pass.
+ *   - A table of `count` tensors is validated and uploaded once by pcnn_optim_create; the library allocates the state, zero-filled:
+ *     SGD with momentum != 0 has one buffer per tensor (state0 = the momentum buffer b), SGD with momentum 0 none, AdamW two
+ *     (state0 = m, state1 = v).  param and grad are fp32 device arrays of n elements; the caller keeps them alive.
+ *   - plan_part 1: param is the fp32 master of the plan's filters (KRSC, K R S C elements) or of a linear plan's weights ([O][P][Q][C],
+ *     O P Q C elements); 2: the master of its bias (K, or O, elements; the plan must have one); 0: no plan (plan must be NULL),
+ *     e.g. batch normalization's gamma and beta.  After the update the plan holds exactly what pcnn_conv_plan_set_params(param) would
+ *     give it: wide and linear operands get bf16_rn(p) element by element from the update kernel itself (pad never written), the
+ *     bias copy p; a row-Toeplitz plan's filters, where one filter element feeds several operand entries, are gathered afresh from
+ *     the updated master by the plan's own kernel, enqueued right after the update (one launch per such plan).
+ *   - pcnn_optim_step(ctx, opt, lr): one update kernel over every tensor (CTAs walk fixed chunks of the concatenated tensors; a chunk
+ *     table built at creation maps chunk -> tensor), plus the row-Toeplitz gathers.  Stream-ordered, no allocation, no host
+ *     synchronisation.  Call it after every backward pass of the step: pcnn_linear_dgrad reads the plan's bf16 weights, which the step
+ *     replaces, exactly as the layers' own sgd().  The step count t (kept on the host) is incremented by each call, first call t = 1.
+ *     lr < 0 and NaN lr are PCNN_ERR_ARG.
+ * Update rules.  Every operation is fp32 round to nearest with no contraction (RN below; a product, then a sum, never an FMA); sqrt
+ * and "/" are the correctly rounded IEEE operations.  Element by element, so no result bit depends on the grid or the SM count; NaN
+ * and Inf in grads or params propagate by IEEE rules (no clipping, no skipping).  wd is the tensor's weight_decay.
+ *   SGD (momentum mu, dampening delta, nesterov):
+ *     g' = wd != 0 ? RN(g + RN(wd * p)) : g            (skipped, not multiplied by 0, at wd = 0: 0 * Inf would be NaN)
+ *     mu != 0:  b = g' at t = 1 (no dampening on the first step), else b = RN(RN(mu * b) + RN(omega * g')), omega = fp32(1 - delta);
+ *               d = nesterov ? RN(g' + RN(mu * b)) : b
+ *     mu == 0:  d = g'
+ *     p = RN(p + RN((-lr) * d))                          (mu = 0, wd = 0: exactly pcnn_apply_grad_scaled(p, g, n, -lr))
+ *   AdamW (beta1, beta2, eps; with the host forming, in double at each step, c2 = fp32(sqrt(1 - beta2^t)) and s = fp32(lr / (1 - beta1^t)),
+ *   and per tensor lambda = fp32(1 - double(lr) * double(wd))):
+ *     p = RN(p * lambda) when wd != 0
+ *     m = RN(m + RN(a1 * RN(g - m))),                    a1 = fp32(1 - beta1)
+ *     v = RN(RN(beta2 * v) + RN(RN(a2 * g) * g)),        a2 = fp32(1 - beta2)
+ *     den = RN(RN(RN(sqrt(v)) / c2) + eps)
+ *     p = RN(p + RN((-s) * RN(m / den)))
+ *   AdamW with wd = 0 is Adam.  There is no coupled-L2 Adam, amsgrad, gradient clipping or loss scaling.
+ * Vector path: a tensor whose param, grad, state and operand are 16-byte aligned (8-byte for the bf16 operand), with n % 4 == 0 and
+ * (with a plan operand) cols % 4 == 0 and pitch % 4 == 0, moves 4 elements per access; any other takes the scalar path.  Both give
+ * the same bits.
+ * pcnn_optim_create refuses, with PCNN_ERR_ARG and a message naming the rule: NULL ctx, cfg, table or out, count < 1, a NULL param or
+ * grad, n <= 0; an unknown kind; momentum < 0, nesterov with momentum <= 0 or dampening != 0, beta1 or beta2 outside [0, 1), eps < 0,
+ * weight_decay < 0, any NaN hyperparameter; plan_part outside 0..2, plan_part 0 with a plan or 1..2 without one; plan_part 1 with n
+ * other than the plan's master size, plan_part 2 with n != K or for a plan without bias; the same (plan, part) twice; any two of the
+ * params, grads and plan operands (bf16 operand rows, bias copy) overlapping.
+ * pcnn_optim_state: device pointers of tensor i's state (NULL where the kind keeps none).  pcnn_optim_info: out6 = { tensors,
+ * elements, tensors on the vector path, chunks, grid of the update kernel, steps taken }.  pcnn_optim_destroy frees the state and
+ * the tables (after the stream's pending work). */
+#define PCNN_OPTIM_SGD 0
+#define PCNN_OPTIM_ADAMW 1
+typedef struct {
+    float *param;
+    const float *grad;
+    long n;
+    float weight_decay;
+    pcnn_conv_plan *plan;
+    int plan_part;          /* 0 none, 1 filters / weights, 2 bias */
+} pcnn_optim_tensor;
+typedef struct {
+    int kind;               /* PCNN_OPTIM_SGD or PCNN_OPTIM_ADAMW */
+    float momentum, dampening;
+    int nesterov;
+    float beta1, beta2, eps;
+} pcnn_optim_config;
+typedef struct pcnn_optim pcnn_optim;
+int pcnn_optim_create(pcnn_ctx *ctx, const pcnn_optim_config *cfg, const pcnn_optim_tensor *tensors, int count, pcnn_optim **out);
+int pcnn_optim_step(pcnn_ctx *ctx, pcnn_optim *opt, float lr);
+int pcnn_optim_state(pcnn_optim *opt, int i, float **state0_dev, float **state1_dev);
+int pcnn_optim_info(pcnn_optim *opt, long *out6);
+int pcnn_optim_destroy(pcnn_ctx *ctx, pcnn_optim *opt);
 
 #ifdef __cplusplus
 }

@@ -16,6 +16,7 @@ U8, F32 = 0, 1
 MODE_AUTO, MODE_GRAPH, MODE_PERSISTENT = 0, 1, 2
 TRAIN_SET, TEST_SET = 0, 1
 ACT_NONE, ACT_SIGMOID, ACT_RELU = 0, 1, 3     # PCNN_ACT_*: the `act` of the device-trained layers (2 is not a code)
+OPTIM_SGD, OPTIM_ADAMW = 0, 1                 # PCNN_OPTIM_*: the `kind` of pcnn_optim_config
 
 
 class PcnnError(RuntimeError):
@@ -28,6 +29,16 @@ class PcnnError(RuntimeError):
 
 _vp, _i, _l, _f, _sz = C.c_void_p, C.c_int, C.c_long, C.c_float, C.c_size_t
 _pvp = C.POINTER(C.c_void_p)
+
+
+class OptimTensor(C.Structure):
+    """pcnn_optim_tensor"""
+    _fields_ = [("param", _vp), ("grad", _vp), ("n", _l), ("weight_decay", _f), ("plan", _vp), ("plan_part", _i)]
+
+
+class OptimConfig(C.Structure):
+    """pcnn_optim_config"""
+    _fields_ = [("kind", _i), ("momentum", _f), ("dampening", _f), ("nesterov", _i), ("beta1", _f), ("beta2", _f), ("eps", _f)]
 
 # name -> argtypes (every function returns int unless listed in _RESTYPE)
 _SIG = {
@@ -155,6 +166,11 @@ _SIG = {
     "pcnn_linear_dgrad": [_vp, _vp, _vp, _vp],
     "pcnn_linear_info": [_i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_softmax_ce_bf16": [_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp],
+    "pcnn_optim_create": [_vp, _vp, _vp, _i, _pvp],
+    "pcnn_optim_step": [_vp, _vp, _f],
+    "pcnn_optim_state": [_vp, _i, _pvp, _pvp],
+    "pcnn_optim_info": [_vp, _vp],
+    "pcnn_optim_destroy": [_vp, _vp],
 }
 _RESTYPE = {"pcnn_last_error_string": C.c_char_p, "pcnn_mnist_free": None}
 

@@ -258,6 +258,13 @@ pcnn_conv_plan *conv_plan_wrap_linear(LinearPlan *l) {
 
 LinearPlan *conv_plan_linear(pcnn_conv_plan *plan) { return plan->linear; }
 
+void conv_plan_operand(pcnn_conv_plan *plan, PlanOperand *out) {
+    if (plan->wide) return conv_wide_operand(plan->wide, out);
+    if (plan->linear) return linear_operand(plan->linear, out);
+    const ConvTcParams &p = plan->p;
+    *out = PlanOperand{nullptr, 0, 0, (long long)p.K * p.R * plan->S * p.C, plan->d_bias, p.K};
+}
+
 // the Toeplitz operand of the plan from fp32 KRSC filters in device memory, enqueued on the context's stream
 static int conv_tc_load_filters(pcnn_ctx *ctx, pcnn_conv_plan *pl, const float *filt_dev) {
     const long total = (long)pl->p.V * pl->p.R * pl->p.npad * TC_KCHUNK;
@@ -401,10 +408,10 @@ extern "C" int pcnn_conv_plan_set_params(pcnn_ctx *ctx, pcnn_conv_plan *plan, co
     PCNN_REQUIRE(ctx && plan, PCNN_ERR_ARG, "pcnn_conv_plan_set_params: NULL context or plan");
     PCNN_REQUIRE(filt_f32_dev || bias_f32_dev, PCNN_ERR_ARG,
                  "pcnn_conv_plan_set_params: filters and bias are both NULL (at least one must be given)");
-    int K = plan->p.K;
-    float *d_bias = plan->d_bias;
-    if (plan->wide) d_bias = conv_wide_bias(plan->wide, &K);
-    if (plan->linear) d_bias = linear_bias(plan->linear, &K);
+    PlanOperand op;
+    conv_plan_operand(plan, &op);
+    const int K = op.K;
+    float *d_bias = op.bias;
     PCNN_REQUIRE(!bias_f32_dev || d_bias, PCNN_ERR_ARG,
                  "pcnn_conv_plan_set_params: a bias for a plan created without one (bias_host NULL): only a plan with a bias can "
                  "refresh it");

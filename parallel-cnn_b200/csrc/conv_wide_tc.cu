@@ -298,9 +298,10 @@ void conv_wide_free(ConvWidePlan *w) {
     delete w;
 }
 
-float *conv_wide_bias(ConvWidePlan *w, int *K) {
-    *K = w->p.K;
-    return w->d_bias;
+// d_filt is [K][R*S*C]: the KRSC master with rows of R*S*C elements and no pad
+void conv_wide_operand(ConvWidePlan *w, PlanOperand *out) {
+    const int rsc = w->p.R * w->p.S * w->C;
+    *out = PlanOperand{w->d_filt, rsc, rsc, (long long)w->p.K * rsc, w->d_bias, w->p.K};
 }
 
 // fp32 KRSC filters in device memory -> d_filt [K][R*S][C] bf16 (the same order), enqueued on the context's stream

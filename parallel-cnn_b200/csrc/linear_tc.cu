@@ -479,9 +479,9 @@ void linear_free(LinearPlan *l) {
     delete l;
 }
 
-float *linear_bias(LinearPlan *l, int *O) {
-    *O = l->sh.O;
-    return l->d_bias;
+// d_w is [O][P][wpitch]: rows of Q*C in-row elements; the pad columns were zeroed at creation and nothing writes them again
+void linear_operand(LinearPlan *l, PlanOperand *out) {
+    *out = PlanOperand{l->d_w, l->sh.QC, l->sh.wpitch, (long long)l->sh.O * l->sh.F, l->d_bias, l->sh.O};
 }
 
 // fp32 [O][P][Q][C] in device memory -> the plan's bf16 [O][P][wpitch] (pad columns zero), on the context's stream

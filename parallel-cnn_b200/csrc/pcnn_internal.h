@@ -232,16 +232,28 @@ struct ConvWidePlan;
 int conv_wide_fwd(pcnn_ctx *ctx, const ConvWidePlan *w, const void *x_bf16, void *y_bf16);
 void conv_wide_free(ConvWidePlan *w);
 pcnn_conv_plan *conv_plan_wrap_wide(ConvWidePlan *w);   // conv_tc.cu; takes ownership
-// the plan's bias buffer (null for a plan without bias) and its filter count; the filters from fp32 KRSC in device memory,
-// rounded to bf16 on the context's stream (pcnn_conv_plan_set_params and the create calls)
-float *conv_wide_bias(ConvWidePlan *w, int *K);
+// What a plan holds of its parameters, for refreshing them from fp32 masters in device memory (conv_plan_operand):
+//   - w: the bf16 operand, element i of the fp32 master (KRSC, or [O][P][Q][C] for a linear plan) at w[(i / cols) * pitch + i % cols],
+//     or null for a row-Toeplitz plan, where one filter element feeds V * Qt operand entries (pcnn_conv_plan_set_params gathers them);
+//   - n: the elements of that master; bias: the plan's fp32 copy of the bias ([K]), null for a plan without one.
+// Nothing but the plan module knows the operand's layout: pcnn_conv_plan_set_params and the optimizer (optim.cu) ask this.
+struct PlanOperand {
+    void *w;
+    int cols, pitch;
+    long long n;
+    float *bias;
+    int K;
+};
+void conv_plan_operand(pcnn_conv_plan *plan, PlanOperand *out);   // conv_tc.cu
+void conv_wide_operand(ConvWidePlan *w, PlanOperand *out);
+// the filters from fp32 KRSC in device memory, rounded to bf16 on the context's stream (pcnn_conv_plan_set_params and the create calls)
 int conv_wide_load_filters(pcnn_ctx *ctx, ConvWidePlan *w, const float *filt_dev);
 // linear_tc.cu: a plan of pcnn_linear_plan_create is a pcnn_conv_plan holding a LinearPlan, run, refreshed and freed like the
 // wide one; conv_plan_linear is null for a convolution plan
 struct LinearPlan;
 int linear_fwd(pcnn_ctx *ctx, const LinearPlan *l, const void *x_bf16, void *y_bf16);
 void linear_free(LinearPlan *l);
-float *linear_bias(LinearPlan *l, int *O);
+void linear_operand(LinearPlan *l, PlanOperand *out);
 int linear_load_weights(pcnn_ctx *ctx, LinearPlan *l, const float *w_dev);
 pcnn_conv_plan *conv_plan_wrap_linear(LinearPlan *l);   // conv_tc.cu; takes ownership
 LinearPlan *conv_plan_linear(pcnn_conv_plan *plan);

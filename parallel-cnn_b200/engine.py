@@ -4,8 +4,8 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import (F32, NPARAM, TEST_SET, TRAIN_SET, U8, PcnnError, avgpool_nhwc_info, batchnorm_nhwc_info, check, conv_layer_family,
-                   global_avgpool_nhwc_info, lib, linear_info, maxpool_nhwc_info)
+from ._lib import (F32, NPARAM, OPTIM_ADAMW, OPTIM_SGD, TEST_SET, TRAIN_SET, U8, OptimConfig, OptimTensor, PcnnError, avgpool_nhwc_info,
+                   batchnorm_nhwc_info, check, conv_layer_family, global_avgpool_nhwc_info, lib, linear_info, maxpool_nhwc_info)
 
 
 def _pixel_type(arr_or_dtype):
@@ -638,6 +638,10 @@ class ConvLayer:
             self.engine.apply_grad_scaled(self.bias, self.db, self.shape[4], -lr)
         self.plan.set_params(self.filt, self.bias)
 
+    def optim_tensors(self):
+        """(param, grad, plan, plan part, is norm or bias) of each trainable tensor: the table SGD and AdamW are built from"""
+        return [(self.filt, self.dw, self.plan, 1, False)] + ([] if self.bias is None else [(self.bias, self.db, self.plan, 2, True)])
+
     def params(self):
         """host copies (filters [K][R][S][C], bias [K] or None) of the fp32 masters"""
         return self.filt.to_host(), None if self.bias is None else self.bias.to_host()
@@ -702,6 +706,10 @@ class BatchNormLayer:
         C = self.shape[3]
         self.engine.apply_grad_scaled(self.gamma, self.dgamma, C, -lr)
         self.engine.apply_grad_scaled(self.beta, self.dbeta, C, -lr)
+
+    def optim_tensors(self):
+        """(param, grad, plan, plan part, is norm or bias) of gamma and beta, as ConvLayer.optim_tensors"""
+        return [(self.gamma, self.dgamma, None, 0, True), (self.beta, self.dbeta, None, 0, True)]
 
     def params(self):
         """host copies of gamma, beta, the running mean and the running variance"""
@@ -770,6 +778,10 @@ class LinearLayer:
         if self.bias is not None:
             self.engine.apply_grad_scaled(self.bias, self.db, O, -lr)
         self.plan.set_params(self.w, self.bias)
+
+    def optim_tensors(self):
+        """(param, grad, plan, plan part, is norm or bias) of w and the bias, as ConvLayer.optim_tensors"""
+        return [(self.w, self.dw, self.plan, 1, False)] + ([] if self.bias is None else [(self.bias, self.db, self.plan, 2, True)])
 
     def params(self):
         """host copies (w [O][P][Q][C], bias [O] or None) of the fp32 masters"""
@@ -882,6 +894,97 @@ class GlobalAvgPoolLayer:
         pass
 
 
+class FusedOptimizer:
+    """One fused update of many fp32 parameter tensors per step (pcnn_optim_*; the rules and their order are in include/pcnn.h).
+    tensors: (param, grad, n, weight_decay, plan, plan part) with plan None (part 0) or the ConvPlan / LinearPlan whose filters (part 1)
+    or bias (part 2) param is the master of; the plan's operands are refreshed by the step.  kind OPTIM_SGD or OPTIM_ADAMW.  SGD and
+    AdamW build the table from layers; this class takes it directly."""
+
+    def __init__(self, engine, kind, tensors, momentum=0.0, dampening=0.0, nesterov=False, betas=(0.9, 0.999), eps=1e-8):
+        self.engine, self.opt = engine, None
+        self.sizes = [int(t[2]) for t in tensors]
+        tab = (OptimTensor * len(tensors))()
+        for e, (param, grad, n, wd, plan, part) in zip(tab, tensors):
+            e.param, e.grad, e.n, e.weight_decay, e.plan, e.plan_part = _p(param), _p(grad), int(n), float(wd), _plan(plan), int(part)
+        cfg = OptimConfig(int(kind), float(momentum), float(dampening), int(bool(nesterov)), float(betas[0]), float(betas[1]), float(eps))
+        h = C_.c_void_p()
+        check("pcnn_optim_create", lib().pcnn_optim_create(engine.ctx, C_.byref(cfg), tab, len(tensors), C_.byref(h)))
+        self.opt = h
+
+    def step(self, lr):
+        """one update of every tensor with learning rate lr (rounded to fp32), enqueued on the engine's stream after the backward
+        passes; a row-Toeplitz plan's filters take a second launch"""
+        check("pcnn_optim_step", lib().pcnn_optim_step(self.engine.ctx, self.opt, float(lr)))
+
+    def state(self):
+        """host copies of each tensor's state: (momentum buffer, None) for SGD with momentum, (m, v) for AdamW, (None, None) for
+        SGD without momentum"""
+        out = []
+        for i, n in enumerate(self.sizes):
+            ptrs = (C_.c_void_p(), C_.c_void_p())
+            check("pcnn_optim_state", lib().pcnn_optim_state(self.opt, i, C_.byref(ptrs[0]), C_.byref(ptrs[1])))
+            pair = []
+            for p in ptrs:
+                if not p.value:
+                    pair.append(None)
+                    continue
+                a = np.empty(n, np.float32)
+                check("pcnn_d2h", lib().pcnn_d2h(self.engine.ctx, a.ctypes.data, p.value, a.nbytes))
+                pair.append(a)
+            out.append(tuple(pair))
+        return out
+
+    def info(self):
+        """pcnn_optim_info: tensors, elements, tensors on the 16-byte vector path, chunks, grid of the update kernel, steps taken"""
+        v = (C_.c_long * 6)()
+        check("pcnn_optim_info", lib().pcnn_optim_info(self.opt, v))
+        return dict(tensors=v[0], elements=v[1], vector_tensors=v[2], chunks=v[3], grid=v[4], steps=v[5])
+
+    @property
+    def steps(self):
+        return self.info()["steps"]
+
+    def close(self):
+        if self.opt and self.engine.ctx:
+            lib().pcnn_optim_destroy(self.engine.ctx, self.opt)
+        self.opt = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def _plan(plan):
+    """the pcnn_conv_plan handle of a ConvPlan / LinearPlan (or of a raw c_void_p), None for none"""
+    plan = getattr(plan, "plan", plan)
+    return getattr(plan, "value", plan)
+
+
+def _layer_tensors(layers, weight_decay, decay_norm_and_bias):
+    return [(param, grad, param.nbytes // 4, 0.0 if norm_or_bias and not decay_norm_and_bias else weight_decay, plan, part)
+            for layer in layers for param, grad, plan, part, norm_or_bias in layer.optim_tensors()]
+
+
+class SGD(FusedOptimizer):
+    """torch.optim.SGD over the trainable tensors of ConvLayers, LinearLayers and BatchNormLayers, in one launch per step with the
+    layers' plans refreshed: step(lr) replaces every layer.sgd(lr) of a training step (momentum 0 and weight decay 0 give the same
+    bits).  decay_norm_and_bias=False gives batch normalization's gamma and beta and the biases weight decay 0; the default decays
+    every tensor, as torch.optim does with one parameter group."""
+
+    def __init__(self, engine, layers, momentum=0.0, dampening=0.0, nesterov=False, weight_decay=0.0, decay_norm_and_bias=True):
+        super().__init__(engine, OPTIM_SGD, _layer_tensors(layers, weight_decay, decay_norm_and_bias), momentum=momentum,
+                         dampening=dampening, nesterov=nesterov)
+
+
+class AdamW(FusedOptimizer):
+    """torch.optim.AdamW (decoupled weight decay; weight_decay 0 is Adam) over the trainable tensors of the layers, as SGD"""
+
+    def __init__(self, engine, layers, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2, decay_norm_and_bias=True):
+        super().__init__(engine, OPTIM_ADAMW, _layer_tensors(layers, weight_decay, decay_norm_and_bias), betas=betas, eps=eps)
+
+
 def f32_to_bf16_bits(a):
     """numpy float32 -> uint16 bf16 bit patterns (round to nearest even), the rounding the kernels use; NaN -> the quiet NaN
     0x7FC0 (rounding the payload could carry into the exponent and the sign: 0x7FFFFFFF would become -0)"""
@@ -896,4 +999,4 @@ def bf16_bits_to_f32(b):
 
 
 C_ = C
-__all__ = ["Engine", "DeviceArray", "ConvPlan", "WideConvPlan", "LinearPlan", "ConvLayer", "LinearLayer", "MaxPoolLayer", "AvgPoolLayer", "GlobalAvgPoolLayer", "BatchNormLayer", "f32_to_bf16_bits", "bf16_bits_to_f32", "TRAIN_SET", "TEST_SET", "U8", "F32"]
+__all__ = ["Engine", "DeviceArray", "ConvPlan", "WideConvPlan", "LinearPlan", "ConvLayer", "LinearLayer", "MaxPoolLayer", "AvgPoolLayer", "GlobalAvgPoolLayer", "BatchNormLayer", "FusedOptimizer", "SGD", "AdamW", "f32_to_bf16_bits", "bf16_bits_to_f32", "TRAIN_SET", "TEST_SET", "U8", "F32"]

@@ -727,6 +727,110 @@ def run_resnetgap(N, iters):
                       "gpu": gpu, "power_limit": power}), flush=True)
 
 
+def run_optim(iters):
+    """one fused optimizer step (pcnn_optim_step) over the 62 tensors of ResNet-18 (tests/optim_ref.py, 11.69 M fp32 elements) with
+    the 19 convolutions of C % 8 == 0 carrying wide plans created at N = 1 with their real spatial sizes (a 512-filter convolution is
+    two 256-filter plans over the two halves of its KRSC master: the wide plan takes K <= 256), whose bf16 operands the step rewrites;
+    conv1 (C = 3) and the fc carry none.  Bytes per element: SGD with momentum reads p, g, b and writes p, b (20), AdamW reads p, g, m,
+    v and writes p, m, v (28), plus 2 per operand element.  Beside it torch's fused SGD / AdamW on the same fp32 tensors, and
+    torch._foreach_copy_ of the 19 masters into bf16 copies (the operand refresh torch would need)."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import optim_ref as OR
+    gpu, power = card()
+    gen = torch.Generator(device="cuda").manual_seed(5)
+    ps, gs, table, plans, op_src, n_op = [], [], [], [], [], 0
+    for name, shape, h in OR.resnet18_tensors():
+        n = int(np.prod(shape))
+        p = torch.randn(n, device="cuda", generator=gen) * 0.05
+        g = torch.randn(n, device="cuda", generator=gen) * 1e-2
+        ps.append(p)
+        gs.append(g)
+        if len(shape) == 4 and h > 0 and shape[3] % 8 == 0:
+            K, R_, S, C = shape
+            stride = 2 if (".0.conv1" in name or ".0.down" in name) and not name.startswith("layer1") else 1
+            host_f = p.cpu().numpy().reshape(shape)
+            for k0 in range(0, K, 256):
+                k = min(256, K - k0)
+                plan = pkg.WideConvPlan(eng, 1, h, h, C, k, R_, S, host_f[k0:k0 + k], None, stride=stride, padding=(R_ // 2, S // 2))
+                plans.append(plan)
+                off = k0 * R_ * S * C * 4
+                table.append((p.data_ptr() + off, g.data_ptr() + off, k * R_ * S * C, 5e-4, plan, 1))
+            op_src.append(p)
+            n_op += n
+        else:
+            table.append((p, g, n, 5e-4, None, 0))
+    n_all = sum(p.numel() for p in ps)
+    torch.cuda.synchronize()
+    res = {"case": "fused optimizer step, ResNet-18 table", "tensors": len(ps), "table_entries": len(table), "elements": n_all,
+           "operand_elements": n_op, "gpu": gpu, "power_limit": power}
+    for kind, kw, lr, per_el in (("sgd_momentum", dict(momentum=0.9), 0.1, 20), ("adamw", dict(betas=(0.9, 0.999), eps=1e-8), 1e-3, 28)):
+        opt = pkg.FusedOptimizer(eng, pkg.OPTIM_SGD if kind.startswith("sgd") else pkg.OPTIM_ADAMW, table, **kw)
+        ms = timed(lambda: opt.step(lr), iters)
+        info = opt.info()
+        opt.close()
+        nbytes = per_el * n_all + 2 * n_op
+        tp = [p.clone() for p in ps]
+        for t, g in zip(tp, gs):
+            t.grad = g
+        topt = (torch.optim.SGD(tp, lr=lr, momentum=0.9, weight_decay=5e-4, fused=True) if kind.startswith("sgd")
+                else torch.optim.AdamW(tp, lr=lr, weight_decay=5e-4, fused=True))
+        ms_t = timed(topt.step, iters)
+        res.update({f"{kind}_us": ms * 1e3, f"{kind}_bytes": nbytes, f"{kind}_GBps": nbytes / ms / 1e6,
+                    f"{kind}_share_of_3350": nbytes / ms / 1e6 / HBM, f"{kind}_grid": info["grid"], f"{kind}_chunks": info["chunks"],
+                    f"torch_fused_{kind}_us": ms_t * 1e3})
+        del tp, topt
+    bf = [torch.empty(p.numel(), dtype=torch.bfloat16, device="cuda") for p in op_src]
+    res["torch_foreach_copy_bf16_us"] = timed(lambda: torch._foreach_copy_(bf, op_src), iters) * 1e3
+    print(json.dumps(res), flush=True)
+    for plan in plans:
+        plan.close()
+
+
+def run_resnetgap_optim(N, iters, rounds=3):
+    """the GAP ResNet training step of run_resnetgap with every layer's sgd(lr) and with the fused SGD at momentum 0 (the same bits),
+    alternated in this one call; then momentum SGD and AdamW.  The update alone (gradients left in place) is timed the same way."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import test_avgpool_nhwc_gpu as T
+    gpu, power = card()
+    net = T.ResNetGAP(eng, pkg, T.init_params())
+    xl = torch.randint(0, 0x3F80, (N * 28, 32), dtype=torch.int16, device="cuda")
+    labels = torch.randint(0, 10, (N,), dtype=torch.uint8, device="cuda")
+    torch.cuda.synchronize()
+    opts = {"fused_sgd": (pkg.SGD(eng, net.layers()), 0.2), "fused_sgd_momentum": (pkg.SGD(eng, net.layers(), momentum=0.9, weight_decay=5e-4), 0.02),
+            "fused_adamw": (pkg.AdamW(eng, net.layers()), 1e-3)}
+    updates = {"layer_sgd": lambda: net.sgd(0.2)}
+    updates.update({k: (lambda o=o, lr=lr: o.step(lr)) for k, (o, lr) in opts.items()})
+
+    def step(update):
+        net.forward(xl.data_ptr(), labels)
+        net.backward()
+        update()
+
+    out = {k: [] for k in updates}
+    upd = {k: [] for k in updates}
+    for _ in range(rounds):
+        for k, u in updates.items():
+            out[k].append(timed(lambda u=u: step(u), iters))
+            upd[k].append(timed(u, iters))
+    launches = {}
+    for k, u in updates.items():
+        n0 = eng.launch_count()
+        u()
+        launches[k] = eng.launch_count() - n0
+    torch.cuda.synchronize()
+    for o, _ in opts.values():
+        o.close()
+    net.close()
+    print(json.dumps({"case": f"GAP ResNet training step N={N}, update variants alternated over {rounds} rounds",
+                      "step_ms_median": {k: float(np.median(v)) for k, v in out.items()}, "step_ms_all": out,
+                      "update_only_us_median": {k: float(np.median(v)) * 1e3 for k, v in upd.items()},
+                      "kernel_launches_per_update": launches, "gpu": gpu, "power_limit": power}), flush=True)
+
+
+if only == "optim":                                                    # the fused optimizers over the ResNet-18 table, torch beside them
+    run_optim(50)
+if only == "resnetgap-optim":                                          # the GAP ResNet step with each update, alternated
+    run_resnetgap_optim(128, 20)
 if only == "avgpool":                                                  # average pooling between layers, torch beside it
     run_avgpool("112x112x64, 2x2/2", 128, 112, 112, 64, 2, 2, 0, 1, 20)
     run_avgpool("56x56x128, 2x2/2", 128, 56, 56, 128, 2, 2, 0, 1, 20)

@@ -1,8 +1,14 @@
 #!/usr/bin/env python
 """scripts/resnetgap_replica.py -- float32 torch CPU replica of the GAP ResNet of tests/test_avgpool_nhwc_gpu.py
 (test_resnet_gap_mnist): the same layers, initialisation, batch order (8 batches of 128 over the 1024 golden training digits per
-epoch), softmax cross-entropy over the batch and plain SGD, evaluated on the 256 golden test digits with the running statistics.
-Its accuracy sets the test's threshold.  Usage: resnetgap_replica.py [step ...]"""
+epoch), softmax cross-entropy over the batch and an optimizer step, evaluated on the 256 golden test digits with the running
+statistics.  Its accuracy sets the thresholds of the end-to-end tests.
+
+Usage: resnetgap_replica.py [--optim sgd | momentum | adamw] [lr ...]
+  sgd       plain SGD, p += -lr * grad (the layers' own sgd(lr); tests/test_avgpool_nhwc_gpu.py)
+  momentum  torch.optim.SGD with momentum 0.9 and weight decay 5e-4 on every parameter (tests/test_optim_gpu.py)
+  adamw     torch.optim.AdamW with betas (0.9, 0.999), eps 1e-8 and weight decay 1e-2 on every parameter (tests/test_optim_gpu.py)"""
+import argparse
 import os
 import sys
 
@@ -16,7 +22,7 @@ from test_avgpool_nhwc_gpu import EPOCHS, NB, init_params  # noqa: E402
 F = torch.nn.functional
 
 
-def run(lr):
+def run(lr, optim="sgd"):
     torch.manual_seed(0)
     g = np.load(os.path.join(ROOT, "tests", "golden", "mnist_subset.npz"))
     img = lambda u8: torch.from_numpy(u8.reshape(-1, 1, 28, 28).astype(np.float32) / 255.0).bfloat16().float()   # the device's bf16 input
@@ -41,21 +47,27 @@ def run(lr):
         return F.linear(F.adaptive_avg_pool2d(h, 1).flatten(1), w["w8"], w["b8"])
 
     params = list(w.values()) + [t for ga, be, _, _ in bn for t in (ga, be)]
+    opt = {"sgd": lambda: torch.optim.SGD(params, lr=lr),
+           "momentum": lambda: torch.optim.SGD(params, lr=lr, momentum=0.9, weight_decay=5e-4),
+           "adamw": lambda: torch.optim.AdamW(params, lr=lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2)}[optim]()
     losses = []
     for ep in range(EPOCHS):
         for s in range(1024 // NB):
             loss = F.cross_entropy(net(xs[s * NB:(s + 1) * NB], True), ys[s * NB:(s + 1) * NB])
-            for t in params:
-                t.grad = None
+            opt.zero_grad(set_to_none=True)
             loss.backward()
-            with torch.no_grad():
-                for t in params:
-                    t.add_(t.grad, alpha=-lr)
+            opt.step()
             losses.append(float(loss))
     with torch.no_grad():
         acc = float((net(xt, False).argmax(1) == yt).float().mean())
-    print(f"step {lr}: mean loss epoch 1 {np.mean(losses[:8]):.4f} -> epoch {EPOCHS} {np.mean(losses[-8:]):.4f}; test accuracy {acc:.4f}", flush=True)
+    print(f"{optim} lr {lr}: mean loss epoch 1 {np.mean(losses[:8]):.4f} -> epoch {EPOCHS} {np.mean(losses[-8:]):.4f}; test accuracy {acc:.4f}",
+          flush=True)
 
 
-for lr in [float(a) for a in sys.argv[1:]] or [0.1]:
-    run(lr)
+if __name__ == "__main__":
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--optim", default="sgd", choices=["sgd", "momentum", "adamw"])
+    ap.add_argument("lr", nargs="*", type=float)
+    a = ap.parse_args()
+    for lr in a.lr or [0.1]:
+        run(lr, a.optim)
