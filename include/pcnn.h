@@ -582,6 +582,47 @@ int pcnn_linear_plan_create(pcnn_ctx *ctx, int N, int P, int Q, int C, int O, in
 int pcnn_linear_wgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *x_bf16_dev, const void *dy_bf16_dev, float *dw_f32_dev);
 int pcnn_linear_dgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *dy_bf16_dev, void *dx_bf16_dev);
 int pcnn_linear_info(int N, int P, int Q, int C, int O, int row_pitch, int image_rows, int *out12);
+/* Depthwise convolution (csrc/dwconv_nhwc.cu), as torch.nn.functional.conv2d(x, w, b, stride, padding=(pad_h, pad_w), groups=C)
+ * with w [C][1][R][S]: each channel is filtered by its own R x S filter.
+ *   - x and dx are dense bf16 [N][H][W][C], y and dy dense bf16 [N][P][Q][C]: what the conv forwards and batch norm write and
+ *     what batch norm, the global average pool and pcnn_conv_bias_act_bwd read;
+ *     P = (H + 2 pad_h - R) / stride + 1,   Q = (W + 2 pad_w - S) / stride + 1;
+ *   - filters fp32 [C][R][S] (KRSC with one input channel: torch's weight reshaped), bias fp32 [C], dw fp32 [C][R][S].
+ * pcnn_dwconv_plan_create returns a pcnn_conv_plan: pcnn_conv_tc_fwd runs it, pcnn_conv_plan_set_params refreshes its filters and
+ * bias from device memory, pcnn_optim_step refreshes them with the update, and pcnn_conv_tc_plan_destroy frees it.  The plan holds
+ * the filters rounded to bf16 (round to nearest even, on the device) in the master's [C][R][S] order.
+ * Rules (fp32 round to nearest; every product float(bf16) * float(bf16) is exact in fp32, so an FMA gives the bits of a product
+ * followed by an add).  The window of output (p, q) starts at (h0, w0) = (p stride - pad_h, q stride - pad_w); a tap outside the
+ * image reads x = +0 and is multiplied like any other (0 * Inf is NaN), as torch does.
+ *   Forward: acc = the sum over r = 0..R-1, then s = 0..S-1, of float(x[n][h0 + r][w0 + s][c]) * float(wbf16[c][r][s]), starting
+ *     from the first term; v = acc + b[c] with a bias; y = bf16_rn(act(v)), act 0 (none) or 3 (the ReLU of the conv epilogues:
+ *     v < 0 ? +0 : v, NaN and -0 unchanged).  Act 1 is refused: the sigmoid uses tanh.approx, which no reference can replay.
+ *   Input gradient: dx[n][h][w][c] = the sum of float(dy[n][p][q][c]) * float(wbf16[c][r][s]) over the taps with h = p stride -
+ *     pad_h + r and w = q stride - pad_w + s for some 0 <= p < P, 0 <= q < Q, in ascending r, then ascending s, starting from the
+ *     first term, rounded to bf16 once; +0 with no term.  Every element of dx is written, with no memset and no atomics.  It uses
+ *     the plan's bf16 filters, the bits the forward multiplied: call it before the filters are refreshed.
+ *   Weight gradient: dw[c][r][s] = the sum over n, p, q of float(dy[n][p][q][c]) * float(x~[n][h0 + r][w0 + s][c]) (x~ = +0 outside
+ *     the image).  The N P Q output pixels are cut into ranges of `pixels per range` (a function of the shape alone, never of the SM
+ *     count); in a range, lane l sums the pixels l, l + lanes, ... from its first one, the lanes holding a pixel are added in lane
+ *     order, and with several ranges each range writes an fp32 slot in the context's scratch block which
+ *     pcnn_conv_wgrad_reduce_slots adds in a fixed order.  dw is overwritten, not accumulated.
+ * Both gradients take the shape from the plan; a plan not made by pcnn_dwconv_plan_create is PCNN_ERR_ARG.  All calls are
+ * stream-ordered and give the same bits on every run and SM count.
+ * Domain (anything else is PCNN_ERR_ARG with the function and the rule in the message; pcnn_dwconv_info makes the create call's
+ * refusals):
+ *   - N, H, W, C >= 1 (C has no upper limit); 1 <= R, S <= 7; stride 1..4;
+ *   - 0 <= pad_h <= R - 1, 0 <= pad_w <= S - 1, H + 2 pad_h >= R and W + 2 pad_w >= S;
+ *   - H W C, P Q C and C R S within the 32-bit index range;  act 0 or 3;
+ *   - every pointer 16-byte aligned; x and y disjoint, dy and dx disjoint, dw disjoint from x and dy.
+ * With C % 8 == 0 the passes move 16-byte vectors of 8 channels, otherwise single elements.
+ * pcnn_dwconv_info: host only (no GPU, no context).  out9 = { P, Q, channels per thread (8 or 1), channel groups per CTA, channel
+ * slices, weight-gradient pixel lanes per range, pixels per range, ranges, n_acc: the fp32 additions on the longest path of one
+ * dw sum (pixels of a lane - 1, lanes - 1, and with several ranges ceil(ranges / 8) + 3 in pcnn_conv_wgrad_reduce_slots) }. */
+int pcnn_dwconv_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int act,
+                            const float *filt_host, const float *bias_host, pcnn_conv_plan **out);
+int pcnn_dwconv_wgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *x_bf16_dev, const void *dy_bf16_dev, float *dw_f32_dev);
+int pcnn_dwconv_dgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *dy_bf16_dev, void *dx_bf16_dev);
+int pcnn_dwconv_info(int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int *out9);
 /* Softmax cross-entropy on bf16 logits [N][O], 1 <= O <= 256, labels uint8 [N]:
  *   p = softmax(row) evaluated in double: m = max, den = sum exp(z - m), p_t = exp(z_t - m) / den;
  *   dlogits[n][t] = bf16_rn(float_rn((p_t - [t == label]) * scale)), double -> fp32 -> bf16, each round to nearest even: the

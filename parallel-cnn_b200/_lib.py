@@ -165,6 +165,10 @@ _SIG = {
     "pcnn_linear_wgrad": [_vp, _vp, _vp, _vp, _vp],
     "pcnn_linear_dgrad": [_vp, _vp, _vp, _vp],
     "pcnn_linear_info": [_i, _i, _i, _i, _i, _i, _i, _vp],
+    "pcnn_dwconv_plan_create": [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _pvp],
+    "pcnn_dwconv_wgrad": [_vp, _vp, _vp, _vp, _vp],
+    "pcnn_dwconv_dgrad": [_vp, _vp, _vp, _vp],
+    "pcnn_dwconv_info": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_softmax_ce_bf16": [_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp],
     "pcnn_optim_create": [_vp, _vp, _vp, _i, _pvp],
     "pcnn_optim_step": [_vp, _vp, _f],
@@ -327,6 +331,17 @@ def linear_info(N, P, Q, C, O, row_pitch=0, image_rows=0):
     check("pcnn_linear_info", lib().pcnn_linear_info(int(N), int(P), int(Q), int(C), int(O), int(row_pitch), int(image_rows), out))
     return dict(row_pitch=out[0], image_tiles=out[1], fwd_steps=out[2], fwd_splits=out[3], fwd_stages=out[4], wgrad_pairs=out[5],
                 wgrad_splits=out[6], wgrad_stages=out[7], dgrad_tiles=out[8], dgrad_chunks=out[9], dgrad_stages=out[10], npad=out[11])
+
+
+def dwconv_info(N, H, W, C, R, S, stride=1, padding=(0, 0)):
+    """The output size and the weight-gradient split of the depthwise convolution (pcnn_dwconv_info; host only, no GPU), refused
+    as pcnn_dwconv_plan_create refuses.  vec: channels per thread (8 or 1); the N*P*Q output pixels are cut into `ranges` of
+    `pixels_per_range`, a function of the shape alone; n_acc: fp32 additions on the longest path of one dw sum."""
+    ph, pw = (int(v) for v in padding)
+    out = (_i * 9)()
+    check("pcnn_dwconv_info", lib().pcnn_dwconv_info(int(N), int(H), int(W), int(C), int(R), int(S), int(stride), ph, pw, out))
+    return dict(P=out[0], Q=out[1], vec=out[2], groups_per_cta=out[3], slices=out[4], lanes=out[5], pixels_per_range=out[6],
+                ranges=out[7], n_acc=out[8])
 
 
 def conv_bwd_plan_info(N, H, W, C, K, R, S, stride=1):

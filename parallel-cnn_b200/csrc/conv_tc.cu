@@ -242,6 +242,7 @@ struct pcnn_conv_plan {
     CUtensorMap map_b;
     ConvWidePlan *wide = nullptr;   // non-null: a plan of pcnn_conv_wide_plan_create (conv_wide_tc.cu), nothing above is used
     LinearPlan *linear = nullptr;   // non-null: a plan of pcnn_linear_plan_create (linear_tc.cu), nothing above is used
+    DwConvPlan *dw = nullptr;       // non-null: a plan of pcnn_dwconv_plan_create (dwconv_nhwc.cu), nothing above is used
 };
 
 pcnn_conv_plan *conv_plan_wrap_wide(ConvWidePlan *w) {
@@ -258,9 +259,18 @@ pcnn_conv_plan *conv_plan_wrap_linear(LinearPlan *l) {
 
 LinearPlan *conv_plan_linear(pcnn_conv_plan *plan) { return plan->linear; }
 
+pcnn_conv_plan *conv_plan_wrap_dw(DwConvPlan *d) {
+    pcnn_conv_plan *pl = new pcnn_conv_plan();
+    pl->dw = d;
+    return pl;
+}
+
+DwConvPlan *conv_plan_dw(pcnn_conv_plan *plan) { return plan->dw; }
+
 void conv_plan_operand(pcnn_conv_plan *plan, PlanOperand *out) {
     if (plan->wide) return conv_wide_operand(plan->wide, out);
     if (plan->linear) return linear_operand(plan->linear, out);
+    if (plan->dw) return dwconv_operand(plan->dw, out);
     const ConvTcParams &p = plan->p;
     *out = PlanOperand{nullptr, 0, 0, (long long)p.K * p.R * plan->S * p.C, plan->d_bias, p.K};
 }
@@ -278,6 +288,7 @@ static void free_plan(pcnn_conv_plan *plan) {
     if (!plan) return;
     if (plan->wide) conv_wide_free(plan->wide);
     if (plan->linear) linear_free(plan->linear);
+    if (plan->dw) dwconv_free(plan->dw);
     if (plan->d_toeplitz) cudaFree(plan->d_toeplitz);
     if (plan->d_bias) cudaFree(plan->d_bias);
     delete plan;
@@ -419,6 +430,7 @@ extern "C" int pcnn_conv_plan_set_params(pcnn_ctx *ctx, pcnn_conv_plan *plan, co
     if (filt_f32_dev) {
         const int rc = plan->wide     ? conv_wide_load_filters(ctx, plan->wide, filt_f32_dev)
                        : plan->linear ? linear_load_weights(ctx, plan->linear, filt_f32_dev)
+                       : plan->dw     ? dwconv_load_filters(ctx, plan->dw, filt_f32_dev)
                                       : conv_tc_load_filters(ctx, plan, filt_f32_dev);
         if (rc) return rc;
     }
@@ -432,6 +444,7 @@ extern "C" int pcnn_conv_tc_fwd(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void 
     pcnn_device_guard g(ctx->device);
     if (plan->wide) return conv_wide_fwd(ctx, plan->wide, x_bf16, y_bf16);
     if (plan->linear) return linear_fwd(ctx, plan->linear, x_bf16, y_bf16);
+    if (plan->dw) return dwconv_fwd(ctx, plan->dw, x_bf16, y_bf16);
     ConvTcParams p = plan->p;
     p.y = reinterpret_cast<__nv_bfloat16 *>(y_bf16);
     CUtensorMap map_x;

@@ -257,6 +257,15 @@ void linear_operand(LinearPlan *l, PlanOperand *out);
 int linear_load_weights(pcnn_ctx *ctx, LinearPlan *l, const float *w_dev);
 pcnn_conv_plan *conv_plan_wrap_linear(LinearPlan *l);   // conv_tc.cu; takes ownership
 LinearPlan *conv_plan_linear(pcnn_conv_plan *plan);
+// dwconv_nhwc.cu: a plan of pcnn_dwconv_plan_create holds a DwConvPlan, run, refreshed and freed like the linear one; its bf16
+// operand is [C][R][S], the fp32 master's element order (one row of C R S elements); conv_plan_dw is null for any other plan
+struct DwConvPlan;
+int dwconv_fwd(pcnn_ctx *ctx, const DwConvPlan *d, const void *x_bf16, void *y_bf16);
+void dwconv_free(DwConvPlan *d);
+void dwconv_operand(DwConvPlan *d, PlanOperand *out);
+int dwconv_load_filters(pcnn_ctx *ctx, DwConvPlan *d, const float *filt_dev);
+pcnn_conv_plan *conv_plan_wrap_dw(DwConvPlan *d);   // conv_tc.cu; takes ownership
+DwConvPlan *conv_plan_dw(pcnn_conv_plan *plan);
 // a temporary device copy of host data (the create calls upload their filters through one); freed when it goes out of scope
 struct pcnn_dev_temp {
     float *p = nullptr;

@@ -5,7 +5,7 @@ import ctypes as C
 import numpy as np
 
 from ._lib import (F32, NPARAM, OPTIM_ADAMW, OPTIM_SGD, TEST_SET, TRAIN_SET, U8, OptimConfig, OptimTensor, PcnnError, avgpool_nhwc_info,
-                   batchnorm_nhwc_info, check, conv_layer_family, global_avgpool_nhwc_info, lib, linear_info, maxpool_nhwc_info)
+                   batchnorm_nhwc_info, check, conv_layer_family, dwconv_info, global_avgpool_nhwc_info, lib, linear_info, maxpool_nhwc_info)
 
 
 def _pixel_type(arr_or_dtype):
@@ -490,6 +490,15 @@ class Engine:
         """pcnn_linear_dgrad: dx = dy W with the plan's bf16 weights, written in x's layout (pad untouched)"""
         self._call("pcnn_linear_dgrad", plan.plan, _p(dy), _p(dx))
 
+    def dwconv_wgrad(self, plan, x, dy, dw):
+        """pcnn_dwconv_wgrad: dw fp32 [C][R][S] = the sum over the pixels of dy * x (x +0 outside the image), overwritten; the shape
+        from the DepthwiseConvPlan"""
+        self._call("pcnn_dwconv_wgrad", plan.plan, _p(x), _p(dy), _p(dw))
+
+    def dwconv_dgrad(self, plan, dy, dx):
+        """pcnn_dwconv_dgrad: dx dense bf16 [N][H][W][C] from dy with the plan's bf16 filters, every element written"""
+        self._call("pcnn_dwconv_dgrad", plan.plan, _p(dy), _p(dx))
+
 
 class ConvPlan:
     """bf16 tensor-core convolution plan (pcnn_conv_tc_*): filters fp32 KRSC on the host, activations NHWC bf16.  act is
@@ -576,6 +585,26 @@ class LinearPlan(ConvPlan):
         self.out_shape = (N, O)
 
 
+class DepthwiseConvPlan(ConvPlan):
+    """A depthwise convolution's plan (pcnn_dwconv_plan_create): conv2d(x, w, b, stride, padding, groups=C) with x dense bf16
+    [N][H][W][C], y dense bf16 [N][P][Q][C], filters fp32 [C][R][S] (torch's weight [C][1][R][S] reshaped), bias fp32 [C].  act
+    ACT_NONE (0) or ACT_RELU (3).  Run, refreshed and closed like ConvPlan; its gradients are Engine.dwconv_wgrad / dwconv_dgrad."""
+
+    def __init__(self, engine, N, H, W, C, R, S, filt, bias=None, act=0, stride=1, padding=(0, 0)):
+        self.engine = engine
+        self.shape = (N, H, W, C, R, S)
+        ph, pw = (int(v) for v in padding)
+        filt = np.ascontiguousarray(filt, np.float32)
+        assert filt.size == C * R * S
+        b = None if bias is None else np.ascontiguousarray(bias, np.float32)
+        plan = C_.c_void_p()
+        check("pcnn_dwconv_plan_create",
+              lib().pcnn_dwconv_plan_create(engine.ctx, N, H, W, C, R, S, int(stride), ph, pw, int(act), filt.ctypes.data,
+                                            None if b is None else b.ctypes.data, C_.byref(plan)))
+        self.plan = plan
+        self.out_shape = (N, (H + 2 * ph - R) // stride + 1, (W + 2 * pw - S) // stride + 1, C)
+
+
 class ConvLayer:
     """One bf16 convolution layer trained on the device: forward, backward and an SGD step with no host round trip.
 
@@ -644,6 +673,76 @@ class ConvLayer:
 
     def params(self):
         """host copies (filters [K][R][S][C], bias [K] or None) of the fp32 masters"""
+        return self.filt.to_host(), None if self.bias is None else self.bias.to_host()
+
+    def close(self):
+        self.plan.close()
+        for a in (self.filt, self.bias, self.dw, self.db):
+            if a is not None:
+                a.free()
+
+
+class DepthwiseConvLayer:
+    """A depthwise convolution trained on the device (groups = C: each channel filtered by its own R x S filter), with ConvLayer's
+    interface: fp32 masters filt [C][R][S] and bias [C], their gradients dw and db, and a DepthwiseConvPlan holding the filters in
+    bf16.  x and dx are dense bf16 [N][H][W][C], y and dy dense [N][P][Q][C]: what a ConvLayer or a BatchNormLayer writes and reads,
+    so an inverted-residual block runs with no copies:
+
+        expand.forward(x, ye);  bn1.forward(ye, ze);  dw.forward(ze, yd);  bn2.forward(yd, zd);  project.forward(zd, yp)
+        ...;  bn2.backward(zd, dzd, dyd);  dw.backward(yd, dyd, dze);  bn1.backward(ze, dze, dye)
+
+    act ACT_RELU (3) is a ReLU after the bias, ACT_NONE (0) none; the sigmoid is refused.  With a bias or an activation, backward
+    first runs pcnn_conv_bias_act_bwd over dy, which takes at most 256 channels: such a layer needs C <= 256.  Without either
+    (the usual case in front of a batch norm) C is unlimited."""
+
+    def __init__(self, engine, N, H, W, C, R, S, filt, bias=None, act=0, stride=1, padding=(0, 0)):
+        self.engine = engine
+        self.shape = (N, H, W, C, R, S)
+        self.act, self.stride = int(act), int(stride)
+        self.padding = tuple(int(v) for v in padding)
+        self.info = dwconv_info(N, H, W, C, R, S, self.stride, self.padding)
+        filt = np.ascontiguousarray(filt, np.float32).reshape(C, R, S)
+        bias = None if bias is None else np.ascontiguousarray(bias, np.float32).reshape(C)
+        self.plan = DepthwiseConvPlan(engine, N, H, W, C, R, S, filt, bias, act=act, stride=self.stride, padding=self.padding)
+        self.out_shape = self.plan.out_shape
+        self.pixels = int(np.prod(self.out_shape[:3]))
+        self.filt = DeviceArray.from_host(engine, filt)
+        self.bias = None if bias is None else DeviceArray.from_host(engine, bias)
+        self.dw = engine.array((C, R, S))
+        self.db = None if bias is None else engine.array(C)
+        self._x = None
+
+    def forward(self, x, y):
+        """y = act(dwconv(x) + bias) with the plan's bf16 filters.  The layer keeps x: backward's weight gradient reads it."""
+        self.plan.fwd(x, y)
+        self._x = x
+
+    def backward(self, y, dy, dx=None):
+        """Gradients of the most recent forward, whose output y was: dw, db (with a bias) and dx (when given).  dy is CONSUMED with
+        a ReLU: it is overwritten in place by the gradient at the pre-activation (pcnn_conv_bias_act_bwd, skipped without
+        activation and bias).  dx uses the plan's bf16 filters, so call it before sgd or an optimizer step."""
+        C = self.shape[3]
+        e = self.engine
+        if self.act or self.bias is not None:
+            e.conv_bias_act_bwd(y if self.act else None, dy, dy if self.act else None, self.db, self.pixels, C, self.act)
+        e.dwconv_wgrad(self.plan, self._x, dy, self.dw)
+        if dx is not None:
+            e.dwconv_dgrad(self.plan, dy, dx)
+
+    def sgd(self, lr):
+        """w += (-lr) * dw and b += (-lr) * db in fp32 on the masters, then the plan refreshed from them, all on the engine's stream"""
+        N, H, W, C, R, S = self.shape
+        self.engine.apply_grad_scaled(self.filt, self.dw, C * R * S, -lr)
+        if self.bias is not None:
+            self.engine.apply_grad_scaled(self.bias, self.db, C, -lr)
+        self.plan.set_params(self.filt, self.bias)
+
+    def optim_tensors(self):
+        """(param, grad, plan, plan part, is norm or bias) of the filters and the bias, as ConvLayer.optim_tensors"""
+        return [(self.filt, self.dw, self.plan, 1, False)] + ([] if self.bias is None else [(self.bias, self.db, self.plan, 2, True)])
+
+    def params(self):
+        """host copies (filters [C][R][S], bias [C] or None) of the fp32 masters"""
         return self.filt.to_host(), None if self.bias is None else self.bias.to_host()
 
     def close(self):
@@ -896,8 +995,9 @@ class GlobalAvgPoolLayer:
 
 class FusedOptimizer:
     """One fused update of many fp32 parameter tensors per step (pcnn_optim_*; the rules and their order are in include/pcnn.h).
-    tensors: (param, grad, n, weight_decay, plan, plan part) with plan None (part 0) or the ConvPlan / LinearPlan whose filters (part 1)
-    or bias (part 2) param is the master of; the plan's operands are refreshed by the step.  kind OPTIM_SGD or OPTIM_ADAMW.  SGD and
+    tensors: (param, grad, n, weight_decay, plan, plan part) with plan None (part 0) or the ConvPlan / LinearPlan / DepthwiseConvPlan
+    whose filters (part 1) or bias (part 2) param is the master of; the plan's operands are refreshed by the step.  kind OPTIM_SGD or
+    OPTIM_ADAMW.  SGD and
     AdamW build the table from layers; this class takes it directly."""
 
     def __init__(self, engine, kind, tensors, momentum=0.0, dampening=0.0, nesterov=False, betas=(0.9, 0.999), eps=1e-8):
@@ -968,8 +1068,8 @@ def _layer_tensors(layers, weight_decay, decay_norm_and_bias):
 
 
 class SGD(FusedOptimizer):
-    """torch.optim.SGD over the trainable tensors of ConvLayers, LinearLayers and BatchNormLayers, in one launch per step with the
-    layers' plans refreshed: step(lr) replaces every layer.sgd(lr) of a training step (momentum 0 and weight decay 0 give the same
+    """torch.optim.SGD over the trainable tensors of ConvLayers, DepthwiseConvLayers, LinearLayers and BatchNormLayers, in one launch
+    per step with the layers' plans refreshed: step(lr) replaces every layer.sgd(lr) of a training step (momentum 0 and weight decay 0 give the same
     bits).  decay_norm_and_bias=False gives batch normalization's gamma and beta and the biases weight decay 0; the default decays
     every tensor, as torch.optim does with one parameter group."""
 

@@ -827,6 +827,118 @@ def run_resnetgap_optim(N, iters, rounds=3):
                       "kernel_launches_per_update": launches, "gpu": gpu, "power_limit": power}), flush=True)
 
 
+def run_dwconv(name, N, H, W, C, R, stride, pad, iters):
+    """the three passes of a depthwise convolution (pcnn_conv_tc_fwd on a DepthwiseConvPlan, pcnn_dwconv_dgrad, pcnn_dwconv_wgrad)
+    next to F.conv2d(groups=C) and aten.convolution_backward on the same bf16 channels-last tensors.  Bytes per pass: x and y (or
+    dy and dx, or x and dy) crossing HBM once, N (H W + P Q) C 2; the weight gradient adds its fp32 slots, written and read once,
+    and dw."""
+    info = pkg.dwconv_info(N, H, W, C, R, R, stride, (pad, pad))
+    P, Q = info["P"], info["Q"]
+    w = rng.uniform(-0.5, 0.5, (C, R, R)).astype(np.float32)
+    plan = pkg.DepthwiseConvPlan(eng, N, H, W, C, R, R, w, None, act=0, stride=stride, padding=(pad, pad))
+    bits = lambda *shape: torch.randint(0, 0x3F80, shape, dtype=torch.int16, device="cuda")
+    x, dy = bits(N, H, W, C), bits(N, P, Q, C)
+    y, dx = torch.empty((N, P, Q, C), dtype=torch.int16, device="cuda"), torch.empty((N, H, W, C), dtype=torch.int16, device="cuda")
+    dw = torch.empty((C, R, R), dtype=torch.float32, device="cuda")
+    gpu, power = card()
+    act_bytes = N * (H * W + P * Q) * C * 2
+    slot_bytes = (2 * info["ranges"] * C * R * R * 4 if info["ranges"] > 1 else 0) + C * R * R * 4
+    xt = x.view(torch.bfloat16).permute(0, 3, 1, 2)
+    dyt = dy.view(torch.bfloat16).permute(0, 3, 1, 2)
+    wt = torch.from_numpy(w).to("cuda").to(torch.bfloat16)[:, None].contiguous(memory_format=torch.channels_last)
+    F = torch.nn.functional
+    cb = torch.ops.aten.convolution_backward
+    passes = (
+        ("fwd", lambda: plan.fwd(x, y), lambda: F.conv2d(xt, wt, None, stride, pad, groups=C), act_bytes),
+        ("dgrad", lambda: eng.dwconv_dgrad(plan, dy, dx),
+         lambda: cb(dyt, xt, wt, None, [stride] * 2, [pad] * 2, [1, 1], False, [0, 0], C, [True, False, False]), act_bytes),
+        ("wgrad", lambda: eng.dwconv_wgrad(plan, x, dy, dw),
+         lambda: cb(dyt, xt, wt, None, [stride] * 2, [pad] * 2, [1, 1], False, [0, 0], C, [False, True, False]), act_bytes + slot_bytes),
+    )
+    for what, ours, theirs, nbytes in passes:
+        ms, ms_torch = timed(ours, iters), timed(theirs, iters)
+        print(json.dumps({"case": f"dwconv {name} {what}", "N": N, "us": ms * 1e3, "MB": nbytes / 1e6,
+                          "share_of_3350": nbytes / (ms * 1e-3) / 1e9 / HBM, "torch_us": ms_torch * 1e3, "torch_over_ours": ms_torch / ms,
+                          "vec": info["vec"], "wgrad_ranges": info["ranges"], "gpu": gpu, "power_limit": power}), flush=True)
+    plan.close()
+
+
+def run_mbblock(N, iters, k=3):
+    """one training step of an inverted-residual block at 28x28x40, N = 128: 1x1 expand to 240 -> BN + ReLU -> depthwise k x k pad
+    k // 2 -> BN + ReLU -> 1x1 project to 40 -> BN + x0, its backward (the shortcut's gradient dres left apart, as run_resblock)
+    and the sgd of the six layers, on the engine's stream.  Next to it the torch eager step of the same block on bf16 channels-last
+    tensors (fp32 masters, w -= lr * grad, re-cast to bf16)."""
+    H = W = 28
+    C, E = 40, 240
+    r = np.random.default_rng(12)
+    u = lambda shape, fan: r.uniform(-1, 1, shape).astype(np.float32) / np.float32(np.sqrt(fan))
+    fe, fd, fp = u((E, 1, 1, C), C), u((E, k, k), k * k), u((C, 1, 1, E), E)
+    ex = pkg.ConvLayer(eng, N, H, W, C, E, 1, 1, fe, None, act=0)
+    dwl = pkg.DepthwiseConvLayer(eng, N, H, W, E, k, k, fd, None, act=0, padding=(k // 2, k // 2))
+    pr = pkg.ConvLayer(eng, N, H, W, E, C, 1, 1, fp, None, act=0)
+    b1, b2 = pkg.BatchNormLayer(eng, N, H, W, E, act=pkg.ACT_RELU), pkg.BatchNormLayer(eng, N, H, W, E, act=pkg.ACT_RELU)
+    b3 = pkg.BatchNormLayer(eng, N, H, W, C, act=0)
+    wide = lambda: torch.empty((N, H, W, E), dtype=torch.int16, device="cuda")
+    narrow = lambda: torch.empty((N, H, W, C), dtype=torch.int16, device="cuda")
+    x0 = torch.randint(0, 0x3F80, (N, H, W, C), dtype=torch.int16, device="cuda")
+    dout = torch.randint(0, 0x3F80, (N, H, W, C), dtype=torch.int16, device="cuda")
+    dout ^= torch.randint(0, 2, (N, H, W, C), dtype=torch.int16, device="cuda") << 15
+    ye, ze, yd, zd, dze, dye, dyd, dzd = (wide() for _ in range(8))
+    yp, out, dyp, dres, dx0 = (narrow() for _ in range(5))
+    lr = 0.05
+    gpu, power = card()
+
+    def step():
+        ex.forward(x0, ye); b1.forward(ye, ze); dwl.forward(ze, yd); b2.forward(yd, zd); pr.forward(zd, yp); b3.forward(yp, out, r=x0)
+        b3.backward(out, dout, dyp, dr=dres); pr.backward(yp, dyp, dzd); b2.backward(zd, dzd, dyd); dwl.backward(yd, dyd, dze)
+        b1.backward(ze, dze, dye); ex.backward(ye, dye, dx0)
+        for layer in (ex, b1, dwl, b2, pr, b3):
+            layer.sgd(lr)
+
+    ms = timed(step, iters)
+    F = torch.nn.functional
+    xt = x0.view(torch.bfloat16).permute(0, 3, 1, 2).detach().requires_grad_(True)
+    dt = dout.view(torch.bfloat16).permute(0, 3, 1, 2)
+    cl = lambda a: torch.from_numpy(a).to("cuda").contiguous(memory_format=torch.channels_last)
+    m32 = {"fe": cl(fe.transpose(0, 3, 1, 2)), "fd": cl(fd[:, None]), "fp": cl(fp.transpose(0, 3, 1, 2))}
+    for i, ch in ((1, E), (2, E), (3, C)):
+        m32[f"g{i}"], m32[f"b{i}"] = torch.ones(ch, device="cuda"), torch.zeros(ch, device="cuda")
+    mb = {kk: (v.to(torch.bfloat16) if kk.startswith("f") else v.clone()).requires_grad_(True) for kk, v in m32.items()}
+    stats = [torch.zeros(ch, device="cuda") if j % 2 == 0 else torch.ones(ch, device="cuda") for ch in (E, E, C) for j in range(2)]
+
+    def torch_step():
+        for v in mb.values():
+            v.grad = None
+        xt.grad = None
+        h = torch.relu(F.batch_norm(F.conv2d(xt, mb["fe"]), stats[0], stats[1], mb["g1"], mb["b1"], training=True))
+        h = torch.relu(F.batch_norm(F.conv2d(h, mb["fd"], padding=k // 2, groups=E), stats[2], stats[3], mb["g2"], mb["b2"], training=True))
+        h = F.batch_norm(F.conv2d(h, mb["fp"]), stats[4], stats[5], mb["g3"], mb["b3"], training=True) + xt
+        h.backward(dt)
+        with torch.no_grad():
+            for kk in m32:
+                m32[kk].add_(mb[kk].grad.float(), alpha=-lr)
+                mb[kk].copy_(m32[kk])
+
+    ms_torch = timed(torch_step, iters)
+    ms_dw = {"fwd": timed(lambda: dwl.forward(ze, yd), iters), "bwd": timed(lambda: (eng.dwconv_wgrad(dwl.plan, ze, dyd, dwl.dw),
+                                                                                      eng.dwconv_dgrad(dwl.plan, dyd, dze)), iters)}
+    print(json.dumps({"case": f"inverted-residual block 28x28x40 -> 240 dw {k}x{k} training step N={N}", "ms": ms, "torch_eager_ms": ms_torch,
+                      "ours_over_torch": ms / ms_torch, "dw_fwd_ms": ms_dw["fwd"], "dw_bwd_ms": ms_dw["bwd"], "families": [ex.family, pr.family],
+                      "gpu": gpu, "power_limit": power}), flush=True)
+    for layer in (ex, b1, dwl, b2, pr, b3):
+        layer.close()
+
+
+if only == "dwconv":                                                   # depthwise convolution passes, torch beside them
+    for args in (("112x112x32 3x3/1", 128, 112, 112, 32, 3, 1, 1), ("112x112x96 3x3/2", 128, 112, 112, 96, 3, 2, 1),
+                 ("56x56x144 3x3/1", 128, 56, 56, 144, 3, 1, 1), ("56x56x144 3x3/2", 128, 56, 56, 144, 3, 2, 1),
+                 ("28x28x192 3x3/1", 128, 28, 28, 192, 3, 1, 1), ("14x14x384 3x3/1", 128, 14, 14, 384, 3, 1, 1),
+                 ("7x7x960 3x3/1", 128, 7, 7, 960, 3, 1, 1), ("28x28x240 5x5/1", 128, 28, 28, 240, 5, 1, 2),
+                 ("28x28x240 5x5/2", 128, 28, 28, 240, 5, 2, 2), ("56x56x6 3x3/1 (scalar path)", 128, 56, 56, 6, 3, 1, 1)):
+        run_dwconv(*args, 20)
+if only == "mbblock":                                                  # one step of an inverted-residual block, torch eager beside it
+    run_mbblock(128, 20, 3)
+    run_mbblock(128, 20, 5)
 if only == "optim":                                                    # the fused optimizers over the ResNet-18 table, torch beside them
     run_optim(50)
 if only == "resnetgap-optim":                                          # the GAP ResNet step with each update, alternated
