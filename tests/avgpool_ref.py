@@ -8,6 +8,8 @@ import numpy as np
 
 from maxpool_ref import out_size
 
+U = 2.0 ** -24
+
 
 def counts(H, W, R, S, stride, pad_h, pad_w, count_include_pad):
     """cnt[p][q]: R*S, or the window's in-image positions"""
@@ -89,6 +91,19 @@ def global_fwd(x, info):
 def global_f64(x):
     """the float64 mean over the pixels of each image and channel: [N][C]"""
     return x.astype(np.float64).mean(axis=(1, 2))
+
+
+def gap_bound(pkg, xf, info):
+    """[lo, hi] of the error model of the global pool's y (test_avgpool_nhwc_gpu.py's docstring) for every y, as float32 values:
+    returns the float64 mean m, the bound E of |fp32 sum / (H*W) - m|, and m - E and m + E rounded to bf16"""
+    N, H, W, C = xf.shape
+    n_acc = (info["pixels_per_cta"] // info["lanes"] - 1) + (info["lanes"] - 1) + (info["ranges"] - 1)
+    gamma = n_acc * U / (1 - n_acc * U)
+    x64 = xf.astype(np.float64)
+    S, A = x64.sum(axis=(1, 2)), np.abs(x64).sum(axis=(1, 2))
+    m, E = S / (H * W), (gamma * A + U * (np.abs(S) + gamma * A)) / (H * W)
+    bf, f32 = pkg.f32_to_bf16_bits, pkg.bf16_bits_to_f32
+    return m, E, f32(bf((m - E).astype(np.float32))), f32(bf((m + E).astype(np.float32)))
 
 
 def global_bwd(dy, H, W):

@@ -6,10 +6,39 @@
 - numpy float32 replays of the formulas of include/pcnn.h, every operation rounded as the kernels round it, given the statistics,
   dgamma and dbeta the device computed: fwd_bits, eval_rstd, running_update, grad_bits and dx_bits.
 
-numpy float32 arithmetic is IEEE round to nearest with no contraction, which is what the kernels use."""
+numpy float32 arithmetic is IEEE round to nearest with no contraction, which is what the kernels use.
+
+n_stat, n_acc and check_stats state the error model of the device's statistics and gradient sums (test_batchnorm_gpu.py's
+docstring derives it)."""
 import numpy as np
 
 F32 = np.float32
+U = 2.0 ** -24
+ITERS = 16
+
+
+def n_stat(pkg, pixels, C):
+    return ITERS + pkg.batchnorm_nhwc_info(pixels, C)["lanes"] + 3
+
+
+def n_acc(pkg, pixels, C):
+    info = pkg.batchnorm_nhwc_info(pixels, C)
+    return ITERS + info["lanes"] + -(-info["grad_slots"] // 8) + 3
+
+
+def check_stats(pkg, xb, mean, rstd, eps):
+    """the device's batch mean and variance (read back from rstd) within the error model of float64 over x's bf16 bits [pixels][C];
+    returns the float64 mean, variance and the variance bound"""
+    pixels, C = xb.shape
+    x = pkg.bf16_bits_to_f32(xb).astype(np.float64)
+    m64, v64 = x.mean(0), ((x - x.mean(0)) ** 2).mean(0)
+    R = x.max(0) - x.min(0)
+    n = n_stat(pkg, pixels, C)
+    var = 1.0 / rstd.astype(np.float64) ** 2 - np.float64(np.float32(eps))
+    assert np.all(np.abs(mean - m64) <= n * U * R + U * np.abs(m64)), np.abs(mean - m64).max()
+    bound = 5 * n * U * R ** 2 + 4 * U * (v64 + eps)
+    assert np.all(np.abs(var - v64) <= bound), (np.abs(var - v64) / bound).max()
+    return m64, v64, bound
 
 
 def relu(v):

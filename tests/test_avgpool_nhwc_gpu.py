@@ -15,6 +15,7 @@ import torch
 
 import avgpool_ref as AR
 import maxpool_ref as MR
+from avgpool_ref import gap_bound
 
 pytestmark = pytest.mark.gpu
 
@@ -136,18 +137,6 @@ def test_windowed(eng, pkg, case, cip):
 
 
 GSHAPES = [(3, H, W, C) for C in (1, 6, 8, 300, 2048) for H, W in ((1, 1), (7, 7), (56, 56))] + [(8, 56, 56, 256)]
-
-
-def gap_bound(pkg, xf, info):
-    """[lo, hi] of the error model (module docstring) for every y, as float32 values"""
-    N, H, W, C = xf.shape
-    n_acc = (info["pixels_per_cta"] // info["lanes"] - 1) + (info["lanes"] - 1) + (info["ranges"] - 1)
-    gamma = n_acc * U / (1 - n_acc * U)
-    x64 = xf.astype(np.float64)
-    S, A = x64.sum(axis=(1, 2)), np.abs(x64).sum(axis=(1, 2))
-    m, E = S / (H * W), (gamma * A + U * (np.abs(S) + gamma * A)) / (H * W)
-    bf, f32 = pkg.f32_to_bf16_bits, pkg.bf16_bits_to_f32
-    return m, E, f32(bf((m - E).astype(np.float32))), f32(bf((m + E).astype(np.float32)))
 
 
 @pytest.mark.parametrize("shape", GSHAPES, ids=["x".join(map(str, s)) for s in GSHAPES])

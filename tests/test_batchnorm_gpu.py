@@ -18,28 +18,18 @@ import torch
 import batchnorm_ref as BR
 import conv_ref as CR
 import conv_ref_strided as CS
+from batchnorm_ref import ITERS, U, check_stats, n_acc, n_stat  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
 NAN_BF16 = 0x7FC0
 DEV = torch.device("cuda", 0)
 TAIL = 64
-U = 2.0 ** -24
-ITERS = 16
 
 CS_ = [1, 6, 8, 16, 64, 120, 256]
 PIXELS = [2, 7, 1001]
 GRID = [(C, p) for C in CS_ for p in PIXELS] + [(64, 128 * 56 * 56)]
 GIDS = [f"C{C}-px{p}" for C, p in GRID]
-
-
-def n_stat(pkg, pixels, C):
-    return ITERS + pkg.batchnorm_nhwc_info(pixels, C)["lanes"] + 3
-
-
-def n_acc(pkg, pixels, C):
-    info = pkg.batchnorm_nhwc_info(pixels, C)
-    return ITERS + info["lanes"] + -(-info["grad_slots"] // 8) + 3
 
 
 def bits(pkg, a):
@@ -81,19 +71,6 @@ def run_fwd(eng, xb, rb, st, act, training, eps=1e-5, momentum=0.1):
         if a is not None:
             a.free()
     return out
-
-
-def check_stats(pkg, xb, mean, rstd, eps):
-    pixels, C = xb.shape
-    x = pkg.bf16_bits_to_f32(xb).astype(np.float64)
-    m64, v64 = x.mean(0), ((x - x.mean(0)) ** 2).mean(0)
-    R = x.max(0) - x.min(0)
-    n = n_stat(pkg, pixels, C)
-    var = 1.0 / rstd.astype(np.float64) ** 2 - np.float64(np.float32(eps))
-    assert np.all(np.abs(mean - m64) <= n * U * R + U * np.abs(m64)), np.abs(mean - m64).max()
-    bound = 5 * n * U * R ** 2 + 4 * U * (v64 + eps)
-    assert np.all(np.abs(var - v64) <= bound), (np.abs(var - v64) / bound).max()
-    return m64, v64, bound
 
 
 # ------------------------------------------------------------------------------------------------ forward
