@@ -623,6 +623,45 @@ int pcnn_dwconv_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C, int R, in
 int pcnn_dwconv_wgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *x_bf16_dev, const void *dy_bf16_dev, float *dw_f32_dev);
 int pcnn_dwconv_dgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *dy_bf16_dev, void *dx_bf16_dev);
 int pcnn_dwconv_info(int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int *out9);
+/* Squeeze-and-excitation channel gating (csrc/se_nhwc.cu): y = act(x * s[n][c] + r), s = sigmoid(fc2(relu(fc1(GAP(x))))) a gate per
+ * image and channel, as in SE-ResNet, MnasNet, MobileNetV3 and EfficientNet.  The squeeze branch runs on the existing layers:
+ * pcnn_global_avgpool_nhwc_bf16_fwd writes the x of a linear layer, and linear layers with act 3 and act 1 give s.
+ *   - x, r, y, dy, dy2, g and dx are dense bf16 [N][H][W][C]: what the conv forwards and batch norm write as y and read as dy;
+ *   - s and ds are dense bf16 [N][C]: the y and dy of a linear layer with O = C;
+ *   - dpool is bf16 [N][dpool_row_pitch]: the dy of the global average pool (the dx of the squeeze branch's first linear layer);
+ *     row pitch 0 = C rounded up to 8, otherwise >= C and a multiple of 8, as pcnn_global_avgpool_nhwc_bf16_bwd.
+ * Rules: every fp32 operation rounds to nearest with no contraction (RN below; a bf16 x bf16 product is exact in fp32 but for
+ * underflow, and the kernels round it on its own before any add).
+ *   Forward: v = RN(float(x) * float(s[n][c])); v = RN(v + float(r)) when r is given; y = bf16_rn(act(v)), act 0 (none) or 3 (the
+ *     ReLU of the conv epilogues: v < 0 ? +0 : v, NaN and -0 unchanged).  Act 1 is refused: the sigmoid uses tanh.approx, which no
+ *     reference can replay bit for bit.
+ *   Gate gradient (before the squeeze branch's backward): t = float(dy), or RN(float(dy) + float(dy2)) when dy2 (a second gradient
+ *     arriving at a residual join) is given; g = bf16_rn(act'(t)) as batch norm's backward: at act 3 float(y) <= 0 gives +0 (a NaN y
+ *     passes t); without dy2 dy's bits pass.  g is the gradient of r and the input of the input gradient; g == dy (in place) is
+ *     allowed.  ds[n][c] = bf16_rn(the fp32 sum of RN(float(g) * float(x)) over the H W pixels), summed in the order of the global
+ *     average pool's partition: the pixels cut into ranges of `pixels per CTA`; in a range, lane l sums the pixels l, l + lanes, ...
+ *     from its first one; the lanes holding a pixel are added in lane order; the ranges of an image in range order, through fp32
+ *     slots in the context's scratch block when there are several.  The partition depends on (N, H, W, C) alone, never on the SM
+ *     count; pcnn_se_scale_nhwc_info reports it.  ds is the dy of the sigmoid linear layer that wrote s.
+ *   Input gradient (after the squeeze branch's backward has written dpool): dx = bf16_rn(RN(float(g) * float(s[n][c]))) without
+ *     dpool; with it dx = bf16_rn(RN(RN(float(g) * float(s[n][c])) + RN(float(dpool[n][c]) / float(H W)))), the quotient being the one
+ *     pcnn_global_avgpool_nhwc_bf16_bwd rounds: the squeeze branch's gradient joins in the same pass.  dx == g is allowed.  Every
+ *     element of dx is written, with no memset and no atomics; the pad of dpool is never read.
+ * Domain (anything else is PCNN_ERR_ARG with the function and the rule in the message): N, H, W, C >= 1 (C has no upper limit);
+ * H W C within the 32-bit index range of one image, as the global average pool; act 0 or 3; y not NULL at act 3 in the gate pass;
+ * every pointer 16-byte aligned; only g == dy and dx == g may share memory.  With C % 8 == 0 the passes move 16-byte vectors of 8
+ * channels, otherwise single elements.  Stream-ordered; elements past the tensors are never written; the same bits on every run
+ * and SM count.
+ * pcnn_se_scale_nhwc_info: host only (no GPU, no context).  out8 = { channels per thread (8 or 1), channel groups per CTA, channel
+ * slices, pixel lanes per CTA, pixels per CTA (8 per lane), pixel ranges per image, CTAs of the gate pass, n_acc: the fp32 additions
+ * on the longest path of one ds sum (pixels of a lane - 1, lanes holding a pixel - 1, ranges - 1) }. */
+int pcnn_se_scale_nhwc_bf16_fwd(pcnn_ctx *ctx, const void *x_bf16_dev, const void *s_bf16_dev, const void *r_bf16_dev, void *y_bf16_dev,
+                                int N, int H, int W, int C, int act);
+int pcnn_se_scale_nhwc_bf16_bwd_gate(pcnn_ctx *ctx, const void *x_bf16_dev, const void *y_bf16_dev, const void *dy_bf16_dev,
+                                     const void *dy2_bf16_dev, void *g_bf16_dev, void *ds_bf16_dev, int N, int H, int W, int C, int act);
+int pcnn_se_scale_nhwc_bf16_bwd_input(pcnn_ctx *ctx, const void *g_bf16_dev, const void *s_bf16_dev, const void *dpool_bf16_dev,
+                                      int dpool_row_pitch, void *dx_bf16_dev, int N, int H, int W, int C);
+int pcnn_se_scale_nhwc_info(int N, int H, int W, int C, int *out8);
 /* Softmax cross-entropy on bf16 logits [N][O], 1 <= O <= 256, labels uint8 [N]:
  *   p = softmax(row) evaluated in double: m = max, den = sum exp(z - m), p_t = exp(z_t - m) / den;
  *   dlogits[n][t] = bf16_rn(float_rn((p_t - [t == label]) * scale)), double -> fp32 -> bf16, each round to nearest even: the

@@ -169,6 +169,10 @@ _SIG = {
     "pcnn_dwconv_wgrad": [_vp, _vp, _vp, _vp, _vp],
     "pcnn_dwconv_dgrad": [_vp, _vp, _vp, _vp],
     "pcnn_dwconv_info": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
+    "pcnn_se_scale_nhwc_bf16_fwd": [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i],
+    "pcnn_se_scale_nhwc_bf16_bwd_gate": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i],
+    "pcnn_se_scale_nhwc_bf16_bwd_input": [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i],
+    "pcnn_se_scale_nhwc_info": [_i, _i, _i, _i, _vp],
     "pcnn_softmax_ce_bf16": [_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp],
     "pcnn_optim_create": [_vp, _vp, _vp, _i, _pvp],
     "pcnn_optim_step": [_vp, _vp, _f],
@@ -342,6 +346,16 @@ def dwconv_info(N, H, W, C, R, S, stride=1, padding=(0, 0)):
     check("pcnn_dwconv_info", lib().pcnn_dwconv_info(int(N), int(H), int(W), int(C), int(R), int(S), int(stride), ph, pw, out))
     return dict(P=out[0], Q=out[1], vec=out[2], groups_per_cta=out[3], slices=out[4], lanes=out[5], pixels_per_range=out[6],
                 ranges=out[7], n_acc=out[8])
+
+
+def se_scale_nhwc_info(N, H, W, C):
+    """How the squeeze-and-excitation gate gradient partitions a shape (pcnn_se_scale_nhwc_info; host only, no GPU): the global
+    average pool's partition (global_avgpool_nhwc_info), refused as the three passes refuse.  vec: channels per thread (8 or 1);
+    n_acc: fp32 additions on the longest path of one ds sum."""
+    out = (_i * 8)()
+    check("pcnn_se_scale_nhwc_info", lib().pcnn_se_scale_nhwc_info(int(N), int(H), int(W), int(C), out))
+    return dict(vec=out[0], groups_per_cta=out[1], slices=out[2], lanes=out[3], pixels_per_cta=out[4], ranges=out[5], ctas=out[6],
+                n_acc=out[7])
 
 
 def conv_bwd_plan_info(N, H, W, C, K, R, S, stride=1):

@@ -282,6 +282,36 @@ struct ConvWideShape { int Pt, Qt, nch, stages, tiles, n_pb, n_qb, npad, P, Q; C
 int conv_wide_shape(const char *fn, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch,
                     int image_rows, ConvWideShape *out);
 long long conv_wide_pixel_block(int P, int Q, int *Pt, int *Qt);
+// pool_nhwc.cu: the partition of the global average pool's reduction over the pixels of an image, which the gate gradient of
+// squeeze-and-excitation (se_nhwc.cu) shares so that both sum in one order.  CTA (n, range, slice) of GAP_THREADS threads owns
+// pixels [range * per_cta, (range + 1) * per_cta) and channel groups [slice * Gc, (slice + 1) * Gc); thread t keeps group t % Gc of
+// the pixels lane, lane + lanes, ... (lane = t / Gc, GAP_ITERS of them), summed from the first; the lanes are then added in lane
+// order, and with several ranges the ranges in range order through fp32 slots.  gap_shape is the domain (refused with
+// PCNN_ERR_ARG and a message naming `fn`) and the partition, a function of (N, H, W, C) and the row pitch alone.
+constexpr int GAP_THREADS = 256;
+constexpr int GAP_ITERS = 8;                // pixels per lane
+struct GapArgs {
+    int HW, C, G;           // pixels per image, channels, channel groups of VEC
+    int Gc, slices;         // groups per CTA, channel slices
+    int lanes, per_cta, ranges;
+    int pitch;              // row pitch of the pooled [N][pitch] rows
+    double hw, rhw;         // float(H W), the divisor, and RN(1 / double(float(H W))) for div_rn
+};
+int gap_shape(const char *fn, int N, int H, int W, int C, int row_pitch, GapArgs *a);
+#ifdef __CUDACC__
+// The IEEE quotient RN(a / b) for b >= 1 given rb = RN(1 / double(b)), with no out-of-line slow path: __fdiv_rn branches to one
+// for extreme exponents, and the call's register convention spills the sums held across it.  In double, a / b of a float a
+// neither overflows nor underflows, so two FMA remainder steps give RN_double(a / b) (Markstein: rb correctly rounded, the
+// second step starts from a faithful quotient); rounding that to float is RN(a / b) (53 >= 2 * 24 + 2 bits: double rounding is
+// innocuous for a quotient).  Zeros, infinities and NaN take a * rb, which keeps the sign of a zero and propagates the rest.
+__device__ __forceinline__ float div_rn(float a, double b, double rb) {
+    const double ad = a;
+    double q = ad * rb;
+    q = fma(fma(-b, q, ad), rb, q);
+    q = fma(fma(-b, q, ad), rb, q);
+    return a == 0.0f || !isfinite(a) ? a * (float)rb : __double2float_rn(q);
+}
+#endif
 // conv_wgrad_tc.cu: dw[o] = sum over i of slots[i][o] for o < nout, in a fixed order (deterministic, no atomics)
 int pcnn_conv_wgrad_reduce_slots(pcnn_ctx *ctx, const float *slots, float *dw, int nslots, int nout);
 // pcnn_abi.cu: at least `bytes` of device scratch, valid until the next call that asks for more (work using it must be

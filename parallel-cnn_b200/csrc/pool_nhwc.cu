@@ -131,19 +131,6 @@ __global__ void __launch_bounds__(POOL_THREADS) k_maxpool_nhwc_bwd(const __nv_bf
     *reinterpret_cast<BfVec<VEC> *>(dx + (((long)n * a.H + h) * a.W + w) * a.C + g * VEC) = out;
 }
 
-// The IEEE quotient RN(a / b) for b >= 1 given rb = RN(1 / double(b)), with no out-of-line slow path: __fdiv_rn branches to one
-// for extreme exponents, and the call's register convention spills the sums held across it.  In double, a / b of a float a
-// neither overflows nor underflows, so two FMA remainder steps give RN_double(a / b) (Markstein: rb correctly rounded, the
-// second step starts from a faithful quotient); rounding that to float is RN(a / b) (53 >= 2 * 24 + 2 bits: double rounding is
-// innocuous for a quotient).  Zeros, infinities and NaN take a * rb, which keeps the sign of a zero and propagates the rest.
-__device__ __forceinline__ float div_rn(float a, double b, double rb) {
-    const double ad = a;
-    double q = ad * rb;
-    q = fma(fma(-b, q, ad), rb, q);
-    q = fma(fma(-b, q, ad), rb, q);
-    return a == 0.0f || !isfinite(a) ? a * (float)rb : __double2float_rn(q);
-}
-
 // RN(1 / k) for the window counts k = 1..49 (constant-folded in IEEE double)
 struct RcpTable {
     double v[POOL_MAX_TAPS * POOL_MAX_TAPS + 1];
@@ -224,16 +211,9 @@ __global__ void __launch_bounds__(POOL_THREADS) k_avgpool_nhwc_bwd(const __nv_bf
 // channel groups [slice * Gc, (slice + 1) * Gc); thread t keeps group t % Gc of the pixels lane, lane + lanes, ... (lane = t / Gc,
 // lanes = 256 / Gc, GAP_ITERS pixels each), summed from the first; the lanes that hold a pixel are then added in lane order
 // through shared memory.  One range per image writes y; more write fp32 slots [n][range][C] that k_gap_finish adds in range order.
-constexpr int GAP_ITERS = 8;                               // pixels per thread
+// GapArgs, GAP_ITERS and gap_shape are in pcnn_internal.h: the squeeze-and-excitation gate gradient sums in the same partition.
 constexpr int GAP_MAX_GROUPS = POOL_THREADS;               // channel groups per CTA: C up to 2048 in one slice on the 16-byte path
-
-struct GapArgs {
-    int HW, C, G;           // pixels per image, channels, channel groups of VEC
-    int Gc, slices;         // groups per CTA, channel slices
-    int lanes, per_cta, ranges;
-    int pitch;              // row pitch of y / dy
-    double hw, rhw;         // float(H W), the divisor, and RN(1 / double(float(H W))) for div_rn
-};
+static_assert(GAP_THREADS == POOL_THREADS, "the partition of gap_shape is that of a POOL_THREADS CTA");
 
 template <int VEC>
 __global__ void __launch_bounds__(POOL_THREADS) k_gap_fwd(const __nv_bfloat16 *__restrict__ x, __nv_bfloat16 *__restrict__ y,
@@ -395,7 +375,9 @@ int include_pad_flag(const char *fn, int count_include_pad) {
     return PCNN_OK;
 }
 
-// the global pool's domain and partition, a function of (N, H, W, C) and the row pitch alone
+}  // namespace
+
+// the global pool's domain and partition, a function of (N, H, W, C) and the row pitch alone (pcnn_internal.h)
 int gap_shape(const char *fn, int N, int H, int W, int C, int row_pitch, GapArgs *a) {
     PCNN_REQUIRE(N >= 1 && H >= 1 && W >= 1 && C >= 1, PCNN_ERR_ARG, "%s: N = %d, H = %d, W = %d, C = %d: each must be >= 1", fn, N, H, W,
                  C);
@@ -420,8 +402,6 @@ int gap_shape(const char *fn, int N, int H, int W, int C, int row_pitch, GapArgs
                  PCNN_ERR_ARG, "%s: %d images of %dx%dx%d exceed the grid", fn, N, H, W, C);
     return PCNN_OK;
 }
-
-}  // namespace
 
 extern "C" int pcnn_maxpool_nhwc_info(int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int row_pitch,
                                       int image_rows, int *out5) {

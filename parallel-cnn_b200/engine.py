@@ -5,7 +5,8 @@ import ctypes as C
 import numpy as np
 
 from ._lib import (F32, NPARAM, OPTIM_ADAMW, OPTIM_SGD, TEST_SET, TRAIN_SET, U8, OptimConfig, OptimTensor, PcnnError, avgpool_nhwc_info,
-                   batchnorm_nhwc_info, check, conv_layer_family, dwconv_info, global_avgpool_nhwc_info, lib, linear_info, maxpool_nhwc_info)
+                   batchnorm_nhwc_info, check, conv_layer_family, dwconv_info, global_avgpool_nhwc_info, lib, linear_info, maxpool_nhwc_info,
+                   se_scale_nhwc_info, ACT_RELU, ACT_SIGMOID)
 
 
 def _pixel_type(arr_or_dtype):
@@ -498,6 +499,24 @@ class Engine:
     def dwconv_dgrad(self, plan, dy, dx):
         """pcnn_dwconv_dgrad: dx dense bf16 [N][H][W][C] from dy with the plan's bf16 filters, every element written"""
         self._call("pcnn_dwconv_dgrad", plan.plan, _p(dy), _p(dx))
+
+    def se_scale_fwd(self, x, s, y, N, H, W, Cin, r=None, act=0):
+        """pcnn_se_scale_nhwc_bf16_fwd: y = bf16(act(x * s[n][c] (+ r))) over dense bf16 [N][H][W][C], s dense bf16 [N][C] (a
+        LinearLayer's y with O = C); act ACT_NONE or ACT_RELU"""
+        self._call("pcnn_se_scale_nhwc_bf16_fwd", _p(x), _p(s), _p(r), _p(y), int(N), int(H), int(W), int(Cin), int(act))
+
+    def se_scale_bwd_gate(self, x, y, dy, g, ds, N, H, W, Cin, dy2=None, act=0):
+        """pcnn_se_scale_nhwc_bf16_bwd_gate: g = bf16(act'(dy (+ dy2))) (may be dy itself; the gradient of the forward's r) and
+        ds[n][c] = bf16 of the sum over the pixels of g * x in GAP's order, the dy of the linear layer that wrote s; y (the forward's
+        output) is read at ACT_RELU only"""
+        self._call("pcnn_se_scale_nhwc_bf16_bwd_gate", _p(x), _p(y), _p(dy), _p(dy2), _p(g), _p(ds), int(N), int(H), int(W), int(Cin),
+                   int(act))
+
+    def se_scale_bwd_input(self, g, s, dx, N, H, W, Cin, dpool=None, dpool_row_pitch=None):
+        """pcnn_se_scale_nhwc_bf16_bwd_input: dx = bf16(g * s[n][c] (+ dpool[n][c] / (H*W))), every element written (dx may be g);
+        dpool [N][dpool_row_pitch] is the squeeze branch's gradient at the pooled x (row pitch None = C rounded up to 8)"""
+        self._call("pcnn_se_scale_nhwc_bf16_bwd_input", _p(g), _p(s), _p(dpool), int(dpool_row_pitch or 0), _p(dx), int(N), int(H), int(W),
+                   int(Cin))
 
 
 class ConvPlan:
@@ -993,6 +1012,83 @@ class GlobalAvgPoolLayer:
         pass
 
 
+class SqueezeExcitationLayer:
+    """Squeeze-and-excitation trained on the device, with BatchNormLayer's interface: y = act(x * s + r) with the gate
+    s = sigmoid(fc2(relu(fc1(GAP(x))))) per image and channel (pcnn_se_scale_nhwc_* for the gating, GlobalAvgPoolLayer and two
+    LinearLayers for the squeeze branch).  x, r, y, dy, dy2, dx and dr are dense bf16 [N][H][W][C]: what a BatchNormLayer writes
+    and reads.  w1 [hidden][C], b1 [hidden], w2 [C][hidden], b2 [C] are the fp32 masters of fc1 (ReLU) and fc2 (sigmoid); the layer
+    owns them with the branch's small bf16 buffers: h (pooled x), a (fc1's y), s (the gate), ds, da and dh.  act ACT_RELU (3) is a
+    ReLU after the add, ACT_NONE (0) none.  In an SE-ResNet basic block the block's last batch norm runs without r and ReLU and the
+    SE layer carries both:
+
+        conv_a.forward(x0, ya); bn_a.forward(ya, za); conv_b.forward(za, yb); bn_b.forward(yb, zb); se.forward(zb, out, r=x0)
+        se.backward(out, dout, dzb, dr=dres); bn_b.backward(zb, dzb, dyb); ...
+
+    Limits: hidden % 8 == 0 (fc2 reads a as rows of hidden), C <= 256 and hidden <= 256 (LinearLayer's O)."""
+
+    def __init__(self, engine, N, H, W, C, hidden, w1, b1, w2, b2, act=0):
+        if hidden % 8 or not 1 <= hidden <= 256 or not 1 <= C <= 256:
+            raise PcnnError("SqueezeExcitationLayer", -1,
+                            f"C = {C}, hidden = {hidden}: 1 <= C <= 256 and 8 <= hidden <= 256 with hidden % 8 == 0 are required (the "
+                            "linear layers' O limit and row-pitch rule)")
+        if int(act) not in (0, ACT_RELU):
+            raise PcnnError("SqueezeExcitationLayer", -1, f"act {act}: 0 (none) or 3 (ReLU) is required")
+        self.engine = engine
+        self.shape = (N, H, W, C)
+        self.hidden, self.act = int(hidden), int(act)
+        self.info = se_scale_nhwc_info(N, H, W, C)
+        self.gap = GlobalAvgPoolLayer(engine, N, H, W, C)
+        self.row_pitch = self.gap.row_pitch
+        self.fc1 = LinearLayer(engine, N, 1, 1, C, hidden, np.asarray(w1, np.float32).reshape(hidden, 1, 1, C), b1, act=ACT_RELU,
+                               row_pitch=self.row_pitch)
+        self.fc2 = LinearLayer(engine, N, 1, 1, hidden, C, np.asarray(w2, np.float32).reshape(C, 1, 1, hidden), b2, act=ACT_SIGMOID)
+        bf = lambda *shape: engine.array(shape, np.uint16)
+        self.h, self.dh = bf(N, self.row_pitch), bf(N, self.row_pitch)
+        self.a, self.da = bf(N, hidden), bf(N, hidden)
+        self.s, self.ds = bf(N, C), bf(N, C)
+        self._x = None
+
+    def forward(self, x, y, r=None):
+        """y = act(x * s + r), s the gate of this x.  The layer keeps x: backward reads it."""
+        N, H, W, C = self.shape
+        self.gap.forward(x, self.h)
+        self.fc1.forward(self.h, self.a)
+        self.fc2.forward(self.a, self.s)
+        self.engine.se_scale_fwd(x, self.s, y, N, H, W, C, r=r, act=self.act)
+        self._x = x
+
+    def backward(self, y, dy, dx, dr=None, dy2=None):
+        """Gradients of the most recent forward, whose output y was: fc1's and fc2's dw and db, and dx, the gradient through both the
+        scale and the squeeze branch.  dy2 is a second gradient added to dy before the activation; dr receives the gradient of the
+        forward's r.  Without dr, dy is CONSUMED: it is overwritten in place by that gradient, as LinearLayer does.  dx may be dy."""
+        N, H, W, C = self.shape
+        e = self.engine
+        g = dy if dr is None else dr
+        e.se_scale_bwd_gate(self._x, y, dy, g, self.ds, N, H, W, C, dy2=dy2, act=self.act)
+        self.fc2.backward(self.s, self.ds, self.da)
+        self.fc1.backward(self.a, self.da, self.dh)
+        e.se_scale_bwd_input(g, self.s, dx, N, H, W, C, dpool=self.dh, dpool_row_pitch=self.row_pitch)
+
+    def sgd(self, lr):
+        """plain SGD on both linear layers' masters, their plans refreshed (LinearLayer.sgd)"""
+        self.fc1.sgd(lr)
+        self.fc2.sgd(lr)
+
+    def optim_tensors(self):
+        """(param, grad, plan, plan part, is norm or bias) of w1, b1, w2 and b2, as ConvLayer.optim_tensors"""
+        return self.fc1.optim_tensors() + self.fc2.optim_tensors()
+
+    def params(self):
+        """host copies of the fp32 masters w1 [hidden][1][1][C], b1, w2 [C][1][1][hidden], b2"""
+        return self.fc1.params() + self.fc2.params()
+
+    def close(self):
+        for layer in (self.fc1, self.fc2, self.gap):
+            layer.close()
+        for a in (self.h, self.dh, self.a, self.da, self.s, self.ds):
+            a.free()
+
+
 class FusedOptimizer:
     """One fused update of many fp32 parameter tensors per step (pcnn_optim_*; the rules and their order are in include/pcnn.h).
     tensors: (param, grad, n, weight_decay, plan, plan part) with plan None (part 0) or the ConvPlan / LinearPlan / DepthwiseConvPlan
@@ -1068,7 +1164,8 @@ def _layer_tensors(layers, weight_decay, decay_norm_and_bias):
 
 
 class SGD(FusedOptimizer):
-    """torch.optim.SGD over the trainable tensors of ConvLayers, DepthwiseConvLayers, LinearLayers and BatchNormLayers, in one launch
+    """torch.optim.SGD over the trainable tensors of ConvLayers, DepthwiseConvLayers, LinearLayers, BatchNormLayers and
+    SqueezeExcitationLayers, in one launch
     per step with the layers' plans refreshed: step(lr) replaces every layer.sgd(lr) of a training step (momentum 0 and weight decay 0 give the same
     bits).  decay_norm_and_bias=False gives batch normalization's gamma and beta and the biases weight decay 0; the default decays
     every tensor, as torch.optim does with one parameter group."""

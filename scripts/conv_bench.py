@@ -929,6 +929,111 @@ def run_mbblock(N, iters, k=3):
         layer.close()
 
 
+def run_se(name, N, H, W, C, iters):
+    """the three squeeze-and-excitation passes (pcnn_se_scale_nhwc_bf16_fwd / _bwd_gate / _bwd_input) next to torch eager on the
+    same bf16 channels-last tensors.  Bytes per pass, each [N][H][W][C] tensor crossing HBM once: forward x and y (plus r), gate
+    x, dy, y read and g written plus its fp32 slots (written and read once) and ds, input gradient g and dx."""
+    info = pkg.se_scale_nhwc_info(N, H, W, C)
+    bits = lambda *shape: torch.randint(0, 0x3F80, shape, dtype=torch.int16, device="cuda") ^ (torch.randint(0, 2, shape, dtype=torch.int16, device="cuda") << 15)
+    x, r, dy, y = (bits(N, H, W, C) for _ in range(4))
+    g, dx = torch.empty_like(x), torch.empty_like(x)
+    s = torch.rand((N, C), device="cuda").to(torch.bfloat16).view(torch.int16)
+    pitch = (C + 7) // 8 * 8
+    dpool, ds = bits(N, pitch), torch.empty((N, C), dtype=torch.int16, device="cuda")
+    eng.se_scale_fwd(x, s, y, N, H, W, C, r=r, act=pkg.ACT_RELU)
+    gpu, power = card()
+    t = N * H * W * C * 2
+    slot_bytes = 2 * N * info["ranges"] * C * 4 if info["ranges"] > 1 else 0
+    cl = lambda a: a.view(torch.bfloat16).permute(0, 3, 1, 2)
+    xt, rt, dyt, yt = cl(x), cl(r), cl(dy), cl(y)
+    st, dpt = s.view(torch.bfloat16)[:, :, None, None], dpool.view(torch.bfloat16)[:, :C, None, None]
+    passes = (
+        ("fwd", lambda: eng.se_scale_fwd(x, s, y, N, H, W, C), lambda: xt * st, 2 * t),
+        ("fwd + r + ReLU", lambda: eng.se_scale_fwd(x, s, y, N, H, W, C, r=r, act=pkg.ACT_RELU), lambda: torch.relu(xt * st + rt), 3 * t),
+        ("gate (ReLU)", lambda: eng.se_scale_bwd_gate(x, y, dy, g, ds, N, H, W, C, act=pkg.ACT_RELU),
+         lambda: (lambda gt: (gt, (gt * xt).sum((2, 3))))(torch.where(yt > 0, dyt, 0)), 4 * t + slot_bytes + N * C * 2),
+        ("input + dpool", lambda: eng.se_scale_bwd_input(dy, s, dx, N, H, W, C, dpool=dpool, dpool_row_pitch=pitch),
+         lambda: dyt * st + dpt / (H * W), 2 * t),
+    )
+    for what, ours, theirs, nbytes in passes:
+        ms, ms_torch = timed(ours, iters), timed(theirs, iters)
+        print(json.dumps({"case": f"se {name} {what}", "N": N, "us": ms * 1e3, "MB": nbytes / 1e6, "share_of_3350": nbytes / (ms * 1e-3) / 1e9 / HBM,
+                          "torch_us": ms_torch * 1e3, "torch_over_ours": ms_torch / ms, "vec": info["vec"], "gate_ranges": info["ranges"],
+                          "gate_ctas": info["ctas"], "gpu": gpu, "power_limit": power}), flush=True)
+
+
+def run_seblock(N, iters, hid=8):
+    """one training step of an SE basic block, 56x56x64 at N = 128: conv_a 3x3 pad 1 -> BN + ReLU -> conv_b -> BN -> SE (64 -> hid ->
+    64, hid 8: the smallest width the linear row pitch allows, where SE-ResNet's reduction 16 would give 4) carrying + x0 and the
+    ReLU, its backward (dx0 and the shortcut's gradient dres left apart, as run_resblock) and the sgd of the five layers, on the
+    engine's stream.  Next to it the torch eager step of the same block on bf16 channels-last tensors (fp32 masters, w -= lr * grad,
+    re-cast to bf16)."""
+    H = W = 56
+    C = 64
+    r = np.random.default_rng(13)
+    u = lambda shape, fan: r.uniform(-1, 1, shape).astype(np.float32) / np.float32(np.sqrt(fan))
+    fa, fb = u((C, 3, 3, C), 9 * C), u((C, 3, 3, C), 9 * C)
+    w1, b1, w2, b2 = u((hid, C), C), u(hid, C), u((C, hid), hid), u(C, hid)
+    ca = pkg.ConvLayer(eng, N, H, W, C, C, 3, 3, fa, None, act=0, padding=(1, 1))
+    cb = pkg.ConvLayer(eng, N, H, W, C, C, 3, 3, fb, None, act=0, padding=(1, 1))
+    ba, bb = pkg.BatchNormLayer(eng, N, H, W, C, act=pkg.ACT_RELU), pkg.BatchNormLayer(eng, N, H, W, C, act=0)
+    se = pkg.SqueezeExcitationLayer(eng, N, H, W, C, hid, w1, b1, w2, b2, act=pkg.ACT_RELU)
+    e = lambda: torch.empty((N, H, W, C), dtype=torch.int16, device="cuda")
+    x0 = torch.randint(0, 0x3F80, (N, H, W, C), dtype=torch.int16, device="cuda")
+    dout = torch.randint(0, 0x3F80, (N, H, W, C), dtype=torch.int16, device="cuda")
+    dout ^= torch.randint(0, 2, (N, H, W, C), dtype=torch.int16, device="cuda") << 15
+    ya, za, yb, zb, out, dzb, dyb, dres, dza, dya, dx0 = (e() for _ in range(11))
+    lr = 0.05
+    gpu, power = card()
+
+    def step():
+        ca.forward(x0, ya); ba.forward(ya, za); cb.forward(za, yb); bb.forward(yb, zb); se.forward(zb, out, r=x0)
+        se.backward(out, dout, dzb, dr=dres); bb.backward(zb, dzb, dyb); cb.backward(yb, dyb, dza); ba.backward(za, dza, dya)
+        ca.backward(ya, dya, dx0)
+        for layer in (ca, ba, cb, bb, se):
+            layer.sgd(lr)
+
+    ms = timed(step, iters)
+    ms_se = {"fwd": timed(lambda: se.forward(zb, out, r=x0), iters), "bwd": timed(lambda: se.backward(out, dout, dzb, dr=dres), iters)}
+    F = torch.nn.functional
+    xt = x0.view(torch.bfloat16).permute(0, 3, 1, 2).detach().requires_grad_(True)
+    dt = dout.view(torch.bfloat16).permute(0, 3, 1, 2)
+    m32 = {k: torch.from_numpy(v).to("cuda").permute(0, 3, 1, 2).contiguous(memory_format=torch.channels_last) for k, v in
+           (("fa", fa), ("fb", fb))}
+    m32.update(ga=torch.ones(C, device="cuda"), ba=torch.zeros(C, device="cuda"), gb=torch.ones(C, device="cuda"), bb=torch.zeros(C, device="cuda"))
+    m32.update({k: torch.from_numpy(v).to("cuda") for k, v in (("w1", w1), ("b1", b1), ("w2", w2), ("b2", b2))})
+    mb = {k: (v.to(torch.bfloat16) if k[0] in "fwb" and k not in ("ba", "bb") else v.clone()).requires_grad_(True) for k, v in m32.items()}
+    stats = [torch.zeros(C, device="cuda"), torch.ones(C, device="cuda"), torch.zeros(C, device="cuda"), torch.ones(C, device="cuda")]
+
+    def torch_step():
+        for v in mb.values():
+            v.grad = None
+        xt.grad = None
+        h = torch.relu(F.batch_norm(F.conv2d(xt, mb["fa"], padding=1), stats[0], stats[1], mb["ga"], mb["ba"], training=True))
+        h = F.batch_norm(F.conv2d(h, mb["fb"], padding=1), stats[2], stats[3], mb["gb"], mb["bb"], training=True)
+        s = torch.sigmoid(F.linear(torch.relu(F.linear(h.mean((2, 3)), mb["w1"], mb["b1"])), mb["w2"], mb["b2"]))
+        h = torch.relu(h * s[:, :, None, None] + xt)
+        h.backward(dt)
+        with torch.no_grad():
+            for k in m32:
+                m32[k].add_(mb[k].grad.float(), alpha=-lr)
+                mb[k].copy_(m32[k])
+
+    ms_torch = timed(torch_step, iters)
+    print(json.dumps({"case": f"SE basic block 56x56x64 (SE 64 -> {hid} -> 64) training step N={N}", "ms": ms, "torch_eager_ms": ms_torch,
+                      "ours_over_torch": ms / ms_torch, "se_fwd_ms": ms_se["fwd"], "se_bwd_ms": ms_se["bwd"], "gpu": gpu,
+                      "power_limit": power}), flush=True)
+    for layer in (ca, cb, ba, bb, se):
+        layer.close()
+
+
+if only == "se":                                                       # squeeze-and-excitation passes, torch beside them
+    for args in (("56x56x256", 128, 56, 56, 256), ("28x28x512", 128, 28, 28, 512), ("14x14x1024", 128, 14, 14, 1024),
+                 ("7x7x2048", 128, 7, 7, 2048), ("112x112x32", 128, 112, 112, 32), ("56x56x144", 128, 56, 56, 144),
+                 ("28x28x240", 128, 28, 28, 240), ("7x7x1152", 128, 7, 7, 1152)):
+        run_se(*args, 20)
+if only == "seblock":                                                  # one step of an SE basic block, torch eager beside it
+    run_seblock(128, 20)
 if only == "dwconv":                                                   # depthwise convolution passes, torch beside them
     for args in (("112x112x32 3x3/1", 128, 112, 112, 32, 3, 1, 1), ("112x112x96 3x3/2", 128, 112, 112, 96, 3, 2, 1),
                  ("56x56x144 3x3/1", 128, 56, 56, 144, 3, 1, 1), ("56x56x144 3x3/2", 128, 56, 56, 144, 3, 2, 1),
