@@ -287,6 +287,11 @@ int pcnn_l5_forward(pcnn_ctx *ctx, const float *params_dev, const void *images_d
 #define PCNN_ACT_NONE 0
 #define PCNN_ACT_SIGMOID 1
 #define PCNN_ACT_RELU 3
+/* Codes 4-6 are taken by pcnn_batchnorm_nhwc_bf16_fwd and pcnn_batchnorm_nhwc_bf16_bwd_preact only (every call above and below
+ * keeps its domain and refuses them); batch normalization below states their formulas. */
+#define PCNN_ACT_SILU 4
+#define PCNN_ACT_HARDSWISH 5
+#define PCNN_ACT_RELU6 6
 typedef struct pcnn_conv_plan pcnn_conv_plan;
 int pcnn_conv_tc_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int row_pitch,
                              int image_rows /* rows between consecutive images in memory, >= H; 0 = H */,
@@ -510,7 +515,7 @@ int pcnn_global_avgpool_nhwc_bf16_bwd(pcnn_ctx *ctx, const void *dy_bf16_dev, vo
                                       int dy_row_pitch);
 int pcnn_global_avgpool_nhwc_info(int N, int H, int W, int C, int row_pitch, int *out8);
 /* Batch normalization between convolution layers (csrc/batchnorm_nhwc.cu), as torch.nn.functional.batch_norm with affine
- * parameters, followed by an optional residual add and ReLU.  x, r, y, dy, dy2, dx and dr are dense bf16 [pixels][C] (pixels =
+ * parameters, followed by an optional residual add and ReLU, SiLU, hard-swish or ReLU6.  x, r, y, dy, dy2, dx and dr are dense bf16 [pixels][C] (pixels =
  * N H W: the layout both conv forwards write as y and the gradients read as dy); gamma, beta, the running and the saved
  * statistics, dgamma and dbeta are fp32 [C].  M = pixels.  Every fp32 operation below rounds to nearest with no contraction.
  * Forward, training = 1:
@@ -525,7 +530,26 @@ int pcnn_global_avgpool_nhwc_info(int N, int H, int W, int C, int row_pitch, int
  * but y is written (save_mean, save_rstd and momentum are not used).
  * Then per element, with mean and rstd those of the channel:
  *   xhat = (float(x) - mean) * rstd;  v = xhat * gamma + beta;  v = v + float(r) when r is given;
- *   y = bf16_rn(act(v)), act 0 none or 3 the ReLU of the conv epilogues (v < 0 ? +0 : v, NaN and -0 unchanged).
+ *   y = bf16_rn(act(v)), act 0 none or 3 the ReLU of the conv epilogues (v < 0 ? +0 : v, NaN and -0 unchanged), or one of
+ *   the activations of EfficientNet, MobileNetV3 and MobileNetV2 (RN = fp32 round to nearest, "/" the IEEE quotient):
+ *     4 SiLU:       RN(v / RN(1 + E(-v)))                                     (torch: x / (1 + exp(-x)))
+ *     5 hard-swish: RN(RN(v * u) / 6), u = min(max(RN(v + 3), 0), 6)          (torch: x * min(max(x + 3, 0), 6) / 6)
+ *     6 ReLU6:      min(max(v, 0), 6) as v < 0 ? +0 : (v > 6 ? 6 : v)          (torch: hardtanh(x, 0, 6))
+ *   with NaN passing every min / max (NaN in, NaN out) and -0 kept by ReLU6, as torch.  Where fp32 departs from torch's
+ *   float64: SiLU gives -0 for v < -88.7228317 (E(-v) = +Inf; the exact value is below 2^-119 in magnitude) and NaN at v = -Inf
+ *   (as torch); hard-swish gives +Inf for v > FLT_MAX / 6 (RN(v * 6) overflows) and NaN at v = -Inf (as torch).
+ *   E(x) is the library's exponential, a fixed sequence of fp32 operations a numpy float32 replay reproduces bit for bit
+ *   (expf and __expf cannot be replayed):
+ *     x > 88.7228317 (0x42B17217) -> +Inf;  x < -103.972076 (0xC2CFF1B4) -> +0;  NaN -> NaN;  otherwise
+ *     k = rint(RN(x * log2e)), log2e = 0x3FB8AA3B;
+ *     r = RN(RN(x - RN(k * ln2_hi)) - RN(k * ln2_lo)), ln2_hi = 0x3F317200 (15 significant bits: k * ln2_hi and x - k * ln2_hi
+ *       are exact), ln2_lo = 0x35BFBE8E;
+ *     p = c6, then p = RN(RN(p * r) + c_i) for i = 5 .. 0 (Horner), c0 = c1 = 1, c2 = 0x3EFFFFFE, c3 = 0x3E2AAA0C,
+ *       c4 = 0x3D2AAC12, c5 = 0x3C0933ED, c6 = 0x3AB5736C (a minimax fit on |r| <= ln2 / 2);
+ *     E = RN(RN(p * 2^k1) * 2^k2), k1 = floor(k / 2), k2 = k - k1: the first product is exact, so a subnormal result is rounded
+ *       once and a result near FLT_MAX overflows only when it should.
+ *   Its error over the finite inputs is at most 1.30 ulp of exp(x) (measured 1.2965 at every 97th bit pattern, the thresholds
+ *   and the subnormal results; 99.5 % correctly rounded).
  * Act 1 is refused: the sigmoid of the conv epilogues uses tanh.approx, which no reference can replay bit for bit.
  * Backward (of a training forward; save_mean and save_rstd are what it wrote, y its output):
  *   t = float(dy), or float(dy) + float(dy2) when dy2 (a second gradient arriving at a residual join) is given;
@@ -535,10 +559,21 @@ int pcnn_global_avgpool_nhwc_info(int N, int H, int W, int C, int row_pitch, int
  *   dx = bf16_rn(((float(g) - dbeta / Mf) - xhat * (dgamma / Mf)) * (gamma * rstd)), Mf = float(M), the two quotients and
  *     gamma * rstd formed once per channel from the dgamma and dbeta just written;
  *   dr = g when dr is given: the gradient of the residual input r.
+ * Backward at codes 4-6 (pcnn_batchnorm_nhwc_bf16_bwd_preact; pcnn_batchnorm_nhwc_bf16_bwd refuses them, and this entry refuses
+ * 0 and 3, so each code has one backward): y cannot give the derivative (SiLU and hard-swish are not monotonic, and bf16 rounds
+ * every v in (5.984, 6) to a ReLU6 y of 6), so each pass recomputes v from x, save_mean, save_rstd, gamma, beta and r exactly as
+ * the forward formed it (r must be the forward's r, unchanged, or NULL if it had none), and with t as above
+ *     4 SiLU:       s = RN(1 / RN(1 + E(-v))), d = RN(s * RN(1 + RN(v * RN(1 - s)))), g = bf16_rn(RN(t * d))
+ *                   (torch's silu_backward multiplies t * s first; the float64 results agree)
+ *     5 hard-swish: v <= -3 -> +0;  v >= 3 -> t passes;  otherwise g = bf16_rn(RN(t * RN(RN(v / 3) + 0.5)))  (hardswish_backward;
+ *                   NaN gives NaN, as torch's vectorised loop; its scalar tail passes t)
+ *     6 ReLU6:      0 < v < 6 -> t passes;  otherwise +0, NaN included  (hardtanh_backward)
+ *   where a passed t is bf16_rn(t) (dy's bits without dy2).  dbeta, dgamma, dx and dr then follow the rules above with this g.
  * dx == dy (in place) is allowed; no other two buffers may overlap.  Domain (anything else is PCNN_ERR_ARG with the function and
  * the rule in the message; the shape rules read the same in pcnn_batchnorm_nhwc_info):
  *   - 1 <= C <= 256; training 0 or 1; M >= 2 when training and for the backward, M >= 1 in eval;
- *   - eps finite and >= 0; 0 <= momentum <= 1; act 0 or 3;
+ *   - eps finite and >= 0; 0 <= momentum <= 1; act 0, 3, 4, 5 or 6 in the forward, 0 or 3 in pcnn_batchnorm_nhwc_bf16_bwd, 4, 5
+ *     or 6 in pcnn_batchnorm_nhwc_bf16_bwd_preact (which also needs beta; r, dy2 and dr may be NULL);
  *   - every pointer 16-byte aligned; x, y, gamma, beta not NULL; save_mean and save_rstd not NULL when training; running_mean
  *     and running_var not NULL in eval; x, y, dy, gamma, the saved statistics, dx, dgamma and dbeta not NULL in the backward.
  * With C % 8 == 0 the passes move 16-byte vectors of 8 channels, otherwise single elements.  No atomics: reruns and every H100
@@ -552,6 +587,10 @@ int pcnn_batchnorm_nhwc_bf16_fwd(pcnn_ctx *ctx, const void *x_bf16_dev, const vo
 int pcnn_batchnorm_nhwc_bf16_bwd(pcnn_ctx *ctx, const void *x_bf16_dev, const void *y_bf16_dev, const void *dy_bf16_dev,
                                  const void *dy2_bf16_dev, const float *gamma_dev, const float *save_mean_dev, const float *save_rstd_dev,
                                  void *dx_bf16_dev, void *dr_bf16_dev, float *dgamma_dev, float *dbeta_dev, long pixels, int C, int act);
+int pcnn_batchnorm_nhwc_bf16_bwd_preact(pcnn_ctx *ctx, const void *x_bf16_dev, const void *r_bf16_dev, const void *dy_bf16_dev,
+                                        const void *dy2_bf16_dev, const float *gamma_dev, const float *beta_dev, const float *save_mean_dev,
+                                        const float *save_rstd_dev, void *dx_bf16_dev, void *dr_bf16_dev, float *dgamma_dev,
+                                        float *dbeta_dev, long pixels, int C, int act);
 int pcnn_batchnorm_nhwc_info(long pixels, int C, int training, int *out5);
 /* Fully connected layers (csrc/linear_tc.cu), bf16 on the tensor cores with fp32 accumulation:
  *   - x is [N][image_rows][row_pitch] bf16 with P x Q pixels of C channels per image: the layout a plan reads as x and the NHWC

@@ -10,6 +10,7 @@ it as the module ``parallel_cnn_b200``).
 """
 from ._lib import (  # noqa: F401
     LIB_PATH, NPARAM, OFF, PcnnError, U8, F32, TRAIN_SET, TEST_SET, MODE_AUTO, MODE_GRAPH, MODE_PERSISTENT, ACT_NONE, ACT_SIGMOID, ACT_RELU,
+    ACT_SILU, ACT_HARDSWISH, ACT_RELU6,
     lib, declared_symbols, init_params_reference, mnist_load_u8, conv_tc_plan_info, conv_wide_plan_info, conv_wide_bwd_info,
     conv_bwd_plan_info, conv_layer_family, maxpool_nhwc_info, avgpool_nhwc_info, global_avgpool_nhwc_info, batchnorm_nhwc_info,
     linear_info, dwconv_info, se_scale_nhwc_info, OPTIM_SGD, OPTIM_ADAMW,
@@ -21,5 +22,6 @@ from .engine import SGD, AdamW, FusedOptimizer  # noqa: F401
 __all__ = ["Engine", "DeviceArray", "PcnnError", "lib", "declared_symbols", "init_params_reference",
            "mnist_load_u8", "conv_tc_plan_info", "conv_wide_plan_info", "conv_wide_bwd_info", "conv_bwd_plan_info", "conv_layer_family", "maxpool_nhwc_info", "avgpool_nhwc_info", "global_avgpool_nhwc_info", "batchnorm_nhwc_info", "linear_info", "ConvLayer", "BatchNormLayer", "MaxPoolLayer", "AvgPoolLayer", "GlobalAvgPoolLayer", "LinearLayer", "ConvPlan", "LinearPlan",
            "WideConvPlan", "NPARAM", "OFF", "U8", "F32", "TRAIN_SET", "TEST_SET", "LIB_PATH", "ACT_NONE", "ACT_SIGMOID", "ACT_RELU",
+           "ACT_SILU", "ACT_HARDSWISH", "ACT_RELU6",
            "SGD", "AdamW", "FusedOptimizer", "OPTIM_SGD", "OPTIM_ADAMW", "dwconv_info", "DepthwiseConvLayer", "DepthwiseConvPlan",
            "se_scale_nhwc_info", "SqueezeExcitationLayer"]

@@ -16,6 +16,7 @@ U8, F32 = 0, 1
 MODE_AUTO, MODE_GRAPH, MODE_PERSISTENT = 0, 1, 2
 TRAIN_SET, TEST_SET = 0, 1
 ACT_NONE, ACT_SIGMOID, ACT_RELU = 0, 1, 3     # PCNN_ACT_*: the `act` of the device-trained layers (2 is not a code)
+ACT_SILU, ACT_HARDSWISH, ACT_RELU6 = 4, 5, 6  # taken by batch normalization only (BatchNormLayer, Engine.batchnorm_fwd / _bwd_preact)
 OPTIM_SGD, OPTIM_ADAMW = 0, 1                 # PCNN_OPTIM_*: the `kind` of pcnn_optim_config
 
 
@@ -152,6 +153,7 @@ _SIG = {
     "pcnn_global_avgpool_nhwc_info": [_i, _i, _i, _i, _i, _vp],
     "pcnn_batchnorm_nhwc_bf16_fwd": [_vp, _vp, _vp, _vp, _l, _i, _i, _i, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp],
     "pcnn_batchnorm_nhwc_bf16_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _l, _i, _i],
+    "pcnn_batchnorm_nhwc_bf16_bwd_preact": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _l, _i, _i],
     "pcnn_batchnorm_nhwc_info": [_l, _i, _i, _vp],
     "pcnn_conv_bwd_plan_info": [_i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_pad_nhwc_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i],

@@ -1,8 +1,10 @@
 // parallel-cnn_b200/csrc/batchnorm_nhwc.cu -- batch normalization of the dense bf16 NHWC [pixels][C] activations the conv
 // forwards write (pcnn_batchnorm_nhwc_bf16_fwd / _bwd), with the residual add and the ReLU of a ResNet block fused into the
-// elementwise pass.  The contract, every operation in its order, is in include/pcnn.h.
+// elementwise pass, or SiLU, hard-swish or ReLU6, whose backward (pcnn_batchnorm_nhwc_bf16_bwd_preact) takes the derivative at the
+// pre-activation recomputed from x, beta and r instead of from y.  The contract, every operation in its order, is in include/pcnn.h.
 //
-// Every pass is HBM-bound.  With C % 8 == 0 a thread moves 16-byte vectors of 8 channels of one pixel, otherwise single
+// The passes at codes 0, 3 and 6 are HBM-bound; those at 4 (SiLU) and 5 (hard-swish) are bound by instruction issue (the
+// exponential and the quotients per element).  With C % 8 == 0 a thread moves 16-byte vectors of 8 channels of one pixel, otherwise single
 // elements.  All passes share one partition: CTA b owns the pixels [b * BN_ITERS * lanes, (b + 1) * BN_ITERS * lanes), thread
 // t keeps channel group g = t % G (G = C / VEC groups, lanes = 256 / G) of the pixels lane, lane + lanes, ... (lane = t / G), so
 // consecutive threads touch consecutive bytes.  A thread loads bn_unroll pixels before it uses any (in place, dx == dy, each
@@ -57,6 +59,53 @@ __device__ __forceinline__ __nv_bfloat16 bn_dgrad(__nv_bfloat16 dy, __nv_bfloat1
     __nv_bfloat16 g = has_dy2 ? __float2bfloat16_rn(__fadd_rn(__bfloat162float(dy), __bfloat162float(dy2))) : dy;
     if (ACT == PCNN_ACT_RELU && __bfloat162float(y) <= 0.0f) g = __ushort_as_bfloat16((unsigned short)0);
     return g;
+}
+
+// codes 4-6 take their backward from the recomputed fp32 pre-activation v rather than from y
+template <int ACT>
+__host__ __device__ constexpr bool bn_preact() { return ACT == PCNN_ACT_SILU || ACT == PCNN_ACT_HARDSWISH || ACT == PCNN_ACT_RELU6; }
+
+// the pre-activation v = RN(RN(xhat * gamma) + beta) (+ float(r)), as the forward forms it
+__device__ __forceinline__ float bn_pre(float xh, float ga, float be, const __nv_bfloat16 *r, __nv_bfloat16 rv) {
+    const float v = __fadd_rn(__fmul_rn(xh, ga), be);
+    return r ? __fadd_rn(v, __bfloat162float(rv)) : v;
+}
+
+// act(v) in fp32 before the one bf16 rounding (pcnn.h states each in its order).  Every "/" is __fdiv_rn, the IEEE quotient: ptxas
+// shows a 0-byte stack and no spills in every instantiation with it, and a divisor of +Inf gives +-0 for a finite dividend.
+template <int ACT>
+__device__ __forceinline__ float bn_act_f32(float v) {
+    if (ACT == PCNN_ACT_RELU) return pcnn_tc::relu_f32(v);
+    if (ACT == PCNN_ACT_SILU) return __fdiv_rn(v, __fadd_rn(1.0f, exp_f32(-v)));
+    if (ACT == PCNN_ACT_HARDSWISH) {
+        float u = __fadd_rn(v, 3.0f);
+        u = u < 0.0f ? 0.0f : u;
+        u = u > 6.0f ? 6.0f : u;                                        // NaN passes both
+        return __fdiv_rn(__fmul_rn(v, u), 6.0f);
+    }
+    if (ACT == PCNN_ACT_RELU6) {
+        const float u = v < 0.0f ? 0.0f : v;                            // NaN and -0 pass
+        return u > 6.0f ? 6.0f : u;
+    }
+    return v;
+}
+
+// g = bf16_rn(act'(t)) at the pre-activation v, t = float(dy) or RN(float(dy) + float(dy2)): a multiplied derivative gives
+// bf16_rn(RN(t * d)); a passed t gives bf16_rn(t) (dy's bits without dy2); a cut one +0
+template <int ACT>
+__device__ __forceinline__ __nv_bfloat16 bn_dgrad_pre(__nv_bfloat16 dy, __nv_bfloat16 dy2, bool has_dy2, float v) {
+    const float t = has_dy2 ? __fadd_rn(__bfloat162float(dy), __bfloat162float(dy2)) : __bfloat162float(dy);
+    const __nv_bfloat16 pass = has_dy2 ? __float2bfloat16_rn(t) : dy, zero = __ushort_as_bfloat16((unsigned short)0);
+    if (ACT == PCNN_ACT_RELU6) return v > 0.0f && v < 6.0f ? pass : zero;                       // NaN gives +0
+    if (ACT == PCNN_ACT_HARDSWISH) {
+        if (v <= -3.0f) return zero;
+        if (v >= 3.0f) return pass;
+        return __float2bfloat16_rn(__fmul_rn(t, __fadd_rn(__fdiv_rn(v, 3.0f), 0.5f)));  // NaN gives NaN
+    }
+    // SiLU: s = RN(1 / RN(1 + E(-v))), d = RN(s * RN(1 + RN(v * RN(1 - s))))
+    const float s = __fdiv_rn(1.0f, __fadd_rn(1.0f, exp_f32(-v)));
+    const float d = __fmul_rn(s, __fadd_rn(1.0f, __fmul_rn(v, __fsub_rn(1.0f, s))));
+    return __float2bfloat16_rn(__fmul_rn(t, d));
 }
 
 // per-CTA sums of the lanes of two [lanes][C] planes in lane order -> slots[plane][cta][C]
@@ -209,35 +258,50 @@ __global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) k_bn_apply(const __nv
             for (int i = 0; i < VEC; ++i) {
                 float v = __fadd_rn(__fmul_rn(bn_xhat(xv[u].h[i], mu[i], rs[i]), ga[i]), be[i]);
                 if (r) v = __fadd_rn(v, __bfloat162float(rv[u].h[i]));
-                if (ACT == PCNN_ACT_RELU) v = pcnn_tc::relu_f32(v);
-                out.h[i] = __float2bfloat16_rn(v);
+                out.h[i] = __float2bfloat16_rn(bn_act_f32<ACT>(v));
             }
             st<VEC>(y + px * C + g * VEC, out);
         }
     }
 }
 
-// first backward pass: per-CTA slots [0][cta][C] = sum g~, [1][cta][C] = sum g~ * xhat
+// first backward pass: per-CTA slots [0][cta][C] = sum g~, [1][cta][C] = sum g~ * xhat.  At codes 4-6 g~ comes from the
+// pre-activation recomputed from x, beta and r (y is not read); their per-channel constants live in shared memory.
 template <int VEC, int ACT>
 __global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) k_bn_bwd_reduce(const __nv_bfloat16 *__restrict__ x, const __nv_bfloat16 *__restrict__ y,
-                                                              const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ dy2,
-                                                              const float *__restrict__ mean, const float *__restrict__ rstd,
-                                                              float *__restrict__ slots, long pixels, int C, long ctas) {
+                                                              const __nv_bfloat16 *__restrict__ r, const __nv_bfloat16 *__restrict__ dy,
+                                                              const __nv_bfloat16 *__restrict__ dy2, const float *__restrict__ mean,
+                                                              const float *__restrict__ rstd, const float *__restrict__ gamma,
+                                                              const float *__restrict__ beta, float *__restrict__ slots, long pixels, int C,
+                                                              long ctas) {
+    constexpr bool PRE = bn_preact<ACT>();
     __shared__ float part[2 * BN_THREADS * 8];
+    __shared__ float cmu[PRE ? BN_MAX_C : 1], crs[PRE ? BN_MAX_C : 1], cga[PRE ? BN_MAX_C : 1], cbe[PRE ? BN_MAX_C : 1];
     constexpr int U = bn_unroll<VEC>();
     const int G = C / VEC, lanes = BN_THREADS / G;
     const int lane = threadIdx.x / G, g = threadIdx.x % G;
+    if (PRE) {
+        for (int c = threadIdx.x; c < C; c += BN_THREADS) {
+            cmu[c] = mean[c];
+            crs[c] = rstd[c];
+            cga[c] = gamma[c];
+            cbe[c] = beta[c];
+        }
+        __syncthreads();
+    }
     if (lane < lanes) {
-        float mu[VEC], rs[VEC], sb[VEC], sg[VEC];
+        float mu[PRE ? 1 : VEC], rs[PRE ? 1 : VEC], sb[VEC], sg[VEC];
 #pragma unroll
         for (int i = 0; i < VEC; ++i) {
-            mu[i] = mean[g * VEC + i];
-            rs[i] = rstd[g * VEC + i];
+            if (!PRE) {
+                mu[i] = mean[g * VEC + i];
+                rs[i] = rstd[g * VEC + i];
+            }
             sb[i] = sg[i] = 0.0f;
         }
         const long p0 = (long)blockIdx.x * BN_ITERS * lanes + lane;
         for (int j0 = 0; j0 < BN_ITERS; j0 += U) {
-            BfVec<VEC> xv[U], yv[U], dv[U], d2[U];
+            BfVec<VEC> xv[U], yv[U], dv[U], d2[U], rv[U];
 #pragma unroll
             for (int u = 0; u < U; ++u) {
                 const long px = p0 + (long)(j0 + u) * lanes;
@@ -246,6 +310,7 @@ __global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) k_bn_bwd_reduce(const
                     xv[u] = ld<VEC>(x + off);
                     dv[u] = ld<VEC>(dy + off);
                     if (ACT == PCNN_ACT_RELU) yv[u] = ld<VEC>(y + off);
+                    if (PRE && r) rv[u] = ld<VEC>(r + off);
                     if (dy2) d2[u] = ld<VEC>(dy2 + off);
                 }
             }
@@ -254,9 +319,18 @@ __global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) k_bn_bwd_reduce(const
                 if (p0 + (long)(j0 + u) * lanes >= pixels) continue;
 #pragma unroll
                 for (int i = 0; i < VEC; ++i) {
-                    const float gt = __bfloat162float(bn_dgrad<ACT>(dv[u].h[i], d2[u].h[i], dy2 != nullptr, yv[u].h[i]));
-                    sb[i] = __fadd_rn(sb[i], gt);
-                    sg[i] = __fadd_rn(sg[i], __fmul_rn(gt, bn_xhat(xv[u].h[i], mu[i], rs[i])));
+                    if constexpr (PRE) {
+                        const int c = g * VEC + i;
+                        const float xh = bn_xhat(xv[u].h[i], cmu[c], crs[c]);
+                        const float gt =
+                            __bfloat162float(bn_dgrad_pre<ACT>(dv[u].h[i], d2[u].h[i], dy2 != nullptr, bn_pre(xh, cga[c], cbe[c], r, rv[u].h[i])));
+                        sb[i] = __fadd_rn(sb[i], gt);
+                        sg[i] = __fadd_rn(sg[i], __fmul_rn(gt, xh));
+                    } else {
+                        const float gt = __bfloat162float(bn_dgrad<ACT>(dv[u].h[i], d2[u].h[i], dy2 != nullptr, yv[u].h[i]));
+                        sb[i] = __fadd_rn(sb[i], gt);
+                        sg[i] = __fadd_rn(sg[i], __fmul_rn(gt, bn_xhat(xv[u].h[i], mu[i], rs[i])));
+                    }
                 }
             }
         }
@@ -273,28 +347,35 @@ __global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) k_bn_bwd_reduce(const
 // second backward pass: dx = bf16_rn(((g~ - dbeta / M) - xhat * (dgamma / M)) * (gamma * rstd)), dr = g~.  dx may be dy.
 template <int VEC, int ACT>
 __global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) k_bn_bwd_dx(const __nv_bfloat16 *__restrict__ x, const __nv_bfloat16 *__restrict__ y,
-                                                          const __nv_bfloat16 *dy, const __nv_bfloat16 *__restrict__ dy2,
-                                                          const float *__restrict__ mean, const float *__restrict__ rstd,
-                                                          const float *__restrict__ gamma, const float *__restrict__ dgamma,
+                                                          const __nv_bfloat16 *__restrict__ r, const __nv_bfloat16 *dy,
+                                                          const __nv_bfloat16 *__restrict__ dy2, const float *__restrict__ mean,
+                                                          const float *__restrict__ rstd, const float *__restrict__ gamma,
+                                                          const float *__restrict__ beta, const float *__restrict__ dgamma,
                                                           const float *__restrict__ dbeta, __nv_bfloat16 *dx, __nv_bfloat16 *__restrict__ dr,
                                                           long pixels, int C, float Mf) {
+    constexpr bool PRE = bn_preact<ACT>();
     constexpr int U = bn_unroll<VEC>();
     const int G = C / VEC, lanes = BN_THREADS / G;
     const int lane = threadIdx.x / G, g = threadIdx.x % G;
     // the per-channel constants live in shared memory: forty of them in registers next to the loads spill on the 8-channel path
     __shared__ float mu[BN_MAX_C], rs[BN_MAX_C], mb[BN_MAX_C], mg[BN_MAX_C], sc[BN_MAX_C];
+    __shared__ float ga[PRE ? BN_MAX_C : 1], be[PRE ? BN_MAX_C : 1];
     for (int c = threadIdx.x; c < C; c += BN_THREADS) {
         mu[c] = mean[c];
         rs[c] = rstd[c];
         mb[c] = __fdiv_rn(dbeta[c], Mf);
         mg[c] = __fdiv_rn(dgamma[c], Mf);
         sc[c] = __fmul_rn(gamma[c], rs[c]);
+        if (PRE) {
+            ga[c] = gamma[c];
+            be[c] = beta[c];
+        }
     }
     __syncthreads();
     if (lane >= lanes) return;
     const long p0 = (long)blockIdx.x * BN_ITERS * lanes + lane;
     for (int j0 = 0; j0 < BN_ITERS; j0 += U) {
-        BfVec<VEC> xv[U], yv[U], dv[U], d2[U];
+        BfVec<VEC> xv[U], yv[U], dv[U], d2[U], rv[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
             const long px = p0 + (long)(j0 + u) * lanes;
@@ -303,6 +384,7 @@ __global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) k_bn_bwd_dx(const __n
                 xv[u] = ld<VEC>(x + off);
                 dv[u] = ld<VEC>(dy + off);
                 if (ACT == PCNN_ACT_RELU) yv[u] = ld<VEC>(y + off);
+                if (PRE && r) rv[u] = ld<VEC>(r + off);
                 if (dy2) d2[u] = ld<VEC>(dy2 + off);
             }
         }
@@ -313,9 +395,13 @@ __global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) k_bn_bwd_dx(const __n
             BfVec<VEC> o, gv;
 #pragma unroll
             for (int i = 0; i < VEC; ++i) {
-                gv.h[i] = bn_dgrad<ACT>(dv[u].h[i], d2[u].h[i], dy2 != nullptr, yv[u].h[i]);
                 const int c = g * VEC + i;
-                const float t = __fsub_rn(__fsub_rn(__bfloat162float(gv.h[i]), mb[c]), __fmul_rn(bn_xhat(xv[u].h[i], mu[c], rs[c]), mg[c]));
+                const float xh = bn_xhat(xv[u].h[i], mu[c], rs[c]);
+                if constexpr (PRE)
+                    gv.h[i] = bn_dgrad_pre<ACT>(dv[u].h[i], d2[u].h[i], dy2 != nullptr, bn_pre(xh, ga[c], be[c], r, rv[u].h[i]));
+                else
+                    gv.h[i] = bn_dgrad<ACT>(dv[u].h[i], d2[u].h[i], dy2 != nullptr, yv[u].h[i]);
+                const float t = __fsub_rn(__fsub_rn(__bfloat162float(gv.h[i]), mb[c]), __fmul_rn(xh, mg[c]));
                 o.h[i] = __float2bfloat16_rn(__fmul_rn(t, sc[c]));
             }
             const long off = px * C + g * VEC;
@@ -347,13 +433,34 @@ int bn_geom(const char *fn, long pixels, int C, int training, BnGeom *out) {
     return PCNN_OK;
 }
 
-int bn_act(const char *fn, int act) {
+enum BnPass { BN_FWD, BN_BWD, BN_BWD_PREACT };
+
+bool act_from_preact(int act) { return act == PCNN_ACT_SILU || act == PCNN_ACT_HARDSWISH || act == PCNN_ACT_RELU6; }
+
+// the codes each entry takes: the forward 0 and 3-6, the backward 0 and 3, the pre-activation backward 4-6
+int bn_act(const char *fn, int act, BnPass pass) {
     PCNN_REQUIRE(act != PCNN_ACT_SIGMOID, PCNN_ERR_ARG,
                  "%s: act 1 (sigmoid) is not available after batch normalization: sigmoid_bf16 uses tanh.approx, which no reference "
-                 "can replay bit for bit; act 0 (none) or 3 (ReLU) is required", fn);
-    PCNN_REQUIRE(act == PCNN_ACT_NONE || act == PCNN_ACT_RELU, PCNN_ERR_ARG, "%s: act %d is not 0 (none) or 3 (ReLU)", fn, act);
+                 "can replay bit for bit; %s is required", fn,
+                 pass == BN_BWD_PREACT ? "act 4 (SiLU), 5 (hard-swish) or 6 (ReLU6)" : "act 0 (none) or 3 (ReLU)");
+    const bool plain = act == PCNN_ACT_NONE || act == PCNN_ACT_RELU, pre = act_from_preact(act);
+    if (pass == BN_FWD)
+        PCNN_REQUIRE(plain || pre, PCNN_ERR_ARG, "%s: act %d is not 0 (none) or 3 (ReLU), nor 4 (SiLU), 5 (hard-swish) or 6 (ReLU6)", fn, act);
+    if (pass == BN_BWD) {
+        PCNN_REQUIRE(!pre, PCNN_ERR_ARG,
+                     "%s: act %d takes its gradient from the recomputed pre-activation, not from y: pcnn_batchnorm_nhwc_bf16_bwd_preact "
+                     "is its backward", fn, act);
+        PCNN_REQUIRE(plain, PCNN_ERR_ARG, "%s: act %d is not 0 (none) or 3 (ReLU)", fn, act);
+    }
+    if (pass == BN_BWD_PREACT) {
+        PCNN_REQUIRE(!plain, PCNN_ERR_ARG, "%s: act %d takes its gradient from y: pcnn_batchnorm_nhwc_bf16_bwd is its backward", fn, act);
+        PCNN_REQUIRE(pre, PCNN_ERR_ARG, "%s: act %d is not 4 (SiLU), 5 (hard-swish) or 6 (ReLU6)", fn, act);
+    }
     return PCNN_OK;
 }
+
+// column of an accepted code in the kernel tables: 0, 3, 4, 5, 6 -> 0 .. 4
+int act_col(int act) { return act == PCNN_ACT_NONE ? 0 : act - 2; }
 
 struct Buf {
     const void *p;
@@ -378,10 +485,42 @@ bool disjoint(const Buf *b, int n, const void *same_a = nullptr, const void *sam
 
 typedef void (*apply_fn)(const __nv_bfloat16 *, const __nv_bfloat16 *, __nv_bfloat16 *, const float *, const float *, const float *, float,
                          const float *, const float *, long, int);
-typedef void (*reduce_fn)(const __nv_bfloat16 *, const __nv_bfloat16 *, const __nv_bfloat16 *, const __nv_bfloat16 *, const float *,
-                          const float *, float *, long, int, long);
-typedef void (*dx_fn)(const __nv_bfloat16 *, const __nv_bfloat16 *, const __nv_bfloat16 *, const __nv_bfloat16 *, const float *, const float *,
-                      const float *, const float *, const float *, __nv_bfloat16 *, __nv_bfloat16 *, long, int, float);
+typedef void (*reduce_fn)(const __nv_bfloat16 *, const __nv_bfloat16 *, const __nv_bfloat16 *, const __nv_bfloat16 *, const __nv_bfloat16 *,
+                          const float *, const float *, const float *, const float *, float *, long, int, long);
+typedef void (*dx_fn)(const __nv_bfloat16 *, const __nv_bfloat16 *, const __nv_bfloat16 *, const __nv_bfloat16 *, const __nv_bfloat16 *,
+                      const float *, const float *, const float *, const float *, const float *, const float *, __nv_bfloat16 *,
+                      __nv_bfloat16 *, long, int, float);
+
+#define BN_ACTS(K, V) {K<V, PCNN_ACT_NONE>, K<V, PCNN_ACT_RELU>, K<V, PCNN_ACT_SILU>, K<V, PCNN_ACT_HARDSWISH>, K<V, PCNN_ACT_RELU6>}
+
+// both backward entries: the reduce pass, the fixed-order slot sums into dbeta and dgamma, the dx pass.  y is read at act 3, beta
+// and r at codes 4-6.
+int bn_bwd_launch(pcnn_ctx *ctx, const BnGeom &gm, const void *x_bf16, const void *y_bf16, const void *r_bf16, const void *dy_bf16,
+                  const void *dy2_bf16, const float *gamma, const float *beta, const float *save_mean, const float *save_rstd, void *dx_bf16,
+                  void *dr_bf16, float *dgamma, float *dbeta, long pixels, int C, int act) {
+    pcnn_device_guard dg(ctx->device);
+    float *slots = nullptr;
+    int rc;
+    if ((rc = pcnn_scratch(ctx, (size_t)2 * gm.ctas * C * sizeof(float), (void **)&slots))) return rc;
+    const auto *x = static_cast<const __nv_bfloat16 *>(x_bf16);
+    const auto *y = static_cast<const __nv_bfloat16 *>(y_bf16);
+    const auto *r = static_cast<const __nv_bfloat16 *>(r_bf16);
+    const auto *dy = static_cast<const __nv_bfloat16 *>(dy_bf16);
+    const auto *dy2 = static_cast<const __nv_bfloat16 *>(dy2_bf16);
+    const int v8 = gm.vec == 8 ? 1 : 0, col = act_col(act);
+    static const reduce_fn rtable[2][5] = {BN_ACTS(k_bn_bwd_reduce, 1), BN_ACTS(k_bn_bwd_reduce, 8)};
+    rtable[v8][col]<<<(unsigned)gm.ctas, BN_THREADS, 0, ctx->stream>>>(x, y, r, dy, dy2, save_mean, save_rstd, gamma, beta, slots, pixels, C,
+                                                                       gm.ctas);
+    PCNN_CHECK_LAUNCH(ctx);
+    if ((rc = pcnn_conv_wgrad_reduce_slots(ctx, slots, dbeta, (int)gm.ctas, C))) return rc;
+    if ((rc = pcnn_conv_wgrad_reduce_slots(ctx, slots + gm.ctas * C, dgamma, (int)gm.ctas, C))) return rc;
+    static const dx_fn dtable[2][5] = {BN_ACTS(k_bn_bwd_dx, 1), BN_ACTS(k_bn_bwd_dx, 8)};
+    dtable[v8][col]<<<(unsigned)gm.ctas, BN_THREADS, 0, ctx->stream>>>(x, y, r, dy, dy2, save_mean, save_rstd, gamma, beta, dgamma, dbeta,
+                                                                       static_cast<__nv_bfloat16 *>(dx_bf16),
+                                                                       static_cast<__nv_bfloat16 *>(dr_bf16), pixels, C, (float)pixels);
+    PCNN_CHECK_LAUNCH(ctx);
+    return PCNN_OK;
+}
 
 }  // namespace
 
@@ -404,7 +543,7 @@ extern "C" int pcnn_batchnorm_nhwc_bf16_fwd(pcnn_ctx *ctx, const void *x_bf16, c
                                             float *running_mean, float *running_var, float *save_mean, float *save_rstd) {
     const char *fn = "pcnn_batchnorm_nhwc_bf16_fwd";
     PCNN_REQUIRE(ctx && x_bf16 && y_bf16 && gamma && beta, PCNN_ERR_ARG, "%s: NULL context, x, y, gamma or beta (only r may be NULL)", fn);
-    int rc = bn_act(fn, act);
+    int rc = bn_act(fn, act, BN_FWD);
     if (rc) return rc;
     BnGeom gm;
     if ((rc = bn_geom(fn, pixels, C, training, &gm))) return rc;
@@ -429,7 +568,7 @@ extern "C" int pcnn_batchnorm_nhwc_bf16_fwd(pcnn_ctx *ctx, const void *x_bf16, c
     const auto *x = static_cast<const __nv_bfloat16 *>(x_bf16);
     const auto *r = static_cast<const __nv_bfloat16 *>(r_bf16);
     auto *y = static_cast<__nv_bfloat16 *>(y_bf16);
-    const int v8 = gm.vec == 8 ? 1 : 0, relu = act == PCNN_ACT_RELU ? 1 : 0;
+    const int v8 = gm.vec == 8 ? 1 : 0;
     if (training) {
         float *slots = nullptr;
         if ((rc = pcnn_scratch(ctx, (size_t)3 * gm.ctas * C * sizeof(float), (void **)&slots))) return rc;
@@ -442,9 +581,8 @@ extern "C" int pcnn_batchnorm_nhwc_bf16_fwd(pcnn_ctx *ctx, const void *x_bf16, c
                                                               running_mean, running_var);
         PCNN_CHECK_LAUNCH(ctx);
     }
-    static const apply_fn table[2][2] = {{k_bn_apply<1, PCNN_ACT_NONE>, k_bn_apply<1, PCNN_ACT_RELU>},
-                                         {k_bn_apply<8, PCNN_ACT_NONE>, k_bn_apply<8, PCNN_ACT_RELU>}};
-    table[v8][relu]<<<(unsigned)gm.ctas, BN_THREADS, 0, ctx->stream>>>(x, r, y, training ? save_mean : running_mean,
+    static const apply_fn table[2][5] = {BN_ACTS(k_bn_apply, 1), BN_ACTS(k_bn_apply, 8)};
+    table[v8][act_col(act)]<<<(unsigned)gm.ctas, BN_THREADS, 0, ctx->stream>>>(x, r, y, training ? save_mean : running_mean,
                                                                        training ? save_rstd : nullptr, training ? nullptr : running_var, eps,
                                                                        gamma, beta, pixels, C);
     PCNN_CHECK_LAUNCH(ctx);
@@ -457,7 +595,7 @@ extern "C" int pcnn_batchnorm_nhwc_bf16_bwd(pcnn_ctx *ctx, const void *x_bf16, c
     const char *fn = "pcnn_batchnorm_nhwc_bf16_bwd";
     PCNN_REQUIRE(ctx && x_bf16 && y_bf16 && dy_bf16 && gamma && save_mean && save_rstd && dx_bf16 && dgamma && dbeta, PCNN_ERR_ARG,
                  "%s: NULL context, x, y, dy, gamma, save_mean, save_rstd, dx, dgamma or dbeta (only dy2 and dr may be NULL)", fn);
-    int rc = bn_act(fn, act);
+    int rc = bn_act(fn, act, BN_BWD);
     if (rc) return rc;
     BnGeom gm;
     if ((rc = bn_geom(fn, pixels, C, 1, &gm))) return rc;
@@ -469,25 +607,30 @@ extern "C" int pcnn_batchnorm_nhwc_bf16_bwd(pcnn_ctx *ctx, const void *x_bf16, c
                           {save_rstd, cb}, {dx_bf16, tb},   {dr_bf16, tb}, {dgamma, cb},   {dbeta, cb}};
     PCNN_REQUIRE(disjoint(bufs, 11, dx_bf16, dy_bf16), PCNN_ERR_ARG,
                  "%s: overlapping buffers: only dx == dy (in place) may share memory", fn);
-    pcnn_device_guard dg(ctx->device);
-    float *slots = nullptr;
-    if ((rc = pcnn_scratch(ctx, (size_t)2 * gm.ctas * C * sizeof(float), (void **)&slots))) return rc;
-    const auto *x = static_cast<const __nv_bfloat16 *>(x_bf16);
-    const auto *y = static_cast<const __nv_bfloat16 *>(y_bf16);
-    const auto *dy = static_cast<const __nv_bfloat16 *>(dy_bf16);
-    const auto *dy2 = static_cast<const __nv_bfloat16 *>(dy2_bf16);
-    const int v8 = gm.vec == 8 ? 1 : 0, relu = act == PCNN_ACT_RELU ? 1 : 0;
-    static const reduce_fn rtable[2][2] = {{k_bn_bwd_reduce<1, PCNN_ACT_NONE>, k_bn_bwd_reduce<1, PCNN_ACT_RELU>},
-                                           {k_bn_bwd_reduce<8, PCNN_ACT_NONE>, k_bn_bwd_reduce<8, PCNN_ACT_RELU>}};
-    rtable[v8][relu]<<<(unsigned)gm.ctas, BN_THREADS, 0, ctx->stream>>>(x, y, dy, dy2, save_mean, save_rstd, slots, pixels, C, gm.ctas);
-    PCNN_CHECK_LAUNCH(ctx);
-    if ((rc = pcnn_conv_wgrad_reduce_slots(ctx, slots, dbeta, (int)gm.ctas, C))) return rc;
-    if ((rc = pcnn_conv_wgrad_reduce_slots(ctx, slots + gm.ctas * C, dgamma, (int)gm.ctas, C))) return rc;
-    static const dx_fn dtable[2][2] = {{k_bn_bwd_dx<1, PCNN_ACT_NONE>, k_bn_bwd_dx<1, PCNN_ACT_RELU>},
-                                       {k_bn_bwd_dx<8, PCNN_ACT_NONE>, k_bn_bwd_dx<8, PCNN_ACT_RELU>}};
-    dtable[v8][relu]<<<(unsigned)gm.ctas, BN_THREADS, 0, ctx->stream>>>(x, y, dy, dy2, save_mean, save_rstd, gamma, dgamma, dbeta,
-                                                                        static_cast<__nv_bfloat16 *>(dx_bf16),
-                                                                        static_cast<__nv_bfloat16 *>(dr_bf16), pixels, C, (float)pixels);
-    PCNN_CHECK_LAUNCH(ctx);
-    return PCNN_OK;
+    return bn_bwd_launch(ctx, gm, x_bf16, y_bf16, nullptr, dy_bf16, dy2_bf16, gamma, nullptr, save_mean, save_rstd, dx_bf16, dr_bf16, dgamma,
+                         dbeta, pixels, C, act);
+}
+
+extern "C" int pcnn_batchnorm_nhwc_bf16_bwd_preact(pcnn_ctx *ctx, const void *x_bf16, const void *r_bf16, const void *dy_bf16,
+                                                   const void *dy2_bf16, const float *gamma, const float *beta, const float *save_mean,
+                                                   const float *save_rstd, void *dx_bf16, void *dr_bf16, float *dgamma, float *dbeta, long pixels,
+                                                   int C, int act) {
+    const char *fn = "pcnn_batchnorm_nhwc_bf16_bwd_preact";
+    PCNN_REQUIRE(ctx && x_bf16 && dy_bf16 && gamma && beta && save_mean && save_rstd && dx_bf16 && dgamma && dbeta, PCNN_ERR_ARG,
+                 "%s: NULL context, x, dy, gamma, beta, save_mean, save_rstd, dx, dgamma or dbeta (only r, dy2 and dr may be NULL)", fn);
+    int rc = bn_act(fn, act, BN_BWD_PREACT);
+    if (rc) return rc;
+    BnGeom gm;
+    if ((rc = bn_geom(fn, pixels, C, 1, &gm))) return rc;
+    const void *ptrs[12] = {x_bf16, r_bf16, dy_bf16, dy2_bf16, gamma, beta, save_mean, save_rstd, dx_bf16, dr_bf16, dgamma, dbeta};
+    for (const void *q : ptrs)
+        PCNN_REQUIRE(aligned16(q), PCNN_ERR_ARG,
+                     "%s: x, r, dy, dy2, dx, dr, gamma, beta, dgamma, dbeta and the statistics must be 16-byte aligned", fn);
+    const size_t tb = (size_t)pixels * C * 2, cb = (size_t)C * sizeof(float);
+    const Buf bufs[12] = {{x_bf16, tb}, {r_bf16, tb},    {dy_bf16, tb},   {dy2_bf16, tb}, {gamma, cb},  {beta, cb},
+                          {save_mean, cb}, {save_rstd, cb}, {dx_bf16, tb}, {dr_bf16, tb},  {dgamma, cb}, {dbeta, cb}};
+    PCNN_REQUIRE(disjoint(bufs, 12, dx_bf16, dy_bf16), PCNN_ERR_ARG,
+                 "%s: overlapping buffers: only dx == dy (in place) may share memory", fn);
+    return bn_bwd_launch(ctx, gm, x_bf16, nullptr, r_bf16, dy_bf16, dy2_bf16, gamma, beta, save_mean, save_rstd, dx_bf16, dr_bf16, dgamma,
+                         dbeta, pixels, C, act);
 }

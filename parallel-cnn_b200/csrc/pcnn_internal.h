@@ -311,6 +311,26 @@ __device__ __forceinline__ float div_rn(float a, double b, double rb) {
     q = fma(fma(-b, q, ad), rb, q);
     return a == 0.0f || !isfinite(a) ? a * (float)rb : __double2float_rn(q);
 }
+// E(x) = exp(x) in fp32 as a fixed sequence of round-to-nearest operations with no contraction, so that a numpy float32 replay
+// gives the same bits (expf / __expf cannot be replayed).  include/pcnn.h states the sequence and the constants; max error 1.30
+// ulp over the finite inputs.  Cody-Waite: k = rint(x log2e); k ln2_hi is exact (15 significant bits times |k| <= 150) and so is
+// x - k ln2_hi (Sterbenz); a degree-6 Horner polynomial on |r| <= ln2 / 2; 2^k as two exact powers of two, so that a subnormal
+// result is rounded once.  x > 88.7228317 gives +Inf, x < -103.972076 gives +0, NaN gives NaN.
+__device__ __forceinline__ float exp_f32(float x) {
+    if (x > 88.7228317f) return __int_as_float(0x7f800000);
+    if (x < -103.972076f) return 0.0f;
+    const float k = rintf(__fmul_rn(x, 1.44269502f));
+    const float r = __fsub_rn(__fsub_rn(x, __fmul_rn(k, 0.693145752f)), __fmul_rn(k, 1.42860677e-06f));
+    float p = 0.00138436025f;
+    p = __fadd_rn(__fmul_rn(p, r), 0.00837419648f);
+    p = __fadd_rn(__fmul_rn(p, r), 0.0416680053f);
+    p = __fadd_rn(__fmul_rn(p, r), 0.166664302f);
+    p = __fadd_rn(__fmul_rn(p, r), 0.49999994f);
+    p = __fadd_rn(__fmul_rn(p, r), 1.0f);
+    p = __fadd_rn(__fmul_rn(p, r), 1.0f);
+    const int ki = __float2int_rn(k), k1 = ki >> 1, k2 = ki - k1;      // a NaN x gives ki = 0 and p = NaN
+    return __fmul_rn(__fmul_rn(p, __int_as_float((k1 + 127) << 23)), __int_as_float((k2 + 127) << 23));
+}
 #endif
 // conv_wgrad_tc.cu: dw[o] = sum over i of slots[i][o] for o < nout, in a fixed order (deterministic, no atomics)
 int pcnn_conv_wgrad_reduce_slots(pcnn_ctx *ctx, const float *slots, float *dw, int nslots, int nout);

@@ -6,7 +6,9 @@ import numpy as np
 
 from ._lib import (F32, NPARAM, OPTIM_ADAMW, OPTIM_SGD, TEST_SET, TRAIN_SET, U8, OptimConfig, OptimTensor, PcnnError, avgpool_nhwc_info,
                    batchnorm_nhwc_info, check, conv_layer_family, dwconv_info, global_avgpool_nhwc_info, lib, linear_info, maxpool_nhwc_info,
-                   se_scale_nhwc_info, ACT_RELU, ACT_SIGMOID)
+                   se_scale_nhwc_info, ACT_RELU, ACT_SIGMOID, ACT_SILU, ACT_HARDSWISH, ACT_RELU6)
+
+PREACT_CODES = (ACT_SILU, ACT_HARDSWISH, ACT_RELU6)   # batch normalization's codes whose backward recomputes the pre-activation
 
 
 def _pixel_type(arr_or_dtype):
@@ -459,7 +461,7 @@ class Engine:
                       act=0, training=True, eps=1e-5, momentum=0.1):
         """pcnn_batchnorm_nhwc_bf16_fwd: y = bf16(act((x - mean) * rstd * gamma + beta (+ r))) over dense bf16 [pixels][C].
         training: batch statistics into save_mean / save_rstd and, when given, the running statistics updated with momentum;
-        eval: the running statistics.  act ACT_NONE or ACT_RELU"""
+        eval: the running statistics.  act ACT_NONE, ACT_RELU, ACT_SILU, ACT_HARDSWISH or ACT_RELU6"""
         self._call("pcnn_batchnorm_nhwc_bf16_fwd", _p(x), _p(r), _p(y), int(pixels), int(C), int(act), 1 if training else 0, float(eps),
                    float(momentum), _p(gamma), _p(beta), _p(running_mean), _p(running_var), _p(save_mean), _p(save_rstd))
 
@@ -468,6 +470,14 @@ class Engine:
         dx (may be dy itself) and, when given, dr = g (the gradient of the forward's residual input)"""
         self._call("pcnn_batchnorm_nhwc_bf16_bwd", _p(x), _p(y), _p(dy), _p(dy2), _p(gamma), _p(save_mean), _p(save_rstd), _p(dx), _p(dr),
                    _p(dgamma), _p(dbeta), int(pixels), int(C), int(act))
+
+    def batchnorm_bwd_preact(self, x, dy, gamma, beta, save_mean, save_rstd, dx, dgamma, dbeta, pixels, C, act, r=None, dy2=None,
+                             dr=None):
+        """pcnn_batchnorm_nhwc_bf16_bwd_preact of a training forward at ACT_SILU, ACT_HARDSWISH or ACT_RELU6: as batchnorm_bwd, with
+        g = bf16(act'(v) * (dy (+ dy2))) taken at the pre-activation v recomputed from x, the saved statistics, gamma, beta and r (the
+        forward's r, unchanged, or None if it had none) instead of from y"""
+        self._call("pcnn_batchnorm_nhwc_bf16_bwd_preact", _p(x), _p(r), _p(dy), _p(dy2), _p(gamma), _p(beta), _p(save_mean), _p(save_rstd),
+                   _p(dx), _p(dr), _p(dgamma), _p(dbeta), int(pixels), int(C), int(act))
 
     def pad_nhwc(self, src_bf16, dst_bf16, N, H, W, Cin, pad_h, pad_w, dst_row_pitch=0, dst_image_rows=0):
         self._call("pcnn_pad_nhwc_bf16", _p(src_bf16), _p(dst_bf16), N, H, W, Cin, int(pad_h), int(pad_w), int(dst_row_pitch), int(dst_image_rows))
@@ -778,7 +788,9 @@ class BatchNormLayer:
     and the saved mean and rstd of the last training forward, all in DeviceArrays.
 
     x, r, y, dy, dy2, dx and dr are dense bf16 [N][H][W][C]: what a ConvLayer writes as y and reads as dy.  act ACT_RELU (3) is
-    a ReLU after the add, ACT_NONE (0) none.  A ResNet basic block, x0 being a previous BatchNormLayer's output:
+    a ReLU after the add, ACT_NONE (0) none; ACT_SILU (4), ACT_HARDSWISH (5) and ACT_RELU6 (6) are the activations of EfficientNet,
+    MobileNetV3 and MobileNetV2, whose backward works from the pre-activation recomputed from x and r rather than from y, so at those
+    codes the layer keeps r as well as x.  A ResNet basic block, x0 being a previous BatchNormLayer's output:
 
         conv_a.forward(x0, ya); bn_a.forward(ya, za); conv_b.forward(za, yb); bn_b.forward(yb, out, r=x0)
         bn_b.backward(out, dout, dyb, dr=dres); conv_b.backward(yb, dyb, dza); bn_a.backward(za, dza, dya)
@@ -800,22 +812,30 @@ class BatchNormLayer:
         self.running_mean = DeviceArray.from_host(engine, np.zeros(C, np.float32))
         self.running_var = DeviceArray.from_host(engine, np.ones(C, np.float32))
         self.save_mean, self.save_rstd = engine.array(C), engine.array(C)
-        self._x = None
+        self._x = self._r = None
 
     def forward(self, x, y, r=None, training=True):
         """y = act(bn(x) + r).  training: batch statistics, saved for backward, and the running statistics updated; otherwise the
-        running statistics.  The layer keeps x: backward reads it."""
+        running statistics.  The layer keeps x (and r at ACT_SILU, ACT_HARDSWISH and ACT_RELU6): backward reads them, so they must
+        stay unchanged until then."""
         N, H, W, C = self.shape
         self.engine.batchnorm_fwd(x, y, self.pixels, C, self.gamma, self.beta, self.running_mean, self.running_var, self.save_mean,
                                   self.save_rstd, r=r, act=self.act, training=training, eps=self.eps, momentum=self.momentum)
         if training:
             self._x = x
+            if self.act in PREACT_CODES:
+                self._r = r
 
     def backward(self, y, dy, dx, dr=None, dy2=None):
         """Gradients of the most recent training forward, whose output y was: dgamma, dbeta and dx (dx may be dy).  dy2 is a second
         gradient added to dy before the activation (the other branch of a residual join); dr receives the gradient of the
-        forward's r."""
+        forward's r.  At ACT_SILU, ACT_HARDSWISH and ACT_RELU6 y is not read: the gradient is taken at the recomputed
+        pre-activation (Engine.batchnorm_bwd_preact)."""
         N, H, W, C = self.shape
+        if self.act in PREACT_CODES:
+            self.engine.batchnorm_bwd_preact(self._x, dy, self.gamma, self.beta, self.save_mean, self.save_rstd, dx, self.dgamma, self.dbeta,
+                                             self.pixels, C, self.act, r=self._r, dy2=dy2, dr=dr)
+            return
         self.engine.batchnorm_bwd(self._x, y, dy, self.gamma, self.save_mean, self.save_rstd, dx, self.dgamma, self.dbeta, self.pixels, C,
                                   act=self.act, dy2=dy2, dr=dr)
 

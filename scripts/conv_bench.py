@@ -1027,6 +1027,143 @@ def run_seblock(N, iters, hid=8):
         layer.close()
 
 
+def run_bnact(name, N, H, W, C, iters, rounds=3):
+    """batch normalization followed by ReLU (3), SiLU (4), hard-swish (5) or ReLU6 (6): training forward, eval forward and backward
+    (pcnn_batchnorm_nhwc_bf16_bwd at 3, pcnn_batchnorm_nhwc_bf16_bwd_preact at 4-6), each with and without the residual r, the
+    codes alternated over `rounds` rounds (the best of each kept), next to torch's F.batch_norm (+ add) + relu / silu / hardswish /
+    relu6 and its autograd backward on the same channels-last bf16 tensors.  Bytes, T = N*H*W*C*2: the forwards as run_bn; the
+    backward 7T at code 3 (x, y, dy read twice, dx written) and 5T at 4-6 (x, dy read twice, dx written), + 2T for reading r twice
+    at 4-6, + T for writing dr."""
+    M = N * H * W
+    T = M * C * 2
+    rnd = lambda: torch.randint(-0x4000, 0x4000, (M, C), dtype=torch.int16, device="cuda") & 0x3FFF | 0x3C00   # bf16 in [1, 2) * 2^k
+    x, r, dy = rnd(), rnd(), rnd()
+    r ^= torch.randint(0, 2, (M, C), dtype=torch.int16, device="cuda") << 15
+    dy ^= torch.randint(0, 2, (M, C), dtype=torch.int16, device="cuda") << 15
+    y, dx, dr = (torch.empty((M, C), dtype=torch.int16, device="cuda") for _ in range(3))
+    info = pkg.batchnorm_nhwc_info(M, C)
+    f = lambda v: eng.to_device(np.full(C, v, np.float32))
+    gamma, beta, rm, rv, sm, sr, dg, db = f(1), f(0), f(0), f(1), f(0), f(1), f(0), f(0)
+    gpu, power = card()
+    F = torch.nn.functional
+    acts = {3: torch.relu, 4: F.silu, 5: F.hardswish, 6: F.relu6}
+    bf = lambda t: t.view(torch.bfloat16).reshape(N, H, W, C).permute(0, 3, 1, 2)         # channels-last NCHW views
+    xt, rt, dyt = bf(x).detach().clone().requires_grad_(True), bf(r).detach().clone().requires_grad_(True), bf(dy)
+    gt, bt = torch.ones(C, device="cuda", requires_grad=True), torch.zeros(C, device="cuda", requires_grad=True)
+    rmt, rvt = torch.zeros(C, device="cuda"), torch.ones(C, device="cuda")
+
+    def torch_fwd(act, with_r, training):
+        v = F.batch_norm(xt, rmt, rvt, gt, bt, training=training, momentum=0.1, eps=1e-5)
+        return acts[act](v + rt if with_r else v)
+
+    def ours_bwd(act, rr, drr):
+        if act == 3:
+            return eng.batchnorm_bwd(x, y, dy, gamma, sm, sr, dx, dg, db, M, C, act=3, dr=drr)
+        return eng.batchnorm_bwd_preact(x, dy, gamma, beta, sm, sr, dx, dg, db, M, C, act, r=rr, dr=drr)
+
+    for with_r in (False, True):
+        rr, drr = (r, dr) if with_r else (None, None)
+        ins = [xt, gt, bt] + ([rt] if with_r else [])
+        outs = {a: torch_fwd(a, with_r, True) for a in acts}
+        best = {}
+        for _ in range(rounds):
+            for act in acts:
+                eng.batchnorm_fwd(x, y, M, C, gamma, beta, rm, rv, sm, sr, r=rr, act=act)      # warm the training forward's path
+                # the backward right after the training forward, so that at act 3 it reads that forward's y
+                passes = (("training fwd", lambda: eng.batchnorm_fwd(x, y, M, C, gamma, beta, rm, rv, sm, sr, r=rr, act=act),
+                           lambda: torch_fwd(act, with_r, True), 3 * T + (T if with_r else 0)),
+                          ("bwd", lambda: ours_bwd(act, rr, drr), lambda: torch.autograd.grad(outs[act], ins, dyt, retain_graph=True),
+                           (7 * T if act == 3 else 5 * T + (2 * T if with_r else 0)) + (T if with_r else 0)),
+                          ("eval fwd", lambda: eng.batchnorm_fwd(x, y, M, C, gamma, beta, rm, rv, r=rr, act=act, training=False),
+                           lambda: torch_fwd(act, with_r, False), 2 * T + (T if with_r else 0)))
+                for what, fn, tfn, nbytes in passes:
+                    ms, ms_torch = timed(fn, iters), timed(tfn, iters)
+                    old = best.get((act, what))
+                    best[(act, what)] = (min(ms, old[0]) if old else ms, min(ms_torch, old[1]) if old else ms_torch, nbytes)
+        for what in ("training fwd", "eval fwd", "bwd"):
+            ms3 = best[(3, what)][0]
+            for act in acts:
+                ms, ms_torch, nbytes = best[(act, what)]
+                print(json.dumps({"case": f"{name} {what}" + (" + r" if with_r else ""), "act": act, "N": N, "us": ms * 1e3, "MB": nbytes / 1e6,
+                                  "hbm_frac": nbytes / (ms * 1e-3) / 1e9 / HBM, "over_act3": ms / ms3, "torch_us": ms_torch * 1e3,
+                                  "torch_over_ours": ms_torch / ms, "vec": info["vec"], "gpu": gpu, "power_limit": power}), flush=True)
+    for a in (gamma, beta, rm, rv, sm, sr, dg, db):
+        a.free()
+    del x, r, dy, y, dx, dr, xt, rt
+
+
+def run_mbconv(N, iters, hid=16):
+    """one training step of an EfficientNet MBConv block with SiLU and squeeze-and-excitation at 28x28x40, N = 128: 1x1 expand to
+    240 -> BN + SiLU -> depthwise 5x5 pad 2 -> BN + SiLU -> SE 240 -> hid -> 240 -> 1x1 project to 40 -> BN + x0, its backward (the
+    shortcut's gradient dres left apart, as run_mbblock) and the sgd of the eight layers, on the engine's stream.  Next to it the
+    torch eager step of the same block on bf16 channels-last tensors (fp32 masters, w -= lr * grad, re-cast to bf16)."""
+    H = W = 28
+    C, E, k = 40, 240, 5
+    r = np.random.default_rng(14)
+    u = lambda shape, fan: r.uniform(-1, 1, shape).astype(np.float32) / np.float32(np.sqrt(fan))
+    fe, fd, fp = u((E, 1, 1, C), C), u((E, k, k), k * k), u((C, 1, 1, E), E)
+    w1, b1_, w2, b2_ = u((hid, E), E), u(hid, E), u((E, hid), hid), u(E, hid)
+    ex = pkg.ConvLayer(eng, N, H, W, C, E, 1, 1, fe, None, act=0)
+    dwl = pkg.DepthwiseConvLayer(eng, N, H, W, E, k, k, fd, None, act=0, padding=(k // 2, k // 2))
+    pr = pkg.ConvLayer(eng, N, H, W, E, C, 1, 1, fp, None, act=0)
+    se = pkg.SqueezeExcitationLayer(eng, N, H, W, E, hid, w1, b1_, w2, b2_, act=0)
+    b1, b2 = pkg.BatchNormLayer(eng, N, H, W, E, act=pkg.ACT_SILU), pkg.BatchNormLayer(eng, N, H, W, E, act=pkg.ACT_SILU)
+    b3 = pkg.BatchNormLayer(eng, N, H, W, C, act=0)
+    wide = lambda: torch.empty((N, H, W, E), dtype=torch.int16, device="cuda")
+    narrow = lambda: torch.empty((N, H, W, C), dtype=torch.int16, device="cuda")
+    x0 = torch.randint(0, 0x3F80, (N, H, W, C), dtype=torch.int16, device="cuda")
+    dout = torch.randint(0, 0x3F80, (N, H, W, C), dtype=torch.int16, device="cuda")
+    dout ^= torch.randint(0, 2, (N, H, W, C), dtype=torch.int16, device="cuda") << 15
+    ye, ze, yd, zd, ys, dys, dze, dye, dyd, dzd = (wide() for _ in range(10))
+    yp, out, dyp, dres, dx0 = (narrow() for _ in range(5))
+    lr = 0.05
+    gpu, power = card()
+    layers = (ex, b1, dwl, b2, se, pr, b3)
+
+    def step():
+        ex.forward(x0, ye); b1.forward(ye, ze); dwl.forward(ze, yd); b2.forward(yd, zd); se.forward(zd, ys); pr.forward(ys, yp)
+        b3.forward(yp, out, r=x0)
+        b3.backward(out, dout, dyp, dr=dres); pr.backward(yp, dyp, dys); se.backward(ys, dys, dzd); b2.backward(zd, dzd, dyd)
+        dwl.backward(yd, dyd, dze); b1.backward(ze, dze, dye); ex.backward(ye, dye, dx0)
+        for layer in layers:
+            layer.sgd(lr)
+
+    ms = timed(step, iters)
+    ms_bn = {"fwd": timed(lambda: b2.forward(yd, zd), iters), "bwd": timed(lambda: b2.backward(zd, dzd, dyd), iters)}
+    F = torch.nn.functional
+    xt = x0.view(torch.bfloat16).permute(0, 3, 1, 2).detach().requires_grad_(True)
+    dt = dout.view(torch.bfloat16).permute(0, 3, 1, 2)
+    cl = lambda a: torch.from_numpy(a).to("cuda").contiguous(memory_format=torch.channels_last)
+    m32 = {"fe": cl(fe.transpose(0, 3, 1, 2)), "fd": cl(fd[:, None]), "fp": cl(fp.transpose(0, 3, 1, 2))}
+    m32.update({kk: torch.from_numpy(v).to("cuda") for kk, v in (("w1", w1), ("v1", b1_), ("w2", w2), ("v2", b2_))})
+    for i, ch in ((1, E), (2, E), (3, C)):
+        m32[f"g{i}"], m32[f"b{i}"] = torch.ones(ch, device="cuda"), torch.zeros(ch, device="cuda")
+    mb = {kk: (v.to(torch.bfloat16) if kk[0] in "fwv" else v.clone()).requires_grad_(True) for kk, v in m32.items()}
+    stats = [torch.zeros(ch, device="cuda") if j % 2 == 0 else torch.ones(ch, device="cuda") for ch in (E, E, C) for j in range(2)]
+
+    def torch_step():
+        for v in mb.values():
+            v.grad = None
+        xt.grad = None
+        h = F.silu(F.batch_norm(F.conv2d(xt, mb["fe"]), stats[0], stats[1], mb["g1"], mb["b1"], training=True))
+        h = F.silu(F.batch_norm(F.conv2d(h, mb["fd"], padding=k // 2, groups=E), stats[2], stats[3], mb["g2"], mb["b2"], training=True))
+        s = torch.sigmoid(F.linear(torch.relu(F.linear(h.mean((2, 3)), mb["w1"], mb["v1"])), mb["w2"], mb["v2"]))
+        h = h * s[:, :, None, None]
+        h = F.batch_norm(F.conv2d(h, mb["fp"]), stats[4], stats[5], mb["g3"], mb["b3"], training=True) + xt
+        h.backward(dt)
+        with torch.no_grad():
+            for kk in m32:
+                m32[kk].add_(mb[kk].grad.float(), alpha=-lr)
+                mb[kk].copy_(m32[kk])
+
+    ms_torch = timed(torch_step, iters)
+    print(json.dumps({"case": f"MBConv 28x28x40 -> 240 dw 5x5, SiLU, SE 240 -> {hid} -> 240 training step N={N}", "ms": ms,
+                      "torch_eager_ms": ms_torch, "ours_over_torch": ms / ms_torch, "bn_silu_fwd_ms": ms_bn["fwd"],
+                      "bn_silu_bwd_ms": ms_bn["bwd"], "families": [ex.family, pr.family], "gpu": gpu, "power_limit": power}), flush=True)
+    for layer in layers:
+        layer.close()
+
+
 if only == "se":                                                       # squeeze-and-excitation passes, torch beside them
     for args in (("56x56x256", 128, 56, 56, 256), ("28x28x512", 128, 28, 28, 512), ("14x14x1024", 128, 14, 14, 1024),
                  ("7x7x2048", 128, 7, 7, 2048), ("112x112x32", 128, 112, 112, 32), ("56x56x144", 128, 56, 56, 144),
@@ -1062,6 +1199,14 @@ if only == "gap":                                                      # global 
     run_gap("56x56x256 (split path)", 8, 56, 56, 256, 50)
 if only == "resnetgap":                                                # one step of the GAP ResNet, torch eager beside it
     run_resnetgap(128, 20)
+if only == "bnact":                                                    # BN + ReLU / SiLU / hard-swish / ReLU6, torch beside them
+    run_bnact("56x56x64", 128, 56, 56, 64, 50)
+    run_bnact("28x28x128", 128, 28, 28, 128, 50)
+    run_bnact("14x14x256", 128, 14, 14, 256, 50)
+    run_bnact("7x7x256", 128, 7, 7, 256, 50)
+    run_bnact("24x24x6 (scalar path)", 1024, 24, 24, 6, 50)
+if only == "mbconv":                                                   # one step of an MBConv block with SiLU and SE, torch beside it
+    run_mbconv(128, 20)
 if only == "bn":                                                       # batch normalization passes, torch beside them
     run_bn("56x56x64", 128, 56, 56, 64, 50)
     run_bn("28x28x128", 128, 28, 28, 128, 50)
