@@ -662,6 +662,57 @@ int pcnn_dwconv_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C, int R, in
 int pcnn_dwconv_wgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *x_bf16_dev, const void *dy_bf16_dev, float *dw_f32_dev);
 int pcnn_dwconv_dgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *dy_bf16_dev, void *dx_bf16_dev);
 int pcnn_dwconv_info(int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int *out9);
+/* Grouped convolution (csrc/gconv_nhwc.cu), as torch.nn.functional.conv2d(x, w, b, stride, padding=(pad_h, pad_w), groups=G) with
+ * w [K][Cg][R][S], 1 < G: each group g of Cg = C / G input channels feeds its own Kg = K / G filters; output k belongs to group
+ * g = k / Kg (ResNeXt, RegNet, ShuffleNet, and a depthwise layer with a channel multiplier: Cg = 1, Kg > 1).
+ *   - x and dx are dense bf16 [N][H][W][C], y and dy dense bf16 [N][P][Q][K]: the layouts of the conv forwards, batch norm and the
+ *     global average pool; P = (H + 2 pad_h - R) / stride + 1,   Q = (W + 2 pad_w - S) / stride + 1;
+ *   - filters fp32 [K][R][S][Cg] (KRSC with the group's Cg input channels: torch's weight permuted), bias fp32 [K], dw fp32
+ *     [K][R][S][Cg].
+ * pcnn_gconv_plan_create returns a pcnn_conv_plan: pcnn_conv_tc_fwd runs it, pcnn_conv_plan_set_params refreshes its filters and
+ * bias from device memory, pcnn_optim_step refreshes them with the update, and pcnn_conv_tc_plan_destroy frees it.  The plan holds
+ * the filters rounded to bf16 (round to nearest even, on the device) in the master's [K][R][S][Cg] order, as one row.
+ * Rules (fp32 round to nearest; every product float(bf16) * float(bf16) is exact in fp32, so an FMA gives the bits of a product
+ * followed by an add).  The window of output (p, q) starts at (h0, w0) = (p stride - pad_h, q stride - pad_w); a tap outside the
+ * image reads x = +0 and is multiplied like any other (0 * Inf is NaN), as torch does.
+ *   Forward: acc = the sum over r = 0..R-1, then s = 0..S-1, then c = 0..Cg-1, of float(x[n][h0 + r][w0 + s][g Cg + c]) *
+ *     float(wbf16[k][r][s][c]), starting from the first term; v = acc + b[k] with a bias; y = bf16_rn(act(v)), act 0 (none) or 3
+ *     (the ReLU of the conv epilogues: v < 0 ? +0 : v, NaN and -0 unchanged).  Act 1 is refused: the sigmoid uses tanh.approx, which
+ *     no reference can replay.
+ *   Input gradient: dx[n][h][w][g Cg + c] = the sum of float(dy[n][p][q][g Kg + k]) * float(wbf16[g Kg + k][r][s][c]) over the taps
+ *     with h = p stride - pad_h + r and w = q stride - pad_w + s for some 0 <= p < P, 0 <= q < Q, in ascending r, then ascending s,
+ *     then ascending k = 0..Kg-1, starting from the first term, rounded to bf16 once; +0 with no term.  Every element of dx is
+ *     written, with no memset and no atomics.  It uses the plan's bf16 filters, the bits the forward multiplied: call it before the
+ *     filters are refreshed.
+ *   Weight gradient: dw[k][r][s][c] = the sum over n, p, q of float(dy[n][p][q][k]) * float(x~[n][h0 + r][w0 + s][g Cg + c]) (x~ = +0
+ *     outside the image).  The N P Q output pixels are cut into ranges of `pixels per range` (a function of the shape alone, never of
+ *     the SM count); in a range, lane l of `lanes` sums the pixels l, l + lanes, ... from its first one, the lanes holding a pixel are
+ *     added in lane order, and with several ranges each range writes an fp32 slot in the context's scratch block which
+ *     pcnn_conv_wgrad_reduce_slots adds in a fixed order.  dw is overwritten, not accumulated.
+ * Both gradients take the shape from the plan; a plan not made by pcnn_gconv_plan_create is PCNN_ERR_ARG, and the other plan kinds'
+ * gradient calls refuse a grouped plan.  All calls are stream-ordered and give the same bits on every run and SM count.
+ * Domain (anything else is PCNN_ERR_ARG with the function and the rule in the message; pcnn_gconv_info makes the create call's
+ * refusals):
+ *   - the window rules of the depthwise convolution: N, H, W, C >= 1; 1 <= R, S <= 7; stride 1..4; 0 <= pad_h <= R - 1,
+ *     0 <= pad_w <= S - 1, H + 2 pad_h >= R and W + 2 pad_w >= S;
+ *   - K >= 1; G >= 2 (G = 1, a dense convolution, is refused with a message naming the dense plans); C % G == 0 and K % G == 0;
+ *     Cg = Kg = 1 (a depthwise convolution) is refused with a message naming pcnn_dwconv_plan_create; Cg = 1 with Kg > 1 is taken;
+ *   - one group's filters Kg Cg R S <= 36864 (72 KiB of bf16: a CTA stages the filters it applies through shared memory), which
+ *     admits every 1x1 and 3x3 filter with Cg, Kg <= 64 and every 5x5 and 7x7 with Cg Kg <= 64;
+ *   - H W C, P Q K and K R S Cg within the 32-bit index range (C and K have no other limit);  act 0 or 3;
+ *   - every pointer 16-byte aligned; x and y disjoint, dy and dx disjoint, dw disjoint from x and dy.
+ * Each pass loads vectors of the largest of 8, 4, 2, 1 channels that divides its reduced axis (Cg for the forward and the weight
+ * gradient, Kg for the input gradient): Cg % 8 == 0 moves 16-byte vectors of x, any other Cg a narrower path.
+ * pcnn_gconv_info: host only (no GPU, no context).  out16 = { P, Q, Cg, Kg, x channels per load (8, 4, 2 or 1: the largest dividing
+ * Cg), output channels per forward thread and dy channels per input-gradient load (the largest dividing Kg), forward k tiles per
+ * CTA, forward k slices, input-gradient c tiles per CTA, input-gradient c slices, weight-gradient items, weight-gradient item
+ * blocks, pixels per range, ranges, n_acc: the fp32 additions on the longest path of one dw sum (pixels of a lane - 1, lanes - 1,
+ * and with several ranges ceil(ranges / 8) + 3 in pcnn_conv_wgrad_reduce_slots), weight-gradient pixel lanes per range }. */
+int pcnn_gconv_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C, int K, int G, int R, int S, int stride, int pad_h, int pad_w,
+                           int act, const float *filt_host, const float *bias_host, pcnn_conv_plan **out);
+int pcnn_gconv_wgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *x_bf16_dev, const void *dy_bf16_dev, float *dw_f32_dev);
+int pcnn_gconv_dgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *dy_bf16_dev, void *dx_bf16_dev);
+int pcnn_gconv_info(int N, int H, int W, int C, int K, int G, int R, int S, int stride, int pad_h, int pad_w, int *out16);
 /* Squeeze-and-excitation channel gating (csrc/se_nhwc.cu): y = act(x * s[n][c] + r), s = sigmoid(fc2(relu(fc1(GAP(x))))) a gate per
  * image and channel, as in SE-ResNet, MnasNet, MobileNetV3 and EfficientNet.  The squeeze branch runs on the existing layers:
  * pcnn_global_avgpool_nhwc_bf16_fwd writes the x of a linear layer, and linear layers with act 3 and act 1 give s.

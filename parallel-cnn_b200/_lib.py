@@ -171,6 +171,10 @@ _SIG = {
     "pcnn_dwconv_wgrad": [_vp, _vp, _vp, _vp, _vp],
     "pcnn_dwconv_dgrad": [_vp, _vp, _vp, _vp],
     "pcnn_dwconv_info": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
+    "pcnn_gconv_plan_create": [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _pvp],
+    "pcnn_gconv_wgrad": [_vp, _vp, _vp, _vp, _vp],
+    "pcnn_gconv_dgrad": [_vp, _vp, _vp, _vp],
+    "pcnn_gconv_info": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_se_scale_nhwc_bf16_fwd": [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i],
     "pcnn_se_scale_nhwc_bf16_bwd_gate": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i],
     "pcnn_se_scale_nhwc_bf16_bwd_input": [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i],
@@ -348,6 +352,21 @@ def dwconv_info(N, H, W, C, R, S, stride=1, padding=(0, 0)):
     check("pcnn_dwconv_info", lib().pcnn_dwconv_info(int(N), int(H), int(W), int(C), int(R), int(S), int(stride), ph, pw, out))
     return dict(P=out[0], Q=out[1], vec=out[2], groups_per_cta=out[3], slices=out[4], lanes=out[5], pixels_per_range=out[6],
                 ranges=out[7], n_acc=out[8])
+
+
+def gconv_info(N, H, W, C, K, G, R, S, stride=1, padding=(0, 0)):
+    """The output size, the tiling and the weight-gradient split of the grouped convolution (pcnn_gconv_info; host only, no GPU),
+    refused as pcnn_gconv_plan_create refuses.  vec: x channels per load (8, 4, 2 or 1, the largest dividing Cg; 8 is the 16-byte
+    path); kt: output channels per forward thread and dy channels per input-gradient load (the largest dividing Kg); the N*P*Q
+    output pixels are cut into `ranges` of `pixels_per_range`, a function of the shape alone; n_acc: fp32 additions on the longest
+    path of one dw sum."""
+    ph, pw = (int(v) for v in padding)
+    out = (_i * 16)()
+    check("pcnn_gconv_info", lib().pcnn_gconv_info(int(N), int(H), int(W), int(C), int(K), int(G), int(R), int(S), int(stride), ph, pw,
+                                                   out))
+    return dict(P=out[0], Q=out[1], Cg=out[2], Kg=out[3], vec=out[4], kt=out[5], fwd_tiles_per_cta=out[6], fwd_slices=out[7],
+                dgrad_tiles_per_cta=out[8], dgrad_slices=out[9], wgrad_items=out[10], wgrad_item_blocks=out[11], pixels_per_range=out[12],
+                ranges=out[13], n_acc=out[14], lanes=out[15])
 
 
 def se_scale_nhwc_info(N, H, W, C):

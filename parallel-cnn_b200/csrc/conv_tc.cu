@@ -243,6 +243,7 @@ struct pcnn_conv_plan {
     ConvWidePlan *wide = nullptr;   // non-null: a plan of pcnn_conv_wide_plan_create (conv_wide_tc.cu), nothing above is used
     LinearPlan *linear = nullptr;   // non-null: a plan of pcnn_linear_plan_create (linear_tc.cu), nothing above is used
     DwConvPlan *dw = nullptr;       // non-null: a plan of pcnn_dwconv_plan_create (dwconv_nhwc.cu), nothing above is used
+    GConvPlan *gc = nullptr;        // non-null: a plan of pcnn_gconv_plan_create (gconv_nhwc.cu), nothing above is used
 };
 
 pcnn_conv_plan *conv_plan_wrap_wide(ConvWidePlan *w) {
@@ -267,10 +268,19 @@ pcnn_conv_plan *conv_plan_wrap_dw(DwConvPlan *d) {
 
 DwConvPlan *conv_plan_dw(pcnn_conv_plan *plan) { return plan->dw; }
 
+pcnn_conv_plan *conv_plan_wrap_gconv(GConvPlan *g) {
+    pcnn_conv_plan *pl = new pcnn_conv_plan();
+    pl->gc = g;
+    return pl;
+}
+
+GConvPlan *conv_plan_gconv(pcnn_conv_plan *plan) { return plan->gc; }
+
 void conv_plan_operand(pcnn_conv_plan *plan, PlanOperand *out) {
     if (plan->wide) return conv_wide_operand(plan->wide, out);
     if (plan->linear) return linear_operand(plan->linear, out);
     if (plan->dw) return dwconv_operand(plan->dw, out);
+    if (plan->gc) return gconv_operand(plan->gc, out);
     const ConvTcParams &p = plan->p;
     *out = PlanOperand{nullptr, 0, 0, (long long)p.K * p.R * plan->S * p.C, plan->d_bias, p.K};
 }
@@ -289,6 +299,7 @@ static void free_plan(pcnn_conv_plan *plan) {
     if (plan->wide) conv_wide_free(plan->wide);
     if (plan->linear) linear_free(plan->linear);
     if (plan->dw) dwconv_free(plan->dw);
+    if (plan->gc) gconv_free(plan->gc);
     if (plan->d_toeplitz) cudaFree(plan->d_toeplitz);
     if (plan->d_bias) cudaFree(plan->d_bias);
     delete plan;
@@ -431,6 +442,7 @@ extern "C" int pcnn_conv_plan_set_params(pcnn_ctx *ctx, pcnn_conv_plan *plan, co
         const int rc = plan->wide     ? conv_wide_load_filters(ctx, plan->wide, filt_f32_dev)
                        : plan->linear ? linear_load_weights(ctx, plan->linear, filt_f32_dev)
                        : plan->dw     ? dwconv_load_filters(ctx, plan->dw, filt_f32_dev)
+                       : plan->gc     ? gconv_load_filters(ctx, plan->gc, filt_f32_dev)
                                       : conv_tc_load_filters(ctx, plan, filt_f32_dev);
         if (rc) return rc;
     }
@@ -445,6 +457,7 @@ extern "C" int pcnn_conv_tc_fwd(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void 
     if (plan->wide) return conv_wide_fwd(ctx, plan->wide, x_bf16, y_bf16);
     if (plan->linear) return linear_fwd(ctx, plan->linear, x_bf16, y_bf16);
     if (plan->dw) return dwconv_fwd(ctx, plan->dw, x_bf16, y_bf16);
+    if (plan->gc) return gconv_fwd(ctx, plan->gc, x_bf16, y_bf16);
     ConvTcParams p = plan->p;
     p.y = reinterpret_cast<__nv_bfloat16 *>(y_bf16);
     CUtensorMap map_x;

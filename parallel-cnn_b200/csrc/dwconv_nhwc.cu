@@ -226,8 +226,9 @@ __global__ void __launch_bounds__(DW_THREADS) k_dwconv_wgrad(const __nv_bfloat16
     }
 }
 
-// the domain of pcnn.h, refused with PCNN_ERR_ARG and a message naming `fn`, and the partition, a function of the shape alone
-int dw_shape(const char *fn, int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, DwArgs *a) {
+}  // namespace
+
+int nhwc_window_check(const char *fn, int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int *P, int *Q) {
     PCNN_REQUIRE(N >= 1 && H >= 1 && W >= 1 && C >= 1, PCNN_ERR_ARG, "%s: N = %d, H = %d, W = %d, C = %d: each must be >= 1", fn, N, H, W,
                  C);
     PCNN_REQUIRE(R >= 1 && R <= DW_MAX_TAPS && S >= 1 && S <= DW_MAX_TAPS, PCNN_ERR_ARG, "%s: %dx%d filter: 1 <= R, S <= 7 is required",
@@ -239,7 +240,18 @@ int dw_shape(const char *fn, int N, int H, int W, int C, int R, int S, int strid
     PCNN_REQUIRE(H + 2 * pad_h >= R && W + 2 * pad_w >= S, PCNN_ERR_ARG,
                  "%s: a %dx%d filter does not fit the %dx%d image padded by (%d, %d): H + 2 pad_h >= R and W + 2 pad_w >= S are required",
                  fn, R, S, H, W, pad_h, pad_w);
-    const int P = (H + 2 * pad_h - R) / stride + 1, Q = (W + 2 * pad_w - S) / stride + 1;
+    *P = (H + 2 * pad_h - R) / stride + 1;
+    *Q = (W + 2 * pad_w - S) / stride + 1;
+    return PCNN_OK;
+}
+
+namespace {
+
+// the domain of pcnn.h, refused with PCNN_ERR_ARG and a message naming `fn`, and the partition, a function of the shape alone
+int dw_shape(const char *fn, int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, DwArgs *a) {
+    int P, Q;
+    const int rc = nhwc_window_check(fn, N, H, W, C, R, S, stride, pad_h, pad_w, &P, &Q);
+    if (rc) return rc;
     PCNN_REQUIRE((long)H * W * C <= INT32_MAX && (long)P * Q * C <= INT32_MAX && (long)C * R * S <= INT32_MAX, PCNN_ERR_ARG,
                  "%s: one %dx%dx%d image (or its %d x %d x %d filters) exceeds the 32-bit index range: H W C, P Q C and C R S < 2^31 are "
                  "required", fn, H, W, C, C, R, S);

@@ -266,6 +266,18 @@ void dwconv_operand(DwConvPlan *d, PlanOperand *out);
 int dwconv_load_filters(pcnn_ctx *ctx, DwConvPlan *d, const float *filt_dev);
 pcnn_conv_plan *conv_plan_wrap_dw(DwConvPlan *d);   // conv_tc.cu; takes ownership
 DwConvPlan *conv_plan_dw(pcnn_conv_plan *plan);
+// the window rules the depthwise and the grouped convolutions share (dwconv_nhwc.cu): N, H, W, C >= 1, 1 <= R, S <= 7, stride 1..4,
+// 0 <= pad <= taps - 1 and a window that fits; refused with PCNN_ERR_ARG and a message naming `fn`; P and Q on success
+int nhwc_window_check(const char *fn, int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int *P, int *Q);
+// gconv_nhwc.cu: a plan of pcnn_gconv_plan_create holds a GConvPlan, run, refreshed and freed like the depthwise one; its bf16
+// operand is [K][R][S][Cg], the fp32 master's element order (one row of K R S Cg elements); conv_plan_gconv is null for any other plan
+struct GConvPlan;
+int gconv_fwd(pcnn_ctx *ctx, const GConvPlan *g, const void *x_bf16, void *y_bf16);
+void gconv_free(GConvPlan *g);
+void gconv_operand(GConvPlan *g, PlanOperand *out);
+int gconv_load_filters(pcnn_ctx *ctx, GConvPlan *g, const float *filt_dev);
+pcnn_conv_plan *conv_plan_wrap_gconv(GConvPlan *g);   // conv_tc.cu; takes ownership
+GConvPlan *conv_plan_gconv(pcnn_conv_plan *plan);
 // a temporary device copy of host data (the create calls upload their filters through one); freed when it goes out of scope
 struct pcnn_dev_temp {
     float *p = nullptr;

@@ -5,7 +5,7 @@ import ctypes as C
 import numpy as np
 
 from ._lib import (F32, NPARAM, OPTIM_ADAMW, OPTIM_SGD, TEST_SET, TRAIN_SET, U8, OptimConfig, OptimTensor, PcnnError, avgpool_nhwc_info,
-                   batchnorm_nhwc_info, check, conv_layer_family, dwconv_info, global_avgpool_nhwc_info, lib, linear_info, maxpool_nhwc_info,
+                   batchnorm_nhwc_info, check, conv_layer_family, dwconv_info, gconv_info, global_avgpool_nhwc_info, lib, linear_info, maxpool_nhwc_info,
                    se_scale_nhwc_info, ACT_RELU, ACT_SIGMOID, ACT_SILU, ACT_HARDSWISH, ACT_RELU6)
 
 PREACT_CODES = (ACT_SILU, ACT_HARDSWISH, ACT_RELU6)   # batch normalization's codes whose backward recomputes the pre-activation
@@ -510,6 +510,15 @@ class Engine:
         """pcnn_dwconv_dgrad: dx dense bf16 [N][H][W][C] from dy with the plan's bf16 filters, every element written"""
         self._call("pcnn_dwconv_dgrad", plan.plan, _p(dy), _p(dx))
 
+    def gconv_wgrad(self, plan, x, dy, dw):
+        """pcnn_gconv_wgrad: dw fp32 [K][R][S][Cg] = the sum over the pixels of dy * x of the filter's group (x +0 outside the image),
+        overwritten; the shape from the GroupedConvPlan"""
+        self._call("pcnn_gconv_wgrad", plan.plan, _p(x), _p(dy), _p(dw))
+
+    def gconv_dgrad(self, plan, dy, dx):
+        """pcnn_gconv_dgrad: dx dense bf16 [N][H][W][C] from dy with the plan's bf16 filters, every element written"""
+        self._call("pcnn_gconv_dgrad", plan.plan, _p(dy), _p(dx))
+
     def se_scale_fwd(self, x, s, y, N, H, W, Cin, r=None, act=0):
         """pcnn_se_scale_nhwc_bf16_fwd: y = bf16(act(x * s[n][c] (+ r))) over dense bf16 [N][H][W][C], s dense bf16 [N][C] (a
         LinearLayer's y with O = C); act ACT_NONE or ACT_RELU"""
@@ -632,6 +641,26 @@ class DepthwiseConvPlan(ConvPlan):
                                             None if b is None else b.ctypes.data, C_.byref(plan)))
         self.plan = plan
         self.out_shape = (N, (H + 2 * ph - R) // stride + 1, (W + 2 * pw - S) // stride + 1, C)
+
+
+class GroupedConvPlan(ConvPlan):
+    """A grouped convolution's plan (pcnn_gconv_plan_create): conv2d(x, w, b, stride, padding, groups=G) with x dense bf16
+    [N][H][W][C], y dense bf16 [N][P][Q][K], filters fp32 [K][R][S][Cg] (torch's weight [K][Cg][R][S] permuted), bias fp32 [K].  act
+    ACT_NONE (0) or ACT_RELU (3).  Run, refreshed and closed like ConvPlan; its gradients are Engine.gconv_wgrad / gconv_dgrad."""
+
+    def __init__(self, engine, N, H, W, C, K, G, R, S, filt, bias=None, act=0, stride=1, padding=(0, 0)):
+        self.engine = engine
+        self.shape = (N, H, W, C, K, G, R, S)
+        ph, pw = (int(v) for v in padding)
+        filt = np.ascontiguousarray(filt, np.float32)
+        assert G >= 1 and filt.size == K * R * S * (C // G)
+        b = None if bias is None else np.ascontiguousarray(bias, np.float32)
+        plan = C_.c_void_p()
+        check("pcnn_gconv_plan_create",
+              lib().pcnn_gconv_plan_create(engine.ctx, N, H, W, C, K, G, R, S, int(stride), ph, pw, int(act), filt.ctypes.data,
+                                           None if b is None else b.ctypes.data, C_.byref(plan)))
+        self.plan = plan
+        self.out_shape = (N, (H + 2 * ph - R) // stride + 1, (W + 2 * pw - S) // stride + 1, K)
 
 
 class ConvLayer:
@@ -772,6 +801,80 @@ class DepthwiseConvLayer:
 
     def params(self):
         """host copies (filters [C][R][S], bias [C] or None) of the fp32 masters"""
+        return self.filt.to_host(), None if self.bias is None else self.bias.to_host()
+
+    def close(self):
+        self.plan.close()
+        for a in (self.filt, self.bias, self.dw, self.db):
+            if a is not None:
+                a.free()
+
+
+class GroupedConvLayer:
+    """A grouped convolution trained on the device (groups = G: each group of C / G input channels feeds its own K / G filters), with
+    ConvLayer's interface: fp32 masters filt [K][R][S][Cg] and bias [K], their gradients dw and db, and a GroupedConvPlan holding the
+    filters in bf16.  x and dx are dense bf16 [N][H][W][C], y and dy dense [N][P][Q][K]: what a ConvLayer or a BatchNormLayer writes
+    and reads, so a ResNeXt bottleneck runs with no copies:
+
+        reduce.forward(x, yr);  bn1.forward(yr, zr);  grouped.forward(zr, yg);  bn2.forward(yg, zg);  expand.forward(zg, ye)
+        ...;  bn2.backward(zg, dzg, dyg);  grouped.backward(yg, dyg, dzr);  bn1.backward(zr, dzr, dyr)
+
+    act ACT_RELU (3) is a ReLU after the bias, ACT_NONE (0) none; the sigmoid is refused.  With a bias or an activation, backward
+    first runs pcnn_conv_bias_act_bwd over dy, which takes at most 256 channels: such a layer needs K <= 256 and is refused
+    otherwise.  Without either (the usual case in front of a batch norm) C and K are unlimited."""
+
+    def __init__(self, engine, N, H, W, C, K, G, R, S, filt, bias=None, act=0, stride=1, padding=(0, 0)):
+        if (int(act) or bias is not None) and K > 256:
+            raise PcnnError("GroupedConvLayer", -1, f"K = {K} with a bias or an activation: the bias / activation backward "
+                            "(pcnn_conv_bias_act_bwd) takes K <= 256; put a BatchNormLayer after a layer with no bias and act 0")
+        self.engine = engine
+        self.shape = (N, H, W, C, K, G, R, S)
+        self.act, self.stride = int(act), int(stride)
+        self.padding = tuple(int(v) for v in padding)
+        self.info = gconv_info(N, H, W, C, K, G, R, S, self.stride, self.padding)
+        Cg = self.info["Cg"]
+        filt = np.ascontiguousarray(filt, np.float32).reshape(K, R, S, Cg)
+        bias = None if bias is None else np.ascontiguousarray(bias, np.float32).reshape(K)
+        self.plan = GroupedConvPlan(engine, N, H, W, C, K, G, R, S, filt, bias, act=act, stride=self.stride, padding=self.padding)
+        self.out_shape = self.plan.out_shape
+        self.pixels = int(np.prod(self.out_shape[:3]))
+        self.filt = DeviceArray.from_host(engine, filt)
+        self.bias = None if bias is None else DeviceArray.from_host(engine, bias)
+        self.dw = engine.array((K, R, S, Cg))
+        self.db = None if bias is None else engine.array(K)
+        self._x = None
+
+    def forward(self, x, y):
+        """y = act(gconv(x) + bias) with the plan's bf16 filters.  The layer keeps x: backward's weight gradient reads it."""
+        self.plan.fwd(x, y)
+        self._x = x
+
+    def backward(self, y, dy, dx=None):
+        """Gradients of the most recent forward, whose output y was: dw, db (with a bias) and dx (when given).  dy is CONSUMED with
+        a ReLU: it is overwritten in place by the gradient at the pre-activation (pcnn_conv_bias_act_bwd, skipped without
+        activation and bias).  dx uses the plan's bf16 filters, so call it before sgd or an optimizer step."""
+        K = self.shape[4]
+        e = self.engine
+        if self.act or self.bias is not None:
+            e.conv_bias_act_bwd(y if self.act else None, dy, dy if self.act else None, self.db, self.pixels, K, self.act)
+        e.gconv_wgrad(self.plan, self._x, dy, self.dw)
+        if dx is not None:
+            e.gconv_dgrad(self.plan, dy, dx)
+
+    def sgd(self, lr):
+        """w += (-lr) * dw and b += (-lr) * db in fp32 on the masters, then the plan refreshed from them, all on the engine's stream"""
+        K, R, S = self.shape[4], self.shape[6], self.shape[7]
+        self.engine.apply_grad_scaled(self.filt, self.dw, K * R * S * self.info["Cg"], -lr)
+        if self.bias is not None:
+            self.engine.apply_grad_scaled(self.bias, self.db, K, -lr)
+        self.plan.set_params(self.filt, self.bias)
+
+    def optim_tensors(self):
+        """(param, grad, plan, plan part, is norm or bias) of the filters and the bias, as ConvLayer.optim_tensors"""
+        return [(self.filt, self.dw, self.plan, 1, False)] + ([] if self.bias is None else [(self.bias, self.db, self.plan, 2, True)])
+
+    def params(self):
+        """host copies (filters [K][R][S][Cg], bias [K] or None) of the fp32 masters"""
         return self.filt.to_host(), None if self.bias is None else self.bias.to_host()
 
     def close(self):
@@ -1184,7 +1287,7 @@ def _layer_tensors(layers, weight_decay, decay_norm_and_bias):
 
 
 class SGD(FusedOptimizer):
-    """torch.optim.SGD over the trainable tensors of ConvLayers, DepthwiseConvLayers, LinearLayers, BatchNormLayers and
+    """torch.optim.SGD over the trainable tensors of ConvLayers, DepthwiseConvLayers, GroupedConvLayers, LinearLayers, BatchNormLayers and
     SqueezeExcitationLayers, in one launch
     per step with the layers' plans refreshed: step(lr) replaces every layer.sgd(lr) of a training step (momentum 0 and weight decay 0 give the same
     bits).  decay_norm_and_bias=False gives batch normalization's gamma and beta and the biases weight decay 0; the default decays

@@ -929,6 +929,112 @@ def run_mbblock(N, iters, k=3):
         layer.close()
 
 
+def run_gconv(name, N, H, W, C, K, G, R, stride, pad, iters):
+    """the three passes of a grouped convolution (pcnn_conv_tc_fwd on a GroupedConvPlan, pcnn_gconv_dgrad, pcnn_gconv_wgrad) next
+    to F.conv2d(groups=G) and aten.convolution_backward on the same bf16 channels-last tensors.  The bound of each pass is the larger
+    of two times: bytes N (H W C + P Q K) 2 (x and y, or dy and dx, or x and dy crossing HBM once; the weight gradient adds its fp32
+    slots, written and read once, and dw) over 3.35 TB/s, and 2 N P Q K Cg R S FLOPs over the 67 TFLOP/s fp32 data-sheet rate."""
+    info = pkg.gconv_info(N, H, W, C, K, G, R, R, stride, (pad, pad))
+    P, Q, Cg = info["P"], info["Q"], info["Cg"]
+    w = rng.uniform(-0.5, 0.5, (K, R, R, Cg)).astype(np.float32)
+    plan = pkg.GroupedConvPlan(eng, N, H, W, C, K, G, R, R, w, None, act=0, stride=stride, padding=(pad, pad))
+    bits = lambda *shape: torch.randint(0, 0x3F80, shape, dtype=torch.int16, device="cuda")
+    x, dy = bits(N, H, W, C), bits(N, P, Q, K)
+    y, dx = torch.empty((N, P, Q, K), dtype=torch.int16, device="cuda"), torch.empty((N, H, W, C), dtype=torch.int16, device="cuda")
+    dw = torch.empty((K, R, R, Cg), dtype=torch.float32, device="cuda")
+    gpu, power = card()
+    act_bytes = N * (H * W * C + P * Q * K) * 2
+    nw = K * R * R * Cg
+    slot_bytes = (2 * info["ranges"] * nw * 4 if info["ranges"] > 1 else 0) + nw * 4
+    flops = 2.0 * N * P * Q * K * Cg * R * R
+    xt = x.view(torch.bfloat16).permute(0, 3, 1, 2)
+    dyt = dy.view(torch.bfloat16).permute(0, 3, 1, 2)
+    wt = torch.from_numpy(w).to("cuda").to(torch.bfloat16).permute(0, 3, 1, 2).contiguous(memory_format=torch.channels_last)
+    F = torch.nn.functional
+    cb = torch.ops.aten.convolution_backward
+    passes = (
+        ("fwd", lambda: plan.fwd(x, y), lambda: F.conv2d(xt, wt, None, stride, pad, groups=G), act_bytes),
+        ("dgrad", lambda: eng.gconv_dgrad(plan, dy, dx),
+         lambda: cb(dyt, xt, wt, None, [stride] * 2, [pad] * 2, [1, 1], False, [0, 0], G, [True, False, False]), act_bytes),
+        ("wgrad", lambda: eng.gconv_wgrad(plan, x, dy, dw),
+         lambda: cb(dyt, xt, wt, None, [stride] * 2, [pad] * 2, [1, 1], False, [0, 0], G, [False, True, False]), act_bytes + slot_bytes),
+    )
+    for what, ours, theirs, nbytes in passes:
+        ms, ms_torch = timed(ours, iters), timed(theirs, iters)
+        t_mem, t_flop = nbytes / (HBM * 1e9), flops / 67e12
+        print(json.dumps({"case": f"gconv {name} {what}", "N": N, "us": ms * 1e3, "MB": nbytes / 1e6, "GFLOP": flops / 1e9,
+                          "share_of_bound": max(t_mem, t_flop) / (ms * 1e-3), "bound": "HBM" if t_mem >= t_flop else "fp32",
+                          "torch_us": ms_torch * 1e3, "torch_over_ours": ms_torch / ms, "Cg": Cg, "Kg": info["Kg"], "vec": info["vec"],
+                          "kt": info["kt"], "wgrad_ranges": info["ranges"], "gpu": gpu, "power_limit": power}), flush=True)
+    plan.close()
+
+
+def run_resnextblock(N, iters):
+    """one training step of a ResNeXt bottleneck at 56x56x256, N = 128: 1x1 reduce to 128 -> BN + ReLU -> grouped 3x3 pad 1, G = 32
+    (Cg = 4) -> BN + ReLU -> 1x1 expand to 256 -> BN + x0 -> ReLU, its backward (the shortcut's gradient dres left apart, as
+    run_resblock) and the sgd of the six layers, on the engine's stream.  Next to it the torch eager step of the same block on bf16
+    channels-last tensors (fp32 masters, w -= lr * grad, re-cast to bf16)."""
+    H = W = 56
+    C, Dm, G = 256, 128, 32
+    r = np.random.default_rng(13)
+    u = lambda shape, fan: r.uniform(-1, 1, shape).astype(np.float32) / np.float32(np.sqrt(fan))
+    fr, fg, fe = u((Dm, 1, 1, C), C), u((Dm, 3, 3, Dm // G), 9 * Dm // G), u((C, 1, 1, Dm), Dm)
+    rd = pkg.ConvLayer(eng, N, H, W, C, Dm, 1, 1, fr, None, act=0)
+    gl = pkg.GroupedConvLayer(eng, N, H, W, Dm, Dm, G, 3, 3, fg, None, act=0, padding=(1, 1))
+    ex = pkg.ConvLayer(eng, N, H, W, Dm, C, 1, 1, fe, None, act=0)
+    b1, b2 = pkg.BatchNormLayer(eng, N, H, W, Dm, act=pkg.ACT_RELU), pkg.BatchNormLayer(eng, N, H, W, Dm, act=pkg.ACT_RELU)
+    b3 = pkg.BatchNormLayer(eng, N, H, W, C, act=pkg.ACT_RELU)
+    mid = lambda: torch.empty((N, H, W, Dm), dtype=torch.int16, device="cuda")
+    full = lambda: torch.empty((N, H, W, C), dtype=torch.int16, device="cuda")
+    x0 = torch.randint(0, 0x3F80, (N, H, W, C), dtype=torch.int16, device="cuda")
+    dout = torch.randint(0, 0x3F80, (N, H, W, C), dtype=torch.int16, device="cuda")
+    dout ^= torch.randint(0, 2, (N, H, W, C), dtype=torch.int16, device="cuda") << 15
+    yr, zr, yg, zg, dzg, dyg, dzr, dyr = (mid() for _ in range(8))
+    ye, out, dye, dres, dx0 = (full() for _ in range(5))
+    lr = 0.05
+    gpu, power = card()
+
+    def step():
+        rd.forward(x0, yr); b1.forward(yr, zr); gl.forward(zr, yg); b2.forward(yg, zg); ex.forward(zg, ye); b3.forward(ye, out, r=x0)
+        b3.backward(out, dout, dye, dr=dres); ex.backward(ye, dye, dzg); b2.backward(zg, dzg, dyg); gl.backward(yg, dyg, dzr)
+        b1.backward(zr, dzr, dyr); rd.backward(yr, dyr, dx0)
+        for layer in (rd, b1, gl, b2, ex, b3):
+            layer.sgd(lr)
+
+    ms = timed(step, iters)
+    F = torch.nn.functional
+    xt = x0.view(torch.bfloat16).permute(0, 3, 1, 2).detach().requires_grad_(True)
+    dt = dout.view(torch.bfloat16).permute(0, 3, 1, 2)
+    cl = lambda a: torch.from_numpy(np.ascontiguousarray(a.transpose(0, 3, 1, 2))).to("cuda").contiguous(memory_format=torch.channels_last)
+    m32 = {"fr": cl(fr), "fg": cl(fg), "fe": cl(fe)}
+    for i, ch in ((1, Dm), (2, Dm), (3, C)):
+        m32[f"g{i}"], m32[f"b{i}"] = torch.ones(ch, device="cuda"), torch.zeros(ch, device="cuda")
+    mb = {kk: (v.to(torch.bfloat16) if kk.startswith("f") else v.clone()).requires_grad_(True) for kk, v in m32.items()}
+    stats = [torch.zeros(ch, device="cuda") if j % 2 == 0 else torch.ones(ch, device="cuda") for ch in (Dm, Dm, C) for j in range(2)]
+
+    def torch_step():
+        for v in mb.values():
+            v.grad = None
+        xt.grad = None
+        h = torch.relu(F.batch_norm(F.conv2d(xt, mb["fr"]), stats[0], stats[1], mb["g1"], mb["b1"], training=True))
+        h = torch.relu(F.batch_norm(F.conv2d(h, mb["fg"], padding=1, groups=G), stats[2], stats[3], mb["g2"], mb["b2"], training=True))
+        h = torch.relu(F.batch_norm(F.conv2d(h, mb["fe"]), stats[4], stats[5], mb["g3"], mb["b3"], training=True) + xt)
+        h.backward(dt)
+        with torch.no_grad():
+            for kk in m32:
+                m32[kk].add_(mb[kk].grad.float(), alpha=-lr)
+                mb[kk].copy_(m32[kk])
+
+    ms_torch = timed(torch_step, iters)
+    ms_g = {"fwd": timed(lambda: gl.forward(zr, yg), iters), "bwd": timed(lambda: (eng.gconv_wgrad(gl.plan, zr, dyg, gl.dw),
+                                                                                    eng.gconv_dgrad(gl.plan, dyg, dzr)), iters)}
+    print(json.dumps({"case": f"ResNeXt bottleneck 56x56x256 -> 128 G{G} training step N={N}", "ms": ms, "torch_eager_ms": ms_torch,
+                      "ours_over_torch": ms / ms_torch, "grouped_fwd_ms": ms_g["fwd"], "grouped_bwd_ms": ms_g["bwd"],
+                      "families": [rd.family, ex.family], "gpu": gpu, "power_limit": power}), flush=True)
+    for layer in (rd, b1, gl, b2, ex, b3):
+        layer.close()
+
+
 def run_se(name, N, H, W, C, iters):
     """the three squeeze-and-excitation passes (pcnn_se_scale_nhwc_bf16_fwd / _bwd_gate / _bwd_input) next to torch eager on the
     same bf16 channels-last tensors.  Bytes per pass, each [N][H][W][C] tensor crossing HBM once: forward x and y (plus r), gate
@@ -1181,6 +1287,19 @@ if only == "dwconv":                                                   # depthwi
 if only == "mbblock":                                                  # one step of an inverted-residual block, torch eager beside it
     run_mbblock(128, 20, 3)
     run_mbblock(128, 20, 5)
+if only == "gconv":                                                    # grouped convolution passes, torch beside them
+    for args in (("resnext 56x56x128 G32 3x3/1", 128, 56, 56, 128, 128, 32, 3, 1, 1),
+                 ("resnext 56x56x256->28x28 G32 3x3/2", 128, 56, 56, 256, 256, 32, 3, 2, 1),
+                 ("resnext 28x28x256 G32 3x3/1", 128, 28, 28, 256, 256, 32, 3, 1, 1),
+                 ("resnext 14x14x512 G32 3x3/1 (Cg 16)", 128, 14, 14, 512, 512, 32, 3, 1, 1),
+                 ("resnext 7x7x1024 G32 3x3/1 (Cg 32)", 128, 7, 7, 1024, 1024, 32, 3, 1, 1),
+                 ("regnet 28x28x64 G4 3x3/1 (Cg 16)", 128, 28, 28, 64, 64, 4, 3, 1, 1),
+                 ("regnet 7x7x384 G24 3x3/1 (Cg 16)", 128, 7, 7, 384, 384, 24, 3, 1, 1),
+                 ("multiplier 56x56x32->64 G32 3x3/1", 128, 56, 56, 32, 64, 32, 3, 1, 1),
+                 ("shufflenet 28x28x384 G8 1x1", 128, 28, 28, 384, 384, 8, 1, 1, 0)):
+        run_gconv(*args, 20)
+if only == "resnextblock":                                             # one step of a ResNeXt bottleneck, torch eager beside it
+    run_resnextblock(128, 20)
 if only == "optim":                                                    # the fused optimizers over the ResNet-18 table, torch beside them
     run_optim(50)
 if only == "resnetgap-optim":                                          # the GAP ResNet step with each update, alternated
