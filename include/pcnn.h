@@ -752,6 +752,33 @@ int pcnn_se_scale_nhwc_bf16_bwd_gate(pcnn_ctx *ctx, const void *x_bf16_dev, cons
 int pcnn_se_scale_nhwc_bf16_bwd_input(pcnn_ctx *ctx, const void *g_bf16_dev, const void *s_bf16_dev, const void *dpool_bf16_dev,
                                       int dpool_row_pitch, void *dx_bf16_dev, int N, int H, int W, int C);
 int pcnn_se_scale_nhwc_info(int N, int H, int W, int C, int *out8);
+/* Dropout and stochastic depth (csrc/dropout.cu): y = x * m (+ r) with m = 0 for a dropped element and 1 / (1 - p) for a kept one,
+ * as torch's dropout (element mode) and the drop path of EfficientNet's residual blocks (per-sample mode: one draw per image).
+ *   - x, r and y are bf16 arrays of N rows of row_elems elements, consecutive rows row_pitch elements apart (row_pitch 0 = dense,
+ *     otherwise >= row_elems).  A dense NHWC activation is N rows of H W C; a global average pool's output is N rows of C at its
+ *     row pitch; a dense linear layer's output [N][O] is N rows of O.  The pad (elements row_elems .. row_pitch - 1 of a row) is
+ *     never read or written.
+ *   - Index: element j of row n is i = n row_elems + j in element mode (per_sample 0) and i = n in per-sample mode (per_sample 1).
+ *     It depends on neither the pitch nor the grid nor the SM count: the same arguments give the same bits on every H100.
+ *   - Generator: Philox4x32-10 (Salmon et al., SC'11, as Random123) with key (seed lo, seed hi) and counter (q lo, q hi, call lo,
+ *     call hi), q = i >> 2; the draw of element i is output word i & 3.  Element i is dropped iff draw < T, T = the uint32 nearest
+ *     to p 2^32 (ties to even; p 2^32 above 2^32 - 1/2 gives 2^32 - 1), so the keep probability is 1 - T / 2^32: one 32-bit draw
+ *     per element, as torch.  scale = fp32(1 / (1 - p)) evaluated in double and rounded once.  Both are formed on the host and
+ *     reported by pcnn_dropout_bf16_info.  p = 0 gives T = 0 and scale 1, and a kernel without the generator.
+ *   - Values, fp32 round to nearest with no contraction: m = dropped ? 0.0f : scale; without r y = bf16_rn(float(x) * m); with r
+ *     y = bf16_rn(float(r) + RN(float(x) * m)).  A product rather than a select, as torch's native_dropout: a dropped NaN stays
+ *     NaN, a dropped Inf gives NaN, a dropped -x gives -0 (and r + -0 = r).
+ *   - Backward: dx is this call on dy with the forward's (seed, call, p, per_sample) and no r.  The gradient of r is dy itself.
+ *   - y == x and y == r (in place) are allowed; x, r and y must each be the same buffer or share no byte.
+ * Domain (anything else is PCNN_ERR_ARG with the function and the rule in the message): N, row_elems >= 1; row_pitch 0 or
+ * >= row_elems; p finite with 0 <= p < 1; per_sample 0 or 1; x and y not NULL; every pointer 16-byte aligned.  With row_elems % 8
+ * == 0 and row_pitch % 8 == 0 the kernel moves 16-byte vectors of 8 elements of a row (two Philox calls each in element mode, one
+ * in per-sample mode), otherwise single elements.  Stream-ordered; a grid-stride loop whose grid depends on the shape alone.
+ * pcnn_dropout_bf16_info: host only (no GPU, no context), refused as the call refuses.  out5 = { T, the bits of scale, elements per
+ * vector (8 or 1), the grid (CTAs of 256 threads), elements of the busiest thread }. */
+int pcnn_dropout_bf16(pcnn_ctx *ctx, const void *x_bf16_dev, const void *r_bf16_dev, void *y_bf16_dev, int N, int row_elems, int row_pitch,
+                      double p, int per_sample, unsigned long long seed, unsigned long long call);
+int pcnn_dropout_bf16_info(int N, int row_elems, int row_pitch, double p, int per_sample, long long *out5);
 /* Softmax cross-entropy on bf16 logits [N][O], 1 <= O <= 256, labels uint8 [N]:
  *   p = softmax(row) evaluated in double: m = max, den = sum exp(z - m), p_t = exp(z_t - m) / den;
  *   dlogits[n][t] = bf16_rn(float_rn((p_t - [t == label]) * scale)), double -> fp32 -> bf16, each round to nearest even: the

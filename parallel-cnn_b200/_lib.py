@@ -179,6 +179,8 @@ _SIG = {
     "pcnn_se_scale_nhwc_bf16_bwd_gate": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i],
     "pcnn_se_scale_nhwc_bf16_bwd_input": [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i],
     "pcnn_se_scale_nhwc_info": [_i, _i, _i, _i, _vp],
+    "pcnn_dropout_bf16": [_vp, _vp, _vp, _vp, _i, _i, _i, C.c_double, _i, C.c_ulonglong, C.c_ulonglong],
+    "pcnn_dropout_bf16_info": [_i, _i, _i, C.c_double, _i, _vp],
     "pcnn_softmax_ce_bf16": [_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp],
     "pcnn_optim_create": [_vp, _vp, _vp, _i, _pvp],
     "pcnn_optim_step": [_vp, _vp, _f],
@@ -377,6 +379,15 @@ def se_scale_nhwc_info(N, H, W, C):
     check("pcnn_se_scale_nhwc_info", lib().pcnn_se_scale_nhwc_info(int(N), int(H), int(W), int(C), out))
     return dict(vec=out[0], groups_per_cta=out[1], slices=out[2], lanes=out[3], pixels_per_cta=out[4], ranges=out[5], ctas=out[6],
                 n_acc=out[7])
+
+
+def dropout_info(N, row_elems, row_pitch=0, p=0.0, per_sample=False):
+    """The mask rule and the launch of the dropout kernel (pcnn_dropout_bf16_info; host only, no GPU), refused as pcnn_dropout_bf16
+    refuses.  row_pitch 0 = dense.  T: an element is dropped iff its Philox draw < T; scale_bits: the fp32 bits of 1 / (1 - p);
+    vec: elements per vector (8 is the 16-byte path); grid: CTAs of 256 threads; per_thread: elements of the busiest thread."""
+    out = (C.c_longlong * 5)()
+    check("pcnn_dropout_bf16_info", lib().pcnn_dropout_bf16_info(int(N), int(row_elems), int(row_pitch), float(p), int(per_sample), out))
+    return dict(T=out[0], scale_bits=out[1], vec=out[2], grid=out[3], per_thread=out[4])
 
 
 def conv_bwd_plan_info(N, H, W, C, K, R, S, stride=1):

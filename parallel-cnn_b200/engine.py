@@ -5,7 +5,8 @@ import ctypes as C
 import numpy as np
 
 from ._lib import (F32, NPARAM, OPTIM_ADAMW, OPTIM_SGD, TEST_SET, TRAIN_SET, U8, OptimConfig, OptimTensor, PcnnError, avgpool_nhwc_info,
-                   batchnorm_nhwc_info, check, conv_layer_family, dwconv_info, gconv_info, global_avgpool_nhwc_info, lib, linear_info, maxpool_nhwc_info,
+                   batchnorm_nhwc_info, check, conv_layer_family, dropout_info, dwconv_info, gconv_info, global_avgpool_nhwc_info, lib, linear_info,
+                   maxpool_nhwc_info,
                    se_scale_nhwc_info, ACT_RELU, ACT_SIGMOID, ACT_SILU, ACT_HARDSWISH, ACT_RELU6)
 
 PREACT_CODES = (ACT_SILU, ACT_HARDSWISH, ACT_RELU6)   # batch normalization's codes whose backward recomputes the pre-activation
@@ -536,6 +537,13 @@ class Engine:
         dpool [N][dpool_row_pitch] is the squeeze branch's gradient at the pooled x (row pitch None = C rounded up to 8)"""
         self._call("pcnn_se_scale_nhwc_bf16_bwd_input", _p(g), _p(s), _p(dpool), int(dpool_row_pitch or 0), _p(dx), int(N), int(H), int(W),
                    int(Cin))
+
+    def dropout(self, x, y, N, row_elems, p, seed, call, per_sample=False, r=None, row_pitch=None):
+        """pcnn_dropout_bf16: y = bf16(x * m (+ r)) over N bf16 rows of row_elems elements, row_pitch apart (None = dense), m = 0 or
+        1 / (1 - p) from the Philox draw of (seed, call) at each element (per_sample False) or each row (True).  y may be x or r.
+        The backward is the same call on dy with the forward's (p, seed, call, per_sample) and no r."""
+        self._call("pcnn_dropout_bf16", _p(x), _p(r), _p(y), int(N), int(row_elems), int(row_pitch or 0), float(p), int(per_sample),
+                   int(seed), int(call))
 
 
 class ConvPlan:
@@ -1130,6 +1138,55 @@ class GlobalAvgPoolLayer:
 
         with dh in h's layout (its pad never read) and dz dense [N][H][W][C]."""
         self.engine.global_avgpool_nhwc_bwd(dy, dx, *self.shape, self.row_pitch)
+
+    def close(self):
+        pass
+
+
+class DropoutLayer:
+    """Dropout (per_sample False: each element dropped with probability p) or stochastic depth (per_sample True: each row, an
+    image, dropped whole) on the device (pcnn_dropout_bf16): y = x * m (+ r), m = 0 or 1 / (1 - p).  x, r, y, dy and dx are N bf16
+    rows of row_elems elements, row_pitch apart (None = dense): a dense NHWC activation (row_elems = H*W*C), a GlobalAvgPoolLayer's
+    output (row_elems = C, row_pitch = gap.row_pitch) or a dense LinearLayer output [N][O].  It has no parameters, so no
+    optim_tensors.
+
+    The mask of a training forward is the Philox draw of (seed, call) at each index, call being incremented by every training
+    forward; `call` is a plain attribute, so a checkpoint can save and restore it and replay the same masks.  backward applies the
+    mask of the most recent training forward.  Dropout in place before a classifier:
+
+        gap.forward(z, h);  drop.forward(h, h);  fc.forward(h, logits)
+        fc.backward(logits, dlogits, dh);  drop.backward(dh, dh);  gap.backward(dh, dz)
+
+    Stochastic depth on a residual block: the branch's last batch norm runs without r, and the layer adds the skip path:
+
+        bn.forward(yb, b)                   # the branch's last BN, without r
+        drop.forward(b, out, r=x_in)        # out = x_in + drop_path(b)
+        drop.backward(dout, db)             # dout still feeds the skip path as dy2
+
+    dx may be dy (in place), but not when dy is still needed, as here, where dout is also the gradient of x_in."""
+
+    def __init__(self, engine, N, row_elems, p, seed, per_sample=False, row_pitch=None):
+        self.info = dropout_info(N, row_elems, row_pitch or 0, p, per_sample)
+        self.engine = engine
+        self.shape = (int(N), int(row_elems))
+        self.row_pitch = int(row_pitch or 0)
+        self.p, self.seed, self.per_sample = float(p), int(seed), bool(per_sample)
+        self.call = 0
+
+    def forward(self, x, y, r=None, training=True):
+        """training: call += 1, then y = x * m (+ r) with this call's mask.  Eval: y = x (+ r), nothing launched when y is x and
+        there is no r.  y may be x or r."""
+        if training:
+            self.call += 1
+            self.engine.dropout(x, y, *self.shape, self.p, self.seed, self.call, self.per_sample, r=r, row_pitch=self.row_pitch)
+        elif r is not None or _p(y) != _p(x):
+            self.engine.dropout(x, y, *self.shape, 0.0, self.seed, 0, False, r=r, row_pitch=self.row_pitch)
+
+    def backward(self, dy, dx):
+        """dx = dy * m, the mask of the most recent training forward (the gradient of r is dy itself).  dx may be dy."""
+        if self.call == 0:
+            raise PcnnError("DropoutLayer.backward", -1, "no training forward has drawn a mask (call = 0)")
+        self.engine.dropout(dy, dx, *self.shape, self.p, self.seed, self.call, self.per_sample, row_pitch=self.row_pitch)
 
     def close(self):
         pass

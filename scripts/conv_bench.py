@@ -1198,11 +1198,60 @@ def run_bnact(name, N, H, W, C, iters, rounds=3):
     del x, r, dy, y, dx, dr, xt, rt
 
 
-def run_mbconv(N, iters, hid=16):
+def run_dropout(name, N, H, W, C, iters, per_sample, p=0.2, rounds=3):
+    """dropout (element mode) or stochastic depth with r (per-sample mode) at p: the forward and the backward (the same call on dy,
+    without r), ours and torch's alternated over `rounds` rounds (the best of each kept), on the same bf16 channels-last tensors.
+    torch: F.dropout and aten.native_dropout_backward, which write and read a bool mask; for stochastic depth the eager
+    x * bernoulli(N, 1, 1, 1) / (1 - p) + r and dy * that multiplier.  Bytes, T = N*H*W*C*2: ours 2T each way, + T for r; torch's
+    element mode T / 2 more each way (the mask)."""
+    E = H * W * C
+    T = N * E * 2
+    rnd = lambda: torch.randint(-0x4000, 0x4000, (N, E), dtype=torch.int16, device="cuda") & 0x3FFF | 0x3C00   # bf16 in [1, 2) * 2^k
+    x, r, dy = rnd(), rnd(), rnd()
+    y, dx = torch.empty_like(x), torch.empty_like(x)
+    gpu, power = card()
+    F = torch.nn.functional
+    bf = lambda t: t.view(torch.bfloat16).reshape(N, H, W, C).permute(0, 3, 1, 2)         # channels-last NCHW views
+    xt, rt, dyt = bf(x), bf(r), bf(dy)
+    rr = r if per_sample else None
+    calls = iter(range(1, 1 << 40))
+    ours = {"fwd": lambda: eng.dropout(x, y, N, E, p, 1, next(calls), per_sample, r=rr),
+            "bwd": lambda: eng.dropout(dy, dx, N, E, p, 1, 7, per_sample)}
+    if per_sample:
+        m = torch.empty((N, 1, 1, 1), dtype=torch.bfloat16, device="cuda").bernoulli_(1 - p).div_(1 - p)
+        theirs = {"fwd": lambda: xt * torch.empty((N, 1, 1, 1), dtype=torch.bfloat16, device="cuda").bernoulli_(1 - p).div_(1 - p) + rt,
+                  "bwd": lambda: dyt * m}
+        nbytes = {"fwd": 3 * T, "bwd": 2 * T}
+        torch_bytes = nbytes
+    else:
+        _, mask = torch.ops.aten.native_dropout(xt, p, True)
+        theirs = {"fwd": lambda: F.dropout(xt, p, training=True),
+                  "bwd": lambda: torch.ops.aten.native_dropout_backward(dyt, mask, 1.0 / (1.0 - p))}
+        nbytes = {"fwd": 2 * T, "bwd": 2 * T}
+        torch_bytes = {k: v + T // 2 for k, v in nbytes.items()}
+    info = pkg.dropout_info(N, E, 0, p, per_sample)
+    best = {}
+    for _ in range(rounds):
+        for what in ("fwd", "bwd"):
+            ms, ms_torch = timed(ours[what], iters), timed(theirs[what], iters)
+            old = best.get(what, (ms, ms_torch))
+            best[what] = (min(ms, old[0]), min(ms_torch, old[1]))
+    for what in ("fwd", "bwd"):
+        ms, ms_torch = best[what]
+        print(json.dumps({"case": f"{'stochastic depth + r' if per_sample else 'dropout'} {name} {what}", "N": N, "p": p, "us": ms * 1e3,
+                          "MB": nbytes[what] / 1e6, "hbm_frac": nbytes[what] / (ms * 1e-3) / 1e9 / HBM, "torch_us": ms_torch * 1e3,
+                          "torch_hbm_frac": torch_bytes[what] / (ms_torch * 1e-3) / 1e9 / HBM, "torch_over_ours": ms_torch / ms,
+                          "vec": info["vec"], "grid": info["grid"], "gpu": gpu, "power_limit": power}), flush=True)
+    del x, r, dy, y, dx
+
+
+def run_mbconv(N, iters, hid=16, drop_p=0.0):
     """one training step of an EfficientNet MBConv block with SiLU and squeeze-and-excitation at 28x28x40, N = 128: 1x1 expand to
     240 -> BN + SiLU -> depthwise 5x5 pad 2 -> BN + SiLU -> SE 240 -> hid -> 240 -> 1x1 project to 40 -> BN + x0, its backward (the
     shortcut's gradient dres left apart, as run_mbblock) and the sgd of the eight layers, on the engine's stream.  Next to it the
-    torch eager step of the same block on bf16 channels-last tensors (fp32 masters, w -= lr * grad, re-cast to bf16)."""
+    torch eager step of the same block on bf16 channels-last tensors (fp32 masters, w -= lr * grad, re-cast to bf16).  With drop_p,
+    instead of torch: the same step with stochastic depth (the last BN without r, a DropoutLayer adding x0 to the dropped branch),
+    the two steps alternated over three rounds, the best of each kept."""
     H = W = 28
     C, E, k = 40, 240, 5
     r = np.random.default_rng(14)
@@ -1234,8 +1283,31 @@ def run_mbconv(N, iters, hid=16):
         for layer in layers:
             layer.sgd(lr)
 
+    if drop_p:
+        dp = pkg.DropoutLayer(eng, N, H * W * C, drop_p, seed=5, per_sample=True)
+        bo, dbo = narrow(), narrow()
+
+        def step_drop():
+            ex.forward(x0, ye); b1.forward(ye, ze); dwl.forward(ze, yd); b2.forward(yd, zd); se.forward(zd, ys); pr.forward(ys, yp)
+            b3.forward(yp, bo); dp.forward(bo, out, r=x0)
+            dp.backward(dout, dbo); b3.backward(bo, dbo, dyp); pr.backward(yp, dyp, dys); se.backward(ys, dys, dzd)
+            b2.backward(zd, dzd, dyd); dwl.backward(yd, dyd, dze); b1.backward(ze, dze, dye); ex.backward(ye, dye, dx0)
+            for layer in layers:
+                layer.sgd(lr)
+
+        fused, dropped = float("inf"), float("inf")
+        for _ in range(3):
+            fused, dropped = min(fused, timed(step, iters)), min(dropped, timed(step_drop, iters))
+        ms_dp = {"fwd": timed(lambda: dp.forward(bo, out, r=x0), iters), "bwd": timed(lambda: dp.backward(dout, dbo), iters)}
+        print(json.dumps({"case": f"MBConv 28x28x40 -> 240 dw 5x5, SiLU, SE 240 -> {hid} -> 240 training step N={N}, stochastic depth "
+                          f"p={drop_p} vs residual fused in BN", "fused_ms": fused, "drop_path_ms": dropped, "extra_ms": dropped - fused,
+                          "drop_over_fused": dropped / fused, "drop_fwd_us": ms_dp["fwd"] * 1e3, "drop_bwd_us": ms_dp["bwd"] * 1e3,
+                          "gpu": gpu, "power_limit": power}), flush=True)
+        for layer in layers:
+            layer.close()
+        return
     ms = timed(step, iters)
-    ms_bn = {"fwd": timed(lambda: b2.forward(yd, zd), iters), "bwd": timed(lambda: b2.backward(zd, dzd, dyd), iters)}
+    ms_bn ={"fwd": timed(lambda: b2.forward(yd, zd), iters), "bwd": timed(lambda: b2.backward(zd, dzd, dyd), iters)}
     F = torch.nn.functional
     xt = x0.view(torch.bfloat16).permute(0, 3, 1, 2).detach().requires_grad_(True)
     dt = dout.view(torch.bfloat16).permute(0, 3, 1, 2)
@@ -1326,6 +1398,13 @@ if only == "bnact":                                                    # BN + Re
     run_bnact("24x24x6 (scalar path)", 1024, 24, 24, 6, 50)
 if only == "mbconv":                                                   # one step of an MBConv block with SiLU and SE, torch beside it
     run_mbconv(128, 20)
+if only == "dropout":                                                  # dropout and stochastic depth, torch beside them
+    for args in (("56x56x64", 128, 56, 56, 64), ("28x28x240", 128, 28, 28, 240), ("7x7x1280", 128, 7, 7, 1280), ("fc 4096", 128, 1, 1, 4096)):
+        run_dropout(*args, 50, per_sample=False)
+    for args in (("56x56x24", 128, 56, 56, 24), ("28x28x40", 128, 28, 28, 40), ("14x14x112", 128, 14, 14, 112), ("7x7x320", 128, 7, 7, 320)):
+        run_dropout(*args, 50, per_sample=True)
+if only == "mbconvdrop":                                               # the MBConv step with stochastic depth against the fused residual
+    run_mbconv(128, 20, drop_p=0.2)
 if only == "bn":                                                       # batch normalization passes, torch beside them
     run_bn("56x56x64", 128, 56, 56, 64, 50)
     run_bn("28x28x128", 128, 28, 28, 128, 50)
