@@ -779,6 +779,50 @@ int pcnn_se_scale_nhwc_info(int N, int H, int W, int C, int *out8);
 int pcnn_dropout_bf16(pcnn_ctx *ctx, const void *x_bf16_dev, const void *r_bf16_dev, void *y_bf16_dev, int N, int row_elems, int row_pitch,
                       double p, int per_sample, unsigned long long seed, unsigned long long call);
 int pcnn_dropout_bf16_info(int N, int row_elems, int row_pitch, double p, int per_sample, long long *out5);
+/* Input pipeline (csrc/augment.cu): positions first .. first + N - 1 of an epoch of a uint8 dataset in device memory become one
+ * bf16 batch in the x layout of every plan, plus its labels, in one launch: a per-epoch shuffle, torchvision's
+ * RandomCrop(size = (H, W), padding = pad, fill = 0) and RandomHorizontalFlip on the uint8 image, then ToTensor and
+ * Normalize(mean, std).
+ *   - Layouts: images dense [n][H][W][C] uint8; labels [n] uint8 or NULL.  x [N][image_rows][row_pitch] bf16 holding H x W pixels
+ *     of C_out channels per image (row_pitch 0 = W C_out rounded up to 8, otherwise a multiple of 8 >= W C_out; image_rows 0 = H,
+ *     otherwise >= H).  Pad columns and pad rows of x are never written.  labels_out[j] = labels[i]; both label pointers are NULL
+ *     or neither is.
+ *   - Which image: position j of the batch is epoch position e = first + j and dataset index i = shuffle ? pi(e) : e.  pi is a
+ *     permutation of [0, n) that depends on (seed, epoch, n) alone, not on N, first, the grid or the GPU: a balanced Feistel
+ *     network of 6 rounds over 2b bits, b the least with 4^b >= n (4 rounds are measurably biased on domains of a few bits).
+ *     With v = (L << b) | R, L and R of b bits, round r = 0..5 maps
+ *     (L, R) to (R, L ^ (F_r(R) & (2^b - 1))), F_r(R) = word x of the Philox4x32-10 block at counter (R, 0xC0000000 | r,
+ *     epoch lo, epoch hi) with key (seed lo, seed hi).  pi(e) applies the network to e, then again to the result, until the value
+ *     is below n (cycle walking: a bijection, with fewer than 4 applications expected since 4^b < 4n; no sort, no scratch).
+ *   - Draws: image i's block is Philox4x32-10 at counter (i lo, i hi | 0x80000000, epoch lo, epoch hi) with key (seed lo,
+ *     seed hi); oy = umulhi(w.x, 2 pad + 1), ox = umulhi(w.y, 2 pad + 1), flip_i = flip && (w.z >> 31) (probability exactly 1/2).
+ *     They depend on the dataset index, not on the batch position: an image gets the same crop in an epoch whatever N or first.
+ *     Domains: bit 31 of counter word 1 is set in every counter of this call and bit 30 in the permutation's; word 1 of a dropout
+ *     counter (pcnn_dropout_bf16) is the high word of an index below 2^62, so no crop draw or round function coincides with a
+ *     dropout draw for any seed, call or epoch, and no round function with a crop draw (i < 2^62).
+ *   - Geometry: x[j][h][w][c] = v(c, src[i][h + oy - pad][w' + ox - pad][c]), w' = flip_i ? W - 1 - w : w; a source pixel outside
+ *     the image is the byte 0 (so a crop may be all fill).  Channels C <= c < C_out are +0.
+ *   - Values: v(c, u) = bf16_rn(RN(RN(RN(float(u) / 255) - mean[c]) / std[c])), ToTensor then Normalize in fp32, each operation an
+ *     IEEE round to nearest with no contraction.  The host forms these 256 C values into a table the kernel looks up;
+ *     mean_host = NULL means mean 0 and std_host = NULL means std 1, which gives bf16_rn(u / 255).
+ * Domain (anything else is PCNN_ERR_ARG with the function and the rule in the message): n, N, H, W >= 1; 0 <= first and first + N
+ * <= n; 1 <= C <= 4; C <= C_out <= 8; 0 <= pad <= 64; shuffle and flip 0 or 1; H W C < 2^31 (one image; the dataset is indexed
+ * in 64 bits); n H W C < 2^62; row_pitch and image_rows as above; x below 2^62 bytes; mean finite; std finite and > 0; images and
+ * x not NULL; x 16-byte aligned; x sharing no byte with images or labels_out, labels_out none with labels or images.
+ * Kernel: a CTA of 256 threads per (batch position, block of rows_per_cta output rows), rows_per_cta = ceil(16 KB / (W C_out 2))
+ * clamped to 1 .. H; thread 0 runs the generator once for the CTA.  Rows are written as 16-byte vectors of 8 elements when
+ * W C_out % 8 == 0, otherwise as single elements, the choice made from the shape.  Stream-ordered; no atomics; the grid depends on
+ * the shape alone.
+ * pcnn_augment_u8_bf16_info: host only (no GPU, no context), refused as the call refuses.  out8 = { row_pitch, image_rows, b,
+ * elements per vector (8 or 1), grid (CTAs), rows_per_cta, row blocks per image, threads per CTA }; lut_out, when not NULL,
+ * receives the table, 256 C bf16 bits at [c][u]. */
+int pcnn_augment_u8_bf16(pcnn_ctx *ctx, const uint8_t *images_dev, const uint8_t *labels_dev, long long n, int H, int W, int C,
+                         long long first, int N, int shuffle, int pad, int flip, unsigned long long seed, unsigned long long epoch,
+                         const float *mean_host, const float *std_host, void *x_bf16_dev, int C_out, int row_pitch, int image_rows,
+                         uint8_t *labels_out_dev);
+int pcnn_augment_u8_bf16_info(long long n, int H, int W, int C, long long first, int N, int shuffle, int pad, int flip, int C_out,
+                              int row_pitch, int image_rows, const float *mean_host, const float *std_host, long long *out8,
+                              uint16_t *lut_out);
 /* Softmax cross-entropy on bf16 logits [N][O], 1 <= O <= 256, labels uint8 [N]:
  *   p = softmax(row) evaluated in double: m = max, den = sum exp(z - m), p_t = exp(z_t - m) / den;
  *   dlogits[n][t] = bf16_rn(float_rn((p_t - [t == label]) * scale)), double -> fp32 -> bf16, each round to nearest even: the

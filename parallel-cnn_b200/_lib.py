@@ -30,6 +30,7 @@ class PcnnError(RuntimeError):
 
 _vp, _i, _l, _f, _sz = C.c_void_p, C.c_int, C.c_long, C.c_float, C.c_size_t
 _pvp = C.POINTER(C.c_void_p)
+_ll = C.c_longlong
 
 
 class OptimTensor(C.Structure):
@@ -181,6 +182,9 @@ _SIG = {
     "pcnn_se_scale_nhwc_info": [_i, _i, _i, _i, _vp],
     "pcnn_dropout_bf16": [_vp, _vp, _vp, _vp, _i, _i, _i, C.c_double, _i, C.c_ulonglong, C.c_ulonglong],
     "pcnn_dropout_bf16_info": [_i, _i, _i, C.c_double, _i, _vp],
+    "pcnn_augment_u8_bf16": [_vp, _vp, _vp, C.c_longlong, _i, _i, _i, C.c_longlong, _i, _i, _i, _i, C.c_ulonglong, C.c_ulonglong, _vp, _vp,
+                             _vp, _i, _i, _i, _vp],
+    "pcnn_augment_u8_bf16_info": [C.c_longlong, _i, _i, _i, C.c_longlong, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp],
     "pcnn_softmax_ce_bf16": [_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp],
     "pcnn_optim_create": [_vp, _vp, _vp, _i, _pvp],
     "pcnn_optim_step": [_vp, _vp, _f],
@@ -388,6 +392,36 @@ def dropout_info(N, row_elems, row_pitch=0, p=0.0, per_sample=False):
     out = (C.c_longlong * 5)()
     check("pcnn_dropout_bf16_info", lib().pcnn_dropout_bf16_info(int(N), int(row_elems), int(row_pitch), float(p), int(per_sample), out))
     return dict(T=out[0], scale_bits=out[1], vec=out[2], grid=out[3], per_thread=out[4])
+
+
+def channel_stats(values, C, name):
+    """mean or std of the input pipeline as a float32 array of C values (None stays None: mean 0 / std 1); a scalar is every channel's"""
+    if values is None:
+        return None
+    a = np.asarray(values, np.float32).reshape(-1)
+    if np.ndim(values) == 0:
+        a = np.repeat(a, int(C))
+    if a.size != int(C):
+        raise PcnnError("augment", -1, f"{name} has {a.size} values for C = {C} channels")
+    return a
+
+
+def augment_info(n, H, W, C, first, N, shuffle=1, pad=0, flip=0, C_out=None, row_pitch=0, image_rows=0, mean=None, std=None):
+    """The layout, permutation width, launch and value table of the input pipeline (pcnn_augment_u8_bf16_info; host only, no GPU),
+    refused as pcnn_augment_u8_bf16 refuses.  C_out None = C; row_pitch / image_rows 0 = dense; mean / std None = 0 / 1.
+    Returns (info, lut): info holds row_pitch and image_rows as used, b (the Feistel half width), vec (elements per vector, 8 is the
+    16-byte path), grid, rows_per_cta, row_blocks (per image) and threads; lut is uint16 [C][256], the bf16 bits of each value."""
+    Cin = int(C)
+    C_out = Cin if C_out is None else int(C_out)
+    m, s = channel_stats(mean, Cin, "mean"), channel_stats(std, Cin, "std")
+    out = (_ll * 8)()
+    lut = np.zeros((max(Cin, 1), 256), np.uint16)
+    check("pcnn_augment_u8_bf16_info", lib().pcnn_augment_u8_bf16_info(
+        int(n), int(H), int(W), Cin, int(first), int(N), int(shuffle), int(pad), int(flip), C_out, int(row_pitch or 0),
+        int(image_rows or 0), None if m is None else m.ctypes.data, None if s is None else s.ctypes.data, out,
+        lut.ctypes.data if 1 <= Cin <= 4 else None))
+    keys = ("row_pitch", "image_rows", "b", "vec", "grid", "rows_per_cta", "row_blocks", "threads")
+    return dict(zip(keys, list(out))), lut
 
 
 def conv_bwd_plan_info(N, H, W, C, K, R, S, stride=1):

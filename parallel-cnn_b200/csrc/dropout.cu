@@ -8,6 +8,7 @@
 // A grid-stride loop whose grid is a function of the shape alone walks the vectors; which thread handles an element never
 // changes a bit, since the draw is a function of (seed, call, index).  p = 0 takes a kernel without the generator.
 #include "pcnn_internal.h"
+#include "philox.cuh"
 
 #include <cuda_bf16.h>
 
@@ -35,23 +36,6 @@ struct DropArgs {
     float scale;
     unsigned k0, k1, c2, c3;    // the Philox key (seed lo, hi) and the counter's upper words (call lo, hi)
 };
-
-// Philox4x32-10 (Salmon et al., SC'11; Random123): ten rounds of two 32x32->64 multiplies, the key bumped by the Weyl constants
-// between rounds
-__device__ __forceinline__ uint4 philox4x32_10(unsigned c0, unsigned c1, unsigned c2, unsigned c3, unsigned k0, unsigned k1) {
-#pragma unroll
-    for (int i = 0; i < 10; ++i) {
-        const unsigned lo0 = 0xD2511F53u * c0, hi0 = __umulhi(0xD2511F53u, c0);
-        const unsigned lo1 = 0xCD9E8D57u * c2, hi1 = __umulhi(0xCD9E8D57u, c2);
-        c0 = hi1 ^ c1 ^ k0;
-        c1 = lo1;
-        c2 = hi0 ^ c3 ^ k1;
-        c3 = lo0;
-        k0 += 0x9E3779B9u;
-        k1 += 0xBB67AE85u;
-    }
-    return make_uint4(c0, c1, c2, c3);
-}
 
 // word (i & 3) of the block of counter (i >> 2, call)
 __device__ __forceinline__ unsigned draw(unsigned long long i, const DropArgs &a) {

@@ -4,8 +4,8 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import (F32, NPARAM, OPTIM_ADAMW, OPTIM_SGD, TEST_SET, TRAIN_SET, U8, OptimConfig, OptimTensor, PcnnError, avgpool_nhwc_info,
-                   batchnorm_nhwc_info, check, conv_layer_family, dropout_info, dwconv_info, gconv_info, global_avgpool_nhwc_info, lib, linear_info,
+from ._lib import (F32, NPARAM, OPTIM_ADAMW, OPTIM_SGD, TEST_SET, TRAIN_SET, U8, OptimConfig, OptimTensor, PcnnError, augment_info,
+                   avgpool_nhwc_info, batchnorm_nhwc_info, channel_stats, check, conv_layer_family, dropout_info, dwconv_info, gconv_info, global_avgpool_nhwc_info, lib, linear_info,
                    maxpool_nhwc_info,
                    se_scale_nhwc_info, ACT_RELU, ACT_SIGMOID, ACT_SILU, ACT_HARDSWISH, ACT_RELU6)
 
@@ -544,6 +544,17 @@ class Engine:
         The backward is the same call on dy with the forward's (p, seed, call, per_sample) and no r."""
         self._call("pcnn_dropout_bf16", _p(x), _p(r), _p(y), int(N), int(row_elems), int(row_pitch or 0), float(p), int(per_sample),
                    int(seed), int(call))
+
+    def augment(self, images, labels, n, H, W, C, first, N, x, labels_out=None, shuffle=1, pad=0, flip=0, seed=0, epoch=0, mean=None,
+                std=None, C_out=None, row_pitch=0, image_rows=0):
+        """pcnn_augment_u8_bf16: epoch positions first .. first + N - 1 of the uint8 dataset images [n][H][W][C] (labels [n] or None)
+        into x [N][image_rows][row_pitch] bf16 with C_out channels (None = C) and labels_out [N]: image pi(e) when shuffle, cropped
+        from the image padded by pad with zeros, flipped when flip, then (u / 255 - mean) / std per channel (None = 0 / 1)."""
+        Cin = int(C)
+        m, s = channel_stats(mean, Cin, "mean"), channel_stats(std, Cin, "std")
+        self._call("pcnn_augment_u8_bf16", _p(images), _p(labels), int(n), int(H), int(W), Cin, int(first), int(N), int(shuffle), int(pad),
+                   int(flip), int(seed), int(epoch), None if m is None else m.ctypes.data, None if s is None else s.ctypes.data, _p(x),
+                   Cin if C_out is None else int(C_out), int(row_pitch or 0), int(image_rows or 0), _p(labels_out))
 
 
 class ConvPlan:
@@ -1190,6 +1201,68 @@ class DropoutLayer:
 
     def close(self):
         pass
+
+
+class ImageBatcher:
+    """The input path of a device-trained network (pcnn_augment_u8_bf16): a uint8 dataset [n][H][W] or [n][H][W][C] (a device
+    tensor, a DeviceArray, or a host array uploaded once) and its uint8 labels [n] (or None) become batches of N images in the x
+    layout a plan reads, in one launch per batch.  Training batches take the epoch in a fresh order (shuffle), each image cropped
+    from the image zero-padded by pad (RandomCrop) and mirrored with probability 1/2 (flip), then normalised per channel by mean /
+    std (None = 0 / 1, a scalar for every channel).  x has C_out channels (None = C) at row_pitch / image_rows (0 = dense), so a
+    network's first layer reads it as it is: for the example networks' MNIST layer, C_out 1, row_pitch 32, image_rows 28.
+
+    The batcher owns x and the label buffer; batch(step) overwrites them in stream order and returns (x pointer, labels), the
+    arguments of the networks' forward(x, labels).  Everything random is a function of (seed, epoch, dataset index), so a
+    checkpoint that saves `epoch`, a plain attribute the caller sets, replays the same batches.  The last partial batch of an
+    epoch is dropped: steps_per_epoch = n // N.
+
+        for ep in range(epochs):
+            batcher.epoch = ep
+            for s in range(batcher.steps_per_epoch):
+                net.forward(*batcher.batch(s)); net.backward(); net.sgd(lr)
+        net.forward(*test_batcher.batch(0, training=False), training=False)
+
+    batch(step, training=False) is the eval path: identity order, no crop and no flip."""
+
+    def __init__(self, engine, images, labels, N, pad=0, flip=False, shuffle=True, seed=0, mean=None, std=None, C_out=None,
+                 row_pitch=0, image_rows=0):
+        shape = tuple(int(d) for d in images.shape)
+        if len(shape) not in (3, 4):
+            raise PcnnError("ImageBatcher", -1, f"images must be [n][H][W] or [n][H][W][C], got shape {shape}")
+        if "uint8" not in str(images.dtype):
+            raise PcnnError("ImageBatcher", -1, f"images must be uint8, got {images.dtype}")
+        self.n, self.H, self.W = shape[:3]
+        self.C = shape[3] if len(shape) == 4 else 1
+        self.N, self.pad, self.flip, self.shuffle, self.seed = int(N), int(pad), bool(flip), bool(shuffle), int(seed)
+        self.mean, self.std = channel_stats(mean, self.C, "mean"), channel_stats(std, self.C, "std")
+        self.C_out = self.C if C_out is None else int(C_out)
+        self.info, self.lut = augment_info(self.n, self.H, self.W, self.C, 0, self.N, int(self.shuffle), self.pad, int(self.flip),
+                                           self.C_out, row_pitch, image_rows, self.mean, self.std)
+        if labels is not None and int(labels.shape[0]) != self.n:
+            raise PcnnError("ImageBatcher", -1, f"{labels.shape[0]} labels for {self.n} images")
+        self.engine = engine
+        self.images = engine.to_device(images) if isinstance(images, np.ndarray) else images
+        self.labels = engine.to_device(np.asarray(labels, np.uint8)) if isinstance(labels, np.ndarray) else labels
+        self.x = engine.array((self.N, self.info["image_rows"], self.info["row_pitch"]), np.uint16)    # zeroed: the pad stays 0
+        self.labels_out = engine.array((self.N,), np.uint8) if labels is not None else None
+        self.steps_per_epoch = self.n // self.N
+        self.epoch = 0
+
+    def batch(self, step, training=True):
+        """(x pointer, labels) of batch `step` of epoch self.epoch: positions step N .. step N + N - 1"""
+        if not 0 <= int(step) < self.steps_per_epoch:
+            raise PcnnError("ImageBatcher.batch", -1, f"step = {step}: 0 <= step < steps_per_epoch = {self.steps_per_epoch} is required")
+        aug = bool(training)
+        self.engine.augment(self.images, self.labels, self.n, self.H, self.W, self.C, int(step) * self.N, self.N, self.x, self.labels_out,
+                            shuffle=int(aug and self.shuffle), pad=self.pad if aug else 0, flip=int(aug and self.flip), seed=self.seed,
+                            epoch=self.epoch, mean=self.mean, std=self.std, C_out=self.C_out, row_pitch=self.info["row_pitch"],
+                            image_rows=self.info["image_rows"])
+        return self.x.ptr, self.labels_out
+
+    def close(self):
+        for a in (self.x, self.labels_out):
+            if a is not None:
+                a.free()
 
 
 class SqueezeExcitationLayer:

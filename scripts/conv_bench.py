@@ -1245,6 +1245,90 @@ def run_dropout(name, N, H, W, C, iters, per_sample, p=0.2, rounds=3):
     del x, r, dy, y, dx
 
 
+def run_augment(name, N, H, W, C, C_out, pad, iters, batches=4, row_pitch=0, image_rows=0, rounds=3):
+    """one batch of the input pipeline (pcnn_augment_u8_bf16): shuffle over a dataset of `batches` batches, crop with pad, flip,
+    normalise, into x with C_out channels; the calls walk the epoch's batches.  Beside it the torch eager pipeline of
+    tests/test_augment_gpu.py (torch_batch: gather, pad, crop and flip by advanced indexing, normalise, cast) on the same indices,
+    offsets and flips, plus the label gather, alternated over `rounds` rounds (the best of each kept).  Bytes: N H W C read,
+    N H W C_out 2 written, 2 N for the labels."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import augment_ref as A
+    from test_augment_gpu import torch_batch
+    n = N * batches
+    images = torch.randint(0, 256, (n, H, W, C), dtype=torch.uint8, device="cuda")
+    labels = torch.randint(0, 10, (n,), dtype=torch.uint8, device="cuda")
+    flip = True
+    mean, std = ((0.485, 0.456, 0.406), (0.229, 0.224, 0.225)) if C == 3 else (None, None)
+    info, _ = pkg.augment_info(n, H, W, C, 0, N, 1, pad, int(flip), C_out, row_pitch, image_rows, mean, std)
+    x = torch.empty(N * info["image_rows"] * info["row_pitch"], dtype=torch.int16, device="cuda")
+    lo = torch.empty(N, dtype=torch.uint8, device="cuda")
+    steps = iter(range(1 << 40))
+    seed, epoch = 11, 3
+
+    def ours():
+        eng.augment(images, labels, n, H, W, C, (next(steps) % batches) * N, N, x, lo, shuffle=1, pad=pad, flip=int(flip), seed=seed,
+                    epoch=epoch, mean=mean, std=std, C_out=C_out, row_pitch=row_pitch, image_rows=image_rows)
+
+    draws = []
+    for b in range(batches):
+        i = A.indices(n, b * N, N, 1, seed, epoch)
+        oy, ox, fl = A.draws(i.astype(np.uint64), pad, int(flip), seed, epoch)
+        draws.append([torch.as_tensor(a, device="cuda") for a in (i, oy, ox, fl)])
+    tsteps = iter(range(1 << 40))
+
+    def theirs():
+        i, oy, ox, fl = draws[next(tsteps) % batches]
+        return torch_batch(images, i, oy, ox, fl, pad, mean, std, C_out), labels[i]
+
+    gpu, power = card()
+    best = None
+    for _ in range(rounds):
+        ms, ms_torch = timed(ours, iters), timed(theirs, iters)
+        best = (ms, ms_torch) if best is None else (min(ms, best[0]), min(ms_torch, best[1]))
+    ms, ms_torch = best
+    nbytes = N * H * W * C + N * H * W * C_out * 2 + 2 * N
+    print(json.dumps({"case": f"augment {name}", "N": N, "n": n, "pad": pad, "flip": flip, "us": ms * 1e3, "MB": nbytes / 1e6,
+                      "hbm_frac": nbytes / (ms * 1e-3) / 1e9 / HBM, "torch_us": ms_torch * 1e3, "torch_over_ours": ms_torch / ms,
+                      "vec": info["vec"], "grid": info["grid"], "rows_per_cta": info["rows_per_cta"], "gpu": gpu, "power_limit": power}),
+          flush=True)
+
+
+def run_resnetgap_augment(iters, rounds=3):
+    """one training step of the GAP ResNet of tests/test_avgpool_nhwc_gpu.py at N = 128 on the 1024 golden digits, its batch built
+    by pkg.ImageBatcher (shuffle, random crop of pad 2) against the same step on a slice of the pre-converted mnist_device rows,
+    alternated over `rounds` rounds (the best of each kept)"""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import test_avgpool_nhwc_gpu as T
+    g = np.load(os.path.join(ROOT, "tests", "golden", "mnist_subset.npz"))
+    xs, ys = T.mnist_device(pkg, g["train_u8"]), torch.from_numpy(g["train_labels"]).cuda()
+    net = T.ResNetGAP(eng, pkg, T.init_params())
+    batcher = pkg.ImageBatcher(eng, g["train_u8"].reshape(-1, 28, 28), g["train_labels"], T.NB, pad=2, shuffle=True, seed=5,
+                               row_pitch=32, image_rows=28)
+    row_bytes = 28 * 32 * 2
+    k = iter(range(1 << 40))
+
+    def step(batch):
+        s = next(k) % batcher.steps_per_epoch
+        net.forward(*batch(s))
+        net.backward()
+        net.sgd(T.LR_STEP)
+
+    aug = lambda: step(batcher.batch)
+    plain = lambda: step(lambda s: (xs.data_ptr() + s * T.NB * row_bytes, ys[s * T.NB:(s + 1) * T.NB]))
+    batch_only = lambda: batcher.batch(next(k) % batcher.steps_per_epoch)
+    gpu, power = card()
+    best = None
+    for _ in range(rounds):
+        r = (timed(aug, iters), timed(plain, iters), timed(batch_only, iters))
+        best = r if best is None else tuple(min(a, b) for a, b in zip(r, best))
+    ms_aug, ms_plain, ms_batch = best
+    print(json.dumps({"case": f"GAP ResNet training step N={T.NB}, batch from ImageBatcher (shuffle, pad 2) vs pre-converted slice",
+                      "ms_batcher": ms_aug, "ms_slice": ms_plain, "batcher_over_slice": ms_aug / ms_plain, "batch_us": ms_batch * 1e3,
+                      "gpu": gpu, "power_limit": power}), flush=True)
+    batcher.close()
+    net.close()
+
+
 def run_mbconv(N, iters, hid=16, drop_p=0.0):
     """one training step of an EfficientNet MBConv block with SiLU and squeeze-and-excitation at 28x28x40, N = 128: 1x1 expand to
     240 -> BN + SiLU -> depthwise 5x5 pad 2 -> BN + SiLU -> SE 240 -> hid -> 240 -> 1x1 project to 40 -> BN + x0, its backward (the
@@ -1403,6 +1487,14 @@ if only == "dropout":                                                  # dropout
         run_dropout(*args, 50, per_sample=False)
     for args in (("56x56x24", 128, 56, 56, 24), ("28x28x40", 128, 28, 28, 40), ("14x14x112", 128, 14, 14, 112), ("7x7x320", 128, 7, 7, 320)):
         run_dropout(*args, 50, per_sample=True)
+if only == "augment":                                                  # the input pipeline, torch eager beside it
+    run_augment("28x28x1 -> [28][32]", 1024, 28, 28, 1, 1, 2, 50, row_pitch=32, image_rows=28)
+    run_augment("32x32x3 -> 3", 512, 32, 32, 3, 3, 4, 50)
+    run_augment("32x32x3 -> 8", 512, 32, 32, 3, 8, 4, 50)
+    run_augment("64x64x3 -> 8", 256, 64, 64, 3, 8, 4, 50)
+    run_augment("224x224x3 -> 8", 256, 224, 224, 3, 8, 4, 20)
+if only == "resnetgap-augment":                                        # the GAP ResNet step fed by the batcher vs the pre-converted slice
+    run_resnetgap_augment(20)
 if only == "mbconvdrop":                                               # the MBConv step with stochastic depth against the fused residual
     run_mbconv(128, 20, drop_p=0.2)
 if only == "bn":                                                       # batch normalization passes, torch beside them

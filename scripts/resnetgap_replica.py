@@ -4,10 +4,12 @@
 epoch), softmax cross-entropy over the batch and an optimizer step, evaluated on the 256 golden test digits with the running
 statistics.  Its accuracy sets the thresholds of the end-to-end tests.
 
-Usage: resnetgap_replica.py [--optim sgd | momentum | adamw] [lr ...]
+Usage: resnetgap_replica.py [--optim sgd | momentum | adamw] [--augment] [lr ...]
   sgd       plain SGD, p += -lr * grad (the layers' own sgd(lr); tests/test_avgpool_nhwc_gpu.py)
   momentum  torch.optim.SGD with momentum 0.9 and weight decay 5e-4 on every parameter (tests/test_optim_gpu.py)
-  adamw     torch.optim.AdamW with betas (0.9, 0.999), eps 1e-8 and weight decay 1e-2 on every parameter (tests/test_optim_gpu.py)"""
+  adamw     torch.optim.AdamW with betas (0.9, 0.999), eps 1e-8 and weight decay 1e-2 on every parameter (tests/test_optim_gpu.py)
+  --augment each epoch's batches as pkg.ImageBatcher draws them with a shuffle and a random crop of pad 2, no flip, at the seed
+            of tests/test_augment_gpu.py, replayed by tests/augment_ref.py (the device run: test_resnet_gap_through_the_batcher)"""
 import argparse
 import os
 import sys
@@ -19,10 +21,12 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 from test_avgpool_nhwc_gpu import EPOCHS, NB, init_params  # noqa: E402
 
+AUG_SEED, AUG_PAD = 0x0123456789ABCDEF, 2       # tests/test_augment_gpu.py
+
 F = torch.nn.functional
 
 
-def run(lr, optim="sgd"):
+def run(lr, optim="sgd", augment=False):
     torch.manual_seed(0)
     g = np.load(os.path.join(ROOT, "tests", "golden", "mnist_subset.npz"))
     img = lambda u8: torch.from_numpy(u8.reshape(-1, 1, 28, 28).astype(np.float32) / 255.0).bfloat16().float()   # the device's bf16 input
@@ -53,21 +57,29 @@ def run(lr, optim="sgd"):
     losses = []
     for ep in range(EPOCHS):
         for s in range(1024 // NB):
-            loss = F.cross_entropy(net(xs[s * NB:(s + 1) * NB], True), ys[s * NB:(s + 1) * NB])
+            if augment:
+                import augment_ref
+                xb, lab, *_ = augment_ref.batch(g["train_u8"].reshape(-1, 28, 28, 1), s * NB, NB, 1, AUG_PAD, 0, AUG_SEED, ep,
+                                                labels=g["train_labels"])
+                x = torch.from_numpy((xb.astype(np.uint32) << 16).view(np.float32).reshape(NB, 1, 28, 28))
+                loss = F.cross_entropy(net(x, True), torch.from_numpy(lab).long())
+            else:
+                loss = F.cross_entropy(net(xs[s * NB:(s + 1) * NB], True), ys[s * NB:(s + 1) * NB])
             opt.zero_grad(set_to_none=True)
             loss.backward()
             opt.step()
             losses.append(float(loss))
     with torch.no_grad():
         acc = float((net(xt, False).argmax(1) == yt).float().mean())
-    print(f"{optim} lr {lr}: mean loss epoch 1 {np.mean(losses[:8]):.4f} -> epoch {EPOCHS} {np.mean(losses[-8:]):.4f}; test accuracy {acc:.4f}",
+    print(f"{optim}{' augmented' if augment else ''} lr {lr}: mean loss epoch 1 {np.mean(losses[:8]):.4f} -> epoch {EPOCHS} {np.mean(losses[-8:]):.4f}; test accuracy {acc:.4f}",
           flush=True)
 
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--optim", default="sgd", choices=["sgd", "momentum", "adamw"])
+    ap.add_argument("--augment", action="store_true")
     ap.add_argument("lr", nargs="*", type=float)
     a = ap.parse_args()
     for lr in a.lr or [0.1]:
-        run(lr, a.optim)
+        run(lr, a.optim, a.augment)
