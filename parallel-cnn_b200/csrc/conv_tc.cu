@@ -27,6 +27,8 @@
 // 0-63 and 64-127 of a tile), warp 8 = TMA producer.
 #include "tc_common.cuh"
 
+#include <memory>
+
 using namespace pcnn_tc;
 
 namespace {
@@ -234,75 +236,45 @@ int make_map_2d(CUtensorMap *map, void *base, uint64_t inner, uint64_t outer, ui
 
 }  // namespace
 
-struct pcnn_conv_plan {
+// a plan of pcnn_conv_tc_plan_create(_strided): its operand is the Toeplitz matrices, not an image of the master, so w stays null
+struct ToeplitzPlan : pcnn_conv_plan {
     ConvTcParams p;
     int W, S, row_pitch, stride, in_image_rows;
     void *d_toeplitz = nullptr;     // [V][R][npad][32] bf16
-    float *d_bias = nullptr;
     CUtensorMap map_b;
-    ConvWidePlan *wide = nullptr;   // non-null: a plan of pcnn_conv_wide_plan_create (conv_wide_tc.cu), nothing above is used
-    LinearPlan *linear = nullptr;   // non-null: a plan of pcnn_linear_plan_create (linear_tc.cu), nothing above is used
-    DwConvPlan *dw = nullptr;       // non-null: a plan of pcnn_dwconv_plan_create (dwconv_nhwc.cu), nothing above is used
-    GConvPlan *gc = nullptr;        // non-null: a plan of pcnn_gconv_plan_create (gconv_nhwc.cu), nothing above is used
+    ~ToeplitzPlan() override {
+        if (d_toeplitz) cudaFree(d_toeplitz);
+    }
+    int fwd(pcnn_ctx *ctx, const void *x_bf16, void *y_bf16) override;
+    // the Toeplitz operand from fp32 KRSC filters in device memory, enqueued on the context's stream
+    int load_filters(pcnn_ctx *ctx, const float *filt_dev) override {
+        const long total = (long)p.V * p.R * p.npad * TC_KCHUNK;
+        k_conv_tc_toeplitz<<<(int)((total + 255) / 256), 256, 0, ctx->stream>>>(filt_dev, reinterpret_cast<__nv_bfloat16 *>(d_toeplitz),
+                                                                                 p, S);
+        PCNN_CHECK_LAUNCH(ctx);
+        return PCNN_OK;
+    }
 };
 
-pcnn_conv_plan *conv_plan_wrap_wide(ConvWidePlan *w) {
-    pcnn_conv_plan *pl = new pcnn_conv_plan();
-    pl->wide = w;
-    return pl;
-}
-
-pcnn_conv_plan *conv_plan_wrap_linear(LinearPlan *l) {
-    pcnn_conv_plan *pl = new pcnn_conv_plan();
-    pl->linear = l;
-    return pl;
-}
-
-LinearPlan *conv_plan_linear(pcnn_conv_plan *plan) { return plan->linear; }
-
-pcnn_conv_plan *conv_plan_wrap_dw(DwConvPlan *d) {
-    pcnn_conv_plan *pl = new pcnn_conv_plan();
-    pl->dw = d;
-    return pl;
-}
-
-DwConvPlan *conv_plan_dw(pcnn_conv_plan *plan) { return plan->dw; }
-
-pcnn_conv_plan *conv_plan_wrap_gconv(GConvPlan *g) {
-    pcnn_conv_plan *pl = new pcnn_conv_plan();
-    pl->gc = g;
-    return pl;
-}
-
-GConvPlan *conv_plan_gconv(pcnn_conv_plan *plan) { return plan->gc; }
-
-void conv_plan_operand(pcnn_conv_plan *plan, PlanOperand *out) {
-    if (plan->wide) return conv_wide_operand(plan->wide, out);
-    if (plan->linear) return linear_operand(plan->linear, out);
-    if (plan->dw) return dwconv_operand(plan->dw, out);
-    if (plan->gc) return gconv_operand(plan->gc, out);
-    const ConvTcParams &p = plan->p;
-    *out = PlanOperand{nullptr, 0, 0, (long long)p.K * p.R * plan->S * p.C, plan->d_bias, p.K};
-}
-
-// the Toeplitz operand of the plan from fp32 KRSC filters in device memory, enqueued on the context's stream
-static int conv_tc_load_filters(pcnn_ctx *ctx, pcnn_conv_plan *pl, const float *filt_dev) {
-    const long total = (long)pl->p.V * pl->p.R * pl->p.npad * TC_KCHUNK;
-    k_conv_tc_toeplitz<<<(int)((total + 255) / 256), 256, 0, ctx->stream>>>(filt_dev, reinterpret_cast<__nv_bfloat16 *>(pl->d_toeplitz),
-                                                                             pl->p, pl->S);
-    PCNN_CHECK_LAUNCH(ctx);
+int pcnn_plan_upload(pcnn_ctx *ctx, pcnn_conv_plan *plan, void **operand, size_t bytes, const float *filt_host, const float *bias_host) {
+    PCNN_CUDA(cudaMalloc(operand, bytes));
+    {                                        // the same device conversion as pcnn_conv_plan_set_params
+        struct DevTemp {
+            float *p = nullptr;
+            ~DevTemp() { if (p) cudaFree(p); }
+        } tf;
+        const size_t nf = (size_t)plan->n;
+        PCNN_CUDA(cudaMalloc((void **)&tf.p, nf * sizeof(float)));
+        PCNN_CUDA(cudaMemcpyAsync(tf.p, filt_host, nf * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+        const int rc = plan->load_filters(ctx, tf.p);
+        if (rc) return rc;
+        PCNN_CUDA(cudaStreamSynchronize(ctx->stream));
+    }
+    if (bias_host) {
+        PCNN_CUDA(cudaMalloc((void **)&plan->bias, (size_t)plan->K * sizeof(float)));
+        PCNN_CUDA(cudaMemcpy(plan->bias, bias_host, (size_t)plan->K * sizeof(float), cudaMemcpyHostToDevice));
+    }
     return PCNN_OK;
-}
-
-static void free_plan(pcnn_conv_plan *plan) {
-    if (!plan) return;
-    if (plan->wide) conv_wide_free(plan->wide);
-    if (plan->linear) linear_free(plan->linear);
-    if (plan->dw) dwconv_free(plan->dw);
-    if (plan->gc) gconv_free(plan->gc);
-    if (plan->d_toeplitz) cudaFree(plan->d_toeplitz);
-    if (plan->d_bias) cudaFree(plan->d_bias);
-    delete plan;
 }
 
 extern "C" int pcnn_conv_tc_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int row_pitch,
@@ -374,11 +346,9 @@ extern "C" int pcnn_conv_tc_plan_create_strided(pcnn_ctx *ctx, int N, int H, int
     if (image_rows <= 0) image_rows = H;
     const int Qt = sh.Qt, V = sh.V;
     pcnn_device_guard g(ctx->device);
-    struct PlanGuard {                       // frees a half-built plan on every early return below
-        pcnn_conv_plan *p;
-        ~PlanGuard() { free_plan(p); }
-    } guard{new pcnn_conv_plan()};
-    pcnn_conv_plan *pl = guard.p;
+    std::unique_ptr<ToeplitzPlan> pl(new ToeplitzPlan());   // frees a half-built plan on every early return below
+    pl->n = (long long)K * R * S * C;
+    pl->K = K;
     pl->W = W; pl->S = S; pl->row_pitch = row_pitch; pl->stride = stride; pl->in_image_rows = image_rows;
     ConvTcParams &p = pl->p;
     // rows are counted in units of `stride` input rows: tile row m = n * (image_rows / stride) + p
@@ -387,21 +357,8 @@ extern "C" int pcnn_conv_tc_plan_create_strided(pcnn_ctx *ctx, int N, int H, int
     p.n_mtiles = sh.n_mtiles; p.n_qtiles = sh.n_qtiles;
     p.act = act;
     p.y_row_elems = (long long)sh.Q * K;
-    // Toeplitz operands: the same device conversion as pcnn_conv_plan_set_params, from a temporary copy of the host filters
-    PCNN_CUDA(cudaMalloc(&pl->d_toeplitz, (size_t)V * R * p.npad * TC_KCHUNK * 2));
-    {
-        const size_t nf = (size_t)K * R * S * C;
-        pcnn_dev_temp tf;
-        PCNN_CUDA(cudaMalloc((void **)&tf.p, nf * sizeof(float)));
-        PCNN_CUDA(cudaMemcpyAsync(tf.p, filt_host, nf * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-        if ((rc = conv_tc_load_filters(ctx, pl, tf.p))) return rc;
-        PCNN_CUDA(cudaStreamSynchronize(ctx->stream));
-    }
-    if (bias_host) {
-        PCNN_CUDA(cudaMalloc((void **)&pl->d_bias, K * sizeof(float)));
-        PCNN_CUDA(cudaMemcpy(pl->d_bias, bias_host, K * sizeof(float), cudaMemcpyHostToDevice));
-    }
-    p.bias = pl->d_bias;
+    if ((rc = pcnn_plan_upload(ctx, pl.get(), &pl->d_toeplitz, (size_t)V * R * p.npad * TC_KCHUNK * 2, filt_host, bias_host))) return rc;
+    p.bias = pl->bias;
     rc = make_map_2d(&pl->map_b, pl->d_toeplitz, TC_KCHUNK, (uint64_t)V * R * p.npad, TC_KCHUNK * 2, TC_KCHUNK, (uint32_t)p.npad);
     if (rc) return rc;
     static bool configured[64] = {};        // function attributes are per device
@@ -412,8 +369,7 @@ extern "C" int pcnn_conv_tc_plan_create_strided(pcnn_ctx *ctx, int N, int H, int
                                                TC_SMEM_BUDGET + 2048));
         configured[ctx->device & 63] = true;
     }
-    guard.p = nullptr;
-    *out = pl;
+    *out = pl.release();
     return PCNN_OK;
 }
 
@@ -422,7 +378,7 @@ extern "C" int pcnn_conv_tc_plan_destroy(pcnn_ctx *ctx, pcnn_conv_plan *plan) {
     if (!plan) return PCNN_OK;
     pcnn_device_guard g(ctx->device);
     cudaStreamSynchronize(ctx->stream);
-    free_plan(plan);
+    delete plan;
     return PCNN_OK;
 }
 
@@ -430,23 +386,16 @@ extern "C" int pcnn_conv_plan_set_params(pcnn_ctx *ctx, pcnn_conv_plan *plan, co
     PCNN_REQUIRE(ctx && plan, PCNN_ERR_ARG, "pcnn_conv_plan_set_params: NULL context or plan");
     PCNN_REQUIRE(filt_f32_dev || bias_f32_dev, PCNN_ERR_ARG,
                  "pcnn_conv_plan_set_params: filters and bias are both NULL (at least one must be given)");
-    PlanOperand op;
-    conv_plan_operand(plan, &op);
-    const int K = op.K;
-    float *d_bias = op.bias;
-    PCNN_REQUIRE(!bias_f32_dev || d_bias, PCNN_ERR_ARG,
+    PCNN_REQUIRE(!bias_f32_dev || plan->bias, PCNN_ERR_ARG,
                  "pcnn_conv_plan_set_params: a bias for a plan created without one (bias_host NULL): only a plan with a bias can "
                  "refresh it");
     pcnn_device_guard g(ctx->device);
     if (filt_f32_dev) {
-        const int rc = plan->wide     ? conv_wide_load_filters(ctx, plan->wide, filt_f32_dev)
-                       : plan->linear ? linear_load_weights(ctx, plan->linear, filt_f32_dev)
-                       : plan->dw     ? dwconv_load_filters(ctx, plan->dw, filt_f32_dev)
-                       : plan->gc     ? gconv_load_filters(ctx, plan->gc, filt_f32_dev)
-                                      : conv_tc_load_filters(ctx, plan, filt_f32_dev);
+        const int rc = plan->load_filters(ctx, filt_f32_dev);
         if (rc) return rc;
     }
-    if (bias_f32_dev) PCNN_CUDA(cudaMemcpyAsync(d_bias, bias_f32_dev, (size_t)K * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
+    if (bias_f32_dev)
+        PCNN_CUDA(cudaMemcpyAsync(plan->bias, bias_f32_dev, (size_t)plan->K * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
     return PCNN_OK;
 }
 
@@ -454,11 +403,11 @@ extern "C" int pcnn_conv_tc_fwd(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void 
     PCNN_REQUIRE(ctx && plan && x_bf16 && y_bf16, PCNN_ERR_ARG, "pcnn_conv_tc_fwd: NULL argument");
     PCNN_REQUIRE(((uintptr_t)x_bf16 & 15) == 0, PCNN_ERR_ARG, "pcnn_conv_tc_fwd: activations must be 16-byte aligned");
     pcnn_device_guard g(ctx->device);
-    if (plan->wide) return conv_wide_fwd(ctx, plan->wide, x_bf16, y_bf16);
-    if (plan->linear) return linear_fwd(ctx, plan->linear, x_bf16, y_bf16);
-    if (plan->dw) return dwconv_fwd(ctx, plan->dw, x_bf16, y_bf16);
-    if (plan->gc) return gconv_fwd(ctx, plan->gc, x_bf16, y_bf16);
-    ConvTcParams p = plan->p;
+    return plan->fwd(ctx, x_bf16, y_bf16);
+}
+
+int ToeplitzPlan::fwd(pcnn_ctx *ctx, const void *x_bf16, void *y_bf16) {
+    ConvTcParams p = this->p;
     p.y = reinterpret_cast<__nv_bfloat16 *>(y_bf16);
     CUtensorMap map_x;
     // the input viewed as [N * rows / s][s][W * C] with rows `row_pitch` elements apart (stride s; s = 1 is the plain [N * rows][W * C]).
@@ -466,8 +415,8 @@ extern "C" int pcnn_conv_tc_fwd(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void 
     // elements hold (rows past H are never read by a valid output) cannot reach a result, not even a NaN through the zero
     // entries of the Toeplitz operand.  The boxes are {32 elements, 1, 128 rows}: the same 8 KB tile as a 2-D box.
     {
-        const uint64_t dims[3] = {(uint64_t)plan->W * p.C, (uint64_t)plan->stride, (uint64_t)p.n_img * p.H};
-        const uint64_t str[2] = {(uint64_t)plan->row_pitch * 2, (uint64_t)plan->row_pitch * plan->stride * 2};
+        const uint64_t dims[3] = {(uint64_t)W * p.C, (uint64_t)stride, (uint64_t)p.n_img * p.H};
+        const uint64_t str[2] = {(uint64_t)row_pitch * 2, (uint64_t)row_pitch * stride * 2};
         const uint32_t box[3] = {TC_KCHUNK, 1, TC_M};
         int rc = make_map_bf16(&map_x, const_cast<void *>(x_bf16), 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B,
                                CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
@@ -475,7 +424,7 @@ extern "C" int pcnn_conv_tc_fwd(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void 
     }
     const int ntiles = p.n_mtiles * p.n_qtiles;
     const int grid = ntiles < ctx->sm_count ? ntiles : ctx->sm_count;
-    void *args[] = {&map_x, &plan->map_b, &p};
+    void *args[] = {&map_x, &map_b, &p};
     PCNN_CUDA(cudaLaunchKernel(conv_tc_fwd_variant(p.act, p.npad), dim3((unsigned)grid), dim3(TC_THREADS), args,
                                conv_tc_smem_bytes(p.V, p.R, p.npad, p.stages), ctx->stream));
     PCNN_CHECK_LAUNCH(ctx);

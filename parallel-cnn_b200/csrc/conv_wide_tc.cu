@@ -26,6 +26,8 @@
 // Warp roles (288 threads, 1 CTA/SM, persistent over tiles): warps 0-7 = two consumer warpgroups, warp 8 = TMA producer.
 #include "tc_common.cuh"
 
+#include <memory>
+
 using namespace pcnn_tc;
 
 namespace {
@@ -282,33 +284,14 @@ int conv_wide_x_maps(CUtensorMap *maps, const void *x_bf16, int N, int H, int W,
     return PCNN_OK;
 }
 
-struct ConvWidePlan {
+// a plan of pcnn_conv_wide_plan_create(_padded): w is [K][R*S*C], the KRSC master with rows of R*S*C elements and no pad
+struct ConvWidePlan : pcnn_conv_plan {
     ConvWideParams p;
     ConvWideShape sh;
     int N, H, W, C, row_pitch, image_rows, act;
-    void *d_filt = nullptr;      // [K][R*S][C] bf16
-    float *d_bias = nullptr;
     CUtensorMap map_w;
+    int fwd(pcnn_ctx *ctx, const void *x_bf16, void *y_bf16) override;
 };
-
-void conv_wide_free(ConvWidePlan *w) {
-    if (!w) return;
-    if (w->d_filt) cudaFree(w->d_filt);
-    if (w->d_bias) cudaFree(w->d_bias);
-    delete w;
-}
-
-// d_filt is [K][R*S*C]: the KRSC master with rows of R*S*C elements and no pad
-void conv_wide_operand(ConvWidePlan *w, PlanOperand *out) {
-    const int rsc = w->p.R * w->p.S * w->C;
-    *out = PlanOperand{w->d_filt, rsc, rsc, (long long)w->p.K * rsc, w->d_bias, w->p.K};
-}
-
-// fp32 KRSC filters in device memory -> d_filt [K][R*S][C] bf16 (the same order), enqueued on the context's stream
-int conv_wide_load_filters(pcnn_ctx *ctx, ConvWidePlan *w, const float *filt_dev) {
-    const int rsc = w->p.R * w->p.S * w->C;
-    return pcnn_f32_to_bf16_rows(ctx, filt_dev, w->d_filt, w->p.K, rsc, rsc);
-}
 
 // the query of the create call `fn` (its refusals name that call)
 static int wide_plan_info(const char *fn, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w,
@@ -342,11 +325,7 @@ static int wide_plan_create(const char *fn, pcnn_ctx *ctx, int N, int H, int W, 
     int rc = conv_wide_shape(fn, N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows, &sh);
     if (rc) return rc;
     pcnn_device_guard g(ctx->device);
-    struct PlanGuard {                       // frees a half-built plan on every early return below
-        ConvWidePlan *p;
-        ~PlanGuard() { conv_wide_free(p); }
-    } guard{new ConvWidePlan()};
-    ConvWidePlan *pl = guard.p;
+    std::unique_ptr<ConvWidePlan> pl(new ConvWidePlan());   // frees a half-built plan on every early return below
     pl->sh = sh;
     pl->N = N; pl->H = H; pl->W = W; pl->C = C; pl->row_pitch = row_pitch; pl->image_rows = image_rows > 0 ? image_rows : H;
     pl->act = act;
@@ -354,25 +333,16 @@ static int wide_plan_create(const char *fn, pcnn_ctx *ctx, int N, int H, int W, 
     p.Pt = sh.Pt; p.Qt = sh.Qt; p.n_pb = sh.n_pb; p.n_qb = sh.n_qb; p.tiles = sh.tiles;
     p.R = R; p.S = S; p.stride = stride; p.nch = sh.nch; p.stages = sh.stages; p.K = K;
     p.taps = sh.taps;
-    const size_t nf = (size_t)K * R * S * C;
-    PCNN_CUDA(cudaMalloc(&pl->d_filt, nf * 2));
-    {                                        // the same device conversion as pcnn_conv_plan_set_params
-        pcnn_dev_temp tf;
-        PCNN_CUDA(cudaMalloc((void **)&tf.p, nf * sizeof(float)));
-        PCNN_CUDA(cudaMemcpyAsync(tf.p, filt_host, nf * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-        if ((rc = conv_wide_load_filters(ctx, pl, tf.p))) return rc;
-        PCNN_CUDA(cudaStreamSynchronize(ctx->stream));
-    }
-    if (bias_host) {
-        PCNN_CUDA(cudaMalloc((void **)&pl->d_bias, K * sizeof(float)));
-        PCNN_CUDA(cudaMemcpy(pl->d_bias, bias_host, K * sizeof(float), cudaMemcpyHostToDevice));
-    }
-    p.bias = pl->d_bias;
+    pl->cols = pl->pitch = R * S * C;
+    pl->n = (long long)K * R * S * C;
+    pl->K = K;
+    if ((rc = pcnn_plan_upload(ctx, pl.get(), &pl->w, (size_t)pl->n * 2, filt_host, bias_host))) return rc;
+    p.bias = pl->bias;
     {
         const uint64_t dims[3] = {(uint64_t)C, (uint64_t)R * S, (uint64_t)K};
         const uint64_t str[2] = {(uint64_t)C * 2, (uint64_t)R * S * C * 2};
         const uint32_t box[3] = {WD_KC, 1, (uint32_t)sh.npad};
-        rc = make_map_bf16(&pl->map_w, pl->d_filt, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+        rc = make_map_bf16(&pl->map_w, pl->w, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
         if (rc) return rc;
     }
     static bool configured[64] = {};        // function attributes are per device
@@ -383,8 +353,7 @@ static int wide_plan_create(const char *fn, pcnn_ctx *ctx, int N, int H, int W, 
                                                WD_SMEM_BUDGET + 2048));
         configured[ctx->device & 63] = true;
     }
-    *out = conv_plan_wrap_wide(pl);
-    guard.p = nullptr;
+    *out = pl.release();
     return PCNN_OK;
 }
 
@@ -402,27 +371,23 @@ extern "C" int pcnn_conv_wide_plan_create_padded(pcnn_ctx *ctx, int N, int H, in
                             act, filt_host, bias_host, out);
 }
 
-int conv_wide_fwd(pcnn_ctx *ctx, const ConvWidePlan *pl, const void *x_bf16, void *y_bf16) {
+int ConvWidePlan::fwd(pcnn_ctx *ctx, const void *x_bf16, void *y_bf16) {
     PCNN_REQUIRE(((uintptr_t)y_bf16 & 15) == 0, PCNN_ERR_ARG, "pcnn_conv_tc_fwd: the output must be 16-byte aligned (TMA stores)");
-    const ConvWideShape &sh = pl->sh;
-    const int st = pl->p.stride, C = pl->C, K = pl->p.K;
     ConvWideMaps m;
     memset(&m, 0, sizeof(m));
-    m.w = pl->map_w;
-    int rc = conv_wide_x_maps(m.x, x_bf16, pl->N, pl->H, pl->W, C, pl->p.R, pl->p.S, st, sh.taps, pl->row_pitch, pl->image_rows, sh.Pt,
-                              sh.Qt);
+    m.w = map_w;
+    int rc = conv_wide_x_maps(m.x, x_bf16, N, H, W, C, p.R, p.S, p.stride, sh.taps, row_pitch, image_rows, sh.Pt, sh.Qt);
     if (rc) return rc;
     {
-        const uint64_t dims[4] = {(uint64_t)K, (uint64_t)sh.Q, (uint64_t)sh.P, (uint64_t)pl->N};
+        const uint64_t dims[4] = {(uint64_t)K, (uint64_t)sh.Q, (uint64_t)sh.P, (uint64_t)N};
         const uint64_t str[3] = {(uint64_t)K * 2, (uint64_t)sh.Q * K * 2, (uint64_t)sh.P * sh.Q * K * 2};
         const uint32_t box[4] = {64, (uint32_t)(sh.Pt >= 2 ? sh.Qt : 64), (uint32_t)(sh.Pt >= 2 ? sh.Pt / 2 : 1), 1};
         rc = make_map_bf16(&m.y, y_bf16, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE);
         if (rc) return rc;
     }
-    ConvWideParams p = pl->p;
     const int grid = p.tiles < ctx->sm_count ? p.tiles : ctx->sm_count;
     void *args[] = {&m, &p};
-    PCNN_CUDA(cudaLaunchKernel(conv_wide_variant(pl->act, sh.npad), dim3((unsigned)grid), dim3(WD_THREADS), args,
+    PCNN_CUDA(cudaLaunchKernel(conv_wide_variant(act, sh.npad), dim3((unsigned)grid), dim3(WD_THREADS), args,
                                wide_smem_bytes(sh.npad, p.stages), ctx->stream));
     PCNN_CHECK_LAUNCH(ctx);
     return PCNN_OK;

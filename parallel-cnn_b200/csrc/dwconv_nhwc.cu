@@ -18,6 +18,8 @@
 
 #include <cuda_bf16.h>
 
+#include <memory>
+
 namespace {
 
 constexpr int DW_THREADS = 256;
@@ -301,28 +303,13 @@ wgrad_fn wgrad_variant(int S) {
 
 }  // namespace
 
-struct DwConvPlan {
+// a plan of pcnn_dwconv_plan_create: w is [C][R][S], the fp32 master's element order (one row of n elements)
+struct DwConvPlan : pcnn_conv_plan {
+    static constexpr const char *made_by = "pcnn_dwconv_plan_create";
     DwArgs a;
-    __nv_bfloat16 *d_w = nullptr;    // [C][R][S]: the fp32 master's element order
-    float *d_bias = nullptr;
+    const __nv_bfloat16 *wop() const { return static_cast<const __nv_bfloat16 *>(w); }
+    int fwd(pcnn_ctx *ctx, const void *x_bf16, void *y_bf16) override;
 };
-
-void dwconv_free(DwConvPlan *d) {
-    if (!d) return;
-    if (d->d_w) cudaFree(d->d_w);
-    if (d->d_bias) cudaFree(d->d_bias);
-    delete d;
-}
-
-void dwconv_operand(DwConvPlan *d, PlanOperand *out) {
-    const int n = d->a.C * d->a.R * d->a.S;
-    *out = PlanOperand{d->d_w, n, n, (long long)n, d->d_bias, d->a.C};
-}
-
-int dwconv_load_filters(pcnn_ctx *ctx, DwConvPlan *d, const float *filt_dev) {
-    const int n = d->a.C * d->a.R * d->a.S;
-    return pcnn_f32_to_bf16_rows(ctx, filt_dev, d->d_w, 1, n, n);
-}
 
 extern "C" int pcnn_dwconv_info(int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int *out9) {
     const char *fn = "pcnn_dwconv_info";
@@ -348,33 +335,18 @@ extern "C" int pcnn_dwconv_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C
     if (rc) return rc;
     a.act = act;
     pcnn_device_guard g(ctx->device);
-    struct PlanGuard {                       // frees a half-built plan on every early return below
-        DwConvPlan *p;
-        ~PlanGuard() { dwconv_free(p); }
-    } guard{new DwConvPlan()};
-    DwConvPlan *pl = guard.p;
+    std::unique_ptr<DwConvPlan> pl(new DwConvPlan());   // frees a half-built plan on every early return below
     pl->a = a;
-    const size_t nf = (size_t)C * R * S;
-    PCNN_CUDA(cudaMalloc((void **)&pl->d_w, nf * 2));
-    {                                        // the same device conversion as pcnn_conv_plan_set_params
-        pcnn_dev_temp tf;
-        PCNN_CUDA(cudaMalloc((void **)&tf.p, nf * sizeof(float)));
-        PCNN_CUDA(cudaMemcpyAsync(tf.p, filt_host, nf * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-        if ((rc = dwconv_load_filters(ctx, pl, tf.p))) return rc;
-        PCNN_CUDA(cudaStreamSynchronize(ctx->stream));
-    }
-    if (bias_host) {
-        PCNN_CUDA(cudaMalloc((void **)&pl->d_bias, (size_t)C * sizeof(float)));
-        PCNN_CUDA(cudaMemcpy(pl->d_bias, bias_host, (size_t)C * sizeof(float), cudaMemcpyHostToDevice));
-    }
-    *out = conv_plan_wrap_dw(pl);
-    guard.p = nullptr;
+    pl->n = (long long)C * R * S;
+    pl->cols = pl->pitch = (int)pl->n;
+    pl->K = C;
+    if ((rc = pcnn_plan_upload(ctx, pl.get(), &pl->w, (size_t)pl->n * 2, filt_host, bias_host))) return rc;
+    *out = pl.release();
     return PCNN_OK;
 }
 
-int dwconv_fwd(pcnn_ctx *ctx, const DwConvPlan *pl, const void *x_bf16, void *y_bf16) {
+int DwConvPlan::fwd(pcnn_ctx *ctx, const void *x_bf16, void *y_bf16) {
     const char *fn = "pcnn_conv_tc_fwd";
-    const DwArgs &a = pl->a;
     PCNN_REQUIRE(aligned16(y_bf16), PCNN_ERR_ARG, "%s: the output must be 16-byte aligned", fn);
     const size_t xb = (size_t)a.N * a.H * a.W * a.C * 2, yb = (size_t)a.M * a.C * 2;
     PCNN_REQUIRE(!overlap(x_bf16, xb, y_bf16, yb), PCNN_ERR_ARG, "%s: overlapping buffers: x and y of a depthwise plan must not share memory",
@@ -383,16 +355,10 @@ int dwconv_fwd(pcnn_ctx *ctx, const DwConvPlan *pl, const void *x_bf16, void *y_
     const auto *x = static_cast<const __nv_bfloat16 *>(x_bf16);
     auto *y = static_cast<__nv_bfloat16 *>(y_bf16);
     if (a.C % 8 == 0)
-        k_dwconv_fwd<8><<<grid, DW_THREADS, 0, ctx->stream>>>(x, pl->d_w, pl->d_bias, y, a);
+        k_dwconv_fwd<8><<<grid, DW_THREADS, 0, ctx->stream>>>(x, wop(), bias, y, a);
     else
-        k_dwconv_fwd<1><<<grid, DW_THREADS, 0, ctx->stream>>>(x, pl->d_w, pl->d_bias, y, a);
+        k_dwconv_fwd<1><<<grid, DW_THREADS, 0, ctx->stream>>>(x, wop(), bias, y, a);
     PCNN_CHECK_LAUNCH(ctx);
-    return PCNN_OK;
-}
-
-static int dw_of(const char *fn, pcnn_conv_plan *plan, DwConvPlan **out) {
-    *out = plan ? conv_plan_dw(plan) : nullptr;
-    PCNN_REQUIRE(*out, PCNN_ERR_ARG, "%s: the plan was not made by pcnn_dwconv_plan_create", fn);
     return PCNN_OK;
 }
 
@@ -400,7 +366,7 @@ extern "C" int pcnn_dwconv_wgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void
     const char *fn = "pcnn_dwconv_wgrad";
     PCNN_REQUIRE(ctx && plan && x_bf16 && dy_bf16 && dw_f32, PCNN_ERR_ARG, "%s: NULL argument", fn);
     DwConvPlan *pl;
-    int rc = dw_of(fn, plan, &pl);
+    int rc = plan_as(fn, plan, &pl);
     if (rc) return rc;
     PCNN_REQUIRE(aligned16(x_bf16) && aligned16(dy_bf16) && aligned16(dw_f32), PCNN_ERR_ARG, "%s: x, dy and dw must be 16-byte aligned", fn);
     const DwArgs &a = pl->a;
@@ -423,7 +389,7 @@ extern "C" int pcnn_dwconv_dgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void
     const char *fn = "pcnn_dwconv_dgrad";
     PCNN_REQUIRE(ctx && plan && dy_bf16 && dx_bf16, PCNN_ERR_ARG, "%s: NULL argument", fn);
     DwConvPlan *pl;
-    int rc = dw_of(fn, plan, &pl);
+    int rc = plan_as(fn, plan, &pl);
     if (rc) return rc;
     PCNN_REQUIRE(aligned16(dy_bf16) && aligned16(dx_bf16), PCNN_ERR_ARG, "%s: dy and dx must be 16-byte aligned", fn);
     const DwArgs &a = pl->a;
@@ -434,9 +400,9 @@ extern "C" int pcnn_dwconv_dgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void
     const auto *dy = static_cast<const __nv_bfloat16 *>(dy_bf16);
     auto *dx = static_cast<__nv_bfloat16 *>(dx_bf16);
     if (a.C % 8 == 0)
-        k_dwconv_dgrad<8><<<grid, DW_THREADS, 0, ctx->stream>>>(dy, pl->d_w, dx, a);
+        k_dwconv_dgrad<8><<<grid, DW_THREADS, 0, ctx->stream>>>(dy, pl->wop(), dx, a);
     else
-        k_dwconv_dgrad<1><<<grid, DW_THREADS, 0, ctx->stream>>>(dy, pl->d_w, dx, a);
+        k_dwconv_dgrad<1><<<grid, DW_THREADS, 0, ctx->stream>>>(dy, pl->wop(), dx, a);
     PCNN_CHECK_LAUNCH(ctx);
     return PCNN_OK;
 }

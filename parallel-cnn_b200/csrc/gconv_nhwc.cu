@@ -20,6 +20,7 @@
 #include <cuda_bf16.h>
 
 #include <algorithm>
+#include <memory>
 
 namespace {
 
@@ -348,28 +349,13 @@ int smem_opt_in(const void *k, size_t bytes) {
 
 }  // namespace
 
-struct GConvPlan {
+// a plan of pcnn_gconv_plan_create: w is [K][R][S][Cg], the fp32 master's element order (one row of n elements)
+struct GConvPlan : pcnn_conv_plan {
+    static constexpr const char *made_by = "pcnn_gconv_plan_create";
     GcArgs a;
-    __nv_bfloat16 *d_w = nullptr;    // [K][R][S][Cg]: the fp32 master's element order
-    float *d_bias = nullptr;
+    const __nv_bfloat16 *wop() const { return static_cast<const __nv_bfloat16 *>(w); }
+    int fwd(pcnn_ctx *ctx, const void *x_bf16, void *y_bf16) override;
 };
-
-void gconv_free(GConvPlan *d) {
-    if (!d) return;
-    if (d->d_w) cudaFree(d->d_w);
-    if (d->d_bias) cudaFree(d->d_bias);
-    delete d;
-}
-
-void gconv_operand(GConvPlan *d, PlanOperand *out) {
-    const int n = d->a.K * d->a.RSC;
-    *out = PlanOperand{d->d_w, n, n, (long long)n, d->d_bias, d->a.K};
-}
-
-int gconv_load_filters(pcnn_ctx *ctx, GConvPlan *d, const float *filt_dev) {
-    const int n = d->a.K * d->a.RSC;
-    return pcnn_f32_to_bf16_rows(ctx, filt_dev, d->d_w, 1, n, n);
-}
 
 extern "C" int pcnn_gconv_info(int N, int H, int W, int C, int K, int G, int R, int S, int stride, int pad_h, int pad_w, int *out16) {
     const char *fn = "pcnn_gconv_info";
@@ -396,33 +382,18 @@ extern "C" int pcnn_gconv_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C,
     if (rc) return rc;
     a.act = act;
     pcnn_device_guard g(ctx->device);
-    struct PlanGuard {                       // frees a half-built plan on every early return below
-        GConvPlan *p;
-        ~PlanGuard() { gconv_free(p); }
-    } guard{new GConvPlan()};
-    GConvPlan *pl = guard.p;
+    std::unique_ptr<GConvPlan> pl(new GConvPlan());   // frees a half-built plan on every early return below
     pl->a = a;
-    const size_t nf = (size_t)K * a.RSC;
-    PCNN_CUDA(cudaMalloc((void **)&pl->d_w, nf * 2));
-    {                                        // the same device conversion as pcnn_conv_plan_set_params
-        pcnn_dev_temp tf;
-        PCNN_CUDA(cudaMalloc((void **)&tf.p, nf * sizeof(float)));
-        PCNN_CUDA(cudaMemcpyAsync(tf.p, filt_host, nf * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-        if ((rc = gconv_load_filters(ctx, pl, tf.p))) return rc;
-        PCNN_CUDA(cudaStreamSynchronize(ctx->stream));
-    }
-    if (bias_host) {
-        PCNN_CUDA(cudaMalloc((void **)&pl->d_bias, (size_t)K * sizeof(float)));
-        PCNN_CUDA(cudaMemcpy(pl->d_bias, bias_host, (size_t)K * sizeof(float), cudaMemcpyHostToDevice));
-    }
-    *out = conv_plan_wrap_gconv(pl);
-    guard.p = nullptr;
+    pl->n = (long long)K * a.RSC;
+    pl->cols = pl->pitch = (int)pl->n;
+    pl->K = K;
+    if ((rc = pcnn_plan_upload(ctx, pl.get(), &pl->w, (size_t)pl->n * 2, filt_host, bias_host))) return rc;
+    *out = pl.release();
     return PCNN_OK;
 }
 
-int gconv_fwd(pcnn_ctx *ctx, const GConvPlan *pl, const void *x_bf16, void *y_bf16) {
+int GConvPlan::fwd(pcnn_ctx *ctx, const void *x_bf16, void *y_bf16) {
     const char *fn = "pcnn_conv_tc_fwd";
-    const GcArgs &a = pl->a;
     PCNN_REQUIRE(aligned16(y_bf16), PCNN_ERR_ARG, "%s: the output must be 16-byte aligned", fn);
     const size_t xb = (size_t)a.N * a.H * a.W * a.C * 2, yb = (size_t)a.M * a.K * 2;
     PCNN_REQUIRE(!overlap(x_bf16, xb, y_bf16, yb), PCNN_ERR_ARG, "%s: overlapping buffers: x and y of a grouped plan must not share memory",
@@ -432,15 +403,9 @@ int gconv_fwd(pcnn_ctx *ctx, const GConvPlan *pl, const void *x_bf16, void *y_bf
     int rc = smem_opt_in((const void *)k, smem);
     if (rc) return rc;
     const dim3 grid((unsigned)((a.fstrips + a.flanes - 1) / a.flanes), (unsigned)a.fslices);
-    k<<<grid, GC_THREADS, smem, ctx->stream>>>(static_cast<const __nv_bfloat16 *>(x_bf16), pl->d_w, pl->d_bias,
+    k<<<grid, GC_THREADS, smem, ctx->stream>>>(static_cast<const __nv_bfloat16 *>(x_bf16), wop(), bias,
                                                 static_cast<__nv_bfloat16 *>(y_bf16), a);
     PCNN_CHECK_LAUNCH(ctx);
-    return PCNN_OK;
-}
-
-static int gc_of(const char *fn, pcnn_conv_plan *plan, GConvPlan **out) {
-    *out = plan ? conv_plan_gconv(plan) : nullptr;
-    PCNN_REQUIRE(*out, PCNN_ERR_ARG, "%s: the plan was not made by pcnn_gconv_plan_create", fn);
     return PCNN_OK;
 }
 
@@ -448,7 +413,7 @@ extern "C" int pcnn_gconv_wgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void 
     const char *fn = "pcnn_gconv_wgrad";
     PCNN_REQUIRE(ctx && plan && x_bf16 && dy_bf16 && dw_f32, PCNN_ERR_ARG, "%s: NULL argument", fn);
     GConvPlan *pl;
-    int rc = gc_of(fn, plan, &pl);
+    int rc = plan_as(fn, plan, &pl);
     if (rc) return rc;
     PCNN_REQUIRE(aligned16(x_bf16) && aligned16(dy_bf16) && aligned16(dw_f32), PCNN_ERR_ARG, "%s: x, dy and dw must be 16-byte aligned", fn);
     const GcArgs &a = pl->a;
@@ -469,7 +434,7 @@ extern "C" int pcnn_gconv_dgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void 
     const char *fn = "pcnn_gconv_dgrad";
     PCNN_REQUIRE(ctx && plan && dy_bf16 && dx_bf16, PCNN_ERR_ARG, "%s: NULL argument", fn);
     GConvPlan *pl;
-    int rc = gc_of(fn, plan, &pl);
+    int rc = plan_as(fn, plan, &pl);
     if (rc) return rc;
     PCNN_REQUIRE(aligned16(dy_bf16) && aligned16(dx_bf16), PCNN_ERR_ARG, "%s: dy and dx must be 16-byte aligned", fn);
     const GcArgs &a = pl->a;
@@ -480,7 +445,7 @@ extern "C" int pcnn_gconv_dgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void 
     const size_t smem = (size_t)a.dwid * a.vc * a.R * a.S * a.Kg * 2;
     if ((rc = smem_opt_in((const void *)k, smem))) return rc;
     const dim3 grid((unsigned)((a.dstrips + a.dlanes - 1) / a.dlanes), (unsigned)a.dslices);
-    k<<<grid, GC_THREADS, smem, ctx->stream>>>(static_cast<const __nv_bfloat16 *>(dy_bf16), pl->d_w, static_cast<__nv_bfloat16 *>(dx_bf16),
+    k<<<grid, GC_THREADS, smem, ctx->stream>>>(static_cast<const __nv_bfloat16 *>(dy_bf16), pl->wop(), static_cast<__nv_bfloat16 *>(dx_bf16),
                                                 a);
     PCNN_CHECK_LAUNCH(ctx);
     return PCNN_OK;

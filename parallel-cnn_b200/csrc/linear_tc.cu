@@ -29,6 +29,7 @@
 
 #include <cuda_bf16.h>
 #include <math.h>
+#include <memory>
 
 using namespace pcnn_tc;
 
@@ -463,31 +464,16 @@ static int linear_shape(int N, int P, int Q, int C, int O, int row_pitch, int im
     return PCNN_OK;
 }
 
-struct LinearPlan {
+// a plan of pcnn_linear_plan_create: w is [O][P][wpitch], rows of Q*C in-row elements; the pad columns are zeroed at creation and
+// nothing writes them again
+struct LinearPlan : pcnn_conv_plan {
+    static constexpr const char *made_by = "pcnn_linear_plan_create";
     LinearShape sh;
     int act;
-    __nv_bfloat16 *d_w = nullptr;    // [O][P][wpitch]
-    float *d_bias = nullptr;
     CUtensorMap map_w_fwd;           // {QC, P, O}, box {64, 1, npad}: K-major B of the forward
     CUtensorMap map_w_dgrad;         // the same tensor, box {64, 1, 64}: MN-major B of the input gradient
+    int fwd(pcnn_ctx *ctx, const void *x_bf16, void *y_bf16) override;
 };
-
-void linear_free(LinearPlan *l) {
-    if (!l) return;
-    if (l->d_w) cudaFree(l->d_w);
-    if (l->d_bias) cudaFree(l->d_bias);
-    delete l;
-}
-
-// d_w is [O][P][wpitch]: rows of Q*C in-row elements; the pad columns were zeroed at creation and nothing writes them again
-void linear_operand(LinearPlan *l, PlanOperand *out) {
-    *out = PlanOperand{l->d_w, l->sh.QC, l->sh.wpitch, (long long)l->sh.O * l->sh.F, l->d_bias, l->sh.O};
-}
-
-// fp32 [O][P][Q][C] in device memory -> the plan's bf16 [O][P][wpitch] (pad columns zero), on the context's stream
-int linear_load_weights(pcnn_ctx *ctx, LinearPlan *l, const float *w_dev) {
-    return pcnn_f32_to_bf16_rows(ctx, w_dev, l->d_w, (long)l->sh.O * l->sh.P, l->sh.QC, l->sh.wpitch);
-}
 
 typedef void (*linear_fn)(const LinearMaps, const LinearFwdParams);
 typedef void (*wgrad_fn)(const LinearMaps, const LinearWgradParams);
@@ -573,49 +559,35 @@ extern "C" int pcnn_linear_plan_create(pcnn_ctx *ctx, int N, int P, int Q, int C
     if (rc) return rc;
     pcnn_device_guard g(ctx->device);
     if ((rc = configure(ctx))) return rc;
-    struct PlanGuard {                       // frees a half-built plan on every early return below
-        LinearPlan *p;
-        ~PlanGuard() { linear_free(p); }
-    } guard{new LinearPlan()};
-    LinearPlan *pl = guard.p;
+    std::unique_ptr<LinearPlan> pl(new LinearPlan());   // frees a half-built plan on every early return below
     pl->sh = s;
     pl->act = act;
-    const size_t nw = (size_t)O * s.F;
-    PCNN_CUDA(cudaMalloc((void **)&pl->d_w, (size_t)O * P * s.wpitch * 2));
-    {                                        // the same device conversion as pcnn_conv_plan_set_params
-        pcnn_dev_temp tf;
-        PCNN_CUDA(cudaMalloc((void **)&tf.p, nw * sizeof(float)));
-        PCNN_CUDA(cudaMemcpyAsync(tf.p, w_host, nw * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-        if ((rc = linear_load_weights(ctx, pl, tf.p))) return rc;
-        PCNN_CUDA(cudaStreamSynchronize(ctx->stream));
-    }
-    if (b_host) {
-        PCNN_CUDA(cudaMalloc((void **)&pl->d_bias, O * sizeof(float)));
-        PCNN_CUDA(cudaMemcpy(pl->d_bias, b_host, O * sizeof(float), cudaMemcpyHostToDevice));
-    }
+    pl->cols = s.QC; pl->pitch = s.wpitch;
+    pl->n = (long long)O * s.F;
+    pl->K = O;
+    if ((rc = pcnn_plan_upload(ctx, pl.get(), &pl->w, (size_t)O * P * s.wpitch * 2, w_host, b_host))) return rc;
     const uint64_t dims[3] = {(uint64_t)s.QC, (uint64_t)P, (uint64_t)O};
     const uint64_t str[2] = {(uint64_t)s.wpitch * 2, (uint64_t)P * s.wpitch * 2};
     const uint32_t box_f[3] = {LN_KC, 1, (uint32_t)s.npad}, box_d[3] = {LN_KC, 1, 64};
-    if ((rc = make_map_bf16(&pl->map_w_fwd, pl->d_w, 3, dims, str, box_f, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B)))
+    if ((rc = make_map_bf16(&pl->map_w_fwd, pl->w, 3, dims, str, box_f, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B)))
         return rc;
-    if ((rc = make_map_bf16(&pl->map_w_dgrad, pl->d_w, 3, dims, str, box_d, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B)))
+    if ((rc = make_map_bf16(&pl->map_w_dgrad, pl->w, 3, dims, str, box_d, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B)))
         return rc;
-    *out = conv_plan_wrap_linear(pl);
-    guard.p = nullptr;
+    *out = pl.release();
     return PCNN_OK;
 }
 
-int linear_fwd(pcnn_ctx *ctx, const LinearPlan *pl, const void *x_bf16, void *y_bf16) {
+int LinearPlan::fwd(pcnn_ctx *ctx, const void *x_bf16, void *y_bf16) {
     PCNN_REQUIRE(((uintptr_t)y_bf16 & 15) == 0, PCNN_ERR_ARG, "pcnn_conv_tc_fwd: the output must be 16-byte aligned");
-    const LinearShape &s = pl->sh;
+    const LinearShape &s = sh;
     LinearMaps m;
     memset(&m, 0, sizeof(m));
     int rc = x_map(&m.a, x_bf16, s);
     if (rc) return rc;
-    m.b = pl->map_w_fwd;
+    m.b = map_w_fwd;
     LinearFwdParams p;
     p.N = s.N; p.O = s.O; p.nch = s.nch; p.steps = s.fsteps; p.splits = s.fsplits; p.mtiles = s.mtiles; p.units = s.funits;
-    p.stages = s.fstages; p.act = pl->act; p.bias = pl->d_bias;
+    p.stages = s.fstages; p.act = act; p.bias = bias;
     p.y = static_cast<__nv_bfloat16 *>(y_bf16);
     p.slots = nullptr;
     const long total = (long)s.N * s.O;
@@ -628,15 +600,9 @@ int linear_fwd(pcnn_ctx *ctx, const LinearPlan *pl, const void *x_bf16, void *y_
     if (s.fsplits > 1) {
         long blocks = (total + 255) / 256;
         if (blocks > (long)ctx->sm_count * 8) blocks = (long)ctx->sm_count * 8;
-        k_linear_fwd_reduce<<<(int)blocks, 256, 0, ctx->stream>>>(p.slots, s.fsplits, pl->d_bias, pl->act, p.y, total, s.O);
+        k_linear_fwd_reduce<<<(int)blocks, 256, 0, ctx->stream>>>(p.slots, s.fsplits, bias, act, p.y, total, s.O);
         PCNN_CHECK_LAUNCH(ctx);
     }
-    return PCNN_OK;
-}
-
-static int linear_of(const char *fn, pcnn_conv_plan *plan, LinearPlan **out) {
-    *out = plan ? conv_plan_linear(plan) : nullptr;
-    PCNN_REQUIRE(*out, PCNN_ERR_ARG, "%s: the plan was not made by pcnn_linear_plan_create", fn);
     return PCNN_OK;
 }
 
@@ -644,7 +610,7 @@ extern "C" int pcnn_linear_wgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void
     const char *fn = "pcnn_linear_wgrad";
     PCNN_REQUIRE(ctx && plan && x_bf16 && dy_bf16 && dw_f32, PCNN_ERR_ARG, "%s: NULL argument", fn);
     LinearPlan *pl;
-    int rc = linear_of(fn, plan, &pl);
+    int rc = plan_as(fn, plan, &pl);
     if (rc) return rc;
     PCNN_REQUIRE(((uintptr_t)x_bf16 & 15) == 0 && ((uintptr_t)dy_bf16 & 15) == 0 && ((uintptr_t)dw_f32 & 15) == 0, PCNN_ERR_ARG,
                  "%s: x, dy and dw must be 16-byte aligned", fn);
@@ -674,7 +640,7 @@ extern "C" int pcnn_linear_dgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void
     const char *fn = "pcnn_linear_dgrad";
     PCNN_REQUIRE(ctx && plan && dy_bf16 && dx_bf16, PCNN_ERR_ARG, "%s: NULL argument", fn);
     LinearPlan *pl;
-    int rc = linear_of(fn, plan, &pl);
+    int rc = plan_as(fn, plan, &pl);
     if (rc) return rc;
     PCNN_REQUIRE(((uintptr_t)dy_bf16 & 15) == 0 && ((uintptr_t)dx_bf16 & 15) == 0, PCNN_ERR_ARG, "%s: dy and dx must be 16-byte aligned",
                  fn);

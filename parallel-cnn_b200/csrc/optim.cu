@@ -210,24 +210,23 @@ extern "C" int pcnn_optim_create(pcnn_ctx *ctx, const pcnn_optim_config *cfg, co
             for (int j = 0; j < i; ++j)
                 PCNN_REQUIRE(!(t[j].plan == x.plan && t[j].plan_part == x.plan_part), PCNN_ERR_ARG,
                              "%s: tensors %d and %d: the same plan part (%d) listed twice", fn, j, i, x.plan_part);
-            PlanOperand op;
-            conv_plan_operand(x.plan, &op);
+            const pcnn_conv_plan &pl = *x.plan;
             if (x.plan_part == 1) {
-                PCNN_REQUIRE(x.n == op.n, PCNN_ERR_ARG, "%s: tensor %d: n = %ld, but the plan's filters / weights have %lld elements", fn, i,
-                             x.n, op.n);
-                if (op.w) {
-                    e.dst = static_cast<__nv_bfloat16 *>(op.w);
-                    e.cols = op.cols; e.pitch = op.pitch;
-                    const long long rows = op.n / op.cols;
-                    ranges.push_back({(uintptr_t)op.w, (uintptr_t)op.w + (size_t)((rows - 1) * op.pitch + op.cols) * 2, i, "plan operand"});
-                    vec_ok = vec_ok && aligned(op.w, 8) && op.cols % 4 == 0 && op.pitch % 4 == 0;
+                PCNN_REQUIRE(x.n == pl.n, PCNN_ERR_ARG, "%s: tensor %d: n = %ld, but the plan's filters / weights have %lld elements", fn, i,
+                             x.n, pl.n);
+                if (pl.w) {
+                    e.dst = static_cast<__nv_bfloat16 *>(pl.w);
+                    e.cols = pl.cols; e.pitch = pl.pitch;
+                    const long long rows = pl.n / pl.cols;
+                    ranges.push_back({(uintptr_t)pl.w, (uintptr_t)pl.w + (size_t)((rows - 1) * pl.pitch + pl.cols) * 2, i, "plan operand"});
+                    vec_ok = vec_ok && aligned(pl.w, 8) && pl.cols % 4 == 0 && pl.pitch % 4 == 0;
                 }
             } else {
-                PCNN_REQUIRE(op.bias, PCNN_ERR_ARG, "%s: tensor %d: a bias for a plan created without one", fn, i);
-                PCNN_REQUIRE(x.n == op.K, PCNN_ERR_ARG, "%s: tensor %d: n = %ld, but the plan's bias has %d elements", fn, i, x.n, op.K);
-                e.mirror = op.bias;
-                ranges.push_back({(uintptr_t)op.bias, (uintptr_t)op.bias + (size_t)op.K * sizeof(float), i, "plan bias"});
-                vec_ok = vec_ok && aligned(op.bias, 16);
+                PCNN_REQUIRE(pl.bias, PCNN_ERR_ARG, "%s: tensor %d: a bias for a plan created without one", fn, i);
+                PCNN_REQUIRE(x.n == pl.K, PCNN_ERR_ARG, "%s: tensor %d: n = %ld, but the plan's bias has %d elements", fn, i, x.n, pl.K);
+                e.mirror = pl.bias;
+                ranges.push_back({(uintptr_t)pl.bias, (uintptr_t)pl.bias + (size_t)pl.K * sizeof(float), i, "plan bias"});
+                vec_ok = vec_ok && aligned(pl.bias, 16);
             }
         }
         e.vec = vec_ok ? 1 : 0;

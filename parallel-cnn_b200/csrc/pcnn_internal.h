@@ -226,63 +226,45 @@ int pcnn_persist_run(pcnn_ctx *ctx, const pcnn_split_binding &s, int B, long nst
 int pcnn_persist_check(pcnn_ctx *ctx);
 // comm.cu
 int pcnn_comm_allreduce_packed(pcnn_ctx *ctx);
-// conv_wide_tc.cu: the wide-channel forward.  conv_tc.cu owns the opaque pcnn_conv_plan; a plan made by
-// pcnn_conv_wide_plan_create holds a ConvWidePlan, which pcnn_conv_tc_fwd runs and pcnn_conv_tc_plan_destroy frees.
-struct ConvWidePlan;
-int conv_wide_fwd(pcnn_ctx *ctx, const ConvWidePlan *w, const void *x_bf16, void *y_bf16);
-void conv_wide_free(ConvWidePlan *w);
-pcnn_conv_plan *conv_plan_wrap_wide(ConvWidePlan *w);   // conv_tc.cu; takes ownership
-// What a plan holds of its parameters, for refreshing them from fp32 masters in device memory (conv_plan_operand):
-//   - w: the bf16 operand, element i of the fp32 master (KRSC, or [O][P][Q][C] for a linear plan) at w[(i / cols) * pitch + i % cols],
-//     or null for a row-Toeplitz plan, where one filter element feeds V * Qt operand entries (pcnn_conv_plan_set_params gathers them);
+// The opaque plan of include/pcnn.h: what every kernel family's plan holds of its parameters, which pcnn_conv_plan_set_params and
+// the optimizer (optim.cu) refresh from fp32 masters in device memory, and the family's forward.  Each family derives from it:
+// ToeplitzPlan (conv_tc.cu), ConvWidePlan (conv_wide_tc.cu), LinearPlan (linear_tc.cu), DwConvPlan (dwconv_nhwc.cu) and GConvPlan
+// (gconv_nhwc.cu).  pcnn_conv_tc_fwd runs fwd, pcnn_conv_tc_plan_destroy deletes the plan.
+//   - w: the bf16 operand, element i of the fp32 master (KRSC, [O][P][Q][C] for a linear plan, [C][R][S] for a depthwise one,
+//     [K][R][S][Cg] for a grouped one) at w[(i / cols) * pitch + i % cols], or null for a row-Toeplitz plan, where one filter
+//     element feeds V * Qt operand entries (its load_filters gathers them; the optimizer leaves them to pcnn_conv_plan_set_params);
 //   - n: the elements of that master; bias: the plan's fp32 copy of the bias ([K]), null for a plan without one.
-// Nothing but the plan module knows the operand's layout: pcnn_conv_plan_set_params and the optimizer (optim.cu) ask this.
-struct PlanOperand {
-    void *w;
-    int cols, pitch;
-    long long n;
-    float *bias;
-    int K;
+struct pcnn_conv_plan {
+    void *w = nullptr;
+    int cols = 0, pitch = 0;
+    long long n = 0;
+    float *bias = nullptr;
+    int K = 0;
+    virtual ~pcnn_conv_plan() {
+        if (w) cudaFree(w);
+        if (bias) cudaFree(bias);
+    }
+    // y from x with the plan's operand, enqueued on the context's stream (pcnn_conv_tc_fwd has checked the arguments and x's alignment)
+    virtual int fwd(pcnn_ctx *ctx, const void *x_bf16, void *y_bf16) = 0;
+    // the operand from the fp32 master in device memory, rounded to bf16 on the context's stream; by default the layout of w above
+    virtual int load_filters(pcnn_ctx *ctx, const float *filt_dev) {
+        return pcnn_f32_to_bf16_rows(ctx, filt_dev, w, (long)(n / cols), cols, pitch);
+    }
 };
-void conv_plan_operand(pcnn_conv_plan *plan, PlanOperand *out);   // conv_tc.cu
-void conv_wide_operand(ConvWidePlan *w, PlanOperand *out);
-// the filters from fp32 KRSC in device memory, rounded to bf16 on the context's stream (pcnn_conv_plan_set_params and the create calls)
-int conv_wide_load_filters(pcnn_ctx *ctx, ConvWidePlan *w, const float *filt_dev);
-// linear_tc.cu: a plan of pcnn_linear_plan_create is a pcnn_conv_plan holding a LinearPlan, run, refreshed and freed like the
-// wide one; conv_plan_linear is null for a convolution plan
-struct LinearPlan;
-int linear_fwd(pcnn_ctx *ctx, const LinearPlan *l, const void *x_bf16, void *y_bf16);
-void linear_free(LinearPlan *l);
-void linear_operand(LinearPlan *l, PlanOperand *out);
-int linear_load_weights(pcnn_ctx *ctx, LinearPlan *l, const float *w_dev);
-pcnn_conv_plan *conv_plan_wrap_linear(LinearPlan *l);   // conv_tc.cu; takes ownership
-LinearPlan *conv_plan_linear(pcnn_conv_plan *plan);
-// dwconv_nhwc.cu: a plan of pcnn_dwconv_plan_create holds a DwConvPlan, run, refreshed and freed like the linear one; its bf16
-// operand is [C][R][S], the fp32 master's element order (one row of C R S elements); conv_plan_dw is null for any other plan
-struct DwConvPlan;
-int dwconv_fwd(pcnn_ctx *ctx, const DwConvPlan *d, const void *x_bf16, void *y_bf16);
-void dwconv_free(DwConvPlan *d);
-void dwconv_operand(DwConvPlan *d, PlanOperand *out);
-int dwconv_load_filters(pcnn_ctx *ctx, DwConvPlan *d, const float *filt_dev);
-pcnn_conv_plan *conv_plan_wrap_dw(DwConvPlan *d);   // conv_tc.cu; takes ownership
-DwConvPlan *conv_plan_dw(pcnn_conv_plan *plan);
+// The tail every create call shares (conv_tc.cu): `bytes` of device memory at *operand (the plan's operand: w, or the Toeplitz
+// matrices), the n host filters converted into it by load_filters through a temporary device copy, a synchronisation, and the K
+// host bias values copied to plan->bias when bias_host is given.
+int pcnn_plan_upload(pcnn_ctx *ctx, pcnn_conv_plan *plan, void **operand, size_t bytes, const float *filt_host, const float *bias_host);
+// The plan as family T, or PCNN_ERR_ARG with "fn: the plan was not made by T::made_by" for a plan of any other family
+template <class T>
+int plan_as(const char *fn, pcnn_conv_plan *plan, T **out) {
+    *out = dynamic_cast<T *>(plan);
+    PCNN_REQUIRE(*out, PCNN_ERR_ARG, "%s: the plan was not made by %s", fn, T::made_by);
+    return PCNN_OK;
+}
 // the window rules the depthwise and the grouped convolutions share (dwconv_nhwc.cu): N, H, W, C >= 1, 1 <= R, S <= 7, stride 1..4,
 // 0 <= pad <= taps - 1 and a window that fits; refused with PCNN_ERR_ARG and a message naming `fn`; P and Q on success
 int nhwc_window_check(const char *fn, int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int *P, int *Q);
-// gconv_nhwc.cu: a plan of pcnn_gconv_plan_create holds a GConvPlan, run, refreshed and freed like the depthwise one; its bf16
-// operand is [K][R][S][Cg], the fp32 master's element order (one row of K R S Cg elements); conv_plan_gconv is null for any other plan
-struct GConvPlan;
-int gconv_fwd(pcnn_ctx *ctx, const GConvPlan *g, const void *x_bf16, void *y_bf16);
-void gconv_free(GConvPlan *g);
-void gconv_operand(GConvPlan *g, PlanOperand *out);
-int gconv_load_filters(pcnn_ctx *ctx, GConvPlan *g, const float *filt_dev);
-pcnn_conv_plan *conv_plan_wrap_gconv(GConvPlan *g);   // conv_tc.cu; takes ownership
-GConvPlan *conv_plan_gconv(pcnn_conv_plan *plan);
-// a temporary device copy of host data (the create calls upload their filters through one); freed when it goes out of scope
-struct pcnn_dev_temp {
-    float *p = nullptr;
-    ~pcnn_dev_temp() { if (p) cudaFree(p); }
-};
 // The domain and tiling of the wide forward, which its gradients (conv_wide_bwd_tc.cu) share: one rule, refused with
 // PCNN_ERR_ARG and a message that names `fn`, the caller's entry point.  conv_wide_pixel_block picks the Pt x Qt = 128 block
 // of a P x Q image and returns the blocks per image.

@@ -562,18 +562,21 @@ class ConvPlan:
     ACT_NONE (0), ACT_SIGMOID (1) or ACT_RELU (3), fused after the bias; any other value is refused."""
 
     def __init__(self, engine, N, H, W, C, K, R, S, filt, bias=None, act=0, row_pitch=None, image_rows=0, stride=1):
-        self.engine = engine
         self.shape = (N, H, W, C, K, R, S)
         self.row_pitch = int(row_pitch if row_pitch is not None else (W * C + 7) // 8 * 8)
+        self._create(engine, "pcnn_conv_tc_plan_create_strided", filt, K * R * S * C, bias,
+                     N, H, W, C, K, R, S, int(stride), self.row_pitch, int(image_rows), int(act))
+        self.out_shape = (N, (H - R) // stride + 1, (W - S) // stride + 1, K)
+
+    def _create(self, engine, fn, filt, nf, bias, *args):
+        """self.plan from the create call fn(ctx, *args, filters, bias, &plan): filt (nf elements) and bias (or None) as fp32"""
+        self.engine = engine
         filt = np.ascontiguousarray(filt, np.float32)
-        assert filt.size == K * R * S * C
+        assert filt.size == nf
         b = None if bias is None else np.ascontiguousarray(bias, np.float32)
         plan = C_.c_void_p()
-        check("pcnn_conv_tc_plan_create_strided",
-              lib().pcnn_conv_tc_plan_create_strided(engine.ctx, N, H, W, C, K, R, S, int(stride), self.row_pitch, int(image_rows), int(act),
-                                                     filt.ctypes.data, None if b is None else b.ctypes.data, C_.byref(plan)))
+        check(fn, getattr(lib(), fn)(engine.ctx, *args, filt.ctypes.data, None if b is None else b.ctypes.data, C_.byref(plan)))
         self.plan = plan
-        self.out_shape = (N, (H - R) // stride + 1, (W - S) // stride + 1, K)
 
     def fwd(self, x_bf16_dev, y_bf16_dev):
         check("pcnn_conv_tc_fwd", lib().pcnn_conv_tc_fwd(self.engine.ctx, self.plan, _p(x_bf16_dev), _p(y_bf16_dev)))
@@ -601,24 +604,12 @@ class WideConvPlan(ConvPlan):
     Run and closed like ConvPlan."""
 
     def __init__(self, engine, N, H, W, C, K, R, S, filt, bias=None, act=0, row_pitch=None, image_rows=0, stride=1, padding=(0, 0)):
-        self.engine = engine
         self.shape = (N, H, W, C, K, R, S)
         self.row_pitch = int(row_pitch if row_pitch is not None else (W * C + 7) // 8 * 8)
-        filt = np.ascontiguousarray(filt, np.float32)
-        assert filt.size == K * R * S * C
-        b = None if bias is None else np.ascontiguousarray(bias, np.float32)
-        plan = C_.c_void_p()
         ph, pw = (int(v) for v in padding)
-        if (ph, pw) == (0, 0):
-            check("pcnn_conv_wide_plan_create",
-                  lib().pcnn_conv_wide_plan_create(engine.ctx, N, H, W, C, K, R, S, int(stride), self.row_pitch, int(image_rows), int(act),
-                                                   filt.ctypes.data, None if b is None else b.ctypes.data, C_.byref(plan)))
-        else:
-            check("pcnn_conv_wide_plan_create_padded",
-                  lib().pcnn_conv_wide_plan_create_padded(engine.ctx, N, H, W, C, K, R, S, int(stride), ph, pw, self.row_pitch,
-                                                          int(image_rows), int(act), filt.ctypes.data,
-                                                          None if b is None else b.ctypes.data, C_.byref(plan)))
-        self.plan = plan
+        pad = () if (ph, pw) == (0, 0) else (ph, pw)
+        self._create(engine, "pcnn_conv_wide_plan_create" + ("_padded" if pad else ""), filt, K * R * S * C, bias,
+                     N, H, W, C, K, R, S, int(stride), *pad, self.row_pitch, int(image_rows), int(act))
         self.out_shape = (N, (H + 2 * ph - R) // stride + 1, (W + 2 * pw - S) // stride + 1, K)
 
 
@@ -628,17 +619,9 @@ class LinearPlan(ConvPlan):
     refreshed and closed like ConvPlan; its gradients are Engine.linear_wgrad / linear_dgrad."""
 
     def __init__(self, engine, N, P, Q, C, O, w, bias=None, act=0, row_pitch=None, image_rows=0):
-        self.engine = engine
         self.shape = (N, P, Q, C, O)
         self.row_pitch = int(row_pitch or (Q * C + 7) // 8 * 8)
-        w = np.ascontiguousarray(w, np.float32)
-        assert w.size == O * P * Q * C
-        b = None if bias is None else np.ascontiguousarray(bias, np.float32)
-        plan = C_.c_void_p()
-        check("pcnn_linear_plan_create",
-              lib().pcnn_linear_plan_create(engine.ctx, N, P, Q, C, O, self.row_pitch, int(image_rows), int(act), w.ctypes.data,
-                                            None if b is None else b.ctypes.data, C_.byref(plan)))
-        self.plan = plan
+        self._create(engine, "pcnn_linear_plan_create", w, O * P * Q * C, bias, N, P, Q, C, O, self.row_pitch, int(image_rows), int(act))
         self.out_shape = (N, O)
 
 
@@ -648,17 +631,9 @@ class DepthwiseConvPlan(ConvPlan):
     ACT_NONE (0) or ACT_RELU (3).  Run, refreshed and closed like ConvPlan; its gradients are Engine.dwconv_wgrad / dwconv_dgrad."""
 
     def __init__(self, engine, N, H, W, C, R, S, filt, bias=None, act=0, stride=1, padding=(0, 0)):
-        self.engine = engine
         self.shape = (N, H, W, C, R, S)
         ph, pw = (int(v) for v in padding)
-        filt = np.ascontiguousarray(filt, np.float32)
-        assert filt.size == C * R * S
-        b = None if bias is None else np.ascontiguousarray(bias, np.float32)
-        plan = C_.c_void_p()
-        check("pcnn_dwconv_plan_create",
-              lib().pcnn_dwconv_plan_create(engine.ctx, N, H, W, C, R, S, int(stride), ph, pw, int(act), filt.ctypes.data,
-                                            None if b is None else b.ctypes.data, C_.byref(plan)))
-        self.plan = plan
+        self._create(engine, "pcnn_dwconv_plan_create", filt, C * R * S, bias, N, H, W, C, R, S, int(stride), ph, pw, int(act))
         self.out_shape = (N, (H + 2 * ph - R) // stride + 1, (W + 2 * pw - S) // stride + 1, C)
 
 
@@ -668,80 +643,49 @@ class GroupedConvPlan(ConvPlan):
     ACT_NONE (0) or ACT_RELU (3).  Run, refreshed and closed like ConvPlan; its gradients are Engine.gconv_wgrad / gconv_dgrad."""
 
     def __init__(self, engine, N, H, W, C, K, G, R, S, filt, bias=None, act=0, stride=1, padding=(0, 0)):
-        self.engine = engine
         self.shape = (N, H, W, C, K, G, R, S)
         ph, pw = (int(v) for v in padding)
-        filt = np.ascontiguousarray(filt, np.float32)
-        assert G >= 1 and filt.size == K * R * S * (C // G)
-        b = None if bias is None else np.ascontiguousarray(bias, np.float32)
-        plan = C_.c_void_p()
-        check("pcnn_gconv_plan_create",
-              lib().pcnn_gconv_plan_create(engine.ctx, N, H, W, C, K, G, R, S, int(stride), ph, pw, int(act), filt.ctypes.data,
-                                           None if b is None else b.ctypes.data, C_.byref(plan)))
-        self.plan = plan
+        assert G >= 1
+        self._create(engine, "pcnn_gconv_plan_create", filt, K * R * S * (C // G), bias, N, H, W, C, K, G, R, S, int(stride), ph, pw,
+                     int(act))
         self.out_shape = (N, (H + 2 * ph - R) // stride + 1, (W + 2 * pw - S) // stride + 1, K)
 
 
-class ConvLayer:
-    """One bf16 convolution layer trained on the device: forward, backward and an SGD step with no host round trip.
+class _PlanLayer:
+    """What the plan-backed layers share: fp32 master filters and bias, their gradients dw and db, all in DeviceArrays, and a plan
+    holding the filters in bf16.  A subclass builds its plan, calls _own(engine, plan, filt, bias) with the host masters in the
+    plan's element order, and supplies _grads(dy, dx): the weight gradient into dw and, when dx is given, the input gradient."""
 
-    It owns fp32 master filters (KRSC) and bias, their gradients dw and db, all in DeviceArrays, and a forward plan of the family
-    that serves the shape (conv_layer_family: the row-Toeplitz plan for few channels without padding, the wide plan otherwise).
-    Activations are NHWC bf16: x with row_pitch (None = W*C rounded up to 8) and image_rows (0 = H), y and dy dense
-    [N][P][Q][K], dx in x's layout.  act ACT_SIGMOID (1) is a sigmoid after the bias, ACT_RELU (3) a ReLU, ACT_NONE (0) none."""
-
-    def __init__(self, engine, N, H, W, C, K, R, S, filt, bias=None, act=0, stride=1, padding=(0, 0), row_pitch=None, image_rows=0):
-        self.engine = engine
-        self.shape = (N, H, W, C, K, R, S)
-        self.act, self.stride = int(act), int(stride)
-        self.padding = tuple(int(v) for v in padding)
-        self.row_pitch = int(row_pitch if row_pitch is not None else (W * C + 7) // 8 * 8)
-        self.image_rows = int(image_rows)
-        self.family = conv_layer_family(N, H, W, C, K, R, S, self.stride, self.padding, self.row_pitch, self.image_rows)
-        filt = np.ascontiguousarray(filt, np.float32).reshape(K, R, S, C)
-        bias = None if bias is None else np.ascontiguousarray(bias, np.float32).reshape(K)
-        if self.family == "narrow":
-            self.plan = ConvPlan(engine, N, H, W, C, K, R, S, filt, bias, act=act, row_pitch=self.row_pitch, image_rows=self.image_rows,
-                                 stride=self.stride)
-        else:
-            self.plan = WideConvPlan(engine, N, H, W, C, K, R, S, filt, bias, act=act, row_pitch=self.row_pitch,
-                                     image_rows=self.image_rows, stride=self.stride, padding=self.padding)
-        self.out_shape = self.plan.out_shape
-        self.pixels = int(np.prod(self.out_shape[:3]))
+    def _own(self, engine, plan, filt, bias):
+        self.engine, self.plan = engine, plan
+        self.out_shape = plan.out_shape
+        self.pixels = int(np.prod(self.out_shape[:-1]))
         self.filt = DeviceArray.from_host(engine, filt)
         self.bias = None if bias is None else DeviceArray.from_host(engine, bias)
-        self.dw = engine.array((K, R, S, C))
-        self.db = None if bias is None else engine.array(K)
+        self.dw = engine.array(filt.shape)
+        self.db = None if bias is None else engine.array(bias.size)
         self._x = None
 
     def forward(self, x, y):
-        """y = act(conv(x) + bias) with the plan's bf16 filters.  The layer keeps x: backward's weight gradient reads it."""
+        """y = act(layer(x) + bias) with the plan's bf16 filters.  The layer keeps x: backward's weight gradient reads it."""
         self.plan.fwd(x, y)
         self._x = x
 
     def backward(self, y, dy, dx=None):
         """Gradients of the most recent forward, whose output y was: dw, db (with a bias) and dx (when given; a first layer
         passes None).  dy is CONSUMED: with a sigmoid or a ReLU it is overwritten in place by the gradient at the pre-activation,
-        which the weight and input gradients then read (pcnn_conv_bias_act_bwd, skipped without activation and bias)."""
-        N, H, W, C, K, R, S = self.shape
-        e = self.engine
+        which the weight and input gradients then read (pcnn_conv_bias_act_bwd over the output's pixels, skipped without
+        activation and bias)."""
         if self.act or self.bias is not None:
-            e.conv_bias_act_bwd(y if self.act else None, dy, dy if self.act else None, self.db, self.pixels, K, self.act)
-        if self.family == "narrow":
-            e.conv_wgrad(self._x, dy, self.dw, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride)
-            if dx is not None:
-                e.conv_dgrad(dy, self.filt, dx, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride)
-        else:
-            e.conv_wide_wgrad(self._x, dy, self.dw, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride, self.padding)
-            if dx is not None:
-                e.conv_wide_dgrad(dy, self.filt, dx, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride, self.padding)
+            self.engine.conv_bias_act_bwd(y if self.act else None, dy, dy if self.act else None, self.db, self.pixels, self.out_shape[-1],
+                                          self.act)
+        self._grads(dy, dx)
 
     def sgd(self, lr):
         """w += (-lr) * dw and b += (-lr) * db in fp32 on the masters, then the plan refreshed from them, all on the engine's stream"""
-        n = int(np.prod(self.shape[4:])) * self.shape[3]
-        self.engine.apply_grad_scaled(self.filt, self.dw, n, -lr)
+        self.engine.apply_grad_scaled(self.filt, self.dw, int(np.prod(self.filt.shape)), -lr)
         if self.bias is not None:
-            self.engine.apply_grad_scaled(self.bias, self.db, self.shape[4], -lr)
+            self.engine.apply_grad_scaled(self.bias, self.db, self.out_shape[-1], -lr)
         self.plan.set_params(self.filt, self.bias)
 
     def optim_tensors(self):
@@ -749,7 +693,7 @@ class ConvLayer:
         return [(self.filt, self.dw, self.plan, 1, False)] + ([] if self.bias is None else [(self.bias, self.db, self.plan, 2, True)])
 
     def params(self):
-        """host copies (filters [K][R][S][C], bias [K] or None) of the fp32 masters"""
+        """host copies (filters in the plan's element order, bias or None) of the fp32 masters"""
         return self.filt.to_host(), None if self.bias is None else self.bias.to_host()
 
     def close(self):
@@ -759,7 +703,45 @@ class ConvLayer:
                 a.free()
 
 
-class DepthwiseConvLayer:
+class ConvLayer(_PlanLayer):
+    """One bf16 convolution layer trained on the device: forward, backward and an SGD step with no host round trip.
+
+    It owns fp32 master filters (KRSC) and bias, their gradients dw and db, all in DeviceArrays, and a forward plan of the family
+    that serves the shape (conv_layer_family: the row-Toeplitz plan for few channels without padding, the wide plan otherwise).
+    Activations are NHWC bf16: x with row_pitch (None = W*C rounded up to 8) and image_rows (0 = H), y and dy dense
+    [N][P][Q][K], dx in x's layout.  act ACT_SIGMOID (1) is a sigmoid after the bias, ACT_RELU (3) a ReLU, ACT_NONE (0) none."""
+
+    def __init__(self, engine, N, H, W, C, K, R, S, filt, bias=None, act=0, stride=1, padding=(0, 0), row_pitch=None, image_rows=0):
+        self.shape = (N, H, W, C, K, R, S)
+        self.act, self.stride = int(act), int(stride)
+        self.padding = tuple(int(v) for v in padding)
+        self.row_pitch = int(row_pitch if row_pitch is not None else (W * C + 7) // 8 * 8)
+        self.image_rows = int(image_rows)
+        self.family = conv_layer_family(N, H, W, C, K, R, S, self.stride, self.padding, self.row_pitch, self.image_rows)
+        filt = np.ascontiguousarray(filt, np.float32).reshape(K, R, S, C)
+        bias = None if bias is None else np.ascontiguousarray(bias, np.float32).reshape(K)
+        if self.family == "narrow":
+            plan = ConvPlan(engine, N, H, W, C, K, R, S, filt, bias, act=act, row_pitch=self.row_pitch, image_rows=self.image_rows,
+                            stride=self.stride)
+        else:
+            plan = WideConvPlan(engine, N, H, W, C, K, R, S, filt, bias, act=act, row_pitch=self.row_pitch, image_rows=self.image_rows,
+                                stride=self.stride, padding=self.padding)
+        self._own(engine, plan, filt, bias)
+
+    def _grads(self, dy, dx):
+        N, H, W, C, K, R, S = self.shape
+        e = self.engine
+        if self.family == "narrow":
+            e.conv_wgrad(self._x, dy, self.dw, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride)
+            if dx is not None:
+                e.conv_dgrad(dy, self.filt, dx, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride)
+        else:
+            e.conv_wide_wgrad(self._x, dy, self.dw, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride, self.padding)
+            if dx is not None:
+                e.conv_wide_dgrad(dy, self.filt, dx, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride, self.padding)
+
+
+class DepthwiseConvLayer(_PlanLayer):
     """A depthwise convolution trained on the device (groups = C: each channel filtered by its own R x S filter), with ConvLayer's
     interface: fp32 masters filt [C][R][S] and bias [C], their gradients dw and db, and a DepthwiseConvPlan holding the filters in
     bf16.  x and dx are dense bf16 [N][H][W][C], y and dy dense [N][P][Q][C]: what a ConvLayer or a BatchNormLayer writes and reads,
@@ -770,66 +752,26 @@ class DepthwiseConvLayer:
 
     act ACT_RELU (3) is a ReLU after the bias, ACT_NONE (0) none; the sigmoid is refused.  With a bias or an activation, backward
     first runs pcnn_conv_bias_act_bwd over dy, which takes at most 256 channels: such a layer needs C <= 256.  Without either
-    (the usual case in front of a batch norm) C is unlimited."""
+    (the usual case in front of a batch norm) C is unlimited.  dx uses the plan's bf16 filters, so call backward before sgd or an
+    optimizer step."""
 
     def __init__(self, engine, N, H, W, C, R, S, filt, bias=None, act=0, stride=1, padding=(0, 0)):
-        self.engine = engine
         self.shape = (N, H, W, C, R, S)
         self.act, self.stride = int(act), int(stride)
         self.padding = tuple(int(v) for v in padding)
         self.info = dwconv_info(N, H, W, C, R, S, self.stride, self.padding)
         filt = np.ascontiguousarray(filt, np.float32).reshape(C, R, S)
         bias = None if bias is None else np.ascontiguousarray(bias, np.float32).reshape(C)
-        self.plan = DepthwiseConvPlan(engine, N, H, W, C, R, S, filt, bias, act=act, stride=self.stride, padding=self.padding)
-        self.out_shape = self.plan.out_shape
-        self.pixels = int(np.prod(self.out_shape[:3]))
-        self.filt = DeviceArray.from_host(engine, filt)
-        self.bias = None if bias is None else DeviceArray.from_host(engine, bias)
-        self.dw = engine.array((C, R, S))
-        self.db = None if bias is None else engine.array(C)
-        self._x = None
+        plan = DepthwiseConvPlan(engine, N, H, W, C, R, S, filt, bias, act=act, stride=self.stride, padding=self.padding)
+        self._own(engine, plan, filt, bias)
 
-    def forward(self, x, y):
-        """y = act(dwconv(x) + bias) with the plan's bf16 filters.  The layer keeps x: backward's weight gradient reads it."""
-        self.plan.fwd(x, y)
-        self._x = x
-
-    def backward(self, y, dy, dx=None):
-        """Gradients of the most recent forward, whose output y was: dw, db (with a bias) and dx (when given).  dy is CONSUMED with
-        a ReLU: it is overwritten in place by the gradient at the pre-activation (pcnn_conv_bias_act_bwd, skipped without
-        activation and bias).  dx uses the plan's bf16 filters, so call it before sgd or an optimizer step."""
-        C = self.shape[3]
-        e = self.engine
-        if self.act or self.bias is not None:
-            e.conv_bias_act_bwd(y if self.act else None, dy, dy if self.act else None, self.db, self.pixels, C, self.act)
-        e.dwconv_wgrad(self.plan, self._x, dy, self.dw)
+    def _grads(self, dy, dx):
+        self.engine.dwconv_wgrad(self.plan, self._x, dy, self.dw)
         if dx is not None:
-            e.dwconv_dgrad(self.plan, dy, dx)
-
-    def sgd(self, lr):
-        """w += (-lr) * dw and b += (-lr) * db in fp32 on the masters, then the plan refreshed from them, all on the engine's stream"""
-        N, H, W, C, R, S = self.shape
-        self.engine.apply_grad_scaled(self.filt, self.dw, C * R * S, -lr)
-        if self.bias is not None:
-            self.engine.apply_grad_scaled(self.bias, self.db, C, -lr)
-        self.plan.set_params(self.filt, self.bias)
-
-    def optim_tensors(self):
-        """(param, grad, plan, plan part, is norm or bias) of the filters and the bias, as ConvLayer.optim_tensors"""
-        return [(self.filt, self.dw, self.plan, 1, False)] + ([] if self.bias is None else [(self.bias, self.db, self.plan, 2, True)])
-
-    def params(self):
-        """host copies (filters [C][R][S], bias [C] or None) of the fp32 masters"""
-        return self.filt.to_host(), None if self.bias is None else self.bias.to_host()
-
-    def close(self):
-        self.plan.close()
-        for a in (self.filt, self.bias, self.dw, self.db):
-            if a is not None:
-                a.free()
+            self.engine.dwconv_dgrad(self.plan, dy, dx)
 
 
-class GroupedConvLayer:
+class GroupedConvLayer(_PlanLayer):
     """A grouped convolution trained on the device (groups = G: each group of C / G input channels feeds its own K / G filters), with
     ConvLayer's interface: fp32 masters filt [K][R][S][Cg] and bias [K], their gradients dw and db, and a GroupedConvPlan holding the
     filters in bf16.  x and dx are dense bf16 [N][H][W][C], y and dy dense [N][P][Q][K]: what a ConvLayer or a BatchNormLayer writes
@@ -840,13 +782,13 @@ class GroupedConvLayer:
 
     act ACT_RELU (3) is a ReLU after the bias, ACT_NONE (0) none; the sigmoid is refused.  With a bias or an activation, backward
     first runs pcnn_conv_bias_act_bwd over dy, which takes at most 256 channels: such a layer needs K <= 256 and is refused
-    otherwise.  Without either (the usual case in front of a batch norm) C and K are unlimited."""
+    otherwise.  Without either (the usual case in front of a batch norm) C and K are unlimited.  dx uses the plan's bf16 filters, so
+    call backward before sgd or an optimizer step."""
 
     def __init__(self, engine, N, H, W, C, K, G, R, S, filt, bias=None, act=0, stride=1, padding=(0, 0)):
         if (int(act) or bias is not None) and K > 256:
             raise PcnnError("GroupedConvLayer", -1, f"K = {K} with a bias or an activation: the bias / activation backward "
                             "(pcnn_conv_bias_act_bwd) takes K <= 256; put a BatchNormLayer after a layer with no bias and act 0")
-        self.engine = engine
         self.shape = (N, H, W, C, K, G, R, S)
         self.act, self.stride = int(act), int(stride)
         self.padding = tuple(int(v) for v in padding)
@@ -854,53 +796,13 @@ class GroupedConvLayer:
         Cg = self.info["Cg"]
         filt = np.ascontiguousarray(filt, np.float32).reshape(K, R, S, Cg)
         bias = None if bias is None else np.ascontiguousarray(bias, np.float32).reshape(K)
-        self.plan = GroupedConvPlan(engine, N, H, W, C, K, G, R, S, filt, bias, act=act, stride=self.stride, padding=self.padding)
-        self.out_shape = self.plan.out_shape
-        self.pixels = int(np.prod(self.out_shape[:3]))
-        self.filt = DeviceArray.from_host(engine, filt)
-        self.bias = None if bias is None else DeviceArray.from_host(engine, bias)
-        self.dw = engine.array((K, R, S, Cg))
-        self.db = None if bias is None else engine.array(K)
-        self._x = None
+        plan = GroupedConvPlan(engine, N, H, W, C, K, G, R, S, filt, bias, act=act, stride=self.stride, padding=self.padding)
+        self._own(engine, plan, filt, bias)
 
-    def forward(self, x, y):
-        """y = act(gconv(x) + bias) with the plan's bf16 filters.  The layer keeps x: backward's weight gradient reads it."""
-        self.plan.fwd(x, y)
-        self._x = x
-
-    def backward(self, y, dy, dx=None):
-        """Gradients of the most recent forward, whose output y was: dw, db (with a bias) and dx (when given).  dy is CONSUMED with
-        a ReLU: it is overwritten in place by the gradient at the pre-activation (pcnn_conv_bias_act_bwd, skipped without
-        activation and bias).  dx uses the plan's bf16 filters, so call it before sgd or an optimizer step."""
-        K = self.shape[4]
-        e = self.engine
-        if self.act or self.bias is not None:
-            e.conv_bias_act_bwd(y if self.act else None, dy, dy if self.act else None, self.db, self.pixels, K, self.act)
-        e.gconv_wgrad(self.plan, self._x, dy, self.dw)
+    def _grads(self, dy, dx):
+        self.engine.gconv_wgrad(self.plan, self._x, dy, self.dw)
         if dx is not None:
-            e.gconv_dgrad(self.plan, dy, dx)
-
-    def sgd(self, lr):
-        """w += (-lr) * dw and b += (-lr) * db in fp32 on the masters, then the plan refreshed from them, all on the engine's stream"""
-        K, R, S = self.shape[4], self.shape[6], self.shape[7]
-        self.engine.apply_grad_scaled(self.filt, self.dw, K * R * S * self.info["Cg"], -lr)
-        if self.bias is not None:
-            self.engine.apply_grad_scaled(self.bias, self.db, K, -lr)
-        self.plan.set_params(self.filt, self.bias)
-
-    def optim_tensors(self):
-        """(param, grad, plan, plan part, is norm or bias) of the filters and the bias, as ConvLayer.optim_tensors"""
-        return [(self.filt, self.dw, self.plan, 1, False)] + ([] if self.bias is None else [(self.bias, self.db, self.plan, 2, True)])
-
-    def params(self):
-        """host copies (filters [K][R][S][Cg], bias [K] or None) of the fp32 masters"""
-        return self.filt.to_host(), None if self.bias is None else self.bias.to_host()
-
-    def close(self):
-        self.plan.close()
-        for a in (self.filt, self.bias, self.dw, self.db):
-            if a is not None:
-                a.free()
+            self.engine.gconv_dgrad(self.plan, dy, dx)
 
 
 class BatchNormLayer:
@@ -980,7 +882,7 @@ class BatchNormLayer:
             a.free()
 
 
-class LinearLayer:
+class LinearLayer(_PlanLayer):
     """A fully connected layer trained on the device, with ConvLayer's interface: fp32 masters w [O][P][Q][C] and bias [O], their
     gradients dw and db, and a LinearPlan holding w in bf16.
 
@@ -995,10 +897,11 @@ class LinearLayer:
         engine.softmax_ce_bf16(z, labels, N, 10, 1 / N, dz, loss, pred)
         fc2.backward(z, dz, dy3);  fc1.backward(y3, dy3, dx3);  pool2.backward(dx3, dy2)
         conv2.backward(y2, dy2, dx2);  pool1.backward(dx2, dy1);  conv1.backward(y1, dy1, None)
-        for layer in (conv1, conv2, fc1, fc2): layer.sgd(lr)"""
+        for layer in (conv1, conv2, fc1, fc2): layer.sgd(lr)
+
+    dx uses the plan's bf16 weights, so call backward before sgd."""
 
     def __init__(self, engine, N, P, Q, C, O, w, bias=None, act=0, row_pitch=None, image_rows=0):
-        self.engine = engine
         self.shape = (N, P, Q, C, O)
         self.act = int(act)
         self.row_pitch = int(row_pitch or (Q * C + 7) // 8 * 8)
@@ -1006,52 +909,18 @@ class LinearLayer:
         self.info = linear_info(N, P, Q, C, O, self.row_pitch, self.image_rows)
         w = np.ascontiguousarray(w, np.float32).reshape(O, P, Q, C)
         bias = None if bias is None else np.ascontiguousarray(bias, np.float32).reshape(O)
-        self.plan = LinearPlan(engine, N, P, Q, C, O, w, bias, act=act, row_pitch=self.row_pitch, image_rows=self.image_rows)
-        self.out_shape = (N, O)
-        self.w = DeviceArray.from_host(engine, w)
-        self.bias = None if bias is None else DeviceArray.from_host(engine, bias)
-        self.dw = engine.array((O, P, Q, C))
-        self.db = None if bias is None else engine.array(O)
-        self._x = None
+        plan = LinearPlan(engine, N, P, Q, C, O, w, bias, act=act, row_pitch=self.row_pitch, image_rows=self.image_rows)
+        self._own(engine, plan, w, bias)
 
-    def forward(self, x, y):
-        """y = act(x W^T + bias) with the plan's bf16 weights.  The layer keeps x: backward's weight gradient reads it."""
-        self.plan.fwd(x, y)
-        self._x = x
+    @property
+    def w(self):
+        """the fp32 master weights [O][P][Q][C]"""
+        return self.filt
 
-    def backward(self, y, dy, dx=None):
-        """Gradients of the most recent forward, whose output y was: dw, db (with a bias) and dx (when given).  dy is CONSUMED:
-        with a sigmoid or a ReLU it is overwritten in place by the gradient at the pre-activation (pcnn_conv_bias_act_bwd with
-        pixels = N, K = O; skipped without activation and bias).  dx uses the plan's bf16 weights, so call it before sgd."""
-        N, P, Q, C, O = self.shape
-        e = self.engine
-        if self.act or self.bias is not None:
-            e.conv_bias_act_bwd(y if self.act else None, dy, dy if self.act else None, self.db, N, O, self.act)
-        e.linear_wgrad(self.plan, self._x, dy, self.dw)
+    def _grads(self, dy, dx):
+        self.engine.linear_wgrad(self.plan, self._x, dy, self.dw)
         if dx is not None:
-            e.linear_dgrad(self.plan, dy, dx)
-
-    def sgd(self, lr):
-        """w += (-lr) * dw and b += (-lr) * db in fp32 on the masters, then the plan refreshed from them, all on the engine's stream"""
-        N, P, Q, C, O = self.shape
-        self.engine.apply_grad_scaled(self.w, self.dw, O * P * Q * C, -lr)
-        if self.bias is not None:
-            self.engine.apply_grad_scaled(self.bias, self.db, O, -lr)
-        self.plan.set_params(self.w, self.bias)
-
-    def optim_tensors(self):
-        """(param, grad, plan, plan part, is norm or bias) of w and the bias, as ConvLayer.optim_tensors"""
-        return [(self.w, self.dw, self.plan, 1, False)] + ([] if self.bias is None else [(self.bias, self.db, self.plan, 2, True)])
-
-    def params(self):
-        """host copies (w [O][P][Q][C], bias [O] or None) of the fp32 masters"""
-        return self.w.to_host(), None if self.bias is None else self.bias.to_host()
-
-    def close(self):
-        self.plan.close()
-        for a in (self.w, self.bias, self.dw, self.db):
-            if a is not None:
-                a.free()
+            self.engine.linear_dgrad(self.plan, dy, dx)
 
 
 class MaxPoolLayer:

@@ -258,7 +258,8 @@ def test_refusals(eng, pkg):
     lin = pkg.LinearPlan(eng, 2, 1, 1, 8, 8, np.ones((8, 8), np.float32))
     conv = pkg.WideConvPlan(eng, 2, 8, 8, 64, 64, 3, 3, np.ones((64, 3, 3, 64), np.float32))
     dwp = pkg.DepthwiseConvPlan(eng, 2, 8, 8, 8, 3, 3, np.ones((8, 3, 3), np.float32), padding=(1, 1))
-    for other in (lin, conv, dwp):
+    narrow = pkg.ConvPlan(eng, 2, 8, 8, 1, 8, 3, 3, np.ones((8, 3, 3, 1), np.float32))
+    for other in (lin, conv, dwp, narrow):
         refused(eng.gconv_wgrad, "was not made by pcnn_gconv_plan_create", other, x, y, dw)
         refused(eng.gconv_dgrad, "was not made by pcnn_gconv_plan_create", other, x, y)
     refused(eng.linear_dgrad, "was not made by pcnn_linear_plan_create", plan, x, y)
@@ -267,7 +268,7 @@ def test_refusals(eng, pkg):
     refused(eng.dwconv_wgrad, "was not made by pcnn_dwconv_plan_create", plan, x, y, dw)
     # a bias for a plan created without one
     refused(plan.set_params, "created without one", None, eng.array(16))
-    for p in (plan, lin, conv, dwp):
+    for p in (plan, lin, conv, dwp, narrow):
         p.close()
 
 
