@@ -673,17 +673,17 @@ def run_gap(name, N, H, W, C, iters):
 
 
 def run_resnetgap(N, iters):
-    """one training step of the GAP ResNet of tests/test_avgpool_nhwc_gpu.py (test_resnet_gap_mnist) at batch N: forward, softmax
+    """one training step of the GAP ResNet of tests/example_nets.py (test_resnet_gap_mnist) at batch N: forward, softmax
     cross-entropy, backward and the sgd of every layer on the engine's stream; next to it the torch eager step of the same layers on
     bf16 channels-last tensors (fp32 masters, w -= lr * grad, re-cast to bf16)."""
     sys.path.insert(0, os.path.join(ROOT, "tests"))
-    import test_avgpool_nhwc_gpu as T
-    assert N == T.NB
-    p = T.init_params()
-    net = T.ResNetGAP(eng, pkg, p)
+    from example_nets import ResNetGAP
+    assert N == ResNetGAP.NB
+    p = ResNetGAP.init_params()
+    net = ResNetGAP(eng, pkg, p)
     xl = torch.randint(0, 0x3F80, (N * 28, 32), dtype=torch.int16, device="cuda")
     labels = torch.randint(0, 10, (N,), dtype=torch.uint8, device="cuda")
-    lr = T.LR_STEP
+    lr = ResNetGAP.LR_STEP
     gpu, power = card()
 
     def step():
@@ -790,9 +790,9 @@ def run_resnetgap_optim(N, iters, rounds=3):
     """the GAP ResNet training step of run_resnetgap with every layer's sgd(lr) and with the fused SGD at momentum 0 (the same bits),
     alternated in this one call; then momentum SGD and AdamW.  The update alone (gradients left in place) is timed the same way."""
     sys.path.insert(0, os.path.join(ROOT, "tests"))
-    import test_avgpool_nhwc_gpu as T
+    from example_nets import ResNetGAP
     gpu, power = card()
-    net = T.ResNetGAP(eng, pkg, T.init_params())
+    net = ResNetGAP(eng, pkg, ResNetGAP.init_params())
     xl = torch.randint(0, 0x3F80, (N * 28, 32), dtype=torch.int16, device="cuda")
     labels = torch.randint(0, 10, (N,), dtype=torch.uint8, device="cuda")
     torch.cuda.synchronize()
@@ -1248,12 +1248,11 @@ def run_dropout(name, N, H, W, C, iters, per_sample, p=0.2, rounds=3):
 def run_augment(name, N, H, W, C, C_out, pad, iters, batches=4, row_pitch=0, image_rows=0, rounds=3):
     """one batch of the input pipeline (pcnn_augment_u8_bf16): shuffle over a dataset of `batches` batches, crop with pad, flip,
     normalise, into x with C_out channels; the calls walk the epoch's batches.  Beside it the torch eager pipeline of
-    tests/test_augment_gpu.py (torch_batch: gather, pad, crop and flip by advanced indexing, normalise, cast) on the same indices,
+    tests/augment_ref.py (torch_batch: gather, pad, crop and flip by advanced indexing, normalise, cast) on the same indices,
     offsets and flips, plus the label gather, alternated over `rounds` rounds (the best of each kept).  Bytes: N H W C read,
     N H W C_out 2 written, 2 N for the labels."""
     sys.path.insert(0, os.path.join(ROOT, "tests"))
     import augment_ref as A
-    from test_augment_gpu import torch_batch
     n = N * batches
     images = torch.randint(0, 256, (n, H, W, C), dtype=torch.uint8, device="cuda")
     labels = torch.randint(0, 10, (n,), dtype=torch.uint8, device="cuda")
@@ -1278,7 +1277,7 @@ def run_augment(name, N, H, W, C, C_out, pad, iters, batches=4, row_pitch=0, ima
 
     def theirs():
         i, oy, ox, fl = draws[next(tsteps) % batches]
-        return torch_batch(images, i, oy, ox, fl, pad, mean, std, C_out), labels[i]
+        return A.torch_batch(images, i, oy, ox, fl, pad, mean, std, C_out), labels[i]
 
     gpu, power = card()
     best = None
@@ -1294,27 +1293,26 @@ def run_augment(name, N, H, W, C, C_out, pad, iters, batches=4, row_pitch=0, ima
 
 
 def run_resnetgap_augment(iters, rounds=3):
-    """one training step of the GAP ResNet of tests/test_avgpool_nhwc_gpu.py at N = 128 on the 1024 golden digits, its batch built
+    """one training step of the GAP ResNet of tests/example_nets.py at N = 128 on the 1024 golden digits, its batch built
     by pkg.ImageBatcher (shuffle, random crop of pad 2) against the same step on a slice of the pre-converted mnist_device rows,
     alternated over `rounds` rounds (the best of each kept)"""
     sys.path.insert(0, os.path.join(ROOT, "tests"))
-    import test_avgpool_nhwc_gpu as T
+    from example_nets import ResNetGAP, Slices
     g = np.load(os.path.join(ROOT, "tests", "golden", "mnist_subset.npz"))
-    xs, ys = T.mnist_device(pkg, g["train_u8"]), torch.from_numpy(g["train_labels"]).cuda()
-    net = T.ResNetGAP(eng, pkg, T.init_params())
-    batcher = pkg.ImageBatcher(eng, g["train_u8"].reshape(-1, 28, 28), g["train_labels"], T.NB, pad=2, shuffle=True, seed=5,
+    slices = Slices(pkg, g["train_u8"], g["train_labels"], ResNetGAP.NB)
+    net = ResNetGAP(eng, pkg, ResNetGAP.init_params())
+    batcher = pkg.ImageBatcher(eng, g["train_u8"].reshape(-1, 28, 28), g["train_labels"], ResNetGAP.NB, pad=2, shuffle=True, seed=5,
                                row_pitch=32, image_rows=28)
-    row_bytes = 28 * 32 * 2
     k = iter(range(1 << 40))
 
     def step(batch):
         s = next(k) % batcher.steps_per_epoch
         net.forward(*batch(s))
         net.backward()
-        net.sgd(T.LR_STEP)
+        net.sgd(ResNetGAP.LR_STEP)
 
     aug = lambda: step(batcher.batch)
-    plain = lambda: step(lambda s: (xs.data_ptr() + s * T.NB * row_bytes, ys[s * T.NB:(s + 1) * T.NB]))
+    plain = lambda: step(slices.batch)
     batch_only = lambda: batcher.batch(next(k) % batcher.steps_per_epoch)
     gpu, power = card()
     best = None
@@ -1322,7 +1320,7 @@ def run_resnetgap_augment(iters, rounds=3):
         r = (timed(aug, iters), timed(plain, iters), timed(batch_only, iters))
         best = r if best is None else tuple(min(a, b) for a, b in zip(r, best))
     ms_aug, ms_plain, ms_batch = best
-    print(json.dumps({"case": f"GAP ResNet training step N={T.NB}, batch from ImageBatcher (shuffle, pad 2) vs pre-converted slice",
+    print(json.dumps({"case": f"GAP ResNet training step N={ResNetGAP.NB}, batch from ImageBatcher (shuffle, pad 2) vs pre-converted slice",
                       "ms_batcher": ms_aug, "ms_slice": ms_plain, "batcher_over_slice": ms_aug / ms_plain, "batch_us": ms_batch * 1e3,
                       "gpu": gpu, "power_limit": power}), flush=True)
     batcher.close()

@@ -1,42 +1,35 @@
 #!/usr/bin/env python
-"""scripts/efficientnet_replica.py -- float32 torch CPU replica of the EfficientNet-style network of tests/test_bnact_gpu.py
-(test_efficientnet_mnist): a SiLU stem, an MBConv with ReLU6, an MBConv with SiLU and squeeze-and-excitation carrying the residual,
+"""scripts/efficientnet_replica.py -- float32 torch CPU replica of EfficientNetLite in tests/example_nets.py (test_bnact_gpu's
+test_efficientnet_mnist): a SiLU stem, an MBConv with ReLU6, an MBConv with SiLU and squeeze-and-excitation carrying the residual,
 and a hard-swish head; the same initialisation, batch order (8 batches of 128 over the 1024 golden training digits per epoch),
 softmax cross-entropy over the batch and plain SGD, evaluated on the 256 golden test digits with the running statistics.  Its
 accuracy sets the threshold of the end-to-end test.
 
 Usage: efficientnet_replica.py [lr ...]"""
 import argparse
-import os
-import sys
 
-import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-from test_bnact_gpu import EPOCHS, LR_STEP, NB, init_params  # noqa: E402
+import replica as R  # puts tests/ on the path
+from example_nets import EfficientNetLite
 
 F = torch.nn.functional
 
 
-def run(lr):
-    torch.manual_seed(0)
-    g = np.load(os.path.join(ROOT, "tests", "golden", "mnist_subset.npz"))
-    img = lambda u8: torch.from_numpy(u8.reshape(-1, 1, 28, 28).astype(np.float32) / 255.0).bfloat16().float()   # the device's bf16 input
-    xs, ys, xt, yt = img(g["train_u8"]), torch.from_numpy(g["train_labels"]).long(), img(g["test_u8"]), torch.from_numpy(g["test_labels"]).long()
-    p = init_params()
+def masters(p):
+    """the network's masters in torch's layouts, as leaves that take gradients"""
     conv = lambda k: torch.from_numpy(p[k]).permute(0, 3, 1, 2).contiguous().requires_grad_(True)         # KRSC -> KCRS
     dw = lambda k: torch.from_numpy(p[k]).unsqueeze(1).contiguous().requires_grad_(True)                   # [C][R][S] -> [C][1][R][S]
     w = {k: conv(k) for k in ("f0", "e1", "p1", "e2", "p2", "h")}
     w.update(d1=dw("d1"), d2=dw("d2"))
     w.update({k: torch.from_numpy(p[k].reshape(10, -1) if k == "w8" else p[k]).requires_grad_(True) for k in ("w8", "b8", "s1", "sb1", "s2", "sb2")})
-    bn = [(torch.ones(c, requires_grad=True), torch.zeros(c, requires_grad=True), torch.zeros(c), torch.ones(c))
-          for c in (48, 96, 96, 48, 96, 96, 48, 128)]
+    return w
 
-    def b(i, v, training):
-        ga, be, rm, rv = bn[i]
-        return F.batch_norm(v, rm, rv, ga, be, training=training, momentum=0.1, eps=1e-5)
+
+def run(lr):
+    w = masters(EfficientNetLite.init_params())
+    bn = R.bn_state((48, 96, 96, 48, 96, 96, 48, 128))
+    b = lambda i, v, training: R.batch_norm(bn[i], v, training)
 
     def net(x, training):
         h = F.avg_pool2d(F.silu(b(0, F.conv2d(x, w["f0"]), training)), 2)
@@ -52,24 +45,12 @@ def run(lr):
         return F.linear(F.adaptive_avg_pool2d(h, 1).flatten(1), w["w8"], w["b8"])
 
     params = list(w.values()) + [t for ga, be, _, _ in bn for t in (ga, be)]
-    opt = torch.optim.SGD(params, lr=lr)
-    losses = []
-    for ep in range(EPOCHS):
-        for s in range(1024 // NB):
-            loss = F.cross_entropy(net(xs[s * NB:(s + 1) * NB], True), ys[s * NB:(s + 1) * NB])
-            opt.zero_grad(set_to_none=True)
-            loss.backward()
-            opt.step()
-            losses.append(float(loss.detach()))
-    with torch.no_grad():
-        acc = float((net(xt, False).argmax(1) == yt).float().mean())
-    print(f"sgd lr {lr}: mean loss epoch 1 {np.mean(losses[:8]):.4f} -> epoch {EPOCHS} {np.mean(losses[-8:]):.4f}; test accuracy {acc:.4f}",
-          flush=True)
+    R.run(net, params, lr, EfficientNetLite.EPOCHS, EfficientNetLite.NB)
 
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("lr", nargs="*", type=float)
     a = ap.parse_args()
-    for lr in a.lr or [LR_STEP]:
+    for lr in a.lr or [EfficientNetLite.LR_STEP]:
         run(lr)

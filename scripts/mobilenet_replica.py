@@ -1,38 +1,26 @@
 #!/usr/bin/env python
-"""scripts/mobilenet_replica.py -- float32 torch CPU replica of the MobileNet-style network of tests/test_dwconv_gpu.py
-(test_mobilenet_mnist): the same layers, initialisation, batch order (8 batches of 128 over the 1024 golden training digits per
+"""scripts/mobilenet_replica.py -- float32 torch CPU replica of MobileNetLite in tests/example_nets.py (test_dwconv_gpu's
+test_mobilenet_mnist): the same layers, initialisation, batch order (8 batches of 128 over the 1024 golden training digits per
 epoch), softmax cross-entropy over the batch and plain SGD, evaluated on the 256 golden test digits with the running statistics.
 Its accuracy sets the test's threshold.
 
 Usage: mobilenet_replica.py [lr ...]"""
-import os
 import sys
 
-import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, ROOT)
-from test_dwconv_gpu import EPOCHS, NB, init_params  # noqa: E402
+import replica as R  # puts tests/ on the path
+from example_nets import MobileNetLite
 
 F = torch.nn.functional
 
 
 def run(lr):
-    torch.manual_seed(0)
-    g = np.load(os.path.join(ROOT, "tests", "golden", "mnist_subset.npz"))
-    img = lambda u8: torch.from_numpy(u8.reshape(-1, 1, 28, 28).astype(np.float32) / 255.0).bfloat16().float()   # the device's bf16 input
-    xs, ys, xt, yt = img(g["train_u8"]), torch.from_numpy(g["train_labels"]).long(), img(g["test_u8"]), torch.from_numpy(g["test_labels"]).long()
-    p = {k: torch.from_numpy(v) for k, v in init_params().items()}
+    p = {k: torch.from_numpy(v) for k, v in MobileNetLite.init_params().items()}
     w = {k: (p[k][:, None] if k.startswith("d") else p[k].reshape(10, -1) if k == "w8" else p[k] if k == "b8" else
              p[k].permute(0, 3, 1, 2)).contiguous().requires_grad_(True) for k in p}
-    bn = [(torch.ones(c, requires_grad=True), torch.zeros(c, requires_grad=True), torch.zeros(c), torch.ones(c))
-          for c in (48, 96, 96, 48, 96, 96, 64)]
-
-    def b(i, v, training):
-        ga, be, rm, rv = bn[i]
-        return F.batch_norm(v, rm, rv, ga, be, training=training, momentum=0.1, eps=1e-5)
+    bn = R.bn_state((48, 96, 96, 48, 96, 96, 64))
+    b = lambda i, v, training: R.batch_norm(bn[i], v, training)
 
     def net(x, training):
         x0 = F.relu(b(0, F.conv2d(x, w["f0"]), training))
@@ -45,19 +33,7 @@ def run(lr):
         return F.linear(F.adaptive_avg_pool2d(h, 1).flatten(1), w["w8"], w["b8"])
 
     params = list(w.values()) + [t for ga, be, _, _ in bn for t in (ga, be)]
-    opt = torch.optim.SGD(params, lr=lr)
-    losses = []
-    for ep in range(EPOCHS):
-        for s in range(1024 // NB):
-            loss = F.cross_entropy(net(xs[s * NB:(s + 1) * NB], True), ys[s * NB:(s + 1) * NB])
-            opt.zero_grad(set_to_none=True)
-            loss.backward()
-            opt.step()
-            losses.append(loss.item())
-    with torch.no_grad():
-        acc = float((net(xt, False).argmax(1) == yt).float().mean())
-    print(f"lr {lr}: mean loss epoch 1 {np.mean(losses[:8]):.4f} -> epoch {EPOCHS} {np.mean(losses[-8:]):.4f}; test accuracy {acc:.4f}",
-          flush=True)
+    R.run(net, params, lr, MobileNetLite.EPOCHS, MobileNetLite.NB, head="")
 
 
 if __name__ == "__main__":

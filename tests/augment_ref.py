@@ -3,6 +3,7 @@ walk, the crop and flip draws of each image, the ToTensor + Normalize table, and
 
 Philox4x32-10 is dropout_ref's; the counters carry the domain bits of pcnn.h in word 1."""
 import numpy as np
+import torch
 
 from dropout_ref import LO, S32, philox4x32_10
 from se_ref import bf16
@@ -112,3 +113,23 @@ def batch(images, first, N, shuffle=1, pad=0, flip=0, seed=0, epoch=0, mean=None
     for c in range(C):
         x[..., c] = lut[c][u[..., c]]
     return x, (None if labels is None else np.asarray(labels)[i]), i, oy, ox, fl
+
+
+def torch_batch(images, i, oy, ox, fl, pad, mean, std, C_out):
+    """torch eager on the GPU: the batch of images [n][H][W][C] uint8 (device) at indices i with crop offsets (oy, ox) and flips fl
+    as NHWC bf16 [N][H][W][C_out].  The divisors are device tensors, so each division is IEEE (a CPU scalar divisor becomes a
+    multiply by its reciprocal)."""
+    n, H, W, C = images.shape
+    N = len(i)
+    t = lambda a, dt=torch.long: (a if torch.is_tensor(a) else torch.as_tensor(np.asarray(a))).to(device=images.device, dtype=dt)
+    crop = torch.nn.functional.pad(images[t(i)].permute(0, 3, 1, 2), (pad, pad, pad, pad))    # [N][C][H + 2 pad][W + 2 pad]
+    w = torch.arange(W, device=images.device)
+    rows = t(oy)[:, None] + torch.arange(H, device=images.device)[None, :]
+    cols = t(ox)[:, None] + torch.where(t(fl, torch.bool)[:, None], W - 1 - w[None, :], w[None, :])
+    u = crop[torch.arange(N, device=images.device)[:, None, None], :, rows[:, :, None], cols[:, None, :]]     # [N][H][W][C]
+    m = t(np.zeros(C) if mean is None else mean, torch.float32)
+    s = t(np.ones(C) if std is None else std, torch.float32)
+    v = u.float().div(torch.full((C,), 255.0, device=images.device)).sub(m).div(s).to(torch.bfloat16)
+    out = torch.zeros((N, H, W, C_out), dtype=torch.bfloat16, device=images.device)
+    out[..., :C] = v
+    return out

@@ -3,20 +3,20 @@ augment_ref.py in the example networks' MNIST layout, CIFAR-sized RGB into the r
 odd shapes with pitched rows and padded images, pad > H, N = 1, N = n, batches in mid-epoch and an ImageNet-sized batch from a
 dataset larger than L2; untouched pads and tails, reruns, batch sizes that split an epoch differently, every image once per
 epoch, the eval path against mnist_device, torch eager building the same batch, refusals; and the GAP ResNet of
-test_avgpool_nhwc_gpu trained through the batcher, first as a drop-in for its pre-converted slices, then with a shuffle and a
+example_nets trained through the batcher, first as a drop-in for its pre-converted slices, then with a shuffle and a
 random crop."""
-import importlib
-
 import numpy as np
 import pytest
 import torch
 
 import augment_ref as A
+from augment_ref import torch_batch
+from example_nets import DEV, NAN_BF16, ResNetGAP, Slices, mnist_device, same_bits, train
 
 pytestmark = pytest.mark.gpu
 
-AP = importlib.import_module("test_avgpool_nhwc_gpu")
-DEV, NAN_BF16, ResNetGAP, NB, EPOCHS, LR_STEP, ACC_MIN = AP.DEV, AP.NAN_BF16, AP.ResNetGAP, AP.NB, AP.EPOCHS, AP.LR_STEP, AP.ACC_MIN
+NB, EPOCHS, LR_STEP = ResNetGAP.NB, ResNetGAP.EPOCHS, ResNetGAP.LR_STEP
+ACC_MIN = 0.88            # the threshold of the GAP ResNet trained on the pre-converted slices (test_avgpool_nhwc_gpu)
 TAIL = 64                 # elements past x that must stay untouched
 LABEL_SENTINEL = 0xAA
 SEED = 0x0123456789ABCDEF
@@ -117,26 +117,6 @@ def test_replay(eng, pkg, golden, name):
     print(f"{name}: vec {info['vec']}, grid {info['grid']}, rows per CTA {info['rows_per_cta']}, b {info['b']}")
 
 
-def torch_batch(images, i, oy, ox, fl, pad, mean, std, C_out):
-    """torch eager on the GPU: the batch of images [n][H][W][C] uint8 (device) at indices i with crop offsets (oy, ox) and flips fl
-    as NHWC bf16 [N][H][W][C_out].  The divisors are device tensors, so each division is IEEE (a CPU scalar divisor becomes a
-    multiply by its reciprocal)."""
-    n, H, W, C = images.shape
-    N = len(i)
-    t = lambda a, dt=torch.long: (a if torch.is_tensor(a) else torch.as_tensor(np.asarray(a))).to(device=images.device, dtype=dt)
-    crop = torch.nn.functional.pad(images[t(i)].permute(0, 3, 1, 2), (pad, pad, pad, pad))    # [N][C][H + 2 pad][W + 2 pad]
-    w = torch.arange(W, device=images.device)
-    rows = t(oy)[:, None] + torch.arange(H, device=images.device)[None, :]
-    cols = t(ox)[:, None] + torch.where(t(fl, torch.bool)[:, None], W - 1 - w[None, :], w[None, :])
-    u = crop[torch.arange(N, device=images.device)[:, None, None], :, rows[:, :, None], cols[:, None, :]]     # [N][H][W][C]
-    m = t(np.zeros(C) if mean is None else mean, torch.float32)
-    s = t(np.ones(C) if std is None else std, torch.float32)
-    v = u.float().div(torch.full((C,), 255.0, device=images.device)).sub(m).div(s).to(torch.bfloat16)
-    out = torch.zeros((N, H, W, C_out), dtype=torch.bfloat16, device=images.device)
-    out[..., :C] = v
-    return out
-
-
 @pytest.mark.parametrize("name", ["cifar-32x32x3-cout8", "odd-5x7x4-cout5", "imagenet-224-cout8"])
 def test_torch_eager_builds_the_same_batch(eng, pkg, golden, name):
     spec, first, N, shuffle, pad, flip, epoch, mean, std, C_out, row_pitch, image_rows = CASES[name]
@@ -196,7 +176,7 @@ def test_eval_path_is_mnist_device(eng, pkg, golden):
     included (the batcher's x starts zeroed and the pad is never written)"""
     b = pkg.ImageBatcher(eng, golden["test_u8"].reshape(-1, 28, 28), golden["test_labels"], NB, pad=2, flip=True, shuffle=True,
                          seed=SEED, row_pitch=32, image_rows=28)
-    old = bits(AP.mnist_device(pkg, golden["test_u8"])).reshape(-1, NB, 28, 32)
+    old = bits(mnist_device(pkg, golden["test_u8"])).reshape(-1, NB, 28, 32)
     for s in range(b.steps_per_epoch):
         _, lab = b.batch(s, training=False)
         assert np.array_equal(b.x.to_host(), old[s])
@@ -243,40 +223,6 @@ def test_refusals(eng, pkg):
 
 
 # ------------------------------------------------------------------------------------------------ end to end
-def train(eng, pkg, golden, batcher, epochs, check_first=None):
-    """ResNetGAP trained through batcher for `epochs`: (params after 5 steps, epoch mean losses, test accuracy through a test batcher
-    with training=False).  check_first(step, x bits, labels) runs on each of the first 5 batches."""
-    net = ResNetGAP(eng, pkg, AP.init_params())
-    losses, after5, step = [], None, 0
-    for ep in range(epochs):
-        batcher.epoch = ep
-        for s in range(batcher.steps_per_epoch):
-            x, lab = batcher.batch(s)
-            if check_first and step < 5:
-                check_first(step, batcher.x.to_host(), lab.to_host())
-            net.forward(x, lab)
-            net.backward()
-            net.sgd(LR_STEP)
-            losses.append(net.loss)
-            net.loss = torch.zeros(NB, dtype=torch.float32, device=DEV)
-            step += 1
-            if step == 5:
-                eng.sync()
-                after5 = net.params()
-    eng.sync()
-    spe = batcher.steps_per_epoch
-    ep_loss = [float(torch.stack(losses[e * spe:(e + 1) * spe]).double().mean()) for e in range(epochs)]
-    tb = pkg.ImageBatcher(eng, golden["test_u8"].reshape(-1, 28, 28), golden["test_labels"], NB, row_pitch=32, image_rows=28)
-    right = 0
-    for s in range(tb.steps_per_epoch):
-        net.forward(*tb.batch(s, training=False), training=False)
-        eng.sync()
-        right += int((net.pred.cpu().numpy() == golden["test_labels"][s * NB:(s + 1) * NB]).sum())
-    tb.close()
-    net.close()
-    return after5, ep_loss, right / (tb.steps_per_epoch * NB)
-
-
 def mnist_batcher(pkg, eng, golden, **k):
     return pkg.ImageBatcher(eng, golden["train_u8"].reshape(-1, 28, 28), golden["train_labels"], NB, row_pitch=32, image_rows=28, **k)
 
@@ -287,39 +233,46 @@ def test_resnet_gap_through_the_batcher(eng, pkg, golden):
     images): the first 5 batches and labels are bit-exact against the replay, a fresh run reproduces the parameters after 5
     steps, the loss falls over EPOCHS epochs and test accuracy, evaluated through the batcher with training=False, exceeds
     ACC_MIN."""
-    xs, ys = AP.mnist_device(pkg, golden["train_u8"]), torch.from_numpy(golden["train_labels"]).to(DEV)
-    row_bytes = 28 * 32 * 2
-    net = ResNetGAP(eng, pkg, AP.init_params())
-    for s in range(5):
-        net.forward(xs.data_ptr() + s * NB * row_bytes, ys[s * NB:(s + 1) * NB])
-        net.backward()
-        net.sgd(LR_STEP)
-    eng.sync()
-    old5 = net.params()
-    net.close()
+    slices = Slices(pkg, golden["train_u8"], golden["train_labels"], NB)
+    net = ResNetGAP(eng, pkg, ResNetGAP.init_params())
+    try:
+        for s in range(5):
+            net.forward(*slices.batch(s))
+            net.backward()
+            net.sgd(LR_STEP)
+        eng.sync()
+        old5 = net.params()
+    finally:
+        net.close()
 
+    make = lambda: ResNetGAP(eng, pkg, ResNetGAP.init_params())
+    tests = pkg.ImageBatcher(eng, golden["test_u8"].reshape(-1, 28, 28), golden["test_labels"], NB, row_pitch=32, image_rows=28)
     plain = mnist_batcher(pkg, eng, golden, shuffle=False)
-    old = bits(xs).reshape(-1, NB, 28, 32)
+    old = bits(slices.x).reshape(-1, NB, 28, 32)
 
-    def same_as_slices(step, xb, lab):
-        assert np.array_equal(xb, old[step]) and np.array_equal(lab, golden["train_labels"][step * NB:(step + 1) * NB])
+    def same_as_slices(net, step, x, lab):
+        assert np.array_equal(plain.x.to_host(), old[step]) and np.array_equal(lab.to_host(), golden["train_labels"][step * NB:(step + 1) * NB])
+        net.forward(x, lab)
+        net.backward()
 
-    p5, loss_plain, acc_plain = train(eng, pkg, golden, plain, EPOCHS, same_as_slices)
+    loss_plain, acc_plain, p5 = train(eng, pkg, golden, make, EPOCHS, batches=plain, tests=tests, check_step=same_as_slices)
     plain.close()
-    assert all(np.array_equal(a.view(np.uint32), b.view(np.uint32)) for a, b in zip(p5, old5))
+    assert same_bits(p5, old5)
 
     train_u8 = golden["train_u8"].reshape(-1, 28, 28, 1)
+    aug = mnist_batcher(pkg, eng, golden, pad=2, flip=False, shuffle=True, seed=SEED)
 
-    def replayed(step, xb, lab):
+    def replayed(net, step, x, lab):
+        xb = aug.x.to_host()
         wx, wl, *_ = A.batch(train_u8, step * NB, NB, 1, 2, 0, SEED, 0, labels=golden["train_labels"])
         assert np.array_equal(xb[:, :, :28], wx.reshape(NB, 28, 28)) and (xb[:, :, 28:] == 0).all()
-        assert np.array_equal(lab, wl)
+        assert np.array_equal(lab.to_host(), wl)
+        net.forward(x, lab)
+        net.backward()
 
-    aug = mnist_batcher(pkg, eng, golden, pad=2, flip=False, shuffle=True, seed=SEED)
-    a5, _, _ = train(eng, pkg, golden, aug, 1, replayed)
-    b5, loss_aug, acc_aug = train(eng, pkg, golden, aug, EPOCHS)
+    loss_aug, acc_aug, _ = train(eng, pkg, golden, make, EPOCHS, batches=aug, tests=tests, check_step=replayed)
     aug.close()
-    assert all(np.array_equal(a.view(np.uint32), b.view(np.uint32)) for a, b in zip(a5, b5))
+    tests.close()
     print(f"GAP ResNet through the batcher: plain mean loss {loss_plain[0]:.4f} -> {loss_plain[-1]:.4f}, test accuracy {acc_plain:.4f}; "
           f"shuffle + crop (pad 2) {loss_aug[0]:.4f} -> {loss_aug[-1]:.4f}, test accuracy {acc_aug:.4f} (threshold {ACC_MIN})")
     assert np.isfinite(loss_aug).all() and loss_aug[-1] < loss_aug[0]

@@ -16,11 +16,10 @@ import torch
 import avgpool_ref as AR
 import maxpool_ref as MR
 from avgpool_ref import gap_bound
+from example_nets import DEV, NAN_BF16, ResNetGAP, host, train
 
 pytestmark = pytest.mark.gpu
 
-DEV = torch.device("cuda", 0)
-NAN_BF16 = 0x7FC0
 U = 2.0 ** -24
 
 CASES = [  # id, N, H, W, C, R, S, stride, pad_h, pad_w, row_pitch (0 = Q*C rounded up to 8), image_rows (0 = P)
@@ -237,119 +236,7 @@ def test_refusals(eng, pkg):
 
 
 # ------------------------------------------------------------------------------------------------ end to end
-NB = 128
-LR_STEP = 0.2
-EPOCHS = 40
 ACC_MIN = 0.88          # a float32 torch CPU replica of this network, initialisation and step reaches 0.949 (DESIGN 3.16)
-
-
-def init_params(seed=9):
-    rng = np.random.default_rng(seed)
-    u = lambda shape, fan: rng.uniform(-1, 1, shape).astype(np.float32) / np.float32(np.sqrt(fan))
-    return dict(f1=u((8, 5, 5, 1), 25), f2=u((16, 3, 3, 8), 72), f3=u((16, 3, 3, 16), 144), f4=u((16, 3, 3, 16), 144),
-                f5=u((32, 3, 3, 16), 144), f6=u((32, 3, 3, 32), 288), f7=u((32, 3, 3, 16), 144), w8=u((10, 1, 1, 32), 32), b8=u(10, 32))
-
-
-class ResNetGAP:
-    """conv 8@5x5 -> BN+ReLU -> avg pool 2 -> conv 16@3x3 pad 1 -> BN+ReLU (x0) -> [conv 16@3x3 pad 1 -> BN+ReLU -> conv 16@3x3
-    pad 1 -> BN + x0 -> ReLU] (x1) -> [conv 32@3x3 stride 2 pad 1 -> BN+ReLU -> conv 32@3x3 pad 1 -> BN + s -> ReLU, s = BN(conv
-    32@3x3 stride 2 pad 1 (x1))] -> GAP -> fc 32->10 -> softmax CE (1/B).  The convs have no bias.  The projection is 3x3 rather
-    than ResNet's 1x1: a 1x1 stride-2 conv over 16 channels is a row-Toeplitz layer, whose input gradient has no 1x1 kernel."""
-
-    def __init__(self, eng, pkg, p):
-        self.eng = eng
-        relu, none = pkg.ACT_RELU, pkg.ACT_NONE
-        B = NB
-        conv = lambda H, C, K, R, f, **k: pkg.ConvLayer(eng, B, H, H, C, K, R, R, p[f], None, act=none, **k)
-        self.c1 = conv(28, 1, 8, 5, "f1")
-        self.c2 = conv(12, 8, 16, 3, "f2", padding=(1, 1))
-        self.c3, self.c4 = conv(12, 16, 16, 3, "f3", padding=(1, 1)), conv(12, 16, 16, 3, "f4", padding=(1, 1))
-        self.c5 = conv(12, 16, 32, 3, "f5", padding=(1, 1), stride=2)
-        self.c6 = conv(6, 32, 32, 3, "f6", padding=(1, 1))
-        self.c7 = conv(12, 16, 32, 3, "f7", padding=(1, 1), stride=2)
-        assert self.c5.out_shape == self.c7.out_shape == (B, 6, 6, 32)
-        BN = lambda H, C, act: pkg.BatchNormLayer(eng, B, H, H, C, act=act)
-        self.bn = [BN(24, 8, relu), BN(12, 16, relu), BN(12, 16, relu), BN(12, 16, relu), BN(6, 32, relu), BN(6, 32, relu), BN(6, 32, none)]
-        self.pool = pkg.AvgPoolLayer(eng, B, 24, 24, 8, 2, row_pitch=self.c2.row_pitch, image_rows=self.c2.image_rows)
-        self.gap = pkg.GlobalAvgPoolLayer(eng, B, 6, 6, 32)
-        self.fc = pkg.LinearLayer(eng, B, 1, 1, 32, 10, p["w8"], p["b8"], act=none, row_pitch=self.gap.row_pitch)
-        buf = lambda *shape: torch.full(shape, NAN_BF16, dtype=torch.int16, device=DEV)
-        self.y1, self.z1, self.dz1, self.dy1 = (buf(B, 24, 24, 8) for _ in range(4))
-        self.x2, self.dx2 = buf(B, 12, self.c2.row_pitch), buf(B, 12, self.c2.row_pitch)
-        (self.y2, self.x0, self.y3, self.z3, self.y4, self.x1, self.dx1, self.dx1p, self.dy4, self.dres, self.dz3, self.dy3, self.dx0,
-         self.dy2) = (buf(B, 12, 12, 16) for _ in range(14))
-        (self.y5, self.z5, self.y6, self.out, self.y7, self.s, self.dout, self.dy6, self.ds, self.dy7, self.dz5,
-         self.dy5) = (buf(B, 6, 6, 32) for _ in range(12))
-        self.h, self.dh = buf(B, self.gap.row_pitch), buf(B, self.gap.row_pitch)
-        self.z, self.dz = buf(B, 10), buf(B, 10)
-        self.loss = torch.zeros(B, dtype=torch.float32, device=DEV)
-        self.pred = torch.zeros(B, dtype=torch.int32, device=DEV)
-
-    def forward(self, x, labels, training=True):
-        b1, b2, b3, b4, b5, b6, b7 = self.bn
-        self.c1.forward(x, self.y1)
-        b1.forward(self.y1, self.z1, training=training)
-        self.pool.forward(self.z1, self.x2)
-        self.c2.forward(self.x2, self.y2)
-        b2.forward(self.y2, self.x0, training=training)
-        self.c3.forward(self.x0, self.y3)
-        b3.forward(self.y3, self.z3, training=training)
-        self.c4.forward(self.z3, self.y4)
-        b4.forward(self.y4, self.x1, r=self.x0, training=training)
-        self.c5.forward(self.x1, self.y5)
-        b5.forward(self.y5, self.z5, training=training)
-        self.c6.forward(self.z5, self.y6)
-        self.c7.forward(self.x1, self.y7)
-        b7.forward(self.y7, self.s, training=training)
-        b6.forward(self.y6, self.out, r=self.s, training=training)
-        self.gap.forward(self.out, self.h)
-        self.fc.forward(self.h, self.z)
-        self.eng.softmax_ce_bf16(self.z, labels, NB, 10, 1.0 / NB, self.dz, self.loss, self.pred)
-
-    def backward(self):
-        b1, b2, b3, b4, b5, b6, b7 = self.bn
-        self.fc.backward(self.z, self.dz, self.dh)
-        self.gap.backward(self.dh, self.dout)
-        b6.backward(self.out, self.dout, self.dy6, dr=self.ds)
-        self.c6.backward(self.y6, self.dy6, self.dz5)
-        b5.backward(self.z5, self.dz5, self.dy5)
-        self.c5.backward(self.y5, self.dy5, self.dx1)
-        b7.backward(self.s, self.ds, self.dy7)
-        self.c7.backward(self.y7, self.dy7, self.dx1p)
-        b4.backward(self.x1, self.dx1, self.dy4, dr=self.dres, dy2=self.dx1p)      # main path and projection meet at x1
-        self.c4.backward(self.y4, self.dy4, self.dz3)
-        b3.backward(self.z3, self.dz3, self.dy3)
-        self.c3.backward(self.y3, self.dy3, self.dx0)
-        b2.backward(self.x0, self.dx0, self.dy2, dy2=self.dres)
-        self.c2.backward(self.y2, self.dy2, self.dx2)
-        self.pool.backward(self.dx2, self.dz1)
-        b1.backward(self.z1, self.dz1, self.dy1)
-        self.c1.backward(self.y1, self.dy1, None)
-
-    def layers(self):
-        return (self.c1, self.c2, self.c3, self.c4, self.c5, self.c6, self.c7, self.fc, *self.bn)
-
-    def sgd(self, lr):
-        for layer in self.layers():
-            layer.sgd(lr)
-
-    def params(self):
-        return [a for layer in self.layers() for a in layer.params() if a is not None]
-
-    def close(self):
-        for layer in (*self.layers(), self.pool, self.gap):
-            layer.close()
-
-
-def mnist_device(pkg, u8):
-    n = u8.shape[0]
-    xl = np.zeros((n * 28, 32), np.uint16)
-    xl[:, :28] = pkg.f32_to_bf16_bits(u8.reshape(n, 28, 28).astype(np.float32) / 255.0).reshape(n * 28, 28)
-    return torch.from_numpy(xl.view(np.int16)).to(DEV)
-
-
-def host(t):
-    return t.cpu().numpy().view(np.uint16)
 
 
 def test_resnet_gap_mnist(eng, pkg, golden):
@@ -357,15 +244,11 @@ def test_resnet_gap_mnist(eng, pkg, golden):
     tensors, and GAP's y lies within its error model.  A fresh run reproduces the parameters after 5 steps bit for bit.  After
     EPOCHS epochs over the 1024 training digits the mean loss has fallen, and test accuracy on the 256 test digits, evaluated with
     the running statistics, exceeds ACC_MIN."""
-    xs, ys = mnist_device(pkg, golden["train_u8"]), torch.from_numpy(golden["train_labels"]).to(DEV)
-    xt, yt = mnist_device(pkg, golden["test_u8"]), torch.from_numpy(golden["test_labels"]).to(DEV)
-    row_bytes = 28 * 32 * 2
-    batch = lambda s, xs=xs, ys=ys: (xs.data_ptr() + s * NB * row_bytes, ys[s * NB:(s + 1) * NB])
     bf, f32 = pkg.f32_to_bf16_bits, pkg.bf16_bits_to_f32
+    NB = ResNetGAP.NB
 
-    net = ResNetGAP(eng, pkg, init_params())
-    for it in range(5):
-        net.forward(*batch(it))
+    def check_step(net, it, x, labels):
+        net.forward(x, labels)
         eng.sync()
         z1, x2, out, h = host(net.z1), host(net.x2), host(net.out), host(net.h)
         net.backward()
@@ -377,32 +260,8 @@ def test_resnet_gap_mnist(eng, pkg, golden):
         _, _, lo, hi = gap_bound(pkg, f32(out).reshape(NB, 6, 6, 32), net.gap.info)
         yf = f32(h[:, :32])
         assert np.all((yf >= lo) & (yf <= hi)), it
-        net.sgd(LR_STEP)
-        eng.sync()
-    after5 = net.params()
-    net.close()
 
-    net = ResNetGAP(eng, pkg, init_params())
-    losses = []
-    for ep in range(EPOCHS):
-        for s in range(1024 // NB):
-            net.forward(*batch(s))
-            net.backward()
-            net.sgd(LR_STEP)
-            losses.append(net.loss)
-            net.loss = torch.zeros(NB, dtype=torch.float32, device=DEV)
-            if ep == 0 and s == 4:
-                eng.sync()
-                assert all(np.array_equal(a.view(np.uint32), b_.view(np.uint32)) for a, b_ in zip(net.params(), after5))
-    eng.sync()
-    ep_loss = [float(torch.stack(losses[e * 8:(e + 1) * 8]).double().mean()) for e in range(EPOCHS)]
-    right = 0
-    for s in range(2):
-        net.forward(*batch(s, xt, yt), training=False)
-        eng.sync()
-        right += int((net.pred.cpu().numpy() == golden["test_labels"][s * NB:(s + 1) * NB]).sum())
-    acc = right / 256
-    net.close()
+    ep_loss, acc, _ = train(eng, pkg, golden, lambda: ResNetGAP(eng, pkg, ResNetGAP.init_params()), ResNetGAP.EPOCHS, check_step=check_step)
     print(f"GAP ResNet: mean loss by epoch {ep_loss[0]:.4f} -> {ep_loss[-1]:.4f}; test accuracy {acc:.4f} (threshold {ACC_MIN})")
     assert np.isfinite(ep_loss).all() and ep_loss[-1] < ep_loss[0]
     assert acc > ACC_MIN

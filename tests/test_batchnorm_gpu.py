@@ -19,11 +19,10 @@ import batchnorm_ref as BR
 import conv_ref as CR
 import conv_ref_strided as CS
 from batchnorm_ref import ITERS, U, check_stats, n_acc, n_stat  # noqa: F401
+from example_nets import NAN_BF16, ResNet, host, train
 
 pytestmark = pytest.mark.gpu
 
-NAN_BF16 = 0x7FC0
-DEV = torch.device("cuda", 0)
 TAIL = 64
 
 CS_ = [1, 6, 8, 16, 64, 120, 256]
@@ -396,102 +395,7 @@ def test_conv_bn_relu_step(eng, pkg):
 
 
 # ------------------------------------------------------------------------------------------------ end to end
-NB = 128
-LR_STEP = 0.05
-EPOCHS = 40
 ACC_MIN = 0.90          # a float32 torch CPU replica of this network, initialisation and step reaches 0.973
-
-
-def init_params(seed=7):
-    rng = np.random.default_rng(seed)
-    u = lambda shape, fan: rng.uniform(-1, 1, shape).astype(np.float32) / np.float32(np.sqrt(fan))
-    return dict(f1=u((8, 5, 5, 1), 25), f2=u((16, 3, 3, 8), 72), f3=u((16, 3, 3, 16), 144), f4=u((16, 3, 3, 16), 144),
-                w5=u((10, 6, 6, 16), 576), b5=u(10, 576))
-
-
-class ResNet:
-    """conv 8@5x5 -> BN+ReLU -> pool 2 -> conv 16@3x3 pad 1 -> BN+ReLU (x0) -> [conv 16@3x3 pad 1 -> BN+ReLU -> conv 16@3x3 pad 1
-    -> BN + x0 -> ReLU] -> pool 2 -> fc 576->10 -> softmax CE (1/B).  The convs have no bias."""
-
-    def __init__(self, eng, pkg, p):
-        self.eng = eng
-        relu, none = pkg.ACT_RELU, pkg.ACT_NONE
-        B = NB
-        self.c1 = pkg.ConvLayer(eng, B, 28, 28, 1, 8, 5, 5, p["f1"], None, act=none)
-        self.c2 = pkg.ConvLayer(eng, B, 12, 12, 8, 16, 3, 3, p["f2"], None, act=none, padding=(1, 1))
-        self.c3 = pkg.ConvLayer(eng, B, 12, 12, 16, 16, 3, 3, p["f3"], None, act=none, padding=(1, 1))
-        self.c4 = pkg.ConvLayer(eng, B, 12, 12, 16, 16, 3, 3, p["f4"], None, act=none, padding=(1, 1))
-        assert self.c3.row_pitch == 12 * 16 and self.c4.row_pitch == 12 * 16     # a dense BN output is their x layout
-        self.fc = pkg.LinearLayer(eng, B, 6, 6, 16, 10, p["w5"], p["b5"], act=none)
-        self.bn = [pkg.BatchNormLayer(eng, B, 24, 24, 8, act=relu)] + [pkg.BatchNormLayer(eng, B, 12, 12, 16, act=relu) for _ in range(3)]
-        self.p1 = pkg.MaxPoolLayer(eng, B, 24, 24, 8, 2, row_pitch=self.c2.row_pitch, image_rows=self.c2.image_rows)
-        self.p2 = pkg.MaxPoolLayer(eng, B, 12, 12, 16, 2, row_pitch=self.fc.row_pitch, image_rows=self.fc.image_rows)
-        buf = lambda *shape: torch.full(shape, NAN_BF16, dtype=torch.int16, device=DEV)
-        self.y1, self.z1, self.dz1, self.dy1 = (buf(B, 24, 24, 8) for _ in range(4))
-        self.x2, self.dx2 = buf(B, 12, self.c2.row_pitch), buf(B, 12, self.c2.row_pitch)
-        (self.y2, self.x0, self.y3, self.z3, self.y4, self.out, self.dout, self.dy4, self.dres, self.dz3, self.dy3, self.dx0,
-         self.dy2) = (buf(B, 12, 12, 16) for _ in range(13))
-        self.x5, self.dx5 = buf(B, 6, self.fc.row_pitch), buf(B, 6, self.fc.row_pitch)
-        self.z, self.dz = buf(B, 10), buf(B, 10)
-        self.loss = torch.zeros(B, dtype=torch.float32, device=DEV)
-        self.pred = torch.zeros(B, dtype=torch.int32, device=DEV)
-
-    def forward(self, x, labels, training=True):
-        b1, b2, b3, b4 = self.bn
-        self.c1.forward(x, self.y1)
-        b1.forward(self.y1, self.z1, training=training)
-        self.p1.forward(self.z1, self.x2)
-        self.c2.forward(self.x2, self.y2)
-        b2.forward(self.y2, self.x0, training=training)
-        self.c3.forward(self.x0, self.y3)
-        b3.forward(self.y3, self.z3, training=training)
-        self.c4.forward(self.z3, self.y4)
-        b4.forward(self.y4, self.out, r=self.x0, training=training)
-        self.p2.forward(self.out, self.x5)
-        self.fc.forward(self.x5, self.z)
-        self.eng.softmax_ce_bf16(self.z, labels, NB, 10, 1.0 / NB, self.dz, self.loss, self.pred)
-
-    def backward(self):
-        b1, b2, b3, b4 = self.bn
-        self.fc.backward(self.z, self.dz, self.dx5)
-        self.p2.backward(self.dx5, self.dout)
-        b4.backward(self.out, self.dout, self.dy4, dr=self.dres)
-        self.c4.backward(self.y4, self.dy4, self.dz3)
-        b3.backward(self.z3, self.dz3, self.dy3)
-        self.c3.backward(self.y3, self.dy3, self.dx0)
-        b2.backward(self.x0, self.dx0, self.dy2, dy2=self.dres)
-        self.c2.backward(self.y2, self.dy2, self.dx2)
-        self.p1.backward(self.dx2, self.dz1)
-        b1.backward(self.z1, self.dz1, self.dy1)
-        self.c1.backward(self.y1, self.dy1, None)
-
-    # (BN layer, its x, r, y, dy, dy2, dx) for the replays
-    def bn_tensors(self):
-        b1, b2, b3, b4 = self.bn
-        return [(b1, self.y1, None, self.z1, self.dz1, None, self.dy1), (b2, self.y2, None, self.x0, self.dx0, self.dres, self.dy2),
-                (b3, self.y3, None, self.z3, self.dz3, None, self.dy3), (b4, self.y4, self.x0, self.out, self.dout, None, self.dy4)]
-
-    def sgd(self, lr):
-        for layer in (self.c1, self.c2, self.c3, self.c4, self.fc, *self.bn):
-            layer.sgd(lr)
-
-    def params(self):
-        return [a for layer in (self.c1, self.c2, self.c3, self.c4, self.fc, *self.bn) for a in layer.params() if a is not None]
-
-    def close(self):
-        for layer in (self.c1, self.c2, self.c3, self.c4, self.fc, *self.bn, self.p1, self.p2):
-            layer.close()
-
-
-def mnist_device(pkg, u8):
-    n = u8.shape[0]
-    xl = np.zeros((n * 28, 32), np.uint16)
-    xl[:, :28] = pkg.f32_to_bf16_bits(u8.reshape(n, 28, 28).astype(np.float32) / 255.0).reshape(n * 28, 28)
-    return torch.from_numpy(xl.view(np.int16)).to(DEV)
-
-
-def host(t):
-    return t.cpu().numpy().view(np.uint16)
 
 
 def test_resnet_mnist(eng, pkg, golden):
@@ -499,14 +403,9 @@ def test_resnet_mnist(eng, pkg, golden):
     statistics and gradient sums.  A second fresh run reproduces the parameters after 5 steps bit for bit.  After EPOCHS epochs
     over the 1024 training digits the mean loss has fallen, and test accuracy on the 256 test digits, evaluated with the running
     statistics, exceeds ACC_MIN."""
-    xs, ys = mnist_device(pkg, golden["train_u8"]), torch.from_numpy(golden["train_labels"]).to(DEV)
-    xt, yt = mnist_device(pkg, golden["test_u8"]), torch.from_numpy(golden["test_labels"]).to(DEV)
-    row_bytes = 28 * 32 * 2
-    batch = lambda s, xs=xs, ys=ys: (xs.data_ptr() + s * NB * row_bytes, ys[s * NB:(s + 1) * NB])
 
-    net = ResNet(eng, pkg, init_params())
-    for it in range(5):
-        net.forward(*batch(it))
+    def check_step(net, it, x, labels):
+        net.forward(x, labels)
         eng.sync()
         fwd = [(bn, host(x), None if r is None else host(r), host(y), bn.save_mean.to_host(), bn.save_rstd.to_host(), bn.params())
                for bn, x, r, y, _, _, _ in net.bn_tensors()]
@@ -521,32 +420,8 @@ def test_resnet_mnist(eng, pkg, golden):
             assert np.array_equal(host(dx).reshape(-1, C), want), it
             frac = float((pkg.bf16_bits_to_f32(yb) > 0).mean())
             assert 0.1 < frac < 0.95, (it, frac)        # the ReLU is neither dead nor linear
-        net.sgd(LR_STEP)
-        eng.sync()
-    after5 = net.params()
-    net.close()
 
-    net = ResNet(eng, pkg, init_params())
-    losses = []
-    for ep in range(EPOCHS):
-        for s in range(1024 // NB):
-            net.forward(*batch(s))
-            net.backward()
-            net.sgd(LR_STEP)
-            losses.append(net.loss)
-            net.loss = torch.zeros(NB, dtype=torch.float32, device=DEV)
-            if ep == 0 and s == 4:
-                eng.sync()
-                assert all(np.array_equal(a.view(np.uint32), b_.view(np.uint32)) for a, b_ in zip(net.params(), after5))
-    eng.sync()
-    ep_loss = [float(torch.stack(losses[e * 8:(e + 1) * 8]).double().mean()) for e in range(EPOCHS)]
-    right = 0
-    for s in range(2):
-        net.forward(*batch(s, xt, yt), training=False)
-        eng.sync()
-        right += int((net.pred.cpu().numpy() == golden["test_labels"][s * NB:(s + 1) * NB]).sum())
-    acc = right / 256
-    net.close()
+    ep_loss, acc, _ = train(eng, pkg, golden, lambda: ResNet(eng, pkg, ResNet.init_params()), ResNet.EPOCHS, check_step=check_step)
     print(f"BN ResNet: mean loss by epoch {ep_loss[0]:.4f} -> {ep_loss[-1]:.4f}; test accuracy {acc:.4f} (threshold {ACC_MIN})")
     assert np.isfinite(ep_loss).all() and ep_loss[-1] < ep_loss[0]
     assert acc > ACC_MIN

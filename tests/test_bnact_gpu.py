@@ -6,17 +6,15 @@ refusals; a BatchNormLayer step at each code with SGD and AdamW over it; and an 
 digits, checked bit for bit at every new-code BN in its first steps."""
 import numpy as np
 import pytest
-import torch
 
 import batchnorm_ref as BR
 import bnact_ref as AR
 import optim_ref as OR
 from batchnorm_ref import U, n_acc
+from example_nets import NAN_BF16, EfficientNetLite, host, train
 
 pytestmark = pytest.mark.gpu
 
-NAN_BF16 = 0x7FC0
-DEV = torch.device("cuda", 0)
 TAIL = 64
 IDS = {c: AR.NAMES[c] for c in AR.CODES}
 
@@ -345,138 +343,7 @@ def test_optimizers(eng, pkg, kind):
 
 
 # ------------------------------------------------------------------------------------------------ end to end
-NB = 128
-LR_STEP = 0.2
-EPOCHS = 30
 ACC_MIN = 0.85          # the float32 torch CPU replica (scripts/efficientnet_replica.py) of this network reaches 0.902 (DESIGN 3.20)
-
-
-def init_params(seed=31):
-    rng = np.random.default_rng(seed)
-    u = lambda shape, fan: rng.uniform(-1, 1, shape).astype(np.float32) / np.float32(np.sqrt(fan))
-    return dict(f0=u((48, 5, 5, 1), 25), e1=u((96, 1, 1, 48), 48), d1=u((96, 3, 3), 9), p1=u((48, 1, 1, 96), 96),
-                e2=u((96, 1, 1, 48), 48), d2=u((96, 5, 5), 25), p2=u((48, 1, 1, 96), 96), h=u((128, 1, 1, 48), 48),
-                w8=u((10, 1, 1, 128), 128), b8=u(10, 128),
-                s1=u((8, 96), 96), sb1=u(8, 96), s2=u((96, 8), 8), sb2=u(96, 8))
-
-
-class EfficientNetLite:
-    """stem conv 48@5x5 -> BN+SiLU -> avg pool 2 (12x12x48) -> MBConv [1x1 48->96, BN+ReLU6, depthwise 3x3/2 pad 1, BN+ReLU6,
-    1x1 96->48, BN] (x1, 6x6x48) -> MBConv [1x1 48->96, BN+SiLU, depthwise 5x5 pad 2, BN+SiLU, SE 96->8->96, 1x1 96->48, BN + x1]
-    -> 1x1 48->128, BN+hard-swish -> GAP -> fc 128->10 -> softmax CE (1/B).  The convs have no bias.  Every 1x1 conv reads >= 48
-    channels, so each is a wide-family layer, which has a 1x1 input gradient.  Each new-code BN also writes dr (= g) so that the
-    test can read the gradient it formed."""
-
-    def __init__(self, eng, pkg, p):
-        self.eng = eng
-        none, silu, hs, r6 = pkg.ACT_NONE, pkg.ACT_SILU, pkg.ACT_HARDSWISH, pkg.ACT_RELU6
-        B = NB
-        conv = lambda H, C, K, R, f: pkg.ConvLayer(eng, B, H, H, C, K, R, R, p[f], None, act=none)
-        self.stem = conv(28, 1, 48, 5, "f0")
-        self.e1, self.p1 = conv(12, 48, 96, 1, "e1"), conv(6, 96, 48, 1, "p1")
-        self.e2, self.p2, self.hd = conv(6, 48, 96, 1, "e2"), conv(6, 96, 48, 1, "p2"), conv(6, 48, 128, 1, "h")
-        assert all(c.family == "wide" for c in (self.e1, self.p1, self.e2, self.p2, self.hd))
-        self.d1 = pkg.DepthwiseConvLayer(eng, B, 12, 12, 96, 3, 3, p["d1"], None, act=none, stride=2, padding=(1, 1))
-        self.d2 = pkg.DepthwiseConvLayer(eng, B, 6, 6, 96, 5, 5, p["d2"], None, act=none, stride=1, padding=(2, 2))
-        assert self.d1.out_shape == (B, 6, 6, 96) and self.d2.out_shape == (B, 6, 6, 96)
-        self.se = pkg.SqueezeExcitationLayer(eng, B, 6, 6, 96, 8, p["s1"], p["sb1"], p["s2"], p["sb2"], act=none)
-        BN = lambda H, C, act: pkg.BatchNormLayer(eng, B, H, H, C, act=act)
-        self.bn = [BN(24, 48, silu), BN(12, 96, r6), BN(6, 96, r6), BN(6, 48, none), BN(6, 96, silu), BN(6, 96, silu), BN(6, 48, none),
-                   BN(6, 128, hs)]
-        self.pool = pkg.AvgPoolLayer(eng, B, 24, 24, 48, 2, row_pitch=self.e1.row_pitch, image_rows=self.e1.image_rows)
-        self.gap = pkg.GlobalAvgPoolLayer(eng, B, 6, 6, 128)
-        self.fc = pkg.LinearLayer(eng, B, 1, 1, 128, 10, p["w8"], p["b8"], act=none, row_pitch=self.gap.row_pitch)
-        buf = lambda *shape: torch.full(shape, NAN_BF16, dtype=torch.int16, device=DEV)
-        self.y0, self.z0, self.dz0, self.dy0, self.g0 = (buf(B, 24, 24, 48) for _ in range(5))
-        self.x1p, self.dx1p = buf(B, 12, self.e1.row_pitch), buf(B, 12, self.e1.row_pitch)
-        self.ye1, self.ze1, self.dze1, self.dye1, self.ge1 = (buf(B, 12, 12, 96) for _ in range(5))
-        (self.yd1, self.zd1, self.dzd1, self.dyd1, self.gd1, self.ye2, self.ze2, self.dze2, self.dye2, self.ge2, self.yd2, self.zd2,
-         self.dzd2, self.dyd2, self.gd2, self.se_y, self.dse_y) = (buf(B, 6, 6, 96) for _ in range(17))
-        (self.yp1, self.x1, self.dx1, self.dyp1, self.yp2, self.x2, self.dx2, self.dyp2, self.dres, self.dx1b) = (buf(B, 6, 6, 48) for _ in range(10))
-        self.yh, self.zh, self.dzh, self.dyh, self.gh = (buf(B, 6, 6, 128) for _ in range(5))
-        self.hp, self.dhp = buf(B, self.gap.row_pitch), buf(B, self.gap.row_pitch)
-        self.z, self.dz = buf(B, 10), buf(B, 10)
-        self.loss = torch.zeros(B, dtype=torch.float32, device=DEV)
-        self.pred = torch.zeros(B, dtype=torch.int32, device=DEV)
-
-    def forward(self, x, labels, training=True):
-        b0, be1, bd1, bp1, be2, bd2, bp2, bh = self.bn
-        self.stem.forward(x, self.y0)
-        b0.forward(self.y0, self.z0, training=training)
-        self.pool.forward(self.z0, self.x1p)
-        self.e1.forward(self.x1p, self.ye1)
-        be1.forward(self.ye1, self.ze1, training=training)
-        self.d1.forward(self.ze1, self.yd1)
-        bd1.forward(self.yd1, self.zd1, training=training)
-        self.p1.forward(self.zd1, self.yp1)
-        bp1.forward(self.yp1, self.x1, training=training)
-        self.e2.forward(self.x1, self.ye2)
-        be2.forward(self.ye2, self.ze2, training=training)
-        self.d2.forward(self.ze2, self.yd2)
-        bd2.forward(self.yd2, self.zd2, training=training)
-        self.se.forward(self.zd2, self.se_y)
-        self.p2.forward(self.se_y, self.yp2)
-        bp2.forward(self.yp2, self.x2, r=self.x1, training=training)
-        self.hd.forward(self.x2, self.yh)
-        bh.forward(self.yh, self.zh, training=training)
-        self.gap.forward(self.zh, self.hp)
-        self.fc.forward(self.hp, self.z)
-        self.eng.softmax_ce_bf16(self.z, labels, NB, 10, 1.0 / NB, self.dz, self.loss, self.pred)
-
-    def backward(self):
-        b0, be1, bd1, bp1, be2, bd2, bp2, bh = self.bn
-        self.fc.backward(self.z, self.dz, self.dhp)
-        self.gap.backward(self.dhp, self.dzh)
-        bh.backward(self.zh, self.dzh, self.dyh, dr=self.gh)
-        self.hd.backward(self.yh, self.dyh, self.dx2)
-        bp2.backward(self.x2, self.dx2, self.dyp2, dr=self.dres)
-        self.p2.backward(self.yp2, self.dyp2, self.dse_y)
-        self.se.backward(self.se_y, self.dse_y, self.dzd2)
-        bd2.backward(self.zd2, self.dzd2, self.dyd2, dr=self.gd2)
-        self.d2.backward(self.yd2, self.dyd2, self.dze2)
-        be2.backward(self.ze2, self.dze2, self.dye2, dr=self.ge2)
-        self.e2.backward(self.ye2, self.dye2, self.dx1b)
-        bp1.backward(self.x1, self.dx1b, self.dyp1, dy2=self.dres)                  # the block's two paths meet at x1
-        self.p1.backward(self.yp1, self.dyp1, self.dzd1)
-        bd1.backward(self.zd1, self.dzd1, self.dyd1, dr=self.gd1)
-        self.d1.backward(self.yd1, self.dyd1, self.dze1)
-        be1.backward(self.ze1, self.dze1, self.dye1, dr=self.ge1)
-        self.e1.backward(self.ye1, self.dye1, self.dx1p)
-        self.pool.backward(self.dx1p, self.dz0)
-        b0.backward(self.z0, self.dz0, self.dy0, dr=self.g0)
-        self.stem.backward(self.y0, self.dy0, None)
-
-    # (new-code BN layer, its x, y, dy, dx, g) for the replays
-    def bn_tensors(self):
-        b0, be1, bd1, bp1, be2, bd2, bp2, bh = self.bn
-        return [(b0, self.y0, self.z0, self.dz0, self.dy0, self.g0), (be1, self.ye1, self.ze1, self.dze1, self.dye1, self.ge1),
-                (bd1, self.yd1, self.zd1, self.dzd1, self.dyd1, self.gd1), (be2, self.ye2, self.ze2, self.dze2, self.dye2, self.ge2),
-                (bd2, self.yd2, self.zd2, self.dzd2, self.dyd2, self.gd2), (bh, self.yh, self.zh, self.dzh, self.dyh, self.gh)]
-
-    def layers(self):
-        return (self.stem, self.e1, self.d1, self.p1, self.e2, self.d2, self.p2, self.hd, self.fc, self.se, *self.bn)
-
-    def sgd(self, lr):
-        for layer in self.layers():
-            layer.sgd(lr)
-
-    def params(self):
-        return [a for layer in self.layers() for a in layer.params() if a is not None]
-
-    def close(self):
-        for layer in (*self.layers(), self.pool, self.gap):
-            layer.close()
-
-
-def mnist_device(pkg, u8):
-    n = u8.shape[0]
-    xl = np.zeros((n * 28, 32), np.uint16)
-    xl[:, :28] = pkg.f32_to_bf16_bits(u8.reshape(n, 28, 28).astype(np.float32) / 255.0).reshape(n * 28, 28)
-    return torch.from_numpy(xl.view(np.int16)).to(DEV)
-
-
-def host(t):
-    return t.cpu().numpy().view(np.uint16)
 
 
 def test_efficientnet_mnist(eng, pkg, golden):
@@ -484,57 +351,25 @@ def test_efficientnet_mnist(eng, pkg, golden):
     dy, statistics and gradient sums.  A second fresh run reproduces the parameters after 5 steps bit for bit.  After EPOCHS epochs
     over the 1024 training digits the mean loss has fallen, and test accuracy on the 256 test digits, evaluated with the running
     statistics, exceeds ACC_MIN."""
-    xs, ys = mnist_device(pkg, golden["train_u8"]), torch.from_numpy(golden["train_labels"]).to(DEV)
-    xt, yt = mnist_device(pkg, golden["test_u8"]), torch.from_numpy(golden["test_labels"]).to(DEV)
-    row_bytes = 28 * 32 * 2
-    batch = lambda s, xs=xs, ys=ys: (xs.data_ptr() + s * NB * row_bytes, ys[s * NB:(s + 1) * NB])
 
-    net = EfficientNetLite(eng, pkg, init_params())
-    try:
-        for it in range(5):
-            net.forward(*batch(it))
-            net.backward()
-            eng.sync()
-            for bn, x, y, dy, dx, g in net.bn_tensors():
-                C = bn.shape[3]
-                ga, be = bn.gamma.to_host(), bn.beta.to_host()
-                mean, rstd = bn.save_mean.to_host(), bn.save_rstd.to_host()
-                xb, yb, dyb = host(x).reshape(-1, C), host(y).reshape(-1, C), host(dy).reshape(-1, C)
-                v = AR.pre32(pkg, xb, ga, be, mean, rstd)
-                assert np.array_equal(yb, AR.act_bits(pkg, v, bn.act)), (it, IDS[bn.act], C)
-                gb = AR.grad_bits(pkg, v, dyb, None, bn.act)
-                assert np.array_equal(host(g).reshape(-1, C), gb), (it, IDS[bn.act], C)
-                want = BR.dx_bits(pkg, xb, gb, ga, mean, rstd, bn.dgamma.to_host(), bn.dbeta.to_host())
-                assert np.array_equal(host(dx).reshape(-1, C), want), (it, IDS[bn.act], C)
-            net.sgd(LR_STEP)
-            eng.sync()
-        after5 = net.params()
-    finally:
-        net.close()
-
-    net = EfficientNetLite(eng, pkg, init_params())
-    try:
-        losses = []
-        for ep in range(EPOCHS):
-            for s in range(1024 // NB):
-                net.forward(*batch(s))
-                net.backward()
-                net.sgd(LR_STEP)
-                losses.append(net.loss)
-                net.loss = torch.zeros(NB, dtype=torch.float32, device=DEV)
-                if ep == 0 and s == 4:
-                    eng.sync()
-                    assert all(np.array_equal(a.view(np.uint32), b_.view(np.uint32)) for a, b_ in zip(net.params(), after5))
+    def check_step(net, it, x, labels):
+        net.forward(x, labels)
+        net.backward()
         eng.sync()
-        ep_loss = [float(torch.stack(losses[e * 8:(e + 1) * 8]).double().mean()) for e in range(EPOCHS)]
-        right = 0
-        for s in range(2):
-            net.forward(*batch(s, xt, yt), training=False)
-            eng.sync()
-            right += int((net.pred.cpu().numpy() == golden["test_labels"][s * NB:(s + 1) * NB]).sum())
-        acc = right / 256
-    finally:
-        net.close()
+        for bn, x, y, dy, dx, g in net.bn_tensors():
+            C = bn.shape[3]
+            ga, be = bn.gamma.to_host(), bn.beta.to_host()
+            mean, rstd = bn.save_mean.to_host(), bn.save_rstd.to_host()
+            xb, yb, dyb = host(x).reshape(-1, C), host(y).reshape(-1, C), host(dy).reshape(-1, C)
+            v = AR.pre32(pkg, xb, ga, be, mean, rstd)
+            assert np.array_equal(yb, AR.act_bits(pkg, v, bn.act)), (it, IDS[bn.act], C)
+            gb = AR.grad_bits(pkg, v, dyb, None, bn.act)
+            assert np.array_equal(host(g).reshape(-1, C), gb), (it, IDS[bn.act], C)
+            want = BR.dx_bits(pkg, xb, gb, ga, mean, rstd, bn.dgamma.to_host(), bn.dbeta.to_host())
+            assert np.array_equal(host(dx).reshape(-1, C), want), (it, IDS[bn.act], C)
+
+    ep_loss, acc, _ = train(eng, pkg, golden, lambda: EfficientNetLite(eng, pkg, EfficientNetLite.init_params()), EfficientNetLite.EPOCHS,
+                            check_step=check_step)
     print(f"EfficientNet-style network: mean loss by epoch {ep_loss[0]:.4f} -> {ep_loss[-1]:.4f}; test accuracy {acc:.4f} (threshold {ACC_MIN})")
     assert np.isfinite(ep_loss).all() and ep_loss[-1] < ep_loss[0]
     assert acc > ACC_MIN

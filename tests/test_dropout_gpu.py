@@ -10,7 +10,7 @@ import pytest
 import torch
 
 import dropout_ref as D
-from test_bnact_gpu import DEV, NAN_BF16, NB, EPOCHS, LR_STEP, EfficientNetLite, host, init_params, mnist_device, same_or_nan
+from example_nets import DEV, NAN_BF16, EfficientNetDropout, host, train
 
 pytestmark = pytest.mark.gpu
 
@@ -22,6 +22,13 @@ SHAPES = {  # name: (N, row_elems, row_pitch)
     "nhwc-56x56x64": (128, 56 * 56 * 64, 0), "nhwc-7x7x1280": (128, 7 * 7 * 1280, 0), "gap-C12-pitch16": (128, 12, 16),
     "gap-C1280": (128, 1280, 1280), "odd-7x7x3": (33, 147, 0), "N1-odd": (1, 1001, 0), "N1-vec": (1, 4096, 4104)}
 PS = [0.0, 0.1, 0.5, 0.9]
+
+
+def same_or_nan(got, want):
+    """bf16 bits: identical where want is a number; NaN (any payload) where want is NaN"""
+    got, want = np.asarray(got, np.uint16), np.asarray(want, np.uint16)
+    nan, gnan = (want & 0x7FFF) > 0x7F80, (got & 0x7FFF) > 0x7F80
+    return np.array_equal(gnan, nan) and np.array_equal(got[~nan], want[~nan])
 
 
 @functools.lru_cache(maxsize=None)
@@ -173,90 +180,9 @@ def test_refusals(eng, pkg):
 
 
 # ------------------------------------------------------------------------------------------------ end to end
-P_FC, P_PATH = 0.2, 0.2
-SEED_FC, SEED_PATH = 1001, 2002
 ACC_MIN = 0.85          # the float32 torch CPU replica (scripts/efficientnet_dropout_replica.py) reaches 0.8945 (DESIGN 3.22)
-
-
-class EfficientNetDropout(EfficientNetLite):
-    """test_bnact_gpu's EfficientNet-style network with both regularisers: element dropout (p = 0.2) in place on the global
-    average pool's output before the fc, and stochastic depth (p = 0.2, per image) on the residual MBConv, whose last BN runs
-    without r while the DropoutLayer adds x1.  With `trace` the layers' inputs that the in-place calls overwrite are kept."""
-
-    def __init__(self, eng, pkg, p):
-        super().__init__(eng, pkg, p)
-        self.drop_fc = pkg.DropoutLayer(eng, NB, 128, P_FC, SEED_FC, row_pitch=self.gap.row_pitch)
-        self.drop_path = pkg.DropoutLayer(eng, NB, 6 * 6 * 48, P_PATH, SEED_PATH, per_sample=True)
-        self.b2, self.db2 = (torch.full((NB, 6, 6, 48), NAN_BF16, dtype=torch.int16, device=DEV) for _ in range(2))
-        self.trace = False
-
-    def snapshot(self, t):
-        """a copy of t as the engine's stream has written it, taken before the engine's next call overwrites it (torch copies on
-        its own stream)"""
-        self.eng.sync()
-        copy = t.clone()
-        torch.cuda.synchronize()
-        return copy
-
-    def forward(self, x, labels, training=True):
-        b0, be1, bd1, bp1, be2, bd2, bp2, bh = self.bn
-        self.stem.forward(x, self.y0)
-        b0.forward(self.y0, self.z0, training=training)
-        self.pool.forward(self.z0, self.x1p)
-        self.e1.forward(self.x1p, self.ye1)
-        be1.forward(self.ye1, self.ze1, training=training)
-        self.d1.forward(self.ze1, self.yd1)
-        bd1.forward(self.yd1, self.zd1, training=training)
-        self.p1.forward(self.zd1, self.yp1)
-        bp1.forward(self.yp1, self.x1, training=training)
-        self.e2.forward(self.x1, self.ye2)
-        be2.forward(self.ye2, self.ze2, training=training)
-        self.d2.forward(self.ze2, self.yd2)
-        bd2.forward(self.yd2, self.zd2, training=training)
-        self.se.forward(self.zd2, self.se_y)
-        self.p2.forward(self.se_y, self.yp2)
-        bp2.forward(self.yp2, self.b2, training=training)                          # the branch's last BN, without r
-        self.drop_path.forward(self.b2, self.x2, r=self.x1, training=training)       # x2 = x1 + drop_path(b2)
-        self.hd.forward(self.x2, self.yh)
-        bh.forward(self.yh, self.zh, training=training)
-        self.gap.forward(self.zh, self.hp)
-        if self.trace:
-            self.hp_in = self.snapshot(self.hp)
-        self.drop_fc.forward(self.hp, self.hp, training=training)
-        self.fc.forward(self.hp, self.z)
-        self.eng.softmax_ce_bf16(self.z, labels, NB, 10, 1.0 / NB, self.dz, self.loss, self.pred)
-
-    def backward(self):
-        b0, be1, bd1, bp1, be2, bd2, bp2, bh = self.bn
-        self.fc.backward(self.z, self.dz, self.dhp)
-        if self.trace:
-            self.dhp_in = self.snapshot(self.dhp)
-        self.drop_fc.backward(self.dhp, self.dhp)
-        self.gap.backward(self.dhp, self.dzh)
-        bh.backward(self.zh, self.dzh, self.dyh, dr=self.gh)
-        self.hd.backward(self.yh, self.dyh, self.dx2)
-        self.drop_path.backward(self.dx2, self.db2)                                  # dx2 still feeds the skip path
-        bp2.backward(self.b2, self.db2, self.dyp2)
-        self.p2.backward(self.yp2, self.dyp2, self.dse_y)
-        self.se.backward(self.se_y, self.dse_y, self.dzd2)
-        bd2.backward(self.zd2, self.dzd2, self.dyd2, dr=self.gd2)
-        self.d2.backward(self.yd2, self.dyd2, self.dze2)
-        be2.backward(self.ze2, self.dze2, self.dye2, dr=self.ge2)
-        self.e2.backward(self.ye2, self.dye2, self.dx1b)
-        bp1.backward(self.x1, self.dx1b, self.dyp1, dy2=self.dx2)                   # the block's two paths meet at x1
-        self.p1.backward(self.yp1, self.dyp1, self.dzd1)
-        bd1.backward(self.zd1, self.dzd1, self.dyd1, dr=self.gd1)
-        self.d1.backward(self.yd1, self.dyd1, self.dze1)
-        be1.backward(self.ze1, self.dze1, self.dye1, dr=self.ge1)
-        self.e1.backward(self.ye1, self.dye1, self.dx1p)
-        self.pool.backward(self.dx1p, self.dz0)
-        b0.backward(self.z0, self.dz0, self.dy0, dr=self.g0)
-        self.stem.backward(self.y0, self.dy0, None)
-
-    def close(self):
-        super().close()
-        self.drop_fc.close()
-        self.drop_path.close()
+NB, EPOCHS = EfficientNetDropout.NB, EfficientNetDropout.EPOCHS
+P_FC, P_PATH, SEED_FC, SEED_PATH = EfficientNetDropout.P_FC, EfficientNetDropout.P_PATH, EfficientNetDropout.SEED_FC, EfficientNetDropout.SEED_PATH
 
 
 def check_net_dropout(pkg, net):
@@ -281,53 +207,25 @@ def test_efficientnet_dropout_mnist(eng, pkg, golden):
     A second fresh run with the same seeds reproduces the parameters after 5 steps bit for bit.  After EPOCHS epochs over the 1024
     training digits the mean loss has fallen, and test accuracy on the 256 test digits, evaluated with the running statistics and
     without dropout, exceeds ACC_MIN."""
-    xs, ys = mnist_device(pkg, golden["train_u8"]), torch.from_numpy(golden["train_labels"]).to(DEV)
-    xt, yt = mnist_device(pkg, golden["test_u8"]), torch.from_numpy(golden["test_labels"]).to(DEV)
-    row_bytes = 28 * 32 * 2
-    batch = lambda s, xs=xs, ys=ys: (xs.data_ptr() + s * NB * row_bytes, ys[s * NB:(s + 1) * NB])
+    dropped = 0
 
-    net = EfficientNetDropout(eng, pkg, init_params())
-    net.trace = True
-    try:
-        dropped = 0
-        for it in range(5):
-            net.forward(*batch(it))
-            net.backward()
-            eng.sync()
-            check_net_dropout(pkg, net)
-            dropped += int((~mask(NB, 1, P_PATH, SEED_PATH, it + 1, True)).sum())
-            net.sgd(LR_STEP)
-            eng.sync()
-        assert dropped > 0                          # some image's residual branch was dropped
-        after5 = net.params()
-    finally:
-        net.close()
-
-    net = EfficientNetDropout(eng, pkg, init_params())
-    try:
-        losses = []
-        for ep in range(EPOCHS):
-            for s in range(1024 // NB):
-                net.forward(*batch(s))
-                net.backward()
-                net.sgd(LR_STEP)
-                losses.append(net.loss)
-                net.loss = torch.zeros(NB, dtype=torch.float32, device=DEV)
-                if ep == 0 and s == 4:
-                    eng.sync()
-                    assert all(np.array_equal(a.view(np.uint32), b_.view(np.uint32)) for a, b_ in zip(net.params(), after5))
+    def check_step(net, it, x, labels):
+        nonlocal dropped
+        net.trace = True
+        net.forward(x, labels)
+        net.backward()
         eng.sync()
+        check_net_dropout(pkg, net)
+        dropped += int((~mask(NB, 1, P_PATH, SEED_PATH, it + 1, True)).sum())
+        if it == 4:
+            assert dropped > 0                      # some image's residual branch was dropped
+
+    def check_trained(net):
+        """after training and again after eval, which draws no mask"""
         assert net.drop_fc.call == net.drop_path.call == EPOCHS * 8
-        ep_loss = [float(torch.stack(losses[e * 8:(e + 1) * 8]).double().mean()) for e in range(EPOCHS)]
-        right = 0
-        for s in range(2):
-            net.forward(*batch(s, xt, yt), training=False)
-            eng.sync()
-            right += int((net.pred.cpu().numpy() == golden["test_labels"][s * NB:(s + 1) * NB]).sum())
-        assert net.drop_fc.call == EPOCHS * 8
-        acc = right / 256
-    finally:
-        net.close()
+
+    ep_loss, acc, _ = train(eng, pkg, golden, lambda: EfficientNetDropout(eng, pkg, EfficientNetDropout.init_params()), EPOCHS,
+                            check_step=check_step, check_trained=check_trained)
     print(f"EfficientNet-style network with dropout and stochastic depth: mean loss by epoch {ep_loss[0]:.4f} -> {ep_loss[-1]:.4f}; "
           f"test accuracy {acc:.4f} (threshold {ACC_MIN})")
     assert np.isfinite(ep_loss).all() and ep_loss[-1] < ep_loss[0]

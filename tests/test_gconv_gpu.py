@@ -17,11 +17,10 @@ import torch.nn.functional as F
 
 import gconv_ref as GR
 import pcnn_loader
+from example_nets import DEV, NAN_BF16, ResNeXtLite, host, train
 
 pytestmark = pytest.mark.gpu
 
-DEV = torch.device("cuda", 0)
-NAN_BF16 = 0x7FC0
 NAN_F32 = 0x7FC00000
 TAIL = 64
 U = 2.0 ** -24
@@ -360,117 +359,7 @@ def test_sgd_step_matches_layer_sgd(eng, pkg):
 
 
 # ------------------------------------------------------------------------------------------------ end to end
-NB = 128
-LR_STEP = 0.2
-EPOCHS = 40
 ACC_MIN = 0.85          # below the accuracy of the float32 torch CPU replica, scripts/resnext_replica.py (DESIGN 3.21)
-
-
-def init_params(seed=23):
-    rng = np.random.default_rng(seed)
-    u = lambda shape, fan: rng.uniform(-1, 1, shape).astype(np.float32) / np.float32(np.sqrt(fan))
-    return dict(f0=u((48, 5, 5, 1), 25), e1=u((64, 1, 1, 48), 48), g1=u((64, 3, 3, 8), 72), p1=u((48, 1, 1, 64), 64),
-                e2=u((96, 1, 1, 48), 48), g2=u((96, 3, 3, 4), 36), p2=u((64, 1, 1, 96), 96), w8=u((10, 1, 1, 64), 64), b8=u(10, 64))
-
-
-class ResNeXtLite:
-    """stem conv 48@5x5 -> BN+ReLU (x0) -> [1x1 48->64, BN+ReLU, grouped 3x3/1 pad 1 G = 8 (Cg = 8), BN+ReLU, 1x1 64->48,
-    BN + x0 with ReLU] (x1) -> [1x1 48->96, BN+ReLU, grouped 3x3/2 pad 1 G = 24 (Cg = 4, the narrow path), BN+ReLU, 1x1 96->64, BN]
-    -> GAP -> fc 64->10 -> softmax CE (1/B).  The convs have no bias.  Every 1x1 conv reads >= 48 channels, so each is a
-    wide-family layer, which has a 1x1 input gradient."""
-
-    def __init__(self, eng, pkg, p):
-        self.eng = eng
-        relu, none = pkg.ACT_RELU, pkg.ACT_NONE
-        B = NB
-        conv = lambda H, C, K, R, f: pkg.ConvLayer(eng, B, H, H, C, K, R, R, p[f], None, act=none)
-        self.stem = conv(28, 1, 48, 5, "f0")
-        self.e1, self.p1 = conv(24, 48, 64, 1, "e1"), conv(24, 64, 48, 1, "p1")
-        self.e2, self.p2 = conv(24, 48, 96, 1, "e2"), conv(12, 96, 64, 1, "p2")
-        assert self.stem.family == "narrow" and all(c.family == "wide" for c in (self.e1, self.p1, self.e2, self.p2))
-        self.g1 = pkg.GroupedConvLayer(eng, B, 24, 24, 64, 64, 8, 3, 3, p["g1"], None, act=none, stride=1, padding=(1, 1))
-        self.g2 = pkg.GroupedConvLayer(eng, B, 24, 24, 96, 96, 24, 3, 3, p["g2"], None, act=none, stride=2, padding=(1, 1))
-        assert self.g1.out_shape == (B, 24, 24, 64) and self.g2.out_shape == (B, 12, 12, 96)
-        assert self.g1.info["vec"] == 8 and self.g2.info["vec"] == 4
-        BN = lambda H, C, act: pkg.BatchNormLayer(eng, B, H, H, C, act=act)
-        self.bn = [BN(24, 48, relu), BN(24, 64, relu), BN(24, 64, relu), BN(24, 48, relu), BN(24, 96, relu), BN(12, 96, relu),
-                   BN(12, 64, none)]
-        self.gap = pkg.GlobalAvgPoolLayer(eng, B, 12, 12, 64)
-        self.fc = pkg.LinearLayer(eng, B, 1, 1, 64, 10, p["w8"], p["b8"], act=none, row_pitch=self.gap.row_pitch)
-        buf = lambda *shape: torch.full(shape, NAN_BF16, dtype=torch.int16, device=DEV)
-        self.y0, self.x0, self.dx0, self.dy0, self.dres, self.yp1, self.x1, self.dx1, self.dyp1 = (buf(B, 24, 24, 48) for _ in range(9))
-        self.ye1, self.ze1, self.yg1, self.zg1, self.dzg1, self.dyg1, self.dze1, self.dye1 = (buf(B, 24, 24, 64) for _ in range(8))
-        self.ye2, self.ze2, self.dze2, self.dye2 = (buf(B, 24, 24, 96) for _ in range(4))
-        self.yg2, self.zg2, self.dzg2, self.dyg2 = (buf(B, 12, 12, 96) for _ in range(4))
-        self.yp2, self.out, self.dout, self.dyp2 = (buf(B, 12, 12, 64) for _ in range(4))
-        self.h, self.dh = buf(B, self.gap.row_pitch), buf(B, self.gap.row_pitch)
-        self.z, self.dz = buf(B, 10), buf(B, 10)
-        self.loss = torch.zeros(B, dtype=torch.float32, device=DEV)
-        self.pred = torch.zeros(B, dtype=torch.int32, device=DEV)
-
-    def forward(self, x, labels, training=True):
-        b0, be1, bg1, bp1, be2, bg2, bp2 = self.bn
-        self.stem.forward(x, self.y0)
-        b0.forward(self.y0, self.x0, training=training)
-        self.e1.forward(self.x0, self.ye1)
-        be1.forward(self.ye1, self.ze1, training=training)
-        self.g1.forward(self.ze1, self.yg1)
-        bg1.forward(self.yg1, self.zg1, training=training)
-        self.p1.forward(self.zg1, self.yp1)
-        bp1.forward(self.yp1, self.x1, r=self.x0, training=training)
-        self.e2.forward(self.x1, self.ye2)
-        be2.forward(self.ye2, self.ze2, training=training)
-        self.g2.forward(self.ze2, self.yg2)
-        bg2.forward(self.yg2, self.zg2, training=training)
-        self.p2.forward(self.zg2, self.yp2)
-        bp2.forward(self.yp2, self.out, training=training)
-        self.gap.forward(self.out, self.h)
-        self.fc.forward(self.h, self.z)
-        self.eng.softmax_ce_bf16(self.z, labels, NB, 10, 1.0 / NB, self.dz, self.loss, self.pred)
-
-    def backward(self):
-        b0, be1, bg1, bp1, be2, bg2, bp2 = self.bn
-        self.fc.backward(self.z, self.dz, self.dh)
-        self.gap.backward(self.dh, self.dout)
-        bp2.backward(self.out, self.dout, self.dyp2)
-        self.p2.backward(self.yp2, self.dyp2, self.dzg2)
-        bg2.backward(self.zg2, self.dzg2, self.dyg2)
-        self.g2.backward(self.yg2, self.dyg2, self.dze2)
-        be2.backward(self.ze2, self.dze2, self.dye2)
-        self.e2.backward(self.ye2, self.dye2, self.dx1)
-        bp1.backward(self.x1, self.dx1, self.dyp1, dr=self.dres)
-        self.p1.backward(self.yp1, self.dyp1, self.dzg1)
-        bg1.backward(self.zg1, self.dzg1, self.dyg1)
-        self.g1.backward(self.yg1, self.dyg1, self.dze1)
-        be1.backward(self.ze1, self.dze1, self.dye1)
-        self.e1.backward(self.ye1, self.dye1, self.dx0)
-        b0.backward(self.x0, self.dx0, self.dy0, dy2=self.dres)                    # the block's two paths meet at x0
-        self.stem.backward(self.y0, self.dy0, None)
-
-    def layers(self):
-        return (self.stem, self.e1, self.g1, self.p1, self.e2, self.g2, self.p2, self.fc, *self.bn)
-
-    def sgd(self, lr):
-        for layer in self.layers():
-            layer.sgd(lr)
-
-    def params(self):
-        return [a for layer in self.layers() for a in layer.params() if a is not None]
-
-    def close(self):
-        for layer in (*self.layers(), self.gap):
-            layer.close()
-
-
-def mnist_device(pkg, u8):
-    n = u8.shape[0]
-    xl = np.zeros((n * 28, 32), np.uint16)
-    xl[:, :28] = pkg.f32_to_bf16_bits(u8.reshape(n, 28, 28).astype(np.float32) / 255.0).reshape(n * 28, 28)
-    return torch.from_numpy(xl.view(np.int16)).to(DEV)
-
-
-def host(t):
-    return t.cpu().numpy().view(np.uint16)
 
 
 def test_resnext_mnist(eng, pkg, golden):
@@ -478,14 +367,9 @@ def test_resnext_mnist(eng, pkg, golden):
     and dw lies within its bound.  A fresh run reproduces the parameters after 5 steps bit for bit.  After EPOCHS epochs over the
     1024 training digits the mean loss has fallen, and test accuracy on the 256 test digits, evaluated with the running statistics,
     exceeds ACC_MIN."""
-    xs, ys = mnist_device(pkg, golden["train_u8"]), torch.from_numpy(golden["train_labels"]).to(DEV)
-    xt, yt = mnist_device(pkg, golden["test_u8"]), torch.from_numpy(golden["test_labels"]).to(DEV)
-    row_bytes = 28 * 32 * 2
-    batch = lambda s, xs=xs, ys=ys: (xs.data_ptr() + s * NB * row_bytes, ys[s * NB:(s + 1) * NB])
 
-    net = ResNeXtLite(eng, pkg, init_params())
-    for it in range(5):
-        net.forward(*batch(it))
+    def check_step(net, it, x, labels):
+        net.forward(x, labels)
         net.backward()
         eng.sync()
         for layer, x, y, dy, dx in ((net.g1, net.ze1, net.yg1, net.dyg1, net.dze1), (net.g2, net.ze2, net.yg2, net.dyg2, net.dze2)):
@@ -496,32 +380,9 @@ def test_resnext_mnist(eng, pkg, golden):
             assert np.array_equal(host(dx).reshape(N, H, W, Cc), bf(GR.dgrad(dyv, wq, G, H, W, layer.stride, 1, 1)[0])), it
             err = np.abs(layer.dw.to_host().astype(np.float64) - GR.wgrad_f64(xv, dyv, G, R, S, layer.stride, 1, 1))
             assert np.all(err <= 2 * layer.info["n_acc"] * U * GR.wgrad_abs_f64(xv, dyv, G, R, S, layer.stride, 1, 1)), it
-        net.sgd(LR_STEP)
-        eng.sync()
-    after5 = net.params()
-    net.close()
 
-    net = ResNeXtLite(eng, pkg, init_params())
-    losses = []
-    for ep in range(EPOCHS):
-        for s in range(1024 // NB):
-            net.forward(*batch(s))
-            net.backward()
-            net.sgd(LR_STEP)
-            losses.append(net.loss)
-            net.loss = torch.zeros(NB, dtype=torch.float32, device=DEV)
-            if ep == 0 and s == 4:
-                eng.sync()
-                assert all(np.array_equal(a.view(np.uint32), b_.view(np.uint32)) for a, b_ in zip(net.params(), after5))
-    eng.sync()
-    ep_loss = [float(torch.stack(losses[e * 8:(e + 1) * 8]).double().mean()) for e in range(EPOCHS)]
-    right = 0
-    for s in range(2):
-        net.forward(*batch(s, xt, yt), training=False)
-        eng.sync()
-        right += int((net.pred.cpu().numpy() == golden["test_labels"][s * NB:(s + 1) * NB]).sum())
-    acc = right / 256
-    net.close()
+    ep_loss, acc, _ = train(eng, pkg, golden, lambda: ResNeXtLite(eng, pkg, ResNeXtLite.init_params()), ResNeXtLite.EPOCHS,
+                            check_step=check_step)
     print(f"ResNeXt-style network: mean loss by epoch {ep_loss[0]:.4f} -> {ep_loss[-1]:.4f}; test accuracy {acc:.4f} (threshold {ACC_MIN})")
     assert np.isfinite(ep_loss).all() and ep_loss[-1] < ep_loss[0]
     assert acc > ACC_MIN

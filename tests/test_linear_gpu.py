@@ -8,11 +8,9 @@ import torch
 
 import linear_ref as LR
 import maxpool_ref as MR
+from example_nets import DEV, NAN_BF16, Net, host, nan_buf, train
 
 pytestmark = pytest.mark.gpu
-
-NAN_BF16 = 0x7FC0
-DEV = torch.device("cuda", 0)
 
 CASES = [  # id, N, P, Q, C, O, row_pitch (0 = Q*C rounded up to 8), image_rows (0 = P)
     ("n100-qc130-pitched-fwdsplit", 100, 6, 5, 26, 10, 144, 8),
@@ -33,14 +31,6 @@ def layout(case):
     return (pitch or (Q * C + 7) // 8 * 8), (rows or P)
 
 
-def nan_buf(shape):
-    return torch.full(shape, NAN_BF16, dtype=torch.int16, device=DEV)
-
-
-def host(a):
-    return a.cpu().numpy().view(np.uint16)
-
-
 def dev_bits(bits):
     return torch.from_numpy(np.ascontiguousarray(bits).view(np.int16)).to(DEV)
 
@@ -56,7 +46,7 @@ def put_x(pkg, x, pitch, rows):
 def run_all(eng, plan, xd, dyd, case):
     _, N, P, Q, C, O, _, _ = case
     pitch, rows = layout(case)
-    y, dx = nan_buf((N, O)), nan_buf((N, rows, pitch))
+    y, dx = nan_buf(N, O), nan_buf(N, rows, pitch)
     dw = eng.array((O, P, Q, C))
     plan.fwd(xd, y)
     eng.linear_wgrad(plan, xd, dyd, dw)
@@ -123,7 +113,7 @@ def test_layer_random(eng, pkg, case):
     layer = pkg.LinearLayer(eng, N, P, Q, C, O, w, b, act=act, row_pitch=pitch, image_rows=rows)
     pitch, rows = layer.row_pitch, layer.image_rows or P
     xd = put_x(pkg, x, pitch, rows)
-    y, dyd, dx = nan_buf((N, O)), dev_bits(pkg.f32_to_bf16_bits(dy)), nan_buf((N, rows, pitch))
+    y, dyd, dx = nan_buf(N, O), dev_bits(pkg.f32_to_bf16_bits(dy)), nan_buf(N, rows, pitch)
     layer.forward(xd, y)
     eng.sync()
     yh = host(y)
@@ -173,8 +163,8 @@ def test_refresh_matches_fresh_plan_and_is_stream_ordered(eng, pkg):
     fresh2 = pkg.LinearPlan(eng, N, P, Q, C, O, w2, b2, act=1)
     plan = pkg.LinearPlan(eng, N, P, Q, C, O, w1, b1, act=1)
     w2d, b2d = eng.to_device(w2), eng.to_device(b2)
-    outs = [nan_buf((N, O)) for _ in range(4)]
-    dxs = [nan_buf((N, P, Q * C)) for _ in range(2)]
+    outs = [nan_buf(N, O) for _ in range(4)]
+    dxs = [nan_buf(N, P, Q * C) for _ in range(2)]
     fresh1.fwd(xd, outs[0])
     fresh2.fwd(xd, outs[1])
     eng.linear_dgrad(fresh2, dyd, dxs[0])
@@ -201,7 +191,7 @@ def test_refusals(eng, pkg):
     with pytest.raises(pkg.PcnnError, match="hidden width"):
         pkg.LinearPlan(eng, N, 1, 1, 10, O, np.zeros((O, 10), np.float32), row_pitch=10)
     plan = pkg.LinearPlan(eng, N, P, Q, C, O, w)                    # no bias
-    x, dy, dx = nan_buf((N, P, Q * C)), nan_buf((N, O)), nan_buf((N, P, Q * C))
+    x, dy, dx = nan_buf(N, P, Q * C), nan_buf(N, O), nan_buf(N, P, Q * C)
     dw = eng.array((O, P, Q, C))
     with pytest.raises(pkg.PcnnError, match="only a plan with a bias"):
         plan.set_params(None, eng.array(O))
@@ -218,7 +208,7 @@ def test_refusals(eng, pkg):
         eng.linear_dgrad(conv, dy, dx)
     lab = torch.zeros(N, dtype=torch.uint8, device=DEV)
     with pytest.raises(pkg.PcnnError, match="1 <= O <= 256"):
-        eng.softmax_ce_bf16(dy, lab, N, 257, 1.0, nan_buf((N, 257)))
+        eng.softmax_ce_bf16(dy, lab, N, 257, 1.0, nan_buf(N, 257))
     with pytest.raises(pkg.PcnnError, match="overlaps logits"):
         eng.softmax_ce_bf16(dy, lab, N, O, 1.0, dy.data_ptr() + 16)
     eng.sync()
@@ -242,7 +232,7 @@ def test_softmax_ce_bf16(eng, pkg, O):
     labels[[3, 17]] = [O, 255] if O < 255 else [255, 255]
     scale = 1.0 / N
     zd, lab = dev_bits(zb), torch.from_numpy(labels).to(DEV)
-    d = nan_buf((N, O))
+    d = nan_buf(N, O)
     loss = torch.full((N,), float("nan"), dtype=torch.float32, device=DEV)
     pred = torch.full((N,), -7, dtype=torch.int32, device=DEV)
     eng.softmax_ce_bf16(zd, lab, N, O, scale, d, loss, pred)
@@ -269,75 +259,7 @@ def test_softmax_ce_bf16(eng, pkg, O):
 
 
 # ============================================================ end to end: a LeNet-style classifier on MNIST digits
-B = 128
-LR_STEP = 0.3
-EPOCHS = 40
 ACC_MIN = 0.70          # the float32 torch replica of this network, seed and step reaches 0.836 (see DESIGN 3.13)
-
-
-def init_params(seed=5):
-    rng = np.random.default_rng(seed)
-    u = lambda shape, fan: rng.uniform(-1, 1, shape).astype(np.float32) / np.float32(np.sqrt(fan))
-    return dict(f1=u((8, 5, 5, 1), 25), b1=u(8, 25), f2=u((16, 3, 3, 8), 72), b2=u(16, 72), w3=u((128, 6, 6, 16), 576),
-                b3=u(128, 576), w4=u((10, 1, 1, 128), 128), b4=u(10, 128))
-
-
-class Net:
-    """conv 8@5x5 sigmoid -> pool 2 -> conv 16@3x3 pad 1 -> pool 2 -> fc 576->128 sigmoid -> fc 128->10 -> softmax CE (1/B)"""
-
-    def __init__(self, eng, pkg, p):
-        self.eng = eng
-        self.c1 = pkg.ConvLayer(eng, B, 28, 28, 1, 8, 5, 5, p["f1"], p["b1"], act=1)
-        self.c2 = pkg.ConvLayer(eng, B, 12, 12, 8, 16, 3, 3, p["f2"], p["b2"], act=0, padding=(1, 1))
-        self.fc1 = pkg.LinearLayer(eng, B, 6, 6, 16, 128, p["w3"], p["b3"], act=1)
-        self.fc2 = pkg.LinearLayer(eng, B, 1, 1, 128, 10, p["w4"], p["b4"], act=0, row_pitch=128)
-        self.p1 = pkg.MaxPoolLayer(eng, B, 24, 24, 8, 2, row_pitch=self.c2.row_pitch, image_rows=self.c2.image_rows)
-        self.p2 = pkg.MaxPoolLayer(eng, B, 12, 12, 16, 2, row_pitch=self.fc1.row_pitch, image_rows=self.fc1.image_rows)
-        self.y1, self.dy1 = nan_buf((B, 24, 24, 8)), nan_buf((B, 24, 24, 8))
-        self.x2, self.dx2 = nan_buf((B, 12, self.c2.row_pitch)), nan_buf((B, 12, self.c2.row_pitch))
-        self.y2, self.dy2 = nan_buf((B, 12, 12, 16)), nan_buf((B, 12, 12, 16))
-        self.x3, self.dx3 = nan_buf((B, 6, 96)), nan_buf((B, 6, 96))
-        self.y3, self.dy3 = nan_buf((B, 128)), nan_buf((B, 128))
-        self.z, self.dz = nan_buf((B, 10)), nan_buf((B, 10))
-        self.loss = torch.zeros(B, dtype=torch.float32, device=DEV)
-        self.pred = torch.zeros(B, dtype=torch.int32, device=DEV)
-
-    def forward(self, x, labels):
-        self.c1.forward(x, self.y1)
-        self.p1.forward(self.y1, self.x2)
-        self.c2.forward(self.x2, self.y2)
-        self.p2.forward(self.y2, self.x3)
-        self.fc1.forward(self.x3, self.y3)
-        self.fc2.forward(self.y3, self.z)
-        self.eng.softmax_ce_bf16(self.z, labels, B, 10, 1.0 / B, self.dz, self.loss, self.pred)
-
-    def backward(self, hook=lambda name: None):
-        self.fc2.backward(self.z, self.dz, self.dy3)
-        hook("fc2")
-        self.fc1.backward(self.y3, self.dy3, self.dx3)
-        hook("fc1")
-        self.p2.backward(self.dx3, self.dy2)
-        self.c2.backward(self.y2, self.dy2, self.dx2)
-        self.p1.backward(self.dx2, self.dy1)
-        self.c1.backward(self.y1, self.dy1, None)
-
-    def sgd(self, lr):
-        for layer in (self.c1, self.c2, self.fc1, self.fc2):
-            layer.sgd(lr)
-
-    def params(self):
-        return [a for layer in (self.c1, self.c2, self.fc1, self.fc2) for a in layer.params()]
-
-    def close(self):
-        for layer in (self.c1, self.c2, self.fc1, self.fc2, self.p1, self.p2):
-            layer.close()
-
-
-def mnist_device(pkg, u8):
-    n = u8.shape[0]
-    xl = np.zeros((n * 28, 32), np.uint16)
-    xl[:, :28] = pkg.f32_to_bf16_bits(u8.reshape(n, 28, 28).astype(np.float32) / 255.0).reshape(n * 28, 28)
-    return dev_bits(xl)
 
 
 def test_classifier_mnist(eng, pkg, golden):
@@ -346,17 +268,13 @@ def test_classifier_mnist(eng, pkg, golden):
     A second fresh run reproduces the parameters after 5 steps bit for bit.  After EPOCHS epochs over the 1024 training digits
     the mean loss has fallen and test accuracy on the 256 test digits exceeds ACC_MIN."""
     f32 = pkg.bf16_bits_to_f32
-    xs, ys = mnist_device(pkg, golden["train_u8"]), torch.from_numpy(golden["train_labels"]).to(DEV)
-    xt, yt = mnist_device(pkg, golden["test_u8"]), torch.from_numpy(golden["test_labels"]).to(DEV)
-    row_bytes = 28 * 32 * 2
-    batch = lambda s: (xs.data_ptr() + s * B * row_bytes, ys[s * B:(s + 1) * B])
+    B = Net.NB
 
     def bound_ok(got, ref, absref, n):
         return np.all(np.abs(got - ref) <= 2 * n * 2.0 ** -24 * absref + 1e-30)
 
-    net = Net(eng, pkg, init_params())
-    for it in range(5):
-        net.forward(*batch(it))
+    def check_step(net, it, x, labels):
+        net.forward(x, labels)
         eng.sync()
         h = {k: host(getattr(net, k)) for k in ("y1", "x2", "y2", "x3", "y3", "z", "dz")}
         h["am1"], h["am2"] = net.p1.argmax.to_host(), net.p2.argmax.to_host()
@@ -391,32 +309,8 @@ def test_classifier_mnist(eng, pkg, golden):
         ref = LR.dgrad_f64(d3, w3).reshape(B, 6, 96)
         got = f32(h["dx3"]).astype(np.float64)
         assert np.all(np.abs(got - ref) <= 2 * 128 * 2.0 ** -24 * LR.dgrad_f64(np.abs(d3), np.abs(w3)).reshape(B, 6, 96) + 2.0 ** -8 * np.abs(ref)), it
-        net.sgd(LR_STEP)
-        eng.sync()
-    after5 = net.params()
-    net.close()
 
-    net = Net(eng, pkg, init_params())
-    losses = []
-    for ep in range(EPOCHS):
-        for s in range(1024 // B):
-            net.forward(*batch(s))
-            net.backward()
-            net.sgd(LR_STEP)
-            losses.append(net.loss)
-            net.loss = torch.zeros(B, dtype=torch.float32, device=DEV)
-            if ep == 0 and s == 4:
-                eng.sync()
-                assert all(np.array_equal(a.view(np.uint32), b_.view(np.uint32)) for a, b_ in zip(net.params(), after5))
-    eng.sync()
-    ep_loss = [float(torch.stack(losses[e * 8:(e + 1) * 8]).double().mean()) for e in range(EPOCHS)]
-    right = 0
-    for s in range(2):
-        net.forward(xt.data_ptr() + s * B * row_bytes, yt[s * B:(s + 1) * B])
-        eng.sync()
-        right += int((net.pred.cpu().numpy() == golden["test_labels"][s * B:(s + 1) * B]).sum())
-    acc = right / 256
-    net.close()
+    ep_loss, acc, _ = train(eng, pkg, golden, lambda: Net(eng, pkg, Net.init_params()), Net.EPOCHS, check_step=check_step)
     print(f"mean loss by epoch: {ep_loss[0]:.4f} -> {ep_loss[-1]:.4f}; test accuracy {acc:.4f} (threshold {ACC_MIN})")
     assert ep_loss[-1] < ep_loss[0]
     assert acc > ACC_MIN

@@ -1,15 +1,14 @@
 """Every layer of the five device-trained example networks, on the operands the device actually handed it, across training steps
 and in eval (tests/network_tape.py records the calls and holds the checkers).
 
-The networks are the test modules' own classes, run unchanged: the LeNet-style Net (test_linear_gpu.py), ReluNet
-(test_relu_gpu.py), the BN ResNet (test_batchnorm_gpu.py), the GAP ResNet (test_avgpool_nhwc_gpu.py) and MobileNetLite
-(test_dwconv_gpu.py).  Schedule, on the golden MNIST digits:
+The networks are the classes of example_nets.py that the end-to-end tests train, run unchanged: the LeNet-style Net, ReluNet,
+the BN ResNet, the GAP ResNet and MobileNetLite.  Schedule, on the golden MNIST digits:
 - training steps 0 to 3, each followed by the network's own sgd: every checker at steps 0 and 3, the bit-exact ones and the
   batch-norm statistics at steps 1 and 2;
 - after the four steps, each batch norm's running mean against running_update chained over the recorded save_mean of every step,
   bit for bit, and its running variance chained the same way, within the bound of test_batchnorm_gpu.test_forward against
   float64 and within fp32 rounding against the device's own batch variance (read back from save_rstd);
-- eval (training=False where the class has it) over every golden test digit, every checker on its own tape;
+- eval (training=False) over every golden test digit, every checker on its own tape;
 - a fresh run without the tape gives bit-identical masters and batch-norm state after the same four steps.
 Every layer object must appear on the tape in both directions in training and in the forward in eval, and every ReLU output must
 be 5-95 % positive, so no check passes for a trivial reason.  The worst ratio of each check to its bound is printed per network
@@ -18,7 +17,6 @@ and step, with the count of one-ulp softmax cases.
 The tape checks each call against the arguments it was given.  A network class that passes the wrong buffer, or none, at a join
 (a dr or dy2 left out) or between layers is outside what it can see: that needs an end-to-end replica of the whole network, which
 this file does not have."""
-import importlib
 import time
 
 import numpy as np
@@ -27,29 +25,14 @@ import torch
 
 import batchnorm_ref as BR
 import network_tape as NT
+from example_nets import DEV, MobileNetLite, Net, ReluNet, ResNet, ResNetGAP, mnist_device
 
 pytestmark = pytest.mark.gpu
 
-DEV = torch.device("cuda", 0)
 U = 2.0 ** -24
-NETS = {"Net": "test_linear_gpu", "ReluNet": "test_relu_gpu", "ResNet": "test_batchnorm_gpu", "ResNetGAP": "test_avgpool_nhwc_gpu",
-        "MobileNetLite": "test_dwconv_gpu"}
+NETS = {cls.__name__: cls for cls in (Net, ReluNet, ResNet, ResNetGAP, MobileNetLite)}
 STEPS = 4
 FULL = (0, STEPS - 1)
-
-
-def network(name):
-    """(module, class, batch size) of a network"""
-    mod = importlib.import_module(NETS[name])
-    return mod, getattr(mod, name), getattr(mod, "NB", None) or mod.B
-
-
-def run_forward(net, x, labels, training):
-    if "training" in net.forward.__code__.co_varnames:
-        net.forward(x, labels, training=training)
-    else:
-        assert training or not any(type(v).__name__ == "BatchNormLayer" for _, v in NT.layers_of(net))
-        net.forward(x, labels)
 
 
 def state(net):
@@ -92,7 +75,7 @@ def check_coverage(net, calls, training):
             assert tr == training, (n, tr)
 
 
-def tape_run(eng, pkg, golden, name, mod, net, NB, batch, train, test, n_test):
+def tape_run(eng, pkg, golden, name, net, NB, batch, train, test, n_test):
     """the taped schedule on `net`: STEPS training steps, the running-statistics chains, eval over the n_test test digits;
     returns the masters and batch-norm state after the training steps"""
     xs, ys = train
@@ -115,11 +98,11 @@ def tape_run(eng, pkg, golden, name, mod, net, NB, batch, train, test, n_test):
                 keep_stats(e)
                 s.add(e, r)
             tape.sink = sink
-            run_forward(net, x, labels, True)
+            net.forward(x, labels, training=True)
             net.backward()
             check_coverage(net, s.calls, True)
             print(f"{name} step {step} ({'every check' if step in FULL else 'bit-exact checks'}): {s.line()}")
-            net.sgd(mod.LR_STEP)
+            net.sgd(net.LR_STEP)
             eng.sync()
         trained = state(net)
 
@@ -159,7 +142,7 @@ def tape_run(eng, pkg, golden, name, mod, net, NB, batch, train, test, n_test):
                 sb.add(e, r)
                 s.add(e, r)
             tape.sink = sink
-            run_forward(net, x, labels, False)
+            net.forward(x, labels, training=False)
             check_coverage(net, sb.calls, False)
             right += int((net.pred.cpu().numpy() == golden["test_labels"][b * NB:(b + 1) * NB]).sum())
         print(f"{name} eval (accuracy {right / n_test:.4f} after {STEPS} steps): {s.line()}")
@@ -170,9 +153,10 @@ def tape_run(eng, pkg, golden, name, mod, net, NB, batch, train, test, n_test):
 @pytest.mark.parametrize("name", list(NETS))
 def test_network_tape(eng, pkg, golden, name):
     t0 = time.time()
-    mod, cls, NB = network(name)
-    xs, ys = mod.mnist_device(pkg, golden["train_u8"]), torch.from_numpy(golden["train_labels"]).to(DEV)
-    xt, yt = mod.mnist_device(pkg, golden["test_u8"]), torch.from_numpy(golden["test_labels"]).to(DEV)
+    cls = NETS[name]
+    NB = cls.NB
+    xs, ys = mnist_device(pkg, golden["train_u8"]), torch.from_numpy(golden["train_labels"]).to(DEV)
+    xt, yt = mnist_device(pkg, golden["test_u8"]), torch.from_numpy(golden["test_labels"]).to(DEV)
 
     def batch(s, xs, ys):
         rows = xs[s * NB * 28:(s + 1) * NB * 28]
@@ -180,19 +164,19 @@ def test_network_tape(eng, pkg, golden, name):
 
     n_test = len(golden["test_labels"])
     assert n_test % NB == 0, (n_test, NB)
-    net = cls(eng, pkg, mod.init_params())
+    net = cls(eng, pkg, cls.init_params())
     try:
-        trained = tape_run(eng, pkg, golden, name, mod, net, NB, batch, (xs, ys), (xt, yt), n_test)
+        trained = tape_run(eng, pkg, golden, name, net, NB, batch, (xs, ys), (xt, yt), n_test)
     finally:
         net.close()
 
-    fresh = cls(eng, pkg, mod.init_params())              # the tape is harmless: the same steps without it
+    fresh = cls(eng, pkg, cls.init_params())              # the tape is harmless: the same steps without it
     try:
         for step in range(STEPS):
             x, labels, _ = batch(step, xs, ys)
-            run_forward(fresh, x, labels, True)
+            fresh.forward(x, labels, training=True)
             fresh.backward()
-            fresh.sgd(mod.LR_STEP)
+            fresh.sgd(cls.LR_STEP)
         eng.sync()
         again = state(fresh)
     finally:

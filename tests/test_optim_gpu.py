@@ -8,11 +8,10 @@ import pytest
 import torch
 
 import optim_ref as R
-from test_avgpool_nhwc_gpu import NB, ResNetGAP, host, init_params, mnist_device
+from example_nets import DEV, ResNetGAP, Slices, host, same_bits, train
 
 pytestmark = pytest.mark.gpu
 
-DEV = torch.device("cuda", 0)
 
 
 def same(got, want):
@@ -265,20 +264,16 @@ def test_plan_refresh(eng, pkg, kind):
 
 
 # ------------------------------------------------------------------------------------------------ the GAP ResNet
-def batch(xs, ys, s):
-    return xs.data_ptr() + s * NB * 28 * 32 * 2, ys[s * NB:(s + 1) * NB]
-
-
 def test_momentum0_matches_layer_sgd(eng, pkg, golden):
     """SGD with momentum 0 and no decay gives the bits of every layer's sgd(lr): params, running statistics and logits"""
-    xs, ys = mnist_device(pkg, golden["train_u8"]), torch.from_numpy(golden["train_labels"]).to(DEV)
-    a, b = ResNetGAP(eng, pkg, init_params()), ResNetGAP(eng, pkg, init_params())
+    slices = Slices(pkg, golden["train_u8"], golden["train_labels"], ResNetGAP.NB)
+    a, b = ResNetGAP(eng, pkg, ResNetGAP.init_params()), ResNetGAP(eng, pkg, ResNetGAP.init_params())
     torch.cuda.synchronize()
     opt = pkg.SGD(eng, b.layers())
     launches = []
     for it in range(5):
         for net in (a, b):
-            net.forward(*batch(xs, ys, it))
+            net.forward(*slices.batch(it))
             net.backward()
         a.sgd(0.2)
         n0 = eng.launch_count()
@@ -286,7 +281,7 @@ def test_momentum0_matches_layer_sgd(eng, pkg, golden):
         launches.append(eng.launch_count() - n0)
         eng.sync()
         assert np.array_equal(host(a.z), host(b.z)), it
-        assert all(np.array_equal(x.view(np.uint32), y.view(np.uint32)) for x, y in zip(a.params(), b.params())), it
+        assert same_bits(a.params(), b.params()), it
     assert launches == [2] * 5                         # the update and c1's Toeplitz gather
     opt.close()
     a.close()
@@ -305,64 +300,47 @@ def test_resnet_gap_trains(eng, pkg, golden, kind):
     """In each of the first 5 steps the masters after the step are bit-exact against the replay on the device's own gradients; a fresh
     run reproduces them.  After EPOCHS epochs the test accuracy with the running statistics exceeds the threshold."""
     kw, lr, acc_min = E2E[kind]
-    xs, ys = mnist_device(pkg, golden["train_u8"]), torch.from_numpy(golden["train_labels"]).to(DEV)
-    xt, yt = mnist_device(pkg, golden["test_u8"]), torch.from_numpy(golden["test_labels"]).to(DEV)
     Opt = pkg.SGD if kind == "sgd" else pkg.AdamW
 
-    def first5(check):
-        net = ResNetGAP(eng, pkg, init_params())
-        torch.cuda.synchronize()
-        opt = Opt(eng, net.layers(), **kw)
-        tab = [t for layer in net.layers() for t in layer.optim_tensors()]
-        state = None
-        for it in range(5):
-            net.forward(*batch(xs, ys, it))
-            net.backward()
-            eng.sync()
-            if check:
-                ps = [p.to_host().ravel() for p, *_ in tab]
-                gs = [g.to_host().ravel() for _, g, *_ in tab]
-                state = opt.state()
-            opt.step(lr)
-            eng.sync()
-            if check:
-                wd = kw["weight_decay"]
-                for i, (p, g) in enumerate(zip(ps, gs)):
-                    if kind == "sgd":
-                        want, _ = R.sgd32(p, g, state[i][0], lr, it + 1, kw["momentum"], 0.0, False, wd)
-                    else:
-                        want, _, _ = R.adamw32(p, g, state[i][0], state[i][1], lr, it + 1, *kw["betas"], kw["eps"], wd)
-                    assert same(tab[i][0].to_host().ravel(), want), (kind, it, i)
-        out = net.params()
-        opt.close()
-        net.close()
-        return out
+    class Optimized(ResNetGAP):
+        """the GAP ResNet with its own fused optimizer over every layer"""
 
-    after5 = first5(True)
-    assert all(np.array_equal(a.view(np.uint32), b.view(np.uint32)) for a, b in zip(after5, first5(False)))
+        def __init__(self):
+            super().__init__(eng, pkg, ResNetGAP.init_params())
+            torch.cuda.synchronize()
+            self.opt = Opt(eng, self.layers(), **kw)
 
-    net = ResNetGAP(eng, pkg, init_params())
-    torch.cuda.synchronize()
-    opt = Opt(eng, net.layers(), **kw)
-    losses = []
-    for ep in range(EPOCHS):
-        for s in range(1024 // NB):
-            net.forward(*batch(xs, ys, s))
-            net.backward()
-            opt.step(lr)
-            losses.append(net.loss)
-            net.loss = torch.zeros(NB, dtype=torch.float32, device=DEV)
-    eng.sync()
-    ep_loss = [float(torch.stack(losses[e * 8:(e + 1) * 8]).double().mean()) for e in range(EPOCHS)]
-    right = 0
-    for s in range(2):
-        net.forward(*batch(xt, yt, s), training=False)
+        def close(self):
+            self.opt.close()
+            super().close()
+
+    before = {}                                         # the step's operands, from check_step to update
+
+    def check_step(net, it, x, labels):
+        net.forward(x, labels)
+        net.backward()
         eng.sync()
-        right += int((net.pred.cpu().numpy() == golden["test_labels"][s * NB:(s + 1) * NB]).sum())
-    acc = right / 256
-    assert opt.steps == EPOCHS * 8
-    opt.close()
-    net.close()
+        tab = [t for layer in net.layers() for t in layer.optim_tensors()]
+        before.update(it=it, tab=tab, ps=[p.to_host().ravel() for p, *_ in tab], gs=[g.to_host().ravel() for _, g, *_ in tab],
+                      state=net.opt.state())
+
+    def update(net):
+        net.opt.step(lr)
+        if before:
+            eng.sync()
+            it, tab, state, wd = before["it"], before["tab"], before["state"], kw["weight_decay"]
+            for i, (p, g) in enumerate(zip(before["ps"], before["gs"])):
+                if kind == "sgd":
+                    want, _ = R.sgd32(p, g, state[i][0], lr, it + 1, kw["momentum"], 0.0, False, wd)
+                else:
+                    want, _, _ = R.adamw32(p, g, state[i][0], state[i][1], lr, it + 1, *kw["betas"], kw["eps"], wd)
+                assert same(tab[i][0].to_host().ravel(), want), (kind, it, i)
+            before.clear()
+
+    def check_trained(net):
+        assert net.opt.steps == EPOCHS * 8
+
+    ep_loss, acc, _ = train(eng, pkg, golden, Optimized, EPOCHS, update=update, check_step=check_step, check_trained=check_trained)
     print(f"GAP ResNet with {kind} lr {lr}: mean loss by epoch {ep_loss[0]:.4f} -> {ep_loss[-1]:.4f}; test accuracy {acc:.4f} (threshold {acc_min})")
     assert np.isfinite(ep_loss).all() and ep_loss[-1] < ep_loss[0]
     assert acc > acc_min

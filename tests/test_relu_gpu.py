@@ -10,11 +10,10 @@ import conv_ref as CR
 import conv_ref_strided as CS
 import linear_ref as LR
 import relu_ref as RR
+from example_nets import DEV, NAN_BF16, ReluNet, host, nan_buf, train
 
 pytestmark = pytest.mark.gpu
 
-NAN_BF16 = 0x7FC0
-DEV = torch.device("cuda", 0)
 TAIL = 64                      # elements past every output, prefilled with NaN: never written
 
 # N, H, W, C, K, R, S, stride: row-Toeplitz shapes
@@ -47,16 +46,8 @@ def cid(c):
     return "x".join(map(str, c[:7])) + f"-s{c[7]}" + (f"-pad{c[8]}" if len(c) == 9 else "")
 
 
-def host(a):
-    return a.cpu().numpy().view(np.uint16)
-
-
 def dev_bits(bits):
     return torch.from_numpy(np.ascontiguousarray(bits).view(np.int16)).to(DEV)
-
-
-def nan_buf(n):
-    return torch.full((n,), NAN_BF16, dtype=torch.int16, device=DEV)
 
 
 def same_or_nan(got, want):
@@ -428,93 +419,16 @@ def test_linear_layer_step_relu(eng, pkg):
 
 
 # ------------------------------------------------------------------------------------------------ 5. end to end
-B = 128
-LR_STEP = 0.05
-EPOCHS = 40
 ACC_MIN = 0.75          # a float32 torch CPU replica of this network, seed and step reaches 0.844
-
-
-def init_params(seed=5):
-    rng = np.random.default_rng(seed)
-    u = lambda shape, fan: rng.uniform(-1, 1, shape).astype(np.float32) / np.float32(np.sqrt(fan))
-    return dict(f1=u((8, 5, 5, 1), 25), b1=u(8, 25), f2=u((16, 3, 3, 8), 72), b2=u(16, 72), w3=u((128, 6, 6, 16), 576),
-                b3=u(128, 576), w4=u((10, 1, 1, 128), 128), b4=u(10, 128))
-
-
-class ReluNet:
-    """conv 8@5x5 ReLU -> pool 2 -> conv 16@3x3 pad 1 ReLU -> pool 2 -> fc 576->128 ReLU -> fc 128->10 -> softmax CE (1/B)"""
-
-    def __init__(self, eng, pkg, p):
-        self.eng = eng
-        relu = pkg.ACT_RELU
-        self.c1 = pkg.ConvLayer(eng, B, 28, 28, 1, 8, 5, 5, p["f1"], p["b1"], act=relu)
-        self.c2 = pkg.ConvLayer(eng, B, 12, 12, 8, 16, 3, 3, p["f2"], p["b2"], act=relu, padding=(1, 1))
-        self.fc1 = pkg.LinearLayer(eng, B, 6, 6, 16, 128, p["w3"], p["b3"], act=relu)
-        self.fc2 = pkg.LinearLayer(eng, B, 1, 1, 128, 10, p["w4"], p["b4"], act=pkg.ACT_NONE, row_pitch=128)
-        self.p1 = pkg.MaxPoolLayer(eng, B, 24, 24, 8, 2, row_pitch=self.c2.row_pitch, image_rows=self.c2.image_rows)
-        self.p2 = pkg.MaxPoolLayer(eng, B, 12, 12, 16, 2, row_pitch=self.fc1.row_pitch, image_rows=self.fc1.image_rows)
-        buf = lambda *shape: torch.full(shape, NAN_BF16, dtype=torch.int16, device=DEV)
-        self.y1, self.dy1 = buf(B, 24, 24, 8), buf(B, 24, 24, 8)
-        self.x2, self.dx2 = buf(B, 12, self.c2.row_pitch), buf(B, 12, self.c2.row_pitch)
-        self.y2, self.dy2 = buf(B, 12, 12, 16), buf(B, 12, 12, 16)
-        self.x3, self.dx3 = buf(B, 6, 96), buf(B, 6, 96)
-        self.y3, self.dy3 = buf(B, 128), buf(B, 128)
-        self.z, self.dz = buf(B, 10), buf(B, 10)
-        self.loss = torch.zeros(B, dtype=torch.float32, device=DEV)
-        self.pred = torch.zeros(B, dtype=torch.int32, device=DEV)
-
-    def forward(self, x, labels):
-        self.c1.forward(x, self.y1)
-        self.p1.forward(self.y1, self.x2)
-        self.c2.forward(self.x2, self.y2)
-        self.p2.forward(self.y2, self.x3)
-        self.fc1.forward(self.x3, self.y3)
-        self.fc2.forward(self.y3, self.z)
-        self.eng.softmax_ce_bf16(self.z, labels, B, 10, 1.0 / B, self.dz, self.loss, self.pred)
-
-    def backward(self, hook=lambda name, y, dy: None):
-        """hook(name, y, dy) runs before and after each ReLU layer's backward, which rewrites dy in place"""
-        self.fc2.backward(self.z, self.dz, self.dy3)
-        for name, layer, y, dy, dx, pool in (("fc1", self.fc1, self.y3, self.dy3, self.dx3, None),
-                                             ("c2", self.c2, self.y2, self.dy2, self.dx2, (self.p2, self.dx3)),
-                                             ("c1", self.c1, self.y1, self.dy1, None, (self.p1, self.dx2))):
-            if pool is not None:
-                pool[0].backward(pool[1], dy)
-            hook(name + ":before", y, dy)
-            layer.backward(y, dy, dx)
-            hook(name + ":after", y, dy)
-
-    def sgd(self, lr):
-        for layer in (self.c1, self.c2, self.fc1, self.fc2):
-            layer.sgd(lr)
-
-    def params(self):
-        return [a for layer in (self.c1, self.c2, self.fc1, self.fc2) for a in layer.params()]
-
-    def close(self):
-        for layer in (self.c1, self.c2, self.fc1, self.fc2, self.p1, self.p2):
-            layer.close()
-
-
-def mnist_device(pkg, u8):
-    n = u8.shape[0]
-    xl = np.zeros((n * 28, 32), np.uint16)
-    xl[:, :28] = pkg.f32_to_bf16_bits(u8.reshape(n, 28, 28).astype(np.float32) / 255.0).reshape(n * 28, 28)
-    return dev_bits(xl)
 
 
 def test_relu_classifier_mnist(eng, pkg, golden):
     """ReLU in c1, c2 and fc1.  In each of the first 5 steps every ReLU layer's dpre is bit-exact against the replay on the
     device's own y and dy.  A second fresh run reproduces the parameters after 5 steps bit for bit.  After EPOCHS epochs over
     the 1024 training digits the mean loss has fallen and test accuracy on the 256 test digits exceeds ACC_MIN."""
-    xs, ys = mnist_device(pkg, golden["train_u8"]), torch.from_numpy(golden["train_labels"]).to(DEV)
-    xt, yt = mnist_device(pkg, golden["test_u8"]), torch.from_numpy(golden["test_labels"]).to(DEV)
-    row_bytes = 28 * 32 * 2
-    batch = lambda s: (xs.data_ptr() + s * B * row_bytes, ys[s * B:(s + 1) * B])
 
-    net = ReluNet(eng, pkg, init_params())
-    for it in range(5):
-        net.forward(*batch(it))
+    def check_step(net, it, x, labels):
+        net.forward(x, labels)
         seen = {}
 
         def hook(name, y, dy):
@@ -528,32 +442,8 @@ def test_relu_classifier_mnist(eng, pkg, golden):
             assert np.array_equal(dpre, RR.bwd_bits(pkg, y, dy)), (it, name)
             frac = float((pkg.bf16_bits_to_f32(y) > 0).mean())
             assert 0.05 < frac < 0.95, (it, name, frac)          # the layer is neither dead nor linear
-        net.sgd(LR_STEP)
-        eng.sync()
-    after5 = net.params()
-    net.close()
 
-    net = ReluNet(eng, pkg, init_params())
-    losses = []
-    for ep in range(EPOCHS):
-        for s in range(1024 // B):
-            net.forward(*batch(s))
-            net.backward()
-            net.sgd(LR_STEP)
-            losses.append(net.loss)
-            net.loss = torch.zeros(B, dtype=torch.float32, device=DEV)
-            if ep == 0 and s == 4:
-                eng.sync()
-                assert all(np.array_equal(a.view(np.uint32), b_.view(np.uint32)) for a, b_ in zip(net.params(), after5))
-    eng.sync()
-    ep_loss = [float(torch.stack(losses[e * 8:(e + 1) * 8]).double().mean()) for e in range(EPOCHS)]
-    right = 0
-    for s in range(2):
-        net.forward(xt.data_ptr() + s * B * row_bytes, yt[s * B:(s + 1) * B])
-        eng.sync()
-        right += int((net.pred.cpu().numpy() == golden["test_labels"][s * B:(s + 1) * B]).sum())
-    acc = right / 256
-    net.close()
+    ep_loss, acc, _ = train(eng, pkg, golden, lambda: ReluNet(eng, pkg, ReluNet.init_params()), ReluNet.EPOCHS, check_step=check_step)
     print(f"ReLU classifier: mean loss by epoch {ep_loss[0]:.4f} -> {ep_loss[-1]:.4f}; test accuracy {acc:.4f} (threshold {ACC_MIN})")
     assert np.isfinite(ep_loss).all() and ep_loss[-1] < ep_loss[0]
     assert acc > ACC_MIN

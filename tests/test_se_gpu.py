@@ -4,16 +4,12 @@ operands and bit-identical to the replay in the reported partition order on rand
 operands, the fused optimizers over the layer, and an SE-ResNet trained on MNIST digits."""
 import numpy as np
 import pytest
-import torch
 
 import optim_ref as OR
 import se_ref as SR
-from test_avgpool_nhwc_gpu import NB, init_params, mnist_device
+from example_nets import NAN_BF16, SEResNet, host, train
 
 pytestmark = pytest.mark.gpu
-
-DEV = torch.device("cuda", 0)
-NAN_BF16 = 0x7FC0
 TAIL = 64                 # elements past every output, NaN before the call and after it
 
 
@@ -311,112 +307,7 @@ def test_optimizers(eng, pkg, kind):
 
 
 # ------------------------------------------------------------------------------------------------ end to end
-LR_STEP = 0.2
-EPOCHS = 40
 ACC_MIN = 0.90          # the float32 torch CPU replica (scripts/seresnet_replica.py) of this network reaches 0.961 (DESIGN 3.19)
-
-
-def init_se(seed=10):
-    rng = np.random.default_rng(seed)
-    return dict(se1=se_params(rng, 16, 8), se2=se_params(rng, 32, 8))
-
-
-class SEResNet:
-    """The GAP ResNet of test_avgpool_nhwc_gpu.py with squeeze-and-excitation in both residual blocks: each block's last BN runs
-    without r and ReLU, and an SE layer (16 -> 8 -> 16, then 32 -> 8 -> 32) carries the residual add and the ReLU."""
-
-    def __init__(self, eng, pkg, p, q):
-        self.eng = eng
-        relu, none = pkg.ACT_RELU, pkg.ACT_NONE
-        B = NB
-        conv = lambda H, C, K, R, f, **k: pkg.ConvLayer(eng, B, H, H, C, K, R, R, p[f], None, act=none, **k)
-        self.c1 = conv(28, 1, 8, 5, "f1")
-        self.c2 = conv(12, 8, 16, 3, "f2", padding=(1, 1))
-        self.c3, self.c4 = conv(12, 16, 16, 3, "f3", padding=(1, 1)), conv(12, 16, 16, 3, "f4", padding=(1, 1))
-        self.c5 = conv(12, 16, 32, 3, "f5", padding=(1, 1), stride=2)
-        self.c6 = conv(6, 32, 32, 3, "f6", padding=(1, 1))
-        self.c7 = conv(12, 16, 32, 3, "f7", padding=(1, 1), stride=2)
-        BN = lambda H, C, act: pkg.BatchNormLayer(eng, B, H, H, C, act=act)
-        self.bn = [BN(24, 8, relu), BN(12, 16, relu), BN(12, 16, relu), BN(12, 16, none), BN(6, 32, relu), BN(6, 32, none), BN(6, 32, none)]
-        self.se1 = pkg.SqueezeExcitationLayer(eng, B, 12, 12, 16, 8, *q["se1"], act=relu)
-        self.se2 = pkg.SqueezeExcitationLayer(eng, B, 6, 6, 32, 8, *q["se2"], act=relu)
-        self.pool = pkg.AvgPoolLayer(eng, B, 24, 24, 8, 2, row_pitch=self.c2.row_pitch, image_rows=self.c2.image_rows)
-        self.gap = pkg.GlobalAvgPoolLayer(eng, B, 6, 6, 32)
-        self.fc = pkg.LinearLayer(eng, B, 1, 1, 32, 10, p["w8"], p["b8"], act=none, row_pitch=self.gap.row_pitch)
-        buf = lambda *shape: torch.full(shape, NAN_BF16, dtype=torch.int16, device=DEV)
-        self.y1, self.z1, self.dz1, self.dy1 = (buf(B, 24, 24, 8) for _ in range(4))
-        self.x2, self.dx2 = buf(B, 12, self.c2.row_pitch), buf(B, 12, self.c2.row_pitch)
-        (self.y2, self.x0, self.y3, self.z3, self.y4, self.z4, self.x1, self.dx1, self.dx1p, self.dz4, self.dy4, self.dres, self.dz3,
-         self.dy3, self.dx0, self.dy2) = (buf(B, 12, 12, 16) for _ in range(16))
-        (self.y5, self.z5, self.y6, self.z6, self.out, self.y7, self.s, self.dout, self.dz6, self.dy6, self.ds, self.dy7, self.dz5,
-         self.dy5) = (buf(B, 6, 6, 32) for _ in range(14))
-        self.h, self.dh = buf(B, self.gap.row_pitch), buf(B, self.gap.row_pitch)
-        self.z, self.dz = buf(B, 10), buf(B, 10)
-        self.loss = torch.zeros(B, dtype=torch.float32, device=DEV)
-        self.pred = torch.zeros(B, dtype=torch.int32, device=DEV)
-
-    def forward(self, x, labels, training=True):
-        b1, b2, b3, b4, b5, b6, b7 = self.bn
-        self.c1.forward(x, self.y1)
-        b1.forward(self.y1, self.z1, training=training)
-        self.pool.forward(self.z1, self.x2)
-        self.c2.forward(self.x2, self.y2)
-        b2.forward(self.y2, self.x0, training=training)
-        self.c3.forward(self.x0, self.y3)
-        b3.forward(self.y3, self.z3, training=training)
-        self.c4.forward(self.z3, self.y4)
-        b4.forward(self.y4, self.z4, training=training)
-        self.se1.forward(self.z4, self.x1, r=self.x0)
-        self.c5.forward(self.x1, self.y5)
-        b5.forward(self.y5, self.z5, training=training)
-        self.c6.forward(self.z5, self.y6)
-        self.c7.forward(self.x1, self.y7)
-        b7.forward(self.y7, self.s, training=training)
-        b6.forward(self.y6, self.z6, training=training)
-        self.se2.forward(self.z6, self.out, r=self.s)
-        self.gap.forward(self.out, self.h)
-        self.fc.forward(self.h, self.z)
-        self.eng.softmax_ce_bf16(self.z, labels, NB, 10, 1.0 / NB, self.dz, self.loss, self.pred)
-
-    def backward(self):
-        b1, b2, b3, b4, b5, b6, b7 = self.bn
-        self.fc.backward(self.z, self.dz, self.dh)
-        self.gap.backward(self.dh, self.dout)
-        self.se2.backward(self.out, self.dout, self.dz6, dr=self.ds)
-        b6.backward(self.z6, self.dz6, self.dy6)
-        self.c6.backward(self.y6, self.dy6, self.dz5)
-        b5.backward(self.z5, self.dz5, self.dy5)
-        self.c5.backward(self.y5, self.dy5, self.dx1)
-        b7.backward(self.s, self.ds, self.dy7)
-        self.c7.backward(self.y7, self.dy7, self.dx1p)
-        self.se1.backward(self.x1, self.dx1, self.dz4, dr=self.dres, dy2=self.dx1p)   # main path and projection meet at x1
-        b4.backward(self.z4, self.dz4, self.dy4)
-        self.c4.backward(self.y4, self.dy4, self.dz3)
-        b3.backward(self.z3, self.dz3, self.dy3)
-        self.c3.backward(self.y3, self.dy3, self.dx0)
-        b2.backward(self.x0, self.dx0, self.dy2, dy2=self.dres)
-        self.c2.backward(self.y2, self.dy2, self.dx2)
-        self.pool.backward(self.dx2, self.dz1)
-        b1.backward(self.z1, self.dz1, self.dy1)
-        self.c1.backward(self.y1, self.dy1, None)
-
-    def layers(self):
-        return (self.c1, self.c2, self.c3, self.c4, self.c5, self.c6, self.c7, self.fc, *self.bn, self.se1, self.se2)
-
-    def sgd(self, lr):
-        for layer in self.layers():
-            layer.sgd(lr)
-
-    def params(self):
-        return [a for layer in self.layers() for a in layer.params() if a is not None]
-
-    def close(self):
-        for layer in (*self.layers(), self.pool, self.gap):
-            layer.close()
-
-
-def host(t):
-    return t.cpu().numpy().view(np.uint16)
 
 
 def test_seresnet_mnist(eng, pkg, golden):
@@ -424,63 +315,31 @@ def test_seresnet_mnist(eng, pkg, golden):
     device's own tensors (ds through that gradient).  A fresh run reproduces the parameters after 5 steps bit for bit.  After
     EPOCHS epochs over the 1024 training digits the mean loss has fallen, and test accuracy on the 256 test digits, evaluated with
     the running statistics, exceeds ACC_MIN."""
-    xs, ys = mnist_device(pkg, golden["train_u8"]), torch.from_numpy(golden["train_labels"]).to(DEV)
-    xt, yt = mnist_device(pkg, golden["test_u8"]), torch.from_numpy(golden["test_labels"]).to(DEV)
-    row_bytes = 28 * 32 * 2
-    batch = lambda s, xs=xs, ys=ys: (xs.data_ptr() + s * NB * row_bytes, ys[s * NB:(s + 1) * NB])
     bits, val = pkg.f32_to_bf16_bits, pkg.bf16_bits_to_f32
     B = Plain(eng)
+    NB = SEResNet.NB
 
-    net = SEResNet(eng, pkg, init_params(), init_se())
-    try:
-        for it in range(5):
-            net.forward(*batch(it))
-            eng.sync()
-            fwd = {1: (host(net.z4), host(net.x0), host(net.x1)), 2: (host(net.z6), host(net.s), host(net.out))}
-            ss = {1: B.read_plain(net.se1.s, (NB, 16)), 2: B.read_plain(net.se2.s, (NB, 32))}
-            net.backward()
-            eng.sync()
-            for k, L, dy, dy2, g, dx in ((1, net.se1, net.dx1, net.dx1p, net.dres, net.dz4), (2, net.se2, net.dout, None, net.ds, net.dz6)):
-                N, H, W, C = L.shape
-                x, r, y = fwd[k]
-                s = ss[k]
-                assert np.array_equal(y, bits(SR.fwd(val(x), val(s), val(r), 3))), (it, k, "y")
-                gg, dyh = host(g), host(dy)
-                want_g = SR.gate_g(val(dyh), val(y), None if dy2 is None else val(host(dy2)), 3)
-                assert np.array_equal(gg, bits(want_g)), (it, k, "g")
-                want_ds = bits(SR.gate_ds(val(gg), val(x), L.info))
-                assert np.array_equal(B.read_plain(L.ds, (N, C)), bits(SR.sigmoid_bwd(val(want_ds), val(s)))), (it, k, "fc2 dpre")
-                dh = B.read_plain(L.dh, (N, L.row_pitch))[:, :C]
-                assert np.array_equal(host(dx), bits(SR.dx(val(gg), val(s), val(dh), H * W))), (it, k, "dx")
-            net.sgd(LR_STEP)
-            eng.sync()
-        after5 = net.params()
-    finally:
-        net.close()
-
-    net = SEResNet(eng, pkg, init_params(), init_se())
-    try:
-        losses = []
-        for ep in range(EPOCHS):
-            for s in range(1024 // NB):
-                net.forward(*batch(s))
-                net.backward()
-                net.sgd(LR_STEP)
-                losses.append(net.loss)
-                net.loss = torch.zeros(NB, dtype=torch.float32, device=DEV)
-                if ep == 0 and s == 4:
-                    eng.sync()
-                    assert all(np.array_equal(a.view(np.uint32), b_.view(np.uint32)) for a, b_ in zip(net.params(), after5))
+    def check_step(net, it, x, labels):
+        net.forward(x, labels)
         eng.sync()
-        ep_loss = [float(torch.stack(losses[e * 8:(e + 1) * 8]).double().mean()) for e in range(EPOCHS)]
-        right = 0
-        for s in range(2):
-            net.forward(*batch(s, xt, yt), training=False)
-            eng.sync()
-            right += int((net.pred.cpu().numpy() == golden["test_labels"][s * NB:(s + 1) * NB]).sum())
-    finally:
-        net.close()
-    acc = right / 256
+        fwd = {1: (host(net.z4), host(net.x0), host(net.x1)), 2: (host(net.z6), host(net.s), host(net.out))}
+        ss = {1: B.read_plain(net.se1.s, (NB, 16)), 2: B.read_plain(net.se2.s, (NB, 32))}
+        net.backward()
+        eng.sync()
+        for k, L, dy, dy2, g, dx in ((1, net.se1, net.dx1, net.dx1p, net.dres, net.dz4), (2, net.se2, net.dout, None, net.ds, net.dz6)):
+            N, H, W, C = L.shape
+            x, r, y = fwd[k]
+            s = ss[k]
+            assert np.array_equal(y, bits(SR.fwd(val(x), val(s), val(r), 3))), (it, k, "y")
+            gg, dyh = host(g), host(dy)
+            want_g = SR.gate_g(val(dyh), val(y), None if dy2 is None else val(host(dy2)), 3)
+            assert np.array_equal(gg, bits(want_g)), (it, k, "g")
+            want_ds = bits(SR.gate_ds(val(gg), val(x), L.info))
+            assert np.array_equal(B.read_plain(L.ds, (N, C)), bits(SR.sigmoid_bwd(val(want_ds), val(s)))), (it, k, "fc2 dpre")
+            dh = B.read_plain(L.dh, (N, L.row_pitch))[:, :C]
+            assert np.array_equal(host(dx), bits(SR.dx(val(gg), val(s), val(dh), H * W))), (it, k, "dx")
+
+    ep_loss, acc, _ = train(eng, pkg, golden, lambda: SEResNet(eng, pkg, SEResNet.init_params()), SEResNet.EPOCHS, check_step=check_step)
     print(f"SE-ResNet: mean loss by epoch {ep_loss[0]:.4f} -> {ep_loss[-1]:.4f}; test accuracy {acc:.4f} (threshold {ACC_MIN})")
     assert np.isfinite(ep_loss).all() and ep_loss[-1] < ep_loss[0]
     assert acc > ACC_MIN
