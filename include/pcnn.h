@@ -823,6 +823,26 @@ int pcnn_augment_u8_bf16(pcnn_ctx *ctx, const uint8_t *images_dev, const uint8_t
 int pcnn_augment_u8_bf16_info(long long n, int H, int W, int C, long long first, int N, int shuffle, int pad, int flip, int C_out,
                               int row_pitch, int image_rows, const float *mean_host, const float *std_host, long long *out8,
                               uint16_t *lut_out);
+/* Mixed batches (csrc/augment.cu): pcnn_augment_u8_bf16's batch with torchvision's MixUp (mode 1) or CutMix (mode 2) of each
+ * image and its partner, as transforms.v2.MixUp / CutMix apply them to the transformed batch.
+ *   - Partner: position j's partner is j' = (j + N - 1) mod N (torchvision's roll(1, 0)); N = 1 pairs the image with itself.  Each
+ *     image gets its own permutation position, crop and flip exactly as the plain call gives them; a and b below are the fp32
+ *     values v(c, u) (before the bf16 rounding) of j's and j''s augmented pixels.
+ *   - MixUp: x = bf16_rn(RN(RN(b * RN32(1 - lam)) + RN(a * RN32(lam)))), 1 - lam and lam formed in double and rounded to fp32, no
+ *     contraction: what inpt.roll(1, 0).mul_(1.0 - lam).add_(inpt.mul(lam)) computes.  The host forms the fp32 table beside the
+ *     bf16 one.
+ *   - CutMix: output rows y1 <= h < y2 and columns x1 <= w < x2 (output coordinates, after crop and flip) take the partner's
+ *     element, every other pixel j's own: each element has the bits of the plain call's table.
+ *   - labels_out[j] = the label of j, labels_b_out[j] = the label of j'.  Channels C <= c < C_out are +0; pad columns and pad rows
+ *     of x are never written.
+ * Domain: everything pcnn_augment_u8_bf16 requires, with the same messages, plus mode 1 or 2; lam finite with 0 <= lam <= 1;
+ * 0 <= x1 <= x2 <= W and 0 <= y1 <= y2 <= H (an empty box is allowed); labels_b_out NULL exactly when labels is; labels_b_out
+ * sharing no byte with x, images, labels or labels_out.  The launch is the plain call's (grid, rows per CTA, vector width); lane 0
+ * of a second warp walks the partner's permutation and draws its crop beside thread 0's own. */
+int pcnn_augment_mix_u8_bf16(pcnn_ctx *ctx, const uint8_t *images_dev, const uint8_t *labels_dev, long long n, int H, int W, int C,
+                             long long first, int N, int shuffle, int pad, int flip, unsigned long long seed, unsigned long long epoch,
+                             const float *mean_host, const float *std_host, void *x_bf16_dev, int C_out, int row_pitch, int image_rows,
+                             uint8_t *labels_out_dev, int mode, double lam, int x1, int y1, int x2, int y2, uint8_t *labels_b_out_dev);
 /* Softmax cross-entropy on bf16 logits [N][O], 1 <= O <= 256, labels uint8 [N]:
  *   p = softmax(row) evaluated in double: m = max, den = sum exp(z - m), p_t = exp(z_t - m) / den;
  *   dlogits[n][t] = bf16_rn(float_rn((p_t - [t == label]) * scale)), double -> fp32 -> bf16, each round to nearest even: the
@@ -832,6 +852,20 @@ int pcnn_augment_u8_bf16_info(long long n, int H, int W, int C, long long first,
  * still the argmax).  dlogits == logits (in place) is allowed, any other overlap is not. */
 int pcnn_softmax_ce_bf16(pcnn_ctx *ctx, const void *logits_bf16_dev, const uint8_t *labels_dev, int N, int O, float scale,
                          void *dlogits_bf16_dev, float *loss_f32_dev, int *pred_i32_dev);
+/* Softmax cross-entropy against a soft target: pcnn_softmax_ce_bf16's layouts, limits, p and pred, with the target row built in
+ * fp32 (RN: fp32 round to nearest, no contraction) as torchvision's MixUp / CutMix labels and torch's label smoothing build it:
+ *   m_t = RN(RN([t == label_b] RN32(1 - lam)) + RN([t == label] RN32(lam)))   (_mixup_label; labels_b NULL: m_t = [t == label])
+ *   q_t = RN(RN(m_t RN32(1 - eps)) + RN32(eps / O))                               (cross_entropy's label_smoothing = eps)
+ *   dlogits[n][t] = bf16_rn(float_rn((p_t - q_t) * scale)), p_t in double as the hard call computes it;
+ *   loss[n] = fp32 of -sum_t q_t ((z_t - m) - log den) in double, terms with q_t = 0 skipped (may be NULL).
+ * Skipping the zero terms differs from torch, whose probability-target path computes 0 * (-Inf) = NaN for a -Inf logit with a
+ * zero target; here lam = 1 with eps = 0 gives pcnn_softmax_ce_bf16's bits on every row, whatever labels_b, ±Inf logits included.
+ * A row holding a NaN, or a label or label_b >= O, gets a NaN loss and NaN dlogits (pred -1 for NaN, the argmax otherwise).
+ * Domain (PCNN_ERR_ARG, one message per rule): lam finite with 0 <= lam <= 1, 0 <= eps <= 1, plus the hard call's; dlogits ==
+ * logits (in place) is allowed, any other overlap is not. */
+int pcnn_softmax_ce_soft_bf16(pcnn_ctx *ctx, const void *logits_bf16_dev, const uint8_t *labels_dev, const uint8_t *labels_b_dev,
+                              double lam, double smoothing, int N, int O, float scale, void *dlogits_bf16_dev, float *loss_f32_dev,
+                              int *pred_i32_dev);
 /* Optimizers for device-trained layers (csrc/optim.cu): one fused update of every parameter tensor of a network per step, as
  * torch.optim.SGD and torch.optim.AdamW (decoupled weight decay) in their single-tensor form, with the bf16 operands of the plans
  * the parameters belong to refreshed in the same pass.

@@ -17,7 +17,7 @@ from ._lib import (  # noqa: F401
 )
 from .engine import AvgPoolLayer, BatchNormLayer, ConvLayer, GlobalAvgPoolLayer, ConvPlan, LinearLayer, LinearPlan, MaxPoolLayer, DeviceArray, WideConvPlan, Engine, bf16_bits_to_f32, f32_to_bf16_bits  # noqa: F401
 from .engine import DepthwiseConvLayer, DepthwiseConvPlan, DropoutLayer, GroupedConvLayer, GroupedConvPlan, SqueezeExcitationLayer  # noqa: F401
-from .engine import ImageBatcher  # noqa: F401
+from .engine import ImageBatcher, MixedLabels, MIX_MIXUP, MIX_CUTMIX, mix_draws  # noqa: F401
 from .engine import SGD, AdamW, FusedOptimizer  # noqa: F401
 
 __all__ = ["Engine", "DeviceArray", "PcnnError", "lib", "declared_symbols", "init_params_reference",
@@ -26,4 +26,5 @@ __all__ = ["Engine", "DeviceArray", "PcnnError", "lib", "declared_symbols", "ini
            "ACT_SILU", "ACT_HARDSWISH", "ACT_RELU6",
            "SGD", "AdamW", "FusedOptimizer", "OPTIM_SGD", "OPTIM_ADAMW", "dwconv_info", "DepthwiseConvLayer", "DepthwiseConvPlan",
            "gconv_info", "GroupedConvLayer", "GroupedConvPlan", "se_scale_nhwc_info", "SqueezeExcitationLayer",
-           "dropout_info", "DropoutLayer", "augment_info", "ImageBatcher"]
+           "dropout_info", "DropoutLayer", "augment_info", "ImageBatcher",
+           "MixedLabels", "MIX_MIXUP", "MIX_CUTMIX", "mix_draws"]

@@ -185,7 +185,10 @@ _SIG = {
     "pcnn_augment_u8_bf16": [_vp, _vp, _vp, C.c_longlong, _i, _i, _i, C.c_longlong, _i, _i, _i, _i, C.c_ulonglong, C.c_ulonglong, _vp, _vp,
                              _vp, _i, _i, _i, _vp],
     "pcnn_augment_u8_bf16_info": [C.c_longlong, _i, _i, _i, C.c_longlong, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp],
+    "pcnn_augment_mix_u8_bf16": [_vp, _vp, _vp, C.c_longlong, _i, _i, _i, C.c_longlong, _i, _i, _i, _i, C.c_ulonglong, C.c_ulonglong,
+                                 _vp, _vp, _vp, _i, _i, _i, _vp, _i, C.c_double, _i, _i, _i, _i, _vp],
     "pcnn_softmax_ce_bf16": [_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp],
+    "pcnn_softmax_ce_soft_bf16": [_vp, _vp, _vp, _vp, C.c_double, C.c_double, _i, _i, _f, _vp, _vp, _vp],
     "pcnn_optim_create": [_vp, _vp, _vp, _i, _pvp],
     "pcnn_optim_step": [_vp, _vp, _f],
     "pcnn_optim_state": [_vp, _i, _pvp, _pvp],

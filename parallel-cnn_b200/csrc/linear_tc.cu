@@ -349,8 +349,17 @@ __global__ void __launch_bounds__(256) k_linear_pad_rows(const __nv_bfloat16 *__
 
 // ================================================= softmax cross-entropy ========================================================
 // One warp per row, lane t holds logits t, t + 32, ... (O <= 256: 8 each), all read before anything is written (in place).
+// SOFT: the target q_t of pcnn_softmax_ce_soft_bf16, built in fp32 from the labels, labels_b and the weights of SoftTarget.
+struct SoftTarget {
+    const uint8_t *labels_b;  // NULL: m_t = [t == label]
+    float lam, oml;           // RN32(lam), RN32(1 - lam)
+    float ome, eps_o;         // RN32(1 - eps), RN32(eps / O)
+};
+
+template <bool SOFT>
 __global__ void __launch_bounds__(256) k_softmax_ce_bf16(const __nv_bfloat16 *z, const uint8_t *__restrict__ labels, int N, int O,
-                                                         double scale, __nv_bfloat16 *d, float *__restrict__ loss, int *__restrict__ pred) {
+                                                         double scale, __nv_bfloat16 *d, float *__restrict__ loss, int *__restrict__ pred,
+                                                         const SoftTarget st) {
     const int lane = threadIdx.x & 31;
     const long warp = (blockIdx.x * (long)blockDim.x + threadIdx.x) >> 5;
     const long nwarps = ((long)gridDim.x * blockDim.x) >> 5;
@@ -385,18 +394,54 @@ __global__ void __launch_bounds__(256) k_softmax_ce_bf16(const __nv_bfloat16 *z,
             if (lane + 32 * j < O) den += exp((double)v[j] - mx);
         for (int s = 16; s; s >>= 1) den += __shfl_xor_sync(0xffffffffu, den, s);
         const int y = labels[r];
-        const bool bad = nan || y >= O;
+        if constexpr (!SOFT) {
+            const bool bad = nan || y >= O;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int t = lane + 32 * j;
-            if (t >= O) continue;
-            const double g = (exp((double)v[j] - mx) / den - (t == y ? 1.0 : 0.0)) * scale;
-            d[r * O + t] = bad ? __float2bfloat16_rn(NAN) : __float2bfloat16_rn((float)g);
-            if (t == y && loss) loss[r] = nan ? NAN : (float)(-(((double)v[j] - mx) - log(den)));
-        }
-        if (lane == 0) {
-            if (loss && y >= O) loss[r] = NAN;
-            if (pred) pred[r] = nan ? -1 : bi;
+            for (int j = 0; j < 8; ++j) {
+                const int t = lane + 32 * j;
+                if (t >= O) continue;
+                const double g = (exp((double)v[j] - mx) / den - (t == y ? 1.0 : 0.0)) * scale;
+                d[r * O + t] = bad ? __float2bfloat16_rn(NAN) : __float2bfloat16_rn((float)g);
+                if (t == y && loss) loss[r] = nan ? NAN : (float)(-(((double)v[j] - mx) - log(den)));
+            }
+            if (lane == 0) {
+                if (loss && y >= O) loss[r] = NAN;
+                if (pred) pred[r] = nan ? -1 : bi;
+            }
+        } else {
+            const int yb = st.labels_b ? st.labels_b[r] : y;
+            const bool bad = nan || y >= O || yb >= O;
+            const double lden = log(den);
+            double part = 0.0;                            // this lane's terms of sum q_t ((z_t - m) - log den)
+            int terms = 0;
+            bool hot = false;                             // this lane holds a q_t == 1
+            float lhot = 0.0f;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int t = lane + 32 * j;
+                if (t >= O) continue;
+                // m_t = RN(RN([t == yb] (1 - lam)) + RN([t == y] lam)), or [t == y] without labels_b; q_t = RN(RN(m_t (1 - eps)) + eps / O)
+                const float mt = st.labels_b ? __fadd_rn(t == yb ? st.oml : 0.0f, t == y ? st.lam : 0.0f) : (t == y ? 1.0f : 0.0f);
+                const float q = __fadd_rn(__fmul_rn(mt, st.ome), st.eps_o);
+                const double g = (exp((double)v[j] - mx) / den - (double)q) * scale;
+                d[r * O + t] = bad ? __float2bfloat16_rn(NAN) : __float2bfloat16_rn((float)g);
+                if (q != 0.0f) {                          // terms with q_t = 0 skipped
+                    part += (double)q * (((double)v[j] - mx) - lden);
+                    ++terms;
+                    if (q == 1.0f) {
+                        hot = true;
+                        lhot = (float)(-(((double)v[j] - mx) - lden));
+                    }
+                }
+            }
+            for (int s = 16; s; s >>= 1) {
+                part += __shfl_xor_sync(0xffffffffu, part, s);
+                terms += __shfl_xor_sync(0xffffffffu, terms, s);
+            }
+            // a one-hot target takes the hard kernel's expression, so that its loss bits (NaN ones from +-Inf logits included) match
+            const bool one_hot = terms == 1 && __any_sync(0xffffffffu, hot);
+            if (loss && (one_hot ? hot : lane == 0)) loss[r] = bad ? NAN : one_hot ? lhot : (float)(-part);
+            if (lane == 0 && pred) pred[r] = nan ? -1 : bi;
         }
     }
 }
@@ -675,8 +720,35 @@ extern "C" int pcnn_softmax_ce_bf16(pcnn_ctx *ctx, const void *logits_bf16, cons
     pcnn_device_guard g(ctx->device);
     long blocks = ((long)N * 32 + 255) / 256;
     if (blocks > (long)ctx->sm_count * 8) blocks = (long)ctx->sm_count * 8;
-    k_softmax_ce_bf16<<<(int)blocks, 256, 0, ctx->stream>>>(static_cast<const __nv_bfloat16 *>(logits_bf16), labels, N, O, (double)scale,
-                                                            static_cast<__nv_bfloat16 *>(dlogits_bf16), loss_f32, pred_i32);
+    k_softmax_ce_bf16<false><<<(int)blocks, 256, 0, ctx->stream>>>(static_cast<const __nv_bfloat16 *>(logits_bf16), labels, N, O,
+                                                                   (double)scale, static_cast<__nv_bfloat16 *>(dlogits_bf16), loss_f32,
+                                                                   pred_i32, SoftTarget{});
+    PCNN_CHECK_LAUNCH(ctx);
+    return PCNN_OK;
+}
+
+extern "C" int pcnn_softmax_ce_soft_bf16(pcnn_ctx *ctx, const void *logits_bf16, const uint8_t *labels, const uint8_t *labels_b, double lam,
+                                         double smoothing, int N, int O, float scale, void *dlogits_bf16, float *loss_f32, int *pred_i32) {
+    const char *fn = "pcnn_softmax_ce_soft_bf16";
+    PCNN_REQUIRE(ctx && logits_bf16 && labels && dlogits_bf16, PCNN_ERR_ARG, "%s: NULL context, logits, labels or dlogits", fn);
+    PCNN_REQUIRE(N >= 1 && O >= 1 && O <= 256, PCNN_ERR_ARG, "%s: N = %d, O = %d: N >= 1 and 1 <= O <= 256 are required", fn, N, O);
+    PCNN_REQUIRE(std::isfinite(lam) && lam >= 0.0 && lam <= 1.0, PCNN_ERR_ARG, "%s: lam = %g: a finite 0 <= lam <= 1 is required", fn, lam);
+    PCNN_REQUIRE(smoothing >= 0.0 && smoothing <= 1.0, PCNN_ERR_ARG, "%s: smoothing = %g: 0 <= smoothing <= 1 is required", fn, smoothing);
+    const size_t zb = (size_t)N * O * 2;
+    const uintptr_t z = (uintptr_t)logits_bf16, d = (uintptr_t)dlogits_bf16;
+    PCNN_REQUIRE(d == z || d + zb <= z || z + zb <= d, PCNN_ERR_ARG, "%s: dlogits overlaps logits without being the same buffer", fn);
+    SoftTarget st;
+    st.labels_b = labels_b;
+    st.lam = (float)lam;
+    st.oml = (float)(1.0 - lam);
+    st.ome = (float)(1.0 - smoothing);
+    st.eps_o = (float)(smoothing / O);
+    pcnn_device_guard g(ctx->device);
+    long blocks = ((long)N * 32 + 255) / 256;
+    if (blocks > (long)ctx->sm_count * 8) blocks = (long)ctx->sm_count * 8;
+    k_softmax_ce_bf16<true><<<(int)blocks, 256, 0, ctx->stream>>>(static_cast<const __nv_bfloat16 *>(logits_bf16), labels, N, O,
+                                                                  (double)scale, static_cast<__nv_bfloat16 *>(dlogits_bf16), loss_f32,
+                                                                  pred_i32, st);
     PCNN_CHECK_LAUNCH(ctx);
     return PCNN_OK;
 }

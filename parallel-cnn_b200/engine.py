@@ -1,6 +1,8 @@
 """Engine: a thin object wrapper over one pcnn_ctx.  Method names follow include/pcnn.h minus the pcnn_ prefix, which
 in turn follow /root/reference/Sequential/layer.h and Main.cpp (fp_c1, bp_weight_c1, learn, test ...)."""
 import ctypes as C
+import math
+from typing import NamedTuple, Optional
 
 import numpy as np
 
@@ -10,6 +12,7 @@ from ._lib import (F32, NPARAM, OPTIM_ADAMW, OPTIM_SGD, TEST_SET, TRAIN_SET, U8,
                    se_scale_nhwc_info, ACT_RELU, ACT_SIGMOID, ACT_SILU, ACT_HARDSWISH, ACT_RELU6)
 
 PREACT_CODES = (ACT_SILU, ACT_HARDSWISH, ACT_RELU6)   # batch normalization's codes whose backward recomputes the pre-activation
+MIX_MIXUP, MIX_CUTMIX = 1, 2                         # pcnn_augment_mix_u8_bf16's modes
 
 
 def _pixel_type(arr_or_dtype):
@@ -494,6 +497,13 @@ class Engine:
         itself), fp32 loss [N] and int32 pred [N] (each None to skip)"""
         self._call("pcnn_softmax_ce_bf16", _p(logits), _p(labels), int(N), int(O), float(scale), _p(dlogits), _p(loss), _p(pred))
 
+    def softmax_ce_soft_bf16(self, logits, labels, N, O, scale, dlogits, loss=None, pred=None, labels_b=None, lam=1.0, smoothing=0.0):
+        """pcnn_softmax_ce_soft_bf16: as softmax_ce_bf16 against the fp32 target q = (lam onehot(labels) + (1 - lam)
+        onehot(labels_b)) (1 - smoothing) + smoothing / O (labels_b None: onehot(labels)), the target of a MixUp / CutMix batch
+        (MixedLabels) with label smoothing"""
+        self._call("pcnn_softmax_ce_soft_bf16", _p(logits), _p(labels), _p(labels_b), float(lam), float(smoothing), int(N), int(O),
+                   float(scale), _p(dlogits), _p(loss), _p(pred))
+
     def linear_wgrad(self, plan, x, dy, dw):
         """pcnn_linear_wgrad: dW fp32 [O][P][Q][C] = dy^T x, the shape from the LinearPlan"""
         self._call("pcnn_linear_wgrad", plan.plan, _p(x), _p(dy), _p(dw))
@@ -555,6 +565,53 @@ class Engine:
         self._call("pcnn_augment_u8_bf16", _p(images), _p(labels), int(n), int(H), int(W), Cin, int(first), int(N), int(shuffle), int(pad),
                    int(flip), int(seed), int(epoch), None if m is None else m.ctypes.data, None if s is None else s.ctypes.data, _p(x),
                    Cin if C_out is None else int(C_out), int(row_pitch or 0), int(image_rows or 0), _p(labels_out))
+
+    def augment_mix(self, images, labels, n, H, W, C, first, N, x, labels_out=None, labels_b_out=None, mode=MIX_MIXUP, lam=1.0,
+                    box=(0, 0, 0, 0), shuffle=1, pad=0, flip=0, seed=0, epoch=0, mean=None, std=None, C_out=None, row_pitch=0,
+                    image_rows=0):
+        """pcnn_augment_mix_u8_bf16: augment's batch with MixUp (mode MIX_MIXUP: lam j + (1 - lam) j' in fp32) or CutMix
+        (MIX_CUTMIX: the box (x1, y1, x2, y2) of output pixels from j') of each position j and its partner j' = (j + N - 1) mod N;
+        labels_b_out [N] receives the partners' labels"""
+        Cin = int(C)
+        m, s = channel_stats(mean, Cin, "mean"), channel_stats(std, Cin, "std")
+        x1, y1, x2, y2 = (int(v) for v in box)
+        self._call("pcnn_augment_mix_u8_bf16", _p(images), _p(labels), int(n), int(H), int(W), Cin, int(first), int(N), int(shuffle),
+                   int(pad), int(flip), int(seed), int(epoch), None if m is None else m.ctypes.data, None if s is None else s.ctypes.data,
+                   _p(x), Cin if C_out is None else int(C_out), int(row_pitch or 0), int(image_rows or 0), _p(labels_out), int(mode),
+                   float(lam), x1, y1, x2, y2, _p(labels_b_out))
+
+
+class MixedLabels(NamedTuple):
+    """The targets of a mixed training batch: image j is lam parts labels[j] and 1 - lam parts labels_b[j] (lam_adjusted, the
+    box's complement over the image, for CutMix).  kind is "mixup" or "cutmix"; box (x1, y1, x2, y2) the CutMix box, else None."""
+    labels: object
+    labels_b: object
+    lam: float
+    kind: str
+    box: Optional[tuple]
+
+
+def mix_draws(seed, epoch, step, H, W, mixup_alpha, cutmix_alpha):
+    """(kind, lam, box, lam_adjusted) of training batch `step` of `epoch` (box and lam_adjusted None for MixUp), drawn from numpy's
+    Philox generator keyed by seed with counter (0, 0, epoch, step), so a function of (seed, epoch, step) alone.  In order:
+      1. with both alphas > 0, u = random(): CutMix iff u < 1/2 (torchvision's RandomChoice([MixUp, CutMix])); otherwise the kind
+         whose alpha is > 0;
+      2. lam = beta(alpha, alpha) with that kind's alpha;
+      3. CutMix: r_x = integers(W), then r_y = integers(H), and the box and lam_adjusted exactly as v2.CutMix.make_params forms
+         them (double arithmetic, int() truncation, clamping to the image).
+    numpy does not promise the same Generator.beta stream across numpy versions, so a different numpy may draw other batches."""
+    rng = np.random.Generator(np.random.Philox(key=int(seed), counter=np.array([0, 0, int(epoch), int(step)], np.uint64)))
+    cutmix = rng.random() < 0.5 if (mixup_alpha > 0 and cutmix_alpha > 0) else cutmix_alpha > 0
+    alpha = cutmix_alpha if cutmix else mixup_alpha
+    lam = float(rng.beta(alpha, alpha))
+    if not cutmix:
+        return "mixup", lam, None, None
+    r_x, r_y = int(rng.integers(W)), int(rng.integers(H))
+    r = 0.5 * math.sqrt(1.0 - lam)
+    r_w_half, r_h_half = int(r * W), int(r * H)
+    x1, y1 = max(r_x - r_w_half, 0), max(r_y - r_h_half, 0)
+    x2, y2 = min(r_x + r_w_half, W), min(r_y + r_h_half, H)
+    return "cutmix", lam, (x1, y1, x2, y2), float(1.0 - (x2 - x1) * (y2 - y1) / (W * H))
 
 
 class ConvPlan:
@@ -1091,10 +1148,21 @@ class ImageBatcher:
                 net.forward(*batcher.batch(s)); net.backward(); net.sgd(lr)
         net.forward(*test_batcher.batch(0, training=False), training=False)
 
-    batch(step, training=False) is the eval path: identity order, no crop and no flip."""
+    batch(step, training=False) is the eval path: identity order, no crop and no flip.
+
+    mixup_alpha / cutmix_alpha > 0 mix every training batch (pcnn_augment_mix_u8_bf16) with the MixUp or CutMix that
+    mix_draws(seed, epoch, step, ...) picks, and batch(step) then returns (x pointer, MixedLabels), the batcher owning labels_b;
+    softmax_ce_soft_bf16 takes those targets.  Both 0 (the default) is the plain batcher, bit for bit."""
 
     def __init__(self, engine, images, labels, N, pad=0, flip=False, shuffle=True, seed=0, mean=None, std=None, C_out=None,
-                 row_pitch=0, image_rows=0):
+                 row_pitch=0, image_rows=0, mixup_alpha=0.0, cutmix_alpha=0.0):
+        for name, a in (("mixup_alpha", mixup_alpha), ("cutmix_alpha", cutmix_alpha)):
+            if not (isinstance(a, (int, float, np.integer, np.floating)) and math.isfinite(a) and a >= 0):
+                raise PcnnError("ImageBatcher", -1, f"{name} = {a}: a finite alpha >= 0 is required")
+        self.mixup_alpha, self.cutmix_alpha = float(mixup_alpha), float(cutmix_alpha)
+        self.mixing = self.mixup_alpha > 0 or self.cutmix_alpha > 0
+        if self.mixing and labels is None:
+            raise PcnnError("ImageBatcher", -1, "mixup_alpha or cutmix_alpha > 0 needs labels to mix")
         shape = tuple(int(d) for d in images.shape)
         if len(shape) not in (3, 4):
             raise PcnnError("ImageBatcher", -1, f"images must be [n][H][W] or [n][H][W][C], got shape {shape}")
@@ -1114,22 +1182,31 @@ class ImageBatcher:
         self.labels = engine.to_device(np.asarray(labels, np.uint8)) if isinstance(labels, np.ndarray) else labels
         self.x = engine.array((self.N, self.info["image_rows"], self.info["row_pitch"]), np.uint16)    # zeroed: the pad stays 0
         self.labels_out = engine.array((self.N,), np.uint8) if labels is not None else None
+        self.labels_b = engine.array((self.N,), np.uint8) if self.mixing else None
         self.steps_per_epoch = self.n // self.N
         self.epoch = 0
 
     def batch(self, step, training=True):
-        """(x pointer, labels) of batch `step` of epoch self.epoch: positions step N .. step N + N - 1"""
+        """(x pointer, labels) of batch `step` of epoch self.epoch: positions step N .. step N + N - 1; a mixing batcher's training
+        batches return (x pointer, MixedLabels)"""
         if not 0 <= int(step) < self.steps_per_epoch:
             raise PcnnError("ImageBatcher.batch", -1, f"step = {step}: 0 <= step < steps_per_epoch = {self.steps_per_epoch} is required")
         aug = bool(training)
-        self.engine.augment(self.images, self.labels, self.n, self.H, self.W, self.C, int(step) * self.N, self.N, self.x, self.labels_out,
-                            shuffle=int(aug and self.shuffle), pad=self.pad if aug else 0, flip=int(aug and self.flip), seed=self.seed,
-                            epoch=self.epoch, mean=self.mean, std=self.std, C_out=self.C_out, row_pitch=self.info["row_pitch"],
-                            image_rows=self.info["image_rows"])
-        return self.x.ptr, self.labels_out
+        args = (self.images, self.labels, self.n, self.H, self.W, self.C, int(step) * self.N, self.N, self.x, self.labels_out)
+        kw = dict(shuffle=int(aug and self.shuffle), pad=self.pad if aug else 0, flip=int(aug and self.flip), seed=self.seed,
+                  epoch=self.epoch, mean=self.mean, std=self.std, C_out=self.C_out, row_pitch=self.info["row_pitch"],
+                  image_rows=self.info["image_rows"])
+        if not (aug and self.mixing):
+            self.engine.augment(*args, **kw)
+            return self.x.ptr, self.labels_out
+        kind, lam, box, lam_adjusted = mix_draws(self.seed, self.epoch, step, self.H, self.W, self.mixup_alpha, self.cutmix_alpha)
+        weight = lam if kind == "mixup" else lam_adjusted
+        self.engine.augment_mix(*args, labels_b_out=self.labels_b, mode=MIX_MIXUP if kind == "mixup" else MIX_CUTMIX, lam=weight,
+                                box=box or (0, 0, 0, 0), **kw)
+        return self.x.ptr, MixedLabels(self.labels_out, self.labels_b, weight, kind, box)
 
     def close(self):
-        for a in (self.x, self.labels_out):
+        for a in (self.x, self.labels_out, self.labels_b):
             if a is not None:
                 a.free()
 

@@ -1292,6 +1292,97 @@ def run_augment(name, N, H, W, C, C_out, pad, iters, batches=4, row_pitch=0, ima
           flush=True)
 
 
+def run_augment_mix(name, N, H, W, C, C_out, pad, iters, batches=4, row_pitch=0, image_rows=0, rounds=3):
+    """one mixed batch (pcnn_augment_mix_u8_bf16) in each mode against the plain batch (pcnn_augment_u8_bf16) of the same shape,
+    and torchvision's v2.MixUp / v2.CutMix on torch's eager fp32 batch (tests/mix_ref.py's torch_f32_batch, then the cast),
+    alternated over `rounds` rounds (the best of each kept).  Bytes: MixUp reads 2 N H W C, CutMix and the plain call N H W C;
+    each writes N H W C_out 2."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import augment_ref as A
+    from mix_ref import torch_f32_batch
+    from torchvision.transforms import v2
+    n = N * batches
+    images = torch.randint(0, 256, (n, H, W, C), dtype=torch.uint8, device="cuda")
+    labels = torch.randint(0, 10, (n,), dtype=torch.uint8, device="cuda")
+    mean, std = ((0.485, 0.456, 0.406), (0.229, 0.224, 0.225)) if C == 3 else (None, None)
+    info, _ = pkg.augment_info(n, H, W, C, 0, N, 1, pad, 1, C_out, row_pitch, image_rows, mean, std)
+    x = torch.empty(N * info["image_rows"] * info["row_pitch"], dtype=torch.int16, device="cuda")
+    lo, lb = torch.empty(N, dtype=torch.uint8, device="cuda"), torch.empty(N, dtype=torch.uint8, device="cuda")
+    steps = iter(range(1 << 40))
+    seed, epoch, lam = 11, 3, 0.37
+    box = (W // 4, H // 4, W - W // 4, H - H // 4)
+    kw = dict(shuffle=1, pad=pad, flip=1, seed=seed, epoch=epoch, mean=mean, std=std, C_out=C_out, row_pitch=row_pitch,
+              image_rows=image_rows)
+    first = lambda: (next(steps) % batches) * N
+    plain = lambda: eng.augment(images, labels, n, H, W, C, first(), N, x, lo, **kw)
+    mix = {mode: (lambda mode=mode: eng.augment_mix(images, labels, n, H, W, C, first(), N, x, lo, lb, mode=mode, lam=lam, box=box, **kw))
+           for mode in (pkg.MIX_MIXUP, pkg.MIX_CUTMIX)}
+    draws = []
+    for b in range(batches):
+        i = A.indices(n, b * N, N, 1, seed, epoch)
+        oy, ox, fl = A.draws(i.astype(np.uint64), pad, 1, seed, epoch)
+        draws.append((i, oy, ox, fl))
+    tv = {pkg.MIX_MIXUP: v2.MixUp(alpha=1.0, num_classes=10), pkg.MIX_CUTMIX: v2.CutMix(alpha=1.0, num_classes=10)}
+    tv[pkg.MIX_MIXUP].make_params = lambda flat: dict(lam=lam)
+    tv[pkg.MIX_CUTMIX].make_params = lambda flat: dict(box=box, lam_adjusted=lam)
+    tsteps = iter(range(1 << 40))
+
+    def theirs(mode):
+        i, oy, ox, fl = draws[next(tsteps) % batches]
+        out, y = tv[mode](torch_f32_batch(images, i, oy, ox, fl, pad, mean, std), labels[torch.as_tensor(i, device="cuda")].long())
+        return out.permute(0, 2, 3, 1).to(torch.bfloat16), y
+
+    gpu, power = card()
+    for mode, kind in ((pkg.MIX_MIXUP, "MixUp"), (pkg.MIX_CUTMIX, "CutMix")):
+        best = None
+        for _ in range(rounds):
+            r = (timed(mix[mode], iters), timed(plain, iters), timed(lambda: theirs(mode), iters))
+            best = r if best is None else tuple(min(a, b) for a, b in zip(r, best))
+        ms, ms_plain, ms_torch = best
+        nbytes = N * H * W * C * (2 if mode == pkg.MIX_MIXUP else 1) + N * H * W * C_out * 2 + 3 * N
+        print(json.dumps({"case": f"augment-mix {kind} {name}", "N": N, "n": n, "pad": pad, "us": ms * 1e3, "plain_us": ms_plain * 1e3,
+                          "mix_over_plain": ms / ms_plain, "MB": nbytes / 1e6, "hbm_frac": nbytes / (ms * 1e-3) / 1e9 / HBM,
+                          "torchvision_us": ms_torch * 1e3, "torchvision_over_ours": ms_torch / ms, "vec": info["vec"], "grid": info["grid"],
+                          "gpu": gpu, "power_limit": power}), flush=True)
+
+
+def run_resnetgap_mix(iters, rounds=3):
+    """one training step of the GAP ResNet at N = 128 fed by pkg.ImageBatcher with shuffle, pad 2, mixup_alpha 0.2 and
+    cutmix_alpha 1.0 and trained against the soft target (label smoothing 0.1), against the same step on the plain batcher with the
+    hard loss, alternated over `rounds` rounds (the best of each kept)"""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from example_nets import ResNetGAP
+
+    class MixedResNetGAP(ResNetGAP):                                   # the soft loss over the network's z, as test_mix_gpu's
+        def forward(self, x, t, training=True):
+            super().forward(x, t.labels, training)
+            self.eng.softmax_ce_soft_bf16(self.z, t.labels, self.NB, 10, 1.0 / self.NB, self.dz, self.loss, self.pred, labels_b=t.labels_b,
+                                          lam=t.lam, smoothing=0.1)
+    g = np.load(os.path.join(ROOT, "tests", "golden", "mnist_subset.npz"))
+    make = lambda **k: pkg.ImageBatcher(eng, g["train_u8"].reshape(-1, 28, 28), g["train_labels"], ResNetGAP.NB, pad=2, shuffle=True,
+                                        seed=5, row_pitch=32, image_rows=28, **k)
+    plain_b, mix_b = make(), make(mixup_alpha=0.2, cutmix_alpha=1.0)
+    plain_net, mix_net = ResNetGAP(eng, pkg, ResNetGAP.init_params()), MixedResNetGAP(eng, pkg, ResNetGAP.init_params())
+    k = iter(range(1 << 40))
+
+    def step(net, batcher):
+        net.forward(*batcher.batch(next(k) % batcher.steps_per_epoch))
+        net.backward()
+        net.sgd(ResNetGAP.LR_STEP)
+
+    gpu, power = card()
+    best = None
+    for _ in range(rounds):
+        r = (timed(lambda: step(mix_net, mix_b), iters), timed(lambda: step(plain_net, plain_b), iters))
+        best = r if best is None else tuple(min(a, b) for a, b in zip(r, best))
+    ms_mix, ms_plain = best
+    print(json.dumps({"case": f"GAP ResNet training step N={ResNetGAP.NB}, mixed batch + soft loss vs plain batch + hard loss",
+                      "ms_mix": ms_mix, "ms_plain": ms_plain, "mix_over_plain": ms_mix / ms_plain, "gpu": gpu, "power_limit": power}),
+          flush=True)
+    for a in (plain_b, mix_b, plain_net, mix_net):
+        a.close()
+
+
 def run_resnetgap_augment(iters, rounds=3):
     """one training step of the GAP ResNet of tests/example_nets.py at N = 128 on the 1024 golden digits, its batch built
     by pkg.ImageBatcher (shuffle, random crop of pad 2) against the same step on a slice of the pre-converted mnist_device rows,
@@ -1493,6 +1584,14 @@ if only == "augment":                                                  # the inp
     run_augment("224x224x3 -> 8", 256, 224, 224, 3, 8, 4, 20)
 if only == "resnetgap-augment":                                        # the GAP ResNet step fed by the batcher vs the pre-converted slice
     run_resnetgap_augment(20)
+if only == "augment-mix":                                              # mixed batches vs the plain batch and torchvision
+    run_augment_mix("28x28x1 -> [28][32]", 1024, 28, 28, 1, 1, 2, 50, row_pitch=32, image_rows=28)
+    run_augment_mix("32x32x3 -> 3", 512, 32, 32, 3, 3, 4, 50)
+    run_augment_mix("32x32x3 -> 8", 512, 32, 32, 3, 8, 4, 50)
+    run_augment_mix("64x64x3 -> 8", 256, 64, 64, 3, 8, 4, 50)
+    run_augment_mix("224x224x3 -> 8", 256, 224, 224, 3, 8, 4, 20)
+if only == "resnetgap-mix":                                            # the GAP ResNet step, mixed + soft loss vs plain + hard loss
+    run_resnetgap_mix(20)
 if only == "mbconvdrop":                                               # the MBConv step with stochastic depth against the fused residual
     run_mbconv(128, 20, drop_p=0.2)
 if only == "bn":                                                       # batch normalization passes, torch beside them

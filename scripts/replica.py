@@ -11,6 +11,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 F = torch.nn.functional
 AUG_SEED, AUG_PAD = 0x0123456789ABCDEF, 2       # tests/test_augment_gpu.py
+MIX_ALPHAS, MIX_EPS = (0.2, 1.0), 0.1           # tests/test_mix_gpu.py: mixup_alpha, cutmix_alpha and label smoothing
 
 
 def golden():
@@ -30,14 +31,16 @@ def batch_norm(state, v, training):
     return F.batch_norm(v, rm, rv, ga, be, training=training, momentum=0.1, eps=1e-5)
 
 
-def run(net, params, lr, epochs, NB, head="sgd ", optim="sgd", augment=False):
+def run(net, params, lr, epochs, NB, head="sgd ", optim="sgd", augment=False, mix=False):
     """net(x, training) trained for `epochs` epochs of the 1024 golden training digits in order, NB per batch, with softmax
     cross-entropy over the batch and an optimizer step on params, then evaluated on the 256 golden test digits; prints the mean
     loss of the first and last epoch and the accuracy after `head`.
       optim    sgd: plain SGD (the layers' own sgd(lr)); momentum: torch.optim.SGD with momentum 0.9 and weight decay 5e-4;
                adamw: torch.optim.AdamW with betas (0.9, 0.999), eps 1e-8 and weight decay 1e-2
       augment  each epoch's batches as pkg.ImageBatcher draws them with a shuffle and a random crop of pad 2, no flip, at the seed
-               of tests/test_augment_gpu.py, replayed by tests/augment_ref.py"""
+               of tests/test_augment_gpu.py, replayed by tests/augment_ref.py
+      mix      augment's batches, each mixed as an ImageBatcher with MIX_ALPHAS mixes it (tests/mix_ref.py), trained against
+               the soft target of pcnn_softmax_ce_soft_bf16 with label smoothing MIX_EPS"""
     torch.manual_seed(0)
     g, xs, ys, xt, yt = golden()
     opt = {"sgd": lambda: torch.optim.SGD(params, lr=lr),
@@ -47,7 +50,15 @@ def run(net, params, lr, epochs, NB, head="sgd ", optim="sgd", augment=False):
     losses = []
     for ep in range(epochs):
         for s in range(steps):
-            if augment:
+            if mix:
+                import mix_ref
+                kind, _, box, lam, _ = mix_ref.draws(AUG_SEED, ep, s, 28, 28, *MIX_ALPHAS)
+                mode = mix_ref.MIXUP if kind == "mixup" else mix_ref.CUTMIX
+                xb, lab, lab_b = mix_ref.batch(g["train_u8"].reshape(-1, 28, 28, 1), s * NB, NB, mode, lam, box or (0, 0, 0, 0), 1,
+                                               AUG_PAD, 0, AUG_SEED, ep, labels=g["train_labels"])
+                x = torch.from_numpy((xb.astype(np.uint32) << 16).view(np.float32).reshape(NB, 1, 28, 28))
+                y = torch.from_numpy(mix_ref.soft_target(lab, lab_b, lam, MIX_EPS, 10)[1])
+            elif augment:
                 import augment_ref
                 xb, lab, *_ = augment_ref.batch(g["train_u8"].reshape(-1, 28, 28, 1), s * NB, NB, 1, AUG_PAD, 0, AUG_SEED, ep,
                                                 labels=g["train_labels"])
