@@ -843,6 +843,64 @@ int pcnn_augment_mix_u8_bf16(pcnn_ctx *ctx, const uint8_t *images_dev, const uin
                              long long first, int N, int shuffle, int pad, int flip, unsigned long long seed, unsigned long long epoch,
                              const float *mean_host, const float *std_host, void *x_bf16_dev, int C_out, int row_pitch, int image_rows,
                              uint8_t *labels_out_dev, int mode, double lam, int x1, int y1, int x2, int y2, uint8_t *labels_b_out_dev);
+/* Resized batches (csrc/augment.cu): pcnn_augment_u8_bf16's batch at an output size H_out x W_out of its own, with torchvision's
+ * RandomResizedCrop((H_out, W_out), scale, ratio, antialias = True) + RandomHorizontalFlip (mode 1, train) or Resize(resize_size) +
+ * CenterCrop((H_out, W_out)) (mode 2, eval) on the uint8 image, then the plain call's table v(c, u).  No padding argument.
+ *   - Layouts, labels, the permutation pi, the table and channels C <= c < C_out: as pcnn_augment_u8_bf16, with H_out x W_out
+ *     pixels per image in x (row_pitch 0 = W_out C_out rounded up to 8, otherwise a multiple of 8 >= W_out C_out; image_rows 0 =
+ *     H_out, otherwise >= H_out).  flip_i is the plain call's bit, w.z >> 31 of image i's crop block, so a resized batch flips the
+ *     same images as a plain batch of the same (seed, epoch); flip applies in both modes.
+ *   - Box (mode 1): torchvision's get_params.  Box block k of image i is Philox4x32-10 at counter (i lo, 0xC0000000 | (8 + k) << 24 |
+ *     i hi, epoch lo, epoch hi), key (seed lo, seed hi).  Attempt t = 0..9 takes words (x, y) of block t / 2 for even t, (z, w)
+ *     for odd t, as (u_s, u_l); U(u) = RN(RN(RN(float(u >> 8) * 2^-24) * range) + low) in fp32:
+ *       s = U(u_s) over (RN32(s0), RN32(RN32(s1) - RN32(s0))), lr = U(u_l) over (L0, RN32(L1 - L0)), L = RN32(log(RN32(r))) on the host;
+ *       aspect = double(E(lr)), E the replayable fp32 exponential of the SiLU activations (csrc/pcnn_internal.h exp_f32);
+ *       ta = double(H W) * double(s); w = rint(sqrt(ta * aspect)), h = rint(sqrt(ta / aspect)), IEEE double, rint half to even.
+ *     The first attempt with 0 < w <= W and 0 < h <= H gives the box, with top = umulhi(b.x, H - h + 1) and left = umulhi(b.y,
+ *     W - w + 1) of block 5.  With none: torchvision's central crop (W / H < r0: w = W, h = rint(W / r0); W / H > r1: h = H,
+ *     w = rint(H r1); else the image), top = (H - h) / 2, left = (W - w) / 2.  The box is resampled to H_out x W_out.
+ *     Domains: word 1 of a box counter is >= 0xC8000000, above every permutation round's (0xC0000000 | r, r < 6); a crop counter has
+ *     bit 30 clear (i < 2^62) and a dropout counter bit 31 clear, so no box draw coincides with any of them for any seed or epoch.
+ *   - Window (mode 2): the image is resampled to Rh x Rw, the shorter side resize_size and the longer int(resize_size long / short)
+ *     (double quotient).  Per axis of resized size R and crop c, the window starts at int(round((R - c) / 2)) (half to even) when
+ *     c <= R, else at -((c - R) / 2): positions outside the resized image take the byte 0, as CenterCrop pads.  Only the window's
+ *     rows and columns are computed.
+ *   - Resample (torch's uint8 bilinear antialias, PIL-SIMD's fixed point): separable, horizontal pass to a uint8 intermediate, then
+ *     vertical.  An in -> out axis: scale = in / out, support = max(scale, 1), invscale = scale >= 1 ? 1 / scale : 1, taps =
+ *     2 ceil(support) + 1; for output o: centre = scale (o + 0.5), xmin = max(int(centre - support + 0.5), 0), n = clamp(min(int(
+ *     centre + support + 0.5), in) - xmin, 0, taps); tap j < n weighs max(0, 1 - |(j + xmin - centre + 0.5) invscale|), then
+ *     each is divided by their sum (unless it is 0), all in double with no contraction.  prec = the first p in 0..21 with
+ *     int(0.5 + wmax 2^(p+1)) >= 2^15, else 22, wmax the largest weight over every output of the axis (the whole resized axis
+ *     in mode 2); weights become int(w 2^prec + 0.5).  Output = clamp((2^(prec-1) + sum_j w_j src[xmin + j]) >> prec, 0, 255) in
+ *     int32.  An axis whose size does not change gives its input unchanged.
+ *   - x[j][h][w][c] = v(c, u), u the resampled byte at (h, w'), w' = flip_i ? W_out - 1 - w : w.
+ * Domain (PCNN_ERR_ARG, in this order, with the function and the rule in the message): ctx, images and x not NULL; labels and
+ * labels_out both NULL or neither; n, N, H, W, H_out, W_out >= 1; 0 <= first and first + N <= n; n <= 2^56; 1 <= C <= 4;
+ * C <= C_out <= 8; shuffle and flip 0 or 1; mode 1 or 2; H W C < 2^31; n H W C < 2^62; H_out, W_out <= 16384; row_pitch,
+ * image_rows and the x size as above; mean finite; std finite and > 0.  Mode 1: s0, s1, r0, r1 each within fp32's normal range
+ * [2^-126, 3.4028235e38] (so finite and > 0), s0 <= s1 and r0 <= r1 (torchvision only warns); the central fallback crop not empty.
+ * s1 > 1 is allowed: attempts that do not fit fall back.  resize_size is ignored.  Mode 2: 1 <= resize_size <= 16384 and the
+ * longer resized side <= 16384; scale and ratio are ignored.  Both: the worst-case box, the whole image resampled to H_out x W_out
+ * (mode 1) or Rh x Rw (mode 2), needs at most 33 taps per axis (a downscale of at most 16x); one output row of it fits the dynamic
+ * shared memory a launch gets without an opt-in: 48 KB less the kernel's static shared memory (2,224 bytes, out21[20]).  Then x 16-byte aligned, and the plain call's overlap rules.
+ * Kernel: a CTA of 256 threads per (batch position, block of rows_per_cta output rows), rows_per_cta the largest <= min(H_out, 32)
+ * whose worst-case dynamic shared memory (tap tables of W_out columns and of its rows, and an intermediate of rows_cap source rows x
+ * W_out x C bytes) fits that budget.  Thread 0 walks pi and draws the box; the CTA finds both axes' wmax, builds its int16 taps, runs the
+ * horizontal pass over the source rows its rows reach and the vertical pass with flip and table, writing 16-byte vectors when
+ * W_out C_out % 8 == 0.  Stream-ordered; no atomics; the launch depends on the shape alone.
+ * pcnn_augment_resized_u8_bf16_info: host only, refused as the call refuses.  out21 = { row_pitch, image_rows, b, vec, grid,
+ * rows_per_cta, row_blocks, threads, dynamic shared bytes, taps_y, taps_x, rows_cap, Rh, Rw, window top, window left, fallback
+ * top, left, height, width, static shared bytes } (Rh, Rw = H_out, W_out and the window at 0 in mode 1; the fallback 0 in mode 2); lut_out as the plain
+ * info's. */
+int pcnn_augment_resized_u8_bf16(pcnn_ctx *ctx, const uint8_t *images_dev, const uint8_t *labels_dev, long long n, int H, int W, int C,
+                                 long long first, int N, int shuffle, int flip, unsigned long long seed, unsigned long long epoch,
+                                 const float *mean_host, const float *std_host, void *x_bf16_dev, int H_out, int W_out, int C_out,
+                                 int row_pitch, int image_rows, uint8_t *labels_out_dev, int mode, double scale_lo, double scale_hi,
+                                 double ratio_lo, double ratio_hi, int resize_size);
+int pcnn_augment_resized_u8_bf16_info(long long n, int H, int W, int C, long long first, int N, int shuffle, int flip, int H_out,
+                                      int W_out, int C_out, int row_pitch, int image_rows, const float *mean_host, const float *std_host,
+                                      int mode, double scale_lo, double scale_hi, double ratio_lo, double ratio_hi, int resize_size,
+                                      long long *out21, uint16_t *lut_out);
 /* Softmax cross-entropy on bf16 logits [N][O], 1 <= O <= 256, labels uint8 [N]:
  *   p = softmax(row) evaluated in double: m = max, den = sum exp(z - m), p_t = exp(z_t - m) / den;
  *   dlogits[n][t] = bf16_rn(float_rn((p_t - [t == label]) * scale)), double -> fp32 -> bf16, each round to nearest even: the

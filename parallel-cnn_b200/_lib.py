@@ -187,6 +187,10 @@ _SIG = {
     "pcnn_augment_u8_bf16_info": [C.c_longlong, _i, _i, _i, C.c_longlong, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp],
     "pcnn_augment_mix_u8_bf16": [_vp, _vp, _vp, C.c_longlong, _i, _i, _i, C.c_longlong, _i, _i, _i, _i, C.c_ulonglong, C.c_ulonglong,
                                  _vp, _vp, _vp, _i, _i, _i, _vp, _i, C.c_double, _i, _i, _i, _i, _vp],
+    "pcnn_augment_resized_u8_bf16": [_vp, _vp, _vp, C.c_longlong, _i, _i, _i, C.c_longlong, _i, _i, _i, C.c_ulonglong, C.c_ulonglong,
+                                     _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _i, C.c_double, C.c_double, C.c_double, C.c_double, _i],
+    "pcnn_augment_resized_u8_bf16_info": [C.c_longlong, _i, _i, _i, C.c_longlong, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _i,
+                                          C.c_double, C.c_double, C.c_double, C.c_double, _i, _vp, _vp],
     "pcnn_softmax_ce_bf16": [_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp],
     "pcnn_softmax_ce_soft_bf16": [_vp, _vp, _vp, _vp, C.c_double, C.c_double, _i, _i, _f, _vp, _vp, _vp],
     "pcnn_optim_create": [_vp, _vp, _vp, _i, _pvp],
@@ -425,6 +429,32 @@ def augment_info(n, H, W, C, first, N, shuffle=1, pad=0, flip=0, C_out=None, row
         lut.ctypes.data if 1 <= Cin <= 4 else None))
     keys = ("row_pitch", "image_rows", "b", "vec", "grid", "rows_per_cta", "row_blocks", "threads")
     return dict(zip(keys, list(out))), lut
+
+
+RESIZE_TRAIN, RESIZE_EVAL = 1, 2        # pcnn_augment_resized_u8_bf16's modes
+
+
+def augment_resized_info(n, H, W, C, first, N, H_out, W_out, mode=RESIZE_TRAIN, scale=(0.08, 1.0), ratio=(3 / 4, 4 / 3), resize_size=0,
+                         shuffle=1, flip=0, C_out=None, row_pitch=0, image_rows=0, mean=None, std=None):
+    """The layout, launch, resized size, window, fallback box and value table of a resized batch (pcnn_augment_resized_u8_bf16_info;
+    host only, no GPU), refused as pcnn_augment_resized_u8_bf16 refuses.  Returns (info, lut): info holds augment_info's keys plus
+    smem (dynamic shared bytes per CTA), taps_y, taps_x, rows_cap, Rh, Rw (the resized image), ty, tx (the window's offset in it)
+    fallback (top, left, height, width) and static_smem (the kernel's static shared bytes; smem + static_smem <= 48 KB)."""
+    Cin = int(C)
+    C_out = Cin if C_out is None else int(C_out)
+    m, s = channel_stats(mean, Cin, "mean"), channel_stats(std, Cin, "std")
+    out = (_ll * 21)()
+    lut = np.zeros((max(Cin, 1), 256), np.uint16)
+    check("pcnn_augment_resized_u8_bf16_info", lib().pcnn_augment_resized_u8_bf16_info(
+        int(n), int(H), int(W), Cin, int(first), int(N), int(shuffle), int(flip), int(H_out), int(W_out), C_out, int(row_pitch or 0),
+        int(image_rows or 0), None if m is None else m.ctypes.data, None if s is None else s.ctypes.data, int(mode), float(scale[0]),
+        float(scale[1]), float(ratio[0]), float(ratio[1]), int(resize_size or 0), out, lut.ctypes.data if 1 <= Cin <= 4 else None))
+    keys = ("row_pitch", "image_rows", "b", "vec", "grid", "rows_per_cta", "row_blocks", "threads", "smem", "taps_y", "taps_x",
+            "rows_cap", "Rh", "Rw", "ty", "tx")
+    info = dict(zip(keys, list(out)[:16]))
+    info["fallback"] = tuple(out[16:20])
+    info["static_smem"] = out[20]
+    return info, lut
 
 
 def conv_bwd_plan_info(N, H, W, C, K, R, S, stride=1):

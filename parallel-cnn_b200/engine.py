@@ -7,7 +7,7 @@ from typing import NamedTuple, Optional
 import numpy as np
 
 from ._lib import (F32, NPARAM, OPTIM_ADAMW, OPTIM_SGD, TEST_SET, TRAIN_SET, U8, OptimConfig, OptimTensor, PcnnError, augment_info,
-                   avgpool_nhwc_info, batchnorm_nhwc_info, channel_stats, check, conv_layer_family, dropout_info, dwconv_info, gconv_info, global_avgpool_nhwc_info, lib, linear_info,
+                   augment_resized_info, RESIZE_TRAIN, RESIZE_EVAL, avgpool_nhwc_info, batchnorm_nhwc_info, channel_stats, check, conv_layer_family, dropout_info, dwconv_info, gconv_info, global_avgpool_nhwc_info, lib, linear_info,
                    maxpool_nhwc_info,
                    se_scale_nhwc_info, ACT_RELU, ACT_SIGMOID, ACT_SILU, ACT_HARDSWISH, ACT_RELU6)
 
@@ -579,6 +579,19 @@ class Engine:
                    int(pad), int(flip), int(seed), int(epoch), None if m is None else m.ctypes.data, None if s is None else s.ctypes.data,
                    _p(x), Cin if C_out is None else int(C_out), int(row_pitch or 0), int(image_rows or 0), _p(labels_out), int(mode),
                    float(lam), x1, y1, x2, y2, _p(labels_b_out))
+
+    def augment_resized(self, images, labels, n, H, W, C, first, N, x, H_out, W_out, labels_out=None, mode=RESIZE_TRAIN,
+                        scale=(0.08, 1.0), ratio=(3 / 4, 4 / 3), resize_size=0, shuffle=1, flip=0, seed=0, epoch=0, mean=None, std=None,
+                        C_out=None, row_pitch=0, image_rows=0):
+        """pcnn_augment_resized_u8_bf16: augment's batch at H_out x W_out pixels per image.  mode RESIZE_TRAIN:
+        RandomResizedCrop((H_out, W_out), scale, ratio, antialias=True), then the flip when flip; RESIZE_EVAL: Resize(resize_size)
+        + CenterCrop((H_out, W_out)).  Both resample as torch's uint8 bilinear antialiased resize, then (u / 255 - mean) / std."""
+        Cin = int(C)
+        m, s = channel_stats(mean, Cin, "mean"), channel_stats(std, Cin, "std")
+        self._call("pcnn_augment_resized_u8_bf16", _p(images), _p(labels), int(n), int(H), int(W), Cin, int(first), int(N), int(shuffle),
+                   int(flip), int(seed), int(epoch), None if m is None else m.ctypes.data, None if s is None else s.ctypes.data, _p(x),
+                   int(H_out), int(W_out), Cin if C_out is None else int(C_out), int(row_pitch or 0), int(image_rows or 0), _p(labels_out),
+                   int(mode), float(scale[0]), float(scale[1]), float(ratio[0]), float(ratio[1]), int(resize_size or 0))
 
 
 class MixedLabels(NamedTuple):
@@ -1152,10 +1165,16 @@ class ImageBatcher:
 
     mixup_alpha / cutmix_alpha > 0 mix every training batch (pcnn_augment_mix_u8_bf16) with the MixUp or CutMix that
     mix_draws(seed, epoch, step, ...) picks, and batch(step) then returns (x pointer, MixedLabels), the batcher owning labels_b;
-    softmax_ce_soft_bf16 takes those targets.  Both 0 (the default) is the plain batcher, bit for bit."""
+    softmax_ce_soft_bf16 takes those targets.  Both 0 (the default) is the plain batcher, bit for bit.
+
+    crop_size (an int or (h, w)) resizes (pcnn_augment_resized_u8_bf16): training batches take torchvision's
+    RandomResizedCrop(crop_size, scale, ratio, antialias=True) and the flip, eval batches Resize(resize_size) +
+    CenterCrop(crop_size), resize_size defaulting to the crop's shorter side; x then holds crop_size pixels per image.  It excludes
+    pad > 0 and mixing.  crop_size None (the default) is the plain batcher, bit for bit."""
 
     def __init__(self, engine, images, labels, N, pad=0, flip=False, shuffle=True, seed=0, mean=None, std=None, C_out=None,
-                 row_pitch=0, image_rows=0, mixup_alpha=0.0, cutmix_alpha=0.0):
+                 row_pitch=0, image_rows=0, mixup_alpha=0.0, cutmix_alpha=0.0, crop_size=None, scale=(0.08, 1.0), ratio=(3 / 4, 4 / 3),
+                 resize_size=None):
         for name, a in (("mixup_alpha", mixup_alpha), ("cutmix_alpha", cutmix_alpha)):
             if not (isinstance(a, (int, float, np.integer, np.floating)) and math.isfinite(a) and a >= 0):
                 raise PcnnError("ImageBatcher", -1, f"{name} = {a}: a finite alpha >= 0 is required")
@@ -1163,6 +1182,15 @@ class ImageBatcher:
         self.mixing = self.mixup_alpha > 0 or self.cutmix_alpha > 0
         if self.mixing and labels is None:
             raise PcnnError("ImageBatcher", -1, "mixup_alpha or cutmix_alpha > 0 needs labels to mix")
+        self.crop = None if crop_size is None else tuple(int(v) for v in np.broadcast_to(np.asarray(crop_size).reshape(-1), (2,)))
+        if self.crop is not None and int(pad) > 0:
+            raise PcnnError("ImageBatcher", -1, f"crop_size = {crop_size} with pad = {pad}: a resized batch takes no padding")
+        if self.crop is not None and self.mixing:
+            raise PcnnError("ImageBatcher", -1, f"crop_size = {crop_size} with mixup_alpha or cutmix_alpha > 0: resized batches are not mixed")
+        if self.crop is None and resize_size is not None:
+            raise PcnnError("ImageBatcher", -1, f"resize_size = {resize_size} without crop_size: only a resized batcher resizes")
+        self.scale, self.ratio = (float(scale[0]), float(scale[1])), (float(ratio[0]), float(ratio[1]))
+        self.resize_size = None if self.crop is None else int(min(self.crop) if resize_size is None else resize_size)
         shape = tuple(int(d) for d in images.shape)
         if len(shape) not in (3, 4):
             raise PcnnError("ImageBatcher", -1, f"images must be [n][H][W] or [n][H][W][C], got shape {shape}")
@@ -1173,8 +1201,15 @@ class ImageBatcher:
         self.N, self.pad, self.flip, self.shuffle, self.seed = int(N), int(pad), bool(flip), bool(shuffle), int(seed)
         self.mean, self.std = channel_stats(mean, self.C, "mean"), channel_stats(std, self.C, "std")
         self.C_out = self.C if C_out is None else int(C_out)
-        self.info, self.lut = augment_info(self.n, self.H, self.W, self.C, 0, self.N, int(self.shuffle), self.pad, int(self.flip),
-                                           self.C_out, row_pitch, image_rows, self.mean, self.std)
+        if self.crop is None:
+            self.info, self.lut = augment_info(self.n, self.H, self.W, self.C, 0, self.N, int(self.shuffle), self.pad, int(self.flip),
+                                               self.C_out, row_pitch, image_rows, self.mean, self.std)
+        else:
+            self.info, self.lut = augment_resized_info(self.n, self.H, self.W, self.C, 0, self.N, *self.crop, RESIZE_TRAIN, self.scale,
+                                                       self.ratio, 0, int(self.shuffle), int(self.flip), self.C_out, row_pitch,
+                                                       image_rows, self.mean, self.std)
+            augment_resized_info(self.n, self.H, self.W, self.C, 0, self.N, *self.crop, RESIZE_EVAL, resize_size=self.resize_size,
+                                 C_out=self.C_out, row_pitch=row_pitch, image_rows=image_rows, mean=self.mean, std=self.std)
         if labels is not None and int(labels.shape[0]) != self.n:
             raise PcnnError("ImageBatcher", -1, f"{labels.shape[0]} labels for {self.n} images")
         self.engine = engine
@@ -1196,6 +1231,11 @@ class ImageBatcher:
         kw = dict(shuffle=int(aug and self.shuffle), pad=self.pad if aug else 0, flip=int(aug and self.flip), seed=self.seed,
                   epoch=self.epoch, mean=self.mean, std=self.std, C_out=self.C_out, row_pitch=self.info["row_pitch"],
                   image_rows=self.info["image_rows"])
+        if self.crop is not None:
+            del kw["pad"]
+            self.engine.augment_resized(*args[:9], *self.crop, self.labels_out, mode=RESIZE_TRAIN if aug else RESIZE_EVAL,
+                                        scale=self.scale, ratio=self.ratio, resize_size=self.resize_size, **kw)
+            return self.x.ptr, self.labels_out
         if not (aug and self.mixing):
             self.engine.augment(*args, **kw)
             return self.x.ptr, self.labels_out

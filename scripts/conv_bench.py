@@ -6,6 +6,7 @@ the working set of every measured point except the smallest batches exceeds the 
 import json
 import os
 import sys
+import time
 
 import numpy as np
 import torch
@@ -1418,6 +1419,100 @@ def run_resnetgap_augment(iters, rounds=3):
     net.close()
 
 
+def run_resized(name, N, H, W, C, H_out, W_out, C_out, iters, resize_size, batches=4, row_pitch=0, image_rows=0, rounds=3):
+    """one resized batch (pcnn_augment_resized_u8_bf16) in each mode, RandomResizedCrop (default scale and ratio) + flip and
+    Resize(resize_size) + CenterCrop, against the plain batch (pcnn_augment_u8_bf16, pad 0, flip) of the same output size from a
+    dataset of that size, alternated over `rounds` rounds (the best of each kept); and torchvision's per-image CPU path for the same
+    batch (resized_crop or resize + center_crop, flip, ToTensor + Normalize, bf16), which a data loader would otherwise run, timed
+    once.  Bytes: the source bytes the boxes (or the eval window's preimage) cover, plus N H_out W_out C_out 2 written."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import resize_ref as RR
+    import torchvision.transforms.v2.functional as TF
+    n = N * batches
+    images = torch.randint(0, 256, (n, H, W, C), dtype=torch.uint8, device="cuda")
+    small = torch.randint(0, 256, (n, H_out, W_out, C), dtype=torch.uint8, device="cuda")
+    labels = torch.randint(0, 10, (n,), dtype=torch.uint8, device="cuda")
+    mean, std = ((0.485, 0.456, 0.406), (0.229, 0.224, 0.225)) if C == 3 else (None, None)
+    info, _ = pkg.augment_resized_info(n, H, W, C, 0, N, H_out, W_out, C_out=C_out, row_pitch=row_pitch, image_rows=image_rows)
+    x = torch.empty(N * info["image_rows"] * info["row_pitch"], dtype=torch.int16, device="cuda")
+    lo = torch.empty(N, dtype=torch.uint8, device="cuda")
+    steps = iter(range(1 << 40))
+    seed, epoch = 11, 3
+    kw = dict(flip=1, seed=seed, epoch=epoch, mean=mean, std=std, C_out=C_out, row_pitch=row_pitch, image_rows=image_rows)
+    first = lambda: (next(steps) % batches) * N
+    calls = {m: (lambda m=m: eng.augment_resized(images, labels, n, H, W, C, first(), N, x, H_out, W_out, lo, mode=m, shuffle=int(m == 1),
+                                                 resize_size=resize_size, **kw)) for m in (pkg.RESIZE_TRAIN, pkg.RESIZE_EVAL)}
+    plain = lambda: eng.augment(small, labels, n, H_out, W_out, C, first(), N, x, lo, shuffle=1, pad=0, **kw)
+    host = images[:N].cpu().permute(0, 3, 1, 2).contiguous()
+    i = RR.A.indices(n, 0, N, 1, seed, epoch)
+    box = np.stack(RR.boxes(i.astype(np.uint64), H, W, (0.08, 1.0), (3 / 4, 4 / 3), seed, epoch)[:4], -1)
+    Rh, Rw = RR.resized_size(H, W, resize_size)
+    m_t = torch.tensor(mean or (0.0,) * C).view(-1, 1, 1)
+    s_t = torch.tensor(std or (1.0,) * C).view(-1, 1, 1)
+
+    def torchvision_cpu(mode):
+        t0 = time.perf_counter()
+        for j in range(N):
+            if mode == pkg.RESIZE_TRAIN:
+                t, l, h, w = (int(v) for v in box[j])
+                u = TF.horizontal_flip(TF.resized_crop(host[j], t, l, h, w, [H_out, W_out], antialias=True))
+            else:
+                u = TF.center_crop(TF.resize(host[j], resize_size, antialias=True), [H_out, W_out])
+            ((u.float() / 255.0 - m_t) / s_t).to(torch.bfloat16)
+        return time.perf_counter() - t0
+
+    gpu, power = card()
+    for mode, kind in ((pkg.RESIZE_TRAIN, "RandomResizedCrop"), (pkg.RESIZE_EVAL, f"Resize({resize_size}) + CenterCrop")):
+        best = None
+        for _ in range(rounds):
+            r = (timed(calls[mode], iters), timed(plain, iters))
+            best = r if best is None else tuple(min(a, b) for a, b in zip(r, best))
+        ms, ms_plain = best
+        if mode == pkg.RESIZE_TRAIN:
+            src = int((box[:, 2] * box[:, 3]).sum()) * C
+        else:
+            src = N * min(H, -(-H * H_out // Rh)) * min(W, -(-W * W_out // Rw)) * C
+        nbytes = src + N * H_out * W_out * C_out * 2
+        cpu_s = torchvision_cpu(mode)
+        print(json.dumps({"case": f"resized {kind} {name}", "N": N, "us": ms * 1e3, "plain_us": ms_plain * 1e3,
+                          "resized_over_plain": ms / ms_plain, "MB": nbytes / 1e6, "hbm_frac": nbytes / (ms * 1e-3) / 1e9 / HBM,
+                          "plain_hbm_frac": (N * H_out * W_out * (C + 2 * C_out)) / (ms_plain * 1e-3) / 1e9 / HBM,
+                          "torchvision_cpu_ms": cpu_s * 1e3, "torchvision_cpu_over_ours": cpu_s * 1e3 / ms, "vec": info["vec"],
+                          "grid": info["grid"], "rows_per_cta": info["rows_per_cta"], "smem": info["smem"], "gpu": gpu,
+                          "power_limit": power}), flush=True)
+
+
+def run_resnetgap_resized(iters, rounds=3):
+    """one training step of the GAP ResNet at N = 128 fed by pkg.ImageBatcher with crop_size 28 and scale (0.6, 1.0) (shuffle),
+    against the same step on the plain batcher (shuffle, pad 2), alternated over `rounds` rounds (the best of each kept)"""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from example_nets import ResNetGAP
+    g = np.load(os.path.join(ROOT, "tests", "golden", "mnist_subset.npz"))
+    make = lambda **k: pkg.ImageBatcher(eng, g["train_u8"].reshape(-1, 28, 28), g["train_labels"], ResNetGAP.NB, shuffle=True, seed=5,
+                                        row_pitch=32, image_rows=28, **k)
+    plain_b, res_b = make(pad=2), make(crop_size=28, scale=(0.6, 1.0))
+    net = ResNetGAP(eng, pkg, ResNetGAP.init_params())
+    k = iter(range(1 << 40))
+
+    def step(batcher):
+        net.forward(*batcher.batch(next(k) % batcher.steps_per_epoch))
+        net.backward()
+        net.sgd(ResNetGAP.LR_STEP)
+
+    gpu, power = card()
+    best = None
+    for _ in range(rounds):
+        r = (timed(lambda: step(res_b), iters), timed(lambda: step(plain_b), iters),
+             timed(lambda: res_b.batch(next(k) % res_b.steps_per_epoch), iters))
+        best = r if best is None else tuple(min(a, b) for a, b in zip(r, best))
+    ms_res, ms_plain, ms_batch = best
+    print(json.dumps({"case": f"GAP ResNet training step N={ResNetGAP.NB}, RandomResizedCrop(28) batch vs plain batch (pad 2)",
+                      "ms_resized": ms_res, "ms_plain": ms_plain, "resized_over_plain": ms_res / ms_plain, "batch_us": ms_batch * 1e3,
+                      "gpu": gpu, "power_limit": power}), flush=True)
+    for a in (plain_b, res_b, net):
+        a.close()
+
+
 def run_mbconv(N, iters, hid=16, drop_p=0.0):
     """one training step of an EfficientNet MBConv block with SiLU and squeeze-and-excitation at 28x28x40, N = 128: 1x1 expand to
     240 -> BN + SiLU -> depthwise 5x5 pad 2 -> BN + SiLU -> SE 240 -> hid -> 240 -> 1x1 project to 40 -> BN + x0, its backward (the
@@ -1592,6 +1687,15 @@ if only == "augment-mix":                                              # mixed b
     run_augment_mix("224x224x3 -> 8", 256, 224, 224, 3, 8, 4, 20)
 if only == "resnetgap-mix":                                            # the GAP ResNet step, mixed + soft loss vs plain + hard loss
     run_resnetgap_mix(20)
+if only == "resized":                                                  # resized batches vs the plain batch and torchvision's CPU path
+    run_resized("28x28x1 -> 28 [28][32]", 1024, 28, 28, 1, 28, 28, 1, 50, 28, row_pitch=32, image_rows=28)
+    run_resized("32x32x3 -> 32, 3", 512, 32, 32, 3, 32, 32, 3, 50, 36)
+    run_resized("32x32x3 -> 32, 8", 512, 32, 32, 3, 32, 32, 8, 50, 36)
+    run_resized("64x64x3 -> 56, 8", 256, 64, 64, 3, 56, 56, 8, 50, 64)
+    run_resized("256x256x3 -> 224, 8", 256, 256, 256, 3, 224, 224, 8, 20, 256)
+    run_resized("320x240x3 -> 224, 8", 256, 320, 240, 3, 224, 224, 8, 20, 256)
+if only == "resnetgap-resized":                                        # the GAP ResNet step, resized batch vs plain batch
+    run_resnetgap_resized(20)
 if only == "mbconvdrop":                                               # the MBConv step with stochastic depth against the fused residual
     run_mbconv(128, 20, drop_p=0.2)
 if only == "bn":                                                       # batch normalization passes, torch beside them
