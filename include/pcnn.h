@@ -901,6 +901,71 @@ int pcnn_augment_resized_u8_bf16_info(long long n, int H, int W, int C, long lon
                                       int W_out, int C_out, int row_pitch, int image_rows, const float *mean_host, const float *std_host,
                                       int mode, double scale_lo, double scale_hi, double ratio_lo, double ratio_hi, int resize_size,
                                       long long *out21, uint16_t *lut_out);
+/* TrivialAugmentWide and RandomErasing (csrc/augment.cu): a training batch of torchvision's recipe
+ *   (RandomCrop(pad) | RandomResizedCrop) -> RandomHorizontalFlip -> TrivialAugmentWide -> ToTensor -> Normalize -> RandomErasing,
+ * in two launches, with the uint8 crop in a caller-owned workspace between them.
+ *   - Geometry: resize 0 is pcnn_augment_u8_bf16's crop, pad and flip (an h x w = H x W crop); resize 1 is
+ *     pcnn_augment_resized_u8_bf16's mode 1 box, resample and flip (h x w = H_out x W_out; pad must be 0).  Bit for bit those
+ *     calls' bytes: the same kernels run at C_out = C with the table v(c, u) = u, into workspace [N][h][ws_pitch] uint16 (the
+ *     byte in the low 8 bits; ws_pitch = w C rounded up to 8), at least N h ws_pitch 2 bytes, 16-byte aligned.  Permutation,
+ *     labels_out, layouts of x, the table and channels C <= c < C_out: as pcnn_augment_u8_bf16 with H x W replaced by h x w.
+ *   - Draws of image i: trivial block k is Philox4x32-10 at counter (i lo, 0xC0000000 | (16 + k) << 24 | i hi, epoch lo, epoch hi),
+ *     key (seed lo, seed hi).  Block 0: op = umulhi(x, 14), bin = umulhi(y, 31), sign = z >> 31, erase iff U(w) < RN32(p) with
+ *     U(u) = RN(float(u >> 8) 2^-24).  Blocks 1..5: erase attempts t = 0..9 take words (x, y) of block 1 + t / 2 for even t, (z, w)
+ *     for odd t, as the resized call's box attempts; block 6 the erase box's (top, left) words.  Domains: word 1 of a trivial
+ *     counter is in 0xD0000000 .. 0xD6FFFFFF (i < 2^56): above every box counter (0xC8 .. 0xCD in the top byte) and permutation round
+ *     (0xC0), and with bits 31 and 30 set where a crop counter has bit 30 clear and a dropout counter bit 31 clear.
+ *   - TrivialAugmentWide (trivial 1: NEAREST, 2: BILINEAR; 0: none, op Identity), num_magnitude_bins 31, fill None, on the uint8
+ *     crop [C][h][w], C 1 or 3, as v1 transforms.autoaugment._apply_op on a tensor.  Ops in _augmentation_space's order: 0 Identity,
+ *     1 ShearX, 2 ShearY, 3 TranslateX, 4 TranslateY, 5 Rotate, 6 Brightness, 7 Color, 8 Contrast, 9 Sharpness, 10 Posterize,
+ *     11 Solarize, 12 AutoContrast, 13 Equalize; sign negates the magnitude of ops 1..9.  Magnitudes: torch.linspace's fp32 values
+ *     (0..0.99 for shears and blends, 0..32 for translations, 0..135 for Rotate, 255..0 for Solarize), Posterize 8 - round(bin / 5).
+ *     The host forms a table per (op, bin, sign) for this crop size: for ops 1..5, torchvision's _get_inverse_affine_matrix in double
+ *     (center (-w/2, -h/2) for shears, translate int(m), Rotate's angle -m), each entry rounded to fp32 then divided in fp32 by
+ *     0.5 w (row 0) or 0.5 h (row 1), as _gen_affine_grid rescales theta; ratio = 1 + m and 1 - ratio in double, each rounded to fp32;
+ *     Posterize's mask; Solarize's threshold as the least byte >= it.  RN: fp32 round to nearest, no contraction.
+ *       blend(a, b) = trunc(clamp(RN(RN(r a) + RN(s b)), 0, 255)); gray = trunc(RN(RN(RN(0.2989 R) + RN(0.587 G)) + RN(0.114 B)));
+ *       Brightness blend(u, 0); Color blend(u, gray) (identity at C = 1); Contrast blend(u, mean), mean = RN(S / (h w)), S the exact
+ *       sum of gray (C = 3) or of the bytes (C = 1), exact because h w 255 < 2^24; Sharpness (identity when h or w <= 2)
+ *       blend(u, b), b = rint(acc) inside the border and u on it, acc the RN sum in row-major tap order of RN(k u) with k = RN32(1 / 13)
+ *       and RN32(5 / 13) at the centre; Posterize u & mask; Solarize u >= T ? 255 - u : u; AutoContrast per channel trunc(clamp(RN(
+ *       (u - min) scale), 0, 255)), scale = RN(RN(1 / (max - min)) 255) (min 0, scale 1 on a flat channel); Equalize per channel
+ *       _scale_channel's integer LUT from the histogram (identity when step = 0).
+ *       Geometric ops: output pixel (y, x) takes bx = x + 0.5 - w / 2, by = y + 0.5 - h / 2 (exact), gx = RN(RN(RN(bx v0) +
+ *       RN(by v1)) + v2), gy likewise with v3..v5, ix = RN(RN(RN(gx + 1) (0.5 w)) - 0.5), iy likewise; NEAREST takes the byte at
+ *       (rint(iy), rint(ix)) (half to even), BILINEAR RN(RN(RN(RN(v_nw RN(s e)) + RN(v_ne RN(s w'))) + RN(v_sw RN(n e))) +
+ *       RN(v_se RN(n w'))) with w' = ix - floor(ix), e = 1 - w', n = iy - floor(iy), s = 1 - n, then rint; outside the crop 0.
+ *   - Normalise: the table v(c, u) of pcnn_augment_u8_bf16 on the transformed byte.
+ *   - RandomErasing(p, (es0, es1), (er0, er1), value = 0) when erase_p > 0: attempt t draws s = U over (RN32(es0), RN32(RN32(es1) -
+ *     RN32(es0))) and lr over (L0, RN32(L1 - L0)), L = RN32(log(RN32(r))) as the resized call's box; aspect = double(E(lr));
+ *     ea = double(h w) double(s); eh = rint(sqrt(ea aspect)), ew = rint(sqrt(ea / aspect)) in IEEE double.  The first attempt with
+ *     eh < h and ew < w gives the box, top = umulhi(x, h - eh + 1), left = umulhi(y, w - ew + 1) of block 6; with none, no erase.
+ *     Channels c < C of the box's pixels are bf16 +0.
+ * Domain (PCNN_ERR_ARG, in this order): ctx, images, x and the workspace not NULL; labels and labels_out both NULL or neither;
+ * resize 0 or 1; trivial 0, 1 or 2; C 1 or 3 when trivial > 0; erase_p finite in [0, 1]; when erase_p > 0, 0 <= es0 <= es1 <= 1 and
+ * er0 <= er1 within fp32's normal range; resize 1 with pad 0; then the geometry call's own rules with its messages; then the
+ * output layout as pcnn_augment_u8_bf16's at h x w with C_out; h w <= 65536 (256 x 256, so Contrast's sum stays exact); the crop's
+ * h w C bytes, rounded up to 16, within the 227 KB of shared memory a CTA may opt into less the kernel's static shared memory
+ * (out12[10]): every crop of C <= 3 within 256 x 256 fits, a C = 4 crop (erasing only) up to about 56,800 pixels, so 256 x 256 x 4
+ * is refused; x and the workspace 16-byte aligned; workspace_bytes enough; x, labels_out and
+ * the workspace sharing no byte with each other, the images or the labels.
+ * Kernel: after every check, the geometry call's launch, then one CTA of 512 threads per image (grid min(N, 2^20)) with h w C bytes of dynamic shared
+ * memory; shared integer atomics build the histograms (order-free); no other atomics: reruns give the same bits on every H100.
+ * pcnn_augment_trivial_u8_bf16_info: host only, refused as the call refuses (bar the pointers).  out12 = { row_pitch, image_rows,
+ * h, w, ws_pitch, workspace bytes, vec, grid, threads, dynamic shared bytes, static shared bytes, kernel argument bytes };
+ * table_out, when not NULL, receives the table as float [14][31][2][6]; lut_out as the plain info's. */
+int pcnn_augment_trivial_u8_bf16(pcnn_ctx *ctx, const uint8_t *images_dev, const uint8_t *labels_dev, long long n, int H, int W, int C,
+                                 long long first, int N, int shuffle, int pad, int flip, unsigned long long seed, unsigned long long epoch,
+                                 const float *mean_host, const float *std_host, void *x_bf16_dev, int C_out, int row_pitch, int image_rows,
+                                 uint8_t *labels_out_dev, int resize, int H_out, int W_out, double scale_lo, double scale_hi,
+                                 double ratio_lo, double ratio_hi, int trivial, double erase_p, double erase_scale_lo,
+                                 double erase_scale_hi, double erase_ratio_lo, double erase_ratio_hi, void *workspace_dev,
+                                 long long workspace_bytes);
+int pcnn_augment_trivial_u8_bf16_info(long long n, int H, int W, int C, long long first, int N, int shuffle, int pad, int flip, int resize,
+                                      int H_out, int W_out, double scale_lo, double scale_hi, double ratio_lo, double ratio_hi, int trivial,
+                                      double erase_p, double erase_scale_lo, double erase_scale_hi, double erase_ratio_lo,
+                                      double erase_ratio_hi, int C_out, int row_pitch, int image_rows, const float *mean_host,
+                                      const float *std_host, long long *out12, float *table_out, uint16_t *lut_out);
 /* Softmax cross-entropy on bf16 logits [N][O], 1 <= O <= 256, labels uint8 [N]:
  *   p = softmax(row) evaluated in double: m = max, den = sum exp(z - m), p_t = exp(z_t - m) / den;
  *   dlogits[n][t] = bf16_rn(float_rn((p_t - [t == label]) * scale)), double -> fp32 -> bf16, each round to nearest even: the

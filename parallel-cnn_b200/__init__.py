@@ -14,6 +14,7 @@ from ._lib import (  # noqa: F401
     lib, declared_symbols, init_params_reference, mnist_load_u8, conv_tc_plan_info, conv_wide_plan_info, conv_wide_bwd_info,
     conv_bwd_plan_info, conv_layer_family, maxpool_nhwc_info, avgpool_nhwc_info, global_avgpool_nhwc_info, batchnorm_nhwc_info,
     linear_info, dwconv_info, gconv_info, se_scale_nhwc_info, dropout_info, augment_info, augment_resized_info, RESIZE_TRAIN, RESIZE_EVAL, OPTIM_SGD, OPTIM_ADAMW,
+    augment_trivial_info, TRIVIAL_NONE, TRIVIAL_NEAREST, TRIVIAL_BILINEAR, TRIVIAL_OPS,
 )
 from .engine import AvgPoolLayer, BatchNormLayer, ConvLayer, GlobalAvgPoolLayer, ConvPlan, LinearLayer, LinearPlan, MaxPoolLayer, DeviceArray, WideConvPlan, Engine, bf16_bits_to_f32, f32_to_bf16_bits  # noqa: F401
 from .engine import DepthwiseConvLayer, DepthwiseConvPlan, DropoutLayer, GroupedConvLayer, GroupedConvPlan, SqueezeExcitationLayer  # noqa: F401
@@ -27,4 +28,5 @@ __all__ = ["Engine", "DeviceArray", "PcnnError", "lib", "declared_symbols", "ini
            "SGD", "AdamW", "FusedOptimizer", "OPTIM_SGD", "OPTIM_ADAMW", "dwconv_info", "DepthwiseConvLayer", "DepthwiseConvPlan",
            "gconv_info", "GroupedConvLayer", "GroupedConvPlan", "se_scale_nhwc_info", "SqueezeExcitationLayer",
            "dropout_info", "DropoutLayer", "augment_info", "augment_resized_info", "RESIZE_TRAIN", "RESIZE_EVAL", "ImageBatcher",
-           "MixedLabels", "MIX_MIXUP", "MIX_CUTMIX", "mix_draws"]
+           "MixedLabels", "MIX_MIXUP", "MIX_CUTMIX", "mix_draws", "augment_trivial_info", "TRIVIAL_NONE", "TRIVIAL_NEAREST",
+           "TRIVIAL_BILINEAR", "TRIVIAL_OPS"]

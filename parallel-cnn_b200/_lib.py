@@ -191,6 +191,11 @@ _SIG = {
                                      _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _i, C.c_double, C.c_double, C.c_double, C.c_double, _i],
     "pcnn_augment_resized_u8_bf16_info": [C.c_longlong, _i, _i, _i, C.c_longlong, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _i,
                                           C.c_double, C.c_double, C.c_double, C.c_double, _i, _vp, _vp],
+    "pcnn_augment_trivial_u8_bf16": [_vp, _vp, _vp, C.c_longlong, _i, _i, _i, C.c_longlong, _i, _i, _i, _i, C.c_ulonglong,
+                                     C.c_ulonglong, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _i, _i] + [C.c_double] * 4 + [_i]
+                                    + [C.c_double] * 5 + [_vp, C.c_longlong],
+    "pcnn_augment_trivial_u8_bf16_info": [C.c_longlong, _i, _i, _i, C.c_longlong, _i, _i, _i, _i, _i, _i, _i] + [C.c_double] * 4
+                                         + [_i] + [C.c_double] * 5 + [_i, _i, _i, _vp, _vp, _vp, _vp, _vp],
     "pcnn_softmax_ce_bf16": [_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp],
     "pcnn_softmax_ce_soft_bf16": [_vp, _vp, _vp, _vp, C.c_double, C.c_double, _i, _i, _f, _vp, _vp, _vp],
     "pcnn_optim_create": [_vp, _vp, _vp, _i, _pvp],
@@ -455,6 +460,35 @@ def augment_resized_info(n, H, W, C, first, N, H_out, W_out, mode=RESIZE_TRAIN, 
     info["fallback"] = tuple(out[16:20])
     info["static_smem"] = out[20]
     return info, lut
+
+
+TRIVIAL_NONE, TRIVIAL_NEAREST, TRIVIAL_BILINEAR = 0, 1, 2       # pcnn_augment_trivial_u8_bf16's interpolations
+TRIVIAL_OPS = ("Identity", "ShearX", "ShearY", "TranslateX", "TranslateY", "Rotate", "Brightness", "Color", "Contrast", "Sharpness",
+               "Posterize", "Solarize", "AutoContrast", "Equalize")
+
+
+def augment_trivial_info(n, H, W, C, first, N, trivial=TRIVIAL_NEAREST, erase_p=0.0, erase_scale=(0.02, 0.33), erase_ratio=(0.3, 3.3),
+                         crop_size=None, scale=(0.08, 1.0), ratio=(3 / 4, 4 / 3), shuffle=1, pad=0, flip=0, C_out=None, row_pitch=0,
+                         image_rows=0, mean=None, std=None):
+    """The layout, workspace, launch, magnitude table and value table of a TrivialAugmentWide / RandomErasing batch
+    (pcnn_augment_trivial_u8_bf16_info; host only, no GPU), refused as pcnn_augment_trivial_u8_bf16 refuses.  crop_size None is the
+    plain geometry (pad, flip), (h, w) the resized call's RandomResizedCrop.  Returns (info, table, lut): info holds row_pitch,
+    image_rows, h, w, ws_pitch, ws_bytes, vec, grid, threads, smem, static_smem and arg_bytes; table float32 [14][31][2][6]."""
+    Cin = int(C)
+    C_out = Cin if C_out is None else int(C_out)
+    m, s = channel_stats(mean, Cin, "mean"), channel_stats(std, Cin, "std")
+    out = (_ll * 12)()
+    table = np.zeros((14, 31, 2, 6), np.float32)
+    lut = np.zeros((max(Cin, 1), 256), np.uint16)
+    hw = (0, 0) if crop_size is None else tuple(int(v) for v in crop_size)
+    check("pcnn_augment_trivial_u8_bf16_info", lib().pcnn_augment_trivial_u8_bf16_info(
+        int(n), int(H), int(W), Cin, int(first), int(N), int(shuffle), int(pad), int(flip), int(crop_size is not None), *hw,
+        float(scale[0]), float(scale[1]), float(ratio[0]), float(ratio[1]), int(trivial), float(erase_p), float(erase_scale[0]),
+        float(erase_scale[1]), float(erase_ratio[0]), float(erase_ratio[1]), C_out, int(row_pitch or 0), int(image_rows or 0),
+        None if m is None else m.ctypes.data, None if s is None else s.ctypes.data, out, table.ctypes.data,
+        lut.ctypes.data if 1 <= Cin <= 4 else None))
+    keys = ("row_pitch", "image_rows", "h", "w", "ws_pitch", "ws_bytes", "vec", "grid", "threads", "smem", "static_smem", "arg_bytes")
+    return dict(zip(keys, list(out))), table, lut
 
 
 def conv_bwd_plan_info(N, H, W, C, K, R, S, stride=1):

@@ -22,6 +22,7 @@
 #include <climits>
 #include <cmath>
 #include <cstring>
+#include <memory>
 #include <type_traits>
 
 namespace {
@@ -295,6 +296,15 @@ int aug_shape(const char *fn, long long n, int H, int W, int C, long long first,
     return PCNN_OK;
 }
 
+int aug_launch(pcnn_ctx *ctx, const AugShape &s) {
+    if (s.vec == 8)
+        k_augment<8, MIX_NONE><<<s.grid, AUG_THREADS, 0, ctx->stream>>>(s.a);
+    else
+        k_augment<1, MIX_NONE><<<s.grid, AUG_THREADS, 0, ctx->stream>>>(s.a);
+    PCNN_CHECK_LAUNCH(ctx);
+    return PCNN_OK;
+}
+
 bool aligned16(const void *p) { return ((uintptr_t)p & 15) == 0; }
 
 bool disjoint(const void *a, size_t abytes, const void *b, size_t bbytes) {
@@ -363,12 +373,7 @@ extern "C" int pcnn_augment_u8_bf16(pcnn_ctx *ctx, const uint8_t *images_dev, co
                                mean_host, std_host, x_bf16_dev, C_out, row_pitch, image_rows, labels_out_dev, &s, &xbytes);
     if (rc) return rc;
     pcnn_device_guard dg(ctx->device);
-    if (s.vec == 8)
-        k_augment<8, MIX_NONE><<<s.grid, AUG_THREADS, 0, ctx->stream>>>(s.a);
-    else
-        k_augment<1, MIX_NONE><<<s.grid, AUG_THREADS, 0, ctx->stream>>>(s.a);
-    PCNN_CHECK_LAUNCH(ctx);
-    return PCNN_OK;
+    return aug_launch(ctx, s);
 }
 
 // ------------------------------------------------------------------------------------------------ resized batches
@@ -745,6 +750,21 @@ int res_shape(const char *fn, long long n, int H, int W, int C, long long first,
     return PCNN_OK;
 }
 
+// the launch after the budget check; the caller holds the device guard
+int res_launch(const char *fn, pcnn_ctx *ctx, const ResShape &s) {
+    cudaFuncAttributes fa;
+    PCNN_CUDA(cudaFuncGetAttributes(&fa, s.vec == 8 ? k_augment_resized<8> : k_augment_resized<1>));
+    PCNN_REQUIRE(fa.sharedSizeBytes + (size_t)RES_SMEM <= (size_t)RES_SMEM_LIMIT && s.smem <= fa.maxDynamicSharedSizeBytes, PCNN_ERR_CUDA,
+                 "%s: the kernel's %zu bytes of static shared memory leave %d dynamic bytes, below the %d the budget assumes", fn,
+                 fa.sharedSizeBytes, fa.maxDynamicSharedSizeBytes, RES_SMEM);
+    if (s.vec == 8)
+        k_augment_resized<8><<<s.grid, AUG_THREADS, s.smem, ctx->stream>>>(s.a);
+    else
+        k_augment_resized<1><<<s.grid, AUG_THREADS, s.smem, ctx->stream>>>(s.a);
+    PCNN_CHECK_LAUNCH(ctx);
+    return PCNN_OK;
+}
+
 }  // namespace
 
 extern "C" int pcnn_augment_mix_u8_bf16(pcnn_ctx *ctx, const uint8_t *images_dev, const uint8_t *labels_dev, long long n, int H, int W,
@@ -840,15 +860,456 @@ extern "C" int pcnn_augment_resized_u8_bf16(pcnn_ctx *ctx, const uint8_t *images
     a.e0 = (unsigned)epoch;
     a.e1 = (unsigned)(epoch >> 32);
     pcnn_device_guard dg(ctx->device);
+    return res_launch(fn, ctx, s);
+}
+
+// ------------------------------------------------------------------------------------------------ TrivialAugmentWide, RandomErasing
+// pcnn_augment_trivial_u8_bf16: the plain or the resized call's geometry, then torchvision's TrivialAugmentWide on the uint8 crop,
+// the table, and RandomErasing(value = 0) on the normalised values.  The geometry runs as k_augment<., MIX_NONE> or
+// k_augment_resized with the identity table (bf16 bits u for byte u) into a caller-owned uint16 workspace [N][h][ws_pitch] at
+// C_out = C, so its bytes are those kernels' own.  k_trivial then takes one image per CTA: it stages the crop's bytes in shared
+// memory, draws the op and the erase box, builds the op's histogram (integer shared atomics: order-free) and byte map, and writes
+// each output element from one gather over the staged crop.
+namespace {
+
+constexpr int TA_THREADS = 512;
+constexpr int TA_OPS = 14, TA_BINS = 31;
+constexpr int TA_MAX_PIXELS = 65536;          // h w: the Contrast mean's fp32 sum of bytes stays exact (h w 255 < 2^24)
+constexpr int TA_SMEM_LIMIT = 227 * 1024;     // static + dynamic shared memory a CTA may opt into on an H100
+constexpr unsigned DOMAIN_TA = 0xC0000000u;   // counter word 1 of trivial block k: DOMAIN_TA | (16 + k) << 24 | i hi, i < 2^56
+constexpr int TA_NONE = 0, TA_NEAREST = 1, TA_BILINEAR = 2;
+enum TaOp {
+    OP_IDENTITY, OP_SHEAR_X, OP_SHEAR_Y, OP_TRANSLATE_X, OP_TRANSLATE_Y, OP_ROTATE, OP_BRIGHTNESS, OP_COLOR, OP_CONTRAST,
+    OP_SHARPNESS, OP_POSTERIZE, OP_SOLARIZE, OP_AUTOCONTRAST, OP_EQUALIZE
+};
+
+// one (op, bin, sign) of the host table.  Geometric ops: the grid's rescaled inverse matrix, gx = x v0 + y v1 + v2 and
+// gy = x v3 + y v4 + v5.  Brightness, Color, Contrast, Sharpness: v0 = RN32(ratio), v1 = RN32(1 - ratio).  Posterize: v0 = the
+// mask.  Solarize: v0 = the least byte that is inverted (256: none).
+struct TaEntry {
+    float v[6];
+};
+
+struct TaArgs : AugArgs {                     // AugArgs' permutation, keys and the output's layout and table, H x W the crop
+    const unsigned short *ws;                 // [N][H][ws_pitch]: the geometry's bytes
+    long long ws_image;                       // H ws_pitch
+    int ws_pitch, trivial, erase;
+    float erase_p, es0, esr, el0, elr;        // RN32(p), then the erase box's (low, range) pairs as the resized call's
+    TaEntry tab[TA_OPS * TA_BINS * 2];        // [op][bin][sign]
+};
+
+struct TaShared {
+    unsigned short lut[4 * 256];              // the table composed with the op's byte map
+    int hist[3][256];
+    float fmin[3], fscale[3];
+    int step[3];
+    unsigned long long i;
+    int op, bin, sign, erase, et, el, eh, ew;
+    float mean;
+};
+
+__device__ __forceinline__ float unit24(unsigned u) { return __fmul_rn((float)(u >> 8), 5.96046448e-08f); }
+
+// _blend on bytes: RN(RN(r a) + RN(s b)), clamped to [0, 255], truncated
+__device__ __forceinline__ unsigned blend_u8(float a, float b, float r, float s) {
+    return (unsigned)fminf(fmaxf(__fadd_rn(__fmul_rn(r, a), __fmul_rn(s, b)), 0.0f), 255.0f);
+}
+
+// rgb_to_grayscale on bytes: RN(RN(RN(0.2989 r) + RN(0.587 g)) + RN(0.114 b)), truncated
+__device__ __forceinline__ unsigned gray_u8(const uint8_t *p) {
+    return (unsigned)__fadd_rn(__fadd_rn(__fmul_rn(0.2989f, (float)p[0]), __fmul_rn(0.587f, (float)p[1])), __fmul_rn(0.114f, (float)p[2]));
+}
+
+// the byte at (y, x, c) of the transformed crop for the gather ops (geometric, Color, Sharpness); the point ops read img as is
+__device__ __forceinline__ unsigned ta_byte(const uint8_t *img, const TaArgs &a, const TaEntry &e, int op, int y, int x, int c) {
+    const int h = a.H, w = a.W, C = a.C;
+    const unsigned u = img[(y * w + x) * C + c];
+    if (op >= OP_SHEAR_X && op <= OP_ROTATE) {
+        const float bx = __fadd_rn((float)x, 0.5f - 0.5f * (float)w), by = __fadd_rn((float)y, 0.5f - 0.5f * (float)h);
+        const float gx = __fadd_rn(__fadd_rn(__fmul_rn(bx, e.v[0]), __fmul_rn(by, e.v[1])), e.v[2]);
+        const float gy = __fadd_rn(__fadd_rn(__fmul_rn(bx, e.v[3]), __fmul_rn(by, e.v[4])), e.v[5]);
+        const float ix = __fsub_rn(__fmul_rn(__fadd_rn(gx, 1.0f), 0.5f * (float)w), 0.5f);
+        const float iy = __fsub_rn(__fmul_rn(__fadd_rn(gy, 1.0f), 0.5f * (float)h), 0.5f);
+        auto at = [&](float fy, float fx) -> float {
+            return fx >= 0.0f && fx < (float)w && fy >= 0.0f && fy < (float)h ? (float)img[((int)fy * w + (int)fx) * C + c] : 0.0f;
+        };
+        if (a.trivial == TA_NEAREST) return (unsigned)at(rintf(iy), rintf(ix));
+        const float x0 = floorf(ix), y0 = floorf(iy);
+        const float tw = __fsub_rn(ix, x0), te = __fsub_rn(1.0f, tw), tn = __fsub_rn(iy, y0), ts = __fsub_rn(1.0f, tn);
+        float v = __fmul_rn(at(y0, x0), __fmul_rn(ts, te));
+        v = __fadd_rn(v, __fmul_rn(at(y0, x0 + 1.0f), __fmul_rn(ts, tw)));
+        v = __fadd_rn(v, __fmul_rn(at(y0 + 1.0f, x0), __fmul_rn(tn, te)));
+        v = __fadd_rn(v, __fmul_rn(at(y0 + 1.0f, x0 + 1.0f), __fmul_rn(tn, tw)));
+        return (unsigned)fminf(rintf(v), 255.0f);
+    }
+    if (op == OP_COLOR) return C == 3 ? blend_u8((float)u, (float)gray_u8(img + (y * w + x) * 3), e.v[0], e.v[1]) : u;
+    if (op == OP_SHARPNESS) {
+        if (h <= 2 || w <= 2) return u;
+        unsigned b = u;
+        if (y > 0 && y < h - 1 && x > 0 && x < w - 1) {
+            const float w1 = 0.0769230798f, w5 = 0.384615391f;     // RN32(1 / 13), RN32(5 / 13): the kernel / its sum
+            float acc = 0.0f;
+#pragma unroll
+            for (int k = 0; k < 9; ++k) {
+                const float t = __fmul_rn(k == 4 ? w5 : w1, (float)img[((y + k / 3 - 1) * w + x + k % 3 - 1) * C + c]);
+                acc = k == 0 ? t : __fadd_rn(acc, t);
+            }
+            b = (unsigned)fminf(rintf(acc), 255.0f);
+        }
+        return blend_u8((float)u, (float)b, e.v[0], e.v[1]);
+    }
+    return u;
+}
+
+template <int VEC>
+__global__ void __launch_bounds__(TA_THREADS) k_trivial(const __grid_constant__ TaArgs a) {
+    __shared__ TaShared sh;
+    extern __shared__ __align__(16) uint8_t img[];                              // [H][W][C]
+    const int h = a.H, w = a.W, C = a.C, wC = w * C, hw = h * w;
+    for (long long j = blockIdx.x; j < a.units; j += gridDim.x) {
+        if (threadIdx.x == 0) {
+            const unsigned long long e = (unsigned long long)(a.first + j);
+            const unsigned long long i = a.shuffle ? permute(e, a) : e;
+            const unsigned lo = (unsigned)i, hi = (unsigned)(i >> 32);
+            const uint4 d = philox4x32_10(lo, DOMAIN_TA | 16u << 24 | hi, a.e0, a.e1, a.k0, a.k1);
+            sh.op = a.trivial ? (int)__umulhi(d.x, TA_OPS) : OP_IDENTITY;
+            sh.bin = (int)__umulhi(d.y, TA_BINS);
+            sh.sign = (int)(d.z >> 31);
+            int erase = a.erase && unit24(d.w) < a.erase_p, et = 0, el = 0, eh = 0, ew = 0;
+            if (erase) {
+                erase = 0;
+                const double area = __dmul_rn((double)h, (double)w);
+                uint4 b = make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll 1
+                for (int t = 0; t < BOX_ATTEMPTS && !erase; ++t) {
+                    if ((t & 1) == 0) b = philox4x32_10(lo, DOMAIN_TA | (unsigned)(17 + t / 2) << 24 | hi, a.e0, a.e1, a.k0, a.k1);
+                    const float s = __fadd_rn(__fmul_rn(unit24((t & 1) ? b.z : b.x), a.esr), a.es0);
+                    const float lr = __fadd_rn(__fmul_rn(unit24((t & 1) ? b.w : b.y), a.elr), a.el0);
+                    const double aspect = (double)exp_f32(lr), ea = __dmul_rn(area, (double)s);
+                    const double ch = rint(__dsqrt_rn(__dmul_rn(ea, aspect))), cw = rint(__dsqrt_rn(__ddiv_rn(ea, aspect)));
+                    if (ch < (double)h && cw < (double)w) {
+                        eh = (int)ch;
+                        ew = (int)cw;
+                        const uint4 r = philox4x32_10(lo, DOMAIN_TA | (unsigned)(17 + BOX_ATTEMPTS / 2) << 24 | hi, a.e0, a.e1, a.k0, a.k1);
+                        et = (int)__umulhi(r.x, (unsigned)(h - eh + 1));
+                        el = (int)__umulhi(r.y, (unsigned)(w - ew + 1));
+                        erase = 1;
+                    }
+                }
+            }
+            sh.i = i;
+            sh.erase = erase, sh.et = et, sh.el = el, sh.eh = eh, sh.ew = ew;
+        }
+        for (int t = threadIdx.x; t < 3 * 256; t += TA_THREADS) (&sh.hist[0][0])[t] = 0;
+        const unsigned short *ws = a.ws + j * a.ws_image;
+        if ((wC & 7) == 0) {
+            const int vr = wC >> 3;
+            for (int t = threadIdx.x; t < h * vr; t += TA_THREADS) {
+                const int r = t / vr, k = (t - r * vr) << 3;
+                const uint4 v = *reinterpret_cast<const uint4 *>(ws + (long long)r * a.ws_pitch + k);
+                uint2 o;
+                o.x = (v.x & 0xFFu) | (v.x >> 8 & 0xFF00u) | (v.y & 0xFFu) << 16 | (v.y >> 16 & 0xFFu) << 24;
+                o.y = (v.z & 0xFFu) | (v.z >> 8 & 0xFF00u) | (v.w & 0xFFu) << 16 | (v.w >> 16 & 0xFFu) << 24;
+                *reinterpret_cast<uint2 *>(img + r * wC + k) = o;
+            }
+        } else {
+            for (int t = threadIdx.x; t < h * wC; t += TA_THREADS) {
+                const int r = t / wC;
+                img[t] = (uint8_t)ws[(long long)r * a.ws_pitch + (t - r * wC)];
+            }
+        }
+        __syncthreads();
+        const int op = sh.op;
+        const TaEntry &e = a.tab[(op * TA_BINS + sh.bin) * 2 + sh.sign];
+        if (op == OP_CONTRAST) {
+            for (int p = threadIdx.x; p < hw; p += TA_THREADS) atomicAdd(&sh.hist[0][C == 3 ? gray_u8(img + p * 3) : img[p]], 1);
+        } else if (op == OP_AUTOCONTRAST || op == OP_EQUALIZE) {
+            for (int t = threadIdx.x; t < hw * C; t += TA_THREADS) atomicAdd(&sh.hist[t % C][img[t]], 1);
+        }
+        __syncthreads();
+        if (op == OP_CONTRAST && threadIdx.x == 0) {
+            long long sum = 0;
+            for (int g = 0; g < 256; ++g) sum += (long long)g * sh.hist[0][g];
+            sh.mean = __fdiv_rn((float)sum, (float)hw);                // exact sum: hw 255 < 2^24
+        } else if (op == OP_AUTOCONTRAST && threadIdx.x < C) {
+            const int *hc = sh.hist[threadIdx.x];
+            int lo = 0, hi = 255;
+            while (hc[lo] == 0) ++lo;
+            while (hc[hi] == 0) --hi;
+            sh.fmin[threadIdx.x] = hi == lo ? 0.0f : (float)lo;
+            sh.fscale[threadIdx.x] = hi == lo ? 1.0f : __fmul_rn(__frcp_rn((float)(hi - lo)), 255.0f);
+        } else if (op == OP_EQUALIZE && threadIdx.x < C) {
+            int *hc = sh.hist[threadIdx.x];
+            int hi = 255;
+            while (hc[hi] == 0) --hi;
+            int cum = 0;
+            for (int u = 0; u < 256; ++u) cum += hc[u], hc[u] = cum;
+            sh.step[threadIdx.x] = (cum - (hc[hi] - (hi ? hc[hi - 1] : 0))) / 255;
+        }
+        __syncthreads();
+        for (int t = threadIdx.x; t < C * 256; t += TA_THREADS) {
+            const int c = t >> 8;
+            const unsigned u = t & 255;
+            unsigned b = u;
+            if (op == OP_BRIGHTNESS) b = blend_u8((float)u, 0.0f, e.v[0], e.v[1]);
+            else if (op == OP_CONTRAST) b = blend_u8((float)u, sh.mean, e.v[0], e.v[1]);
+            else if (op == OP_POSTERIZE) b = u & (unsigned)e.v[0];
+            else if (op == OP_SOLARIZE) b = u >= (unsigned)e.v[0] ? 255u - u : u;
+            else if (op == OP_AUTOCONTRAST)
+                b = (unsigned)fminf(fmaxf(__fmul_rn(__fsub_rn((float)u, sh.fmin[c]), sh.fscale[c]), 0.0f), 255.0f);
+            else if (op == OP_EQUALIZE && sh.step[c] != 0)
+                b = u == 0 ? 0u : (unsigned)min((sh.hist[c][u - 1] + sh.step[c] / 2) / sh.step[c], 255);
+            sh.lut[t] = a.lut[c * 256 + b];
+        }
+        __syncthreads();
+        const bool gather = (op >= OP_SHEAR_X && op <= OP_ROTATE) || op == OP_COLOR || op == OP_SHARPNESS;
+        const int erase = sh.erase, et = sh.et, el = sh.el, eb = sh.et + sh.eh, er = sh.el + sh.ew;
+        __nv_bfloat16 *xj = a.x + j * a.image_rows * (long long)a.pitch;
+        for (int t = threadIdx.x; t < h * a.vpr; t += TA_THREADS) {
+            const int r = t / a.vpr;
+            const int k = (t - r * a.vpr) * VEC;
+            const bool row_erase = erase && r >= et && r < eb;
+            int x = k / a.C_out, c = k - x * a.C_out;
+            BitsVec<VEC> out;
+#pragma unroll
+            for (int q = 0; q < VEC; ++q) {
+                unsigned short bits = 0;
+                if (c < C && !(row_erase && x >= el && x < er))
+                    bits = sh.lut[c * 256 + (gather ? ta_byte(img, a, e, op, r, x, c) : img[(r * w + x) * C + c])];
+                out.h[q] = bits;
+                if (++c == a.C_out) {
+                    c = 0;
+                    ++x;
+                }
+            }
+            *reinterpret_cast<BitsVec<VEC> *>(xj + (long long)r * a.pitch + k) = out;
+        }
+        __syncthreads();                                           // the shared state is rewritten by the next image
+    }
+}
+
+// torch.linspace(0, 0.99, 31) and torch.linspace(0, 32, 31) in fp32, the magnitudes of TrivialAugmentWide._augmentation_space
+// (torch's vectorised linspace rounds some bins differently from start + i step; Rotate's and Solarize's bins are exact)
+const float TA_MAG_099[TA_BINS] = {
+    0.0f, 0.032999999821186066f, 0.06599999964237213f, 0.0989999994635582f, 0.13199999928474426f, 0.16499999165534973f,
+    0.1979999989271164f, 0.23100000619888306f, 0.2639999985694885f, 0.296999990940094f, 0.32999998331069946f, 0.3630000054836273f,
+    0.3959999978542328f, 0.42899999022483826f, 0.4620000123977661f, 0.4950000047683716f, 0.527999997138977f, 0.5609999895095825f,
+    0.593999981880188f, 0.6270000338554382f, 0.6600000262260437f, 0.6930000185966492f, 0.7260000109672546f, 0.7590000033378601f,
+    0.7919999957084656f, 0.824999988079071f, 0.8580000400543213f, 0.8910000324249268f, 0.9240000247955322f, 0.9570000171661377f,
+    0.9900000095367432f};
+const float TA_MAG_32[TA_BINS] = {
+    0.0f, 1.0666667222976685f, 2.133333444595337f, 3.200000286102295f, 4.266666889190674f, 5.333333492279053f, 6.40000057220459f,
+    7.466667175292969f, 8.533333778381348f, 9.600000381469727f, 10.666666984558105f, 11.733333587646484f, 12.80000114440918f,
+    13.866667747497559f, 14.933334350585938f, 15.999999046325684f, 17.066665649414062f, 18.133333206176758f, 19.19999885559082f,
+    20.266666412353516f, 21.333332061767578f, 22.399999618530273f, 23.46666717529297f, 24.53333282470703f, 25.600000381469727f,
+    26.66666603088379f, 27.733333587646484f, 28.799999237060547f, 29.866666793823242f, 30.933332443237305f, 32.0f};
+
+// the magnitude of (op, bin, sign) as _apply_op receives it: the fp32 bin as a double, negated for a signed op's sign 1
+double ta_magnitude(int op, int bin, int sign) {
+    double m = 0.0;
+    bool signed_op = true;
+    switch (op) {
+    case OP_SHEAR_X: case OP_SHEAR_Y: case OP_BRIGHTNESS: case OP_COLOR: case OP_CONTRAST: case OP_SHARPNESS: m = TA_MAG_099[bin]; break;
+    case OP_TRANSLATE_X: case OP_TRANSLATE_Y: m = TA_MAG_32[bin]; break;
+    case OP_ROTATE: m = (double)(4.5f * (float)bin); break;
+    case OP_POSTERIZE: m = 8 - (int)std::nearbyint((float)bin / 5.0f), signed_op = false; break;
+    case OP_SOLARIZE: m = (double)(255.0f - 8.5f * (float)bin), signed_op = false; break;
+    default: signed_op = false;
+    }
+    return signed_op && sign ? -m : m;
+}
+
+// torchvision's _get_inverse_affine_matrix (inverted, scale 1) in double, in its order of operations
+void inverse_affine(double cx, double cy, double angle, double tx, double ty, double shear_x, double shear_y, double *m) {
+    const double deg2rad = M_PI / 180.0;
+    const double rot = angle * deg2rad, sx = shear_x * deg2rad, sy = shear_y * deg2rad;
+    const double a = std::cos(rot - sy) / std::cos(sy);
+    const double b = -std::cos(rot - sy) * std::tan(sx) / std::cos(sy) - std::sin(rot);
+    const double c = std::sin(rot - sy) / std::cos(sy);
+    const double d = -std::sin(rot - sy) * std::tan(sx) / std::cos(sy) + std::cos(rot);
+    m[0] = d, m[1] = -b, m[2] = 0.0, m[3] = -c, m[4] = a, m[5] = 0.0;
+    m[2] += m[0] * (-cx - tx) + m[1] * (-cy - ty);
+    m[5] += m[3] * (-cx - tx) + m[4] * (-cy - ty);
+    m[2] += cx;
+    m[5] += cy;
+}
+
+// the entry of (op, bin, sign) for an h x w crop
+TaEntry ta_entry(int op, int bin, int sign, int h, int w) {
+    TaEntry e{};
+    const double mag = ta_magnitude(op, bin, sign);
+    if (op >= OP_SHEAR_X && op <= OP_ROTATE) {
+        const double rad2deg = 180.0 / M_PI;
+        double m[6];
+        if (op == OP_SHEAR_X) inverse_affine(-(w * 0.5), -(h * 0.5), 0.0, 0.0, 0.0, std::atan(mag) * rad2deg, 0.0, m);
+        else if (op == OP_SHEAR_Y) inverse_affine(-(w * 0.5), -(h * 0.5), 0.0, 0.0, 0.0, 0.0, std::atan(mag) * rad2deg, m);
+        else if (op == OP_TRANSLATE_X) inverse_affine(0.0, 0.0, 0.0, (double)(long long)mag, 0.0, 0.0, 0.0, m);
+        else if (op == OP_TRANSLATE_Y) inverse_affine(0.0, 0.0, 0.0, 0.0, (double)(long long)mag, 0.0, 0.0, m);
+        else inverse_affine(0.0, 0.0, -mag, 0.0, 0.0, 0.0, 0.0, m);
+        const float sx = (float)(0.5 * w), sy = (float)(0.5 * h);
+        for (int k = 0; k < 3; ++k) e.v[k] = (float)m[k] / sx, e.v[3 + k] = (float)m[3 + k] / sy;
+    } else if (op >= OP_BRIGHTNESS && op <= OP_SHARPNESS) {
+        const double ratio = 1.0 + mag;
+        e.v[0] = (float)ratio;
+        e.v[1] = (float)(1.0 - ratio);
+    } else if (op == OP_POSTERIZE) {
+        e.v[0] = (float)((256 - (1 << (8 - (int)mag))) & 255);
+    } else if (op == OP_SOLARIZE) {
+        e.v[0] = std::ceil((float)mag);                             // img >= threshold over bytes
+    }
+    return e;
+}
+
+struct TaShape {
+    TaArgs a;
+    AugShape geo;                     // the plain geometry (resize 0)
+    ResShape res;                     // the resized geometry (resize 1)
+    int vec, grid, smem;
+    long long ws_bytes;
+};
+
+// the domain, one message per rule, the geometry's and the output's launches and the table: a function of the arguments alone
+int ta_shape(const char *fn, long long n, int H, int W, int C, long long first, int N, int shuffle, int pad, int flip, int resize,
+             int H_out, int W_out, double s0, double s1, double r0, double r1, int trivial, double erase_p, double es0, double es1,
+             double er0, double er1, int C_out, int row_pitch, int image_rows, const float *mean, const float *std_, TaShape *s) {
+    PCNN_REQUIRE(resize == 0 || resize == 1, PCNN_ERR_ARG, "%s: resize = %d: 0 (crop and pad) or 1 (RandomResizedCrop) is required", fn,
+                 resize);
+    PCNN_REQUIRE(trivial == TA_NONE || trivial == TA_NEAREST || trivial == TA_BILINEAR, PCNN_ERR_ARG,
+                 "%s: trivial = %d: 0 (none), 1 (NEAREST) or 2 (BILINEAR) is required", fn, trivial);
+    PCNN_REQUIRE(!trivial || C == 1 || C == 3, PCNN_ERR_ARG, "%s: C = %d: TrivialAugmentWide takes C = 1 or 3", fn, C);
+    PCNN_REQUIRE(std::isfinite(erase_p) && erase_p >= 0.0 && erase_p <= 1.0, PCNN_ERR_ARG,
+                 "%s: erase_p = %g: a finite 0 <= p <= 1 is required", fn, erase_p);
+    if (erase_p > 0.0) {
+        PCNN_REQUIRE(std::isfinite(es0) && std::isfinite(es1) && es0 >= 0.0 && es0 <= es1 && es1 <= 1.0, PCNN_ERR_ARG,
+                     "%s: erase scale = (%g, %g): 0 <= s0 <= s1 <= 1 is required", fn, es0, es1);
+        const double lo = 1.1754943508222875e-38, hi = 3.4028234663852886e+38;
+        PCNN_REQUIRE(er0 >= lo && er1 <= hi && er0 <= er1, PCNN_ERR_ARG,
+                     "%s: erase ratio = (%g, %g): r0 <= r1, each within fp32's normal range [2^-126, 3.4028235e38], is required", fn,
+                     er0, er1);
+    }
+    if (resize) {
+        PCNN_REQUIRE(pad == 0, PCNN_ERR_ARG, "%s: pad = %d: a resized batch takes no padding", fn, pad);
+        const int rc = res_shape(fn, n, H, W, C, first, N, shuffle, flip, H_out, W_out, C, 0, 0, nullptr, nullptr, RES_TRAIN, s0, s1, r0,
+                                 r1, 0, &s->res);
+        if (rc) return rc;
+    } else {
+        const int rc = aug_shape(fn, n, H, W, C, first, N, shuffle, pad, flip, C, 0, 0, nullptr, nullptr, &s->geo);
+        if (rc) return rc;
+        H_out = H, W_out = W;
+    }
+    AugArgs &g = resize ? static_cast<AugArgs &>(s->res.a) : s->geo.a;
+    for (int c = 0; c < C; ++c)
+        for (int u = 0; u < 256; ++u) g.lut[c * 256 + u] = (unsigned short)u;
+    AugShape out;
+    const int rc = aug_shape(fn, n, H_out, W_out, C, first, N, shuffle, 0, 0, C_out, row_pitch, image_rows, mean, std_, &out);
+    if (rc) return rc;
+    const long long hw = (long long)H_out * W_out;
+    PCNN_REQUIRE(hw <= TA_MAX_PIXELS, PCNN_ERR_ARG, "%s: the crop is %d x %d: at most %d pixels (256 x 256) are allowed", fn, H_out, W_out,
+                 TA_MAX_PIXELS);
+    const long long smem = (hw * C + 15) / 16 * 16, smem_max = TA_SMEM_LIMIT - (long long)((sizeof(TaShared) + 15) / 16 * 16);
+    PCNN_REQUIRE(smem <= smem_max, PCNN_ERR_ARG,
+                 "%s: the crop is %d x %d x %d: its %lld bytes, staged in shared memory, must be <= %lld (227 KB less the kernel's "
+                 "static shared memory)", fn, H_out, W_out, C, smem, smem_max);
+    TaArgs &a = s->a;
+    memset(&a, 0, sizeof(a));
+    static_cast<AugArgs &>(a) = out.a;
+    a.units = N;                                              // one image per CTA
+    a.ws_pitch = g.pitch;
+    a.ws_image = (long long)H_out * g.pitch;
+    a.trivial = trivial;
+    a.erase = erase_p > 0.0;
+    a.erase_p = (float)erase_p;
+    if (a.erase) {
+        const float s0f = (float)es0, s1f = (float)es1, l0 = (float)std::log((double)(float)er0), l1 = (float)std::log((double)(float)er1);
+        a.es0 = s0f, a.esr = s1f - s0f, a.el0 = l0, a.elr = l1 - l0;
+    }
+    for (int op = 0; op < TA_OPS; ++op)
+        for (int bin = 0; bin < TA_BINS; ++bin)
+            for (int sign = 0; sign < 2; ++sign) a.tab[(op * TA_BINS + bin) * 2 + sign] = ta_entry(op, bin, sign, H_out, W_out);
+    s->vec = out.vec;
+    s->grid = (int)std::min<long long>(AUG_MAX_GRID, N);
+    s->smem = (int)smem;
+    s->ws_bytes = (long long)N * a.ws_image * 2;
+    return PCNN_OK;
+}
+
+}  // namespace
+
+extern "C" int pcnn_augment_trivial_u8_bf16_info(long long n, int H, int W, int C, long long first, int N, int shuffle, int pad, int flip,
+                                                 int resize, int H_out, int W_out, double scale_lo, double scale_hi, double ratio_lo,
+                                                 double ratio_hi, int trivial, double erase_p, double erase_scale_lo,
+                                                 double erase_scale_hi, double erase_ratio_lo, double erase_ratio_hi, int C_out,
+                                                 int row_pitch, int image_rows, const float *mean_host, const float *std_host,
+                                                 long long *out12, float *table_out, uint16_t *lut_out) {
+    const char *fn = "pcnn_augment_trivial_u8_bf16_info";
+    PCNN_REQUIRE(out12, PCNN_ERR_ARG, "%s: NULL out12", fn);
+    const std::unique_ptr<TaShape> s(new TaShape);             // the table makes it 26 KB
+    const int rc = ta_shape(fn, n, H, W, C, first, N, shuffle, pad, flip, resize, H_out, W_out, scale_lo, scale_hi, ratio_lo, ratio_hi,
+                            trivial, erase_p, erase_scale_lo, erase_scale_hi, erase_ratio_lo, erase_ratio_hi, C_out, row_pitch,
+                            image_rows, mean_host, std_host, s.get());
+    if (rc) return rc;
+    const TaArgs &a = s->a;
+    const long long v[12] = {a.pitch, a.image_rows, a.H, a.W, a.ws_pitch, s->ws_bytes, s->vec, s->grid, TA_THREADS, s->smem,
+                             (long long)((sizeof(TaShared) + 15) / 16 * 16), (long long)sizeof(TaArgs)};
+    memcpy(out12, v, sizeof(v));
+    if (table_out) memcpy(table_out, a.tab, sizeof(a.tab));
+    if (lut_out) memcpy(lut_out, a.lut, sizeof(uint16_t) * 256 * C);
+    return PCNN_OK;
+}
+
+extern "C" int pcnn_augment_trivial_u8_bf16(pcnn_ctx *ctx, const uint8_t *images_dev, const uint8_t *labels_dev, long long n, int H, int W,
+                                            int C, long long first, int N, int shuffle, int pad, int flip, unsigned long long seed,
+                                            unsigned long long epoch, const float *mean_host, const float *std_host, void *x_bf16_dev,
+                                            int C_out, int row_pitch, int image_rows, uint8_t *labels_out_dev, int resize, int H_out,
+                                            int W_out, double scale_lo, double scale_hi, double ratio_lo, double ratio_hi, int trivial,
+                                            double erase_p, double erase_scale_lo, double erase_scale_hi, double erase_ratio_lo,
+                                            double erase_ratio_hi, void *workspace_dev, long long workspace_bytes) {
+    const char *fn = "pcnn_augment_trivial_u8_bf16";
+    PCNN_REQUIRE(ctx && images_dev && x_bf16_dev && workspace_dev, PCNN_ERR_ARG,
+                 "%s: NULL context, images, x or workspace (only the labels may be NULL)", fn);
+    PCNN_REQUIRE(!labels_dev == !labels_out_dev, PCNN_ERR_ARG, "%s: labels and labels_out must both be NULL or neither", fn);
+    const std::unique_ptr<TaShape> holder(new TaShape);
+    TaShape &s = *holder;
+    const int rc = ta_shape(fn, n, H, W, C, first, N, shuffle, pad, flip, resize, H_out, W_out, scale_lo, scale_hi, ratio_lo, ratio_hi,
+                            trivial, erase_p, erase_scale_lo, erase_scale_hi, erase_ratio_lo, erase_ratio_hi, C_out, row_pitch,
+                            image_rows, mean_host, std_host, &s);
+    if (rc) return rc;
+    TaArgs &a = s.a;
+    PCNN_REQUIRE(aligned16(x_bf16_dev) && aligned16(workspace_dev), PCNN_ERR_ARG, "%s: x and the workspace must be 16-byte aligned", fn);
+    PCNN_REQUIRE(workspace_bytes >= s.ws_bytes, PCNN_ERR_ARG, "%s: workspace_bytes = %lld: at least %lld (N h ws_pitch 2) are required", fn,
+                 workspace_bytes, s.ws_bytes);
+    const size_t xbytes = (((size_t)N - 1) * a.image_rows * a.pitch + (size_t)(a.H - 1) * a.pitch + (size_t)a.W * a.C_out) * 2;
+    const size_t ibytes = (size_t)n * H * W * C, wbytes = (size_t)s.ws_bytes;
+    PCNN_REQUIRE(disjoint(x_bf16_dev, xbytes, images_dev, ibytes) && disjoint(x_bf16_dev, xbytes, labels_out_dev, N) &&
+                     disjoint(x_bf16_dev, xbytes, workspace_dev, wbytes),
+                 PCNN_ERR_ARG, "%s: overlapping buffers: x must share no byte with images, labels_out or the workspace", fn);
+    PCNN_REQUIRE(disjoint(labels_out_dev, N, labels_dev, n) && disjoint(labels_out_dev, N, images_dev, ibytes) &&
+                     disjoint(labels_out_dev, N, workspace_dev, wbytes),
+                 PCNN_ERR_ARG, "%s: overlapping buffers: labels_out must share no byte with labels, images or the workspace", fn);
+    PCNN_REQUIRE(disjoint(workspace_dev, wbytes, images_dev, ibytes) && disjoint(workspace_dev, wbytes, labels_dev, n), PCNN_ERR_ARG,
+                 "%s: overlapping buffers: the workspace must share no byte with images or labels", fn);
+    AugArgs &g = resize ? static_cast<AugArgs &>(s.res.a) : s.geo.a;
+    g.img = images_dev;
+    g.lab = labels_dev;
+    g.x = static_cast<__nv_bfloat16 *>(workspace_dev);
+    g.lab_out = labels_out_dev;
+    a.ws = static_cast<const unsigned short *>(workspace_dev);
+    a.x = static_cast<__nv_bfloat16 *>(x_bf16_dev);
+    g.k0 = a.k0 = (unsigned)seed;
+    g.k1 = a.k1 = (unsigned)(seed >> 32);
+    g.e0 = a.e0 = (unsigned)epoch;
+    g.e1 = a.e1 = (unsigned)(epoch >> 32);
+    pcnn_device_guard dg(ctx->device);
+    auto kern = s.vec == 8 ? k_trivial<8> : k_trivial<1>;
     cudaFuncAttributes fa;
-    PCNN_CUDA(cudaFuncGetAttributes(&fa, s.vec == 8 ? k_augment_resized<8> : k_augment_resized<1>));
-    PCNN_REQUIRE(fa.sharedSizeBytes + (size_t)RES_SMEM <= (size_t)RES_SMEM_LIMIT && s.smem <= fa.maxDynamicSharedSizeBytes, PCNN_ERR_CUDA,
-                 "%s: the kernel's %zu bytes of static shared memory leave %d dynamic bytes, below the %d the budget assumes", fn,
-                 fa.sharedSizeBytes, fa.maxDynamicSharedSizeBytes, RES_SMEM);
-    if (s.vec == 8)
-        k_augment_resized<8><<<s.grid, AUG_THREADS, s.smem, ctx->stream>>>(a);
-    else
-        k_augment_resized<1><<<s.grid, AUG_THREADS, s.smem, ctx->stream>>>(a);
+    PCNN_CUDA(cudaFuncGetAttributes(&fa, kern));
+    PCNN_REQUIRE(fa.sharedSizeBytes <= sizeof(TaShared) + 15, PCNN_ERR_CUDA,
+                 "%s: the kernel's %zu bytes of static shared memory exceed the %zu the budget assumes", fn, fa.sharedSizeBytes,
+                 sizeof(TaShared));
+    PCNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, s.smem));
+    const int grc = resize ? res_launch(fn, ctx, s.res) : aug_launch(ctx, s.geo);   // only after every check has passed
+    if (grc) return grc;
+    kern<<<s.grid, TA_THREADS, s.smem, ctx->stream>>>(a);
     PCNN_CHECK_LAUNCH(ctx);
     return PCNN_OK;
 }

@@ -7,7 +7,8 @@ from typing import NamedTuple, Optional
 import numpy as np
 
 from ._lib import (F32, NPARAM, OPTIM_ADAMW, OPTIM_SGD, TEST_SET, TRAIN_SET, U8, OptimConfig, OptimTensor, PcnnError, augment_info,
-                   augment_resized_info, RESIZE_TRAIN, RESIZE_EVAL, avgpool_nhwc_info, batchnorm_nhwc_info, channel_stats, check, conv_layer_family, dropout_info, dwconv_info, gconv_info, global_avgpool_nhwc_info, lib, linear_info,
+                   augment_resized_info, RESIZE_TRAIN, RESIZE_EVAL, augment_trivial_info, TRIVIAL_NONE, TRIVIAL_NEAREST, TRIVIAL_BILINEAR,
+                   avgpool_nhwc_info, batchnorm_nhwc_info, channel_stats, check, conv_layer_family, dropout_info, dwconv_info, gconv_info, global_avgpool_nhwc_info, lib, linear_info,
                    maxpool_nhwc_info,
                    se_scale_nhwc_info, ACT_RELU, ACT_SIGMOID, ACT_SILU, ACT_HARDSWISH, ACT_RELU6)
 
@@ -593,6 +594,24 @@ class Engine:
                    int(H_out), int(W_out), Cin if C_out is None else int(C_out), int(row_pitch or 0), int(image_rows or 0), _p(labels_out),
                    int(mode), float(scale[0]), float(scale[1]), float(ratio[0]), float(ratio[1]), int(resize_size or 0))
 
+    def augment_trivial(self, images, labels, n, H, W, C, first, N, x, workspace, labels_out=None, trivial=TRIVIAL_NEAREST,
+                        erase_p=0.0, erase_scale=(0.02, 0.33), erase_ratio=(0.3, 3.3), crop_size=None, scale=(0.08, 1.0),
+                        ratio=(3 / 4, 4 / 3), shuffle=1, pad=0, flip=0, seed=0, epoch=0, mean=None, std=None, C_out=None, row_pitch=0,
+                        image_rows=0):
+        """pcnn_augment_trivial_u8_bf16: a training batch of augment's crop, pad and flip (crop_size None) or augment_resized's
+        RandomResizedCrop(crop_size, scale, ratio) and flip, then TrivialAugmentWide (trivial TRIVIAL_NEAREST / TRIVIAL_BILINEAR, or
+        TRIVIAL_NONE), (u / 255 - mean) / std, and RandomErasing(erase_p, erase_scale, erase_ratio, value=0).  workspace is a device
+        buffer of at least augment_trivial_info(...)["ws_bytes"] bytes that holds the uint8 crops between the two launches."""
+        Cin = int(C)
+        m, s = channel_stats(mean, Cin, "mean"), channel_stats(std, Cin, "std")
+        hw = (0, 0) if crop_size is None else tuple(int(v) for v in crop_size)
+        self._call("pcnn_augment_trivial_u8_bf16", _p(images), _p(labels), int(n), int(H), int(W), Cin, int(first), int(N), int(shuffle),
+                   int(pad), int(flip), int(seed), int(epoch), None if m is None else m.ctypes.data, None if s is None else s.ctypes.data,
+                   _p(x), Cin if C_out is None else int(C_out), int(row_pitch or 0), int(image_rows or 0), _p(labels_out),
+                   int(crop_size is not None), *hw, float(scale[0]), float(scale[1]), float(ratio[0]), float(ratio[1]), int(trivial),
+                   float(erase_p), float(erase_scale[0]), float(erase_scale[1]), float(erase_ratio[0]), float(erase_ratio[1]),
+                   _p(workspace), 0 if workspace is None else int(workspace.nbytes))
+
 
 class MixedLabels(NamedTuple):
     """The targets of a mixed training batch: image j is lam parts labels[j] and 1 - lam parts labels_b[j] (lam_adjusted, the
@@ -1170,11 +1189,28 @@ class ImageBatcher:
     crop_size (an int or (h, w)) resizes (pcnn_augment_resized_u8_bf16): training batches take torchvision's
     RandomResizedCrop(crop_size, scale, ratio, antialias=True) and the flip, eval batches Resize(resize_size) +
     CenterCrop(crop_size), resize_size defaulting to the crop's shorter side; x then holds crop_size pixels per image.  It excludes
-    pad > 0 and mixing.  crop_size None (the default) is the plain batcher, bit for bit."""
+    pad > 0 and mixing.  crop_size None (the default) is the plain batcher, bit for bit.
+
+    trivial_augment "nearest" or "bilinear" and random_erase > 0 (a probability, with erase_scale and erase_ratio) add
+    torchvision's TrivialAugmentWide after the crop and flip and RandomErasing(value=0) after Normalize to training batches
+    (pcnn_augment_trivial_u8_bf16), the batcher owning the uint8 workspace between its two launches.  TrivialAugmentWide needs
+    C 1 or 3; neither excludes crop_size, both exclude mixing.  Eval batches are unchanged.  trivial_augment None with
+    random_erase 0 (the defaults) is the batcher without them, bit for bit."""
 
     def __init__(self, engine, images, labels, N, pad=0, flip=False, shuffle=True, seed=0, mean=None, std=None, C_out=None,
                  row_pitch=0, image_rows=0, mixup_alpha=0.0, cutmix_alpha=0.0, crop_size=None, scale=(0.08, 1.0), ratio=(3 / 4, 4 / 3),
-                 resize_size=None):
+                 resize_size=None, trivial_augment=None, random_erase=0.0, erase_scale=(0.02, 0.33), erase_ratio=(0.3, 3.3)):
+        modes = {None: TRIVIAL_NONE, "nearest": TRIVIAL_NEAREST, "bilinear": TRIVIAL_BILINEAR}
+        if not isinstance(trivial_augment, (str, type(None))) or trivial_augment not in modes:
+            raise PcnnError("ImageBatcher", -1, f"trivial_augment = {trivial_augment!r}: None, 'nearest' or 'bilinear' is required")
+        if not (isinstance(random_erase, (int, float, np.integer, np.floating)) and math.isfinite(random_erase) and 0 <= random_erase <= 1):
+            raise PcnnError("ImageBatcher", -1, f"random_erase = {random_erase}: a probability 0 <= p <= 1 is required")
+        self.trivial, self.random_erase = modes[trivial_augment], float(random_erase)
+        self.erase_scale, self.erase_ratio = (float(erase_scale[0]), float(erase_scale[1])), (float(erase_ratio[0]), float(erase_ratio[1]))
+        self.augmenting = self.trivial != TRIVIAL_NONE or self.random_erase > 0
+        if self.augmenting and (mixup_alpha > 0 or cutmix_alpha > 0):
+            raise PcnnError("ImageBatcher", -1, "trivial_augment or random_erase with mixup_alpha or cutmix_alpha > 0: these batches are "
+                            "not mixed")
         for name, a in (("mixup_alpha", mixup_alpha), ("cutmix_alpha", cutmix_alpha)):
             if not (isinstance(a, (int, float, np.integer, np.floating)) and math.isfinite(a) and a >= 0):
                 raise PcnnError("ImageBatcher", -1, f"{name} = {a}: a finite alpha >= 0 is required")
@@ -1210,6 +1246,11 @@ class ImageBatcher:
                                                        image_rows, self.mean, self.std)
             augment_resized_info(self.n, self.H, self.W, self.C, 0, self.N, *self.crop, RESIZE_EVAL, resize_size=self.resize_size,
                                  C_out=self.C_out, row_pitch=row_pitch, image_rows=image_rows, mean=self.mean, std=self.std)
+        self.ws_info = None
+        if self.augmenting:
+            self.ws_info = augment_trivial_info(self.n, self.H, self.W, self.C, 0, self.N, self.trivial, self.random_erase,
+                                                self.erase_scale, self.erase_ratio, self.crop, self.scale, self.ratio, int(self.shuffle),
+                                                self.pad, int(self.flip), self.C_out, row_pitch, image_rows, self.mean, self.std)[0]
         if labels is not None and int(labels.shape[0]) != self.n:
             raise PcnnError("ImageBatcher", -1, f"{labels.shape[0]} labels for {self.n} images")
         self.engine = engine
@@ -1218,6 +1259,7 @@ class ImageBatcher:
         self.x = engine.array((self.N, self.info["image_rows"], self.info["row_pitch"]), np.uint16)    # zeroed: the pad stays 0
         self.labels_out = engine.array((self.N,), np.uint8) if labels is not None else None
         self.labels_b = engine.array((self.N,), np.uint8) if self.mixing else None
+        self.workspace = engine.array((self.ws_info["ws_bytes"],), np.uint8) if self.augmenting else None
         self.steps_per_epoch = self.n // self.N
         self.epoch = 0
 
@@ -1231,6 +1273,11 @@ class ImageBatcher:
         kw = dict(shuffle=int(aug and self.shuffle), pad=self.pad if aug else 0, flip=int(aug and self.flip), seed=self.seed,
                   epoch=self.epoch, mean=self.mean, std=self.std, C_out=self.C_out, row_pitch=self.info["row_pitch"],
                   image_rows=self.info["image_rows"])
+        if aug and self.augmenting:
+            self.engine.augment_trivial(*args[:9], self.workspace, self.labels_out, trivial=self.trivial, erase_p=self.random_erase,
+                                        erase_scale=self.erase_scale, erase_ratio=self.erase_ratio, crop_size=self.crop, scale=self.scale,
+                                        ratio=self.ratio, **kw)
+            return self.x.ptr, self.labels_out
         if self.crop is not None:
             del kw["pad"]
             self.engine.augment_resized(*args[:9], *self.crop, self.labels_out, mode=RESIZE_TRAIN if aug else RESIZE_EVAL,
@@ -1246,7 +1293,7 @@ class ImageBatcher:
         return self.x.ptr, MixedLabels(self.labels_out, self.labels_b, weight, kind, box)
 
     def close(self):
-        for a in (self.x, self.labels_out, self.labels_b):
+        for a in (self.x, self.labels_out, self.labels_b, self.workspace):
             if a is not None:
                 a.free()
 

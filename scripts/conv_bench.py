@@ -1482,6 +1482,58 @@ def run_resized(name, N, H, W, C, H_out, W_out, C_out, iters, resize_size, batch
                           "power_limit": power}), flush=True)
 
 
+def run_trivial(name, N, H, W, C, C_out, pad, crop, iters, batches=4, row_pitch=0, image_rows=0, rounds=3, erase_p=0.1):
+    """one training batch with TrivialAugmentWide (BILINEAR) and RandomErasing(erase_p) (pcnn_augment_trivial_u8_bf16) against the
+    same batch without them (pcnn_augment_u8_bf16 with pad, or pcnn_augment_resized_u8_bf16's RandomResizedCrop when crop is set),
+    alternated over `rounds` rounds (the best of each kept); and torchvision's per-image CPU path for the two stages alone
+    (TrivialAugmentWide on the uint8 crop, then ToTensor + Normalize + RandomErasing, bf16), timed once on one thread.  Bytes: the
+    geometry's source bytes, the uint16 workspace written and read, and N h w C_out 2 written."""
+    import torchvision.transforms as T
+    n = N * batches
+    images = torch.randint(0, 256, (n, H, W, C), dtype=torch.uint8, device="cuda")
+    labels = torch.randint(0, 10, (n,), dtype=torch.uint8, device="cuda")
+    mean, std = ((0.485, 0.456, 0.406), (0.229, 0.224, 0.225)) if C == 3 else (None, None)
+    info, _, _ = pkg.augment_trivial_info(n, H, W, C, 0, N, pkg.TRIVIAL_BILINEAR, erase_p, crop_size=crop, pad=pad, flip=1, C_out=C_out,
+                                          row_pitch=row_pitch, image_rows=image_rows)
+    h, w = info["h"], info["w"]
+    x = torch.empty(N * info["image_rows"] * info["row_pitch"], dtype=torch.int16, device="cuda")
+    ws = torch.empty(info["ws_bytes"], dtype=torch.uint8, device="cuda")
+    lo = torch.empty(N, dtype=torch.uint8, device="cuda")
+    steps = iter(range(1 << 40))
+    kw = dict(flip=1, seed=11, epoch=3, mean=mean, std=std, C_out=C_out, row_pitch=row_pitch, image_rows=image_rows)
+    first = lambda: (next(steps) % batches) * N
+    ours = lambda: eng.augment_trivial(images, labels, n, H, W, C, first(), N, x, ws, lo, trivial=pkg.TRIVIAL_BILINEAR, erase_p=erase_p,
+                                       crop_size=crop, pad=pad, **kw)
+    if crop is None:
+        base = lambda: eng.augment(images, labels, n, H, W, C, first(), N, x, lo, pad=pad, **kw)
+    else:
+        base = lambda: eng.augment_resized(images, labels, n, H, W, C, first(), N, x, h, w, lo, **kw)
+    best = None
+    for _ in range(rounds):
+        r = (timed(ours, iters), timed(base, iters))
+        best = r if best is None else tuple(min(a, b) for a, b in zip(r, best))
+    ms, ms_base = best
+    src = N * (H * W if crop is None else h * w) * C                  # the RRC box covers at most the image; its mean is near h w
+    nbytes = src + 2 * N * h * info["ws_pitch"] * 2 + N * h * w * C_out * 2
+    host = torch.randint(0, 256, (N, C, h, w), dtype=torch.uint8)
+    ta = T.TrivialAugmentWide(interpolation=T.InterpolationMode.BILINEAR)
+    er = T.RandomErasing(p=erase_p, value=0)
+    m_t = torch.tensor(mean or (0.0,) * C).view(-1, 1, 1)
+    s_t = torch.tensor(std or (1.0,) * C).view(-1, 1, 1)
+    threads = torch.get_num_threads()
+    torch.set_num_threads(1)
+    t0 = time.perf_counter()
+    for j in range(N):
+        er((ta(host[j]).float() / 255.0 - m_t) / s_t).to(torch.bfloat16)
+    cpu_s = time.perf_counter() - t0
+    torch.set_num_threads(threads)
+    gpu, power = card()
+    print(json.dumps({"case": f"trivial {name}", "N": N, "us": ms * 1e3, "without_us": ms_base * 1e3, "with_over_without": ms / ms_base,
+                      "MB": nbytes / 1e6, "hbm_frac": nbytes / (ms * 1e-3) / 1e9 / HBM, "torchvision_cpu_ms": cpu_s * 1e3,
+                      "torchvision_cpu_over_ours": cpu_s * 1e3 / ms, "smem": info["smem"], "grid": info["grid"], "gpu": gpu,
+                      "power_limit": power}), flush=True)
+
+
 def run_resnetgap_resized(iters, rounds=3):
     """one training step of the GAP ResNet at N = 128 fed by pkg.ImageBatcher with crop_size 28 and scale (0.6, 1.0) (shuffle),
     against the same step on the plain batcher (shuffle, pad 2), alternated over `rounds` rounds (the best of each kept)"""
@@ -1510,6 +1562,38 @@ def run_resnetgap_resized(iters, rounds=3):
                       "ms_resized": ms_res, "ms_plain": ms_plain, "resized_over_plain": ms_res / ms_plain, "batch_us": ms_batch * 1e3,
                       "gpu": gpu, "power_limit": power}), flush=True)
     for a in (plain_b, res_b, net):
+        a.close()
+
+
+def run_resnetgap_trivial(iters, rounds=3):
+    """one training step of the GAP ResNet at N = 128 fed by pkg.ImageBatcher with pad 2, TrivialAugmentWide (BILINEAR) and
+    RandomErasing(0.1) (shuffle), against the same step on the batcher without the two stages, alternated over `rounds` rounds (the
+    best of each kept)"""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from example_nets import ResNetGAP
+    g = np.load(os.path.join(ROOT, "tests", "golden", "mnist_subset.npz"))
+    make = lambda **k: pkg.ImageBatcher(eng, g["train_u8"].reshape(-1, 28, 28), g["train_labels"], ResNetGAP.NB, pad=2, shuffle=True,
+                                        seed=5, row_pitch=32, image_rows=28, **k)
+    plain_b, ta_b = make(), make(trivial_augment="bilinear", random_erase=0.1)
+    net = ResNetGAP(eng, pkg, ResNetGAP.init_params())
+    k = iter(range(1 << 40))
+
+    def step(batcher):
+        net.forward(*batcher.batch(next(k) % batcher.steps_per_epoch))
+        net.backward()
+        net.sgd(ResNetGAP.LR_STEP)
+
+    gpu, power = card()
+    best = None
+    for _ in range(rounds):
+        r = (timed(lambda: step(ta_b), iters), timed(lambda: step(plain_b), iters),
+             timed(lambda: ta_b.batch(next(k) % ta_b.steps_per_epoch), iters))
+        best = r if best is None else tuple(min(a, b) for a, b in zip(r, best))
+    ms_ta, ms_plain, ms_batch = best
+    print(json.dumps({"case": f"GAP ResNet training step N={ResNetGAP.NB}, pad 2 + TrivialAugmentWide + RandomErasing(0.1) vs pad 2",
+                      "ms_trivial": ms_ta, "ms_plain": ms_plain, "trivial_over_plain": ms_ta / ms_plain, "batch_us": ms_batch * 1e3,
+                      "gpu": gpu, "power_limit": power}), flush=True)
+    for a in (plain_b, ta_b, net):
         a.close()
 
 
@@ -1694,6 +1778,12 @@ if only == "resized":                                                  # resized
     run_resized("64x64x3 -> 56, 8", 256, 64, 64, 3, 56, 56, 8, 50, 64)
     run_resized("256x256x3 -> 224, 8", 256, 256, 256, 3, 224, 224, 8, 20, 256)
     run_resized("320x240x3 -> 224, 8", 256, 320, 240, 3, 224, 224, 8, 20, 256)
+if only == "trivial":                                                  # TrivialAugmentWide + RandomErasing vs the batch without them
+    run_trivial("28x28x1 pad 2 [28][32]", 1024, 28, 28, 1, 1, 2, None, 50, row_pitch=32, image_rows=28)
+    run_trivial("32x32x3 pad 4, 3", 512, 32, 32, 3, 3, 4, None, 50)
+    run_trivial("256x256x3 -> 224 RRC, 8", 256, 256, 256, 3, 8, 0, (224, 224), 20)
+if only == "resnetgap-trivial":                                        # the GAP ResNet step, with and without the two stages
+    run_resnetgap_trivial(20)
 if only == "resnetgap-resized":                                        # the GAP ResNet step, resized batch vs plain batch
     run_resnetgap_resized(20)
 if only == "mbconvdrop":                                               # the MBConv step with stochastic depth against the fused residual

@@ -13,6 +13,7 @@ F = torch.nn.functional
 AUG_SEED, AUG_PAD = 0x0123456789ABCDEF, 2       # tests/test_augment_gpu.py
 MIX_ALPHAS, MIX_EPS = (0.2, 1.0), 0.1           # tests/test_mix_gpu.py: mixup_alpha, cutmix_alpha and label smoothing
 DIGIT_SCALE = (0.6, 1.0)                        # tests/test_resize_gpu.py: RandomResizedCrop(28, scale) of the digits
+TRIVIAL_ERASE = 0.25                            # tests/test_trivial_gpu.py: TrivialAugmentWide (BILINEAR) and RandomErasing(p)
 
 
 def golden():
@@ -32,7 +33,7 @@ def batch_norm(state, v, training):
     return F.batch_norm(v, rm, rv, ga, be, training=training, momentum=0.1, eps=1e-5)
 
 
-def run(net, params, lr, epochs, NB, head="sgd ", optim="sgd", augment=False, mix=False, resized=False):
+def run(net, params, lr, epochs, NB, head="sgd ", optim="sgd", augment=False, mix=False, resized=False, trivial=False):
     """net(x, training) trained for `epochs` epochs of the 1024 golden training digits in order, NB per batch, with softmax
     cross-entropy over the batch and an optimizer step on params, then evaluated on the 256 golden test digits; prints the mean
     loss of the first and last epoch and the accuracy after `head`.
@@ -43,7 +44,10 @@ def run(net, params, lr, epochs, NB, head="sgd ", optim="sgd", augment=False, mi
       mix      augment's batches, each mixed as an ImageBatcher with MIX_ALPHAS mixes it (tests/mix_ref.py), trained against
                the soft target of pcnn_softmax_ce_soft_bf16 with label smoothing MIX_EPS
       resized  each epoch's batches as an ImageBatcher with crop_size 28 and scale DIGIT_SCALE draws them (shuffle, no flip),
-               replayed by tests/resize_ref.py; the test digits go through Resize(28) + CenterCrop(28), which leaves them as they are"""
+               replayed by tests/resize_ref.py; the test digits go through Resize(28) + CenterCrop(28), which leaves them as they are
+      trivial  augment's batches with TrivialAugmentWide (BILINEAR) after the crop and RandomErasing(TRIVIAL_ERASE) after
+               Normalize, as an ImageBatcher(trivial_augment="bilinear", random_erase=TRIVIAL_ERASE) draws them, replayed by
+               tests/trivial_ref.py"""
     torch.manual_seed(0)
     g, xs, ys, xt, yt = golden()
     opt = {"sgd": lambda: torch.optim.SGD(params, lr=lr),
@@ -51,6 +55,9 @@ def run(net, params, lr, epochs, NB, head="sgd ", optim="sgd", augment=False, mi
            "adamw": lambda: torch.optim.AdamW(params, lr=lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2)}[optim]()
     steps = len(ys) // NB
     losses = []
+    if trivial:
+        import trivial_ref
+        tab28 = trivial_ref.table(28, 28)
     for ep in range(epochs):
         for s in range(steps):
             if mix:
@@ -61,6 +68,10 @@ def run(net, params, lr, epochs, NB, head="sgd ", optim="sgd", augment=False, mi
                                                AUG_PAD, 0, AUG_SEED, ep, labels=g["train_labels"])
                 x = torch.from_numpy((xb.astype(np.uint32) << 16).view(np.float32).reshape(NB, 1, 28, 28))
                 y = torch.from_numpy(mix_ref.soft_target(lab, lab_b, lam, MIX_EPS, 10)[1])
+            elif trivial:
+                xb, lab, *_ = trivial_ref.batch(g["train_u8"].reshape(-1, 28, 28, 1), s * NB, NB, trivial_ref.BILINEAR, TRIVIAL_ERASE,
+                                                pad=AUG_PAD, seed=AUG_SEED, epoch=ep, labels=g["train_labels"], tab=tab28)
+                x, y = torch.from_numpy((xb.astype(np.uint32) << 16).view(np.float32).reshape(NB, 1, 28, 28)), torch.from_numpy(lab).long()
             elif resized:
                 import resize_ref
                 xb, lab, *_ = resize_ref.batch(g["train_u8"].reshape(-1, 28, 28, 1), s * NB, NB, resize_ref.TRAIN, 28, 28, DIGIT_SCALE,
