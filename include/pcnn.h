@@ -989,6 +989,83 @@ int pcnn_softmax_ce_bf16(pcnn_ctx *ctx, const void *logits_bf16_dev, const uint8
 int pcnn_softmax_ce_soft_bf16(pcnn_ctx *ctx, const void *logits_bf16_dev, const uint8_t *labels_dev, const uint8_t *labels_b_dev,
                               double lam, double smoothing, int N, int O, float scale, void *dlogits_bf16_dev, float *loss_f32_dev,
                               int *pred_i32_dev);
+/* ------------------------------------------------------------------ dense prediction
+ * Transposed convolution (csrc/conv_wide_bwd_tc.cu), as torch.nn.functional.conv_transpose2d(x, w, b, stride, (pad_h, pad_w),
+ * (op_h, op_w)) with groups 1 and dilation 1, followed by act (PCNN_ACT_NONE / _SIGMOID / _RELU, the forward epilogues' rule):
+ *     H_out = (H - 1) stride - 2 pad_h + R + op_h,   W_out = (W - 1) stride - 2 pad_w + S + op_w
+ *     y[n][h][w][co] = act(b[co] + sum_{ci,r,s} x[n][(h + pad_h - r)/stride][(w + pad_w - s)/stride][ci] * f[ci][r][s][co])
+ *                      over the (r, s) that divide exactly and give an x pixel inside H x W.
+ * It is exactly the input gradient of its adjoint convolution (input H_out x W_out x C_out, K = C_in filters, the same stride and
+ * padding, output H x W), pcnn_conv_wide_dgrad_padded(dy = x, filt = f, dx = y), run by a second instantiation of that kernel whose
+ * epilogue forms v = fp32 accumulator + b[co] (the accumulator itself with no bias), then act, then one bf16 rounding; the plain
+ * input-gradient instantiation is unchanged.  So with no bias and act 0 y is bit for bit pcnn_conv_wide_dgrad_padded, and pixels
+ * no window reaches get act(b) (bf16 of +0 with no bias and act 0).
+ *   - x is dense bf16 [N][H][W][C_in]; filt_f32_dev the fp32 master [C_in][R][S][C_out] (torch's weight [C_in][C_out][R][S]
+ *     permuted (0, 2, 3, 1): the adjoint's KRSC), rounded to bf16 (nearest even) on every call by the input gradient's own
+ *     conversion; bias fp32 [C_out] or NULL; y is [N][image_rows][row_pitch] with H_out x W_out pixels of C_out channels
+ *     (row_pitch 0 = W_out C_out, image_rows 0 = H_out), the adjoint's x layout.  Pad columns and rows of y are never written.
+ *   - Training: the bias / activation gradient is pcnn_conv_bias_act_bwd over y; dx (dense like x) is pcnn_conv_tc_fwd of a wide
+ *     plan of the adjoint convolution (no bias, act 0) on dy; dw (fp32 [C_in][R][S][C_out]) is pcnn_conv_wide_wgrad_padded with the
+ *     activations swapped, x = dy and dy = x.  The forward and dx read the same bf16 rounding of the master: the forward converts
+ *     it on every call, the plan holds what pcnn_conv_plan_set_params or the optimizers made of the same master.
+ *   - Domain (PCNN_ERR_ARG, one message per rule naming the called function): N, H, W >= 1; C_in % 8 == 0 and 8 <= C_in <= 256;
+ *     C_out % 8 == 0 and C_out >= 8, and C_out <= 256 with a bias or an activation (pcnn_conv_bias_act_bwd); act 0, 1 or 3;
+ *     stride 1..4; taps 1..7; 0 <= pad <= taps - 1; 0 <= output_padding < stride; 1 <= H_out, W_out < 2^24; H_out >= stride
+ *     when pad_h > 0 (W_out the same); then the adjoint convolution's pitch rules (row_pitch >= W_out C_out and a multiple of 8,
+ *     image_rows >= H_out), and at padding (0, 0) the refusal of an adjoint shape the row-Toeplitz plan serves (C_out <= 16 with
+ *     few taps), with pcnn_conv_wide_dgrad's messages.  x, y 16-byte aligned.  Reruns are bit-identical.
+ * pcnn_conv_transpose_info (host only, no GPU) refuses exactly the same and fills out8 = { H_out, W_out, row_pitch, image_rows,
+ * Pt, Qt of the input gradient's pixel block, channel groups, tiles }. */
+int pcnn_conv_transpose_info(int N, int H, int W, int C_in, int C_out, int R, int S, int stride, int pad_h, int pad_w, int op_h, int op_w,
+                             int row_pitch, int image_rows, int has_bias, int act, int *out8);
+int pcnn_conv_transpose_fwd(pcnn_ctx *ctx, const void *x_bf16_dev, const float *filt_f32_dev, const float *bias_f32_dev, void *y_bf16_dev,
+                            int N, int H, int W, int C_in, int C_out, int R, int S, int stride, int pad_h, int pad_w, int op_h, int op_w,
+                            int row_pitch, int image_rows, int act);
+/* Bilinear resizing (csrc/upsample_nhwc.cu), as torch.nn.functional.interpolate(x, size=(H_out, W_out), mode="bilinear",
+ * align_corners=False) without antialiasing, up or down, on dense bf16 NHWC maps: x and dx [N][H][W][C], y and dy
+ * [N][H_out][W_out][C], any C.  RN is an fp32 operation rounded to nearest, never contracted.  Per axis (in -> out):
+ *     scale = RN32(float(in) / float(out));
+ *     in == out: i0 = i1 = d, l0 = 1, l1 = 0, decided per axis as torch's CPU kernel decides it (compute_source_index_and_lambda);
+ *               torch's CUDA kernel copies only when both axes are unchanged and otherwise takes the general taps, so with one axis
+ *               unchanged it reads the neighbour at weight 0 there: a +-Inf neighbour gives NaN on torch's GPU, not here (the
+ *               same-index 0 * Inf of a non-finite pixel itself is NaN in both);
+ *     otherwise real = RN(RN(scale * RN(d + 0.5)) - 0.5), then real = 0 if real < 0; i0 = min(floor(real), in - 1);
+ *               l1 = min(max(RN(real - i0), 0), 1); l0 = RN(1 - l1); i1 = i0 + 1 if i0 < in - 1, else i0.
+ * Forward: top = RN(RN(lw0 * x[i0][j0]) + RN(lw1 * x[i0][j1])), bot the same on row i1 (bf16_rn writes every NaN as 0x7FFF),
+ *          y[n][h][w][c] = bf16_rn(RN(RN(lh0 * top) + RN(lh1 * bot))).  A 0 weight times +-Inf is NaN, as in torch.
+ * Backward, a gather with no atomics: a tap's weight on input index i is l0 if only i0 == i, l1 if only i1 == i and RN(l0 + l1) if
+ * both are i; dx[n][i][j][c] = bf16_rn(s), s summed in fp32 from +0 over the output rows h ascending, then the output columns w
+ * ascending, whose taps reach (i, j), of RN(RN(wh * ww) * dy[n][h][w][c]).  Reruns give the same bits; torch's CUDA backward adds
+ * with atomics, so parity with it is an error bound, not bits.  Every element of y / dx is written, nothing else.
+ * Domain (PCNN_ERR_ARG, one message per rule): N, C >= 1; H, W, H_out, W_out 1 .. 16384; each map below 2^62 bytes; x and y
+ * 16-byte aligned when C % 8 == 0 (the 8-channel vector path); the two maps must not overlap.
+ * pcnn_upsample_bilinear_info (host only) refuses the same and fills out4 = { channels per thread (8 or 1), forward grid,
+ * backward grid, threads per CTA }. */
+int pcnn_upsample_bilinear_info(int N, int H, int W, int C, int H_out, int W_out, long long *out4);
+int pcnn_upsample_bilinear_nhwc_bf16_fwd(pcnn_ctx *ctx, const void *x_bf16_dev, void *y_bf16_dev, int N, int H, int W, int C, int H_out,
+                                         int W_out);
+int pcnn_upsample_bilinear_nhwc_bf16_bwd(pcnn_ctx *ctx, const void *dy_bf16_dev, void *dx_bf16_dev, int N, int H, int W, int C, int H_out,
+                                         int W_out);
+/* Per-pixel softmax cross-entropy with an ignore index (csrc/linear_tc.cu), as F.cross_entropy(logits, target,
+ * ignore_index=ignore_index) with mean reduction: logits dense bf16 [pixels][O] (1 <= O <= 256), targets uint8 [pixels],
+ * ignore_index 0..255 or -1 (none).  Two launches: the first writes count_i32[0] = the number of targets != ignore_index, counted
+ * exactly with integer atomics; the second forms scale = fp32(1.0 / double(count)) on the device and runs pcnn_softmax_ce_bf16's
+ * kernel with it, so a row whose target is not ignored is bit for bit pcnn_softmax_ce_bf16's row at that scale (a target >= O gives
+ * a NaN row, a NaN logit a NaN row and pred -1).  An ignored row gets dlogits +0 and loss 0 whatever its logits; pred is the
+ * argmax of every row (-1 for a NaN row).  count 0 makes every row ignored: no NaN dlogits, and the mean loss sum(loss) / count is
+ * NaN, as torch's 0 / 0.  loss and pred may be NULL; dlogits == logits (in place) is allowed, no other overlap is.  Domain
+ * (PCNN_ERR_ARG): pixels >= 1, 1 <= O <= 256, -1 <= ignore_index <= 255, no NULL context, logits, targets, dlogits or count. */
+int pcnn_softmax_ce_pixels_bf16(pcnn_ctx *ctx, const void *logits_bf16_dev, const uint8_t *targets_dev, int pixels, int O, int ignore_index,
+                                void *dlogits_bf16_dev, float *loss_f32_dev, int *pred_i32_dev, int *count_i32_dev);
+/* Segmentation masks for pcnn_augment_u8_bf16's batch (csrc/augment.cu): masks uint8 [n][H][W] -> masks_out uint8 dense [N][H][W].
+ * With the same n, H, W, first, N, shuffle, pad, flip, seed and epoch as the image call, position e = first + j takes mask pi(e)
+ * with the crop offsets and flip of the same Philox block the image kernel reads (that kernel is not changed):
+ *     masks_out[j][h][w] = masks[pi(e)][h + oy - pad][w' + ox - pad], w' = flip ? W - 1 - w : w,  mask_fill outside the mask,
+ * as torchvision's v2.RandomCrop(padding=pad, fill={Mask: mask_fill}) and RandomHorizontalFlip on a tv_tensors.Mask.  shuffle 0,
+ * pad 0, flip 0 (an eval batch) copies masks first .. first + N - 1.  Domain: the plain call's rules at C = C_out = 1 with its
+ * messages, 0 <= mask_fill <= 255, masks_out disjoint from masks. */
+int pcnn_augment_mask_u8(pcnn_ctx *ctx, const uint8_t *masks_dev, long long n, int H, int W, long long first, int N, int shuffle, int pad,
+                         int flip, unsigned long long seed, unsigned long long epoch, int mask_fill, uint8_t *masks_out_dev);
 /* Optimizers for device-trained layers (csrc/optim.cu): one fused update of every parameter tensor of a network per step, as
  * torch.optim.SGD and torch.optim.AdamW (decoupled weight decay) in their single-tensor form, with the bf16 operands of the plans
  * the parameters belong to refreshed in the same pass.

@@ -198,6 +198,13 @@ _SIG = {
                                          + [_i] + [C.c_double] * 5 + [_i, _i, _i, _vp, _vp, _vp, _vp, _vp],
     "pcnn_softmax_ce_bf16": [_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp],
     "pcnn_softmax_ce_soft_bf16": [_vp, _vp, _vp, _vp, C.c_double, C.c_double, _i, _i, _f, _vp, _vp, _vp],
+    "pcnn_softmax_ce_pixels_bf16": [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp],
+    "pcnn_conv_transpose_info": [_i] * 16 + [_vp],
+    "pcnn_conv_transpose_fwd": [_vp, _vp, _vp, _vp, _vp] + [_i] * 15,
+    "pcnn_upsample_bilinear_info": [_i] * 6 + [_vp],
+    "pcnn_upsample_bilinear_nhwc_bf16_fwd": [_vp, _vp, _vp] + [_i] * 6,
+    "pcnn_upsample_bilinear_nhwc_bf16_bwd": [_vp, _vp, _vp] + [_i] * 6,
+    "pcnn_augment_mask_u8": [_vp, _vp, C.c_longlong, _i, _i, C.c_longlong, _i, _i, _i, _i, C.c_ulonglong, C.c_ulonglong, _i, _vp],
     "pcnn_optim_create": [_vp, _vp, _vp, _i, _pvp],
     "pcnn_optim_step": [_vp, _vp, _f],
     "pcnn_optim_state": [_vp, _i, _pvp, _pvp],
@@ -284,6 +291,27 @@ def conv_wide_bwd_info(N, H, W, C, K, R, S, stride=1, row_pitch=None, image_rows
               lib().pcnn_conv_wide_bwd_info_padded(N, H, W, C, K, R, S, int(stride), ph, pw, int(pitch), int(image_rows), out))
     return dict(wgrad_row_blocks=out[0], wgrad_splits=out[1], wgrad_blocks_per_split=out[2], wgrad_stages=out[3], wgrad_units=out[4],
                 dgrad_Pt=out[5], dgrad_Qt=out[6], dgrad_groups=out[7], dgrad_stages=out[8], dgrad_tiles=out[9])
+
+
+def conv_transpose_info(N, H, W, C_in, C_out, R, S, stride=1, padding=(0, 0), output_padding=(0, 0), row_pitch=None, image_rows=0,
+                        bias=False, act=0):
+    """The output size, layout and input-gradient tiling of a transposed convolution (pcnn_conv_transpose_info; host only, no GPU),
+    refused as pcnn_conv_transpose_fwd refuses.  row_pitch None = W_out * C_out (dense), image_rows 0 = H_out."""
+    ph, pw = (int(v) for v in padding)
+    oh, ow = (int(v) for v in output_padding)
+    out = (_i * 8)()
+    check("pcnn_conv_transpose_info", lib().pcnn_conv_transpose_info(int(N), int(H), int(W), int(C_in), int(C_out), int(R), int(S), int(stride),
+                                                                     ph, pw, oh, ow, int(row_pitch or 0), int(image_rows), int(bool(bias)),
+                                                                     int(act), out))
+    return dict(H_out=out[0], W_out=out[1], row_pitch=out[2], image_rows=out[3], Pt=out[4], Qt=out[5], groups=out[6], tiles=out[7])
+
+
+def upsample_bilinear_info(N, H, W, Cin, H_out, W_out):
+    """How the bilinear resize partitions a shape (pcnn_upsample_bilinear_info; host only, no GPU), refused as its two passes
+    refuse.  vec: channels per thread (8 or 1)."""
+    out = (C.c_longlong * 4)()
+    check("pcnn_upsample_bilinear_info", lib().pcnn_upsample_bilinear_info(int(N), int(H), int(W), int(Cin), int(H_out), int(W_out), out))
+    return dict(vec=out[0], grid_fwd=out[1], grid_bwd=out[2], threads=out[3])
 
 
 def conv_layer_family(N, H, W, C, K, R, S, stride=1, padding=(0, 0), row_pitch=None, image_rows=0):

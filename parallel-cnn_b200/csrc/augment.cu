@@ -376,6 +376,64 @@ extern "C" int pcnn_augment_u8_bf16(pcnn_ctx *ctx, const uint8_t *images_dev, co
     return aug_launch(ctx, s);
 }
 
+// ------------------------------------------------------------------------------------------------ segmentation masks
+// pcnn_augment_mask_u8: the uint8 masks [n][H][W] of the plain call's batch, each moved exactly as its image: position e of the
+// epoch takes mask pi(e) with the crop and flip of draw_unit, the same Philox block the image kernel reads.  One CTA per batch
+// position; the padding reads fill.
+namespace {
+
+__global__ void __launch_bounds__(AUG_THREADS) k_augment_mask(const __grid_constant__ AugArgs a, const uint8_t *__restrict__ masks,
+                                                              uint8_t *__restrict__ out, long long N, int fill) {
+    __shared__ unsigned long long s_i;
+    __shared__ int s_oy, s_ox, s_fl;
+    const int hw = a.H * a.W;
+    for (long long j = blockIdx.x; j < N; j += gridDim.x) {
+        if (threadIdx.x == 0) {
+            unsigned long long i;
+            int oy, ox, fl;
+            draw_unit((unsigned long long)(a.first + j), a, i, oy, ox, fl);
+            s_i = i;
+            s_oy = oy - a.pad;
+            s_ox = ox - a.pad;
+            s_fl = fl;
+        }
+        __syncthreads();
+        const uint8_t *src = masks + (long long)s_i * hw;
+        for (int p = threadIdx.x; p < hw; p += AUG_THREADS) {
+            const int h = p / a.W, w = p - h * a.W;
+            const int sy = h + s_oy, sx = (s_fl ? a.W - 1 - w : w) + s_ox;
+            out[j * hw + p] = (unsigned)sy < (unsigned)a.H && (unsigned)sx < (unsigned)a.W ? __ldg(src + (long long)sy * a.W + sx)
+                                                                                            : (uint8_t)fill;
+        }
+        __syncthreads();                                    // s_i .. s_fl are rewritten by the next position
+    }
+}
+
+}  // namespace
+
+extern "C" int pcnn_augment_mask_u8(pcnn_ctx *ctx, const uint8_t *masks_dev, long long n, int H, int W, long long first, int N, int shuffle,
+                                    int pad, int flip, unsigned long long seed, unsigned long long epoch, int mask_fill,
+                                    uint8_t *masks_out_dev) {
+    const char *fn = "pcnn_augment_mask_u8";
+    PCNN_REQUIRE(ctx && masks_dev && masks_out_dev, PCNN_ERR_ARG, "%s: NULL context, masks or masks_out", fn);
+    PCNN_REQUIRE(mask_fill >= 0 && mask_fill <= 255, PCNN_ERR_ARG, "%s: mask_fill = %d: 0 .. 255 is required", fn, mask_fill);
+    AugShape s;
+    const int rc = aug_shape(fn, n, H, W, 1, first, N, shuffle, pad, flip, 1, 0, 0, nullptr, nullptr, &s);
+    if (rc) return rc;
+    PCNN_REQUIRE(disjoint(masks_out_dev, (size_t)N * H * W, masks_dev, (size_t)n * H * W), PCNN_ERR_ARG,
+                 "%s: overlapping buffers: masks_out must share no byte with masks", fn);
+    AugArgs &a = s.a;
+    a.k0 = (unsigned)seed;
+    a.k1 = (unsigned)(seed >> 32);
+    a.e0 = (unsigned)epoch;
+    a.e1 = (unsigned)(epoch >> 32);
+    pcnn_device_guard dg(ctx->device);
+    const int grid = (int)std::min<long long>(AUG_MAX_GRID, N);
+    k_augment_mask<<<grid, AUG_THREADS, 0, ctx->stream>>>(a, masks_dev, masks_out_dev, N, mask_fill);
+    PCNN_CHECK_LAUNCH(ctx);
+    return PCNN_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ resized batches
 // pcnn_augment_resized_u8_bf16: RandomResizedCrop (mode 1) or Resize + CenterCrop (mode 2) by torch's uint8 antialiased bilinear
 // resample, the fixed-point separable rule include/pcnn.h states.  A CTA takes one (batch position, block of output rows) unit:

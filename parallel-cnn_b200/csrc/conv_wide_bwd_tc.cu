@@ -37,6 +37,8 @@
 
 #include <cuda_bf16.h>
 
+#include <type_traits>
+
 using namespace pcnn_tc;
 
 namespace {
@@ -179,6 +181,15 @@ struct WideDgradParams {
     int rho_w[4], off_w[4];          // column phase b: the same with pad_w
 };
 
+// what the transposed convolution's epilogue (EPI) adds: bias [C] or NULL, the activation and the channel count C
+struct WideDgradEpiParams : WideDgradParams {
+    const float *bias;
+    int act, C;
+};
+
+template <bool EPI>
+using DgradParamsOf = typename std::conditional<EPI, WideDgradEpiParams, WideDgradParams>::type;
+
 struct WideDgradMaps {
     CUtensorMap dx[16];              // phase (a, b) of dx at index a * st + b: {C, ceil((W-b)/st), ceil((H-a)/st), N}
     CUtensorMap dy;                  // {K, Q, P, N}, box {64, Qt, Pt, 1}
@@ -201,9 +212,12 @@ __device__ __forceinline__ DgradTile dgrad_tile(const WideDgradParams &p, int ti
     return d;
 }
 
-template <int N>   // channels per tile, rounded up to 16
+// EPI false: the input gradient, the accumulator rounded to bf16.  EPI true: the forward of a transposed convolution, whose output
+// is this input gradient, with v = accumulator + bias[c] (the accumulator itself without a bias) and the activation p.act applied in fp32 before the
+// rounding, as the forward epilogues do (PCNN_ACT_*).
+template <int N, bool EPI = false>   // N: channels per tile, rounded up to 16
 __global__ void __launch_bounds__(WB_THREADS, 1)
-k_conv_wide_dgrad(const __grid_constant__ WideDgradMaps m, const WideDgradParams p) {
+k_conv_wide_dgrad(const __grid_constant__ WideDgradMaps m, const DgradParamsOf<EPI> p) {
     constexpr int NSUB = (N + 63) / 64;
     constexpr int B_BYTES = N * WB_KC * 2;
     constexpr int A_BYTES = WB_BOX_BYTES;
@@ -291,7 +305,17 @@ k_conv_wide_dgrad(const __grid_constant__ WideDgradMaps m, const WideDgradParams
             const int row = wg_row(2 * h, wq, lane);
 #pragma unroll
             for (int j = 0; j < N / 8; ++j) {
-                __nv_bfloat162 v = __floats2bfloat162_rn(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+                if constexpr (EPI) {
+                    const int c = d.g * p.G + wg_col(4 * j, lane);
+                    if (p.bias) {
+                        f0 = __fadd_rn(f0, c < p.C ? __ldg(p.bias + c) : 0.0f);
+                        f1 = __fadd_rn(f1, c + 1 < p.C ? __ldg(p.bias + c + 1) : 0.0f);
+                    }
+                    if (p.act == PCNN_ACT_SIGMOID) { f0 = apply_act<PCNN_ACT_SIGMOID>(f0); f1 = apply_act<PCNN_ACT_SIGMOID>(f1); }
+                    else if (p.act == PCNN_ACT_RELU) { f0 = apply_act<PCNN_ACT_RELU>(f0); f1 = apply_act<PCNN_ACT_RELU>(f1); }
+                }
+                __nv_bfloat162 v = __floats2bfloat162_rn(f0, f1);
                 const uint32_t addr = stg_s + (uint32_t)((j / 8) * WB_STG_BYTES + row * 128 + (((j % 8) ^ (row & 7)) << 4) + (lane & 3) * 4);
                 asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(*reinterpret_cast<uint32_t *>(&v)) : "memory");
             }
@@ -391,18 +415,20 @@ int dense_dy_map(CUtensorMap *map, const void *dy, int N, int P, int Q, int K, i
 }
 
 typedef void (*wgrad_fn)(const WideWgradMaps, const WideWgradParams);
-typedef void (*dgrad_fn)(const WideDgradMaps, const WideDgradParams);
 const void *wgrad_variant(int n64) {
     static const wgrad_fn table[4] = {k_conv_wide_wgrad<64>, k_conv_wide_wgrad<128>, k_conv_wide_wgrad<192>, k_conv_wide_wgrad<256>};
     return reinterpret_cast<const void *>(table[n64 / 64 - 1]);
 }
-const void *dgrad_variant(int n16) {
-    static const dgrad_fn table[16] = {k_conv_wide_dgrad<16>,  k_conv_wide_dgrad<32>,  k_conv_wide_dgrad<48>,  k_conv_wide_dgrad<64>,
-                                       k_conv_wide_dgrad<80>,  k_conv_wide_dgrad<96>,  k_conv_wide_dgrad<112>, k_conv_wide_dgrad<128>,
-                                       k_conv_wide_dgrad<144>, k_conv_wide_dgrad<160>, k_conv_wide_dgrad<176>, k_conv_wide_dgrad<192>,
-                                       k_conv_wide_dgrad<208>, k_conv_wide_dgrad<224>, k_conv_wide_dgrad<240>, k_conv_wide_dgrad<256>};
-    return reinterpret_cast<const void *>(table[n16 / 16 - 1]);
+#define PCNN_DGRAD_ROW(N) \
+    {reinterpret_cast<const void *>(k_conv_wide_dgrad<N, false>), reinterpret_cast<const void *>(k_conv_wide_dgrad<N, true>)}
+const void *dgrad_variant(int n16, bool epi = false) {
+    static const void *const table[16][2] = {
+        PCNN_DGRAD_ROW(16),  PCNN_DGRAD_ROW(32),  PCNN_DGRAD_ROW(48),  PCNN_DGRAD_ROW(64),  PCNN_DGRAD_ROW(80),  PCNN_DGRAD_ROW(96),
+        PCNN_DGRAD_ROW(112), PCNN_DGRAD_ROW(128), PCNN_DGRAD_ROW(144), PCNN_DGRAD_ROW(160), PCNN_DGRAD_ROW(176), PCNN_DGRAD_ROW(192),
+        PCNN_DGRAD_ROW(208), PCNN_DGRAD_ROW(224), PCNN_DGRAD_ROW(240), PCNN_DGRAD_ROW(256)};
+    return table[n16 / 16 - 1][epi ? 1 : 0];
 }
+#undef PCNN_DGRAD_ROW
 
 int configure(pcnn_ctx *ctx) {
     static bool configured[64] = {};        // function attributes are per device
@@ -410,7 +436,9 @@ int configure(pcnn_ctx *ctx) {
         for (int v = 1; v <= 4; ++v)
             PCNN_CUDA(cudaFuncSetAttribute(wgrad_variant(64 * v), cudaFuncAttributeMaxDynamicSharedMemorySize, WB_SMEM_BUDGET + 2048));
         for (int v = 1; v <= 16; ++v)
-            PCNN_CUDA(cudaFuncSetAttribute(dgrad_variant(16 * v), cudaFuncAttributeMaxDynamicSharedMemorySize, WB_SMEM_BUDGET + 2048));
+            for (int epi = 0; epi < 2; ++epi)
+                PCNN_CUDA(cudaFuncSetAttribute(dgrad_variant(16 * v, epi != 0), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               WB_SMEM_BUDGET + 2048));
         configured[ctx->device & 63] = true;
     }
     return PCNN_OK;
@@ -457,8 +485,10 @@ static int wide_wgrad(const char *fn, pcnn_ctx *ctx, const void *x_bf16, const v
     return pcnn_conv_wgrad_reduce_slots(ctx, p.slots, dw_f32, p.splits, nout);
 }
 
+// epi: the transposed convolution's forward (bias may be NULL, act PCNN_ACT_*); otherwise bias and act are unused
 static int wide_dgrad(const char *fn, pcnn_ctx *ctx, const void *dy_bf16, const float *filt_f32_dev, void *dx_bf16, int N, int H, int W,
-                      int C, int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch, int image_rows) {
+                      int C, int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch, int image_rows, bool epi = false,
+                      const float *bias = nullptr, int act = PCNN_ACT_NONE) {
     PCNN_REQUIRE(ctx && dy_bf16 && filt_f32_dev && dx_bf16, PCNN_ERR_ARG, "%s: NULL argument", fn);
     WideBwdPlan pl;
     int rc = wide_bwd_plan(fn, N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows, &pl);
@@ -500,9 +530,14 @@ static int wide_dgrad(const char *fn, pcnn_ctx *ctx, const void *dy_bf16, const 
         if ((rc = make_map_bf16(&m.f, ftck, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
     }
     WideDgradParams pp = p;
+    WideDgradEpiParams pe;
+    static_cast<WideDgradParams &>(pe) = p;
+    pe.bias = bias;
+    pe.act = act;
+    pe.C = C;
     const int grid = pl.d_tiles < ctx->sm_count ? pl.d_tiles : ctx->sm_count;
-    void *args[] = {&m, &pp};
-    PCNN_CUDA(cudaLaunchKernel(dgrad_variant(pl.dn), dim3((unsigned)grid), dim3(WB_THREADS), args,
+    void *args[] = {&m, epi ? static_cast<void *>(&pe) : static_cast<void *>(&pp)};
+    PCNN_CUDA(cudaLaunchKernel(dgrad_variant(pl.dn, epi), dim3((unsigned)grid), dim3(WB_THREADS), args,
                                dgrad_staging_bytes(pl.dn) + (size_t)pp.stages * dgrad_stage_bytes(pl.dn) + sizeof(WideCtl) + 1024, ctx->stream));
     PCNN_CHECK_LAUNCH(ctx);
     return PCNN_OK;
@@ -540,4 +575,68 @@ extern "C" int pcnn_conv_wide_dgrad_padded(pcnn_ctx *ctx, const void *dy_bf16, c
                                            int image_rows) {
     return wide_dgrad("pcnn_conv_wide_dgrad_padded", ctx, dy_bf16, filt_f32_dev, dx_bf16, N, H, W, C, K, R, S, stride, pad_h, pad_w,
                       row_pitch, image_rows);
+}
+
+// ================================================= transposed convolution ===============================================
+// conv_transpose2d(x, w, b, stride, padding, output_padding) is the input gradient of its adjoint convolution: input H_out x W_out
+// x C_out, K = C_in filters f[ci][r][s][co] = w[ci][co][r][s], the same stride and padding, whose output is H x W.  The rules below
+// are stated in the transposed convolution's own terms before the adjoint's shape rules (pitch, plan split) are checked.
+static int conv_transpose_shape(const char *fn, int N, int H, int W, int C_in, int C_out, int R, int S, int stride, int pad_h, int pad_w,
+                                int op_h, int op_w, int has_bias, int act, int *H_out, int *W_out, WideBwdPlan *pl, int row_pitch,
+                                int image_rows) {
+    PCNN_REQUIRE(N >= 1 && H >= 1 && W >= 1, PCNN_ERR_ARG, "%s: N = %d, H = %d, W = %d: each must be >= 1", fn, N, H, W);
+    PCNN_REQUIRE(C_in >= 8 && C_in % 8 == 0 && C_in <= 256, PCNN_ERR_ARG,
+                 "%s: C_in = %d: C_in %% 8 == 0 and 8 <= C_in <= 256 are required (the adjoint convolution's filters)", fn, C_in);
+    PCNN_REQUIRE(C_out >= 8 && C_out % 8 == 0, PCNN_ERR_ARG, "%s: C_out = %d: C_out %% 8 == 0 and C_out >= 8 are required", fn, C_out);
+    PCNN_REQUIRE(!(has_bias || act != PCNN_ACT_NONE) || C_out <= 256, PCNN_ERR_ARG,
+                 "%s: C_out = %d with a bias or an activation: C_out <= 256 is required (pcnn_conv_bias_act_bwd)", fn, C_out);
+    PCNN_REQUIRE_ACT(fn, act);
+    PCNN_REQUIRE(stride >= 1 && stride <= 4, PCNN_ERR_ARG, "%s: stride %d outside 1..4", fn, stride);
+    PCNN_REQUIRE(R >= 1 && R <= 7 && S >= 1 && S <= 7, PCNN_ERR_ARG, "%s: R = %d, S = %d: taps must be 1..7 in each direction", fn, R, S);
+    PCNN_REQUIRE(pad_h >= 0 && pad_h < R && pad_w >= 0 && pad_w < S, PCNN_ERR_ARG,
+                 "%s: padding (%d, %d) with R = %d, S = %d taps: 0 <= pad_h <= R - 1 and 0 <= pad_w <= S - 1 are required", fn, pad_h,
+                 pad_w, R, S);
+    PCNN_REQUIRE(op_h >= 0 && op_h < stride && op_w >= 0 && op_w < stride, PCNN_ERR_ARG,
+                 "%s: output_padding (%d, %d) at stride %d: 0 <= output_padding < stride is required", fn, op_h, op_w, stride);
+    const long long ho = (long long)(H - 1) * stride - 2LL * pad_h + R + op_h, wo = (long long)(W - 1) * stride - 2LL * pad_w + S + op_w;
+    PCNN_REQUIRE(ho >= 1 && wo >= 1 && ho < (1 << 24) && wo < (1 << 24), PCNN_ERR_ARG,
+                 "%s: output %lld x %lld: H_out = (H - 1) stride - 2 pad_h + R + output_padding_h (and W_out the same) must be 1 .. 2^24 - 1",
+                 fn, ho, wo);
+    PCNN_REQUIRE((pad_h == 0 || ho >= stride) && (pad_w == 0 || wo >= stride), PCNN_ERR_ARG,
+                 "%s: output %lld x %lld with padding (%d, %d) at stride %d: a padded direction needs an output of at least stride "
+                 "rows / pixels", fn, ho, wo, pad_h, pad_w, stride);
+    *H_out = (int)ho;
+    *W_out = (int)wo;
+    return wide_bwd_plan(fn, N, (int)ho, (int)wo, C_out, C_in, R, S, stride, pad_h, pad_w, row_pitch == 0 ? (int)wo * C_out : row_pitch,
+                         image_rows, pl);
+}
+
+extern "C" int pcnn_conv_transpose_info(int N, int H, int W, int C_in, int C_out, int R, int S, int stride, int pad_h, int pad_w, int op_h,
+                                        int op_w, int row_pitch, int image_rows, int has_bias, int act, int *out8) {
+    const char *fn = "pcnn_conv_transpose_info";
+    PCNN_REQUIRE(out8, PCNN_ERR_ARG, "%s: NULL out8", fn);
+    WideBwdPlan pl;
+    int ho, wo;
+    const int rc = conv_transpose_shape(fn, N, H, W, C_in, C_out, R, S, stride, pad_h, pad_w, op_h, op_w, has_bias, act, &ho, &wo, &pl,
+                                        row_pitch, image_rows);
+    if (rc) return rc;
+    out8[0] = ho; out8[1] = wo;
+    out8[2] = row_pitch == 0 ? wo * C_out : row_pitch; out8[3] = image_rows > 0 ? image_rows : ho;
+    out8[4] = pl.d.Pt; out8[5] = pl.d.Qt; out8[6] = pl.d.ngroups; out8[7] = pl.d_tiles;
+    return PCNN_OK;
+}
+
+extern "C" int pcnn_conv_transpose_fwd(pcnn_ctx *ctx, const void *x_bf16_dev, const float *filt_f32_dev, const float *bias_f32_dev,
+                                       void *y_bf16_dev, int N, int H, int W, int C_in, int C_out, int R, int S, int stride, int pad_h,
+                                       int pad_w, int op_h, int op_w, int row_pitch, int image_rows, int act) {
+    const char *fn = "pcnn_conv_transpose_fwd";
+    PCNN_REQUIRE(ctx && x_bf16_dev && filt_f32_dev && y_bf16_dev, PCNN_ERR_ARG, "%s: NULL context, x, filters or y (only the bias may be NULL)",
+                 fn);
+    WideBwdPlan pl;
+    int ho, wo;
+    const int rc = conv_transpose_shape(fn, N, H, W, C_in, C_out, R, S, stride, pad_h, pad_w, op_h, op_w, bias_f32_dev != nullptr, act, &ho,
+                                        &wo, &pl, row_pitch, image_rows);
+    if (rc) return rc;
+    return wide_dgrad(fn, ctx, x_bf16_dev, filt_f32_dev, y_bf16_dev, N, ho, wo, C_out, C_in, R, S, stride, pad_h, pad_w,
+                      row_pitch == 0 ? wo * C_out : row_pitch, image_rows, true, bias_f32_dev, act);
 }

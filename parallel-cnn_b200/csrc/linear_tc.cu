@@ -354,9 +354,13 @@ struct SoftTarget {
     const uint8_t *labels_b;  // NULL: m_t = [t == label]
     float lam, oml;           // RN32(lam), RN32(1 - lam)
     float ome, eps_o;         // RN32(1 - eps), RN32(eps / O)
+    const int *count;         // PIXELS: the non-ignored rows, counted by k_count_targets
+    int ignore;               // PIXELS: the ignored target, -1 for none
 };
 
-template <bool SOFT>
+// PIXELS (hard target only): pcnn_softmax_ce_pixels_bf16.  The scale is RN32(1 / count) read from the device; a row whose target is
+// st.ignore gets dlogits +0 and loss 0; every other row is exactly the hard call's at that scale.
+template <bool SOFT, bool PIXELS = false>
 __global__ void __launch_bounds__(256) k_softmax_ce_bf16(const __nv_bfloat16 *z, const uint8_t *__restrict__ labels, int N, int O,
                                                          double scale, __nv_bfloat16 *d, float *__restrict__ loss, int *__restrict__ pred,
                                                          const SoftTarget st) {
@@ -394,6 +398,19 @@ __global__ void __launch_bounds__(256) k_softmax_ce_bf16(const __nv_bfloat16 *z,
             if (lane + 32 * j < O) den += exp((double)v[j] - mx);
         for (int s = 16; s; s >>= 1) den += __shfl_xor_sync(0xffffffffu, den, s);
         const int y = labels[r];
+        if constexpr (PIXELS) {
+            if (y == st.ignore) {
+#pragma unroll
+                for (int j = 0; j < 8; ++j)
+                    if (lane + 32 * j < O) d[r * O + lane + 32 * j] = __float2bfloat16_rn(0.0f);
+                if (lane == 0) {
+                    if (loss) loss[r] = 0.0f;
+                    if (pred) pred[r] = nan ? -1 : bi;
+                }
+                continue;
+            }
+            scale = (double)(float)(1.0 / (double)*st.count);
+        }
         if constexpr (!SOFT) {
             const bool bad = nan || y >= O;
 #pragma unroll
@@ -443,6 +460,21 @@ __global__ void __launch_bounds__(256) k_softmax_ce_bf16(const __nv_bfloat16 *z,
             if (loss && (one_hot ? hot : lane == 0)) loss[r] = bad ? NAN : one_hot ? lhot : (float)(-part);
             if (lane == 0 && pred) pred[r] = nan ? -1 : bi;
         }
+    }
+}
+
+// count[0] = the targets that are not `ignore` (-1: all): per-CTA counts added with integer atomics, which are exact in any order
+__global__ void __launch_bounds__(256) k_count_targets(const uint8_t *__restrict__ t, long n, int ignore, int *count) {
+    int c = 0;
+    for (long i = blockIdx.x * 256L + threadIdx.x; i < n; i += (long)gridDim.x * 256) c += (int)t[i] != ignore;
+    for (int s = 16; s; s >>= 1) c += __shfl_xor_sync(0xffffffffu, c, s);
+    __shared__ int part[8];
+    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = c;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int sum = 0;
+        for (int w = 0; w < 8; ++w) sum += part[w];
+        atomicAdd(count, sum);
     }
 }
 
@@ -749,6 +781,36 @@ extern "C" int pcnn_softmax_ce_soft_bf16(pcnn_ctx *ctx, const void *logits_bf16,
     k_softmax_ce_bf16<true><<<(int)blocks, 256, 0, ctx->stream>>>(static_cast<const __nv_bfloat16 *>(logits_bf16), labels, N, O,
                                                                   (double)scale, static_cast<__nv_bfloat16 *>(dlogits_bf16), loss_f32,
                                                                   pred_i32, st);
+    PCNN_CHECK_LAUNCH(ctx);
+    return PCNN_OK;
+}
+
+extern "C" int pcnn_softmax_ce_pixels_bf16(pcnn_ctx *ctx, const void *logits_bf16, const uint8_t *targets, int pixels, int O, int ignore_index,
+                                           void *dlogits_bf16, float *loss_f32, int *pred_i32, int *count_i32) {
+    const char *fn = "pcnn_softmax_ce_pixels_bf16";
+    PCNN_REQUIRE(ctx && logits_bf16 && targets && dlogits_bf16 && count_i32, PCNN_ERR_ARG,
+                 "%s: NULL context, logits, targets, dlogits or count (only loss and pred may be NULL)", fn);
+    PCNN_REQUIRE(pixels >= 1 && O >= 1 && O <= 256, PCNN_ERR_ARG, "%s: pixels = %d, O = %d: pixels >= 1 and 1 <= O <= 256 are required", fn,
+                 pixels, O);
+    PCNN_REQUIRE(ignore_index >= -1 && ignore_index <= 255, PCNN_ERR_ARG, "%s: ignore_index = %d: -1 (none) or 0 .. 255 is required", fn,
+                 ignore_index);
+    const size_t zb = (size_t)pixels * O * 2;
+    const uintptr_t z = (uintptr_t)logits_bf16, d = (uintptr_t)dlogits_bf16;
+    PCNN_REQUIRE(d == z || d + zb <= z || z + zb <= d, PCNN_ERR_ARG, "%s: dlogits overlaps logits without being the same buffer", fn);
+    pcnn_device_guard g(ctx->device);
+    PCNN_CUDA(cudaMemsetAsync(count_i32, 0, sizeof(int), ctx->stream));
+    long cblocks = ((long)pixels + 255) / 256;
+    if (cblocks > (long)ctx->sm_count * 4) cblocks = (long)ctx->sm_count * 4;
+    k_count_targets<<<(int)cblocks, 256, 0, ctx->stream>>>(targets, pixels, ignore_index, count_i32);
+    PCNN_CHECK_LAUNCH(ctx);
+    SoftTarget st{};
+    st.count = count_i32;
+    st.ignore = ignore_index;
+    long blocks = ((long)pixels * 32 + 255) / 256;
+    if (blocks > (long)ctx->sm_count * 8) blocks = (long)ctx->sm_count * 8;
+    k_softmax_ce_bf16<false, true><<<(int)blocks, 256, 0, ctx->stream>>>(static_cast<const __nv_bfloat16 *>(logits_bf16), targets, pixels, O,
+                                                                         0.0, static_cast<__nv_bfloat16 *>(dlogits_bf16), loss_f32,
+                                                                         pred_i32, st);
     PCNN_CHECK_LAUNCH(ctx);
     return PCNN_OK;
 }

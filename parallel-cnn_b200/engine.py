@@ -8,7 +8,7 @@ import numpy as np
 
 from ._lib import (F32, NPARAM, OPTIM_ADAMW, OPTIM_SGD, TEST_SET, TRAIN_SET, U8, OptimConfig, OptimTensor, PcnnError, augment_info,
                    augment_resized_info, RESIZE_TRAIN, RESIZE_EVAL, augment_trivial_info, TRIVIAL_NONE, TRIVIAL_NEAREST, TRIVIAL_BILINEAR,
-                   avgpool_nhwc_info, batchnorm_nhwc_info, channel_stats, check, conv_layer_family, dropout_info, dwconv_info, gconv_info, global_avgpool_nhwc_info, lib, linear_info,
+                   avgpool_nhwc_info, batchnorm_nhwc_info, channel_stats, check, conv_layer_family, conv_transpose_info, upsample_bilinear_info, dropout_info, dwconv_info, gconv_info, global_avgpool_nhwc_info, lib, linear_info,
                    maxpool_nhwc_info,
                    se_scale_nhwc_info, ACT_RELU, ACT_SIGMOID, ACT_SILU, ACT_HARDSWISH, ACT_RELU6)
 
@@ -505,6 +505,39 @@ class Engine:
         self._call("pcnn_softmax_ce_soft_bf16", _p(logits), _p(labels), _p(labels_b), float(lam), float(smoothing), int(N), int(O),
                    float(scale), _p(dlogits), _p(loss), _p(pred))
 
+    def softmax_ce_pixels_bf16(self, logits, targets, pixels, O, ignore_index, dlogits, count, loss=None, pred=None):
+        """pcnn_softmax_ce_pixels_bf16: cross_entropy(ignore_index=ignore_index) with mean reduction over bf16 logits [pixels][O]
+        and uint8 targets [pixels].  count (device int32 [1]) receives the non-ignored pixels; every other row gets
+        softmax_ce_bf16's row at scale RN32(1 / count); ignored rows get dlogits +0 and loss 0.  ignore_index -1 ignores none."""
+        self._call("pcnn_softmax_ce_pixels_bf16", _p(logits), _p(targets), int(pixels), int(O), int(ignore_index), _p(dlogits), _p(loss),
+                   _p(pred), _p(count))
+
+    def conv_transpose_fwd(self, x, filt, bias, y, N, H, W, C_in, C_out, R, S, stride=1, padding=(0, 0), output_padding=(0, 0), row_pitch=0,
+                           image_rows=0, act=0):
+        """pcnn_conv_transpose_fwd: y = act(conv_transpose2d(x, w, bias, stride, padding, output_padding)) with x dense bf16
+        [N][H][W][C_in], filt the fp32 master [C_in][R][S][C_out] (torch's weight permuted (0, 2, 3, 1)), bias fp32 [C_out] or None,
+        y [N][H_out][W_out][C_out] at row_pitch (0 = W_out C_out) / image_rows (0 = H_out)"""
+        ph, pw = (int(v) for v in padding)
+        oh, ow = (int(v) for v in output_padding)
+        self._call("pcnn_conv_transpose_fwd", _p(x), _p(filt), _p(bias), _p(y), int(N), int(H), int(W), int(C_in), int(C_out), int(R), int(S),
+                   int(stride), ph, pw, oh, ow, int(row_pitch or 0), int(image_rows), int(act))
+
+    def upsample_bilinear_fwd(self, x, y, N, H, W, Cin, H_out, W_out):
+        """pcnn_upsample_bilinear_nhwc_bf16_fwd: interpolate(size=(H_out, W_out), mode="bilinear", align_corners=False) of dense
+        bf16 [N][H][W][C] into dense y [N][H_out][W_out][C]"""
+        self._call("pcnn_upsample_bilinear_nhwc_bf16_fwd", _p(x), _p(y), int(N), int(H), int(W), int(Cin), int(H_out), int(W_out))
+
+    def upsample_bilinear_bwd(self, dy, dx, N, H, W, Cin, H_out, W_out):
+        """pcnn_upsample_bilinear_nhwc_bf16_bwd: the gradient of that resize, gathered in a fixed order (no atomics), every dx element
+        written"""
+        self._call("pcnn_upsample_bilinear_nhwc_bf16_bwd", _p(dy), _p(dx), int(N), int(H), int(W), int(Cin), int(H_out), int(W_out))
+
+    def augment_mask(self, masks, n, H, W, first, N, masks_out, shuffle=1, pad=0, flip=0, seed=0, epoch=0, mask_fill=255):
+        """pcnn_augment_mask_u8: the uint8 masks [n][H][W] of augment's batch with the same arguments, each permuted, cropped and
+        flipped exactly as its image, the padding filled with mask_fill, into masks_out [N][H][W]"""
+        self._call("pcnn_augment_mask_u8", _p(masks), int(n), int(H), int(W), int(first), int(N), int(shuffle), int(pad), int(flip), int(seed),
+                   int(epoch), int(mask_fill), _p(masks_out))
+
     def linear_wgrad(self, plan, x, dy, dw):
         """pcnn_linear_wgrad: dW fp32 [O][P][Q][C] = dy^T x, the shape from the LinearPlan"""
         self._call("pcnn_linear_wgrad", plan.plan, _p(x), _p(dy), _p(dw))
@@ -828,6 +861,112 @@ class ConvLayer(_PlanLayer):
             e.conv_wide_wgrad(self._x, dy, self.dw, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride, self.padding)
             if dx is not None:
                 e.conv_wide_dgrad(dy, self.filt, dx, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride, self.padding)
+
+
+class ConvTransposeLayer(_PlanLayer):
+    """A transposed convolution trained on the device, as torch.nn.ConvTranspose2d(C_in, C_out, (R, S), stride, padding,
+    output_padding) with groups 1 and dilation 1:  H_out = (H - 1) stride - 2 pad_h + R + output_padding_h, W_out the same.
+    weight has torch's layout [C_in][C_out][R][S]; the fp32 master `filt` is held as the adjoint convolution's KRSC [C_in][R][S][C_out]
+    (K = C_in filters over C = C_out channels), torch's weight permuted (0, 2, 3, 1).  x is dense bf16 [N][H][W][C_in]; y and dy are
+    [N][H_out][W_out][C_out] at row_pitch (None = dense) and image_rows (0 = H_out); dx is dense like x.
+      forward:  pcnn_conv_transpose_fwd (the wide input gradient with a bias and activation epilogue), from the master on every call;
+      backward: pcnn_conv_bias_act_bwd over y (with a bias or an activation), dx = the forward of the adjoint convolution's
+                WideConvPlan on dy, dw = its weight gradient with the activations swapped (x = dy, dy = x).
+    The adjoint plan holds the master's bf16 rounding for dx and is what the optimizers refresh, so call backward before sgd or an
+    optimizer step.  With a bias or an activation y must be dense (pcnn_conv_bias_act_bwd reads it so) and C_out <= 256."""
+
+    def __init__(self, engine, N, H, W, C_in, C_out, R, S, weight, bias=None, act=0, stride=1, padding=(0, 0), output_padding=(0, 0),
+                 row_pitch=None, image_rows=0):
+        self.act, self.stride = int(act), int(stride)
+        self.padding = tuple(int(v) for v in padding)
+        self.output_padding = tuple(int(v) for v in output_padding)
+        self.info = conv_transpose_info(N, H, W, C_in, C_out, R, S, self.stride, self.padding, self.output_padding, row_pitch, image_rows,
+                                        bias is not None, self.act)
+        H_out, W_out = self.info["H_out"], self.info["W_out"]
+        self.row_pitch, self.image_rows = self.info["row_pitch"], self.info["image_rows"]
+        if (self.act or bias is not None) and (self.row_pitch != W_out * C_out or self.image_rows != H_out):
+            raise PcnnError("ConvTransposeLayer", -1, f"row_pitch {self.row_pitch}, image_rows {self.image_rows} with a bias or an activation: "
+                            "y must be dense (row_pitch W_out C_out, image_rows H_out), as pcnn_conv_bias_act_bwd reads it")
+        self.shape = (N, H, W, C_in, C_out, R, S)
+        filt = np.ascontiguousarray(np.asarray(weight, np.float32).reshape(C_in, C_out, R, S).transpose(0, 2, 3, 1))
+        bias = None if bias is None else np.ascontiguousarray(bias, np.float32).reshape(C_out)
+        plan = WideConvPlan(engine, N, H_out, W_out, C_out, C_in, R, S, filt, None, act=0, row_pitch=self.row_pitch,
+                            image_rows=self.image_rows, stride=self.stride, padding=self.padding)
+        self._own(engine, plan, filt, bias)
+        self.out_shape = (N, H_out, W_out, C_out)
+        self.pixels = N * H_out * W_out
+
+    def forward(self, x, y):
+        """y = act(conv_transpose2d(x) + bias) from the master's bf16 rounding.  The layer keeps x: backward's weight gradient reads it."""
+        N, H, W, C_in, C_out, R, S = self.shape
+        self.engine.conv_transpose_fwd(x, self.filt, self.bias, y, N, H, W, C_in, C_out, R, S, self.stride, self.padding, self.output_padding,
+                                       self.row_pitch, self.image_rows, self.act)
+        self._x = x
+
+    def _grads(self, dy, dx):
+        N, H, W, C_in, C_out, R, S = self.shape
+        _, H_out, W_out, _ = self.out_shape
+        self.engine.conv_wide_wgrad(dy, self._x, self.dw, N, H_out, W_out, C_out, C_in, R, S, self.row_pitch, self.image_rows, self.stride,
+                                    self.padding)
+        if dx is not None:
+            self.plan.fwd(dy, dx)
+
+    def sgd(self, lr):
+        """w += (-lr) * dw and b += (-lr) * db in fp32 on the masters, then the adjoint plan refreshed from the filters"""
+        self.engine.apply_grad_scaled(self.filt, self.dw, int(np.prod(self.filt.shape)), -lr)
+        if self.bias is not None:
+            self.engine.apply_grad_scaled(self.bias, self.db, self.out_shape[-1], -lr)
+        self.plan.set_params(self.filt)
+
+    def optim_tensors(self):
+        """the filters refresh the adjoint plan (part 1); the bias belongs to no plan, the forward reads the master"""
+        return [(self.filt, self.dw, self.plan, 1, False)] + ([] if self.bias is None else [(self.bias, self.db, None, 0, True)])
+
+    def weight(self):
+        """a host copy of the master in torch's layout [C_in][C_out][R][S]"""
+        return self.filt.to_host().reshape(self.filt.shape).transpose(0, 3, 1, 2).copy()
+
+
+class UpsampleBilinearLayer:
+    """Bilinear resizing between two layers (pcnn_upsample_bilinear_nhwc_bf16_fwd / _bwd), as interpolate(size=(H_out, W_out),
+    mode="bilinear", align_corners=False): up- or downsampling, without antialiasing.  x and dx are dense bf16 [N][H][W][C], y and
+    dy dense [N][H_out][W_out][C].  It keeps no state; info is its partition (upsample_bilinear_info).  The backward gathers each dx
+    element in a fixed order, so reruns give the same bits."""
+
+    def __init__(self, engine, N, H, W, C, H_out, W_out):
+        self.engine = engine
+        self.shape = (int(N), int(H), int(W), int(C), int(H_out), int(W_out))
+        self.info = upsample_bilinear_info(*self.shape)
+        self.out_shape = (int(N), int(H_out), int(W_out), int(C))
+
+    def forward(self, x, y):
+        self.engine.upsample_bilinear_fwd(x, y, *self.shape)
+
+    def backward(self, dy, dx):
+        self.engine.upsample_bilinear_bwd(dy, dx, *self.shape)
+
+    def close(self):
+        pass
+
+
+def segmentation_scores(pred, targets, O, ignore_index=255):
+    """Host evaluation of a per-pixel prediction (not a hot path): (confusion, iou, miou).  confusion[t][p] counts the pixels with
+    target t < O, t != ignore_index, predicted p (0 <= p < O; other predictions, such as the -1 of a NaN row, count in no column but
+    still in their target's row total).  iou[c] = confusion[c][c] / (row total + column total - confusion[c][c]), NaN for a class
+    absent from both; miou is the mean over the classes whose IoU is not NaN."""
+    t = np.asarray(targets).reshape(-1).astype(np.int64)
+    p = np.asarray(pred).reshape(-1).astype(np.int64)
+    keep = (t != ignore_index) & (t >= 0) & (t < O)
+    t, p = t[keep], p[keep]
+    rows = np.bincount(t, minlength=O)
+    ok = (p >= 0) & (p < O)
+    conf = np.bincount(t[ok] * O + p[ok], minlength=O * O).reshape(O, O)
+    tp = np.diag(conf).astype(np.float64)
+    union = rows + conf.sum(0) - tp
+    with np.errstate(invalid="ignore", divide="ignore"):
+        iou = np.where(union > 0, tp / np.maximum(union, 1), np.nan)
+    present = ~np.isnan(iou)
+    return conf, iou, float(iou[present].mean()) if present.any() else float("nan")
 
 
 class DepthwiseConvLayer(_PlanLayer):
@@ -1199,7 +1338,17 @@ class ImageBatcher:
 
     def __init__(self, engine, images, labels, N, pad=0, flip=False, shuffle=True, seed=0, mean=None, std=None, C_out=None,
                  row_pitch=0, image_rows=0, mixup_alpha=0.0, cutmix_alpha=0.0, crop_size=None, scale=(0.08, 1.0), ratio=(3 / 4, 4 / 3),
-                 resize_size=None, trivial_augment=None, random_erase=0.0, erase_scale=(0.02, 0.33), erase_ratio=(0.3, 3.3)):
+                 resize_size=None, trivial_augment=None, random_erase=0.0, erase_scale=(0.02, 0.33), erase_ratio=(0.3, 3.3), masks=None,
+                 mask_fill=255):
+        if masks is not None:
+            if crop_size is not None or trivial_augment is not None or random_erase != 0 or mixup_alpha != 0 or cutmix_alpha != 0:
+                raise PcnnError("ImageBatcher", -1, "masks with crop_size, trivial_augment, random_erase or mixing: masks are carried "
+                                "through the plain crop, pad and flip only")
+            mshape = tuple(int(d) for d in masks.shape)
+            if mshape != tuple(int(d) for d in images.shape[:3]) or "uint8" not in str(masks.dtype):
+                raise PcnnError("ImageBatcher", -1, f"masks must be uint8 [n][H][W] = {tuple(images.shape[:3])}, got {masks.dtype} {mshape}")
+            if not (isinstance(mask_fill, (int, np.integer)) and 0 <= mask_fill <= 255):
+                raise PcnnError("ImageBatcher", -1, f"mask_fill = {mask_fill}: an integer 0 .. 255 is required")
         modes = {None: TRIVIAL_NONE, "nearest": TRIVIAL_NEAREST, "bilinear": TRIVIAL_BILINEAR}
         if not isinstance(trivial_augment, (str, type(None))) or trivial_augment not in modes:
             raise PcnnError("ImageBatcher", -1, f"trivial_augment = {trivial_augment!r}: None, 'nearest' or 'bilinear' is required")
@@ -1260,12 +1409,15 @@ class ImageBatcher:
         self.labels_out = engine.array((self.N,), np.uint8) if labels is not None else None
         self.labels_b = engine.array((self.N,), np.uint8) if self.mixing else None
         self.workspace = engine.array((self.ws_info["ws_bytes"],), np.uint8) if self.augmenting else None
+        self.mask_fill = int(mask_fill)
+        self.masks = None if masks is None else engine.to_device(np.ascontiguousarray(masks, np.uint8)) if isinstance(masks, np.ndarray) else masks
+        self.masks_out = None if masks is None else engine.array((self.N, self.H, self.W), np.uint8)
         self.steps_per_epoch = self.n // self.N
         self.epoch = 0
 
     def batch(self, step, training=True):
         """(x pointer, labels) of batch `step` of epoch self.epoch: positions step N .. step N + N - 1; a mixing batcher's training
-        batches return (x pointer, MixedLabels)"""
+        batches return (x pointer, MixedLabels), a batcher with masks (x pointer, labels, masks_out)"""
         if not 0 <= int(step) < self.steps_per_epoch:
             raise PcnnError("ImageBatcher.batch", -1, f"step = {step}: 0 <= step < steps_per_epoch = {self.steps_per_epoch} is required")
         aug = bool(training)
@@ -1285,7 +1437,11 @@ class ImageBatcher:
             return self.x.ptr, self.labels_out
         if not (aug and self.mixing):
             self.engine.augment(*args, **kw)
-            return self.x.ptr, self.labels_out
+            if self.masks is None:
+                return self.x.ptr, self.labels_out
+            self.engine.augment_mask(self.masks, self.n, self.H, self.W, int(step) * self.N, self.N, self.masks_out, shuffle=kw["shuffle"],
+                                     pad=kw["pad"], flip=kw["flip"], seed=self.seed, epoch=self.epoch, mask_fill=self.mask_fill)
+            return self.x.ptr, self.labels_out, self.masks_out
         kind, lam, box, lam_adjusted = mix_draws(self.seed, self.epoch, step, self.H, self.W, self.mixup_alpha, self.cutmix_alpha)
         weight = lam if kind == "mixup" else lam_adjusted
         self.engine.augment_mix(*args, labels_b_out=self.labels_b, mode=MIX_MIXUP if kind == "mixup" else MIX_CUTMIX, lam=weight,
@@ -1293,7 +1449,7 @@ class ImageBatcher:
         return self.x.ptr, MixedLabels(self.labels_out, self.labels_b, weight, kind, box)
 
     def close(self):
-        for a in (self.x, self.labels_out, self.labels_b, self.workspace):
+        for a in (self.x, self.labels_out, self.labels_b, self.workspace, self.masks_out):
             if a is not None:
                 a.free()
 

@@ -97,6 +97,117 @@ def card():
     return name, power
 
 
+def _bf(shape, scale=1.0):
+    return (torch.randn(shape, device="cuda") * scale).to(torch.bfloat16)
+
+
+def _line(case, ms, ms_torch, nbytes=None, **extra):
+    gpu, power = card()
+    d = {"case": case, "us": ms * 1e3, "torch_us": ms_torch * 1e3, "torch_over_ours": ms_torch / ms, "gpu": gpu, "power_limit": power}
+    if nbytes:
+        d.update(MB=nbytes / 1e6, hbm_frac=nbytes / (ms * 1e-3) / 1e9 / HBM)
+    d.update(extra)
+    print(json.dumps(d), flush=True)
+
+
+def run_convt(name, N, H, W, Ci, Co, R, stride, pad, iters, rounds=3):
+    """ConvTransposeLayer forward and backward (dx and dw) against torch eager conv_transpose2d and its autograd, on the same bf16
+    channels-last tensors; FLOPs 2 N H W Ci Co R R per pass"""
+    w = (np.random.default_rng(0).standard_normal((Ci, Co, R, R)) / np.sqrt(Ci * R * R)).astype(np.float32)
+    layer = pkg.ConvTransposeLayer(eng, N, H, W, Ci, Co, R, R, w, stride=stride, padding=(pad, pad))
+    _, Ho, Wo, _ = layer.out_shape
+    x, dy = _bf((N, H, W, Ci)), _bf((N, Ho, Wo, Co))
+    y, dx = torch.empty((N, Ho, Wo, Co), dtype=torch.bfloat16, device="cuda"), torch.empty_like(x)
+    xt = x.permute(0, 3, 1, 2).requires_grad_(True)
+    wt = torch.from_numpy(w).to("cuda", torch.bfloat16).requires_grad_(True)
+    dyt = dy.permute(0, 3, 1, 2)
+    F = torch.nn.functional
+    ours = {"fwd": lambda: layer.forward(x, y), "bwd": lambda: layer.backward(y, dy, dx)}
+    theirs = {"fwd": lambda: F.conv_transpose2d(xt, wt, stride=stride, padding=pad),
+              "bwd": lambda: torch.autograd.grad(F.conv_transpose2d(xt, wt, stride=stride, padding=pad), (xt, wt), dyt)}
+    flops = 2.0 * N * H * W * Ci * Co * R * R
+    best = {}
+    for _ in range(rounds):
+        for k in ours:
+            a, b = timed(ours[k], iters), timed(theirs[k], iters)
+            o = best.get(k, (a, b))
+            best[k] = (min(a, o[0]), min(b, o[1]))
+    for k, (a, b) in best.items():
+        f = flops * (1 if k == "fwd" else 2)
+        _line(f"convt {name} {k}" + (" (torch: fwd + bwd)" if k == "bwd" else ""), a, b, N=N, TFLOPs=f / (a * 1e-3) / 1e12,
+              bf16_peak_frac=f / (a * 1e-3) / 1e12 / 989.0)
+    layer.close()
+
+
+def run_upsample(name, N, H, W, C, f, iters, rounds=3):
+    """bilinear x f forward and backward against torch interpolate and its autograd (channels-last bf16); bytes: x + y each way"""
+    Ho, Wo = H * f, W * f
+    layer = pkg.UpsampleBilinearLayer(eng, N, H, W, C, Ho, Wo)
+    x, dy = _bf((N, H, W, C)), _bf((N, Ho, Wo, C))
+    y, dx = torch.empty_like(dy), torch.empty_like(x)
+    xt = x.permute(0, 3, 1, 2).requires_grad_(True)
+    dyt = dy.permute(0, 3, 1, 2)
+    F = torch.nn.functional
+    up = lambda: F.interpolate(xt, size=(Ho, Wo), mode="bilinear", align_corners=False)
+    yt = up()
+    ours = {"fwd": lambda: layer.forward(x, y), "bwd": lambda: layer.backward(dy, dx)}
+    theirs = {"fwd": up, "bwd": lambda: torch.autograd.grad(yt, xt, dyt, retain_graph=True)}
+    nbytes = 2 * N * C * (H * W + Ho * Wo)
+    best = {}
+    for _ in range(rounds):
+        for k in ours:
+            a, b = timed(ours[k], iters), timed(theirs[k], iters)
+            o = best.get(k, (a, b))
+            best[k] = (min(a, o[0]), min(b, o[1]))
+    for k, (a, b) in best.items():
+        _line(f"upsample {name} x{f} {k}", a, b, nbytes, N=N)
+
+
+def run_segce(N, O, iters, rounds=3):
+    """per-pixel CE with ignore index 255 (about 10 % ignored) against torch cross_entropy(ignore_index=255) forward + backward"""
+    P = N * 224 * 224
+    z = _bf((P, O), 3.0)
+    t = torch.randint(0, O, (P,), dtype=torch.uint8, device="cuda")
+    t[torch.rand(P, device="cuda") < 0.1] = 255
+    d = torch.empty_like(z)
+    loss = torch.empty(P, dtype=torch.float32, device="cuda")
+    pred = torch.empty(P, dtype=torch.int32, device="cuda")
+    cnt = torch.empty(1, dtype=torch.int32, device="cuda")
+    zt = z.clone().requires_grad_(True)
+    tl = t.long()
+    F = torch.nn.functional
+    ours = lambda: eng.softmax_ce_pixels_bf16(z, t, P, O, 255, d, cnt, loss, pred)
+    theirs = lambda: torch.autograd.grad(F.cross_entropy(zt, tl, ignore_index=255), zt)
+    best = None
+    for _ in range(rounds):
+        a, b = timed(ours, iters), timed(theirs, iters)
+        best = (a, b) if best is None else (min(a, best[0]), min(b, best[1]))
+    _line(f"segce {P} pixels x {O} classes", best[0], best[1], P * (4 * O + 1 + 8), pixels=P)
+
+
+def run_fcn(iters):
+    """one FCNLite training step (forward, backward, SGD with momentum) at N = 32 on 28 x 28 digits"""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import segment_nets
+    import segment_ref
+    d = np.load(os.path.join(ROOT, "tests", "golden", "mnist_subset.npz"))
+    cls = segment_nets.FCNLite
+    net = cls(eng, pkg, cls.init_params())
+    opt = pkg.SGD(eng, net.layers(), momentum=0.9)
+    b = pkg.ImageBatcher(eng, d["train_u8"].reshape(-1, 28, 28), d["train_labels"], cls.NB, pad=2, flip=True, C_out=8,
+                         masks=segment_ref.digit_masks(d["train_u8"], d["train_labels"]))
+    def step():
+        net.forward(*b.batch(0))
+        net.backward()
+        opt.step(cls.LR)
+    ms = timed(step, iters)
+    gpu, power = card()
+    print(json.dumps({"case": f"FCNLite training step N={cls.NB}", "us": ms * 1e3, "gpu": gpu, "power_limit": power}), flush=True)
+    b.close()
+    opt.close()
+    net.close()
+
+
 def run_wide(name, N, H, W, C, K, R, S, stride, iters):
     """the wide-channel forward (WideConvPlan) next to torch.nn.functional.conv2d (cuDNN) on the same bf16 channels-last tensors.
     Bound: the larger of flops / 989 TFLOP/s (H100 SXM dense bf16) and bytes / 3.35 TB/s, bytes = N * (H*W*C + P*Q*K) * 2."""
@@ -1878,6 +1989,18 @@ if only == "fwdab":                                                    # forward
 if only in ("all", "cfg5"):
     for N in (1, 8, 32, 128):
         run("224x224x3->64x3x3 bf16 (config 5)", N, 224, 224, 3, 64, 3, 3, 0, 10)
+if only == "convt":                                                   # transposed convolutions of an FCN / DCGAN decoder, N = 128
+    run_convt("7x7x256->128 4x4/2 pad 1", 128, 7, 7, 256, 128, 4, 2, 1, 20)
+    run_convt("14x14x128->64 4x4/2 pad 1", 128, 14, 14, 128, 64, 4, 2, 1, 20)
+    run_convt("28x28x64->32 4x4/2 pad 1", 128, 28, 28, 64, 32, 4, 2, 1, 20)
+if only == "upsample":                                                 # bilinear x2 / x4 / x8
+    run_upsample("28x28x64", 128, 28, 28, 64, 2, 20)
+    run_upsample("28x28x21", 64, 28, 28, 21, 4, 20)
+    run_upsample("28x28x21", 32, 28, 28, 21, 8, 20)
+if only == "segce":                                                    # VOC-sized per-pixel loss
+    run_segce(16, 21, 20)
+if only == "fcn":
+    run_fcn(20)
 eng.close()
 if only == "wprobe":                                                   # what a pure WRITE stream / pure READ stream / copy reach on this GPU
     # library fill / reduce / copy kernels as a yardstick for the store-dominated forward pass (807 MB written, 39 MB read):
