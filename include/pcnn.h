@@ -370,6 +370,41 @@ int pcnn_conv_wide_dgrad_padded(pcnn_ctx *ctx, const void *dy_bf16_dev, const fl
                                 int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch, int image_rows);
 int pcnn_conv_wide_bwd_info_padded(int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch,
                                    int image_rows, int *out10);
+/* The same five with a dilation (dil_h, dil_w) after the padding, as torch.nn.functional.conv2d(padding=(pad_h, pad_w),
+ * dilation=(dil_h, dil_w)) ("atrous" convolution): tap (r, s) sits r*dil_h rows and s*dil_w columns from the window's corner.
+ * With the window's extent E_h = dil_h (R - 1) + 1, E_w = dil_w (S - 1) + 1 and x~ as above,
+ *     P = (H + 2 pad_h - E_h) / stride + 1,   Q = (W + 2 pad_w - E_w) / stride + 1
+ *     y[n][p][q][k]  = b[k] + sum_{r,s,c} x~[n][p*stride - pad_h + r*dil_h][q*stride - pad_w + s*dil_w][c] * f[k][r][s][c]   (then act)
+ *     dw[k][r][s][c] = sum_{n,p,q} dy[n][p][q][k] * x~[n][p*stride - pad_h + r*dil_h][q*stride - pad_w + s*dil_w][c]
+ *     dx[n][h][w][c] = sum_{k,r,s} dy[n][(h + pad_h - r*dil_h)/stride][(w + pad_w - s*dil_w)/stride][k] * f[k][r][s][c]
+ *                      over the (r, s) that divide exactly and give a dy pixel inside P x Q.
+ * The forward and the weight gradient run the padded calls' kernels (only the per-tap phase and offset of x change).  The input
+ * gradient runs the padded call's kernel with two more steps in its tap walk: with g = gcd(dil_h, stride), row phase a of dx has
+ * no taps unless g divides a + pad_h (its elements are written as 0), and otherwise takes the taps r = rho + (stride/g) i, each
+ * reading dy row u - (dil_h/g) i + (a + pad_h - rho dil_h)/stride (columns the same).  Each dx element sums in the order of the
+ * padded call: ascending i, then j, then 64-filter chunk.  out8 / out10 and every other part of the contract are the padded calls'.
+ * The domain is the padded one with, in place of its padding and size rules,
+ *   - 1 <= dil_h, dil_w <= 256;
+ *   - 0 <= pad_h <= dil_h (R - 1) and 0 <= pad_w <= dil_w (S - 1);
+ *   - H + 2 pad_h >= E_h and W + 2 pad_w >= E_w;
+ *   - H >= stride if pad_h > 0 and W >= stride if pad_w > 0: a padded direction may read every phase of x, and each phase map
+ *     must have a row / pixel inside the image (unpadded, the phases read are (r dil_h) mod stride < E_h <= H).
+ * A shape with a dilation other than (1, 1) is never refused for the row-Toeplitz plan (it has no dilation), so no shape has two
+ * forward kernels.  At dilation (1, 1) each is exactly its padded call, refusals and their text included, except that refusals
+ * name the called function (pcnn_conv_wide_plan_create_dilated for both forward calls). */
+int pcnn_conv_wide_plan_create_dilated(pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w,
+                                       int dil_h, int dil_w, int row_pitch, int image_rows, int act, const float *filt_host,
+                                       const float *bias_host, pcnn_conv_plan **plan_out);
+int pcnn_conv_wide_plan_info_dilated(int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w, int dil_h,
+                                     int dil_w, int row_pitch, int image_rows, int *out8);
+int pcnn_conv_wide_wgrad_dilated(pcnn_ctx *ctx, const void *x_bf16_dev, const void *dy_bf16_dev, float *dw_f32_dev, int N, int H, int W,
+                                 int C, int K, int R, int S, int stride, int pad_h, int pad_w, int dil_h, int dil_w, int row_pitch,
+                                 int image_rows);
+int pcnn_conv_wide_dgrad_dilated(pcnn_ctx *ctx, const void *dy_bf16_dev, const float *filt_f32_dev, void *dx_bf16_dev, int N, int H,
+                                 int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w, int dil_h, int dil_w, int row_pitch,
+                                 int image_rows);
+int pcnn_conv_wide_bwd_info_dilated(int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w, int dil_h,
+                                    int dil_w, int row_pitch, int image_rows, int *out10);
 /* Backward passes of the same convolution (bf16 operands, fp32 accumulation, deterministic; wgmma kernels, see
  * pcnn_conv_bwd_select): weight gradient fp32 KRSC [ref: layer.h:371-395 bp_weight_c1, without its /576] and input gradient
  * bf16 NHWC in x's layout.  row_pitch / image_rows as for the forward plan (0 = dense). */
@@ -662,6 +697,21 @@ int pcnn_dwconv_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C, int R, in
 int pcnn_dwconv_wgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *x_bf16_dev, const void *dy_bf16_dev, float *dw_f32_dev);
 int pcnn_dwconv_dgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void *dy_bf16_dev, void *dx_bf16_dev);
 int pcnn_dwconv_info(int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int *out9);
+/* The same depthwise convolution with a dilation (dil_h, dil_w), as conv2d(..., dilation=(dil_h, dil_w), groups=C): tap (r, s)
+ * of the window of output (p, q) reads x~[n][h0 + r dil_h][w0 + s dil_w][c].  With E_h = dil_h (R - 1) + 1, E_w = dil_w (S - 1) + 1,
+ *     P = (H + 2 pad_h - E_h) / stride + 1,   Q = (W + 2 pad_w - E_w) / stride + 1,
+ * and every rule above holds with r dil_h for r and s dil_w for s: the forward sums over ascending r, then s; the input gradient
+ * takes the taps with h = p stride - pad_h + r dil_h and w = q stride - pad_w + s dil_w in ascending r, then s (+0 with no term);
+ * the weight gradient's lanes, ranges and slot reduction are unchanged.  The plan is an ordinary depthwise plan: pcnn_conv_tc_fwd,
+ * pcnn_dwconv_wgrad, pcnn_dwconv_dgrad, pcnn_conv_plan_set_params and pcnn_optim_step take it as they take one of
+ * pcnn_dwconv_plan_create.  The domain is the one above with, in place of its padding and fit rules,
+ *   - 1 <= dil_h, dil_w <= 256;
+ *   - 0 <= pad_h <= dil_h (R - 1), 0 <= pad_w <= dil_w (S - 1), H + 2 pad_h >= E_h and W + 2 pad_w >= E_w.
+ * At dilation (1, 1) each is exactly pcnn_dwconv_plan_create / pcnn_dwconv_info, refusals and their text included, except that
+ * refusals name the called function.  out9 as pcnn_dwconv_info's. */
+int pcnn_dwconv_plan_create_dilated(pcnn_ctx *ctx, int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int dil_h,
+                                    int dil_w, int act, const float *filt_host, const float *bias_host, pcnn_conv_plan **out);
+int pcnn_dwconv_info_dilated(int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int dil_h, int dil_w, int *out9);
 /* Grouped convolution (csrc/gconv_nhwc.cu), as torch.nn.functional.conv2d(x, w, b, stride, padding=(pad_h, pad_w), groups=G) with
  * w [K][Cg][R][S], 1 < G: each group g of Cg = C / G input channels feeds its own Kg = K / G filters; output k belongs to group
  * g = k / Kg (ResNeXt, RegNet, ShuffleNet, and a depthwise layer with a channel multiplier: Cg = 1, Kg > 1).

@@ -140,6 +140,11 @@ _SIG = {
     "pcnn_conv_wide_wgrad_padded": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
     "pcnn_conv_wide_dgrad_padded": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
     "pcnn_conv_wide_bwd_info_padded": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
+    "pcnn_conv_wide_plan_create_dilated": [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _pvp],
+    "pcnn_conv_wide_plan_info_dilated": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
+    "pcnn_conv_wide_wgrad_dilated": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
+    "pcnn_conv_wide_dgrad_dilated": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i],
+    "pcnn_conv_wide_bwd_info_dilated": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_f32_to_bf16_rows": [_vp, _vp, _vp, _l, _i, _i],
     "pcnn_conv_plan_set_params": [_vp, _vp, _vp, _vp],
     "pcnn_conv_bias_act_bwd": [_vp, _vp, _vp, _vp, _vp, _l, _i, _i],
@@ -172,6 +177,8 @@ _SIG = {
     "pcnn_dwconv_wgrad": [_vp, _vp, _vp, _vp, _vp],
     "pcnn_dwconv_dgrad": [_vp, _vp, _vp, _vp],
     "pcnn_dwconv_info": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
+    "pcnn_dwconv_plan_create_dilated": [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _pvp],
+    "pcnn_dwconv_info_dilated": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_gconv_plan_create": [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _pvp],
     "pcnn_gconv_wgrad": [_vp, _vp, _vp, _vp, _vp],
     "pcnn_gconv_dgrad": [_vp, _vp, _vp, _vp],
@@ -260,31 +267,41 @@ def conv_tc_plan_info(N, H, W, C, K, R, S, stride=1, row_pitch=None, image_rows=
     return dict(Qt=out[0], V=out[1], stages=out[2], n_mtiles=out[3], n_qtiles=out[4], tiles=out[3] * out[4])
 
 
-def conv_wide_plan_info(N, H, W, C, K, R, S, stride=1, row_pitch=None, image_rows=0, padding=(0, 0)):
+def conv_wide_plan_info(N, H, W, C, K, R, S, stride=1, row_pitch=None, image_rows=0, padding=(0, 0), dilation=(1, 1)):
     """How the wide-channel forward plan tiles a shape (pcnn_conv_wide_plan_info, or pcnn_conv_wide_plan_info_padded for a
-    padding (pad_h, pad_w) other than (0, 0); host only, no GPU).  row_pitch None = W*C rounded up to 8 elements, as
-    WideConvPlan.  issued_pixels / useful_pixels: output pixels the tiles cover / compute."""
+    padding (pad_h, pad_w) other than (0, 0), or pcnn_conv_wide_plan_info_dilated for a dilation (dil_h, dil_w) other than
+    (1, 1); host only, no GPU).  row_pitch None = W*C rounded up to 8 elements, as WideConvPlan.  issued_pixels / useful_pixels:
+    output pixels the tiles cover / compute."""
     pitch = (W * C + 7) // 8 * 8 if row_pitch is None else row_pitch
     ph, pw = (int(v) for v in padding)
+    dh, dw = (int(v) for v in dilation)
     out = (_i * 8)()
-    if (ph, pw) == (0, 0):
+    if (dh, dw) != (1, 1):
+        check("pcnn_conv_wide_plan_info_dilated",
+              lib().pcnn_conv_wide_plan_info_dilated(N, H, W, C, K, R, S, int(stride), ph, pw, dh, dw, int(pitch), int(image_rows), out))
+    elif (ph, pw) == (0, 0):
         check("pcnn_conv_wide_plan_info", lib().pcnn_conv_wide_plan_info(N, H, W, C, K, R, S, int(stride), int(pitch), int(image_rows), out))
     else:
         check("pcnn_conv_wide_plan_info_padded",
               lib().pcnn_conv_wide_plan_info_padded(N, H, W, C, K, R, S, int(stride), ph, pw, int(pitch), int(image_rows), out))
-    P, Q = (H + 2 * ph - R) // stride + 1, (W + 2 * pw - S) // stride + 1
+    P, Q = (H + 2 * ph - dh * (R - 1) - 1) // stride + 1, (W + 2 * pw - dw * (S - 1) - 1) // stride + 1
     return dict(Pt=out[0], Qt=out[1], chunks=out[2], stages=out[3], tiles=out[4], n_pb=out[5], n_qb=out[6], npad=out[7],
                 issued_pixels=out[4] * out[0] * out[1], useful_pixels=N * P * Q)
 
 
-def conv_wide_bwd_info(N, H, W, C, K, R, S, stride=1, row_pitch=None, image_rows=0, padding=(0, 0)):
+def conv_wide_bwd_info(N, H, W, C, K, R, S, stride=1, row_pitch=None, image_rows=0, padding=(0, 0), dilation=(1, 1)):
     """How the wide-channel gradients tile a shape (pcnn_conv_wide_bwd_info, or pcnn_conv_wide_bwd_info_padded for a padding
-    (pad_h, pad_w) other than (0, 0); host only, no GPU).  row_pitch None = W*C rounded up to 8 elements, as WideConvPlan.
-    wgrad_units = row-block pairs x pixel ranges; wgrad_blocks_per_split is the fewest."""
+    (pad_h, pad_w) other than (0, 0), or pcnn_conv_wide_bwd_info_dilated for a dilation other than (1, 1); host only, no GPU).
+    row_pitch None = W*C rounded up to 8 elements, as WideConvPlan.  wgrad_units = row-block pairs x pixel ranges;
+    wgrad_blocks_per_split is the fewest."""
     pitch = (W * C + 7) // 8 * 8 if row_pitch is None else row_pitch
     ph, pw = (int(v) for v in padding)
+    dh, dw = (int(v) for v in dilation)
     out = (_i * 10)()
-    if (ph, pw) == (0, 0):
+    if (dh, dw) != (1, 1):
+        check("pcnn_conv_wide_bwd_info_dilated",
+              lib().pcnn_conv_wide_bwd_info_dilated(N, H, W, C, K, R, S, int(stride), ph, pw, dh, dw, int(pitch), int(image_rows), out))
+    elif (ph, pw) == (0, 0):
         check("pcnn_conv_wide_bwd_info", lib().pcnn_conv_wide_bwd_info(N, H, W, C, K, R, S, int(stride), int(pitch), int(image_rows), out))
     else:
         check("pcnn_conv_wide_bwd_info_padded",
@@ -314,14 +331,23 @@ def upsample_bilinear_info(N, H, W, Cin, H_out, W_out):
     return dict(vec=out[0], grid_fwd=out[1], grid_bwd=out[2], threads=out[3])
 
 
-def conv_layer_family(N, H, W, C, K, R, S, stride=1, padding=(0, 0), row_pitch=None, image_rows=0):
+def conv_layer_family(N, H, W, C, K, R, S, stride=1, padding=(0, 0), row_pitch=None, image_rows=0, dilation=(1, 1)):
     """Which forward plan serves a convolution layer (host only, no GPU): "narrow" (the row-Toeplitz plan,
     pcnn_conv_tc_plan_create_strided) when pcnn_conv_tc_plan_info accepts the shape and there is no padding, otherwise "wide"
     (pcnn_conv_wide_plan_create[_padded]).  The two domains do not overlap, so there is nothing to choose.  A padded shape the
     wide plan refuses but the row-Toeplitz plan takes unpadded (a narrow shape: few channels) has no padded kernel: it is
     refused with a PcnnError naming pcnn_pad_nhwc_bf16.  Any other shape neither plan takes gets the refusal of the plan its
-    padding points to."""
+    padding points to.  A dilation other than (1, 1) is "wide" (pcnn_conv_wide_plan_create_dilated) or that plan's refusal; with
+    C % 8 != 0 it is refused with a PcnnError: no narrow-channel kernel dilates."""
     ph, pw = (int(v) for v in padding)
+    dh, dw = (int(v) for v in dilation)
+    if (dh, dw) != (1, 1):
+        if C % 8 != 0:
+            raise PcnnError("conv_layer_family", -1,
+                            f"dilation ({dh}, {dw}) with C = {C} channels: no narrow-channel kernel dilates; only the wide plan "
+                            "(C % 8 == 0) takes a dilation")
+        conv_wide_plan_info(N, H, W, C, K, R, S, stride, row_pitch, image_rows, padding=(ph, pw), dilation=(dh, dw))
+        return "wide"
     if (ph, pw) == (0, 0):
         try:
             conv_tc_plan_info(N, H, W, C, K, R, S, stride, row_pitch, image_rows)
@@ -389,13 +415,19 @@ def linear_info(N, P, Q, C, O, row_pitch=0, image_rows=0):
                 wgrad_splits=out[6], wgrad_stages=out[7], dgrad_tiles=out[8], dgrad_chunks=out[9], dgrad_stages=out[10], npad=out[11])
 
 
-def dwconv_info(N, H, W, C, R, S, stride=1, padding=(0, 0)):
-    """The output size and the weight-gradient split of the depthwise convolution (pcnn_dwconv_info; host only, no GPU), refused
-    as pcnn_dwconv_plan_create refuses.  vec: channels per thread (8 or 1); the N*P*Q output pixels are cut into `ranges` of
-    `pixels_per_range`, a function of the shape alone; n_acc: fp32 additions on the longest path of one dw sum."""
+def dwconv_info(N, H, W, C, R, S, stride=1, padding=(0, 0), dilation=(1, 1)):
+    """The output size and the weight-gradient split of the depthwise convolution (pcnn_dwconv_info, or pcnn_dwconv_info_dilated
+    for a dilation other than (1, 1); host only, no GPU), refused as the create call refuses.  vec: channels per thread (8 or 1);
+    the N*P*Q output pixels are cut into `ranges` of `pixels_per_range`, a function of the shape alone; n_acc: fp32 additions on
+    the longest path of one dw sum."""
     ph, pw = (int(v) for v in padding)
+    dh, dw = (int(v) for v in dilation)
     out = (_i * 9)()
-    check("pcnn_dwconv_info", lib().pcnn_dwconv_info(int(N), int(H), int(W), int(C), int(R), int(S), int(stride), ph, pw, out))
+    if (dh, dw) != (1, 1):
+        check("pcnn_dwconv_info_dilated", lib().pcnn_dwconv_info_dilated(int(N), int(H), int(W), int(C), int(R), int(S), int(stride), ph, pw,
+                                                                       dh, dw, out))
+    else:
+        check("pcnn_dwconv_info", lib().pcnn_dwconv_info(int(N), int(H), int(W), int(C), int(R), int(S), int(stride), ph, pw, out))
     return dict(P=out[0], Q=out[1], vec=out[2], groups_per_cta=out[3], slices=out[4], lanes=out[5], pixels_per_range=out[6],
                 ranges=out[7], n_acc=out[8])
 

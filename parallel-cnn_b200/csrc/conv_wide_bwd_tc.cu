@@ -32,11 +32,18 @@
 // a + pad_h = st * off_h + rho_h, phase a takes the taps r = rho_h + st*i (none when rho_h >= R) and reads dy at row u - i + off_h,
 // columns the same with pad_w.  At pad 0, rho_h = a and off_h = 0.
 //
+// Dilation (the _dilated entry points).  Weight gradient: the forward's tap table, device code unchanged.  Input gradient: tap r
+// reaches dx row st*u + a when r*dil_h = a + pad_h (mod st).  With g = gcd(dil_h, st), phase a has no taps unless g divides
+// a + pad_h; then its taps are r = rho_h + (st/g)*i (rho_h the least such r, none when rho_h >= R) and tap i reads dy row
+// u - (dil_h/g)*i + off_h with off_h = (a + pad_h - rho_h*dil_h)/st, exact.  Columns the same with dil_w and pad_w.  The tap step
+// st/g and the dy step dil_h/g are parameters of the producer's addresses only; at dilation 1 they are st and 1.
+//
 // Warp roles (288 threads, 1 CTA/SM, persistent): warps 0-7 = two consumer warpgroups, warp 8 = TMA producer.
 #include "tc_common.cuh"
 
 #include <cuda_bf16.h>
 
+#include <numeric>
 #include <type_traits>
 
 using namespace pcnn_tc;
@@ -177,8 +184,10 @@ struct WideDgradParams {
     int tile0[17];                   // first tile of phase a * st + b; tile0[st * st] = all tiles
     int n_ub[16], n_vb[16];          // pixel blocks down / along the phase's grid
     int Ri[16], Sj[16];              // taps of the phase in each direction
-    int rho_h[4], off_h[4];          // row phase a: taps r = rho_h[a] + st*i, dy row u - i + off_h[a] (a + pad_h = st*off_h + rho_h)
-    int rho_w[4], off_w[4];          // column phase b: the same with pad_w
+    int rho_h[4], off_h[4];          // row phase a: taps r = rho_h[a] + tstep_h*i, dy row u - dystep_h*i + off_h[a]
+    int rho_w[4], off_w[4];          // column phase b: the same with pad_w and dil_w
+    int tstep_h, dystep_h;           // st/g and dil_h/g, g = gcd(dil_h, st): st and 1 at dilation 1
+    int tstep_w, dystep_w;
 };
 
 // what the transposed convolution's epilogue (EPI) adds: bias [C] or NULL, the activation and the channel count C
@@ -186,6 +195,8 @@ struct WideDgradEpiParams : WideDgradParams {
     const float *bias;
     int act, C;
 };
+
+static_assert(sizeof(WideDgradEpiParams) + 18 * sizeof(CUtensorMap) <= 4096, "the input gradient's parameters exceed 4 KB");
 
 template <bool EPI>
 using DgradParamsOf = typename std::conditional<EPI, WideDgradEpiParams, WideDgradParams>::type;
@@ -244,8 +255,8 @@ k_conv_wide_dgrad(const __grid_constant__ WideDgradMaps m, const DgradParamsOf<E
                 const int a = d.ph / st, b = d.ph % st;
                 for (int i = 0; i < p.Ri[d.ph]; ++i)
                     for (int j = 0; j < p.Sj[d.ph]; ++j) {
-                        const int t = (p.rho_h[a] + st * i) * p.S + p.rho_w[b] + st * j;
-                        const int bv = d.v0 - j + p.off_w[b], bu = d.u0 - i + p.off_h[a];
+                        const int t = (p.rho_h[a] + p.tstep_h * i) * p.S + p.rho_w[b] + p.tstep_w * j;
+                        const int bv = d.v0 - p.dystep_w * j + p.off_w[b], bu = d.u0 - p.dystep_h * i + p.off_h[a];
                         for (int kc = 0; kc < p.nkc; ++kc, ++it) {
                             const int stage = it % NST;
                             bar_wait_relaxed(&S.empty[stage], ((unsigned)(it / NST) & 1u) ^ 1u, 32);
@@ -356,10 +367,23 @@ struct WideBwdPlan {
     int dn, d_tiles;                  // input-gradient accumulator columns, tiles
 };
 
-int wide_bwd_plan(const char *fn, int N, int H, int W, int C, int K, int R, int S, int st, int pad_h, int pad_w, int row_pitch,
-                  int image_rows, WideBwdPlan *pl) {
+// the taps of dx's row phase a (see the head of this file): their count, the first tap *rho and the dy offset *off
+int dgrad_phase_taps(int a, int pad, int dil, int st, int R, int *rho, int *off) {
+    const int g = std::gcd(dil, st), v = a + pad, tstep = st / g;
+    *rho = 0;
+    *off = 0;
+    if (v % g != 0) return 0;
+    int r = 0;
+    while ((r * dil - v) % st != 0) ++r;               // r < st/g
+    *rho = r;
+    *off = (v - r * dil) / st;
+    return r < R ? (R - r + tstep - 1) / tstep : 0;
+}
+
+int wide_bwd_plan(const char *fn, int N, int H, int W, int C, int K, int R, int S, int st, int pad_h, int pad_w, int dil_h, int dil_w,
+                  int row_pitch, int image_rows, WideBwdPlan *pl) {
     memset(pl, 0, sizeof(*pl));
-    int rc = conv_wide_shape(fn, N, H, W, C, K, R, S, st, pad_h, pad_w, row_pitch, image_rows, &pl->sh);
+    int rc = conv_wide_shape(fn, N, H, W, C, K, R, S, st, pad_h, pad_w, dil_h, dil_w, row_pitch, image_rows, &pl->sh);
     if (rc) return rc;
     const ConvWideShape &sh = pl->sh;
     WideWgradParams &w = pl->w;
@@ -384,9 +408,12 @@ int wide_bwd_plan(const char *fn, int N, int H, int W, int C, int K, int R, int 
     d.G = d.ngroups == 1 ? C : ((C + d.ngroups - 1) / d.ngroups + 63) / 64 * 64;
     pl->dn = (d.G + 15) / 16 * 16;
     conv_wide_pixel_block((H + st - 1) / st, (W + st - 1) / st, &d.Pt, &d.Qt);    // phase (0, 0) has the largest grid
+    d.tstep_h = st / std::gcd(dil_h, st); d.dystep_h = dil_h / std::gcd(dil_h, st);
+    d.tstep_w = st / std::gcd(dil_w, st); d.dystep_w = dil_w / std::gcd(dil_w, st);
+    int taps_h[4], taps_w[4];
     for (int a = 0; a < st; ++a) {
-        d.rho_h[a] = (a + pad_h) % st; d.off_h[a] = (a + pad_h) / st;
-        d.rho_w[a] = (a + pad_w) % st; d.off_w[a] = (a + pad_w) / st;
+        taps_h[a] = dgrad_phase_taps(a, pad_h, dil_h, st, R, &d.rho_h[a], &d.off_h[a]);
+        taps_w[a] = dgrad_phase_taps(a, pad_w, dil_w, st, S, &d.rho_w[a], &d.off_w[a]);
     }
     long long tiles = 0;
     for (int a = 0; a < st; ++a)
@@ -395,8 +422,8 @@ int wide_bwd_plan(const char *fn, int N, int H, int W, int C, int K, int R, int 
             d.tile0[ph] = (int)tiles;
             d.n_ub[ph] = U > 0 ? (U + d.Pt - 1) / d.Pt : 0;
             d.n_vb[ph] = V > 0 ? (V + d.Qt - 1) / d.Qt : 0;
-            d.Ri[ph] = R > d.rho_h[a] ? (R - d.rho_h[a] + st - 1) / st : 0;
-            d.Sj[ph] = S > d.rho_w[b] ? (S - d.rho_w[b] + st - 1) / st : 0;
+            d.Ri[ph] = taps_h[a];
+            d.Sj[ph] = taps_w[b];
             tiles += (long long)N * d.n_ub[ph] * d.n_vb[ph] * d.ngroups;
             PCNN_REQUIRE(tiles < (1LL << 31), PCNN_ERR_ARG, "%s: %lld input-gradient tiles exceed the int range", fn, tiles);
         }
@@ -447,12 +474,12 @@ int configure(pcnn_ctx *ctx) {
 }  // namespace
 
 // The three passes below are each entry point's body, with its name for the messages; the unpadded entry points run them at
-// padding (0, 0).
-static int wide_bwd_info(const char *fn, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w,
-                         int row_pitch, int image_rows, int *out10) {
+// padding (0, 0), the unpadded and padded ones at dilation (1, 1).
+static int wide_bwd_info(const char *fn, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w, int dil_h,
+                         int dil_w, int row_pitch, int image_rows, int *out10) {
     PCNN_REQUIRE(out10, PCNN_ERR_ARG, "%s: NULL argument", fn);
     WideBwdPlan pl;
-    int rc = wide_bwd_plan(fn, N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows, &pl);
+    int rc = wide_bwd_plan(fn, N, H, W, C, K, R, S, stride, pad_h, pad_w, dil_h, dil_w, row_pitch, image_rows, &pl);
     if (rc) return rc;
     out10[0] = pl.w.rows; out10[1] = pl.w.splits; out10[2] = pl.w.blocks / pl.w.splits; out10[3] = pl.w.stages; out10[4] = pl.w.units;
     out10[5] = pl.d.Pt; out10[6] = pl.d.Qt; out10[7] = pl.d.ngroups; out10[8] = pl.d.stages; out10[9] = pl.d_tiles;
@@ -460,10 +487,10 @@ static int wide_bwd_info(const char *fn, int N, int H, int W, int C, int K, int 
 }
 
 static int wide_wgrad(const char *fn, pcnn_ctx *ctx, const void *x_bf16, const void *dy_bf16, float *dw_f32, int N, int H, int W, int C,
-                      int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch, int image_rows) {
+                      int K, int R, int S, int stride, int pad_h, int pad_w, int dil_h, int dil_w, int row_pitch, int image_rows) {
     PCNN_REQUIRE(ctx && x_bf16 && dy_bf16 && dw_f32, PCNN_ERR_ARG, "%s: NULL argument", fn);
     WideBwdPlan pl;
-    int rc = wide_bwd_plan(fn, N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows, &pl);
+    int rc = wide_bwd_plan(fn, N, H, W, C, K, R, S, stride, pad_h, pad_w, dil_h, dil_w, row_pitch, image_rows, &pl);
     if (rc) return rc;
     PCNN_REQUIRE(((uintptr_t)x_bf16 & 15) == 0 && ((uintptr_t)dy_bf16 & 15) == 0, PCNN_ERR_ARG,
                  "%s: x and dy must be 16-byte aligned (TMA)", fn);
@@ -487,11 +514,11 @@ static int wide_wgrad(const char *fn, pcnn_ctx *ctx, const void *x_bf16, const v
 
 // epi: the transposed convolution's forward (bias may be NULL, act PCNN_ACT_*); otherwise bias and act are unused
 static int wide_dgrad(const char *fn, pcnn_ctx *ctx, const void *dy_bf16, const float *filt_f32_dev, void *dx_bf16, int N, int H, int W,
-                      int C, int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch, int image_rows, bool epi = false,
-                      const float *bias = nullptr, int act = PCNN_ACT_NONE) {
+                      int C, int K, int R, int S, int stride, int pad_h, int pad_w, int dil_h, int dil_w, int row_pitch, int image_rows,
+                      bool epi = false, const float *bias = nullptr, int act = PCNN_ACT_NONE) {
     PCNN_REQUIRE(ctx && dy_bf16 && filt_f32_dev && dx_bf16, PCNN_ERR_ARG, "%s: NULL argument", fn);
     WideBwdPlan pl;
-    int rc = wide_bwd_plan(fn, N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows, &pl);
+    int rc = wide_bwd_plan(fn, N, H, W, C, K, R, S, stride, pad_h, pad_w, dil_h, dil_w, row_pitch, image_rows, &pl);
     if (rc) return rc;
     PCNN_REQUIRE(((uintptr_t)dy_bf16 & 15) == 0 && ((uintptr_t)dx_bf16 & 15) == 0, PCNN_ERR_ARG,
                  "%s: dy and dx must be 16-byte aligned (TMA)", fn);
@@ -545,36 +572,57 @@ static int wide_dgrad(const char *fn, pcnn_ctx *ctx, const void *dy_bf16, const 
 
 extern "C" int pcnn_conv_wide_bwd_info(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows,
                                        int *out10) {
-    return wide_bwd_info("pcnn_conv_wide_bwd_info", N, H, W, C, K, R, S, stride, 0, 0, row_pitch, image_rows, out10);
+    return wide_bwd_info("pcnn_conv_wide_bwd_info", N, H, W, C, K, R, S, stride, 0, 0, 1, 1, row_pitch, image_rows, out10);
 }
 
 extern "C" int pcnn_conv_wide_bwd_info_padded(int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w,
                                               int row_pitch, int image_rows, int *out10) {
-    return wide_bwd_info("pcnn_conv_wide_bwd_info_padded", N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows, out10);
+    return wide_bwd_info("pcnn_conv_wide_bwd_info_padded", N, H, W, C, K, R, S, stride, pad_h, pad_w, 1, 1, row_pitch, image_rows, out10);
+}
+
+extern "C" int pcnn_conv_wide_bwd_info_dilated(int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w,
+                                               int dil_h, int dil_w, int row_pitch, int image_rows, int *out10) {
+    return wide_bwd_info("pcnn_conv_wide_bwd_info_dilated", N, H, W, C, K, R, S, stride, pad_h, pad_w, dil_h, dil_w, row_pitch,
+                         image_rows, out10);
 }
 
 extern "C" int pcnn_conv_wide_wgrad(pcnn_ctx *ctx, const void *x_bf16, const void *dy_bf16, float *dw_f32, int N, int H, int W, int C,
                                     int K, int R, int S, int stride, int row_pitch, int image_rows) {
-    return wide_wgrad("pcnn_conv_wide_wgrad", ctx, x_bf16, dy_bf16, dw_f32, N, H, W, C, K, R, S, stride, 0, 0, row_pitch, image_rows);
+    return wide_wgrad("pcnn_conv_wide_wgrad", ctx, x_bf16, dy_bf16, dw_f32, N, H, W, C, K, R, S, stride, 0, 0, 1, 1, row_pitch,
+                      image_rows);
 }
 
 extern "C" int pcnn_conv_wide_wgrad_padded(pcnn_ctx *ctx, const void *x_bf16, const void *dy_bf16, float *dw_f32, int N, int H, int W,
                                            int C, int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch, int image_rows) {
-    return wide_wgrad("pcnn_conv_wide_wgrad_padded", ctx, x_bf16, dy_bf16, dw_f32, N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch,
-                      image_rows);
+    return wide_wgrad("pcnn_conv_wide_wgrad_padded", ctx, x_bf16, dy_bf16, dw_f32, N, H, W, C, K, R, S, stride, pad_h, pad_w, 1, 1,
+                      row_pitch, image_rows);
+}
+
+extern "C" int pcnn_conv_wide_wgrad_dilated(pcnn_ctx *ctx, const void *x_bf16, const void *dy_bf16, float *dw_f32, int N, int H, int W,
+                                            int C, int K, int R, int S, int stride, int pad_h, int pad_w, int dil_h, int dil_w,
+                                            int row_pitch, int image_rows) {
+    return wide_wgrad("pcnn_conv_wide_wgrad_dilated", ctx, x_bf16, dy_bf16, dw_f32, N, H, W, C, K, R, S, stride, pad_h, pad_w, dil_h,
+                      dil_w, row_pitch, image_rows);
 }
 
 extern "C" int pcnn_conv_wide_dgrad(pcnn_ctx *ctx, const void *dy_bf16, const float *filt_f32_dev, void *dx_bf16, int N, int H, int W,
                                     int C, int K, int R, int S, int stride, int row_pitch, int image_rows) {
-    return wide_dgrad("pcnn_conv_wide_dgrad", ctx, dy_bf16, filt_f32_dev, dx_bf16, N, H, W, C, K, R, S, stride, 0, 0, row_pitch,
+    return wide_dgrad("pcnn_conv_wide_dgrad", ctx, dy_bf16, filt_f32_dev, dx_bf16, N, H, W, C, K, R, S, stride, 0, 0, 1, 1, row_pitch,
                       image_rows);
 }
 
 extern "C" int pcnn_conv_wide_dgrad_padded(pcnn_ctx *ctx, const void *dy_bf16, const float *filt_f32_dev, void *dx_bf16, int N, int H,
                                            int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch,
                                            int image_rows) {
-    return wide_dgrad("pcnn_conv_wide_dgrad_padded", ctx, dy_bf16, filt_f32_dev, dx_bf16, N, H, W, C, K, R, S, stride, pad_h, pad_w,
-                      row_pitch, image_rows);
+    return wide_dgrad("pcnn_conv_wide_dgrad_padded", ctx, dy_bf16, filt_f32_dev, dx_bf16, N, H, W, C, K, R, S, stride, pad_h, pad_w, 1,
+                      1, row_pitch, image_rows);
+}
+
+extern "C" int pcnn_conv_wide_dgrad_dilated(pcnn_ctx *ctx, const void *dy_bf16, const float *filt_f32_dev, void *dx_bf16, int N, int H,
+                                            int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w, int dil_h, int dil_w,
+                                            int row_pitch, int image_rows) {
+    return wide_dgrad("pcnn_conv_wide_dgrad_dilated", ctx, dy_bf16, filt_f32_dev, dx_bf16, N, H, W, C, K, R, S, stride, pad_h, pad_w,
+                      dil_h, dil_w, row_pitch, image_rows);
 }
 
 // ================================================= transposed convolution ===============================================
@@ -607,8 +655,8 @@ static int conv_transpose_shape(const char *fn, int N, int H, int W, int C_in, i
                  "rows / pixels", fn, ho, wo, pad_h, pad_w, stride);
     *H_out = (int)ho;
     *W_out = (int)wo;
-    return wide_bwd_plan(fn, N, (int)ho, (int)wo, C_out, C_in, R, S, stride, pad_h, pad_w, row_pitch == 0 ? (int)wo * C_out : row_pitch,
-                         image_rows, pl);
+    return wide_bwd_plan(fn, N, (int)ho, (int)wo, C_out, C_in, R, S, stride, pad_h, pad_w, 1, 1,
+                         row_pitch == 0 ? (int)wo * C_out : row_pitch, image_rows, pl);
 }
 
 extern "C" int pcnn_conv_transpose_info(int N, int H, int W, int C_in, int C_out, int R, int S, int stride, int pad_h, int pad_w, int op_h,
@@ -637,6 +685,6 @@ extern "C" int pcnn_conv_transpose_fwd(pcnn_ctx *ctx, const void *x_bf16_dev, co
     const int rc = conv_transpose_shape(fn, N, H, W, C_in, C_out, R, S, stride, pad_h, pad_w, op_h, op_w, bias_f32_dev != nullptr, act, &ho,
                                         &wo, &pl, row_pitch, image_rows);
     if (rc) return rc;
-    return wide_dgrad(fn, ctx, x_bf16_dev, filt_f32_dev, y_bf16_dev, N, ho, wo, C_out, C_in, R, S, stride, pad_h, pad_w,
+    return wide_dgrad(fn, ctx, x_bf16_dev, filt_f32_dev, y_bf16_dev, N, ho, wo, C_out, C_in, R, S, stride, pad_h, pad_w, 1, 1,
                       row_pitch == 0 ? wo * C_out : row_pitch, image_rows, true, bias_f32_dev, act);
 }

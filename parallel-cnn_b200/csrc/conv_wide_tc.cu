@@ -22,6 +22,8 @@
 // Zero padding (pcnn_conv_wide_plan_create_padded) moves the box coordinates only: with r - pad_h = st * a_r + rho_r (floor
 // division, 0 <= rho_r < st) tap r reads phase map rho_r at box row p0 + a_r, and columns the same (ConvWideTaps).  A box row
 // or column before the image (a_r < 0) or past it is zero-filled by TMA like the channels >= C; nothing else changes.
+// Dilation (pcnn_conv_wide_plan_create_dilated) is the same table with r * dil_h - pad_h in place of r - pad_h: the device code is
+// the padded forward's, unchanged.
 //
 // Warp roles (288 threads, 1 CTA/SM, persistent over tiles): warps 0-7 = two consumer warpgroups, warp 8 = TMA producer.
 #include "tc_common.cuh"
@@ -41,6 +43,7 @@ constexpr int WD_SMEM_BUDGET = 225 * 1024;
 constexpr int WD_A_BYTES = WD_M * WD_KC * 2;       // 16 KB
 constexpr int WD_STG_BYTES = 64 * WD_KC * 2;       // one staging sub-tile: 64 pixels x 64 channels, 8 KB
 constexpr int WD_MAX_RS = 7;
+constexpr int WD_MAX_DIL = 256;
 
 struct ConvWideParams {
     int Pt, Qt;                  // pixel block: Pt output rows x Qt output columns
@@ -206,31 +209,46 @@ long long conv_wide_pixel_block(int P, int Q, int *Pt, int *Qt) {
     return best;
 }
 
-// r - pad = st * off[r] + ph[r], 0 <= ph[r] < st, for the taps r < R (pad <= R - 1 < 7, so r - pad + 8 * st > 0)
-static void wide_tap_table(int R, int pad, int st, int *ph, int *off) {
+// r * dil - pad = st * off[r] + ph[r], 0 <= ph[r] < st (floor division: r * dil - pad >= -pad may lie many strides before 0)
+static void wide_tap_table(int R, int pad, int dil, int st, int *ph, int *off) {
     for (int r = 0; r < R; ++r) {
-        const int t = r - pad + 8 * st;
-        ph[r] = t % st;
-        off[r] = t / st - 8;
+        const int t = r * dil - pad;
+        ph[r] = ((t % st) + st) % st;
+        off[r] = (t - ph[r]) / st;
     }
 }
 
-int conv_wide_shape(const char *fn, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch,
-                    int image_rows, ConvWideShape *out) {
+int conv_wide_shape(const char *fn, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w, int dil_h,
+                    int dil_w, int row_pitch, int image_rows, ConvWideShape *out) {
     PCNN_REQUIRE(stride >= 1 && stride <= 4, PCNN_ERR_ARG, "%s: stride %d outside 1..4", fn, stride);
     PCNN_REQUIRE(R >= 1 && R <= WD_MAX_RS && S >= 1 && S <= WD_MAX_RS, PCNN_ERR_ARG,
                  "%s: R = %d, S = %d: taps must be 1..7 in each direction", fn, R, S);
-    PCNN_REQUIRE(pad_h >= 0 && pad_h < R && pad_w >= 0 && pad_w < S, PCNN_ERR_ARG,
-                 "%s: padding (%d, %d) with R = %d, S = %d taps: 0 <= pad_h <= R - 1 and 0 <= pad_w <= S - 1 are required", fn, pad_h,
-                 pad_w, R, S);
+    PCNN_REQUIRE(dil_h >= 1 && dil_h <= WD_MAX_DIL && dil_w >= 1 && dil_w <= WD_MAX_DIL, PCNN_ERR_ARG,
+                 "%s: dilation (%d, %d): 1 <= dil_h, dil_w <= %d are required", fn, dil_h, dil_w, WD_MAX_DIL);
+    const bool dilated = dil_h > 1 || dil_w > 1;
+    const int Eh = dil_h * (R - 1) + 1, Ew = dil_w * (S - 1) + 1;     // the window's extent
+    if (!dilated)
+        PCNN_REQUIRE(pad_h >= 0 && pad_h < R && pad_w >= 0 && pad_w < S, PCNN_ERR_ARG,
+                     "%s: padding (%d, %d) with R = %d, S = %d taps: 0 <= pad_h <= R - 1 and 0 <= pad_w <= S - 1 are required", fn, pad_h,
+                     pad_w, R, S);
+    else
+        PCNN_REQUIRE(pad_h >= 0 && pad_h < Eh && pad_w >= 0 && pad_w < Ew, PCNN_ERR_ARG,
+                     "%s: padding (%d, %d) with R = %d, S = %d taps at dilation (%d, %d): 0 <= pad_h <= dil_h*(R - 1) and "
+                     "0 <= pad_w <= dil_w*(S - 1) are required", fn, pad_h, pad_w, R, S, dil_h, dil_w);
     const bool padded = pad_h > 0 || pad_w > 0;
-    if (!padded)
+    if (dilated)
+        PCNN_REQUIRE(N > 0 && H >= Eh - 2 * pad_h && W >= Ew - 2 * pad_w && C > 0 && K > 0, PCNN_ERR_ARG,
+                     "%s: bad shape N=%d H=%d W=%d C=%d K=%d R=%d S=%d padding (%d, %d) dilation (%d, %d): H + 2*pad_h >= dil_h*(R - 1) + 1 "
+                     "and W + 2*pad_w >= dil_w*(S - 1) + 1 are required", fn, N, H, W, C, K, R, S, pad_h, pad_w, dil_h, dil_w);
+    else if (!padded)
         PCNN_REQUIRE(N > 0 && H >= R && W >= S && C > 0 && K > 0, PCNN_ERR_ARG,
                      "%s: bad shape N=%d H=%d W=%d C=%d K=%d R=%d S=%d", fn, N, H, W, C, K, R, S);
     else
         PCNN_REQUIRE(N > 0 && H >= R - 2 * pad_h && W >= S - 2 * pad_w && C > 0 && K > 0, PCNN_ERR_ARG,
                      "%s: bad shape N=%d H=%d W=%d C=%d K=%d R=%d S=%d padding (%d, %d): H + 2*pad_h >= R and W + 2*pad_w >= S are "
                      "required", fn, N, H, W, C, K, R, S, pad_h, pad_w);
+    // a padded direction may read any phase of x (some tap lands on each residue (r*dil - pad) mod st): each must have a row /
+    // pixel inside the image.  Unpadded, the phases read are (r*dil) mod st <= (E - 1) mod st, inside the image since H >= E.
     PCNN_REQUIRE((pad_h == 0 || H >= stride) && (pad_w == 0 || W >= stride), PCNN_ERR_ARG,
                  "%s: H = %d, W = %d with padding (%d, %d) at stride %d: a padded direction needs at least stride rows / pixels, "
                  "so that every phase of x has one inside the image", fn, H, W, pad_h, pad_w, stride);
@@ -242,10 +260,10 @@ int conv_wide_shape(const char *fn, int N, int H, int W, int C, int K, int R, in
                  "%s: row pitch %d must be >= W*C and a multiple of 8 elements (TMA 16-byte strides)", fn, row_pitch);
     if (image_rows <= 0) image_rows = H;
     PCNN_REQUIRE(image_rows >= H, PCNN_ERR_ARG, "%s: image pitch of %d rows is smaller than H = %d", fn, image_rows, H);
-    int tc[5];                              // the row-Toeplitz plan has no padding: a padded shape is this plan's alone
-    PCNN_REQUIRE(padded || pcnn_conv_tc_plan_info(N, H, W, C, K, R, S, stride, row_pitch, image_rows, tc) != PCNN_OK, PCNN_ERR_ARG,
-                 "%s: this shape is served by the row-Toeplitz forward: use pcnn_conv_tc_plan_create", fn);
-    const int P = (H + 2 * pad_h - R) / stride + 1, Q = (W + 2 * pad_w - S) / stride + 1;
+    int tc[5];                              // the row-Toeplitz plan has no padding and no dilation: such a shape is this plan's alone
+    PCNN_REQUIRE(padded || dilated || pcnn_conv_tc_plan_info(N, H, W, C, K, R, S, stride, row_pitch, image_rows, tc) != PCNN_OK,
+                 PCNN_ERR_ARG, "%s: this shape is served by the row-Toeplitz forward: use pcnn_conv_tc_plan_create", fn);
+    const int P = (H + 2 * pad_h - Eh) / stride + 1, Q = (W + 2 * pad_w - Ew) / stride + 1;
     const long long best = conv_wide_pixel_block(P, Q, &out->Pt, &out->Qt);
     out->n_pb = (P + out->Pt - 1) / out->Pt;
     out->n_qb = (Q + out->Qt - 1) / out->Qt;
@@ -257,15 +275,15 @@ int conv_wide_shape(const char *fn, int N, int H, int W, int C, int K, int R, in
     int st = (int)(((size_t)WD_SMEM_BUDGET - fixed) / wide_stage_bytes(out->npad));
     out->stages = st > WD_MAX_STAGES ? WD_MAX_STAGES : st;
     out->P = P; out->Q = Q;
-    wide_tap_table(R, pad_h, stride, out->taps.rph, out->taps.roff);
-    wide_tap_table(S, pad_w, stride, out->taps.sph, out->taps.soff);
+    wide_tap_table(R, pad_h, dil_h, stride, out->taps.rph, out->taps.roff);
+    wide_tap_table(S, pad_w, dil_w, stride, out->taps.sph, out->taps.soff);
     return PCNN_OK;
 }
 
 // x phase (rb, sb) of the window step: input rows rb, rb + st, ... and pixels sb, sb + st, ... of every image; the extents end at
 // the image's last row and pixel, so a box never reads pad rows, pad columns or the next image.  Only the phases some tap reads
 // are encoded (rb < min(st, R) at pad 0; with padding they need not be a prefix); each has a row and a pixel inside the image
-// (H >= R at pad 0, H >= st when padded, and the same for W).
+// (H >= dil_h*(R - 1) + 1 at pad 0, H >= st when padded, and the same for W).
 int conv_wide_x_maps(CUtensorMap *maps, const void *x_bf16, int N, int H, int W, int C, int R, int S, int st, const ConvWideTaps &taps,
                      int row_pitch, int image_rows, int Pt, int Qt) {
     bool row_used[4] = {}, col_used[4] = {};
@@ -284,7 +302,7 @@ int conv_wide_x_maps(CUtensorMap *maps, const void *x_bf16, int N, int H, int W,
     return PCNN_OK;
 }
 
-// a plan of pcnn_conv_wide_plan_create(_padded): w is [K][R*S*C], the KRSC master with rows of R*S*C elements and no pad
+// a plan of pcnn_conv_wide_plan_create(_padded, _dilated): w is [K][R*S*C], the KRSC master with rows of R*S*C elements and no pad
 struct ConvWidePlan : pcnn_conv_plan {
     ConvWideParams p;
     ConvWideShape sh;
@@ -295,9 +313,9 @@ struct ConvWidePlan : pcnn_conv_plan {
 
 // the query of the create call `fn` (its refusals name that call)
 static int wide_plan_info(const char *fn, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w,
-                          int row_pitch, int image_rows, int *out8) {
+                          int dil_h, int dil_w, int row_pitch, int image_rows, int *out8) {
     ConvWideShape sh;
-    int rc = conv_wide_shape(fn, N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows, &sh);
+    int rc = conv_wide_shape(fn, N, H, W, C, K, R, S, stride, pad_h, pad_w, dil_h, dil_w, row_pitch, image_rows, &sh);
     if (rc) return rc;
     out8[0] = sh.Pt; out8[1] = sh.Qt; out8[2] = sh.nch; out8[3] = sh.stages;
     out8[4] = sh.tiles; out8[5] = sh.n_pb; out8[6] = sh.n_qb; out8[7] = sh.npad;
@@ -307,22 +325,30 @@ static int wide_plan_info(const char *fn, int N, int H, int W, int C, int K, int
 extern "C" int pcnn_conv_wide_plan_info(int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch, int image_rows,
                                         int *out8) {
     PCNN_REQUIRE(out8, PCNN_ERR_ARG, "pcnn_conv_wide_plan_info: NULL argument");
-    return wide_plan_info("pcnn_conv_wide_plan_create", N, H, W, C, K, R, S, stride, 0, 0, row_pitch, image_rows, out8);
+    return wide_plan_info("pcnn_conv_wide_plan_create", N, H, W, C, K, R, S, stride, 0, 0, 1, 1, row_pitch, image_rows, out8);
 }
 
 extern "C" int pcnn_conv_wide_plan_info_padded(int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w,
                                                int row_pitch, int image_rows, int *out8) {
     PCNN_REQUIRE(out8, PCNN_ERR_ARG, "pcnn_conv_wide_plan_info_padded: NULL argument");
-    return wide_plan_info("pcnn_conv_wide_plan_create_padded", N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows, out8);
+    return wide_plan_info("pcnn_conv_wide_plan_create_padded", N, H, W, C, K, R, S, stride, pad_h, pad_w, 1, 1, row_pitch, image_rows,
+                          out8);
+}
+
+extern "C" int pcnn_conv_wide_plan_info_dilated(int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w,
+                                                int dil_h, int dil_w, int row_pitch, int image_rows, int *out8) {
+    PCNN_REQUIRE(out8, PCNN_ERR_ARG, "pcnn_conv_wide_plan_info_dilated: NULL argument");
+    return wide_plan_info("pcnn_conv_wide_plan_create_dilated", N, H, W, C, K, R, S, stride, pad_h, pad_w, dil_h, dil_w, row_pitch,
+                          image_rows, out8);
 }
 
 static int wide_plan_create(const char *fn, pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h,
-                            int pad_w, int row_pitch, int image_rows, int act, const float *filt_host, const float *bias_host,
-                            pcnn_conv_plan **out) {
+                            int pad_w, int dil_h, int dil_w, int row_pitch, int image_rows, int act, const float *filt_host,
+                            const float *bias_host, pcnn_conv_plan **out) {
     PCNN_REQUIRE(ctx && filt_host && out, PCNN_ERR_ARG, "%s: NULL argument", fn);
     PCNN_REQUIRE_ACT(fn, act);
     ConvWideShape sh;
-    int rc = conv_wide_shape(fn, N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows, &sh);
+    int rc = conv_wide_shape(fn, N, H, W, C, K, R, S, stride, pad_h, pad_w, dil_h, dil_w, row_pitch, image_rows, &sh);
     if (rc) return rc;
     pcnn_device_guard g(ctx->device);
     std::unique_ptr<ConvWidePlan> pl(new ConvWidePlan());   // frees a half-built plan on every early return below
@@ -360,15 +386,22 @@ static int wide_plan_create(const char *fn, pcnn_ctx *ctx, int N, int H, int W, 
 extern "C" int pcnn_conv_wide_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int stride, int row_pitch,
                                           int image_rows, int act, const float *filt_host, const float *bias_host,
                                           pcnn_conv_plan **out) {
-    return wide_plan_create("pcnn_conv_wide_plan_create", ctx, N, H, W, C, K, R, S, stride, 0, 0, row_pitch, image_rows, act, filt_host,
-                            bias_host, out);
+    return wide_plan_create("pcnn_conv_wide_plan_create", ctx, N, H, W, C, K, R, S, stride, 0, 0, 1, 1, row_pitch, image_rows, act,
+                            filt_host, bias_host, out);
 }
 
 extern "C" int pcnn_conv_wide_plan_create_padded(pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h,
                                                  int pad_w, int row_pitch, int image_rows, int act, const float *filt_host,
                                                  const float *bias_host, pcnn_conv_plan **out) {
-    return wide_plan_create("pcnn_conv_wide_plan_create_padded", ctx, N, H, W, C, K, R, S, stride, pad_h, pad_w, row_pitch, image_rows,
-                            act, filt_host, bias_host, out);
+    return wide_plan_create("pcnn_conv_wide_plan_create_padded", ctx, N, H, W, C, K, R, S, stride, pad_h, pad_w, 1, 1, row_pitch,
+                            image_rows, act, filt_host, bias_host, out);
+}
+
+extern "C" int pcnn_conv_wide_plan_create_dilated(pcnn_ctx *ctx, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h,
+                                                  int pad_w, int dil_h, int dil_w, int row_pitch, int image_rows, int act,
+                                                  const float *filt_host, const float *bias_host, pcnn_conv_plan **out) {
+    return wide_plan_create("pcnn_conv_wide_plan_create_dilated", ctx, N, H, W, C, K, R, S, stride, pad_h, pad_w, dil_h, dil_w, row_pitch,
+                            image_rows, act, filt_host, bias_host, out);
 }
 
 int ConvWidePlan::fwd(pcnn_ctx *ctx, const void *x_bf16, void *y_bf16) {

@@ -14,6 +14,11 @@
 //   - Weight gradient: CTA (pixel range, channel slice) walks filter rows r; each thread keeps S x VEC fp32 sums of one filter row
 //     over the pixels lane, lane + lanes, ... of its range, the lanes are added in lane order through shared memory, and each range
 //     writes an fp32 slot [C][R][S] that pcnn_conv_wgrad_reduce_slots adds in a fixed order.  The ranges depend on the shape only.
+// Dilation (pcnn_dwconv_plan_create_dilated): tap (r, s) sits r*dil_h rows and s*dil_w columns from the window's corner.  Each pass
+// has a second instantiation (DIL), so the undilated ones keep their code.  The DIL forward walks the taps of each output (for r, s,
+// output k: x column q0 st + k st + s dil_w, repeats served by L1), so it loads no column that no output of the strip reads; the DIL
+// input gradient walks each element's taps in ascending s and finds the dy column (w + pad_w - s dil_w) / stride; the DIL weight
+// gradient reads x at w0 + s*dil_w.  The orders stay those stated above.
 #include "pcnn_internal.h"
 
 #include <cuda_bf16.h>
@@ -43,6 +48,7 @@ struct DwArgs {
     long long M;            // N P Q output pixels
     int per_range, ranges;  // weight gradient: pixels per range (lanes * DW_ITERS) and ranges
     int act;
+    int dil_h, dil_w;       // dilation (1 = none)
 };
 
 template <int VEC>
@@ -63,7 +69,7 @@ __device__ __forceinline__ void stage_filters(const __nv_bfloat16 *__restrict__ 
     }
 }
 
-template <int VEC>
+template <int VEC, bool DIL>
 __global__ void __launch_bounds__(DW_THREADS) k_dwconv_fwd(const __nv_bfloat16 *__restrict__ x, const __nv_bfloat16 *__restrict__ wop,
                                                            const float *__restrict__ bias, __nv_bfloat16 *__restrict__ y, DwArgs a) {
     __shared__ __align__(16) __nv_bfloat16 wsm[DW_MAX_TAPS * DW_MAX_TAPS * DW_MAX_GROUPS * VEC];
@@ -85,9 +91,24 @@ __global__ void __launch_bounds__(DW_THREADS) k_dwconv_fwd(const __nv_bfloat16 *
         for (int e = 0; e < VEC; ++e) acc[k][e] = -0.0f;
     const int ncols = (DW_QS - 1) * st + a.S, wstart = q0 * st - a.pad_w;
     for (int r = 0; r < a.R; ++r) {
-        const int h = p * st - a.pad_h + r;
+        const int h = p * st - a.pad_h + r * (DIL ? a.dil_h : 1);
         const bool rowok = h >= 0 && h < a.H;
         const __nv_bfloat16 *row = xi + (long)h * a.W * a.C;
+        if (DIL) {                                         // tap by tap: only the columns some output of the strip reads
+            for (int s = 0; s < a.S; ++s) {
+                const BfVec<VEC> wv = *reinterpret_cast<const BfVec<VEC> *>(wg + (r * a.S + s) * width);
+#pragma unroll
+                for (int k = 0; k < DW_QS; ++k) {
+                    const int w = wstart + k * st + s * a.dil_w;
+                    if (q0 + k >= a.Q) continue;
+                    BfVec<VEC> xv = bf_zero<VEC>();
+                    if (rowok && w >= 0 && w < a.W) xv = *reinterpret_cast<const BfVec<VEC> *>(row + (long)w * a.C);
+#pragma unroll
+                    for (int e = 0; e < VEC; ++e) acc[k][e] = fmaf(__bfloat162float(xv.h[e]), __bfloat162float(wv.h[e]), acc[k][e]);
+                }
+            }
+            continue;
+        }
         for (int j = 0; j < ncols; ++j) {
             const int w = wstart + j;
             BfVec<VEC> xv = bf_zero<VEC>();
@@ -117,7 +138,7 @@ __global__ void __launch_bounds__(DW_THREADS) k_dwconv_fwd(const __nv_bfloat16 *
     }
 }
 
-template <int VEC>
+template <int VEC, bool DIL>
 __global__ void __launch_bounds__(DW_THREADS) k_dwconv_dgrad(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ wop,
                                                              __nv_bfloat16 *__restrict__ dx, DwArgs a) {
     __shared__ __align__(16) __nv_bfloat16 wsm[DW_MAX_TAPS * DW_MAX_TAPS * DW_MAX_GROUPS * VEC];
@@ -137,15 +158,32 @@ __global__ void __launch_bounds__(DW_THREADS) k_dwconv_dgrad(const __nv_bfloat16
     for (int k = 0; k < DW_QS; ++k)
 #pragma unroll
         for (int e = 0; e < VEC; ++e) acc[k][e] = -0.0f;
+    bool khit[DW_QS] = {};                                 // DIL: element k has a term
     // dy columns q with 0 <= w + pad_w - q stride < S for some w of the strip, inside [0, Q)
     const int nw = w0 + a.pad_w - a.S + 1;
     const int qlo = nw <= 0 ? 0 : (nw + st - 1) / st, qhi = min(a.Q - 1, (w0 + DW_QS - 1 + a.pad_w) / st);
     bool rowhit = false;
     for (int r = 0; r < a.R; ++r) {
-        const int t = h + a.pad_h - r;
+        const int t = h + a.pad_h - r * (DIL ? a.dil_h : 1);
         if (t < 0 || t % st != 0 || t / st >= a.P) continue;
         rowhit = true;
         const __nv_bfloat16 *row = dyi + (long)(t / st) * a.Q * a.C;
+        if (DIL) {                                         // element by element, taps in ascending s: only the dy columns read
+#pragma unroll
+            for (int k = 0; k < DW_QS; ++k) {
+                for (int s = 0; s < a.S; ++s) {
+                    const int u = w0 + k + a.pad_w - s * a.dil_w;
+                    if (u < 0) break;
+                    if (u % st != 0 || u / st >= a.Q) continue;
+                    khit[k] = true;
+                    const BfVec<VEC> d = *reinterpret_cast<const BfVec<VEC> *>(row + (long)(u / st) * a.C);
+                    const BfVec<VEC> wv = *reinterpret_cast<const BfVec<VEC> *>(wg + (r * a.S + s) * width);
+#pragma unroll
+                    for (int e = 0; e < VEC; ++e) acc[k][e] = fmaf(__bfloat162float(d.h[e]), __bfloat162float(wv.h[e]), acc[k][e]);
+                }
+            }
+            continue;
+        }
         for (int q = qhi; q >= qlo; --q) {                 // descending q: ascending s for every element of the strip
             const BfVec<VEC> d = *reinterpret_cast<const BfVec<VEC> *>(row + (long)q * a.C);
 #pragma unroll
@@ -166,7 +204,7 @@ __global__ void __launch_bounds__(DW_THREADS) k_dwconv_dgrad(const __nv_bfloat16
         // the taps of (h, w) are the valid rows times the valid columns: none when either set is empty
         const int nk = w + a.pad_w - a.S + 1;
         const int ql = nk <= 0 ? 0 : (nk + st - 1) / st, qh = min(a.Q - 1, (w + a.pad_w) / st);
-        const bool hit = rowhit && ql <= qh;
+        const bool hit = DIL ? khit[k] : rowhit && ql <= qh;
         BfVec<VEC> out;
 #pragma unroll
         for (int e = 0; e < VEC; ++e) out.h[e] = hit ? __float2bfloat16_rn(acc[k][e]) : __ushort_as_bfloat16(0);
@@ -176,7 +214,7 @@ __global__ void __launch_bounds__(DW_THREADS) k_dwconv_dgrad(const __nv_bfloat16
 
 // CTA (range, slice): out[c][r][s] for the slice's channels over the pixels [range * per_range, (range + 1) * per_range) of the
 // N P Q output pixels; `out` is dw itself when there is one range, otherwise slot `range` of the [ranges][C][R][S] partials
-template <int VEC, int S>
+template <int VEC, int S, bool DIL>
 __global__ void __launch_bounds__(DW_THREADS) k_dwconv_wgrad(const __nv_bfloat16 *__restrict__ x, const __nv_bfloat16 *__restrict__ dy,
                                                              float *__restrict__ out, DwArgs a) {
     __shared__ float part[DW_THREADS * 8];                 // [lanes][Gc * VEC]
@@ -199,12 +237,12 @@ __global__ void __launch_bounds__(DW_THREADS) k_dwconv_wgrad(const __nv_bfloat16
                 if (m >= a.M || m >= p0 + a.per_range) break;
                 const int n = (int)(m / PQ), pq = (int)(m - (long long)n * PQ), p = pq / a.Q, q = pq - p * a.Q;
                 const BfVec<VEC> d = *reinterpret_cast<const BfVec<VEC> *>(dy + m * a.C + c);
-                const int h = p * st - a.pad_h + r, w0 = q * st - a.pad_w;
+                const int h = p * st - a.pad_h + r * (DIL ? a.dil_h : 1), w0 = q * st - a.pad_w;
                 const bool rowok = h >= 0 && h < a.H;
                 const __nv_bfloat16 *row = x + ((long)n * a.H + h) * a.W * a.C + c;
 #pragma unroll
                 for (int s = 0; s < S; ++s) {
-                    const int w = w0 + s;
+                    const int w = w0 + s * (DIL ? a.dil_w : 1);
                     BfVec<VEC> xv = bf_zero<VEC>();
                     if (rowok && w >= 0 && w < a.W) xv = *reinterpret_cast<const BfVec<VEC> *>(row + (long)w * a.C);
 #pragma unroll
@@ -230,29 +268,53 @@ __global__ void __launch_bounds__(DW_THREADS) k_dwconv_wgrad(const __nv_bfloat16
 
 }  // namespace
 
-int nhwc_window_check(const char *fn, int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int *P, int *Q) {
+namespace {
+
+constexpr int DW_MAX_DIL = 256;
+
+// nhwc_window_check with a dilation: at (1, 1) exactly it, messages included
+int nhwc_window_check_dilated(const char *fn, int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int dil_h,
+                              int dil_w, int *P, int *Q) {
     PCNN_REQUIRE(N >= 1 && H >= 1 && W >= 1 && C >= 1, PCNN_ERR_ARG, "%s: N = %d, H = %d, W = %d, C = %d: each must be >= 1", fn, N, H, W,
                  C);
     PCNN_REQUIRE(R >= 1 && R <= DW_MAX_TAPS && S >= 1 && S <= DW_MAX_TAPS, PCNN_ERR_ARG, "%s: %dx%d filter: 1 <= R, S <= 7 is required",
                  fn, R, S);
     PCNN_REQUIRE(stride >= 1 && stride <= 4, PCNN_ERR_ARG, "%s: stride %d: 1 <= stride <= 4 is required", fn, stride);
-    PCNN_REQUIRE(pad_h >= 0 && pad_h <= R - 1 && pad_w >= 0 && pad_w <= S - 1, PCNN_ERR_ARG,
-                 "%s: padding (%d, %d) for a %dx%d filter: 0 <= pad_h <= R - 1 and 0 <= pad_w <= S - 1 are required", fn, pad_h, pad_w, R,
-                 S);
-    PCNN_REQUIRE(H + 2 * pad_h >= R && W + 2 * pad_w >= S, PCNN_ERR_ARG,
-                 "%s: a %dx%d filter does not fit the %dx%d image padded by (%d, %d): H + 2 pad_h >= R and W + 2 pad_w >= S are required",
-                 fn, R, S, H, W, pad_h, pad_w);
-    *P = (H + 2 * pad_h - R) / stride + 1;
-    *Q = (W + 2 * pad_w - S) / stride + 1;
+    PCNN_REQUIRE(dil_h >= 1 && dil_h <= DW_MAX_DIL && dil_w >= 1 && dil_w <= DW_MAX_DIL, PCNN_ERR_ARG,
+                 "%s: dilation (%d, %d): 1 <= dil_h, dil_w <= %d are required", fn, dil_h, dil_w, DW_MAX_DIL);
+    const int Eh = dil_h * (R - 1) + 1, Ew = dil_w * (S - 1) + 1;     // the window's extent
+    if (dil_h == 1 && dil_w == 1) {
+        PCNN_REQUIRE(pad_h >= 0 && pad_h <= R - 1 && pad_w >= 0 && pad_w <= S - 1, PCNN_ERR_ARG,
+                     "%s: padding (%d, %d) for a %dx%d filter: 0 <= pad_h <= R - 1 and 0 <= pad_w <= S - 1 are required", fn, pad_h, pad_w,
+                     R, S);
+        PCNN_REQUIRE(H + 2 * pad_h >= R && W + 2 * pad_w >= S, PCNN_ERR_ARG,
+                     "%s: a %dx%d filter does not fit the %dx%d image padded by (%d, %d): H + 2 pad_h >= R and W + 2 pad_w >= S are required",
+                     fn, R, S, H, W, pad_h, pad_w);
+    } else {
+        PCNN_REQUIRE(pad_h >= 0 && pad_h <= Eh - 1 && pad_w >= 0 && pad_w <= Ew - 1, PCNN_ERR_ARG,
+                     "%s: padding (%d, %d) for a %dx%d filter at dilation (%d, %d): 0 <= pad_h <= dil_h (R - 1) and 0 <= pad_w <= dil_w (S - 1) "
+                     "are required", fn, pad_h, pad_w, R, S, dil_h, dil_w);
+        PCNN_REQUIRE(H + 2 * pad_h >= Eh && W + 2 * pad_w >= Ew, PCNN_ERR_ARG,
+                     "%s: a %dx%d filter at dilation (%d, %d) does not fit the %dx%d image padded by (%d, %d): H + 2 pad_h >= dil_h (R - 1) + 1 "
+                     "and W + 2 pad_w >= dil_w (S - 1) + 1 are required", fn, R, S, dil_h, dil_w, H, W, pad_h, pad_w);
+    }
+    *P = (H + 2 * pad_h - Eh) / stride + 1;
+    *Q = (W + 2 * pad_w - Ew) / stride + 1;
     return PCNN_OK;
+}
+
+}  // namespace
+
+int nhwc_window_check(const char *fn, int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int *P, int *Q) {
+    return nhwc_window_check_dilated(fn, N, H, W, C, R, S, stride, pad_h, pad_w, 1, 1, P, Q);
 }
 
 namespace {
 
 // the domain of pcnn.h, refused with PCNN_ERR_ARG and a message naming `fn`, and the partition, a function of the shape alone
-int dw_shape(const char *fn, int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, DwArgs *a) {
+int dw_shape(const char *fn, int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int dil_h, int dil_w, DwArgs *a) {
     int P, Q;
-    const int rc = nhwc_window_check(fn, N, H, W, C, R, S, stride, pad_h, pad_w, &P, &Q);
+    const int rc = nhwc_window_check_dilated(fn, N, H, W, C, R, S, stride, pad_h, pad_w, dil_h, dil_w, &P, &Q);
     if (rc) return rc;
     PCNN_REQUIRE((long)H * W * C <= INT32_MAX && (long)P * Q * C <= INT32_MAX && (long)C * R * S <= INT32_MAX, PCNN_ERR_ARG,
                  "%s: one %dx%dx%d image (or its %d x %d x %d filters) exceeds the 32-bit index range: H W C, P Q C and C R S < 2^31 are "
@@ -275,6 +337,7 @@ int dw_shape(const char *fn, int N, int H, int W, int C, int R, int S, int strid
                  PCNN_ERR_ARG, "%s: %d images of %dx%dx%d exceed the grid", fn, N, H, W, C);
     a->ranges = (int)ranges;
     a->act = 0;
+    a->dil_h = dil_h; a->dil_w = dil_w;
     return PCNN_OK;
 }
 
@@ -294,16 +357,17 @@ bool overlap(const void *p, size_t np, const void *q, size_t nq) {
 bool aligned16(const void *p) { return ((uintptr_t)p & 15) == 0; }
 
 typedef void (*wgrad_fn)(const __nv_bfloat16 *, const __nv_bfloat16 *, float *, DwArgs);
-template <int VEC>
+template <int VEC, bool DIL>
 wgrad_fn wgrad_variant(int S) {
-    static const wgrad_fn t[DW_MAX_TAPS] = {k_dwconv_wgrad<VEC, 1>, k_dwconv_wgrad<VEC, 2>, k_dwconv_wgrad<VEC, 3>, k_dwconv_wgrad<VEC, 4>,
-                                            k_dwconv_wgrad<VEC, 5>, k_dwconv_wgrad<VEC, 6>, k_dwconv_wgrad<VEC, 7>};
+    static const wgrad_fn t[DW_MAX_TAPS] = {k_dwconv_wgrad<VEC, 1, DIL>, k_dwconv_wgrad<VEC, 2, DIL>, k_dwconv_wgrad<VEC, 3, DIL>,
+                                            k_dwconv_wgrad<VEC, 4, DIL>, k_dwconv_wgrad<VEC, 5, DIL>, k_dwconv_wgrad<VEC, 6, DIL>,
+                                            k_dwconv_wgrad<VEC, 7, DIL>};
     return t[S - 1];
 }
 
 }  // namespace
 
-// a plan of pcnn_dwconv_plan_create: w is [C][R][S], the fp32 master's element order (one row of n elements)
+// a plan of pcnn_dwconv_plan_create(_dilated): w is [C][R][S], the fp32 master's element order (one row of n elements)
 struct DwConvPlan : pcnn_conv_plan {
     static constexpr const char *made_by = "pcnn_dwconv_plan_create";
     DwArgs a;
@@ -311,27 +375,35 @@ struct DwConvPlan : pcnn_conv_plan {
     int fwd(pcnn_ctx *ctx, const void *x_bf16, void *y_bf16) override;
 };
 
-extern "C" int pcnn_dwconv_info(int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int *out9) {
-    const char *fn = "pcnn_dwconv_info";
+static int dw_info(const char *fn, int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int dil_h, int dil_w,
+                   int *out9) {
     PCNN_REQUIRE(out9, PCNN_ERR_ARG, "%s: NULL out9", fn);
     DwArgs a;
-    int rc = dw_shape(fn, N, H, W, C, R, S, stride, pad_h, pad_w, &a);
+    int rc = dw_shape(fn, N, H, W, C, R, S, stride, pad_h, pad_w, dil_h, dil_w, &a);
     if (rc) return rc;
     const int v[9] = {a.P, a.Q, C % 8 == 0 ? 8 : 1, a.Gc, a.slices, a.lanes, a.per_range, a.ranges, dw_n_acc(a)};
     memcpy(out9, v, sizeof(v));
     return PCNN_OK;
 }
 
-extern "C" int pcnn_dwconv_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int act,
-                                       const float *filt_host, const float *bias_host, pcnn_conv_plan **out) {
-    const char *fn = "pcnn_dwconv_plan_create";
+extern "C" int pcnn_dwconv_info(int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int *out9) {
+    return dw_info("pcnn_dwconv_info", N, H, W, C, R, S, stride, pad_h, pad_w, 1, 1, out9);
+}
+
+extern "C" int pcnn_dwconv_info_dilated(int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int dil_h, int dil_w,
+                                        int *out9) {
+    return dw_info("pcnn_dwconv_info_dilated", N, H, W, C, R, S, stride, pad_h, pad_w, dil_h, dil_w, out9);
+}
+
+static int dw_plan_create(const char *fn, pcnn_ctx *ctx, int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w,
+                          int dil_h, int dil_w, int act, const float *filt_host, const float *bias_host, pcnn_conv_plan **out) {
     PCNN_REQUIRE(ctx && filt_host && out, PCNN_ERR_ARG, "%s: NULL context, filters or out", fn);
     PCNN_REQUIRE_ACT(fn, act);
     PCNN_REQUIRE(act != PCNN_ACT_SIGMOID, PCNN_ERR_ARG,
                  "%s: act 1 (sigmoid) is not supported: the sigmoid of the conv epilogues uses tanh.approx, which no reference can replay "
                  "bit for bit; use act 0 or 3", fn);
     DwArgs a;
-    int rc = dw_shape(fn, N, H, W, C, R, S, stride, pad_h, pad_w, &a);
+    int rc = dw_shape(fn, N, H, W, C, R, S, stride, pad_h, pad_w, dil_h, dil_w, &a);
     if (rc) return rc;
     a.act = act;
     pcnn_device_guard g(ctx->device);
@@ -345,6 +417,18 @@ extern "C" int pcnn_dwconv_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C
     return PCNN_OK;
 }
 
+extern "C" int pcnn_dwconv_plan_create(pcnn_ctx *ctx, int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w, int act,
+                                       const float *filt_host, const float *bias_host, pcnn_conv_plan **out) {
+    return dw_plan_create("pcnn_dwconv_plan_create", ctx, N, H, W, C, R, S, stride, pad_h, pad_w, 1, 1, act, filt_host, bias_host, out);
+}
+
+extern "C" int pcnn_dwconv_plan_create_dilated(pcnn_ctx *ctx, int N, int H, int W, int C, int R, int S, int stride, int pad_h, int pad_w,
+                                               int dil_h, int dil_w, int act, const float *filt_host, const float *bias_host,
+                                               pcnn_conv_plan **out) {
+    return dw_plan_create("pcnn_dwconv_plan_create_dilated", ctx, N, H, W, C, R, S, stride, pad_h, pad_w, dil_h, dil_w, act, filt_host,
+                          bias_host, out);
+}
+
 int DwConvPlan::fwd(pcnn_ctx *ctx, const void *x_bf16, void *y_bf16) {
     const char *fn = "pcnn_conv_tc_fwd";
     PCNN_REQUIRE(aligned16(y_bf16), PCNN_ERR_ARG, "%s: the output must be 16-byte aligned", fn);
@@ -354,10 +438,11 @@ int DwConvPlan::fwd(pcnn_ctx *ctx, const void *x_bf16, void *y_bf16) {
     const dim3 grid((unsigned)((a.fstrips + a.lanes - 1) / a.lanes), (unsigned)a.slices);
     const auto *x = static_cast<const __nv_bfloat16 *>(x_bf16);
     auto *y = static_cast<__nv_bfloat16 *>(y_bf16);
+    const bool dil = a.dil_h > 1 || a.dil_w > 1;
     if (a.C % 8 == 0)
-        k_dwconv_fwd<8><<<grid, DW_THREADS, 0, ctx->stream>>>(x, wop(), bias, y, a);
+        (dil ? k_dwconv_fwd<8, true> : k_dwconv_fwd<8, false>)<<<grid, DW_THREADS, 0, ctx->stream>>>(x, wop(), bias, y, a);
     else
-        k_dwconv_fwd<1><<<grid, DW_THREADS, 0, ctx->stream>>>(x, wop(), bias, y, a);
+        (dil ? k_dwconv_fwd<1, true> : k_dwconv_fwd<1, false>)<<<grid, DW_THREADS, 0, ctx->stream>>>(x, wop(), bias, y, a);
     PCNN_CHECK_LAUNCH(ctx);
     return PCNN_OK;
 }
@@ -379,7 +464,9 @@ extern "C" int pcnn_dwconv_wgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void
     const dim3 grid((unsigned)a.ranges, (unsigned)a.slices);
     const auto *x = static_cast<const __nv_bfloat16 *>(x_bf16);
     const auto *dy = static_cast<const __nv_bfloat16 *>(dy_bf16);
-    const wgrad_fn k = a.C % 8 == 0 ? wgrad_variant<8>(a.S) : wgrad_variant<1>(a.S);
+    const bool dil = a.dil_h > 1 || a.dil_w > 1;
+    const wgrad_fn k = a.C % 8 == 0 ? (dil ? wgrad_variant<8, true>(a.S) : wgrad_variant<8, false>(a.S))
+                                    : (dil ? wgrad_variant<1, true>(a.S) : wgrad_variant<1, false>(a.S));
     k<<<grid, DW_THREADS, 0, ctx->stream>>>(x, dy, out, a);
     PCNN_CHECK_LAUNCH(ctx);
     return a.ranges > 1 ? pcnn_conv_wgrad_reduce_slots(ctx, out, dw_f32, a.ranges, (int)nout) : PCNN_OK;
@@ -399,10 +486,11 @@ extern "C" int pcnn_dwconv_dgrad(pcnn_ctx *ctx, pcnn_conv_plan *plan, const void
     const dim3 grid((unsigned)((a.dstrips + a.lanes - 1) / a.lanes), (unsigned)a.slices);
     const auto *dy = static_cast<const __nv_bfloat16 *>(dy_bf16);
     auto *dx = static_cast<__nv_bfloat16 *>(dx_bf16);
+    const bool dil = a.dil_h > 1 || a.dil_w > 1;
     if (a.C % 8 == 0)
-        k_dwconv_dgrad<8><<<grid, DW_THREADS, 0, ctx->stream>>>(dy, pl->wop(), dx, a);
+        (dil ? k_dwconv_dgrad<8, true> : k_dwconv_dgrad<8, false>)<<<grid, DW_THREADS, 0, ctx->stream>>>(dy, pl->wop(), dx, a);
     else
-        k_dwconv_dgrad<1><<<grid, DW_THREADS, 0, ctx->stream>>>(dy, pl->wop(), dx, a);
+        (dil ? k_dwconv_dgrad<1, true> : k_dwconv_dgrad<1, false>)<<<grid, DW_THREADS, 0, ctx->stream>>>(dy, pl->wop(), dx, a);
     PCNN_CHECK_LAUNCH(ctx);
     return PCNN_OK;
 }

@@ -268,13 +268,14 @@ int nhwc_window_check(const char *fn, int N, int H, int W, int C, int R, int S, 
 // The domain and tiling of the wide forward, which its gradients (conv_wide_bwd_tc.cu) share: one rule, refused with
 // PCNN_ERR_ARG and a message that names `fn`, the caller's entry point.  conv_wide_pixel_block picks the Pt x Qt = 128 block
 // of a P x Q image and returns the blocks per image.
-// Tap r of a window padded by pad_h reads x row st * (p + roff[r]) + rph[r] for output row p: r - pad_h = st * roff[r] + rph[r]
-// with 0 <= rph[r] < st (floor division, so roff[r] < 0 above the image), i.e. phase rph[r] of x at box row p0 + roff[r].
-// Columns the same with sph / soff and pad_w.  At pad 0 these are r % st and r / st.
+// Tap r of a window padded by pad_h and dilated by dil_h reads x row st * (p + roff[r]) + rph[r] for output row p:
+// r * dil_h - pad_h = st * roff[r] + rph[r] with 0 <= rph[r] < st (floor division, so roff[r] < 0 above the image), i.e. phase
+// rph[r] of x at box row p0 + roff[r].  Columns the same with sph / soff, dil_w and pad_w.  At pad 0, dilation 1 these are r % st
+// and r / st.
 struct ConvWideTaps { int rph[7], roff[7], sph[7], soff[7]; };
 struct ConvWideShape { int Pt, Qt, nch, stages, tiles, n_pb, n_qb, npad, P, Q; ConvWideTaps taps; };
-int conv_wide_shape(const char *fn, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w, int row_pitch,
-                    int image_rows, ConvWideShape *out);
+int conv_wide_shape(const char *fn, int N, int H, int W, int C, int K, int R, int S, int stride, int pad_h, int pad_w, int dil_h,
+                    int dil_w, int row_pitch, int image_rows, ConvWideShape *out);
 long long conv_wide_pixel_block(int P, int Q, int *Pt, int *Qt);
 // pool_nhwc.cu: the partition of the global average pool's reduction over the pixels of an image, which the gate gradient of
 // squeeze-and-excitation (se_nhwc.cu) shares so that both sum in one order.  CTA (n, range, slice) of GAP_THREADS threads owns

@@ -397,24 +397,35 @@ class Engine:
         self._call("pcnn_conv_dgrad_strided", _p(dy_bf16), _p(filt_f32), _p(dx_bf16), N, H, W, Cin, K, R, S, int(stride), int(row_pitch),
                    int(image_rows))
 
-    def conv_wide_wgrad(self, x_bf16, dy_bf16, dw_f32, N, H, W, Cin, K, R, S, row_pitch=None, image_rows=0, stride=1, padding=(0, 0)):
+    def conv_wide_wgrad(self, x_bf16, dy_bf16, dw_f32, N, H, W, Cin, K, R, S, row_pitch=None, image_rows=0, stride=1, padding=(0, 0),
+                        dilation=(1, 1)):
         """weight gradient of WideConvPlan's forward (pcnn_conv_wide_wgrad, or pcnn_conv_wide_wgrad_padded for a zero padding
-        (pad_h, pad_w) other than (0, 0)); row_pitch None = W*Cin rounded up to 8, as the plan"""
+        (pad_h, pad_w) other than (0, 0), or pcnn_conv_wide_wgrad_dilated for a dilation other than (1, 1)); row_pitch None =
+        W*Cin rounded up to 8, as the plan"""
         pitch = (W * Cin + 7) // 8 * 8 if row_pitch is None else row_pitch
         ph, pw = (int(v) for v in padding)
-        if (ph, pw) == (0, 0):
+        dh, dw = (int(v) for v in dilation)
+        if (dh, dw) != (1, 1):
+            self._call("pcnn_conv_wide_wgrad_dilated", _p(x_bf16), _p(dy_bf16), _p(dw_f32), N, H, W, Cin, K, R, S, int(stride), ph, pw,
+                       dh, dw, int(pitch), int(image_rows))
+        elif (ph, pw) == (0, 0):
             self._call("pcnn_conv_wide_wgrad", _p(x_bf16), _p(dy_bf16), _p(dw_f32), N, H, W, Cin, K, R, S, int(stride), int(pitch),
                        int(image_rows))
         else:
             self._call("pcnn_conv_wide_wgrad_padded", _p(x_bf16), _p(dy_bf16), _p(dw_f32), N, H, W, Cin, K, R, S, int(stride), ph, pw,
                        int(pitch), int(image_rows))
 
-    def conv_wide_dgrad(self, dy_bf16, filt_f32, dx_bf16, N, H, W, Cin, K, R, S, row_pitch=None, image_rows=0, stride=1, padding=(0, 0)):
+    def conv_wide_dgrad(self, dy_bf16, filt_f32, dx_bf16, N, H, W, Cin, K, R, S, row_pitch=None, image_rows=0, stride=1, padding=(0, 0),
+                        dilation=(1, 1)):
         """input gradient of WideConvPlan's forward (pcnn_conv_wide_dgrad, or pcnn_conv_wide_dgrad_padded for a zero padding
-        (pad_h, pad_w) other than (0, 0)) into dx in x's layout"""
+        (pad_h, pad_w) other than (0, 0), or pcnn_conv_wide_dgrad_dilated for a dilation other than (1, 1)) into dx in x's layout"""
         pitch = (W * Cin + 7) // 8 * 8 if row_pitch is None else row_pitch
         ph, pw = (int(v) for v in padding)
-        if (ph, pw) == (0, 0):
+        dh, dw = (int(v) for v in dilation)
+        if (dh, dw) != (1, 1):
+            self._call("pcnn_conv_wide_dgrad_dilated", _p(dy_bf16), _p(filt_f32), _p(dx_bf16), N, H, W, Cin, K, R, S, int(stride), ph, pw,
+                       dh, dw, int(pitch), int(image_rows))
+        elif (ph, pw) == (0, 0):
             self._call("pcnn_conv_wide_dgrad", _p(dy_bf16), _p(filt_f32), _p(dx_bf16), N, H, W, Cin, K, R, S, int(stride), int(pitch),
                        int(image_rows))
         else:
@@ -722,17 +733,24 @@ class ConvPlan:
 
 class WideConvPlan(ConvPlan):
     """The wide-channel forward (pcnn_conv_wide_plan_create): the shapes ConvPlan refuses, C % 8 == 0, K % 8 == 0, K <= 256.
-    padding=(pad_h, pad_w) other than (0, 0) zero-pads x as conv2d(padding=...) does (pcnn_conv_wide_plan_create_padded).
+    padding=(pad_h, pad_w) other than (0, 0) zero-pads x as conv2d(padding=...) does (pcnn_conv_wide_plan_create_padded);
+    dilation=(dil_h, dil_w) other than (1, 1) spaces the taps as conv2d(dilation=...) does (pcnn_conv_wide_plan_create_dilated).
     Run and closed like ConvPlan."""
 
-    def __init__(self, engine, N, H, W, C, K, R, S, filt, bias=None, act=0, row_pitch=None, image_rows=0, stride=1, padding=(0, 0)):
+    def __init__(self, engine, N, H, W, C, K, R, S, filt, bias=None, act=0, row_pitch=None, image_rows=0, stride=1, padding=(0, 0),
+                 dilation=(1, 1)):
         self.shape = (N, H, W, C, K, R, S)
         self.row_pitch = int(row_pitch if row_pitch is not None else (W * C + 7) // 8 * 8)
         ph, pw = (int(v) for v in padding)
-        pad = () if (ph, pw) == (0, 0) else (ph, pw)
-        self._create(engine, "pcnn_conv_wide_plan_create" + ("_padded" if pad else ""), filt, K * R * S * C, bias,
-                     N, H, W, C, K, R, S, int(stride), *pad, self.row_pitch, int(image_rows), int(act))
-        self.out_shape = (N, (H + 2 * ph - R) // stride + 1, (W + 2 * pw - S) // stride + 1, K)
+        dh, dw = (int(v) for v in dilation)
+        if (dh, dw) != (1, 1):
+            fn, extra = "pcnn_conv_wide_plan_create_dilated", (ph, pw, dh, dw)
+        elif (ph, pw) != (0, 0):
+            fn, extra = "pcnn_conv_wide_plan_create_padded", (ph, pw)
+        else:
+            fn, extra = "pcnn_conv_wide_plan_create", ()
+        self._create(engine, fn, filt, K * R * S * C, bias, N, H, W, C, K, R, S, int(stride), *extra, self.row_pitch, int(image_rows), int(act))
+        self.out_shape = (N, (H + 2 * ph - dh * (R - 1) - 1) // stride + 1, (W + 2 * pw - dw * (S - 1) - 1) // stride + 1, K)
 
 
 class LinearPlan(ConvPlan):
@@ -750,13 +768,19 @@ class LinearPlan(ConvPlan):
 class DepthwiseConvPlan(ConvPlan):
     """A depthwise convolution's plan (pcnn_dwconv_plan_create): conv2d(x, w, b, stride, padding, groups=C) with x dense bf16
     [N][H][W][C], y dense bf16 [N][P][Q][C], filters fp32 [C][R][S] (torch's weight [C][1][R][S] reshaped), bias fp32 [C].  act
-    ACT_NONE (0) or ACT_RELU (3).  Run, refreshed and closed like ConvPlan; its gradients are Engine.dwconv_wgrad / dwconv_dgrad."""
+    ACT_NONE (0) or ACT_RELU (3).  dilation=(dil_h, dil_w) other than (1, 1) is conv2d(dilation=...)
+    (pcnn_dwconv_plan_create_dilated).  Run, refreshed and closed like ConvPlan; its gradients are Engine.dwconv_wgrad / dwconv_dgrad."""
 
-    def __init__(self, engine, N, H, W, C, R, S, filt, bias=None, act=0, stride=1, padding=(0, 0)):
+    def __init__(self, engine, N, H, W, C, R, S, filt, bias=None, act=0, stride=1, padding=(0, 0), dilation=(1, 1)):
         self.shape = (N, H, W, C, R, S)
         ph, pw = (int(v) for v in padding)
-        self._create(engine, "pcnn_dwconv_plan_create", filt, C * R * S, bias, N, H, W, C, R, S, int(stride), ph, pw, int(act))
-        self.out_shape = (N, (H + 2 * ph - R) // stride + 1, (W + 2 * pw - S) // stride + 1, C)
+        dh, dw = (int(v) for v in dilation)
+        if (dh, dw) != (1, 1):
+            self._create(engine, "pcnn_dwconv_plan_create_dilated", filt, C * R * S, bias, N, H, W, C, R, S, int(stride), ph, pw, dh, dw,
+                         int(act))
+        else:
+            self._create(engine, "pcnn_dwconv_plan_create", filt, C * R * S, bias, N, H, W, C, R, S, int(stride), ph, pw, int(act))
+        self.out_shape = (N, (H + 2 * ph - dh * (R - 1) - 1) // stride + 1, (W + 2 * pw - dw * (S - 1) - 1) // stride + 1, C)
 
 
 class GroupedConvPlan(ConvPlan):
@@ -831,15 +855,18 @@ class ConvLayer(_PlanLayer):
     It owns fp32 master filters (KRSC) and bias, their gradients dw and db, all in DeviceArrays, and a forward plan of the family
     that serves the shape (conv_layer_family: the row-Toeplitz plan for few channels without padding, the wide plan otherwise).
     Activations are NHWC bf16: x with row_pitch (None = W*C rounded up to 8) and image_rows (0 = H), y and dy dense
-    [N][P][Q][K], dx in x's layout.  act ACT_SIGMOID (1) is a sigmoid after the bias, ACT_RELU (3) a ReLU, ACT_NONE (0) none."""
+    [N][P][Q][K], dx in x's layout.  act ACT_SIGMOID (1) is a sigmoid after the bias, ACT_RELU (3) a ReLU, ACT_NONE (0) none.
+    dilation=(dil_h, dil_w) spaces the taps as conv2d(dilation=...); a dilated layer is always the wide plan's (C % 8 == 0)."""
 
-    def __init__(self, engine, N, H, W, C, K, R, S, filt, bias=None, act=0, stride=1, padding=(0, 0), row_pitch=None, image_rows=0):
+    def __init__(self, engine, N, H, W, C, K, R, S, filt, bias=None, act=0, stride=1, padding=(0, 0), row_pitch=None, image_rows=0,
+                 dilation=(1, 1)):
         self.shape = (N, H, W, C, K, R, S)
         self.act, self.stride = int(act), int(stride)
         self.padding = tuple(int(v) for v in padding)
+        self.dilation = tuple(int(v) for v in dilation)
         self.row_pitch = int(row_pitch if row_pitch is not None else (W * C + 7) // 8 * 8)
         self.image_rows = int(image_rows)
-        self.family = conv_layer_family(N, H, W, C, K, R, S, self.stride, self.padding, self.row_pitch, self.image_rows)
+        self.family = conv_layer_family(N, H, W, C, K, R, S, self.stride, self.padding, self.row_pitch, self.image_rows, self.dilation)
         filt = np.ascontiguousarray(filt, np.float32).reshape(K, R, S, C)
         bias = None if bias is None else np.ascontiguousarray(bias, np.float32).reshape(K)
         if self.family == "narrow":
@@ -847,7 +874,7 @@ class ConvLayer(_PlanLayer):
                             stride=self.stride)
         else:
             plan = WideConvPlan(engine, N, H, W, C, K, R, S, filt, bias, act=act, row_pitch=self.row_pitch, image_rows=self.image_rows,
-                                stride=self.stride, padding=self.padding)
+                                stride=self.stride, padding=self.padding, dilation=self.dilation)
         self._own(engine, plan, filt, bias)
 
     def _grads(self, dy, dx):
@@ -858,9 +885,11 @@ class ConvLayer(_PlanLayer):
             if dx is not None:
                 e.conv_dgrad(dy, self.filt, dx, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride)
         else:
-            e.conv_wide_wgrad(self._x, dy, self.dw, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride, self.padding)
+            e.conv_wide_wgrad(self._x, dy, self.dw, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride, self.padding,
+                              self.dilation)
             if dx is not None:
-                e.conv_wide_dgrad(dy, self.filt, dx, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride, self.padding)
+                e.conv_wide_dgrad(dy, self.filt, dx, N, H, W, C, K, R, S, self.row_pitch, self.image_rows, self.stride, self.padding,
+                                  self.dilation)
 
 
 class ConvTransposeLayer(_PlanLayer):
@@ -983,14 +1012,16 @@ class DepthwiseConvLayer(_PlanLayer):
     (the usual case in front of a batch norm) C is unlimited.  dx uses the plan's bf16 filters, so call backward before sgd or an
     optimizer step."""
 
-    def __init__(self, engine, N, H, W, C, R, S, filt, bias=None, act=0, stride=1, padding=(0, 0)):
+    def __init__(self, engine, N, H, W, C, R, S, filt, bias=None, act=0, stride=1, padding=(0, 0), dilation=(1, 1)):
         self.shape = (N, H, W, C, R, S)
         self.act, self.stride = int(act), int(stride)
         self.padding = tuple(int(v) for v in padding)
-        self.info = dwconv_info(N, H, W, C, R, S, self.stride, self.padding)
+        self.dilation = tuple(int(v) for v in dilation)
+        self.info = dwconv_info(N, H, W, C, R, S, self.stride, self.padding, self.dilation)
         filt = np.ascontiguousarray(filt, np.float32).reshape(C, R, S)
         bias = None if bias is None else np.ascontiguousarray(bias, np.float32).reshape(C)
-        plan = DepthwiseConvPlan(engine, N, H, W, C, R, S, filt, bias, act=act, stride=self.stride, padding=self.padding)
+        plan = DepthwiseConvPlan(engine, N, H, W, C, R, S, filt, bias, act=act, stride=self.stride, padding=self.padding,
+                                 dilation=self.dilation)
         self._own(engine, plan, filt, bias)
 
     def _grads(self, dy, dx):

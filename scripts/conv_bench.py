@@ -208,6 +208,143 @@ def run_fcn(iters):
     net.close()
 
 
+def run_dilated(name, N, H, W, C, K, R, dil, iters):
+    """the three wide passes of a "same" 3x3 layer at dilation dil (padding dil), next to cuDNN (conv2d(dilation=dil) and
+    aten.convolution_backward) on the same bf16 channels-last tensors and to the same layer at dilation 1 (padding 1), all in this
+    run.  Bound: bytes = N * (H*W*C + P*Q*K) * 2, flops = 2 * N * P*Q*K * R*R*C, as run_wide_same."""
+    pad = dil * (R - 1) // 2
+    f = rng.uniform(-0.5, 0.5, (K, R, R, C)).astype(np.float32)
+    b = rng.uniform(-0.5, 0.5, K).astype(np.float32)
+    plans = {d: pkg.WideConvPlan(eng, N, H, W, C, K, R, R, f, b, padding=(d * (R - 1) // 2,) * 2, dilation=(d, d)) for d in {1, dil}}
+    P, Q = plans[dil].out_shape[1:3]
+    x = torch.randint(0, 0x3F80, (N, H, W, C), dtype=torch.int16, device="cuda")
+    y = torch.empty((N, P, Q, K), dtype=torch.int16, device="cuda")
+    dy = torch.randint(0, 0x3F80, (N, P, Q, K), dtype=torch.int16, device="cuda")
+    dy ^= (torch.randint(0, 2, (N, P, Q, K), dtype=torch.int16, device="cuda") << 15)
+    fd = torch.from_numpy(f).to("cuda")
+    dw = torch.empty((K, R, R, C), dtype=torch.float32, device="cuda")
+    dx = torch.empty((N, H, W, C), dtype=torch.int16, device="cuda")
+    xt, dyt = x.view(torch.bfloat16).permute(0, 3, 1, 2), dy.view(torch.bfloat16).permute(0, 3, 1, 2)
+    wt = fd.permute(0, 3, 1, 2).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+    bt = torch.from_numpy(b).to("cuda", torch.bfloat16)
+    alg = N * (H * W * C + P * Q * K) * 2
+    flops = 2.0 * N * P * Q * K * R * R * C
+    t_bound = max(flops / 989e12, alg / 3.35e12)
+    gpu, power = card()
+    cb = torch.ops.aten.convolution_backward
+
+    def passes(d):
+        pd = d * (R - 1) // 2
+        return (("fwd", lambda: plans[d].fwd(x, y), lambda: torch.nn.functional.conv2d(xt, wt, bt, 1, pd, d)),
+                ("wgrad", lambda: eng.conv_wide_wgrad(x, dy, dw, N, H, W, C, K, R, R, padding=(pd, pd), dilation=(d, d)),
+                 lambda: cb(dyt, xt, wt, None, [1, 1], [pd, pd], [d, d], False, [0, 0], 1, [False, True, False])),
+                ("dgrad", lambda: eng.conv_wide_dgrad(dy, fd, dx, N, H, W, C, K, R, R, padding=(pd, pd), dilation=(d, d)),
+                 lambda: cb(dyt, xt, wt, None, [1, 1], [pd, pd], [d, d], False, [0, 0], 1, [True, False, False])))
+
+    for (what, ours, theirs), (_, ours1, theirs1) in zip(passes(dil), passes(1)):
+        ms, ms_cudnn, ms1, ms1_cudnn = timed(ours, iters), timed(theirs, iters), timed(ours1, iters), timed(theirs1, iters)
+        print(json.dumps({"case": f"dilated {name} d{dil} {what}", "N": N, "ms": ms, "bound_frac": t_bound / (ms * 1e-3),
+                          "cudnn_ms": ms_cudnn, "cudnn_over_ours": ms_cudnn / ms, "d1_ms": ms1, "ours_over_d1": ms / ms1,
+                          "cudnn_d1_ms": ms1_cudnn, "gpu": gpu, "power_limit": power}), flush=True)
+    for p in plans.values():
+        p.close()
+
+
+def run_dwdilated(name, N, H, W, C, R, dil, iters):
+    """the three passes of a "same" depthwise layer at dilation dil next to torch's conv2d(groups=C, dilation=dil) and
+    aten.convolution_backward on the same bf16 channels-last tensors, and to the same layer at dilation 1 (bytes as run_dwconv)"""
+    w = rng.uniform(-0.5, 0.5, (C, R, R)).astype(np.float32)
+    plans = {d: pkg.DepthwiseConvPlan(eng, N, H, W, C, R, R, w, None, padding=(d * (R - 1) // 2,) * 2, dilation=(d, d)) for d in {1, dil}}
+    bits = lambda *shape: torch.randint(0, 0x3F80, shape, dtype=torch.int16, device="cuda")
+    x, dy = bits(N, H, W, C), bits(N, H, W, C)
+    y, dx = torch.empty((N, H, W, C), dtype=torch.int16, device="cuda"), torch.empty((N, H, W, C), dtype=torch.int16, device="cuda")
+    dw = torch.empty((C, R, R), dtype=torch.float32, device="cuda")
+    xt, dyt = x.view(torch.bfloat16).permute(0, 3, 1, 2), dy.view(torch.bfloat16).permute(0, 3, 1, 2)
+    wt = torch.from_numpy(w).to("cuda").to(torch.bfloat16)[:, None].contiguous(memory_format=torch.channels_last)
+    cb = torch.ops.aten.convolution_backward
+    nbytes = N * 2 * H * W * C * 2
+    gpu, power = card()
+
+    def passes(d):
+        pd = d * (R - 1) // 2
+        return (("fwd", lambda: plans[d].fwd(x, y), lambda: torch.nn.functional.conv2d(xt, wt, None, 1, pd, d, groups=C)),
+                ("dgrad", lambda: eng.dwconv_dgrad(plans[d], dy, dx),
+                 lambda: cb(dyt, xt, wt, None, [1, 1], [pd, pd], [d, d], False, [0, 0], C, [True, False, False])),
+                ("wgrad", lambda: eng.dwconv_wgrad(plans[d], x, dy, dw),
+                 lambda: cb(dyt, xt, wt, None, [1, 1], [pd, pd], [d, d], False, [0, 0], C, [False, True, False])))
+
+    for (what, ours, theirs), (_, ours1, _) in zip(passes(dil), passes(1)):
+        ms, ms_torch, ms1 = timed(ours, iters), timed(theirs, iters), timed(ours1, iters)
+        print(json.dumps({"case": f"dwdilated {name} d{dil} {what}", "N": N, "us": ms * 1e3, "share_of_3350": nbytes / (ms * 1e-3) / 1e9 / HBM,
+                          "torch_us": ms_torch * 1e3, "torch_over_ours": ms_torch / ms, "d1_us": ms1 * 1e3, "ours_over_d1": ms / ms1,
+                          "gpu": gpu, "power_limit": power}), flush=True)
+    for p in plans.values():
+        p.close()
+
+
+def run_deeplab(iters):
+    """one DeepLabLite training step (forward, backward, SGD with momentum) at N = 32, and the same network in torch eager: bf16
+    channels-last convolutions (cuDNN) with batch norm in float32, on one fixed batch"""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import deeplab_nets
+    import segment_ref
+    d = np.load(os.path.join(ROOT, "tests", "golden", "mnist_subset.npz"))
+    cls = deeplab_nets.DeepLabLite
+    p = cls.init_params()
+    net = cls(eng, pkg, p)
+    opt = pkg.SGD(eng, net.layers(), momentum=0.9)
+    b = pkg.ImageBatcher(eng, d["train_u8"].reshape(-1, 28, 28), d["train_labels"], cls.NB, pad=2, flip=True, C_out=8,
+                         masks=segment_ref.digit_masks(d["train_u8"], d["train_labels"]))
+    batch = b.batch(0)
+
+    def step():
+        net.forward(*batch)
+        net.backward()
+        opt.step(cls.LR)
+    ms = timed(step, iters)
+
+    F = torch.nn.functional
+    cl = torch.channels_last
+    w = {}
+    for k, v in p.items():
+        t = torch.from_numpy(v).to("cuda")
+        if k == "wc":
+            t = t.reshape(32, 1, 3, 3)
+        elif k.startswith("f"):
+            t = t.permute(0, 3, 1, 2)
+        elif k == "w":
+            t = t.reshape(t.shape[0], -1)
+        w[k] = t.to(torch.bfloat16).contiguous(memory_format=cl if t.dim() == 4 else torch.contiguous_format).requires_grad_(True)
+    bns = [torch.nn.BatchNorm2d(c).cuda().to(memory_format=cl) for c in (16, 32, 32, 32, 32, 32, 32)]
+    bn = lambda i, v: bns[i](v.float()).to(torch.bfloat16)
+    params = list(w.values()) + [q for m in bns for q in m.parameters()]
+    topt = torch.optim.SGD(params, lr=cls.LR, momentum=0.9)
+    x = torch.randn(cls.NB, 8, 28, 28, device="cuda").to(torch.bfloat16).contiguous(memory_format=cl)
+    tgt = torch.randint(0, 11, (cls.NB, 28, 28), device="cuda")
+
+    def tstep():
+        a = F.relu(bn(0, F.conv2d(x, w["f1"], padding=1)))
+        bb = F.relu(bn(1, F.conv2d(a, w["f2"], padding=1, stride=2)))
+        m = F.relu(bn(2, F.conv2d(bb, w["fd1"], padding=2, dilation=2)))
+        h = F.relu(bn(3, F.conv2d(m, w["fd2"], padding=2, dilation=2)) + bb)
+        sa = bn(4, F.conv2d(m, w["fa"]))
+        sb = bn(5, F.conv2d(h, w["fb"], padding=4, dilation=4)) + sa
+        out = F.relu(bn(6, F.conv2d(F.conv2d(h, w["wc"], padding=6, dilation=6, groups=32), w["fp"])) + sb)
+        z14 = torch.einsum("nchw,oc->nohw", out, w["w"]) + w["bw"][None, :, None, None]
+        z = F.interpolate(z14, size=(28, 28), mode="bilinear", align_corners=False)
+        loss = F.cross_entropy(z.float(), tgt, ignore_index=255)
+        topt.zero_grad(set_to_none=True)
+        loss.backward()
+        topt.step()
+    ms_torch = timed(tstep, iters)
+    gpu, power = card()
+    print(json.dumps({"case": f"DeepLabLite training step N={cls.NB}", "us": ms * 1e3, "torch_eager_us": ms_torch * 1e3,
+                      "torch_over_ours": ms_torch / ms, "gpu": gpu, "power_limit": power}), flush=True)
+    b.close()
+    opt.close()
+    net.close()
+
+
 def run_wide(name, N, H, W, C, K, R, S, stride, iters):
     """the wide-channel forward (WideConvPlan) next to torch.nn.functional.conv2d (cuDNN) on the same bf16 channels-last tensors.
     Bound: the larger of flops / 989 TFLOP/s (H100 SXM dense bf16) and bytes / 3.35 TB/s, bytes = N * (H*W*C + P*Q*K) * 2."""
@@ -2001,6 +2138,19 @@ if only == "segce":                                                    # VOC-siz
     run_segce(16, 21, 20)
 if only == "fcn":
     run_fcn(20)
+if only == "dilated":                                                  # dilated wide passes vs cuDNN and vs dilation 1
+    for d in (1, 2):
+        run_dilated("56x56x64->64 3x3", 128, 56, 56, 64, 64, 3, d, 20)
+    for d in (1, 2, 4):
+        run_dilated("28x28x128->128 3x3", 256, 28, 28, 128, 128, 3, d, 20)
+    for d in (6, 12, 18):                                              # ASPP; N 96 gives every pass more than 2 x stages tiles per CTA
+        run_dilated("ASPP 33x33x512->256 3x3", 96, 33, 33, 512, 256, 3, d, 20)
+if only == "dwdilated":                                                # dilated depthwise passes vs torch and vs dilation 1
+    for d in (1, 2):
+        run_dwdilated("56x56x144 3x3", 128, 56, 56, 144, 3, d, 20)
+        run_dwdilated("28x28x240 5x5", 128, 28, 28, 240, 5, d, 20)
+if only == "deeplab":
+    run_deeplab(20)
 eng.close()
 if only == "wprobe":                                                   # what a pure WRITE stream / pure READ stream / copy reach on this GPU
     # library fill / reduce / copy kernels as a yardstick for the store-dominated forward pass (807 MB written, 39 MB read):
