@@ -287,8 +287,9 @@ int pcnn_l5_forward(pcnn_ctx *ctx, const float *params_dev, const void *images_d
 #define PCNN_ACT_NONE 0
 #define PCNN_ACT_SIGMOID 1
 #define PCNN_ACT_RELU 3
-/* Codes 4-6 are taken by pcnn_batchnorm_nhwc_bf16_fwd and pcnn_batchnorm_nhwc_bf16_bwd_preact only (every call above and below
- * keeps its domain and refuses them); batch normalization below states their formulas. */
+/* Codes 4-6 are taken by pcnn_batchnorm_nhwc_bf16_fwd and pcnn_batchnorm_nhwc_bf16_bwd_preact, and by group normalization's
+ * forward and pre-activation backward, only (every other call above and below keeps its domain and refuses them); batch
+ * normalization below states their formulas. */
 #define PCNN_ACT_SILU 4
 #define PCNN_ACT_HARDSWISH 5
 #define PCNN_ACT_RELU6 6
@@ -627,6 +628,62 @@ int pcnn_batchnorm_nhwc_bf16_bwd_preact(pcnn_ctx *ctx, const void *x_bf16_dev, c
                                         const float *save_rstd_dev, void *dx_bf16_dev, void *dr_bf16_dev, float *dgamma_dev,
                                         float *dbeta_dev, long pixels, int C, int act);
 int pcnn_batchnorm_nhwc_info(long pixels, int C, int training, int *out5);
+/* Group normalization between convolution layers (csrc/groupnorm_nhwc.cu), as torch.nn.functional.group_norm(x, G, gamma, beta,
+ * eps), followed by batch normalization's optional residual add and activation.  x, r, y, dy, dy2, dx and dr are dense bf16
+ * [N][HW][C] (the layout both conv forwards write as y); gamma, beta, dgamma and dbeta are fp32 [C]; save_mean and save_rstd are
+ * fp32 [N][G]; dstat is fp32 [2][N][G].  Cg = C / G; group g of image n is the channels [g Cg, (g + 1) Cg) over all HW pixels,
+ * Mg = HW Cg elements, Mgf = float(Mg).  With G = C this is instance normalization with affine parameters, with G = 1 layer
+ * normalization over (C, H, W) with per-channel parameters.  There are no running statistics: training and evaluation compute the
+ * same y.  Every fp32 operation below rounds to nearest with no contraction.
+ * Forward:
+ *   - mean and the biased variance var of float(x) over each (n, g), accumulated so that a mean large next to the spread does not
+ *     cancel (fp32 sums of x - k per image, channel and pixel range, k the range's first pixel of that channel, merged in double
+ *     in a fixed order; not E[x^2] - E[x]^2): save_mean = float(mean), save_rstd = float(1 / sqrt(var + double(eps))) in double;
+ *   - per element, with mean and rstd those of the element's (n, g): xhat = (float(x) - mean) * rstd;  v = xhat * gamma[c] +
+ *     beta[c];  v = v + float(r) when r is given;  y = bf16_rn(act(v)), act 0, 3, 4, 5 or 6 exactly as in
+ *     pcnn_batchnorm_nhwc_bf16_fwd (act 1 is refused for the reason given there).
+ * Backward at codes 0 and 3 (pcnn_groupnorm_nhwc_bf16_bwd, of a forward whose save_mean and save_rstd it wrote and whose output was
+ * y) and at codes 4-6 (pcnn_groupnorm_nhwc_bf16_bwd_preact, which recomputes v from x, the saved statistics, gamma, beta and r as
+ * the forward formed it; r must be the forward's r, unchanged, or NULL if it had none).  Each entry refuses the other's codes.
+ *   t and g = bf16_rn(act'(t)) are batch normalization's, per element;
+ *   dbeta[c] = sum of float(g), dgamma[c] = sum of float(g) * xhat, each over all N HW pixels (fp32 per-CTA partials over pixel
+ *     ranges, then a fixed-order pass over them);
+ *   A[n][g] = sum of gamma[c] * float(g), B[n][g] = sum of gamma[c] * float(g) * xhat, each over the Mg elements of the group: the
+ *     per-channel fp32 partials of the pixel ranges times gamma[c], added in double in a fixed order, then rounded to float and
+ *     written to dstat[0][n][g] and dstat[1][n][g];
+ *   dx = bf16_rn(RN(RN(RN(RN(float(g) * gamma[c]) - a) - RN(xhat * b)) * rstd)), a = RN(A / Mgf) and b = RN(B / Mgf) formed once
+ *     per (n, g) from the dstat just written, so dx is a stated function of x, g, the saved statistics, gamma and dstat;
+ *   dr = g when dr is given: the gradient of the residual input r.
+ * Partition: the pixel ranges of an image (of `pixels per range` each) and the channel slices (at most 256 channels) depend on
+ * (HW, C, G) alone, never on N.  So an image's y, save_mean, save_rstd, dstat, dx and dr are bit-identical whether it runs alone
+ * or at any position of any batch; dgamma and dbeta, sums over the batch, are not.
+ * dx == dy (in place) is allowed; no other two buffers may overlap.  Domain (anything else is PCNN_ERR_ARG with the function and
+ * the rule in the message; the shape rules read the same in pcnn_groupnorm_nhwc_info):
+ *   - N >= 1; HW >= 1; 1 <= C <= 2048; 1 <= G <= C with C % G == 0; N * ranges * slices < 2^31 CTAs;
+ *   - eps finite and >= 0; act 0, 3, 4, 5 or 6 in the forward, 0 or 3 in pcnn_groupnorm_nhwc_bf16_bwd, 4, 5 or 6 in
+ *     pcnn_groupnorm_nhwc_bf16_bwd_preact;
+ *   - every pointer 16-byte aligned; only r may be NULL in the forward; only dy2 and dr in pcnn_groupnorm_nhwc_bf16_bwd (dstat
+ *     is required); only r, dy2 and dr in pcnn_groupnorm_nhwc_bf16_bwd_preact (beta and dstat are required).
+ * With C % 8 == 0 the passes move 16-byte vectors of 8 channels (which may span several groups when Cg < 8), otherwise single
+ * elements.  No atomics: reruns and every H100 give the same bits.  Elements past N HW C are never written.  All calls are
+ * stream-ordered and use the context's one scratch block for their per-CTA partials.
+ * pcnn_groupnorm_nhwc_info: host only (no GPU, no context).  out11 = { channels per thread (8 or 1), channel groups of that width
+ * per CTA, channel slices, pixel lanes per CTA, pixels per range, ranges per image, CTAs of each elementwise pass (N x ranges x
+ * slices: the statistics, y, the gradient sums and dx), slots per channel (N x ranges), CTAs of the two per-(n, g) merges (8 pairs
+ * each), n_acc of dgamma and dbeta, n_acc of A, B and the statistics }.  n_acc is the number of fp32 roundings on the longest
+ * path of one sum: a bound of 2 n_acc 2^-24 sum |terms| holds. */
+int pcnn_groupnorm_nhwc_bf16_fwd(pcnn_ctx *ctx, const void *x_bf16_dev, const void *r_bf16_dev, void *y_bf16_dev, int N, int HW, int C,
+                                 int G, int act, float eps, const float *gamma_dev, const float *beta_dev, float *save_mean_dev,
+                                 float *save_rstd_dev);
+int pcnn_groupnorm_nhwc_bf16_bwd(pcnn_ctx *ctx, const void *x_bf16_dev, const void *y_bf16_dev, const void *dy_bf16_dev,
+                                 const void *dy2_bf16_dev, const float *gamma_dev, const float *save_mean_dev, const float *save_rstd_dev,
+                                 void *dx_bf16_dev, void *dr_bf16_dev, float *dgamma_dev, float *dbeta_dev, float *dstat_dev, int N, int HW,
+                                 int C, int G, int act);
+int pcnn_groupnorm_nhwc_bf16_bwd_preact(pcnn_ctx *ctx, const void *x_bf16_dev, const void *r_bf16_dev, const void *dy_bf16_dev,
+                                        const void *dy2_bf16_dev, const float *gamma_dev, const float *beta_dev, const float *save_mean_dev,
+                                        const float *save_rstd_dev, void *dx_bf16_dev, void *dr_bf16_dev, float *dgamma_dev,
+                                        float *dbeta_dev, float *dstat_dev, int N, int HW, int C, int G, int act);
+int pcnn_groupnorm_nhwc_info(int N, int HW, int C, int G, int *out11);
 /* Fully connected layers (csrc/linear_tc.cu), bf16 on the tensor cores with fp32 accumulation:
  *   - x is [N][image_rows][row_pitch] bf16 with P x Q pixels of C channels per image: the layout a plan reads as x and the NHWC
  *     pool writes as y.  A previous linear layer's y is the same with P = Q = 1, C = its O, row_pitch = O, image_rows 1.

@@ -16,7 +16,7 @@ U8, F32 = 0, 1
 MODE_AUTO, MODE_GRAPH, MODE_PERSISTENT = 0, 1, 2
 TRAIN_SET, TEST_SET = 0, 1
 ACT_NONE, ACT_SIGMOID, ACT_RELU = 0, 1, 3     # PCNN_ACT_*: the `act` of the device-trained layers (2 is not a code)
-ACT_SILU, ACT_HARDSWISH, ACT_RELU6 = 4, 5, 6  # taken by batch normalization only (BatchNormLayer, Engine.batchnorm_fwd / _bwd_preact)
+ACT_SILU, ACT_HARDSWISH, ACT_RELU6 = 4, 5, 6  # taken by the normalizations only (BatchNormLayer, GroupNormLayer and their Engine calls)
 OPTIM_SGD, OPTIM_ADAMW = 0, 1                 # PCNN_OPTIM_*: the `kind` of pcnn_optim_config
 
 
@@ -161,6 +161,10 @@ _SIG = {
     "pcnn_batchnorm_nhwc_bf16_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _l, _i, _i],
     "pcnn_batchnorm_nhwc_bf16_bwd_preact": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _l, _i, _i],
     "pcnn_batchnorm_nhwc_info": [_l, _i, _i, _vp],
+    "pcnn_groupnorm_nhwc_bf16_fwd": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp, _vp, _vp],
+    "pcnn_groupnorm_nhwc_bf16_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i],
+    "pcnn_groupnorm_nhwc_bf16_bwd_preact": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i],
+    "pcnn_groupnorm_nhwc_info": [_i, _i, _i, _i, _vp],
     "pcnn_conv_bwd_plan_info": [_i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_pad_nhwc_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i],
     "pcnn_crop_nhwc_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i],
@@ -404,6 +408,18 @@ def batchnorm_nhwc_info(pixels, C, training=True):
     out = (_i * 5)()
     check("pcnn_batchnorm_nhwc_info", lib().pcnn_batchnorm_nhwc_info(int(pixels), int(C), 1 if training else 0, out))
     return dict(vec=out[0], lanes=out[1], pixels_per_cta=out[2], stat_slots=out[3], grad_slots=out[4])
+
+
+def groupnorm_nhwc_info(N, HW, C, G):
+    """How group normalization partitions dense [N][HW][C] activations in G groups (pcnn_groupnorm_nhwc_info; host only, no GPU),
+    refused as the entry points refuse.  vec: channels per thread (8 or 1); the C / vec channel groups are cut into `slices` of
+    `groups_per_cta`, each image's HW pixels into `ranges` of `pixels_per_range` (both a function of (HW, C, G) alone); ctas: the
+    grid of every elementwise pass; slots: per-CTA partials per channel (N * ranges); group_ctas: the grid of the per-(n, g) merges;
+    n_acc (dgamma, dbeta) and n_acc_group (A, B, the statistics): fp32 roundings on the longest path of one sum."""
+    out = (_i * 11)()
+    check("pcnn_groupnorm_nhwc_info", lib().pcnn_groupnorm_nhwc_info(int(N), int(HW), int(C), int(G), out))
+    return dict(vec=out[0], groups_per_cta=out[1], slices=out[2], lanes=out[3], pixels_per_range=out[4], ranges=out[5], ctas=out[6],
+                slots=out[7], group_ctas=out[8], n_acc=out[9], n_acc_group=out[10])
 
 
 def linear_info(N, P, Q, C, O, row_pitch=0, image_rows=0):

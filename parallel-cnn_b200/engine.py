@@ -8,11 +8,11 @@ import numpy as np
 
 from ._lib import (F32, NPARAM, OPTIM_ADAMW, OPTIM_SGD, TEST_SET, TRAIN_SET, U8, OptimConfig, OptimTensor, PcnnError, augment_info,
                    augment_resized_info, RESIZE_TRAIN, RESIZE_EVAL, augment_trivial_info, TRIVIAL_NONE, TRIVIAL_NEAREST, TRIVIAL_BILINEAR,
-                   avgpool_nhwc_info, batchnorm_nhwc_info, channel_stats, check, conv_layer_family, conv_transpose_info, upsample_bilinear_info, dropout_info, dwconv_info, gconv_info, global_avgpool_nhwc_info, lib, linear_info,
-                   maxpool_nhwc_info,
+                   avgpool_nhwc_info, batchnorm_nhwc_info, channel_stats, check, conv_layer_family, conv_transpose_info, upsample_bilinear_info, dropout_info, dwconv_info, gconv_info, global_avgpool_nhwc_info, groupnorm_nhwc_info, lib,
+                   linear_info, maxpool_nhwc_info,
                    se_scale_nhwc_info, ACT_RELU, ACT_SIGMOID, ACT_SILU, ACT_HARDSWISH, ACT_RELU6)
 
-PREACT_CODES = (ACT_SILU, ACT_HARDSWISH, ACT_RELU6)   # batch normalization's codes whose backward recomputes the pre-activation
+PREACT_CODES = (ACT_SILU, ACT_HARDSWISH, ACT_RELU6)   # the normalizations' codes whose backward recomputes the pre-activation
 MIX_MIXUP, MIX_CUTMIX = 1, 2                         # pcnn_augment_mix_u8_bf16's modes
 
 
@@ -494,6 +494,27 @@ class Engine:
         forward's r, unchanged, or None if it had none) instead of from y"""
         self._call("pcnn_batchnorm_nhwc_bf16_bwd_preact", _p(x), _p(r), _p(dy), _p(dy2), _p(gamma), _p(beta), _p(save_mean), _p(save_rstd),
                    _p(dx), _p(dr), _p(dgamma), _p(dbeta), int(pixels), int(C), int(act))
+
+    def groupnorm_fwd(self, x, y, N, HW, C, G, gamma, beta, save_mean, save_rstd, r=None, act=0, eps=1e-5):
+        """pcnn_groupnorm_nhwc_bf16_fwd: y = bf16(act((x - mean) * rstd * gamma + beta (+ r))) over dense bf16 [N][HW][C], mean and
+        rstd those of each (image, group of C / G channels), written to save_mean / save_rstd [N][G].  act ACT_NONE, ACT_RELU,
+        ACT_SILU, ACT_HARDSWISH or ACT_RELU6"""
+        self._call("pcnn_groupnorm_nhwc_bf16_fwd", _p(x), _p(r), _p(y), int(N), int(HW), int(C), int(G), int(act), float(eps), _p(gamma),
+                   _p(beta), _p(save_mean), _p(save_rstd))
+
+    def groupnorm_bwd(self, x, y, dy, gamma, save_mean, save_rstd, dx, dgamma, dbeta, dstat, N, HW, C, G, act=0, dy2=None, dr=None):
+        """pcnn_groupnorm_nhwc_bf16_bwd at ACT_NONE or ACT_RELU: g = bf16(act'(dy (+ dy2))), dbeta = sum g, dgamma = sum g * xhat over
+        the batch, dstat [2][N][G] = the group sums A = sum gamma * g and B = sum gamma * g * xhat, dx (may be dy itself) and, when
+        given, dr = g"""
+        self._call("pcnn_groupnorm_nhwc_bf16_bwd", _p(x), _p(y), _p(dy), _p(dy2), _p(gamma), _p(save_mean), _p(save_rstd), _p(dx), _p(dr),
+                   _p(dgamma), _p(dbeta), _p(dstat), int(N), int(HW), int(C), int(G), int(act))
+
+    def groupnorm_bwd_preact(self, x, dy, gamma, beta, save_mean, save_rstd, dx, dgamma, dbeta, dstat, N, HW, C, G, act, r=None, dy2=None,
+                             dr=None):
+        """pcnn_groupnorm_nhwc_bf16_bwd_preact at ACT_SILU, ACT_HARDSWISH or ACT_RELU6: as groupnorm_bwd, with g taken at the
+        pre-activation recomputed from x, the saved statistics, gamma, beta and r (the forward's r, unchanged, or None)"""
+        self._call("pcnn_groupnorm_nhwc_bf16_bwd_preact", _p(x), _p(r), _p(dy), _p(dy2), _p(gamma), _p(beta), _p(save_mean), _p(save_rstd),
+                   _p(dx), _p(dr), _p(dgamma), _p(dbeta), _p(dstat), int(N), int(HW), int(C), int(G), int(act))
 
     def pad_nhwc(self, src_bf16, dst_bf16, N, H, W, Cin, pad_h, pad_w, dst_row_pitch=0, dst_image_rows=0):
         self._call("pcnn_pad_nhwc_bf16", _p(src_bf16), _p(dst_bf16), N, H, W, Cin, int(pad_h), int(pad_w), int(dst_row_pitch), int(dst_image_rows))
@@ -1141,6 +1162,72 @@ class BatchNormLayer:
             a.free()
 
 
+class GroupNormLayer:
+    """Group normalization trained on the device (pcnn_groupnorm_nhwc_bf16_fwd / _bwd / _bwd_preact), as torch's GroupNorm with
+    affine parameters, with BatchNormLayer's residual add and activations after it.  The statistics are those of each image's
+    groups of C / groups channels, so one image's output never depends on another's, and there are no running statistics:
+    forward takes no training flag.  It owns fp32 gamma (default ones) and beta (default zeros), their gradients dgamma and dbeta,
+    the saved mean and rstd [N][groups] of the last forward and the group sums dstat [2][N][groups] of the last backward, all in
+    DeviceArrays.
+
+    x, r, y, dy, dy2, dx and dr are dense bf16 [N][H][W][C], as for a BatchNormLayer, which this layer replaces where a batch
+    holds few images (segmentation, detection heads).  At ACT_SILU, ACT_HARDSWISH and ACT_RELU6 the backward works from the
+    pre-activation recomputed from x and r, so at those codes the layer keeps r as well as x."""
+
+    def __init__(self, engine, N, H, W, C, groups, act=0, eps=1e-5, gamma=None, beta=None):
+        self.engine = engine
+        self.shape = (N, H, W, C)
+        self.groups, self.HW = int(groups), int(H) * int(W)
+        self.act, self.eps = int(act), float(eps)
+        self.info = groupnorm_nhwc_info(N, self.HW, C, self.groups)
+        g = np.ones(C, np.float32) if gamma is None else np.ascontiguousarray(gamma, np.float32).reshape(C)
+        b = np.zeros(C, np.float32) if beta is None else np.ascontiguousarray(beta, np.float32).reshape(C)
+        self.gamma, self.beta = DeviceArray.from_host(engine, g), DeviceArray.from_host(engine, b)
+        self.dgamma, self.dbeta = engine.array(C), engine.array(C)
+        self.save_mean, self.save_rstd = engine.array(N * self.groups), engine.array(N * self.groups)
+        self.dstat = engine.array(2 * N * self.groups)
+        self._x = self._r = None
+
+    def forward(self, x, y, r=None):
+        """y = act(gn(x) + r), the statistics saved for backward.  The layer keeps x (and r at ACT_SILU, ACT_HARDSWISH and
+        ACT_RELU6): backward reads them, so they must stay unchanged until then."""
+        N, H, W, C = self.shape
+        self.engine.groupnorm_fwd(x, y, N, self.HW, C, self.groups, self.gamma, self.beta, self.save_mean, self.save_rstd, r=r,
+                                  act=self.act, eps=self.eps)
+        self._x = x
+        self._r = r if self.act in PREACT_CODES else None
+
+    def backward(self, y, dy, dx, dr=None, dy2=None):
+        """Gradients of the most recent forward, whose output y was: dgamma, dbeta, dstat and dx (dx may be dy).  dy2 is a second
+        gradient added to dy before the activation; dr receives the gradient of the forward's r.  At ACT_SILU, ACT_HARDSWISH and
+        ACT_RELU6 y is not read (Engine.groupnorm_bwd_preact)."""
+        N, H, W, C = self.shape
+        if self.act in PREACT_CODES:
+            self.engine.groupnorm_bwd_preact(self._x, dy, self.gamma, self.beta, self.save_mean, self.save_rstd, dx, self.dgamma,
+                                             self.dbeta, self.dstat, N, self.HW, C, self.groups, self.act, r=self._r, dy2=dy2, dr=dr)
+            return
+        self.engine.groupnorm_bwd(self._x, y, dy, self.gamma, self.save_mean, self.save_rstd, dx, self.dgamma, self.dbeta, self.dstat, N,
+                                  self.HW, C, self.groups, act=self.act, dy2=dy2, dr=dr)
+
+    def sgd(self, lr):
+        """gamma += (-lr) * dgamma and beta += (-lr) * dbeta in fp32, on the engine's stream"""
+        C = self.shape[3]
+        self.engine.apply_grad_scaled(self.gamma, self.dgamma, C, -lr)
+        self.engine.apply_grad_scaled(self.beta, self.dbeta, C, -lr)
+
+    def optim_tensors(self):
+        """(param, grad, plan, plan part, is norm or bias) of gamma and beta, as BatchNormLayer.optim_tensors"""
+        return [(self.gamma, self.dgamma, None, 0, True), (self.beta, self.dbeta, None, 0, True)]
+
+    def params(self):
+        """host copies of gamma and beta"""
+        return self.gamma.to_host(), self.beta.to_host()
+
+    def close(self):
+        for a in (self.gamma, self.beta, self.dgamma, self.dbeta, self.save_mean, self.save_rstd, self.dstat):
+            a.free()
+
+
 class LinearLayer(_PlanLayer):
     """A fully connected layer trained on the device, with ConvLayer's interface: fp32 masters w [O][P][Q][C] and bias [O], their
     gradients dw and db, and a LinearPlan holding w in bf16.
@@ -1669,4 +1756,4 @@ def bf16_bits_to_f32(b):
 
 
 C_ = C
-__all__ = ["Engine", "DeviceArray", "ConvPlan", "WideConvPlan", "LinearPlan", "ConvLayer", "LinearLayer", "MaxPoolLayer", "AvgPoolLayer", "GlobalAvgPoolLayer", "BatchNormLayer", "FusedOptimizer", "SGD", "AdamW", "f32_to_bf16_bits", "bf16_bits_to_f32", "TRAIN_SET", "TEST_SET", "U8", "F32"]
+__all__ = ["Engine", "DeviceArray", "ConvPlan", "WideConvPlan", "LinearPlan", "ConvLayer", "LinearLayer", "MaxPoolLayer", "AvgPoolLayer", "GlobalAvgPoolLayer", "BatchNormLayer", "GroupNormLayer", "FusedOptimizer", "SGD", "AdamW", "f32_to_bf16_bits", "bf16_bits_to_f32", "TRAIN_SET", "TEST_SET", "U8", "F32"]

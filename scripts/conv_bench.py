@@ -1447,6 +1447,60 @@ def run_bnact(name, N, H, W, C, iters, rounds=3):
     del x, r, dy, y, dx, dr, xt, rt
 
 
+def run_gn(name, N, H, W, C, G, iters, rounds=3):
+    """group normalization: the forward at ReLU without and with the residual r, the backward at ReLU (pcnn_groupnorm_nhwc_bf16_bwd,
+    with dr) and, at SiLU with r, the forward and the pre-activation backward with dr (pcnn_groupnorm_nhwc_bf16_bwd_preact), the
+    passes alternated over `rounds` rounds (the best of each kept), next to torch's F.group_norm (+ add) + relu / silu and its
+    autograd backward on the same channels-last bf16 tensors.  Bytes, T = N*H*W*C*2: forward 3T (x read twice, y written) + T for
+    r; backward at ReLU 7T (x, y, dy read twice, dx written) + T for dr; at SiLU 7T (x, r, dy read twice, dx written) + T for dr."""
+    HW = H * W
+    T = N * HW * C * 2
+    rnd = lambda: torch.randint(-0x4000, 0x4000, (N * HW, C), dtype=torch.int16, device="cuda") & 0x3FFF | 0x3C00   # bf16 in [1, 2) * 2^k
+    x, r, dy = rnd(), rnd(), rnd()
+    r ^= torch.randint(0, 2, (N * HW, C), dtype=torch.int16, device="cuda") << 15
+    dy ^= torch.randint(0, 2, (N * HW, C), dtype=torch.int16, device="cuda") << 15
+    y, dx, dr = (torch.empty((N * HW, C), dtype=torch.int16, device="cuda") for _ in range(3))
+    info = pkg.groupnorm_nhwc_info(N, HW, C, G)
+    f = lambda v, n: eng.to_device(np.full(n, v, np.float32))
+    gamma, beta, dg, db = f(1, C), f(0, C), f(0, C), f(0, C)
+    sm, sr, ds = f(0, N * G), f(1, N * G), f(0, 2 * N * G)
+    gpu, power = card()
+    F = torch.nn.functional
+    bf = lambda t: t.view(torch.bfloat16).reshape(N, H, W, C).permute(0, 3, 1, 2)         # channels-last NCHW views
+    xt, rt, dyt = bf(x).detach().clone().requires_grad_(True), bf(r).detach().clone().requires_grad_(True), bf(dy)
+    gt = torch.ones(C, device="cuda", dtype=torch.bfloat16, requires_grad=True)
+    bt = torch.zeros(C, device="cuda", dtype=torch.bfloat16, requires_grad=True)
+
+    def torch_fwd(act, with_r):
+        v = F.group_norm(xt, G, gt, bt, 1e-5)
+        return act(v + rt if with_r else v)
+
+    out_relu, out_silu = torch_fwd(torch.relu, True), torch_fwd(F.silu, True)
+    passes = (("fwd", lambda: eng.groupnorm_fwd(x, y, N, HW, C, G, gamma, beta, sm, sr, act=3), lambda: torch_fwd(torch.relu, False), 3 * T),
+              ("fwd + r", lambda: eng.groupnorm_fwd(x, y, N, HW, C, G, gamma, beta, sm, sr, r=r, act=3), lambda: torch_fwd(torch.relu, True),
+               4 * T),
+              ("bwd + dr", lambda: eng.groupnorm_bwd(x, y, dy, gamma, sm, sr, dx, dg, db, ds, N, HW, C, G, act=3, dr=dr),
+               lambda: torch.autograd.grad(out_relu, [xt, gt, bt, rt], dyt, retain_graph=True), 8 * T),
+              ("SiLU fwd + r", lambda: eng.groupnorm_fwd(x, y, N, HW, C, G, gamma, beta, sm, sr, r=r, act=4), lambda: torch_fwd(F.silu, True),
+               4 * T),
+              ("SiLU preact bwd + dr", lambda: eng.groupnorm_bwd_preact(x, dy, gamma, beta, sm, sr, dx, dg, db, ds, N, HW, C, G, 4, r=r, dr=dr),
+               lambda: torch.autograd.grad(out_silu, [xt, gt, bt, rt], dyt, retain_graph=True), 8 * T))
+    best = {}
+    for _ in range(rounds):
+        for what, fn, tfn, nbytes in passes:
+            ms, ms_torch = timed(fn, iters), timed(tfn, iters)
+            old = best.get(what)
+            best[what] = (min(ms, old[0]) if old else ms, min(ms_torch, old[1]) if old else ms_torch, nbytes)
+    for what, _, _, _ in passes:
+        ms, ms_torch, nbytes = best[what]
+        print(json.dumps({"case": f"{name} {what}", "N": N, "G": G, "us": ms * 1e3, "MB": nbytes / 1e6,
+                          "hbm_frac": nbytes / (ms * 1e-3) / 1e9 / HBM, "torch_us": ms_torch * 1e3, "torch_over_ours": ms_torch / ms,
+                          "vec": info["vec"], "ranges": info["ranges"], "ctas": info["ctas"], "gpu": gpu, "power_limit": power}), flush=True)
+    for a in (gamma, beta, dg, db, sm, sr, ds):
+        a.free()
+    del x, r, dy, y, dx, dr, xt, rt
+
+
 def run_dropout(name, N, H, W, C, iters, per_sample, p=0.2, rounds=3):
     """dropout (element mode) or stochastic depth with r (per-sample mode) at p: the forward and the backward (the same call on dy,
     without r), ours and torch's alternated over `rounds` rounds (the best of each kept), on the same bf16 channels-last tensors.
@@ -2151,6 +2205,11 @@ if only == "dwdilated":                                                # dilated
         run_dwdilated("28x28x240 5x5", 128, 28, 28, 240, 5, d, 20)
 if only == "deeplab":
     run_deeplab(20)
+if only == "gn":                                                       # group normalization passes, torch beside them
+    run_gn("56x56x64 G32 (the bn shape)", 128, 56, 56, 64, 32, 20)
+    run_gn("128x128x64 G32", 8, 128, 128, 64, 32, 20)
+    run_gn("256x256x32 G8, small batch", 2, 256, 256, 32, 8, 20)
+    run_gn("28x28x256 G256 (instance norm)", 16, 28, 28, 256, 256, 20)
 eng.close()
 if only == "wprobe":                                                   # what a pure WRITE stream / pure READ stream / copy reach on this GPU
     # library fill / reduce / copy kernels as a yardstick for the store-dominated forward pass (807 MB written, 39 MB read):
