@@ -684,6 +684,47 @@ int pcnn_groupnorm_nhwc_bf16_bwd_preact(pcnn_ctx *ctx, const void *x_bf16_dev, c
                                         const float *save_rstd_dev, void *dx_bf16_dev, void *dr_bf16_dev, float *dgamma_dev,
                                         float *dbeta_dev, float *dstat_dev, int N, int HW, int C, int G, int act);
 int pcnn_groupnorm_nhwc_info(int N, int HW, int C, int G, int *out11);
+/* ---- self-attention ---------------------------------------------------------------------------------------------------------
+ * Self-attention over the T = H W pixels of each image (csrc/attention_tc.cu), as torch's scaled_dot_product_attention without a
+ * mask or dropout: per image n and head j, O = softmax(scale Q K^T) V.  q, k and v are bf16 with element (n, t, head j, i) at
+ * (n T + t) ld + j d + i, one ld for all three: with a fused qkv projection [N T][3 h d] they are its columns 0, h d and 2 h d, and
+ * ld = 3 h d.  o and dout are dense bf16 [N][T][h][d] (the x and dy of an output projection); lse is fp32 [N][h][T]; dq, dk and dv
+ * are written in q's layout with rows of ld_g elements, so the fused projection's dy is written in place.
+ * Forward, per row (image, head, query t), over key blocks of 64 in order; fp32 rounds to nearest without contraction:
+ *   1. scores s = q . k in fp32 on the tensor cores (bf16 products exact, fp32 accumulation in an order the hardware fixes);
+ *   2. u = RN(s c2), c2 = float(scale log2 e); keys >= T are u = -inf;
+ *   3. running max m = max(m, the block's u) (exact);
+ *   4. exponent p = ex2.approx(RN(u - m)) (relative error below 2^-22), alpha = ex2.approx(RN(m_old - m)) rescales l and acc;
+ *   5. P = bf16_rn(p);
+ *   6. sum l = RN(RN(l alpha) + the block's sum of P in fp32);
+ *   7. acc = RN(acc alpha) + P V in fp32 on the tensor cores;
+ *   8. division: o = bf16_rn(RN(acc RN(1 / l)));
+ *   9. lse = RN(RN(m + lg2.approx(l)) ln 2) (lg2.approx: absolute error below 2^-21), the natural-log logsumexp of scale s.
+ * Backward (pcnn_attention_bf16_bwd, given the forward's o and lse):
+ *   - D = sum over i of float(dout) float(o) per row, fp32 fma in the order i = 0 .. d - 1 (into the context's scratch);
+ *   - P = ex2.approx(RN(RN(s c2) - RN(lse log2 e))) recomputed, 0 for keys (dQ) or queries (dK, dV) >= T; dP = dout . v in fp32;
+ *   - dS = bf16_rn(RN(P RN(dP - D))), from the fp32 P; dV = bf16_rn(sum over queries of bf16_rn(P) dout) in fp32;
+ *   - scale placement: dQ = bf16_rn(RN(scale (sum over keys of dS k))) and dK = bf16_rn(RN(scale (sum over queries of dS q))),
+ *     the scale applied once, to the fp32 sums.
+ * Partition: a tile is (image, head, block of 128 query rows) in the forward and dQ kernels and (image, head, block of 128 keys) in
+ * the dK/dV kernel; each loops over blocks of 64 in a fixed order, with no atomics.  So the bits of one (image, head) do not depend
+ * on N, the other heads, the SM count or the run.  Rows past T, the columns of other heads and everything past the last row of a
+ * buffer are never written.
+ * Domain (anything else is PCNN_ERR_ARG with the called function and the rule in the message; the shape rules read the same in
+ * pcnn_attention_info):
+ *   - d 16, 32, 64 or 128; heads >= 1; N >= 1; 1 <= T <= 16384; N heads ceil(T / 128) tiles < 2^31;
+ *   - ld and ld_g >= heads d and multiples of 8; scale finite and > 0;
+ *   - every pointer 16-byte aligned; dq, dk and dv may share a buffer on disjoint columns; no output overlaps an input or
+ *     another output otherwise.
+ * pcnn_attention_info: host only (no GPU, no context), with ld_g 0 for the forward's rules alone.  out8 = { query rows per tile,
+ * rows per streamed block, stages, tiles of the forward, of the dK/dV kernel and of the dQ kernel, scratch bytes of the backward,
+ * dynamic shared memory of a backward kernel }. */
+int pcnn_attention_bf16_fwd(pcnn_ctx *ctx, const void *q_bf16_dev, const void *k_bf16_dev, const void *v_bf16_dev, int N, int T, int heads,
+                            int d, int ld, float scale, void *o_bf16_dev, float *lse_dev);
+int pcnn_attention_bf16_bwd(pcnn_ctx *ctx, const void *q_bf16_dev, const void *k_bf16_dev, const void *v_bf16_dev, const void *o_bf16_dev,
+                            const void *dout_bf16_dev, const float *lse_dev, int N, int T, int heads, int d, int ld, float scale,
+                            void *dq_bf16_dev, void *dk_bf16_dev, void *dv_bf16_dev, int ld_g);
+int pcnn_attention_info(int N, int T, int heads, int d, int ld, int ld_g, float scale, long long *out8);
 /* Fully connected layers (csrc/linear_tc.cu), bf16 on the tensor cores with fp32 accumulation:
  *   - x is [N][image_rows][row_pitch] bf16 with P x Q pixels of C channels per image: the layout a plan reads as x and the NHWC
  *     pool writes as y.  A previous linear layer's y is the same with P = Q = 1, C = its O, row_pitch = O, image_rows 1.

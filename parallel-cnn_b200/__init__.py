@@ -13,7 +13,7 @@ from ._lib import (  # noqa: F401
     ACT_SILU, ACT_HARDSWISH, ACT_RELU6,
     lib, declared_symbols, init_params_reference, mnist_load_u8, conv_tc_plan_info, conv_wide_plan_info, conv_wide_bwd_info,
     conv_bwd_plan_info, conv_layer_family, maxpool_nhwc_info, avgpool_nhwc_info, global_avgpool_nhwc_info, batchnorm_nhwc_info,
-    groupnorm_nhwc_info,
+    groupnorm_nhwc_info, attention_info,
     linear_info, dwconv_info, gconv_info, se_scale_nhwc_info, dropout_info, augment_info, augment_resized_info, RESIZE_TRAIN, RESIZE_EVAL, OPTIM_SGD, OPTIM_ADAMW,
     augment_trivial_info, TRIVIAL_NONE, TRIVIAL_NEAREST, TRIVIAL_BILINEAR, TRIVIAL_OPS, conv_transpose_info, upsample_bilinear_info,
 )
@@ -22,6 +22,7 @@ from .engine import DepthwiseConvLayer, DepthwiseConvPlan, DropoutLayer, Grouped
 from .engine import ImageBatcher, MixedLabels, MIX_MIXUP, MIX_CUTMIX, mix_draws  # noqa: F401
 from .engine import SGD, AdamW, FusedOptimizer  # noqa: F401
 from .engine import ConvTransposeLayer, UpsampleBilinearLayer, segmentation_scores  # noqa: F401
+from .engine import SelfAttentionLayer  # noqa: F401
 
 __all__ = ["Engine", "DeviceArray", "PcnnError", "lib", "declared_symbols", "init_params_reference",
            "mnist_load_u8", "conv_tc_plan_info", "conv_wide_plan_info", "conv_wide_bwd_info", "conv_bwd_plan_info", "conv_layer_family", "maxpool_nhwc_info", "avgpool_nhwc_info", "global_avgpool_nhwc_info", "batchnorm_nhwc_info", "linear_info", "ConvLayer", "BatchNormLayer", "MaxPoolLayer", "AvgPoolLayer", "GlobalAvgPoolLayer", "LinearLayer", "ConvPlan", "LinearPlan",
@@ -32,4 +33,4 @@ __all__ = ["Engine", "DeviceArray", "PcnnError", "lib", "declared_symbols", "ini
            "dropout_info", "DropoutLayer", "augment_info", "augment_resized_info", "RESIZE_TRAIN", "RESIZE_EVAL", "ImageBatcher",
            "MixedLabels", "MIX_MIXUP", "MIX_CUTMIX", "mix_draws", "augment_trivial_info", "TRIVIAL_NONE", "TRIVIAL_NEAREST",
            "TRIVIAL_BILINEAR", "TRIVIAL_OPS", "conv_transpose_info", "upsample_bilinear_info", "ConvTransposeLayer",
-           "UpsampleBilinearLayer", "segmentation_scores", "groupnorm_nhwc_info", "GroupNormLayer"]
+           "UpsampleBilinearLayer", "segmentation_scores", "groupnorm_nhwc_info", "GroupNormLayer", "attention_info", "SelfAttentionLayer"]

@@ -1,5 +1,6 @@
 """ctypes declarations for every symbol of include/pcnn.h (kept in the same order as the header)."""
 import ctypes as C
+import math
 import os
 import re
 
@@ -165,6 +166,9 @@ _SIG = {
     "pcnn_groupnorm_nhwc_bf16_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i],
     "pcnn_groupnorm_nhwc_bf16_bwd_preact": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i],
     "pcnn_groupnorm_nhwc_info": [_i, _i, _i, _i, _vp],
+    "pcnn_attention_bf16_fwd": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp],
+    "pcnn_attention_bf16_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp, _vp, _i],
+    "pcnn_attention_info": [_i, _i, _i, _i, _i, _i, _f, _vp],
     "pcnn_conv_bwd_plan_info": [_i, _i, _i, _i, _i, _i, _i, _vp],
     "pcnn_pad_nhwc_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i],
     "pcnn_crop_nhwc_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i],
@@ -420,6 +424,17 @@ def groupnorm_nhwc_info(N, HW, C, G):
     check("pcnn_groupnorm_nhwc_info", lib().pcnn_groupnorm_nhwc_info(int(N), int(HW), int(C), int(G), out))
     return dict(vec=out[0], groups_per_cta=out[1], slices=out[2], lanes=out[3], pixels_per_range=out[4], ranges=out[5], ctas=out[6],
                 slots=out[7], group_ctas=out[8], n_acc=out[9], n_acc_group=out[10])
+
+
+def attention_info(N, T, heads, d, ld=None, ld_g=0, scale=None):
+    """How self-attention tiles a shape (pcnn_attention_info; host only, no GPU), refused as the device calls refuse.  ld None =
+    heads * d (separate dense q, k and v); ld_g 0 leaves out the backward's output rule; scale None = 1 / sqrt(d)."""
+    ld = int(heads) * int(d) if ld is None else int(ld)
+    scale = 1.0 / math.sqrt(d) if scale is None else float(scale)
+    out = (_ll * 8)()
+    check("pcnn_attention_info", lib().pcnn_attention_info(int(N), int(T), int(heads), int(d), ld, int(ld_g), scale, out))
+    return dict(query_rows=out[0], block_rows=out[1], stages=out[2], fwd_tiles=out[3], dkdv_tiles=out[4], dq_tiles=out[5],
+                scratch_bytes=out[6], bwd_smem=out[7])
 
 
 def linear_info(N, P, Q, C, O, row_pitch=0, image_rows=0):

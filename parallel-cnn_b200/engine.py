@@ -8,7 +8,7 @@ import numpy as np
 
 from ._lib import (F32, NPARAM, OPTIM_ADAMW, OPTIM_SGD, TEST_SET, TRAIN_SET, U8, OptimConfig, OptimTensor, PcnnError, augment_info,
                    augment_resized_info, RESIZE_TRAIN, RESIZE_EVAL, augment_trivial_info, TRIVIAL_NONE, TRIVIAL_NEAREST, TRIVIAL_BILINEAR,
-                   avgpool_nhwc_info, batchnorm_nhwc_info, channel_stats, check, conv_layer_family, conv_transpose_info, upsample_bilinear_info, dropout_info, dwconv_info, gconv_info, global_avgpool_nhwc_info, groupnorm_nhwc_info, lib,
+                   attention_info, avgpool_nhwc_info, batchnorm_nhwc_info, channel_stats, check, conv_layer_family, conv_transpose_info, upsample_bilinear_info, dropout_info, dwconv_info, gconv_info, global_avgpool_nhwc_info, groupnorm_nhwc_info, lib,
                    linear_info, maxpool_nhwc_info,
                    se_scale_nhwc_info, ACT_RELU, ACT_SIGMOID, ACT_SILU, ACT_HARDSWISH, ACT_RELU6)
 
@@ -515,6 +515,20 @@ class Engine:
         pre-activation recomputed from x, the saved statistics, gamma, beta and r (the forward's r, unchanged, or None)"""
         self._call("pcnn_groupnorm_nhwc_bf16_bwd_preact", _p(x), _p(r), _p(dy), _p(dy2), _p(gamma), _p(beta), _p(save_mean), _p(save_rstd),
                    _p(dx), _p(dr), _p(dgamma), _p(dbeta), _p(dstat), int(N), int(HW), int(C), int(G), int(act))
+
+    def attention_fwd(self, q, k, v, o, lse, N, T, heads, d, ld=None, scale=None):
+        """pcnn_attention_bf16_fwd: o = softmax(scale q k^T) v per image and head over T tokens, lse [N][heads][T] its logsumexp.  q,
+        k and v are bf16 rows of ld elements (default heads * d), head j at columns j d; o is dense [N][T][heads][d].  scale None =
+        1 / sqrt(d)"""
+        self._call("pcnn_attention_bf16_fwd", _p(q), _p(k), _p(v), int(N), int(T), int(heads), int(d), int(heads * d if ld is None else ld),
+                   float(1.0 / math.sqrt(d) if scale is None else scale), _p(o), _p(lse))
+
+    def attention_bwd(self, q, k, v, o, dout, lse, dq, dk, dv, N, T, heads, d, ld=None, ld_g=None, scale=None):
+        """pcnn_attention_bf16_bwd: dq, dk and dv (rows of ld_g elements, default ld) of the forward that wrote o and lse, given
+        dout [N][T][heads][d]; they may be the column blocks of one fused buffer"""
+        ld = int(heads * d if ld is None else ld)
+        self._call("pcnn_attention_bf16_bwd", _p(q), _p(k), _p(v), _p(o), _p(dout), _p(lse), int(N), int(T), int(heads), int(d), ld,
+                   float(1.0 / math.sqrt(d) if scale is None else scale), _p(dq), _p(dk), _p(dv), int(ld if ld_g is None else ld_g))
 
     def pad_nhwc(self, src_bf16, dst_bf16, N, H, W, Cin, pad_h, pad_w, dst_row_pitch=0, dst_image_rows=0):
         self._call("pcnn_pad_nhwc_bf16", _p(src_bf16), _p(dst_bf16), N, H, W, Cin, int(pad_h), int(pad_w), int(dst_row_pitch), int(dst_image_rows))
@@ -1269,6 +1283,76 @@ class LinearLayer(_PlanLayer):
             self.engine.linear_dgrad(self.plan, dy, dx)
 
 
+class SelfAttentionLayer:
+    """Multi-head self-attention over the H x W pixels of each image, trained on the device: a fused qkv LinearLayer (C -> 3 heads
+    head_dim, so heads * head_dim <= 85), the attention core (pcnn_attention_bf16_fwd / _bwd) and an output LinearLayer (heads
+    head_dim -> C).  w_qkv is fp32 [3 heads head_dim][C] with the rows of q, then k, then v, head j at rows j head_dim of each; w_out
+    is [C][heads head_dim].  scale None = 1 / sqrt(head_dim).
+
+    x, y, dy and dx are dense bf16 [N][H][W][C] (C a multiple of 8).  The residual and the normalization of a non-local block stay in
+    the network, joined through dy2 as every residual here is:
+
+        attn.forward(x, wz);  bn.forward(wz, z, r=x)
+        bn.backward(z, dz, dwz, dr=dres);  attn.backward(dwz, dx);  <the layer that wrote x>.backward(..., dx, dy2=dres)
+
+    The layer keeps x and its own activations (qkv, o, lse) for backward.  optim_tensors() lists both projections' tensors, so SGD
+    and AdamW take the layer as they take a LinearLayer."""
+
+    def __init__(self, engine, N, H, W, C, heads, head_dim, w_qkv, b_qkv, w_out, b_out=None, scale=None):
+        self.engine = engine
+        self.shape = (N, H, W, C)
+        self.heads, self.d = int(heads), int(head_dim)
+        self.T = int(H) * int(W)
+        self.scale = 1.0 / math.sqrt(self.d) if scale is None else float(scale)
+        hd = self.heads * self.d
+        rows = int(N) * self.T
+        self.info = attention_info(N, self.T, self.heads, self.d, 3 * hd, 3 * hd, self.scale)
+        self.qkv = LinearLayer(engine, rows, 1, 1, C, 3 * hd, w_qkv, b_qkv)
+        self.out = LinearLayer(engine, rows, 1, 1, hd, C, w_out, b_out)
+        self.qkv_y, self.dqkv = engine.array(rows * 3 * hd, np.uint16), engine.array(rows * 3 * hd, np.uint16)
+        self.o, self.do = engine.array(rows * hd, np.uint16), engine.array(rows * hd, np.uint16)
+        self.lse = engine.array(int(N) * self.heads * self.T)
+
+    def _qkv(self, base):
+        hd2 = self.heads * self.d * 2
+        return base.ptr, base.ptr + hd2, base.ptr + 2 * hd2
+
+    def forward(self, x, y):
+        """y = out(attention(qkv(x))) + b_out"""
+        N, H, W, C = self.shape
+        self.qkv.forward(x, self.qkv_y)
+        self.engine.attention_fwd(*self._qkv(self.qkv_y), self.o, self.lse, N, self.T, self.heads, self.d, ld=3 * self.heads * self.d,
+                                  scale=self.scale)
+        self.out.forward(self.o, y)
+
+    def backward(self, dy, dx):
+        """Gradients of the most recent forward: both projections' dw and db and, when dx is given, dx.  dy is left unchanged."""
+        N, H, W, C = self.shape
+        ld = 3 * self.heads * self.d
+        self.out.backward(None, dy, self.do)
+        self.engine.attention_bwd(*self._qkv(self.qkv_y), self.o, self.do, self.lse, *self._qkv(self.dqkv), N, self.T, self.heads, self.d,
+                                  ld=ld, ld_g=ld, scale=self.scale)
+        self.qkv.backward(None, self.dqkv, dx)
+
+    def sgd(self, lr):
+        self.qkv.sgd(lr)
+        self.out.sgd(lr)
+
+    def optim_tensors(self):
+        """the qkv projection's tensors, then the output projection's, as LinearLayer.optim_tensors"""
+        return self.qkv.optim_tensors() + self.out.optim_tensors()
+
+    def params(self):
+        """host copies (w_qkv, b_qkv, w_out, b_out) of the fp32 masters; b_out None without one"""
+        return (*self.qkv.params(), *self.out.params())
+
+    def close(self):
+        self.qkv.close()
+        self.out.close()
+        for a in (self.qkv_y, self.dqkv, self.o, self.do, self.lse):
+            a.free()
+
+
 class MaxPoolLayer:
     """Max pooling between two ConvLayers (pcnn_maxpool_nhwc_bf16_fwd / _bwd), as max_pool2d(kernel (R, S), stride, padding): S
     defaults to R and stride to R, as torch does.  It owns the uint8 argmax [N][P][Q][C] the backward reads.
@@ -1756,4 +1840,4 @@ def bf16_bits_to_f32(b):
 
 
 C_ = C
-__all__ = ["Engine", "DeviceArray", "ConvPlan", "WideConvPlan", "LinearPlan", "ConvLayer", "LinearLayer", "MaxPoolLayer", "AvgPoolLayer", "GlobalAvgPoolLayer", "BatchNormLayer", "GroupNormLayer", "FusedOptimizer", "SGD", "AdamW", "f32_to_bf16_bits", "bf16_bits_to_f32", "TRAIN_SET", "TEST_SET", "U8", "F32"]
+__all__ = ["Engine", "DeviceArray", "ConvPlan", "WideConvPlan", "LinearPlan", "ConvLayer", "LinearLayer", "MaxPoolLayer", "AvgPoolLayer", "GlobalAvgPoolLayer", "BatchNormLayer", "GroupNormLayer", "SelfAttentionLayer", "FusedOptimizer", "SGD", "AdamW", "f32_to_bf16_bits", "bf16_bits_to_f32", "TRAIN_SET", "TEST_SET", "U8", "F32"]

@@ -645,6 +645,72 @@ def run_pool(name, N, H, W, C, R, stride, pad, iters):
     del x, y, am, dy, dx, xt, dyt, idx
 
 
+def run_nlblock(name, N, H, W, C, h, d, iters):
+    """one non-local block training step (forward and backward, no optimizer): SelfAttentionLayer then BatchNormLayer with r = the
+    block's input, against the same block in torch eager (bf16 linear layers, scaled_dot_product_attention, batch norm and the
+    residual, autograd for the input and parameter gradients)"""
+    hd, T = h * d, H * W
+    g = np.random.default_rng(5)
+    wq, bq = (g.standard_normal((3 * hd, C)) / np.sqrt(C)).astype(np.float32), np.zeros(3 * hd, np.float32)
+    wo, bo = (g.standard_normal((C, hd)) / np.sqrt(hd)).astype(np.float32), np.zeros(C, np.float32)
+    attn = pkg.SelfAttentionLayer(eng, N, H, W, C, h, d, wq, bq, wo, bo)
+    bn = pkg.BatchNormLayer(eng, N, H, W, C)
+    x, dz = _bf((N, H, W, C)), _bf((N, H, W, C))
+    wz, z, dwz, dres, dx = (torch.empty_like(x) for _ in range(5))
+
+    def step():
+        attn.forward(x, wz)
+        bn.forward(wz, z, r=x)
+        bn.backward(z, dz, dwz, dr=dres)
+        attn.backward(dwz, dx)
+
+    ms = timed(step, iters)
+    tq, tbq, to, tbo = (torch.tensor(a, device="cuda", dtype=torch.bfloat16, requires_grad=True) for a in (wq, bq, wo, bo))
+    gamma, beta = (torch.full((C,), v, device="cuda", requires_grad=True) for v in (1.0, 0.0))
+    xt = x.detach().clone().requires_grad_(True)
+
+    def torch_step():
+        t = xt.reshape(N, T, C)
+        q, k, v = torch.nn.functional.linear(t, tq, tbq).reshape(N, T, 3, h, d).permute(2, 0, 3, 1, 4)
+        o = torch.nn.functional.scaled_dot_product_attention(q, k, v).transpose(1, 2).reshape(N, T, hd)
+        y = torch.nn.functional.linear(o, to, tbo).reshape(N, H, W, C).permute(0, 3, 1, 2)
+        zt = torch.nn.functional.batch_norm(y, None, None, gamma, beta, training=True) + xt.permute(0, 3, 1, 2)
+        torch.autograd.grad(zt, (xt, tq, tbq, to, tbo, gamma, beta), dz.permute(0, 3, 1, 2))
+
+    ms_t = timed(torch_step, iters)
+    _line(name, ms, ms_t)
+    attn.close()
+    bn.close()
+
+
+def run_attn(name, N, T, h, d, iters):
+    """self-attention forward and backward (pcnn_attention_bf16_fwd / _bwd) against torch's flash scaled_dot_product_attention
+    and its autograd backward, on the same bf16 [N][T][h][d] tensors.  Useful work: 4 N h T^2 d flops forward, 10 N h T^2 d
+    backward (the five T x T x d products, without the recomputed S); the backward recomputes S, a further 2 N h T^2 d, reported
+    apart.  Shares of the 989 TFLOP/s dense bf16 data-sheet figure."""
+    q, k, v, do = (_bf((N, T, h, d)) for _ in range(4))
+    o = torch.empty_like(q)
+    lse = torch.empty((N, h, T), device="cuda", dtype=torch.float32)
+    dq, dk, dv = (torch.empty_like(q) for _ in range(3))
+    fwd = lambda: eng.attention_fwd(q, k, v, o, lse, N, T, h, d)
+    bwd = lambda: eng.attention_bwd(q, k, v, o, do, lse, dq, dk, dv, N, T, h, d)
+    fwd()
+    ms_f, ms_b = timed(fwd, iters), timed(bwd, iters)
+    from torch.nn.attention import SDPBackend, sdpa_kernel
+    qt, kt, vt = (t.transpose(1, 2).detach().requires_grad_(True) for t in (q, k, v))
+    dot = do.transpose(1, 2)
+    with sdpa_kernel(SDPBackend.FLASH_ATTENTION):
+        ot = torch.nn.functional.scaled_dot_product_attention(qt, kt, vt)
+        ms_tf = timed(lambda: torch.nn.functional.scaled_dot_product_attention(qt, kt, vt), iters)
+        ms_tb = timed(lambda: torch.autograd.grad(ot, (qt, kt, vt), dot, retain_graph=True), iters)
+    diff = (o.float() - ot.detach().transpose(1, 2).float()).abs().max().item()
+    fl = N * h * T * T * d
+    peak = 989e12
+    _line(name + " fwd", ms_f, ms_tf, flops=4 * fl, tflops=4 * fl / ms_f / 1e9, peak_frac=4 * fl / (ms_f * 1e-3) / peak, max_abs_diff_o=diff)
+    _line(name + " bwd", ms_b, ms_tb, flops=10 * fl, recompute_flops=2 * fl, tflops=10 * fl / ms_b / 1e9,
+          peak_frac=10 * fl / (ms_b * 1e-3) / peak, peak_frac_with_recompute=12 * fl / (ms_b * 1e-3) / peak)
+
+
 def timed(fn, iters):
     for _ in range(5):
         fn()
@@ -2210,6 +2276,14 @@ if only == "gn":                                                       # group n
     run_gn("128x128x64 G32", 8, 128, 128, 64, 32, 20)
     run_gn("256x256x32 G8, small batch", 2, 256, 256, 32, 8, 20)
     run_gn("28x28x256 G256 (instance norm)", 16, 28, 28, 256, 256, 20)
+if only == "nlblock":                                                  # one non-local block training step, torch eager beside it
+    run_nlblock("non-local block N128 12x12x16 h1 d16 (NonLocalResNet)", 128, 12, 12, 16, 1, 16, 50)
+    run_nlblock("non-local block N128 28x28x64 h1 d64", 128, 28, 28, 64, 1, 64, 20)
+if only == "attn":                                                     # self-attention, torch's flash SDPA beside it
+    run_attn("BoTNet 14x14 N128 T196 h4 d64", 128, 196, 4, 64, 20)
+    run_attn("non-local Res3 N32 T784 h1 d128", 32, 784, 1, 128, 20)
+    run_attn("N16 T3136 h1 d64", 16, 3136, 1, 64, 10)
+    run_attn("DANet N8 T4096 h1 d64", 8, 4096, 1, 64, 10)
 eng.close()
 if only == "wprobe":                                                   # what a pure WRITE stream / pure READ stream / copy reach on this GPU
     # library fill / reduce / copy kernels as a yardstick for the store-dominated forward pass (807 MB written, 39 MB read):
