@@ -1214,6 +1214,45 @@ int pcnn_softmax_ce_pixels_bf16(pcnn_ctx *ctx, const void *logits_bf16_dev, cons
  * messages, 0 <= mask_fill <= 255, masks_out disjoint from masks. */
 int pcnn_augment_mask_u8(pcnn_ctx *ctx, const uint8_t *masks_dev, long long n, int H, int W, long long first, int N, int shuffle, int pad,
                          int flip, unsigned long long seed, unsigned long long epoch, int mask_fill, uint8_t *masks_out_dev);
+/* ------------------------------------------------------------------ image-to-image regression
+ * Pixel shuffle and unshuffle (csrc/pixel_shuffle_nhwc.cu), as torch.nn.functional.pixel_shuffle / pixel_unshuffle with upscale /
+ * downscale factor r, written for dense bf16 NHWC maps.  With a coarse map [N][H][W][C r^2] and a fine map [N][H r][W r][C]:
+ *     fine[n][h r + i][w r + j][c] = coarse[n][h][w][c r^2 + i r + j],   0 <= i, j < r
+ * (torch's channel order; TensorFlow's depth_to_space, (i r + j) C + c, is a different permutation).
+ *   - pcnn_pixel_shuffle_nhwc_bf16: x is the coarse map [N][H][W][C r^2], y the fine map [N][H r][W r][C];
+ *   - pcnn_pixel_unshuffle_nhwc_bf16: x is the fine map [N][H][W][C] with H % r == W % r == 0, y the coarse map
+ *     [N][H / r][W / r][C r^2].
+ * Each call's own input fixes (N, H, W) and C is the fine map's channel count in both.  The backward of each op is the other op on
+ * dy.  Every element of y is a 16-bit copy of one element of x (NaN payloads, +-Inf and -0 unchanged), every element of y is
+ * written and nothing else; r = 1 is a copy, as in torch.  Channels per thread: 8 (16-byte accesses) when C % 8 == 0, else 1.
+ * Domain (PCNN_ERR_ARG, one message per rule): no NULL context, x or y; N, H, W, C >= 1; 1 <= r <= 8; H and W multiples of r
+ * (unshuffle); each map at most 2^31 - 1 elements; x and y 16-byte aligned; x and y disjoint (a permutation cannot run in place).
+ * pcnn_pixel_shuffle_info (host only, unshuffle 0 or 1 picks the direction) refuses the same, bar the pointers, and fills
+ * out6 = { channels per thread (8 or 1), grid, threads per CTA, shared bytes per CTA, coarse pixels per CTA, fine channels per
+ * CTA (C, or a multiple of 8 channels per thread when C r^2 exceeds one CTA's tile) }. */
+int pcnn_pixel_shuffle_info(int N, int H, int W, int C, int r, int unshuffle, long long *out6);
+int pcnn_pixel_shuffle_nhwc_bf16(pcnn_ctx *ctx, const void *x_bf16_dev, void *y_bf16_dev, int N, int H, int W, int C, int r);
+int pcnn_pixel_unshuffle_nhwc_bf16(pcnn_ctx *ctx, const void *x_bf16_dev, void *y_bf16_dev, int N, int H, int W, int C, int r);
+/* Regression losses (csrc/regress_loss.cu): F.mse_loss / F.l1_loss of a dense bf16 prediction pred [pixels][C] against the first C
+ * channels of a bf16 target [pixels][target_stride] (so a C = 1 prediction compares with channel 0 of a wider map, no copy).
+ * RN32 is one fp32 operation rounded to nearest even, never contracted; bf16_rn writes every NaN as 0x7FFF.  Per element:
+ *     d = RN32(p - t)
+ *     PCNN_LOSS_MSE: term = RN32(d d),  dpred = bf16_rn(RN32(RN32(2 scale) d))
+ *     PCNN_LOSS_L1:  term = |d|,        dpred = bf16_rn(RN32(s(d) scale)),  s(d) = +1 (d > 0), -1 (d < 0), +0 (d = +-0 or NaN)
+ *     loss[px] = the fp32 sum from +0, in ascending c, of the pixel's terms: unscaled, as pcnn_softmax_ce_bf16's row loss; loss may
+ *     be NULL.  The mean loss is sum(loss) / (pixels C), and scale = 1 / (pixels C) makes dpred the gradient of reduction="mean".
+ * Special values, as torch's float32 and float64 CPU autograd give them: MSE's dpred is -0 at d = -0, NaN at a NaN d and +-Inf at
+ * d = +-Inf (a finite p - t can also overflow to +-Inf in fp32); L1's dpred is +0 at d = +-0 and at a NaN d (torch's sign(NaN) is
+ * 0), while its loss term is NaN.  torch's CUDA autograd gives the same classes, with its own roundings (parity within a bf16 ulp).
+ * Each element's dpred and each pixel's loss depend on that pixel alone: no cross-CTA reduction, no atomics, and reruns and grids
+ * give the same bits.  The 16-byte path (8 channels per thread) runs when C and target_stride are multiples of 8.
+ * Domain (PCNN_ERR_ARG, one message per rule): no NULL context, pred, target or dpred; pixels >= 1; 1 <= C <= target_stride; mode
+ * PCNN_LOSS_MSE or PCNN_LOSS_L1; scale finite; pred, target, dpred and loss 16-byte aligned; dpred == pred (in place) is allowed,
+ * any other overlap of dpred or loss with pred, target or each other is not. */
+#define PCNN_LOSS_MSE 0
+#define PCNN_LOSS_L1 1
+int pcnn_regression_loss_bf16(pcnn_ctx *ctx, const void *pred_bf16_dev, const void *target_bf16_dev, int target_stride, int pixels, int C,
+                              int mode, float scale, void *dpred_bf16_dev, float *loss_f32_dev);
 /* Optimizers for device-trained layers (csrc/optim.cu): one fused update of every parameter tensor of a network per step, as
  * torch.optim.SGD and torch.optim.AdamW (decoupled weight decay) in their single-tensor form, with the bf16 operands of the plans
  * the parameters belong to refreshed in the same pass.

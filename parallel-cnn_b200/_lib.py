@@ -19,6 +19,7 @@ TRAIN_SET, TEST_SET = 0, 1
 ACT_NONE, ACT_SIGMOID, ACT_RELU = 0, 1, 3     # PCNN_ACT_*: the `act` of the device-trained layers (2 is not a code)
 ACT_SILU, ACT_HARDSWISH, ACT_RELU6 = 4, 5, 6  # taken by the normalizations only (BatchNormLayer, GroupNormLayer and their Engine calls)
 OPTIM_SGD, OPTIM_ADAMW = 0, 1                 # PCNN_OPTIM_*: the `kind` of pcnn_optim_config
+LOSS_MSE, LOSS_L1 = 0, 1                      # PCNN_LOSS_*: the `mode` of pcnn_regression_loss_bf16
 
 
 class PcnnError(RuntimeError):
@@ -220,6 +221,10 @@ _SIG = {
     "pcnn_upsample_bilinear_nhwc_bf16_fwd": [_vp, _vp, _vp] + [_i] * 6,
     "pcnn_upsample_bilinear_nhwc_bf16_bwd": [_vp, _vp, _vp] + [_i] * 6,
     "pcnn_augment_mask_u8": [_vp, _vp, C.c_longlong, _i, _i, C.c_longlong, _i, _i, _i, _i, C.c_ulonglong, C.c_ulonglong, _i, _vp],
+    "pcnn_pixel_shuffle_info": [_i] * 6 + [_vp],
+    "pcnn_pixel_shuffle_nhwc_bf16": [_vp, _vp, _vp] + [_i] * 5,
+    "pcnn_pixel_unshuffle_nhwc_bf16": [_vp, _vp, _vp] + [_i] * 5,
+    "pcnn_regression_loss_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _f, _vp, _vp],
     "pcnn_optim_create": [_vp, _vp, _vp, _i, _pvp],
     "pcnn_optim_step": [_vp, _vp, _f],
     "pcnn_optim_state": [_vp, _i, _pvp, _pvp],
@@ -337,6 +342,15 @@ def upsample_bilinear_info(N, H, W, Cin, H_out, W_out):
     out = (C.c_longlong * 4)()
     check("pcnn_upsample_bilinear_info", lib().pcnn_upsample_bilinear_info(int(N), int(H), int(W), int(Cin), int(H_out), int(W_out), out))
     return dict(vec=out[0], grid_fwd=out[1], grid_bwd=out[2], threads=out[3])
+
+
+def pixel_shuffle_info(N, H, W, C, r, unshuffle=False):
+    """How the pixel shuffle (unshuffle False: x [N][H][W][C r^2] -> [N][H r][W r][C]) or unshuffle (True: x [N][H][W][C] ->
+    [N][H / r][W / r][C r^2]) partitions a shape (pcnn_pixel_shuffle_info; host only, no GPU), refused as the calls refuse.  vec:
+    channels per thread (8 or 1); each CTA moves tile_pixels coarse pixels times chunk_channels fine channels through smem bytes."""
+    out = (_ll * 6)()
+    check("pcnn_pixel_shuffle_info", lib().pcnn_pixel_shuffle_info(int(N), int(H), int(W), int(C), int(r), int(bool(unshuffle)), out))
+    return dict(vec=out[0], grid=out[1], threads=out[2], smem=out[3], tile_pixels=out[4], chunk_channels=out[5])
 
 
 def conv_layer_family(N, H, W, C, K, R, S, stride=1, padding=(0, 0), row_pitch=None, image_rows=0, dilation=(1, 1)):

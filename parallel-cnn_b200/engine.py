@@ -9,7 +9,7 @@ import numpy as np
 from ._lib import (F32, NPARAM, OPTIM_ADAMW, OPTIM_SGD, TEST_SET, TRAIN_SET, U8, OptimConfig, OptimTensor, PcnnError, augment_info,
                    augment_resized_info, RESIZE_TRAIN, RESIZE_EVAL, augment_trivial_info, TRIVIAL_NONE, TRIVIAL_NEAREST, TRIVIAL_BILINEAR,
                    attention_info, avgpool_nhwc_info, batchnorm_nhwc_info, channel_stats, check, conv_layer_family, conv_transpose_info, upsample_bilinear_info, dropout_info, dwconv_info, gconv_info, global_avgpool_nhwc_info, groupnorm_nhwc_info, lib,
-                   linear_info, maxpool_nhwc_info,
+                   linear_info, maxpool_nhwc_info, pixel_shuffle_info, LOSS_MSE,
                    se_scale_nhwc_info, ACT_RELU, ACT_SIGMOID, ACT_SILU, ACT_HARDSWISH, ACT_RELU6)
 
 PREACT_CODES = (ACT_SILU, ACT_HARDSWISH, ACT_RELU6)   # the normalizations' codes whose backward recomputes the pre-activation
@@ -578,6 +578,27 @@ class Engine:
         written"""
         self._call("pcnn_upsample_bilinear_nhwc_bf16_bwd", _p(dy), _p(dx), int(N), int(H), int(W), int(Cin), int(H_out), int(W_out))
 
+    def pixel_shuffle(self, x, y, N, H, W, Cin, r):
+        """pcnn_pixel_shuffle_nhwc_bf16: F.pixel_shuffle(x, r) on dense bf16 NHWC, x [N][H][W][C r^2] -> y [N][H r][W r][C],
+        y[n][h r + i][w r + j][c] = x[n][h][w][c r^2 + i r + j], every element a bit copy"""
+        self._call("pcnn_pixel_shuffle_nhwc_bf16", _p(x), _p(y), int(N), int(H), int(W), int(Cin), int(r))
+
+    def pixel_unshuffle(self, x, y, N, H, W, Cin, r):
+        """pcnn_pixel_unshuffle_nhwc_bf16: F.pixel_unshuffle(x, r) on dense bf16 NHWC, x [N][H][W][C] -> y [N][H / r][W / r][C r^2],
+        the inverse of pixel_shuffle (and its backward)"""
+        self._call("pcnn_pixel_unshuffle_nhwc_bf16", _p(x), _p(y), int(N), int(H), int(W), int(Cin), int(r))
+
+    def regression_loss_bf16(self, pred, target, pixels, C, dpred, loss=None, mode=LOSS_MSE, target_stride=None, scale=None):
+        """pcnn_regression_loss_bf16: mse_loss (mode LOSS_MSE) or l1_loss (LOSS_L1) of bf16 pred [pixels][C] against the first C
+        channels of bf16 target [pixels][target_stride] (None = C).  dpred (may be pred) receives the gradient at scale (None =
+        1 / (pixels C), the gradient of reduction="mean"); loss (fp32 [pixels] or None) the unscaled sum of each pixel's terms."""
+        ts = int(C) if target_stride is None else int(target_stride)
+        if scale is None:
+            n = int(pixels) * int(C)
+            scale = 1.0 / n if n > 0 else 1.0             # n <= 0: a shape the call refuses
+        self._call("pcnn_regression_loss_bf16", _p(pred), _p(target), ts, int(pixels), int(C), int(mode), float(scale), _p(dpred),
+                   _p(loss))
+
     def augment_mask(self, masks, n, H, W, first, N, masks_out, shuffle=1, pad=0, flip=0, seed=0, epoch=0, mask_fill=255):
         """pcnn_augment_mask_u8: the uint8 masks [n][H][W] of augment's batch with the same arguments, each permuted, cropped and
         flipped exactly as its image, the padding filled with mask_fill, into masks_out [N][H][W]"""
@@ -1011,6 +1032,64 @@ class UpsampleBilinearLayer:
 
     def close(self):
         pass
+
+
+class PixelShuffleLayer:
+    """Sub-pixel upsampling between two layers (pcnn_pixel_shuffle_nhwc_bf16), as F.pixel_shuffle(x, r): x and dx dense bf16
+    [N][H][W][C r^2] (a convolution's or a per-pixel LinearLayer's output with C r^2 channels), y and dy dense [N][H r][W r][C].  It
+    keeps no state; info is its partition (pixel_shuffle_info).  The backward is the unshuffle of dy: a bit copy, like the forward."""
+
+    def __init__(self, engine, N, H, W, C, r):
+        self.engine = engine
+        self.shape = (int(N), int(H), int(W), int(C), int(r))
+        self.info = pixel_shuffle_info(*self.shape)
+        pixel_shuffle_info(N, H * r, W * r, C, r, unshuffle=True)      # the backward's shape, refused here rather than mid-step
+        self.out_shape = (int(N), int(H) * int(r), int(W) * int(r), int(C))
+
+    def forward(self, x, y):
+        self.engine.pixel_shuffle(x, y, *self.shape)
+
+    def backward(self, dy, dx):
+        N, H, W, C, r = self.shape
+        self.engine.pixel_unshuffle(dy, dx, N, H * r, W * r, C, r)
+
+    def close(self):
+        pass
+
+
+class PixelUnshuffleLayer:
+    """Lossless downsampling between two layers (pcnn_pixel_unshuffle_nhwc_bf16), as F.pixel_unshuffle(x, r): x and dx dense bf16
+    [N][H][W][C] with H and W multiples of r, y and dy dense [N][H / r][W / r][C r^2].  It keeps no state; info is its partition
+    (pixel_shuffle_info).  The backward is the shuffle of dy."""
+
+    def __init__(self, engine, N, H, W, C, r):
+        self.engine = engine
+        self.shape = (int(N), int(H), int(W), int(C), int(r))
+        self.info = pixel_shuffle_info(*self.shape, unshuffle=True)
+        pixel_shuffle_info(N, H // r, W // r, C, r)                    # the backward's shape
+        self.out_shape = (int(N), int(H) // int(r), int(W) // int(r), int(C) * int(r) * int(r))
+
+    def forward(self, x, y):
+        self.engine.pixel_unshuffle(x, y, *self.shape)
+
+    def backward(self, dy, dx):
+        N, H, W, C, r = self.shape
+        self.engine.pixel_shuffle(dy, dx, N, H // r, W // r, C, r)
+
+    def close(self):
+        pass
+
+
+def psnr(pred, target, data_range=1.0):
+    """Host evaluation of an image regression (not a hot path): the mean over images (the first axis) of
+    10 log10(data_range^2 / MSE_image), in float64; an image with MSE 0 scores +inf."""
+    p, t = np.asarray(pred, np.float64), np.asarray(target, np.float64)
+    if p.shape != t.shape:
+        raise PcnnError("psnr", -1, f"pred {p.shape} and target {t.shape} differ")
+    p, t = p.reshape(len(p), -1), t.reshape(len(t), -1)
+    mse = ((p - t) ** 2).mean(1)
+    with np.errstate(divide="ignore"):
+        return float(np.mean(10.0 * np.log10(float(data_range) ** 2 / mse)))
 
 
 def segmentation_scores(pred, targets, O, ignore_index=255):

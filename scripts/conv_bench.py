@@ -208,6 +208,102 @@ def run_fcn(iters):
     net.close()
 
 
+def run_pixelshuffle(name, N, H, W, C, r, iters, rounds=3):
+    """pixel shuffle of x [N][H][W][C r^2] -> [N][H r][W r][C] and the unshuffle of that fine map back, against F.pixel_shuffle /
+    F.pixel_unshuffle on the same channels-last bf16 tensors; bytes: each map read or written once"""
+    x, fine = _bf((N, H, W, C * r * r)), _bf((N, H * r, W * r, C))
+    y, u = torch.empty_like(fine), torch.empty_like(x)
+    xt, ft = x.permute(0, 3, 1, 2), fine.permute(0, 3, 1, 2)
+    F = torch.nn.functional
+    info = pkg.pixel_shuffle_info(N, H, W, C, r)
+    ours = {"shuffle": lambda: eng.pixel_shuffle(x, y, N, H, W, C, r), "unshuffle": lambda: eng.pixel_unshuffle(fine, u, N, H * r, W * r, C, r)}
+    theirs = {"shuffle": lambda: F.pixel_shuffle(xt, r), "unshuffle": lambda: F.pixel_unshuffle(ft, r)}
+    best = {}
+    for _ in range(rounds):
+        for k in ours:
+            a, b = timed(ours[k], iters), timed(theirs[k], iters)
+            o = best.get(k, (a, b))
+            best[k] = (min(a, o[0]), min(b, o[1]))
+    for k, (a, b) in best.items():
+        _line(f"pixel {k} {name} r{r}", a, b, 2 * 2 * x.numel(), N=N, path="16-byte" if info["vec"] == 8 else "scalar")
+
+
+def run_regloss(name, N, H, W, C, iters, rounds=3):
+    """the regression loss (dpred and the per-pixel loss) in both modes against torch's mse_loss / l1_loss forward plus autograd
+    backward on the same bf16 tensors; bytes: pred and target read, dpred written (bf16), the loss written (fp32)"""
+    P = N * H * W
+    pred, target = _bf((P, C)), _bf((P, C))
+    d, loss = torch.empty_like(pred), torch.empty(P, dtype=torch.float32, device="cuda")
+    pt = pred.clone().requires_grad_(True)
+    F = torch.nn.functional
+    for mode, fn in ((pkg.LOSS_MSE, F.mse_loss), (pkg.LOSS_L1, F.l1_loss)):
+        ours = lambda: eng.regression_loss_bf16(pred, target, P, C, d, loss, mode=mode)
+        theirs = lambda: torch.autograd.grad(fn(pt, target), pt)
+        best = None
+        for _ in range(rounds):
+            a, b = timed(ours, iters), timed(theirs, iters)
+            best = (a, b) if best is None else (min(a, best[0]), min(b, best[1]))
+        _line(f"regloss {name} {'mse' if mode == pkg.LOSS_MSE else 'l1'}", best[0], best[1], P * C * 2 * 3 + P * 4, N=N,
+              path="16-byte" if C % 8 == 0 else "scalar")
+
+
+def run_restorer(which, iters):
+    """one training step (forward, backward, AdamW) of ESPCNLite or DenoiseNet at N = 32, and the same network in torch eager: bf16
+    channels-last convolutions (cuDNN) with batch norm in float32 and the loss in float32, on one fixed batch"""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import restore_nets
+    d = np.load(os.path.join(ROOT, "tests", "golden", "mnist_subset.npz"))
+    cls = getattr(restore_nets, which)
+    p = cls.init_params()
+    net = cls(eng, pkg, p)
+    opt = pkg.AdamW(eng, net.layers())
+    b = pkg.ImageBatcher(eng, d["train_u8"].reshape(-1, 28, 28), d["train_labels"], cls.NB, pad=2, flip=True, C_out=8)
+    x = b.batch(0)[0]
+
+    def step():
+        net.forward(x)
+        net.backward()
+        opt.step(cls.LR)
+    ms = timed(step, iters)
+
+    F = torch.nn.functional
+    cl = torch.channels_last
+    w = {}
+    for k, v in p.items():
+        t = torch.from_numpy(v).to("cuda")
+        if k.startswith("f"):
+            t = t.permute(0, 3, 1, 2)
+        elif k == "w":
+            t = t.reshape(t.shape[0], -1)
+        w[k] = t.to(torch.bfloat16).contiguous(memory_format=cl if t.dim() == 4 else torch.contiguous_format).requires_grad_(True)
+    bns = [torch.nn.BatchNorm2d(c).cuda().to(memory_format=cl) for c in (16, 64)]
+    bn = lambda i, v: bns[i](v.float()).to(torch.bfloat16)
+    topt = torch.optim.AdamW(list(w.values()) + [q for m in bns for q in m.parameters()], lr=cls.LR)
+    xt = torch.rand(cls.NB, 8, 28, 28, device="cuda").to(torch.bfloat16).contiguous(memory_format=cl)
+    espcn = which == "ESPCNLite"
+
+    def tstep():
+        if espcn:
+            h = F.relu(F.conv2d(F.avg_pool2d(xt, 2), w["f1"], w["b1"], padding=2))
+            h = F.relu(F.conv2d(h, w["f2"], w["b2"], padding=1))
+        else:
+            xn = F.dropout(xt, cls.P_NOISE)
+            h = F.relu(bn(0, F.conv2d(xn, w["f1"], padding=1)))
+            h = F.relu(bn(1, F.conv2d(F.pixel_unshuffle(h, 2), w["f2"], padding=1)))
+        out = F.pixel_shuffle(torch.einsum("nchw,oc->nohw", h, w["w"]) + w["bw"][None, :, None, None], 2)
+        loss = (F.mse_loss if espcn else F.l1_loss)(out.float(), xt[:, :1].float())
+        topt.zero_grad(set_to_none=True)
+        loss.backward()
+        topt.step()
+    ms_torch = timed(tstep, iters)
+    gpu, power = card()
+    print(json.dumps({"case": f"{which} training step N={cls.NB}", "us": ms * 1e3, "torch_eager_us": ms_torch * 1e3,
+                      "torch_over_ours": ms_torch / ms, "gpu": gpu, "power_limit": power}), flush=True)
+    b.close()
+    opt.close()
+    net.close()
+
+
 def run_dilated(name, N, H, W, C, K, R, dil, iters):
     """the three wide passes of a "same" 3x3 layer at dilation dil (padding dil), next to cuDNN (conv2d(dilation=dil) and
     aten.convolution_backward) on the same bf16 channels-last tensors and to the same layer at dilation 1 (padding 1), all in this
@@ -2284,6 +2380,19 @@ if only == "attn":                                                     # self-at
     run_attn("non-local Res3 N32 T784 h1 d128", 32, 784, 1, 128, 20)
     run_attn("N16 T3136 h1 d64", 16, 3136, 1, 64, 10)
     run_attn("DANet N8 T4096 h1 d64", 8, 4096, 1, 64, 10)
+if only == "pixelshuffle":                                             # sub-pixel upsamplers and their inverses, torch beside them
+    run_pixelshuffle("128x128x12 -> 256x256x3", 16, 128, 128, 3, 2, 20)
+    run_pixelshuffle("64x64x48 -> 256x256x3", 16, 64, 64, 3, 4, 20)
+    run_pixelshuffle("EDSR 48x48x256 -> 96x96x64", 16, 48, 48, 64, 2, 20)
+    run_pixelshuffle("EDSR 96x96x256 -> 192x192x64", 16, 96, 96, 64, 2, 20)
+    run_pixelshuffle("28x28x256 -> 56x56x64", 128, 28, 28, 64, 2, 20)
+if only == "regloss":                                                  # MSE and L1 with their gradients, torch beside them
+    run_regloss("16x256x256x3", 16, 256, 256, 3, 20)
+    run_regloss("16x192x192x64", 16, 192, 192, 64, 20)
+if only == "espcn":
+    run_restorer("ESPCNLite", 20)
+if only == "denoise":
+    run_restorer("DenoiseNet", 20)
 eng.close()
 if only == "wprobe":                                                   # what a pure WRITE stream / pure READ stream / copy reach on this GPU
     # library fill / reduce / copy kernels as a yardstick for the store-dominated forward pass (807 MB written, 39 MB read):
