@@ -1253,6 +1253,75 @@ int pcnn_pixel_unshuffle_nhwc_bf16(pcnn_ctx *ctx, const void *x_bf16_dev, void *
 #define PCNN_LOSS_L1 1
 int pcnn_regression_loss_bf16(pcnn_ctx *ctx, const void *pred_bf16_dev, const void *target_bf16_dev, int target_stride, int pixels, int C,
                               int mode, float scale, void *dpred_bf16_dev, float *loss_f32_dev);
+/* ------------------------------------------------------------------ variational autoencoders
+ * Two more replayable fp32 functions (csrc/pcnn_internal.h), in exp_f32's style: a fixed sequence of round-to-nearest operations
+ * with no contraction (RN below), every constant given by its bits, so a numpy float32 replay gives the same bits.
+ *   L(e) = log1p_f32(e), log(1 + e) for -1 < e <= 1:
+ *     u = RN(1 + e); c = RN(e - RN(u - 1)) (exactly the rounding error of u: both subtractions are exact);
+ *     u = 2^k m with m in [sqrt(1/2), sqrt(2)): i = bits(u) + 0x3F800000 - 0x3F3504F3, k = (i >> 23) - 127, m = the float with bits
+ *       (i & 0x7FFFFF) + 0x3F3504F3; f = RN(m - 1) (exact);
+ *     s = RN(f / RN(2 + f)), z = RN(s s), w = RN(z z); R = RN(RN(z RN(g1 + RN(w g3))) + RN(w RN(g2 + RN(w g4)))), g1 = 0x3F2AAAAA,
+ *       g2 = 0x3ECCCCE1, g3 = 0x3E91E9EE, g4 = 0x3E789E26 (fdlibm's logf series in s = f / (2 + f));
+ *     hfsq = RN(RN(0.5 f) f); lo = RN(RN(k ln2_lo) + RN(c / u)), ln2_hi = 0x3F317180, ln2_lo = 0x3717F7D1;
+ *     L = RN(RN(RN(RN(RN(s RN(hfsq + R)) + lo) - hfsq) + f) + RN(k ln2_hi)).
+ *   Its error is at most 0.92 ulp of log1p(e) (measured 0.8684 exhaustively over the 2^24 Box-Muller inputs e = u1 - 1 below, and
+ *   0.9154 exhaustively over [2^-30, 1], the largest in [1/4, 1/2); below 2^-30 the result is e within 0.02 ulp).  L(0) = +0.
+ *   (sin, cos) = sincos_2pi_f32(k), sin and cos of 2 pi k 2^-24 for integer 0 <= k < 2^24:
+ *     octant o = k >> 21, j = k & (2^21 - 1); t = RN(j' 2^-21) with j' = j (o even) or 2^21 - j (o odd): exact, 0 <= t <= 1;
+ *     z = RN(t t); S = RN(t P), P = Horner in z of s4 .. s0, each step RN(RN(p z) + s_i), s0 = 0x3F490FDB, s1 = 0xBDA55DE7,
+ *       s2 = 0x3B2335DE, s3 = 0xB81965B4, s4 = 0x34A60075; C = Horner in z of c5 .. c0, c0 = 1, c1 = 0xBE9DE9E6, c2 = 0x3C81E0F8,
+ *       c3 = 0xB9AAE9DE, c4 = 0x3670F449, c5 = 0xB2D08CC9 (least-squares fits of sin(pi t / 4) / t and cos(pi t / 4) on [0, 1]);
+ *     (sin, cos) = o 0: (S, C), 1: (C, S), 2: (C, -S), 3: (S, -C), 4: (-S, -C), 5: (-C, -S), 6: (-C, S), 7: (-S, C).
+ *   Each is within 1.72 ulp of the exact value (measured 1.7154 for both over all 2^24 inputs; exact zeros come out as zeros).
+ * Gaussian latent (csrc/gaussian_latent.cu): the reparameterization z = mu + exp(lv / 2) eps of a VAE's encoder output, with each
+ * row's KL divergence from N(0, I).
+ *   - Layout: stats is bf16 [R][ld], mu in columns 0 .. L-1 and the log-variance lv in L .. 2L-1 (a LinearLayer with O = 2L, read in
+ *     place; a spatial latent of L channels per pixel is R = N h w rows).  z is bf16 [R][ldz]; kl fp32 [R] or NULL.  Columns 2L ..
+ *     ld-1 of stats and L .. ldz-1 of z are never read or written.
+ *   - eps[r][j]: element i = r L + j (64-bit) is normal i & 3 of the Philox4x32-10 block at counter (q lo, 0xE0000000 | q hi, call
+ *     lo, call hi), q = i >> 2, key (seed lo, seed hi).  A block's words (w0, w1, w2, w3) give normals 0, 1 from the pair (w0, w1) and
+ *     2, 3 from (w2, w3) by Box-Muller: u1 = RN(((wa >> 8) + 1) 2^-24) (in (0, 1], exact), rad = sqrt_rn(RN(-2 L(RN(u1 - 1)))),
+ *     (sn, cs) = sincos_2pi_f32(wb >> 8); normal 2p = RN(rad cs), 2p + 1 = RN(rad sn).
+ *     Domain: word 1 of a latent counter has top byte 0xE0 (q < 2^41 for every allowed shape).  A dropout counter has it below 0x40
+ *     (q < 2^62), a crop counter in 0x80 .. 0xBF, a permutation round 0xC0, a box counter 0xC8 .. 0xCD and a trivial-augment counter
+ *     0xD0 .. 0xD6, so no latent draw coincides with any other draw of the library for any seed, call or epoch.
+ *   - Forward, training 1: z = bf16_rn(RN(mu + RN(E(RN(0.5 lv)) eps))); training 0: z = mu (bit copy, no draw).  mu = lv = 0 gives
+ *     z = bf16_rn(eps) (with eps = -0 written as +0), so the same call samples the prior.
+ *     kl[r] = RN(0.5 S), S the fp32 sum from +0 in ascending j of RN(RN(RN(RN(mu mu) + E(lv)) - 1) - lv); written in both modes.
+ *   - Backward (of a training forward with the same seed and call; nothing is stored, eps is drawn again): with g = float(dz) and
+ *     ks = kl_scale (beta / N for a batch mean of beta KL),
+ *       dmu = bf16_rn(RN(g + RN(ks mu))),
+ *       dlv = bf16_rn(RN(RN(RN(RN(0.5 g) eps) E(RN(0.5 lv))) + RN(RN(ks 0.5) RN(E(lv) - 1))))
+ *     into dstats [R][ld] at the columns of mu and lv.
+ *   - A row's bits depend only on (seed, call, r, L): no atomics, no dependence on the grid.  16-byte accesses when L, ld and ldz are
+ *     multiples of 8, single elements otherwise.
+ * Domain (PCNN_ERR_ARG, one message per rule): no NULL context, stats, z (dz, dstats); R >= 1; 1 <= L <= 4096; ld >= 2L; ldz >= L;
+ * training 0 or 1; call >= 1 for a training forward and for the backward; kl_scale finite; every pointer 16-byte aligned; z == stats
+ * with ldz == ld (in place) or z sharing no byte with stats; kl sharing none with stats or z; dstats == stats (in place) or sharing
+ * no byte with it; dstats sharing none with dz.  pcnn_gaussian_latent_info (host only) refuses the shape rules as the calls do and
+ * fills out6 = { elements per thread (8 or 1), grid, threads per CTA, shared bytes per CTA, rows per CTA, columns per pass }. */
+int pcnn_gaussian_latent_info(int R, int L, int ld, int ldz, long long *out6);
+int pcnn_gaussian_latent_bf16_fwd(pcnn_ctx *ctx, const void *stats_bf16_dev, int ld, void *z_bf16_dev, int ldz, float *kl_f32_dev, int R,
+                                  int L, unsigned long long seed, unsigned long long call, int training);
+int pcnn_gaussian_latent_bf16_bwd(pcnn_ctx *ctx, const void *stats_bf16_dev, int ld, const void *dz_bf16_dev, int ldz, void *dstats_bf16_dev,
+                                  int R, int L, unsigned long long seed, unsigned long long call, float kl_scale);
+/* Binary cross-entropy with logits (csrc/regress_loss.cu): F.binary_cross_entropy_with_logits of bf16 logits [pixels][C] against
+ * the first C channels of bf16 targets [pixels][target_stride], probabilities in [0, 1] (soft targets allowed).  Per element, with
+ * x = float(logit), t = float(target), e = E(-|x|):
+ *     term = RN(RN((x > 0 ? x : +0) - RN(x t)) + L(e)),
+ *     sigma = RN((x >= 0 ? 1 : e) / RN(1 + e)),  dlogits = bf16_rn(RN(scale RN(sigma - t)));
+ *     loss[px] = the fp32 sum from +0, in ascending c, of the pixel's terms (unscaled; NULL allowed); scale = 1 / (pixels C) makes
+ *     dlogits the gradient of reduction="mean".
+ * Special values, against torch's float64 binary_cross_entropy_with_logits and its autograd (sigmoid(x) - t): every finite x gives
+ * a finite term and gradient, and |x| > 103.97 gives e = 0, sigma exactly 0 or 1 and the softplus term 0.  A NaN x or t gives NaN
+ * in both.  x = +Inf: dlogits = bf16_rn(RN(scale (1 - t))) and x = -Inf: bf16_rn(RN(scale (0 - t))), as torch; the term is NaN at
+ * x = +Inf (torch: +Inf for t < 1, NaN at t = 1) and at x = -Inf, t = 0 (torch: NaN), +Inf at x = -Inf, t > 0 (torch: NaN).
+ * No cross-CTA reduction and no atomics; the 16-byte path runs when C and target_stride are multiples of 8.
+ * Domain (PCNN_ERR_ARG, one message per rule): no NULL context, logits, target or dlogits; pixels >= 1; 1 <= C <= target_stride;
+ * scale finite; every pointer 16-byte aligned; dlogits == logits (in place) is allowed, any other overlap of dlogits or loss with
+ * logits, target or each other is not. */
+int pcnn_bce_logits_bf16(pcnn_ctx *ctx, const void *logits_bf16_dev, const void *target_bf16_dev, int target_stride, int pixels, int C,
+                         float scale, void *dlogits_bf16_dev, float *loss_f32_dev);
 /* Optimizers for device-trained layers (csrc/optim.cu): one fused update of every parameter tensor of a network per step, as
  * torch.optim.SGD and torch.optim.AdamW (decoupled weight decay) in their single-tensor form, with the bf16 operands of the plans
  * the parameters belong to refreshed in the same pass.

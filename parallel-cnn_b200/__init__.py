@@ -16,7 +16,7 @@ from ._lib import (  # noqa: F401
     groupnorm_nhwc_info, attention_info,
     linear_info, dwconv_info, gconv_info, se_scale_nhwc_info, dropout_info, augment_info, augment_resized_info, RESIZE_TRAIN, RESIZE_EVAL, OPTIM_SGD, OPTIM_ADAMW,
     augment_trivial_info, TRIVIAL_NONE, TRIVIAL_NEAREST, TRIVIAL_BILINEAR, TRIVIAL_OPS, conv_transpose_info, upsample_bilinear_info,
-    pixel_shuffle_info, LOSS_MSE, LOSS_L1,
+    pixel_shuffle_info, LOSS_MSE, LOSS_L1, gaussian_latent_info,
 )
 from .engine import AvgPoolLayer, BatchNormLayer, GroupNormLayer, ConvLayer, GlobalAvgPoolLayer, ConvPlan, LinearLayer, LinearPlan, MaxPoolLayer, DeviceArray, WideConvPlan, Engine, bf16_bits_to_f32, f32_to_bf16_bits  # noqa: F401
 from .engine import DepthwiseConvLayer, DepthwiseConvPlan, DropoutLayer, GroupedConvLayer, GroupedConvPlan, SqueezeExcitationLayer  # noqa: F401
@@ -25,6 +25,7 @@ from .engine import SGD, AdamW, FusedOptimizer  # noqa: F401
 from .engine import ConvTransposeLayer, UpsampleBilinearLayer, segmentation_scores  # noqa: F401
 from .engine import SelfAttentionLayer  # noqa: F401
 from .engine import PixelShuffleLayer, PixelUnshuffleLayer, psnr  # noqa: F401
+from .engine import GaussianLatentLayer  # noqa: F401
 
 __all__ = ["Engine", "DeviceArray", "PcnnError", "lib", "declared_symbols", "init_params_reference",
            "mnist_load_u8", "conv_tc_plan_info", "conv_wide_plan_info", "conv_wide_bwd_info", "conv_bwd_plan_info", "conv_layer_family", "maxpool_nhwc_info", "avgpool_nhwc_info", "global_avgpool_nhwc_info", "batchnorm_nhwc_info", "linear_info", "ConvLayer", "BatchNormLayer", "MaxPoolLayer", "AvgPoolLayer", "GlobalAvgPoolLayer", "LinearLayer", "ConvPlan", "LinearPlan",
@@ -36,4 +37,5 @@ __all__ = ["Engine", "DeviceArray", "PcnnError", "lib", "declared_symbols", "ini
            "MixedLabels", "MIX_MIXUP", "MIX_CUTMIX", "mix_draws", "augment_trivial_info", "TRIVIAL_NONE", "TRIVIAL_NEAREST",
            "TRIVIAL_BILINEAR", "TRIVIAL_OPS", "conv_transpose_info", "upsample_bilinear_info", "ConvTransposeLayer",
            "UpsampleBilinearLayer", "segmentation_scores", "groupnorm_nhwc_info", "GroupNormLayer", "attention_info", "SelfAttentionLayer",
-           "pixel_shuffle_info", "LOSS_MSE", "LOSS_L1", "PixelShuffleLayer", "PixelUnshuffleLayer", "psnr"]
+           "pixel_shuffle_info", "LOSS_MSE", "LOSS_L1", "PixelShuffleLayer", "PixelUnshuffleLayer", "psnr",
+           "gaussian_latent_info", "GaussianLatentLayer"]

@@ -225,6 +225,10 @@ _SIG = {
     "pcnn_pixel_shuffle_nhwc_bf16": [_vp, _vp, _vp] + [_i] * 5,
     "pcnn_pixel_unshuffle_nhwc_bf16": [_vp, _vp, _vp] + [_i] * 5,
     "pcnn_regression_loss_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _f, _vp, _vp],
+    "pcnn_gaussian_latent_info": [_i] * 4 + [_vp],
+    "pcnn_gaussian_latent_bf16_fwd": [_vp, _vp, _i, _vp, _i, _vp, _i, _i, C.c_ulonglong, C.c_ulonglong, _i],
+    "pcnn_gaussian_latent_bf16_bwd": [_vp, _vp, _i, _vp, _i, _vp, _i, _i, C.c_ulonglong, C.c_ulonglong, _f],
+    "pcnn_bce_logits_bf16": [_vp, _vp, _vp, _i, _i, _i, _f, _vp, _vp],
     "pcnn_optim_create": [_vp, _vp, _vp, _i, _pvp],
     "pcnn_optim_step": [_vp, _vp, _f],
     "pcnn_optim_state": [_vp, _i, _pvp, _pvp],
@@ -351,6 +355,17 @@ def pixel_shuffle_info(N, H, W, C, r, unshuffle=False):
     out = (_ll * 6)()
     check("pcnn_pixel_shuffle_info", lib().pcnn_pixel_shuffle_info(int(N), int(H), int(W), int(C), int(r), int(bool(unshuffle)), out))
     return dict(vec=out[0], grid=out[1], threads=out[2], smem=out[3], tile_pixels=out[4], chunk_channels=out[5])
+
+
+def gaussian_latent_info(R, L, ld=None, ldz=None):
+    """How the Gaussian latent (stats [R][ld] -> z [R][ldz], ld None = 2L, ldz None = L) partitions a shape
+    (pcnn_gaussian_latent_info; host only, no GPU), refused as the calls refuse.  vec: elements per thread (8 or 1); each CTA of
+    threads takes tile_rows rows, chunk_columns columns per pass through smem bytes of KL terms."""
+    out = (_ll * 6)()
+    ld = 2 * int(L) if ld is None else int(ld)
+    ldz = int(L) if ldz is None else int(ldz)
+    check("pcnn_gaussian_latent_info", lib().pcnn_gaussian_latent_info(int(R), int(L), ld, ldz, out))
+    return dict(vec=out[0], grid=out[1], threads=out[2], smem=out[3], tile_rows=out[4], chunk_columns=out[5])
 
 
 def conv_layer_family(N, H, W, C, K, R, S, stride=1, padding=(0, 0), row_pitch=None, image_rows=0, dilation=(1, 1)):

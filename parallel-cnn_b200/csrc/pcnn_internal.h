@@ -326,6 +326,49 @@ __device__ __forceinline__ float exp_f32(float x) {
     const int ki = __float2int_rn(k), k1 = ki >> 1, k2 = ki - k1;      // a NaN x gives ki = 0 and p = NaN
     return __fmul_rn(__fmul_rn(p, __int_as_float((k1 + 127) << 23)), __int_as_float((k2 + 127) << 23));
 }
+// log1p(e) for e in (-1, 1], replayable like exp_f32 (include/pcnn.h states the sequence; max error 0.92 ulp).  u = RN(1 + e)
+// and its rounding error c = e - (u - 1), which both subtractions give exactly; u = 2^k m with m in [sqrt(1/2), sqrt(2)) from the
+// bits, so f = m - 1 is exact; log1p(f) by fdlibm's s = f / (2 + f) series; c / u is the first-order correction for 1 + e != u.
+// One function serves both the Box-Muller radius (e = u1 - 1, exact) and the softplus of the logit losses (e = E(-|x|) in [0, 1]).
+__device__ __forceinline__ float log1p_f32(float e) {
+    const float u = __fadd_rn(1.0f, e);
+    const float c = __fsub_rn(e, __fsub_rn(u, 1.0f));
+    const int ix = __float_as_int(u) + (0x3F800000 - 0x3F3504F3);
+    const float k = (float)((ix >> 23) - 0x7F);
+    const float f = __fsub_rn(__int_as_float((ix & 0x7FFFFF) + 0x3F3504F3), 1.0f);
+    const float s = __fdiv_rn(f, __fadd_rn(2.0f, f));
+    const float z = __fmul_rn(s, s), w = __fmul_rn(z, z);
+    const float t1 = __fmul_rn(w, __fadd_rn(__int_as_float(0x3ECCCCE1), __fmul_rn(w, __int_as_float(0x3E789E26))));
+    const float t2 = __fmul_rn(z, __fadd_rn(__int_as_float(0x3F2AAAAA), __fmul_rn(w, __int_as_float(0x3E91E9EE))));
+    const float hfsq = __fmul_rn(__fmul_rn(0.5f, f), f);
+    const float lo = __fadd_rn(__fmul_rn(k, __int_as_float(0x3717F7D1)), __fdiv_rn(c, u));
+    const float v = __fadd_rn(__fsub_rn(__fadd_rn(__fmul_rn(s, __fadd_rn(hfsq, __fadd_rn(t2, t1))), lo), hfsq), f);
+    return __fadd_rn(v, __fmul_rn(k, __int_as_float(0x3F317180)));
+}
+// sin and cos of 2 pi k 2^-24 for integer 0 <= k < 2^24, replayable (include/pcnn.h; max error 1.72 ulp).  The octant k >> 21
+// and the position in it are exact integers, so the only reduction is a reflection t -> 1 - t in odd octants; then sin(pi t / 4)
+// = t S(t^2) and cos(pi t / 4) = C(t^2) on 0 <= t <= 1, and the octant swaps and negates them.
+__device__ __forceinline__ void sincos_2pi_f32(unsigned k, float *sn, float *cs) {
+    const unsigned o = k >> 21, j = k & 0x1FFFFFu;
+    const float t = __fmul_rn((float)((o & 1) ? 0x200000u - j : j), __int_as_float(0x35000000));   // 2^-21
+    const float z = __fmul_rn(t, t);
+    float p = __int_as_float(0x34A60075);
+    p = __fadd_rn(__fmul_rn(p, z), __int_as_float(0xB81965B4));
+    p = __fadd_rn(__fmul_rn(p, z), __int_as_float(0x3B2335DE));
+    p = __fadd_rn(__fmul_rn(p, z), __int_as_float(0xBDA55DE7));
+    p = __fadd_rn(__fmul_rn(p, z), __int_as_float(0x3F490FDB));
+    const float S = __fmul_rn(t, p);
+    float q = __int_as_float(0xB2D08CC9);
+    q = __fadd_rn(__fmul_rn(q, z), __int_as_float(0x3670F449));
+    q = __fadd_rn(__fmul_rn(q, z), __int_as_float(0xB9AAE9DE));
+    q = __fadd_rn(__fmul_rn(q, z), __int_as_float(0x3C81E0F8));
+    q = __fadd_rn(__fmul_rn(q, z), __int_as_float(0xBE9DE9E6));
+    const float C = __fadd_rn(__fmul_rn(q, z), 1.0f);
+    const bool swap = ((o + 1) >> 1) & 1;                    // octants 1, 2, 5, 6
+    const float a = swap ? C : S, b = swap ? S : C;
+    *sn = o >= 4 ? -a : a;
+    *cs = (o >= 2 && o <= 5) ? -b : b;
+}
 #endif
 // conv_wgrad_tc.cu: dw[o] = sum over i of slots[i][o] for o < nout, in a fixed order (deterministic, no atomics)
 int pcnn_conv_wgrad_reduce_slots(pcnn_ctx *ctx, const float *slots, float *dw, int nslots, int nout);

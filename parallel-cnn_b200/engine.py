@@ -9,7 +9,7 @@ import numpy as np
 from ._lib import (F32, NPARAM, OPTIM_ADAMW, OPTIM_SGD, TEST_SET, TRAIN_SET, U8, OptimConfig, OptimTensor, PcnnError, augment_info,
                    augment_resized_info, RESIZE_TRAIN, RESIZE_EVAL, augment_trivial_info, TRIVIAL_NONE, TRIVIAL_NEAREST, TRIVIAL_BILINEAR,
                    attention_info, avgpool_nhwc_info, batchnorm_nhwc_info, channel_stats, check, conv_layer_family, conv_transpose_info, upsample_bilinear_info, dropout_info, dwconv_info, gconv_info, global_avgpool_nhwc_info, groupnorm_nhwc_info, lib,
-                   linear_info, maxpool_nhwc_info, pixel_shuffle_info, LOSS_MSE,
+                   linear_info, maxpool_nhwc_info, pixel_shuffle_info, LOSS_MSE, gaussian_latent_info,
                    se_scale_nhwc_info, ACT_RELU, ACT_SIGMOID, ACT_SILU, ACT_HARDSWISH, ACT_RELU6)
 
 PREACT_CODES = (ACT_SILU, ACT_HARDSWISH, ACT_RELU6)   # the normalizations' codes whose backward recomputes the pre-activation
@@ -599,6 +599,34 @@ class Engine:
         self._call("pcnn_regression_loss_bf16", _p(pred), _p(target), ts, int(pixels), int(C), int(mode), float(scale), _p(dpred),
                    _p(loss))
 
+    def bce_logits_loss_bf16(self, logits, target, pixels, C, dlogits, loss=None, target_stride=None, scale=None):
+        """pcnn_bce_logits_bf16: binary_cross_entropy_with_logits of bf16 logits [pixels][C] against the first C channels of bf16
+        probabilities target [pixels][target_stride] (None = C).  dlogits (may be logits) receives scale (sigmoid(x) - t), scale None =
+        1 / (pixels C), the gradient of reduction="mean"; loss (fp32 [pixels] or None) the unscaled sum of each pixel's terms."""
+        ts = int(C) if target_stride is None else int(target_stride)
+        if scale is None:
+            n = int(pixels) * int(C)
+            scale = 1.0 / n if n > 0 else 1.0             # n <= 0: a shape the call refuses
+        self._call("pcnn_bce_logits_bf16", _p(logits), _p(target), ts, int(pixels), int(C), float(scale), _p(dlogits), _p(loss))
+
+    def gaussian_latent_fwd(self, stats, z, R, L, seed, call, kl=None, training=True, ld=None, ldz=None):
+        """pcnn_gaussian_latent_bf16_fwd: z [R][ldz] = mu + exp(lv / 2) eps (training) or mu (eval) from stats [R][ld] (mu in
+        columns 0 .. L-1, lv in L .. 2L-1; ld None = 2L, ldz None = L), eps the Philox normals of (seed, call); kl (fp32 [R] or
+        None) each row's KL divergence from N(0, I).  z may be stats when ldz == ld."""
+        ld = 2 * int(L) if ld is None else int(ld)
+        ldz = int(L) if ldz is None else int(ldz)
+        self._call("pcnn_gaussian_latent_bf16_fwd", _p(stats), ld, _p(z), ldz, _p(kl), int(R), int(L), int(seed), int(call),
+                   int(bool(training)))
+
+    def gaussian_latent_bwd(self, stats, dz, dstats, R, L, seed, call, kl_scale, ld=None, ldz=None):
+        """pcnn_gaussian_latent_bf16_bwd: dstats [R][ld] (may be stats) = (dz + kl_scale mu, dz eps exp(lv / 2) / 2 + kl_scale
+        (exp(lv) - 1) / 2), eps drawn again from the training forward's (seed, call); kl_scale weighs the KL term (beta / N for
+        the batch mean)."""
+        ld = 2 * int(L) if ld is None else int(ld)
+        ldz = int(L) if ldz is None else int(ldz)
+        self._call("pcnn_gaussian_latent_bf16_bwd", _p(stats), ld, _p(dz), ldz, _p(dstats), int(R), int(L), int(seed), int(call),
+                   float(kl_scale))
+
     def augment_mask(self, masks, n, H, W, first, N, masks_out, shuffle=1, pad=0, flip=0, seed=0, epoch=0, mask_fill=255):
         """pcnn_augment_mask_u8: the uint8 masks [n][H][W] of augment's batch with the same arguments, each permuted, cropped and
         flipped exactly as its image, the padding filled with mask_fill, into masks_out [N][H][W]"""
@@ -1078,6 +1106,53 @@ class PixelUnshuffleLayer:
 
     def close(self):
         pass
+
+
+class GaussianLatentLayer:
+    """The reparameterized latent of a variational autoencoder (pcnn_gaussian_latent_bf16_fwd / _bwd): stats [R][ld] bf16 holds mu in
+    columns 0 .. L-1 and the log-variance in L .. 2L-1 (an encoder LinearLayer with O = 2L; ld None = 2L), z [R][ldz] (None = L)
+    is mu + exp(lv / 2) eps.  kl (a DeviceArray of R floats) receives each row's KL divergence from N(0, I) at every forward.  It
+    has no parameters, so no optim_tensors.
+
+    eps is the Philox draw of (seed, call) at each element, call being incremented by every training forward; `call` is a plain
+    attribute, so a checkpoint can save and restore it.  backward replays the eps of the most recent training forward:
+
+        enc.forward(h, stats);  lat.forward(stats, z);  dec.forward(z, y)
+        dec.backward(y, dy, dz);  lat.backward(dz, dstats, beta / N);  enc.backward(stats, dstats, dh)
+
+    dstats may be stats itself when the encoder's backward does not read its output (no activation)."""
+
+    def __init__(self, engine, R, L, seed, ld=None, ldz=None):
+        self.engine = engine
+        self.R, self.L = int(R), int(L)
+        self.ld = 2 * self.L if ld is None else int(ld)
+        self.ldz = self.L if ldz is None else int(ldz)
+        self.info = gaussian_latent_info(self.R, self.L, self.ld, self.ldz)
+        self.seed = int(seed)
+        self.call = 0
+        self.kl = engine.array((self.R,), np.float32)
+        self._stats = None
+
+    def forward(self, stats, z, training=True):
+        """training: call += 1, then z = mu + exp(lv / 2) eps with this call's draw; eval: z = mu.  kl is written in both."""
+        if training:
+            self.call += 1
+            self._stats = stats
+        self.engine.gaussian_latent_fwd(stats, z, self.R, self.L, self.seed, self.call, kl=self.kl, training=training, ld=self.ld,
+                                        ldz=self.ldz)
+
+    def backward(self, dz, dstats, kl_scale):
+        """dstats = the gradient of (the loss behind dz) + kl_scale sum(kl) with respect to the stats of the most recent training
+        forward, which must still hold them; dstats may be that buffer (in place)."""
+        if self._stats is None:
+            raise PcnnError("GaussianLatentLayer.backward", -1, "no training forward to differentiate")
+        self.engine.gaussian_latent_bwd(self._stats, dz, dstats, self.R, self.L, self.seed, self.call, kl_scale, ld=self.ld,
+                                        ldz=self.ldz)
+
+    def close(self):
+        if self.kl is not None:
+            self.kl.free()
+            self.kl = None
 
 
 def psnr(pred, target, data_range=1.0):

@@ -247,6 +247,106 @@ def run_regloss(name, N, H, W, C, iters, rounds=3):
               path="16-byte" if C % 8 == 0 else "scalar")
 
 
+def run_latent(name, R, L, iters, rounds=3):
+    """the Gaussian latent forward (z and kl) and backward (dstats) against torch eager mu + exp(0.5 lv) randn_like with the KL
+    and its autograd, on the same bf16 stats; bytes: stats read, z written, kl written (forward); stats and dz read, dstats written
+    (backward).  The kernels also run Philox, a log, a sine and cosine, a square root and two exponentials per element, so they may
+    be bound by issue rather than by HBM."""
+    stats, dz = _bf((R, 2 * L)), _bf((R, L), 0.1)
+    z, ds, kl = torch.empty((R, L), dtype=torch.bfloat16, device="cuda"), torch.empty_like(stats), torch.empty(R, device="cuda")
+    st = stats.clone().requires_grad_(True)
+
+    def theirs():
+        mu, lv = st[:, :L], st[:, L:]
+        zt = mu + torch.exp(0.5 * lv) * torch.randn_like(mu)
+        klt = 0.5 * (mu.float() ** 2 + torch.exp(lv.float()) - 1 - lv.float()).sum(1)
+        torch.autograd.grad((zt, klt.sum() / R), st, (dz, None))
+    info = pkg.gaussian_latent_info(R, L)
+    best = None
+    for _ in range(rounds):
+        a = timed(lambda: eng.gaussian_latent_fwd(stats, z, R, L, 1, 1, kl=kl), iters)
+        b = timed(lambda: eng.gaussian_latent_bwd(stats, dz, ds, R, L, 1, 1, 1.0 / R), iters)
+        c = timed(theirs, iters)
+        best = (a, b, c) if best is None else tuple(min(u, v) for u, v in zip(best, (a, b, c)))
+    a, b, c = best
+    n = R * L
+    _line(f"latent {name} fwd+bwd", a + b, c, n * 16 + R * 4, R=R, L=L,
+          path="16-byte" if info["vec"] == 8 else "scalar", fwd_us=a * 1e3, bwd_us=b * 1e3,
+          fwd_hbm_frac=(n * 6 + R * 4) / (a * 1e-3) / 1e9 / HBM, bwd_hbm_frac=(n * 10) / (b * 1e-3) / 1e9 / HBM)
+
+
+def run_bce(name, P, C, ts, iters, rounds=3):
+    """the binary cross-entropy with logits (dlogits and the per-pixel loss) against F.binary_cross_entropy_with_logits forward plus
+    autograd on the same bf16 tensors; bytes: logits and the C target channels read, dlogits written (bf16), the loss (fp32)"""
+    x, t = _bf((P, C), 4.0), torch.rand((P, ts), device="cuda").to(torch.bfloat16)
+    d, loss = torch.empty_like(x), torch.empty(P, dtype=torch.float32, device="cuda")
+    xt, tt = x.clone().requires_grad_(True), t[:, :C]
+    F = torch.nn.functional
+    best = None
+    for _ in range(rounds):
+        a = timed(lambda: eng.bce_logits_loss_bf16(x, t, P, C, d, loss, target_stride=ts), iters)
+        b = timed(lambda: torch.autograd.grad(F.binary_cross_entropy_with_logits(xt, tt), xt), iters)
+        best = (a, b) if best is None else (min(a, best[0]), min(b, best[1]))
+    _line(f"bce {name}", best[0], best[1], P * C * 2 * 3 + P * 4, P=P, C=C, target_stride=ts,
+          path="16-byte" if C % 8 == 0 and ts % 8 == 0 else "scalar")
+
+
+def run_vae(iters):
+    """one ConvVAE training step (forward, backward, AdamW) at N = 32, and the same network in torch eager: bf16 channels-last
+    convolutions (cuDNN), the latent and the loss in float32, on one fixed batch"""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import vae_nets
+    d = np.load(os.path.join(ROOT, "tests", "golden", "mnist_subset.npz"))
+    cls = vae_nets.ConvVAE
+    B, L = cls.NB, cls.L
+    p = cls.init_params()
+    net = cls(eng, pkg, p)
+    opt = pkg.AdamW(eng, net.layers())
+    b = pkg.ImageBatcher(eng, d["train_u8"].reshape(-1, 28, 28), d["train_labels"], B, pad=2, flip=True, C_out=8)
+    x = b.batch(0)[0]
+
+    def step():
+        net.forward(x)
+        net.backward()
+        opt.step(cls.LR)
+    ms = timed(step, iters)
+    F = torch.nn.functional
+    cl = torch.channels_last
+    w = {}
+    for k, v in p.items():
+        t = torch.from_numpy(v).to("cuda")
+        if k in ("f1", "f2"):
+            t = t.permute(0, 3, 1, 2)
+        elif k in ("we", "wd", "w"):
+            t = t.reshape(t.shape[0], -1)
+        w[k] = t.to(torch.bfloat16).contiguous(memory_format=cl if t.dim() == 4 else torch.contiguous_format).requires_grad_(True)
+    topt = torch.optim.AdamW(list(w.values()), lr=cls.LR)
+    xt = torch.rand(B, 8, 28, 28, device="cuda").to(torch.bfloat16).contiguous(memory_format=cl)
+
+    def tstep():
+        h = F.relu(F.conv2d(xt, w["f1"], w["b1"], stride=2, padding=1))
+        h = F.relu(F.conv2d(h, w["f2"], w["b2"], stride=2, padding=1))
+        st = (h.permute(0, 2, 3, 1).reshape(B, -1) @ w["we"].t() + w["be"]).float()
+        mu, lv = st[:, :L], st[:, L:]
+        z = (mu + torch.exp(0.5 * lv) * torch.randn_like(mu)).to(torch.bfloat16)
+        kl = 0.5 * (mu * mu + torch.exp(lv) - 1 - lv).sum(1)
+        g = F.relu(z @ w["wd"].t() + w["bd"]).reshape(B, 4, 4, 16).permute(0, 3, 1, 2)
+        g = F.relu(F.conv_transpose2d(g, w["t1"], w["tb1"], stride=2, padding=1))
+        g = F.relu(F.conv_transpose2d(g, w["t2"], w["tb2"], stride=2, padding=1, output_padding=1))
+        logits = F.pixel_shuffle(torch.einsum("nchw,oc->nohw", g, w["w"]) + w["bw"][None, :, None, None], 2)
+        loss = (F.binary_cross_entropy_with_logits(logits.float(), xt[:, :1].float(), reduction="sum") + kl.sum()) / B
+        topt.zero_grad(set_to_none=True)
+        loss.backward()
+        topt.step()
+    ms_torch = timed(tstep, iters)
+    gpu, power = card()
+    print(json.dumps({"case": f"ConvVAE training step N={B}", "us": ms * 1e3, "torch_eager_us": ms_torch * 1e3,
+                      "torch_over_ours": ms_torch / ms, "gpu": gpu, "power_limit": power}), flush=True)
+    b.close()
+    opt.close()
+    net.close()
+
+
 def run_restorer(which, iters):
     """one training step (forward, backward, AdamW) of ESPCNLite or DenoiseNet at N = 32, and the same network in torch eager: bf16
     channels-last convolutions (cuDNN) with batch norm in float32 and the loss in float32, on one fixed batch"""
@@ -2389,6 +2489,15 @@ if only == "pixelshuffle":                                             # sub-pix
 if only == "regloss":                                                  # MSE and L1 with their gradients, torch beside them
     run_regloss("16x256x256x3", 16, 256, 256, 3, 20)
     run_regloss("16x192x192x64", 16, 192, 192, 64, 20)
+if only == "latent":                                                   # the VAE latent: a dense head, a spatial latent, a wide one
+    for name, R, L in (("fc 65536x128", 65536, 128), ("spatial 16x256x256x4", 16 * 256 * 256, 4), ("fc 8192x1024", 8192, 1024)):
+        run_latent(name, R, L, 20)
+if only == "bce":                                                      # ConvVAE's head, a segmentation head, a multi-label head
+    run_bce("128x784x1 ts8", 128 * 784, 1, 8, 20)
+    run_bce("16x256x256x8", 16 * 256 * 256, 8, 8, 20)
+    run_bce("65536x80", 65536, 80, 80, 20)
+if only == "vae":
+    run_vae(20)
 if only == "espcn":
     run_restorer("ESPCNLite", 20)
 if only == "denoise":
